@@ -214,6 +214,23 @@ GSB_API size_t gsb_kmeans_workspace_bytes(int64_t n_values, int32_t n_centers);
 GSB_API int gsb_kmeans(const float* values, int64_t n_values, const float* centers_in, int32_t n_centers, float tol, int32_t max_iterations,
                 int32_t* ids, float* centers_out, char* workspace, void* stream);
 
+/* Exact k nearest neighbours of points [P,3] (fp32) — the reference's second extension simple_knn._C (submodules/simple-knn:
+ * distCUDA2, distIndex2, distIndexQ).  Squared distances d = (p - q).(p - q) evaluated as the reference evaluates them; the query
+ * itself (by index, not by value: an exact duplicate counts at distance 0) is never its own neighbour.
+ *   n_queries < 0: every point is a query and row i belongs to point i (query_ids unused); else row t belongs to query_ids[t], and a
+ *                  query id outside [0, P) gives a row of (FLT_MAX, -1).
+ *   n_candidates < 0: every point is a candidate (candidate_ids unused); else only the points listed in the first min(n_candidates,
+ *                  P) entries of candidate_ids (the reference's fillIndex2Pos quirk); ids outside [0, P) are ignored.
+ *   dists [rows*K] / indices [rows*K] (each may be NULL): row r holds its K nearest as (distance, index) ascending, ties by the
+ *                  smaller index; missing neighbours are (FLT_MAX, -1).
+ *   mean3 [rows] (may be NULL; needs K == 3): ((d0 + d1) + d2) / 3, the reference's distCUDA2.
+ * 0 <= K <= GSB_KNN_MAX_K, P < 2^30, n_queries < 2^30.  workspace: gsb_knn_workspace_bytes(P, n_queries) bytes of device memory.  Fully asynchronous on `stream`
+ * (no host synchronisation).  The result is a function of the points alone: identical bytes from run to run. */
+#define GSB_KNN_MAX_K 64
+GSB_API size_t gsb_knn_workspace_bytes(int32_t P, int32_t n_queries);
+GSB_API int gsb_knn(const float* points, int32_t P, int32_t K, const int32_t* query_ids, int32_t n_queries, const int32_t* candidate_ids,
+                int32_t n_candidates, float* mean3, float* dists, int32_t* indices, char* workspace, void* stream);
+
 /* Loss side of the training step: (1 - lambda) * L1 + lambda * (1 - SSIM) of image vs gt, both [C,H,W] fp32
  * (reference utils/loss_utils.py:17-65 l1_loss / ssim with the 11x11 sigma-1.5 window and zero padding, combined as in
  * train.py:110-115).  Forward writes maps [3,C,H,W] (d ssim / d mu_x, E[x^2], E[xy]) and per-CTA partial sums

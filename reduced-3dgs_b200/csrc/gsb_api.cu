@@ -91,7 +91,7 @@ void prof_end(int kid, cudaStream_t stream)
 	t_prof_cur = nullptr;
 }
 static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter", "tile_sort_large", "unused4", "tile_sort", "unused6",
-	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans" };
+	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
 int launch_preprocess(const GsbScene*, const GsbCamera*, const GeomState&, const ImageState&, const BinPlan&, int32_t*, const GsbDebug*, cudaStream_t);
@@ -110,6 +110,8 @@ int launch_l1_ssim_forward(const float*, const float*, int, int, int, float*, fl
 int launch_l1_ssim_backward(const float*, const float*, int, int, int, const float*, float, const float*, float, const float*, float*, cudaStream_t);
 size_t kmeans_workspace_bytes(long long, int);
 int launch_kmeans(const float*, long long, const float*, int, float, int, int*, float*, char*, cudaStream_t);
+size_t knn_workspace_bytes(long long, long long);
+int launch_knn(const float*, long long, int, const int32_t*, long long, const int32_t*, long long, float*, float*, int32_t*, char*, cudaStream_t);
 int launch_render_backward(const ImageState&, const BinningState&, const GeomState&, int, int, int, const float*, const float*, float*, cudaStream_t);
 int launch_preprocess_backward(const GsbScene*, const GsbCamera*, const GeomState&, const int32_t*, const float*, const GsbGrads*, float, cudaStream_t);
 
@@ -359,6 +361,27 @@ int gsb_kmeans(const float* values, int64_t n_values, const float* centers_in, i
 	if (!centers_in || !centers_out || (n_values > 0 && (!values || !ids || !workspace))) { set_error("kmeans: NULL argument"); return GSB_EINVAL; }
 	if (n_values >= (1ll << 30)) { set_error("kmeans: 2^30 or more values (the look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
 	return launch_kmeans(values, n_values, centers_in, n_centers, tol, max_iterations, ids, centers_out, workspace, (cudaStream_t)stream);
+}
+
+size_t gsb_knn_workspace_bytes(int32_t P, int32_t n_queries) { return knn_workspace_bytes(P < 0 ? 0 : P, n_queries); }
+
+int gsb_knn(const float* points, int32_t P, int32_t K, const int32_t* query_ids, int32_t n_queries, const int32_t* candidate_ids,
+	int32_t n_candidates, float* mean3, float* dists, int32_t* indices, char* workspace, void* stream)
+{
+	if (P < 0) { set_error("knn: P < 0"); return GSB_EINVAL; }
+	if (K < 0) { set_error("knn: K < 0"); return GSB_EINVAL; }
+	if (K > GSB_KNN_MAX_K) { set_error("knn: K = %d is above the supported maximum of %d neighbours", K, GSB_KNN_MAX_K); return GSB_EINVAL; }
+	if (mean3 && K != 3) { set_error("knn: the mean of the 3 nearest needs K == 3 (got %d)", K); return GSB_EINVAL; }
+	if (P >= (1 << 30) || n_queries >= (1 << 30))
+	{ set_error("knn: 2^30 or more points or queries (the sort's look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
+	const long long rows = n_queries < 0 ? P : n_queries;
+	if (rows == 0 || K == 0) return GSB_OK;
+	if (n_queries >= 0 && !query_ids) { set_error("knn: query_ids is NULL"); return GSB_EINVAL; }
+	if (n_candidates > 0 && !candidate_ids) { set_error("knn: candidate_ids is NULL"); return GSB_EINVAL; }
+	if (!mean3 && !dists && !indices) { set_error("knn: no output"); return GSB_EINVAL; }
+	if (P > 0 && (!points || !workspace)) { set_error("knn: NULL points / workspace"); return GSB_EINVAL; }
+	return launch_knn(points, P, K, n_queries < 0 ? nullptr : query_ids, rows, candidate_ids, n_candidates, mean3, dists, indices, workspace,
+		(cudaStream_t)stream);
 }
 
 int gsb_min_redundancy_value(int32_t P, const int32_t* redundancy_values, const int32_t* neighbours, const uint8_t* intersection_mask,

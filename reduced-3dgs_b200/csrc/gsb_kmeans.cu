@@ -105,20 +105,25 @@ __global__ void __launch_bounds__(256) km_sort_plan_kernel(const uint32_t* __res
 #define KM_LB_INC 0x80000000u
 #define KM_LB_VAL 0x3fffffffu
 // One onesweep pass: tile = 4096 consecutive keys; warp w ranks keys [512 w, 512 (w+1)) in 16 warp-wide steps with match.any
-// (stable), digit counts are chained across tiles with decoupled look-back.
-__global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint32_t* keys1, long long n, int pass,
-	const KmSortPlan* __restrict__ plan, uint32_t* lookback_all, uint32_t* tickets, size_t n_tiles)
+// (stable), digit counts are chained across tiles with decoupled look-back.  PAIRS: a 32-bit value travels with each key
+// (the kNN's (Morton code, point index) sort); the k-means sorts keys only.
+template <bool PAIRS>
+__global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint32_t* keys1, uint32_t* vals0, uint32_t* vals1, long long n,
+	int pass, const KmSortPlan* __restrict__ plan, uint32_t* lookback_all, uint32_t* tickets, size_t n_tiles)
 {
 	if (plan->skip[pass]) return;
 	const uint32_t srcb = plan->src[pass];
 	const uint32_t* __restrict__ kin = srcb ? keys1 : keys0;
 	uint32_t* __restrict__ kout = srcb ? keys0 : keys1;
+	const uint32_t* __restrict__ vin = srcb ? vals1 : vals0;
+	uint32_t* __restrict__ vout = srcb ? vals0 : vals1;
 	uint32_t* lookback = lookback_all + (size_t)pass * n_tiles * 256;
 
 	__shared__ uint32_t s_whist[8][256];
 	__shared__ uint32_t s_dstart[256];
 	__shared__ uint32_t s_gbase[256];
 	__shared__ uint32_t s_keys[KM_TILE];
+	__shared__ uint32_t s_vals[PAIRS ? KM_TILE : 1];
 	__shared__ uint32_t s_tile;
 
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -130,7 +135,7 @@ __global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint
 	const int count = (int)min((long long)KM_TILE, n - tbase);
 	const int shift = 8 * pass;
 
-	uint32_t key[KM_ITEMS], rank[KM_ITEMS];
+	uint32_t key[KM_ITEMS], rank[KM_ITEMS], val[PAIRS ? KM_ITEMS : 1];
 	const unsigned lt = (1u << lane) - 1u;
 #pragma unroll
 	for (int i = 0; i < KM_ITEMS; i++)
@@ -138,6 +143,7 @@ __global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint
 		const int local = warp * (32 * KM_ITEMS) + i * 32 + lane;
 		const bool valid = local < count;
 		key[i] = valid ? kin[tbase + local] : 0xffffffffu;
+		if (PAIRS) val[i] = valid ? vin[tbase + local] : 0u;
 		const uint32_t d = valid ? ((key[i] >> shift) & 0xff) : 256u;
 		const unsigned vmask = __ballot_sync(0xffffffffu, valid);
 		const unsigned m = __match_any_sync(0xffffffffu, d) & vmask;
@@ -193,7 +199,9 @@ __global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint
 		if (local < count)
 		{
 			const uint32_t d = (key[i] >> shift) & 0xff;
-			s_keys[s_dstart[d] + s_whist[warp][d] + rank[i]] = key[i];
+			const uint32_t pos = s_dstart[d] + s_whist[warp][d] + rank[i];
+			s_keys[pos] = key[i];
+			if (PAIRS) s_vals[pos] = val[i];
 		}
 	}
 	__syncthreads();
@@ -204,7 +212,9 @@ __global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint
 		if (p < count)
 		{
 			const uint32_t k = s_keys[p];
-			kout[s_gbase[(k >> shift) & 0xff] + p] = k;
+			const uint32_t dst = s_gbase[(k >> shift) & 0xff] + p;
+			kout[dst] = k;
+			if (PAIRS) vout[dst] = s_vals[p];
 		}
 	}
 }
@@ -409,7 +419,8 @@ int launch_kmeans(const float* values, long long n, const float* centres_in, int
 		GSB_LAUNCHED();
 		for (int p = 0; p < 4; p++)
 		{
-			km_sort_pass_kernel<<<(unsigned)w.n_tiles, 256, 0, stream>>>(w.keys0, w.keys1, n, p, w.plan, w.lookback, w.tickets, w.n_tiles);
+			km_sort_pass_kernel<false><<<(unsigned)w.n_tiles, 256, 0, stream>>>(w.keys0, w.keys1, nullptr, nullptr, n, p, w.plan, w.lookback,
+				w.tickets, w.n_tiles);
 			GSB_LAUNCHED();
 		}
 		static thread_local KmSortPlan* h_plan = nullptr;
@@ -441,6 +452,44 @@ int launch_kmeans(const float* values, long long n, const float* centres_in, int
 	km_ids_kernel<<<grid_ids, 256, 0, stream>>>(values, n, centres, K, ids);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
+	return GSB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------ pair sort (gsb_knn.cu)
+// The same onesweep sort on (key, value) pairs, keys in keys0 / values in vals0, with the caller's 4 x 256 digit histogram.  Fully
+// asynchronous: the sorted pairs end in buffer *final_buf (0: keys0 / vals0, 1: keys1 / vals1), a DEVICE word the consumer reads.
+static void sort_pairs_carve(char* base, long long n, KmSortPlan** plan, uint32_t** lookback, uint32_t** tickets, size_t* n_tiles, size_t* bytes)
+{
+	Carver c(base);
+	*n_tiles = ((n > 0 ? (size_t)n : 1) + KM_TILE - 1) / KM_TILE;
+	*plan = c.take<KmSortPlan>(1);
+	*lookback = c.take<uint32_t>(4 * *n_tiles * 256);
+	*tickets = c.take<uint32_t>(4);
+	*bytes = c.off + 256;
+}
+
+size_t sort_pairs_scratch_bytes(long long n)
+{
+	KmSortPlan* plan; uint32_t *lookback, *tickets; size_t n_tiles, bytes;
+	sort_pairs_carve(nullptr, n, &plan, &lookback, &tickets, &n_tiles, &bytes);
+	return bytes;
+}
+
+int launch_sort_pairs(uint32_t* keys0, uint32_t* keys1, uint32_t* vals0, uint32_t* vals1, long long n, const uint32_t* hist, char* scratch,
+	const uint32_t** final_buf, cudaStream_t stream)
+{
+	KmSortPlan* plan; uint32_t *lookback, *tickets; size_t n_tiles, bytes;
+	sort_pairs_carve(scratch, n, &plan, &lookback, &tickets, &n_tiles, &bytes);
+	*final_buf = &plan->final_buf;
+	GSB_CUDA_OK(cudaMemsetAsync(lookback, 0, sizeof(uint32_t) * 4 * n_tiles * 256, stream));
+	GSB_CUDA_OK(cudaMemsetAsync(tickets, 0, sizeof(uint32_t) * 4, stream));
+	km_sort_plan_kernel<<<1, 256, 0, stream>>>(hist, n, plan);
+	GSB_LAUNCHED();
+	for (int p = 0; p < 4; p++)
+	{
+		km_sort_pass_kernel<true><<<(unsigned)n_tiles, 256, 0, stream>>>(keys0, keys1, vals0, vals1, n, p, plan, lookback, tickets, n_tiles);
+		GSB_LAUNCHED();
+	}
 	return GSB_OK;
 }
 

@@ -112,6 +112,11 @@ def lib():
         L.gsb_kmeans.restype = C.c_int
         L.gsb_kmeans.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
+        L.gsb_knn_workspace_bytes.restype = C.c_size_t
+        L.gsb_knn_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
+        L.gsb_knn.restype = C.c_int
+        L.gsb_knn.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                              C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_l1_ssim_blocks.restype = C.c_int64
         L.gsb_l1_ssim_blocks.argtypes = [C.c_int32, C.c_int32, C.c_int32]
         L.gsb_l1_ssim_forward.restype = C.c_int
@@ -158,7 +163,7 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_version", "gsb_profile_enable", "gsb_profile_read", "gsb_debug_dequant", "gsb_forward_statistics",
                     "gsb_sh_statistics_update", "gsb_min_projected_pixel_size", "gsb_sphere_ellipsoid_intersection",
                     "gsb_min_redundancy_value", "gsb_kmeans_workspace_bytes", "gsb_kmeans", "gsb_l1_ssim_blocks",
-                    "gsb_l1_ssim_forward", "gsb_l1_ssim_backward"]
+                    "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn"]
 
 
 def check(status: int):
