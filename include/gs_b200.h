@@ -161,6 +161,32 @@ GSB_API int gsb_backward(const GsbScene* scene, const GsbCamera* cam, int64_t nu
                  const float* dL_dout_color /* [3,H,W] */, const GsbGrads* grads,
                  float lambda_sh_sparsity, void* stream);
 
+/* Forward that also renders the inverse-depth and alpha maps in the same pass as the colour image.
+ *   out_invdepth [1,H,W] fp32: invdepth(x,y) = sum_i (1/depth_i) * alpha_i * T_i over exactly the (pixel, Gaussian) pairs that
+ *                composite the colour, with the same alpha and T.  depth_i is the preprocess view-space z (GsbDebug.depths),
+ *                1/depth_i is an IEEE division; no background term, no normalisation by alpha.
+ *   out_alpha    [1,H,W] fp32: 1 - final_T.
+ * Both are required.  P == 0 gives zero maps; a scene with no (Gaussian, tile) instance gives invdepth 0 and alpha 0.
+ * Colour, radii, R and the blobs are bit-identical to gsb_forward's, and the maps are the same bytes on every run.
+ * Everything else as gsb_forward. */
+GSB_API int gsb_forward_maps(const GsbScene* scene, const GsbCamera* cam,
+                gsb_alloc_fn geom_alloc, void* geom_user,
+                gsb_alloc_fn binning_alloc, void* binning_user,
+                gsb_alloc_fn image_alloc, void* image_user,
+                float* out_color, int32_t* radii, int64_t* num_rendered,
+                const GsbDebug* debug, float* out_invdepth, float* out_alpha, void* stream);
+
+/* Backward of gsb_forward_maps (or of gsb_forward: the maps depend only on the blobs): gsb_backward plus the gradients of the
+ * two maps, dL_dinvdepth and dL_dalpha [1,H,W] fp32, each of which may be NULL (= zero).  They add to dL_dopacity, dL_dmeans2D,
+ * the conic-driven dL_dmeans3D / dL_dscales / dL_drotations / dL_dcov3D; invdepth also adds its direct term
+ * -dL/dinvdepth_i / z_i^2 * (view[2], view[6], view[10]) to dL_dmeans3D.  dL_dcolors and dL_dsh are unchanged.
+ * With both NULL this is gsb_backward. */
+GSB_API int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
+                 const char* geom_blob, const char* binning_blob, const char* image_blob,
+                 const float* dL_dout_color /* [3,H,W] */, const GsbGrads* grads,
+                 const float* dL_dinvdepth /* [1,H,W] or NULL */, const float* dL_dalpha /* [1,H,W] or NULL */,
+                 float lambda_sh_sparsity, void* stream);
+
 /* present[i] = view-space z of means3D[i] > 0.2 (auxiliary.h:139-159). */
 GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);

@@ -52,7 +52,8 @@ __device__ __forceinline__ void warp_store(float* __restrict__ dst, long long ba
 // One warp per 32 consecutive Gaussians (lane = Gaussian).  The SH rows of the warp (32 x 3M floats, contiguous in HBM) are
 // staged through shared memory with unit-stride loads, overwritten in place by the SH gradients and written back with
 // unit-stride stores; the seven small outputs go through warp_store.  Every output element is written exactly once.
-template <bool QUANT, bool ACC>
+// MAPS: the render backward also left sum alpha*T*dL/dinvdepth in accumulator slot 9; invdepth = 1/tz adds -slot9/tz^2 to dL/dtz.
+template <bool QUANT, bool ACC, bool MAPS>
 __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs a)
 {
 	extern __shared__ float s_dyn[];
@@ -116,14 +117,15 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 		float* myrow = s_row + lane * RS;
 		// every per-Gaussian input is requested before the visibility flag is known (the flag is itself a load): radius -> accumulator
 		// -> position -> ids used to be a chain of DRAM round trips; a culled Gaussian now costs ~90 wasted bytes
-		float4 acc0 = make_float4(0.f, 0.f, 0.f, 0.f), acc1 = acc0; float cyy = 0.f, mx = 0.f, my = 0.f, mz = 0.f, opac = 0.f;
+		float4 acc0 = make_float4(0.f, 0.f, 0.f, 0.f), acc1 = acc0; float cyy = 0.f, dinvd = 0.f, mx = 0.f, my = 0.f, mz = 0.f, opac = 0.f;
 		float sc[3] = { 0, 0, 0 }, qr = 1, qx = 0, qy = 0, qz = 0;
 		uint32_t isb[3] = { 0, 0, 0 }, irw = 0; int deg_in = 0; unsigned cl_in = 0;
 		if (valid)
 		{
 			acc0 = reinterpret_cast<const float4*>(a.acc)[3 * idx];
 			acc1 = reinterpret_cast<const float4*>(a.acc)[3 * idx + 1];
-			cyy = a.acc[12 * idx + 8];
+			if (MAPS) { const float2 c = reinterpret_cast<const float2*>(a.acc)[6 * idx + 4]; cyy = c.x; dinvd = c.y; }
+			else cyy = a.acc[12 * idx + 8];
 			mx = a.means3D[3 * idx]; my = a.means3D[3 * idx + 1]; mz = a.means3D[3 * idx + 2];
 			opac = a.g.rec[3 * idx + 1].z;
 			if (QUANT)
@@ -209,7 +211,8 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				const float itz = 1.f / tz, tz2 = itz * itz, tz3 = tz2 * itz;
 				const float dL_dtx = x_grad_mul * -h_x * tz2 * dL_dJ02;
 				const float dL_dty = y_grad_mul * -h_y * tz2 * dL_dJ12;
-				const float dL_dtz = -h_x * tz2 * dL_dJ00 - h_y * tz2 * dL_dJ11 + (2 * h_x * tx) * tz3 * dL_dJ02 + (2 * h_y * ty) * tz3 * dL_dJ12;
+				float dL_dtz = -h_x * tz2 * dL_dJ00 - h_y * tz2 * dL_dJ11 + (2 * h_x * tx) * tz3 * dL_dJ02 + (2 * h_y * ty) * tz3 * dL_dJ12;
+				if (MAPS) dL_dtz -= dinvd * tz2;                                          // d(1/tz)/dtz = -1/tz^2
 				dmean[0] = v[0] * dL_dtx + v[1] * dL_dty + v[2] * dL_dtz;                // transformVec4x3Transpose
 				dmean[1] = v[4] * dL_dtx + v[5] * dL_dty + v[6] * dL_dtz;
 				dmean[2] = v[8] * dL_dtx + v[9] * dL_dty + v[10] * dL_dtz;
@@ -371,7 +374,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 }
 
 int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const int32_t* radii, const float* acc,
-	const GsbGrads* grads, float lambda, cudaStream_t stream)
+	const GsbGrads* grads, bool maps, float lambda, cudaStream_t stream)
 {
 	BwdArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
@@ -387,13 +390,18 @@ int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const Ge
 	const int grid = need < GSB_NUM_SMS * 4 ? need : GSB_NUM_SMS * 4;
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * s->M + 1) + 32 * 6) * sizeof(float);
 	ProfScope prof(K_PREPROCESS_BWD, stream);
-#define GSB_LAUNCH_PB(Q, A)                                                                                          \
+#define GSB_LAUNCH_PB(Q, A, MP)                                                                                       \
 	do {                                                                                                             \
-		if (int e = ensure_dyn_smem((const void*)preprocess_backward_kernel<Q, A>, 160 * 1024)) return e;              \
-		preprocess_backward_kernel<Q, A><<<grid, 256, smem, stream>>>(a);                                            \
+		if (int e = ensure_dyn_smem((const void*)preprocess_backward_kernel<Q, A, MP>, 160 * 1024)) return e;          \
+		preprocess_backward_kernel<Q, A, MP><<<grid, 256, smem, stream>>>(a);                                        \
 	} while (0)
-	if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(true, true); else GSB_LAUNCH_PB(true, false); }
-	else { if (grads->accumulate) GSB_LAUNCH_PB(false, true); else GSB_LAUNCH_PB(false, false); }
+#define GSB_LAUNCH_PB_QA(MP)                                                                                         \
+	do {                                                                                                             \
+		if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(true, true, MP); else GSB_LAUNCH_PB(true, false, MP); }  \
+		else { if (grads->accumulate) GSB_LAUNCH_PB(false, true, MP); else GSB_LAUNCH_PB(false, false, MP); }        \
+	} while (0)
+	if (maps) GSB_LAUNCH_PB_QA(true); else GSB_LAUNCH_PB_QA(false);
+#undef GSB_LAUNCH_PB_QA
 #undef GSB_LAUNCH_PB
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());

@@ -58,12 +58,15 @@ __device__ __forceinline__ float2 lds64(uint32_t addr)
 // of the backward (one cp.async.bulk per 48-byte record, completion on an mbarrier): 256 small copies per batch serialise in the
 // copy engine, while the load/store path issues them from 256 threads at once and this kernel has no other use for the time a
 // ring would hide.
-template <bool STATS>
+// MAPS = true also composites the inverse-depth map D = sum (1/depth) * alpha * T over the same pairs, with the colour channels'
+// operation sequence, and writes D and the alpha map 1 - final_T.  1/depth (IEEE division) is computed once per staged instance and
+// replaces the depth in the shared-memory copy of the record (r2.z), which the forward reads nowhere else.
+template <bool STATS, bool MAPS>
 __global__ void __launch_bounds__(256, 6) render_forward_kernel(const uint2* __restrict__ ranges,
 	const uint32_t* __restrict__ point_list,
 	int W, int H, const float4* __restrict__ rec, const float* __restrict__ bg,
 	float* __restrict__ final_T, uint32_t* __restrict__ n_contrib, float* __restrict__ out_color, uint32_t* __restrict__ tile_max,
-	int32_t* __restrict__ touched_pixels, float* __restrict__ transmittance)
+	int32_t* __restrict__ touched_pixels, float* __restrict__ transmittance, float* __restrict__ out_invdepth, float* __restrict__ out_alpha)
 {
 	__shared__ __align__(16) float4 s_rec[256 * 3];
 	__shared__ uint32_t s_id[STATS ? 256 : 1];
@@ -81,7 +84,7 @@ __global__ void __launch_bounds__(256, 6) render_forward_kernel(const uint2* __r
 	if (tid == 0) s_max = 0;
 
 	uint32_t Tb = inside ? 0x3f800000u : 0xbf800000u;      // bits of T; sign set = finished
-	float C0 = 0.0f, C1 = 0.0f, C2 = 0.0f;
+	float C0 = 0.0f, C1 = 0.0f, C2 = 0.0f, D = 0.0f;
 	uint32_t last = 0;
 	for (uint32_t b = range.x; b < range.y; b += 256)
 	{
@@ -91,7 +94,8 @@ __global__ void __launch_bounds__(256, 6) render_forward_kernel(const uint2* __r
 		{
 			const uint32_t id = point_list[b + tid];
 			const float4 r0 = rec[3 * (size_t)id], r1 = rec[3 * (size_t)id + 1], r2 = rec[3 * (size_t)id + 2];
-			s_rec[3 * tid] = r0; s_rec[3 * tid + 1] = r1; s_rec[3 * tid + 2] = r2;
+			s_rec[3 * tid] = r0; s_rec[3 * tid + 1] = r1;
+			s_rec[3 * tid + 2] = MAPS ? make_float4(r2.x, r2.y, __fdiv_rn(1.0f, r2.z), r2.w) : r2;
 			if (STATS) s_id[tid] = id;
 		}
 		__syncthreads();
@@ -117,7 +121,9 @@ __global__ void __launch_bounds__(256, 6) render_forward_kernel(const uint2* __r
 				const int bit = __ffs(mask) - 1; mask &= mask - 1;
 				const uint32_t addr = cbase + bit * SREC_BYTES;
 				const float4 r0 = lds128(addr), r1 = lds128(addr + 16);
-				const float2 gb = lds64(addr + 32);
+				float2 gb; float invd = 0.0f;
+				if (MAPS) { const float4 r2 = lds128(addr + 32); gb = make_float2(r2.x, r2.y); invd = r2.z; }
+				else gb = lds64(addr + 32);
 				const float T = __uint_as_float(Tb);
 				const float dx = __fsub_rn(r1.x, pxf), dy = __fsub_rn(r1.y, pyf);
 				const float power = pair_power(r0.x, r0.y, r0.z, dx, dy);
@@ -149,6 +155,7 @@ __global__ void __launch_bounds__(256, 6) render_forward_kernel(const uint2* __r
 					C0 = __fmaf_rn(T, __fmul_rn(r1.w, alpha), C0);
 					C1 = __fmaf_rn(T, __fmul_rn(gb.x, alpha), C1);
 					C2 = __fmaf_rn(T, __fmul_rn(gb.y, alpha), C2);
+					if (MAPS) D = __fmaf_rn(T, __fmul_rn(invd, alpha), D);
 					Tb = __float_as_uint(test_T);
 					last = nbase + bit;
 				}
@@ -166,6 +173,7 @@ __global__ void __launch_bounds__(256, 6) render_forward_kernel(const uint2* __r
 		out_color[pid] = __fmaf_rn(bg[0], T, C0);
 		out_color[N + pid] = __fmaf_rn(bg[1], T, C1);
 		out_color[2 * N + pid] = __fmaf_rn(bg[2], T, C2);
+		if (MAPS) { out_invdepth[pid] = D; out_alpha[pid] = __fsub_rn(1.0f, T); }
 	}
 	// where the backward pass has to start for this tile
 	uint32_t m = inside ? last : 0u;
@@ -203,9 +211,10 @@ __device__ __forceinline__ void split_tf32(float v, uint32_t& hi, uint32_t& lo)
 	lo = __float_as_uint(v - __uint_as_float(hi));
 }
 
-// acc record written for the preprocess backward (12 floats per Gaussian, 48 B): [dcol.r dcol.g dcol.b dop | sx sy cxx cxy | cyy - - -]
+// acc record written for the preprocess backward (12 floats per Gaussian, 48 B): [dcol.r dcol.g dcol.b dop | sx sy cxx cxy | cyy dinvd - -]
 // sx = sum dL_dG*dG_ddelx, sy = sum dL_dG*dG_ddely, cxx = sum gdx*dx*dL_dG, cxy = sum gdx*dy*dL_dG, cyy = sum gdy*dy*dL_dG;
 // the constant factors (0.5*W, 0.5*H, -0.5) of backward.cu:583-589 are applied once per Gaussian by the consumer.
+// dinvd = sum alpha*T*dL/dinvdepth (written by the MAPS variant only; the memset leaves it 0 otherwise).
 __device__ __forceinline__ float rcp_approx(float x)
 {
 	float r;
@@ -222,35 +231,50 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 #define BWD_STAGES 4
 // Everything one warp owns privately sits in ONE block: a single base address in a register, every member an immediate offset
 // (with separate per-member arrays ptxas re-derived five base addresses inside the hot loop once registers ran out).
-struct BwdWarp {
+// NCH: channels of the u product's B operand, 3 (colour) or 4 (colour + dL/dinvdepth, MAPS).
+template <int NCH> struct BwdWarp {
 	float w[16 * STASH_LD];                // stash of up to 16 surviving Gaussians: w = G * dL/dalpha per pixel lane
 	float u[16 * STASH_LD];                //                                         u = alpha * T per pixel lane
-	float dlp[3 * 32];                     // dL/dpixel of the warp's 32 pixels, channel-major: B operand of the colour product
+	float dlp[NCH * 32];                   // dL/dpixel (and dL/dinvdepth) of the warp's 32 pixels, channel-major: B operand of the u product
 	uint32_t rowid[16];                    // Gaussian id of each stashed row (rows outlive their staging buffer; the flush re-reads the record)
 	uint8_t queue[BWD_BATCH + 16];         // work queue: batch indices of the entries that survived the warp's cull (+ slack: the loop reads one ahead)
 };
 #define BW_OFF_U (16 * STASH_LD * 4)
-#define BW_OFF_ROWID (2 * 16 * STASH_LD * 4 + 3 * 32 * 4)
-#define BW_OFF_QUEUE (BW_OFF_ROWID + 16 * 4)
-struct BwdSmem {
+#define BW_OFF_ROWID(NCH) (2 * 16 * STASH_LD * 4 + (NCH) * 32 * 4)
+#define BW_OFF_QUEUE(NCH) (BW_OFF_ROWID(NCH) + 16 * 4)
+template <int NCH> struct BwdSmem {
 	float4 rec[BWD_STAGES][BWD_BATCH * 3]; // ring of staged batches of the tile's list: one 48-byte TMA bulk copy per instance (the record carries its Gaussian id in r2.w)
 	uint64_t full[BWD_STAGES];             // mbarrier: the stage's copies have landed (64 arrivals + transaction bytes)
 	uint64_t empty[BWD_STAGES];            // mbarrier: all 8 warps are done reading the stage
 	float wgt[8 * 32];                     // (1, qx, qy, qx^2, qx*qy, qy^2, 0, 0) of the 32 warp-local pixels: B operand of the moment product
-	BwdWarp wp[8];
+	BwdWarp<NCH> wp[8];
 };
-static_assert(offsetof(BwdWarp, u) == BW_OFF_U && offsetof(BwdWarp, rowid) == BW_OFF_ROWID && offsetof(BwdWarp, queue) == BW_OFF_QUEUE, "BwdWarp layout");
-static_assert(sizeof(BwdWarp) % 16 == 0, "BwdWarp alignment");
+static_assert(offsetof(BwdWarp<3>, u) == BW_OFF_U && offsetof(BwdWarp<3>, rowid) == BW_OFF_ROWID(3) && offsetof(BwdWarp<3>, queue) == BW_OFF_QUEUE(3), "BwdWarp layout");
+static_assert(offsetof(BwdWarp<4>, u) == BW_OFF_U && offsetof(BwdWarp<4>, rowid) == BW_OFF_ROWID(4) && offsetof(BwdWarp<4>, queue) == BW_OFF_QUEUE(4), "BwdWarp layout");
+static_assert(sizeof(BwdWarp<3>) % 16 == 0 && sizeof(BwdWarp<4>) % 16 == 0, "BwdWarp alignment");
+
+__device__ __forceinline__ void red_add_v2(float* addr, float a, float b)
+{
+	asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(addr), "f"(a), "f"(b) : "memory");
+}
 
 
+// MAPS = true adds the gradients of the inverse-depth and alpha maps (render_forward_kernel<*, true>):
+//  - alpha = 1 - T_final enters every pair exactly like the background term: bg.dL/dpixel becomes bg.dL/dpixel - dL/dalpha_map;
+//  - invdepth is a fourth colour channel (colour 1/depth, no background): its recurrence runs next to the colour one, its
+//    dL/dinvdepth fills the B column of the u product that is zero padding otherwise, and sum_p u_p * dL/dinvdepth(p) lands in
+//    slot 9 of the accumulator, next to cyy (one vector reduction instead of the scalar one).
+// 1/depth is the MUFU reciprocal here (the forward's IEEE value to 1 ulp; the result is a tolerance-compared gradient).
+template <bool MAPS>
 __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __restrict__ ranges,
 	const uint32_t* __restrict__ point_list,
 	int W, int H, const float4* __restrict__ rec, const float* __restrict__ bg,
 	const float* __restrict__ final_Ts, const uint32_t* __restrict__ n_contrib, const uint32_t* __restrict__ tile_max,
-	const float* __restrict__ dL_dpixels, float* __restrict__ acc)
+	const float* __restrict__ dL_dpixels, float* __restrict__ acc, const float* __restrict__ dL_dinvdepth, const float* __restrict__ dL_dalpha)
 {
+	constexpr int NCH = MAPS ? 4 : 3;
 	extern __shared__ __align__(16) unsigned char s_dyn_raw[];
-	BwdSmem& S = *reinterpret_cast<BwdSmem*>(s_dyn_raw);
+	BwdSmem<NCH>& S = *reinterpret_cast<BwdSmem<NCH>*>(s_dyn_raw);
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const int tile = blockIdx.y * gridDim.x + blockIdx.x;
 	const uint32_t hi = tile_max[tile];
@@ -265,7 +289,7 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 	const size_t pid = (size_t)W * py + px, N = (size_t)W * H;
 	uint32_t sbase0 = (uint32_t)__cvta_generic_to_shared(&S.rec[0][0]);
 	asm volatile("" : "+r"(sbase0));
-	BwdWarp& Wp = S.wp[warp];
+	BwdWarp<NCH>& Wp = S.wp[warp];
 	uint32_t wbase = (uint32_t)__cvta_generic_to_shared(&Wp);           // the warp's private block (see BwdWarp)
 	asm volatile("" : "+r"(wbase));
 	const unsigned lt_mask = (1u << lane) - 1u;
@@ -275,7 +299,13 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 	const uint32_t last_contributor = inside ? n_contrib[pid] : 0u;
 	float dLp0 = 0.f, dLp1 = 0.f, dLp2 = 0.f;
 	if (inside) { dLp0 = dL_dpixels[pid]; dLp1 = dL_dpixels[N + pid]; dLp2 = dL_dpixels[2 * N + pid]; }
-	const float bg_dot_dpixel = bg[0] * dLp0 + bg[1] * dLp1 + bg[2] * dLp2;
+	float bg_dot_dpixel = bg[0] * dLp0 + bg[1] * dLp1 + bg[2] * dLp2;
+	float dLd = 0.f, ar3 = 0.f, lc3 = 0.f;                                       // MAPS: dL/dinvdepth and its recurrence
+	if (MAPS && inside)
+	{
+		if (dL_dinvdepth) dLd = dL_dinvdepth[pid];
+		if (dL_dalpha) bg_dot_dpixel -= dL_dalpha[pid];
+	}
 	float ar0 = 0.f, ar1 = 0.f, ar2 = 0.f, lc0 = 0.f, lc1 = 0.f, lc2 = 0.f, last_alpha = 0.f;
 	uint32_t wmax = last_contributor;
 #pragma unroll
@@ -300,6 +330,7 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 		S.wgt[6 * 32 + tid] = 0.0f; S.wgt[7 * 32 + tid] = 0.0f;
 	}
 	Wp.dlp[lane] = dLp0; Wp.dlp[32 + lane] = dLp1; Wp.dlp[64 + lane] = dLp2;
+	if (MAPS) Wp.dlp[96 + lane] = dLd;
 	const float cxw = rx0 + 3.5f, cyw = ry0 + 1.5f;                                // centre of the warp's 8x4 pixel block
 	__syncthreads();
 
@@ -316,7 +347,7 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 			if (fg + 8 < nrows) asm volatile("prefetch.global.L1 [%0];" ::"l"(rec + 3 * (size_t)Wp.rowid[fg + 8]));
 		}
 		float dw[4] = { 0.f, 0.f, 0.f, 0.f }, du[4] = { 0.f, 0.f, 0.f, 0.f };
-		const float* dl = Wp.dlp + (fg < 3 ? fg : 0) * 32;
+		const float* dl = Wp.dlp + (fg < NCH ? fg : 0) * 32;
 #pragma unroll
 		for (int kk = 0; kk < 4; kk++)
 		{
@@ -324,8 +355,8 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 			// B fragments: b0 = B[k = c0][n = fg], b1 = B[k = c1][n = fg]
 			const uint32_t bw0 = __float_as_uint(S.wgt[fg * 32 + c0]), bw1 = __float_as_uint(S.wgt[fg * 32 + c1]);
 			uint32_t buh0, buh1, bul0, bul1;
-			split_tf32(fg < 3 ? dl[c0] : 0.0f, buh0, bul0);
-			split_tf32(fg < 3 ? dl[c1] : 0.0f, buh1, bul1);
+			split_tf32(fg < NCH ? dl[c0] : 0.0f, buh0, bul0);
+			split_tf32(fg < NCH ? dl[c1] : 0.0f, buh1, bul1);
 			uint32_t h0, h1, h2, h3, l0, l1, l2, l3;
 			split_tf32(sw[fg * STASH_LD + c0], h0, l0); split_tf32(sw[(fg + 8) * STASH_LD + c0], h1, l1);
 			split_tf32(sw[fg * STASH_LD + c1], h2, l2); split_tf32(sw[(fg + 8) * STASH_LD + c1], h3, l3);
@@ -338,7 +369,7 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 			mma_tf32(du, h0, h1, h2, h3, bul0, bul1);
 		}
 		// D fragment: d[0] = D[g][2t], d[1] = D[g][2t+1], d[2] = D[g+8][2t], d[3] = D[g+8][2t+1]; columns of the w product:
-		// (M0 Mx | My Mxx | Mxy Myy) in lanes t = 0 | 1 | 2, of the u product (c0 c1 | c2 -) in lanes t = 0 | 1.
+		// (M0 Mx | My Mxx | Mxy Myy) in lanes t = 0 | 1 | 2, of the u product (c0 c1 | c2 -) in lanes t = 0 | 1 ((c0 c1 | c2 dinvd) with MAPS).
 		const int q1 = (lane & ~3) | 1, q2 = (lane & ~3) | 2;
 #pragma unroll
 		for (int h = 0; h < 2; h++)
@@ -346,6 +377,8 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 			const float My = __shfl_sync(0xffffffffu, dw[2 * h], q1), Mxx = __shfl_sync(0xffffffffu, dw[2 * h + 1], q1);
 			const float Mxy = __shfl_sync(0xffffffffu, dw[2 * h], q2), Myy = __shfl_sync(0xffffffffu, dw[2 * h + 1], q2);
 			const float c2 = __shfl_sync(0xffffffffu, du[2 * h], q1);
+			float dinvd = 0.f;
+			if (MAPS) dinvd = __shfl_sync(0xffffffffu, du[2 * h + 1], q1);
 			const uint32_t row = fg + 8 * h;
 			if (ft == 0 && row < nrows)
 			{
@@ -360,7 +393,8 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 				float* a = acc + 12 * (size_t)gid;
 				red_add_v4(a, du[2 * h], du[2 * h + 1], c2, M0);
 				red_add_v4(a + 4, -o * (r0.x * Sx + r0.y * Sy), -o * (r0.z * Sy + r0.y * Sx), o * Sxx, o * Sxy);
-				atomicAdd(a + 8, o * Syy);
+				if (MAPS) red_add_v2(a + 8, o * Syy, dinvd);
+				else atomicAdd(a + 8, o * Syy);
 			}
 		}
 		__syncwarp();
@@ -429,10 +463,10 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 		uint32_t posb = hi - 1 - b;                                            // list position of batch entry 0 (entries run backwards)
 		asm volatile("" : "+r"(posb));
 		uint32_t jj = 0, jnext;
-		if (qn) asm volatile("ld.shared.u8 %0, [%1+%2];" : "=r"(jj) : "r"(wbase), "n"(BW_OFF_QUEUE));
+		if (qn) asm volatile("ld.shared.u8 %0, [%1+%2];" : "=r"(jj) : "r"(wbase), "n"(BW_OFF_QUEUE(NCH)));
 		for (uint32_t q = 0; q < qn; q++, jj = jnext)
 		{
-			asm volatile("ld.shared.u8 %0, [%1+%2];" : "=r"(jnext) : "r"(wbase + q), "n"(BW_OFF_QUEUE + 1));   // next entry's index: off the critical path
+			asm volatile("ld.shared.u8 %0, [%1+%2];" : "=r"(jnext) : "r"(wbase + q), "n"(BW_OFF_QUEUE(NCH) + 1));   // next entry's index: off the critical path
 			const uint32_t pos = posb - jj;
 			const uint32_t addr = sbase + jj * SREC_BYTES;
 			const float4 r0 = lds128(addr), r1 = lds128(addr + 16);
@@ -458,6 +492,14 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 				ar1 = last_alpha * lc1 + oml * ar1; lc1 = cg;
 				ar2 = last_alpha * lc2 + oml * ar2; lc2 = cb;
 				float dL_dalpha = (cr - ar0) * dLp0 + (cg - ar1) * dLp1 + (cb - ar2) * dLp2;
+				if (MAPS)
+				{
+					const float invd = rcp_approx(r2.z);
+					float dLd_p;                                                   // re-read from the B operand: one register less in the loop
+					asm volatile("ld.shared.f32 %0, [%1+%2];" : "=f"(dLd_p) : "r"(wbase + lane * 4), "n"(2 * 16 * STASH_LD * 4 + 96 * 4));
+					ar3 = last_alpha * lc3 + oml * ar3; lc3 = invd;
+					dL_dalpha += (invd - ar3) * dLd_p;
+				}
 				dL_dalpha *= T;
 				last_alpha = alpha;
 				dL_dalpha += (-T_final * inv) * bg_dot_dpixel;                      // backward.cu:569-572
@@ -467,7 +509,7 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 				const uint32_t sa = wbase + (nrows * STASH_LD + lane) * 4;
 				asm volatile("st.shared.f32 [%0], %1;" ::"r"(sa), "f"(wv) : "memory");
 				asm volatile("st.shared.f32 [%0+%2], %1;" ::"r"(sa), "f"(uv), "n"(BW_OFF_U) : "memory");
-				if (lane == 0) asm volatile("st.shared.f32 [%0+%2], %1;" ::"r"(wbase + nrows * 4), "f"(r2.w), "n"(BW_OFF_ROWID) : "memory");
+				if (lane == 0) asm volatile("st.shared.f32 [%0+%2], %1;" ::"r"(wbase + nrows * 4), "f"(r2.w), "n"(BW_OFF_ROWID(NCH)) : "memory");
 			}
 			nrows++;
 			if (nrows == 16) flush_rows();
@@ -480,31 +522,41 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 
 // ------------------------------------------------------------------------------------------------
 int launch_render_forward(const ImageState& img, const BinningState& b, const GeomState& g, int W, int H, const float* bg,
-	float* out_color, int32_t* touched_pixels, float* transmittance, cudaStream_t stream)
+	float* out_color, int32_t* touched_pixels, float* transmittance, float* out_invdepth, float* out_alpha, cudaStream_t stream)
 {
 	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
 	ProfScope prof(K_RENDER_FWD, stream);
 	if (touched_pixels && transmittance)
-		render_forward_kernel<true><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, touched_pixels, transmittance);
+		render_forward_kernel<true, false><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
+			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, touched_pixels, transmittance, nullptr, nullptr);
+	else if (out_invdepth && out_alpha)
+		render_forward_kernel<false, true><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
+			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, nullptr, nullptr, out_invdepth, out_alpha);
 	else
-		render_forward_kernel<false><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, nullptr, nullptr);
+		render_forward_kernel<false, false><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
+			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, nullptr, nullptr, nullptr, nullptr);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
 }
 
 int launch_render_backward(const ImageState& img, const BinningState& b, const GeomState& g, int P, int W, int H, const float* bg,
-	const float* dL_dpix, float* acc, cudaStream_t stream)
+	const float* dL_dpix, const float* dL_dinvdepth, const float* dL_dalpha, float* acc, cudaStream_t stream)
 {
 	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
-	if (int e = ensure_dyn_smem((const void*)render_backward_kernel, (int)sizeof(BwdSmem))) return e;
+	const bool maps = dL_dinvdepth || dL_dalpha;
+	const void* kernel = maps ? (const void*)render_backward_kernel<true> : (const void*)render_backward_kernel<false>;
+	const size_t smem = maps ? sizeof(BwdSmem<4>) : sizeof(BwdSmem<3>);
+	if (int e = ensure_dyn_smem(kernel, (int)smem)) return e;
 	ProfScope prof(K_RENDER_BWD, stream);
 	// the per-Gaussian accumulator the kernel reduces into (12 floats per Gaussian, inside the geometry blob)
 	GSB_CUDA_OK(cudaMemsetAsync(acc, 0, size_t(P) * 48, stream));
-	render_backward_kernel<<<grid, 256, sizeof(BwdSmem), stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-		img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, acc);
+	if (maps)
+		render_backward_kernel<true><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
+			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, acc, dL_dinvdepth, dL_dalpha);
+	else
+		render_backward_kernel<false><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
+			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, acc, nullptr, nullptr);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;

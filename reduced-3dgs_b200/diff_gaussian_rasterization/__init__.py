@@ -4,7 +4,8 @@ GaussianRasterizationSettings (:169-181), GaussianRasterizer (:183-234), rasteri
 _RasterizeGaussians autograd op (:48-167), backed by the H100-native kernels through `_C`.
 
 Differences, all additive: GaussianRasterizer.forward takes keyword-only `prune_mask` and `quant`
-(fused resolution-aware prune mask / codebook de-quantisation, SURVEY §8(b)); the forward no longer forces
+(fused resolution-aware prune mask / codebook de-quantisation, SURVEY §8(b)) and `return_maps` (differentiable inverse-depth
+and alpha maps from the same pass: (color, radii, invdepth, alpha)); the forward no longer forces
 debug=True (reference :85 hard-wires a device sync after every stage); gradients are allocated uninitialised
 because the kernels write every element.
 """
@@ -22,15 +23,15 @@ def cpu_deep_copy_tuple(input_tuple):
 
 
 def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None):
+                        raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False):
     return _RasterizeGaussians.apply(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant)
+                                     cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None):
+                raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False):
         args = (raster_settings.bg, means3D, colors_precomp, opacities, scales, rotations, raster_settings.scale_modifier,
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, raster_settings.image_height, raster_settings.image_width, sh, degrees,
@@ -38,15 +39,14 @@ class _RasterizeGaussians(torch.autograd.Function):
         if raster_settings.debug:
             cpu_args = cpu_deep_copy_tuple(args)   # Copy them before they can be corrupted (reference :90-97)
             try:
-                num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = _C.rasterize_gaussians(
-                    *args, prune_mask=prune_mask, quant=quant)
+                out = _C.rasterize_gaussians(*args, prune_mask=prune_mask, quant=quant, return_maps=return_maps)
             except Exception as ex:
                 torch.save(cpu_args, "snapshot_fw.dump")
                 print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
                 raise ex
         else:
-            num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = _C.rasterize_gaussians(
-                *args, prune_mask=prune_mask, quant=quant)
+            out = _C.rasterize_gaussians(*args, prune_mask=prune_mask, quant=quant, return_maps=return_maps)
+        num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = out[:6]
         ctx.raster_settings = raster_settings
         ctx.num_rendered = num_rendered
         ctx.lambda_sh_sparsity = lambda_sh_sparsity
@@ -55,14 +55,22 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
                               binningBuffer, imgBuffer, degrees)
         ctx.mark_non_differentiable(radii)
+        if return_maps:
+            # a loss on some outputs only: the others' gradients arrive as None and reach the kernels as NULL (zero)
+            ctx.set_materialize_grads(False)
+            return color, radii, out[6], out[7]
         return color, radii
 
     @staticmethod
-    def backward(ctx, grad_out_color, _):
+    def backward(ctx, grad_out_color, _, grad_invdepth=None, grad_alpha=None):
         num_rendered = ctx.num_rendered
         raster_settings = ctx.raster_settings
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer,
          degrees) = ctx.saved_tensors
+        if grad_out_color is None:
+            grad_out_color = torch.zeros((3, raster_settings.image_height, raster_settings.image_width), dtype=torch.float32,
+                                         device=means3D.device)
+        maps = dict(dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha)
         args = (raster_settings.bg, means3D, radii, colors_precomp, scales, rotations, raster_settings.scale_modifier,
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, grad_out_color, sh, degrees, raster_settings.campos, geomBuffer, num_rendered,
@@ -70,13 +78,13 @@ class _RasterizeGaussians(torch.autograd.Function):
         if raster_settings.debug:
             cpu_args = cpu_deep_copy_tuple(args)
             try:
-                grads8 = _C.rasterize_gaussians_backward(*args, prune_mask=ctx.prune_mask, quant=ctx.quant)
+                grads8 = _C.rasterize_gaussians_backward(*args, prune_mask=ctx.prune_mask, quant=ctx.quant, **maps)
             except Exception as ex:
                 torch.save(cpu_args, "snapshot_bw.dump")
                 print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
                 raise ex
         else:
-            grads8 = _C.rasterize_gaussians_backward(*args, prune_mask=ctx.prune_mask, quant=ctx.quant)
+            grads8 = _C.rasterize_gaussians_backward(*args, prune_mask=ctx.prune_mask, quant=ctx.quant, **maps)
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
          grad_rotations) = grads8
         if ctx.quant is not None:
@@ -93,7 +101,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         grads = (grad_means3D, grad_means2D, grad_sh if need[2] else None, None,
                  grad_colors_precomp if need[4] else None, grad_opacities if need[5] else None,
                  grad_scales if need[6] else None, grad_rotations if need[7] else None,
-                 grad_cov3Ds_precomp if need[8] else None, None, None, None, None)
+                 grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None)
         return grads
 
 
@@ -125,7 +133,8 @@ class GaussianRasterizer(nn.Module):
         return visible
 
     def forward(self, means3D, means2D, opacities, shs=None, degrees=None, colors_precomp=None, scales=None,
-                rotations=None, cov3D_precomp=None, lambda_sh_sparsity=0., *, prune_mask=None, quant=None):
+                rotations=None, cov3D_precomp=None, lambda_sh_sparsity=0., *, prune_mask=None, quant=None, return_maps=False):
+        """-> (color, radii); with return_maps, (color, radii, invdepth [1,H,W], alpha [1,H,W]), all three differentiable."""
         raster_settings = self.raster_settings
         if quant is None:
             if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
@@ -147,4 +156,4 @@ class GaussianRasterizer(nn.Module):
         if opacities is None:
             opacities = empty
         return rasterize_gaussians(means3D, means2D, shs, degrees, colors_precomp, opacities, scales, rotations,
-                                   cov3D_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant)
+                                   cov3D_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps)

@@ -5,7 +5,8 @@ per_band_count); `viewpoint_camera` likewise (FoVx, FoVy, image_height, image_wi
 full_proj_transform, camera_center).
 
 Build-defined extras: `pc.prune_mask` (optional tensor) and `pc.quant` (optional QuantScene) are forwarded to the
-fused kernels when present.
+fused kernels when present; `return_maps=True` adds the inverse-depth and alpha maps of the same pass to the dict
+("invdepth", "alpha", [1,H,W] each; differentiable except on the variable-SH inference path).
 """
 import math
 import pkgutil
@@ -45,7 +46,7 @@ def eval_sh(deg, sh, dirs):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-           lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False):
+           lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False, return_maps=False):
     """
     Render the scene.
 
@@ -112,16 +113,21 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         cumsum_count = torch.cumsum(per_band_count, dim=0).to(dtype=torch.int)
         coeffs_num = torch.tensor([i * i for i in range(1, len(pc.per_band_count) + 1)], dtype=torch.int)
         empty = torch.Tensor([])
-        _, rendered_image, radii, _, _, _ = rasterize_gaussians_variableSH_bands(
+        out = rasterize_gaussians_variableSH_bands(
             raster_settings.bg, means3D, empty, opacity, scales, rotations, raster_settings.scale_modifier, empty,
             raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
             raster_settings.image_height, raster_settings.image_width, shs, per_band_count, cumsum_count, coeffs_num,
-            degrees, raster_settings.campos, raster_settings.prefiltered, raster_settings.debug, prune_mask=prune_mask)
+            degrees, raster_settings.campos, raster_settings.prefiltered, raster_settings.debug, prune_mask=prune_mask,
+            return_maps=return_maps)
+        rendered_image, radii = out[1], out[2]
+        maps = out[6:]
     else:
-        rendered_image, radii = rasterizer(
+        out = rasterizer(
             means3D=means3D, means2D=means2D, shs=shs, degrees=degrees, colors_precomp=colors_precomp, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, lambda_sh_sparsity=lambda_sh_sparsity,
-            prune_mask=prune_mask, quant=quant)
+            prune_mask=prune_mask, quant=quant, return_maps=return_maps)
+        rendered_image, radii = out[0], out[1]
+        maps = out[2:]
     if measure_fps:
         end_timer.record()
         torch.cuda.synchronize()
@@ -129,8 +135,11 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
     # Those Gaussians that were frustum culled or had a radius of 0 were not visible.
     # They will be excluded from value updates used in the splitting criteria.
-    return {"render": rendered_image,
-            "viewspace_points": screenspace_points,
-            "visibility_filter": radii > 0,
-            "radii": radii,
-            "FPS": fps}
+    pkg = {"render": rendered_image,
+           "viewspace_points": screenspace_points,
+           "visibility_filter": radii > 0,
+           "radii": radii,
+           "FPS": fps}
+    if return_maps:
+        pkg["invdepth"], pkg["alpha"] = maps
+    return pkg

@@ -93,6 +93,10 @@ def lib():
         L.gsb_forward.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p,
                                   ALLOC_FN, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
                                   C.POINTER(GsbDebug), C.c_void_p]
+        L.gsb_forward_maps.restype = C.c_int
+        L.gsb_forward_maps.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p,
+                                       ALLOC_FN, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
+                                       C.POINTER(GsbDebug), C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_forward_statistics.restype = C.c_int
         L.gsb_forward_statistics.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p,
                                              ALLOC_FN, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
@@ -127,6 +131,9 @@ def lib():
         L.gsb_backward.restype = C.c_int
         L.gsb_backward.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_void_p, C.c_void_p, C.POINTER(GsbGrads), C.c_float, C.c_void_p]
+        L.gsb_backward_maps.restype = C.c_int
+        L.gsb_backward_maps.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.POINTER(GsbGrads), C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
         L.gsb_mark_visible.restype = C.c_int
         L.gsb_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_export_binning.restype = C.c_int
@@ -163,7 +170,8 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_version", "gsb_profile_enable", "gsb_profile_read", "gsb_debug_dequant", "gsb_forward_statistics",
                     "gsb_sh_statistics_update", "gsb_min_projected_pixel_size", "gsb_sphere_ellipsoid_intersection",
                     "gsb_min_redundancy_value", "gsb_kmeans_workspace_bytes", "gsb_kmeans", "gsb_l1_ssim_blocks",
-                    "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn"]
+                    "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn",
+                    "gsb_forward_maps", "gsb_backward_maps"]
 
 
 def check(status: int):
