@@ -187,6 +187,29 @@ GSB_API int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64
                  const float* dL_dinvdepth /* [1,H,W] or NULL */, const float* dL_dalpha /* [1,H,W] or NULL */,
                  float lambda_sh_sparsity, void* stream);
 
+/* Backward with the gradient w.r.t. the camera: gsb_backward_maps plus
+ *   dL_dviewmatrix [16], dL_dprojmatrix [16], dL_dcampos [3]  (fp32, the transposed layouts of GsbCamera; each may be NULL).
+ * The camera gradient is the chain rule through the same expressions whose derivatives the backward already uses for
+ * dL_dmeans3D (the 1.3 tan_fov clamp masks of t, the 0.3 dilation of cov2D, the 1e-7 epsilons of the conic and of 1/w): it is
+ * not a finite-difference derivative of the forward.  Per visible Gaussian (t = m . view, T = W J, ndc = hom.xy * m_w):
+ *   dL/dview[4r+c] = dL/dt_c m_r (r = 0..3, m_3 = 1) + the direct terms through T (r = 0..2);
+ *   dL/dproj[4r+j] for j = 0, 1, 3 through ndc;  dL/dcampos = - the SH view-direction term of dL_dmeans3D.
+ * view[3,7,11,15] and proj[2,6,10,14] are not read by the preprocess: their gradients are exactly 0.  Culled and pruned
+ * Gaussians contribute nothing; P == 0, or no instance, gives zeros.  The camera outputs are always overwritten, also when
+ * grads->accumulate is set (each view has its own camera).  The reduction has a fixed order (per-CTA partial rows in the workspace,
+ * summed in double by one CTA): the same bytes on every run, no host synchronisation.  Per-Gaussian outputs: dL_dmeans2D (and
+ * dL_dmeans2D_view), dL_dcolors, dL_dopacity and dL_dconic are bit-identical to gsb_backward_maps on the same inputs; the others
+ * come from a separately compiled kernel whose multiply-adds may be fused differently and agree to fp32 rounding.  With all three
+ * camera outputs NULL this is gsb_backward_maps.
+ * workspace: gsb_camera_grad_workspace_bytes(P) bytes of device memory, required (non-NULL) when any camera output is requested. */
+GSB_API size_t gsb_camera_grad_workspace_bytes(int32_t P);
+GSB_API int gsb_backward_camera(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
+                 const char* geom_blob, const char* binning_blob, const char* image_blob,
+                 const float* dL_dout_color /* [3,H,W] */, const GsbGrads* grads,
+                 const float* dL_dinvdepth /* [1,H,W] or NULL */, const float* dL_dalpha /* [1,H,W] or NULL */,
+                 float lambda_sh_sparsity, float* dL_dviewmatrix /* [16] */, float* dL_dprojmatrix /* [16] */,
+                 float* dL_dcampos /* [3] */, char* workspace, void* stream);
+
 /* present[i] = view-space z of means3D[i] > 0.2 (auxiliary.h:139-159). */
 GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);

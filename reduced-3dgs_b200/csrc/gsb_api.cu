@@ -91,7 +91,7 @@ void prof_end(int kid, cudaStream_t stream)
 	t_prof_cur = nullptr;
 }
 static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter", "tile_sort_large", "unused4", "tile_sort", "unused6",
-	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn" };
+	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
 int launch_preprocess(const GsbScene*, const GsbCamera*, const GeomState&, const ImageState&, const BinPlan&, int32_t*, const GsbDebug*, cudaStream_t);
@@ -116,7 +116,9 @@ int launch_knn(const float*, long long, int, const int32_t*, long long, const in
 int launch_render_backward(const ImageState&, const BinningState&, const GeomState&, int, int, int, const float*, const float*, const float*,
 	const float*, float*, cudaStream_t);
 int launch_preprocess_backward(const GsbScene*, const GsbCamera*, const GeomState&, const int32_t*, const float*, const GsbGrads*, bool, float,
-	cudaStream_t);
+	float*, cudaStream_t);
+size_t camera_grad_workspace_bytes(int);
+int launch_camera_grad_finish(int, const float*, float*, float*, float*, cudaStream_t);
 
 // geometry blob = GeomState followed by the backward's gradient accumulator (12 floats per Gaussian)
 static size_t geom_state_bytes(int P) { size_t b; GeomState::carve(nullptr, P, &b); return (b + 255) & ~size_t(255); }
@@ -411,13 +413,22 @@ int gsb_min_redundancy_value(int32_t P, const int32_t* redundancy_values, const 
 
 static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
 	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity, void* stream_)
+	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
+	float* dL_dview, float* dL_dproj, float* dL_dcampos, char* cam_workspace, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (int e = check_scene(scene, cam)) return e;
 	if (!grads) { set_error("grads is NULL"); return GSB_EINVAL; }
 	const int P = scene->P, W = cam->width, H = cam->height;
-	if (P == 0) return GSB_OK;
+	const bool want_cam = dL_dview || dL_dproj || dL_dcampos;
+	if (P == 0)
+	{
+		// no Gaussian, no camera gradient (the camera outputs are always written, also in accumulate mode)
+		if (dL_dview) GSB_CUDA_OK(cudaMemsetAsync(dL_dview, 0, 16 * sizeof(float), stream));
+		if (dL_dproj) GSB_CUDA_OK(cudaMemsetAsync(dL_dproj, 0, 16 * sizeof(float), stream));
+		if (dL_dcampos) GSB_CUDA_OK(cudaMemsetAsync(dL_dcampos, 0, 3 * sizeof(float), stream));
+		return GSB_OK;
+	}
 	if (!geom_blob || !binning_blob || !image_blob || !dL_dout_color || !radii) { set_error("backward inputs missing"); return GSB_EINVAL; }
 	if (!grads->dL_dmeans2D || !grads->dL_dcolors || !grads->dL_dopacity || !grads->dL_dmeans3D || !grads->dL_dcov3D ||
 		!grads->dL_dscales || !grads->dL_drotations || (scene->M > 0 && !grads->dL_dsh))
@@ -427,7 +438,10 @@ static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R,
 	BinningState b = BinningState::carve(const_cast<char*>(binning_blob), R);
 	float* acc = reinterpret_cast<float*>(const_cast<char*>(geom_blob) + geom_state_bytes(P));
 	if (int e = launch_render_backward(img, b, g, P, W, H, cam->background, dL_dout_color, dL_dinvdepth, dL_dalpha, acc, stream)) return e;
-	if (int e = launch_preprocess_backward(scene, cam, g, radii, acc, grads, dL_dinvdepth != nullptr, lambda_sh_sparsity, stream)) return e;
+	float* cam_rows = want_cam ? reinterpret_cast<float*>(cam_workspace) : nullptr;
+	if (int e = launch_preprocess_backward(scene, cam, g, radii, acc, grads, dL_dinvdepth != nullptr, lambda_sh_sparsity, cam_rows, stream))
+		return e;
+	if (want_cam) if (int e = launch_camera_grad_finish(P, cam_rows, dL_dview, dL_dproj, dL_dcampos, stream)) return e;
 	return GSB_OK;
 }
 
@@ -436,7 +450,21 @@ int gsb_backward(const GsbScene* scene, const GsbCamera* cam, int64_t R, const i
 	const GsbGrads* grads, float lambda_sh_sparsity, void* stream)
 {
 	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, nullptr, nullptr,
-		lambda_sh_sparsity, stream);
+		lambda_sh_sparsity, nullptr, nullptr, nullptr, nullptr, stream);
+}
+
+size_t gsb_camera_grad_workspace_bytes(int32_t P) { return camera_grad_workspace_bytes(P); }
+
+int gsb_backward_camera(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
+	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
+	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
+	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, void* stream)
+{
+	if (!scene || scene->P < 0) { set_error("backward_camera: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
+	{ set_error("backward_camera: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
+	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, stream);
 }
 
 int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
@@ -445,7 +473,7 @@ int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t R, co
 {
 	if (!scene || scene->P < 0) { set_error("backward_maps: scene is NULL or P < 0"); return GSB_EINVAL; }
 	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, stream);
+		lambda_sh_sparsity, nullptr, nullptr, nullptr, nullptr, stream);
 }
 
 int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present, void* stream)

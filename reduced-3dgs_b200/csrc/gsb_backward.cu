@@ -19,7 +19,13 @@ struct BwdArgs {
 	int quant; GsbQuant q;
 	GeomState g; const float* acc;
 	GsbGrads out;
+	float* cam_rows;          // CAM: one row of GSB_CAM_SLOTS partial sums per CTA (the caller's workspace)
 };
+
+// Camera gradient slots (CAM): 0..11 view[4r+c] (r = 0..3, c = 0..2) at 3r+c; 12..23 proj[4r+j] (j = 0, 1, 3) at 12+3r+{0,1,2};
+// 24..26 campos.  view[3,7,11,15] and proj[2,6,10,14] have no slot: the preprocess never reads them.
+#define GSB_CAM_SLOTS 27
+#define GSB_CAM_ROW 32
 
 // ACC (view-batch accumulation): the sums are formed by the L2 with fire-and-forget reductions (RED.ADD, no value returns to
 // the SM): a load-add-store in the kernel serialises one DRAM round trip per output element behind the previous store.
@@ -53,7 +59,11 @@ __device__ __forceinline__ void warp_store(float* __restrict__ dst, long long ba
 // staged through shared memory with unit-stride loads, overwritten in place by the SH gradients and written back with
 // unit-stride stores; the seven small outputs go through warp_store.  Every output element is written exactly once.
 // MAPS: the render backward also left sum alpha*T*dL/dinvdepth in accumulator slot 9; invdepth = 1/tz adds -slot9/tz^2 to dL/dtz.
-template <bool QUANT, bool ACC, bool MAPS>
+// CAM: also the gradient w.r.t. the camera (DESIGN.md §5d).  Each visible Gaussian keeps the 16 intermediates the camera chain
+// needs (dL/dt, dL/dT, J, the projection terms, the SH direction term of dmean); after the write-back the warp forms the 27 products
+// one at a time and reduces each with an xor butterfly (every lane ends with the same bits), and lane k adds slot k to its running
+// sum.  At the end the CTA sums its 8 warps in warp order into its row of a.cam_rows: no atomics, the same bytes on every run.
+template <bool QUANT, bool ACC, bool MAPS, bool CAM>
 __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs a)
 {
 	extern __shared__ float s_dyn[];
@@ -77,6 +87,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 	// colours given by the caller (override_color): the SH coefficients were not used by the forward, their gradient is zero
 	const bool have_sh = (QUANT || a.shs != nullptr) && a.out.dL_dsh != nullptr && a.colors_precomp == nullptr;
 	const bool have_scales = QUANT || a.scales != nullptr;
+	float cam_sum = 0.f;                                                  // CAM: this warp's running sum of slot `lane`
 	for (long long base = ((long long)blockIdx.x * 8 + warp) * 32; base < a.P; base += (long long)gridDim.x * 8 * 32)
 	{
 		const long long idx = base + lane;
@@ -142,6 +153,10 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 			}
 			if (have_sh) { deg_in = a.degrees[idx]; cl_in = a.g.clamped[idx]; }
 		}
+		// CAM intermediates (zero for culled / invalid lanes): dL/dt, dL/dT0[r], dL/dT1[r], (J00, J02, J11, J12), projection
+		// (g2x*m_w, g2y*m_w, -(g2x*mul1 + g2y*mul2)), SH direction term of dmean
+		float cg_dt[3] = { 0, 0, 0 }, cg_T0[3] = { 0, 0, 0 }, cg_T1[3] = { 0, 0, 0 }, cg_J[4] = { 0, 0, 0, 0 }, cg_p[3] = { 0, 0, 0 };
+		float cg_dir[3] = { 0, 0, 0 };
 		if (!vis)
 		{
 			if (have_sh) for (int k = 0; k < RL; k++) myrow[k] = 0.f;
@@ -216,6 +231,12 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				dmean[0] = v[0] * dL_dtx + v[1] * dL_dty + v[2] * dL_dtz;                // transformVec4x3Transpose
 				dmean[1] = v[4] * dL_dtx + v[5] * dL_dty + v[6] * dL_dtz;
 				dmean[2] = v[8] * dL_dtx + v[9] * dL_dty + v[10] * dL_dtz;
+				if (CAM)
+				{
+					cg_dt[0] = dL_dtx; cg_dt[1] = dL_dty; cg_dt[2] = dL_dtz;
+					cg_T0[0] = dL_dT00; cg_T0[1] = dL_dT01; cg_T0[2] = dL_dT02; cg_T1[0] = dL_dT10; cg_T1[1] = dL_dT11; cg_T1[2] = dL_dT12;
+					cg_J[0] = J00; cg_J[1] = J02; cg_J[2] = J11; cg_J[3] = J12;
+				}
 			}
 			// ---------------- preprocessCUDA, backward.cu:406-423 ----------------
 			{
@@ -227,6 +248,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				dmean[0] += (p[0] * m_w - p[3] * mul1) * g2x + (p[1] * m_w - p[3] * mul2) * g2y;
 				dmean[1] += (p[4] * m_w - p[7] * mul1) * g2x + (p[5] * m_w - p[7] * mul2) * g2y;
 				dmean[2] += (p[8] * m_w - p[11] * mul1) * g2x + (p[9] * m_w - p[11] * mul2) * g2y;
+				if (CAM) { cg_p[0] = g2x * m_w; cg_p[1] = g2y * m_w; cg_p[2] = -(g2x * mul1 + g2y * mul2); }
 			}
 			// ---------------- SH backward, backward.cu:20-172 ----------------
 			if (have_sh)
@@ -297,9 +319,15 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				const float ddz = dRz[0] * dRGB[0] + dRz[1] * dRGB[1] + dRz[2] * dRGB[2];
 				const float sum2 = dox * dox + doy * doy + doz * doz;                       // dnormvdv, auxiliary.h:107-117
 				const float invsum32 = 1.0f / sqrtf(sum2 * sum2 * sum2);
-				dmean[0] += ((+sum2 - dox * dox) * ddx - doy * dox * ddy - doz * dox * ddz) * invsum32;
-				dmean[1] += (-dox * doy * ddx + (sum2 - doy * doy) * ddy - doz * doy * ddz) * invsum32;
-				dmean[2] += (-dox * doz * ddx - doy * doz * ddy + (sum2 - doz * doz) * ddz) * invsum32;
+				const float n0 = (+sum2 - dox * dox) * ddx - doy * dox * ddy - doz * dox * ddz;
+				const float n1 = -dox * doy * ddx + (sum2 - doy * doy) * ddy - doz * doy * ddz;
+				const float n2 = -dox * doz * ddx - doy * doz * ddy + (sum2 - doz * doz) * ddz;
+				dmean[0] += n0 * invsum32;
+				dmean[1] += n1 * invsum32;
+				dmean[2] += n2 * invsum32;
+				// dir = mean - campos.  A product of its own: a second use of n*invsum32 would change how the compiler fuses the
+				// additions above (dL_dmeans3D of the CAM variant then still agrees with CAM = false to rounding only, see gs_b200.h)
+				if (CAM) { cg_dir[0] = __fmul_rn(n0, invsum32); cg_dir[1] = __fmul_rn(n1, invsum32); cg_dir[2] = __fmul_rn(n2, invsum32); }
 			}
 			// ---------------- cov3D -> scale / rotation, backward.cu:311-374 ----------------
 			if (have_scales)
@@ -370,11 +398,94 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 		warp_store<4, ACC>(a.out.dL_drotations, base, n_valid, o_rot, s_tmp, lane);
 		if (a.out.dL_dconic) warp_store<4, ACC>(a.out.dL_dconic, base, n_valid, o_con, s_tmp, lane);
 		__syncwarp();
+		if (CAM && __any_sync(0xffffffffu, vis))
+		{
+			const float m[4] = { vis ? mx : 0.f, vis ? my : 0.f, vis ? mz : 0.f, vis ? 1.f : 0.f };
+			float mine = 0.f;
+#pragma unroll
+			for (int k = 0; k < GSB_CAM_SLOTS; k++)
+			{
+				float c;
+				if (k < 12)
+				{
+					const int r = k / 3, cc = k % 3;
+					c = cg_dt[cc] * m[r];                                             // through t_c = sum_r view[4r+c] m_r
+					if (r < 3)                                                        // direct, through T = W J
+					{
+						if (cc == 0) c += cg_T0[r] * cg_J[0];
+						else if (cc == 1) c += cg_T1[r] * cg_J[2];
+						else c += cg_T0[r] * cg_J[1] + cg_T1[r] * cg_J[3];
+					}
+				}
+				else if (k < 24) c = cg_p[(k - 12) % 3] * m[(k - 12) / 3];
+				else c = -cg_dir[k - 24];
+#pragma unroll
+				for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+				if (lane == k) mine = c;
+			}
+			cam_sum += mine;
+		}
+	}
+	if (CAM)
+	{
+		// every warp is past its last warp_store: its s_tmp is free
+		s_tmp[lane] = cam_sum;
+		__syncthreads();
+		if (threadIdx.x < GSB_CAM_SLOTS)
+		{
+			const float* s0 = s_dyn + (QUANT ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) + 32 * RS + threadIdx.x;
+			float s = 0.f;
+			for (int w = 0; w < 8; w++) s += s0[w * (32 * RS + 32 * 6)];
+			a.cam_rows[(size_t)blockIdx.x * GSB_CAM_ROW + threadIdx.x] = s;
+		}
 	}
 }
 
+// One CTA: the per-CTA rows of preprocess_backward_kernel<.., CAM = true> summed in double, in row order within 8 strided parts and
+// then part order, and scattered into the 4x4 layouts (zeros where the preprocess does not read the matrix).
+__global__ void __launch_bounds__(256) camera_grad_finish_kernel(const float* __restrict__ rows, int n_rows, float* dview, float* dproj,
+	float* dcampos)
+{
+	__shared__ double s_part[8][GSB_CAM_ROW];
+	const int k = threadIdx.x & 31, part = threadIdx.x >> 5;
+	double s = 0.0;
+	if (k < GSB_CAM_SLOTS)
+		for (int r = part; r < n_rows; r += 8) s += (double)rows[(size_t)r * GSB_CAM_ROW + k];
+	s_part[part][k] = s;
+	__syncthreads();
+	if (threadIdx.x < 16)
+	{
+		const int t = threadIdx.x, r = t >> 2, c = t & 3;
+		auto total = [&](int slot) { double v = 0.0; for (int p = 0; p < 8; p++) v += s_part[p][slot]; return (float)v; };
+		if (dview) dview[t] = c == 3 ? 0.f : total(3 * r + c);
+		if (dproj) dproj[t] = c == 2 ? 0.f : total(12 + 3 * r + (c == 3 ? 2 : c));
+		if (dcampos && t < 3) dcampos[t] = total(24 + t);
+	}
+}
+
+static int preprocess_backward_grid(int P)
+{
+	const int need = (P + 255) / 256;
+	return need < GSB_NUM_SMS * 4 ? need : GSB_NUM_SMS * 4;
+}
+
+size_t camera_grad_workspace_bytes(int P)
+{
+	const int rows = P > 0 ? preprocess_backward_grid(P) : 1;
+	return size_t(rows) * GSB_CAM_ROW * sizeof(float);
+}
+
+int launch_camera_grad_finish(int P, const float* rows, float* dview, float* dproj, float* dcampos, cudaStream_t stream)
+{
+	ProfScope prof(K_CAMERA_GRAD, stream);
+	camera_grad_finish_kernel<<<1, 256, 0, stream>>>(rows, P > 0 ? preprocess_backward_grid(P) : 0, dview, dproj, dcampos);
+	GSB_LAUNCHED();
+	GSB_CUDA_OK(cudaGetLastError());
+	return GSB_OK;
+}
+
 int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const int32_t* radii, const float* acc,
-	const GsbGrads* grads, bool maps, float lambda, cudaStream_t stream)
+	const GsbGrads* grads, bool maps, float lambda, float* cam_rows, cudaStream_t stream)
 {
 	BwdArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
@@ -385,22 +496,22 @@ int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const Ge
 	a.shs = s->shs; a.colors_precomp = s->colors_precomp; a.degrees = s->degrees; a.radii = radii;
 	a.view = cam->viewmatrix; a.proj = cam->projmatrix; a.campos = cam->campos;
 	a.quant = s->quant != nullptr; if (s->quant) a.q = *s->quant;
-	a.g = g; a.acc = acc; a.out = *grads;
-	const int need = (s->P + 255) / 256;
-	const int grid = need < GSB_NUM_SMS * 4 ? need : GSB_NUM_SMS * 4;
+	a.g = g; a.acc = acc; a.out = *grads; a.cam_rows = cam_rows;
+	const int grid = preprocess_backward_grid(s->P);
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * s->M + 1) + 32 * 6) * sizeof(float);
 	ProfScope prof(K_PREPROCESS_BWD, stream);
-#define GSB_LAUNCH_PB(Q, A, MP)                                                                                       \
+#define GSB_LAUNCH_PB(Q, A, MP, CM)                                                                                   \
 	do {                                                                                                             \
-		if (int e = ensure_dyn_smem((const void*)preprocess_backward_kernel<Q, A, MP>, 160 * 1024)) return e;          \
-		preprocess_backward_kernel<Q, A, MP><<<grid, 256, smem, stream>>>(a);                                        \
+		if (int e = ensure_dyn_smem((const void*)preprocess_backward_kernel<Q, A, MP, CM>, 160 * 1024)) return e;      \
+		preprocess_backward_kernel<Q, A, MP, CM><<<grid, 256, smem, stream>>>(a);                                    \
 	} while (0)
-#define GSB_LAUNCH_PB_QA(MP)                                                                                         \
+#define GSB_LAUNCH_PB_QA(MP, CM)                                                                                     \
 	do {                                                                                                             \
-		if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(true, true, MP); else GSB_LAUNCH_PB(true, false, MP); }  \
-		else { if (grads->accumulate) GSB_LAUNCH_PB(false, true, MP); else GSB_LAUNCH_PB(false, false, MP); }        \
+		if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(true, true, MP, CM); else GSB_LAUNCH_PB(true, false, MP, CM); }  \
+		else { if (grads->accumulate) GSB_LAUNCH_PB(false, true, MP, CM); else GSB_LAUNCH_PB(false, false, MP, CM); }        \
 	} while (0)
-	if (maps) GSB_LAUNCH_PB_QA(true); else GSB_LAUNCH_PB_QA(false);
+	if (cam_rows) { if (maps) GSB_LAUNCH_PB_QA(true, true); else GSB_LAUNCH_PB_QA(false, true); }
+	else { if (maps) GSB_LAUNCH_PB_QA(true, false); else GSB_LAUNCH_PB_QA(false, false); }
 #undef GSB_LAUNCH_PB_QA
 #undef GSB_LAUNCH_PB
 	GSB_LAUNCHED();

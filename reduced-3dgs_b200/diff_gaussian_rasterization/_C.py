@@ -6,7 +6,8 @@ Build-defined extensions (keyword-only, SURVEY §8(b)): `prune_mask` (u8/bool [P
 (a gs_b200.synth.QuantScene-like object with u8 id planes + [20,256] centres) and `debug_out` (dict that
 receives the forward intermediates in the reference's GeometryState layouts).  `return_maps` (forward) also renders the
 inverse-depth and alpha maps in the same pass; `dL_dinvdepth` / `dL_dalpha` (backward) take their gradients (gs_b200.h
-gsb_forward_maps / gsb_backward_maps).
+gsb_forward_maps / gsb_backward_maps).  `camera_grads` (backward) also returns the gradients w.r.t. viewmatrix, projmatrix and
+campos (gsb_backward_camera).
 """
 from __future__ import annotations
 
@@ -170,12 +171,15 @@ def rasterize_gaussians_variableSH_bands(background, means3D, colors, opacity, s
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                                  projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R,
                                  binningBuffer, imageBuffer, lambda_sh_sparsity, debug, *, prune_mask=None, quant=None,
-                                 accumulate_into=None, want_conic=False, view_means2D=None, dL_dinvdepth=None, dL_dalpha=None):
+                                 accumulate_into=None, want_conic=False, view_means2D=None, dL_dinvdepth=None, dL_dalpha=None,
+                                 camera_grads=False):
     """rasterize_points.h:65-88 RasterizeGaussiansBackwardCUDA ->
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     `accumulate_into`: the same 8-tuple from a previous call; gradients are added in place (view-batch accumulation);
     `view_means2D` ([P,3], accumulate mode): receives THIS view's dL_dmeans2D on its own (per-view densification statistics);
-    `dL_dinvdepth` / `dL_dalpha` ([1,H,W] each, None = zero): gradients of the maps of `return_maps` (gsb_backward_maps)."""
+    `dL_dinvdepth` / `dL_dalpha` ([1,H,W] each, None = zero): gradients of the maps of `return_maps` (gsb_backward_maps);
+    `camera_grads`: the tuple (after dL_dconic when `want_conic`) ends with (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4],
+    dL_dcampos [3]) in the layouts of the inputs (gsb_backward_camera); they are this view's gradients, also with `accumulate_into`."""
     device = _device_of(means3D)
     L = _lib.lib()
     keep = []
@@ -192,10 +196,14 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             if m is not None and m.numel() != H * W:
                 raise RuntimeError(f"dL_dinvdepth / dL_dalpha must have H*W = {H * W} elements, got {m.numel()}")
         keep += dmaps
+        # camera gradients and their workspace ride in the same single allocation as the per-Gaussian outputs
+        cam_shapes = [(4, 4), (4, 4), (3,), ((int(L.gsb_camera_grad_workspace_bytes(P)) + 3) // 4,)] if camera_grads else []
         if accumulate_into is not None:
             outs = list(accumulate_into)
+            cam_out = _carve_f32(device, cam_shapes) if camera_grads else []
         else:
-            outs = _carve_f32(device, [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)])
+            outs = _carve_f32(device, [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)] + cam_shapes)
+            outs, cam_out = outs[:8], outs[8:]
         conic = torch.empty((P, 4), dtype=torch.float32, device=device) if want_conic else None
         if view_means2D is not None and (accumulate_into is None or tuple(view_means2D.shape) != (P, 3) or
                                          view_means2D.dtype != torch.float32 or not view_means2D.is_contiguous()):
@@ -203,7 +211,12 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         g = GsbGrads(ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), ptr(outs[4]), ptr(outs[5]), ptr(outs[6]), ptr(outs[7]),
                      ptr(conic), 1 if accumulate_into is not None else 0, ptr(view_means2D))
         radii = radii.to(device=device, dtype=torch.int32).contiguous()
-        if dmaps[0] is None and dmaps[1] is None:
+        if camera_grads:
+            st = L.gsb_backward_camera(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
+                                       ptr(imageBuffer), ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
+                                       cam_out[0].data_ptr(), cam_out[1].data_ptr(), cam_out[2].data_ptr(), cam_out[3].data_ptr(),
+                                       _lib.current_stream(device))
+        elif dmaps[0] is None and dmaps[1] is None:
             st = L.gsb_backward(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
                                 ptr(imageBuffer), ptr(dL), C.byref(g), float(lambda_sh_sparsity), _lib.current_stream(device))
         else:
@@ -213,9 +226,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         _lib.check(st)
         if debug:
             torch.cuda.synchronize(device)
-    if want_conic:
-        return tuple(outs) + (conic,)
-    return tuple(outs)
+    res = tuple(outs) + ((conic,) if want_conic else ())
+    return res + tuple(cam_out[:3]) if camera_grads else res
 
 
 def calculate_colours_variance(cam_positions, means3D, opacity, scales, rotations, cam_viewmatrices, cam_projmatrices, tan_fovxs,

@@ -5,7 +5,9 @@ _RasterizeGaussians autograd op (:48-167), backed by the H100-native kernels thr
 
 Differences, all additive: GaussianRasterizer.forward takes keyword-only `prune_mask` and `quant`
 (fused resolution-aware prune mask / codebook de-quantisation, SURVEY §8(b)) and `return_maps` (differentiable inverse-depth
-and alpha maps from the same pass: (color, radii, invdepth, alpha)); the forward no longer forces
+and alpha maps from the same pass: (color, radii, invdepth, alpha)); a raster_settings.viewmatrix / projmatrix / campos
+that requires grad receives its gradient (gsb_backward_camera), where the reference silently treats the camera as a
+constant; the forward no longer forces
 debug=True (reference :85 hard-wires a device sync after every stage); gradients are allocated uninitialised
 because the kernels write every element.
 """
@@ -24,14 +26,22 @@ def cpu_deep_copy_tuple(input_tuple):
 
 def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False):
-    return _RasterizeGaussians.apply(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations,
-                                     cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps)
+    args = (means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+            lambda_sh_sparsity, prune_mask, quant, return_maps)
+    camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera):
+        # a learnable camera: the three tensors become inputs of the autograd op so that their gradients have a destination
+        return _RasterizeGaussians.apply(*args, *camera)
+    return _RasterizeGaussians.apply(*args)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False):
+                raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, viewmatrix=None,
+                projmatrix=None, campos=None):
+        # viewmatrix / projmatrix / campos are raster_settings' own tensors, passed again only when the camera is learnable
+        ctx.camera_meta = None if viewmatrix is None else [(t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos)]
         args = (raster_settings.bg, means3D, colors_precomp, opacities, scales, rotations, raster_settings.scale_modifier,
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, raster_settings.image_height, raster_settings.image_width, sh, degrees,
@@ -70,7 +80,9 @@ class _RasterizeGaussians(torch.autograd.Function):
         if grad_out_color is None:
             grad_out_color = torch.zeros((3, raster_settings.image_height, raster_settings.image_width), dtype=torch.float32,
                                          device=means3D.device)
-        maps = dict(dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha)
+        need = ctx.needs_input_grad
+        camera_need = need[14:17] if ctx.camera_meta is not None else (False, False, False)
+        maps = dict(dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need))
         args = (raster_settings.bg, means3D, radii, colors_precomp, scales, rotations, raster_settings.scale_modifier,
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, grad_out_color, sh, degrees, raster_settings.campos, geomBuffer, num_rendered,
@@ -86,7 +98,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         else:
             grads8 = _C.rasterize_gaussians_backward(*args, prune_mask=ctx.prune_mask, quant=ctx.quant, **maps)
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
-         grad_rotations) = grads8
+         grad_rotations) = grads8[:8]
         if ctx.quant is not None:
             # inputs were id planes: the per-Gaussian attribute gradients have no autograd destination; expose them with the
             # semantics of `.grad`: they accumulate over backward calls until the caller resets `quant.grads = None`
@@ -97,11 +109,14 @@ class _RasterizeGaussians(torch.autograd.Function):
                     old[k].add_(g)
             else:
                 ctx.quant.grads = new
-        need = ctx.needs_input_grad
         grads = (grad_means3D, grad_means2D, grad_sh if need[2] else None, None,
                  grad_colors_precomp if need[4] else None, grad_opacities if need[5] else None,
                  grad_scales if need[6] else None, grad_rotations if need[7] else None,
                  grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None)
+        if ctx.camera_meta is not None:
+            grads += tuple(g.reshape(shape).to(dtype) if n else None
+                           for g, n, (shape, dtype) in zip(grads8[8:11] if any(camera_need) else (None,) * 3, camera_need,
+                                                           ctx.camera_meta))
         return grads
 
 

@@ -7,6 +7,11 @@ full_proj_transform, camera_center).
 Build-defined extras: `pc.prune_mask` (optional tensor) and `pc.quant` (optional QuantScene) are forwarded to the
 fused kernels when present; `return_maps=True` adds the inverse-depth and alpha maps of the same pass to the dict
 ("invdepth", "alpha", [1,H,W] each; differentiable except on the variable-SH inference path).
+
+A learnable camera needs no argument: when world_view_transform, full_proj_transform or camera_center requires grad, the
+rasterizer returns their gradients (the variable-SH inference path stays non-differentiable).  The rasterizer takes
+full_proj_transform as its own input, so a camera that builds `full = view @ proj` (and `campos = inverse(view)[3, :3]`) in
+torch gets the gradients of all three paths chained back to its parameters by autograd.
 """
 import math
 import pkgutil

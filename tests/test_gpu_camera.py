@@ -1,0 +1,495 @@
+"""GPU: gradients w.r.t. the camera (viewmatrix, projmatrix, campos; gsb_backward_camera / camera_grads=True).
+  - nothing else moves: with the camera gradients on, the per-Gaussian outputs taken from the accumulator are bit-identical and the
+    computed ones agree to fp32 rounding, and the camera outputs are the same bytes on every run and on any stream;
+  - chain check: the kernel's own screen-space gradients (dL_dmeans2D, dL_dconic, dL_dcolors) chained through a float64 torch
+    restatement of the preprocess w.r.t. view, proj and campos as three independent tensors give the kernel's camera gradients;
+    the same chain applied to the fp64 oracle's screen-space gradients agrees at the oracle gradient bar;
+  - invariance: translating or rotating the whole world together with the camera leaves the image unchanged, so the directional
+    derivative formed from dL_dmeans3D / dL_drotations and the camera gradients vanishes;
+  - maps: the camera gradients of the invdepth and alpha maps equal those of the colour renders that emulate the maps;
+  - end to end: Adam on a 6-vector pose through render() recovers a perturbed camera.
+Observed ratios are printed (pytest -s) so that the bars below can be read against what the kernels actually do."""
+import math
+from types import SimpleNamespace
+
+import numpy as np
+import pytest
+import torch
+
+import ours as O
+from diff_gaussian_rasterization import _C
+from gs_b200 import synth
+from gs_b200.model import GaussianModelView
+
+pytestmark = pytest.mark.gpu
+
+DEV = "cuda"
+F64 = torch.float64
+
+
+def _config(name):
+    """-> (scene, cam, prune_mask or None, quant or None) on the CPU."""
+    if name == "c1":
+        W, H = synth.config_image("C1")
+        return synth.config_scene("C1"), synth.make_camera(W, H), None, None
+    W, H = 320, 200
+    box, ls = (1.9 * W / H, 1.9, 1.0), math.log(0.03)
+    if name == "sh3":
+        return synth.make_scene(20_000, 181, sh_degree=3, box=box, log_scale_mean=ls), _yaw_cam(W, H, 8.0, dev="cpu"), None, None
+    if name == "mixed":
+        return synth.make_scene(20_000, 182, mixed_degrees=True, box=box, log_scale_mean=ls), _yaw_cam(W, H, -5.0, dev="cpu"), None, None
+    if name == "quant":
+        scene = synth.make_scene(20_000, 183, mixed_degrees=True, box=box, log_scale_mean=ls)
+        return scene, _yaw_cam(W, H, 4.0, dev="cpu"), None, synth.quantise_scene(scene)
+    if name == "pruned":
+        scene = synth.make_scene(20_000, 184, sh_degree=2, box=box, log_scale_mean=ls)
+        return scene, _yaw_cam(W, H, -3.0, dev="cpu"), synth.prune_mask(scene.P, 185), None
+    raise ValueError(name)
+
+
+def _yaw_cam(W, H, deg, dev=DEV):
+    th = math.radians(deg)
+    Rc2w = np.array([[math.cos(th), 0, math.sin(th)], [0, 1, 0], [-math.sin(th), 0, math.cos(th)]])
+    C = Rc2w @ np.array([0.0, 0.0, -4.0])
+    return synth.make_camera(W, H, Rc2w, -Rc2w.T @ C).to(dev)
+
+
+def _kw(prune, quant):
+    return dict(prune_mask=None if prune is None else prune.to(DEV), quant=None if quant is None else quant.to(DEV))
+
+
+def _forward(scene, cam, bg, prune, quant, colors=None, maps=False, dbg=None):
+    args = O.forward_args(scene, cam, bg, None if colors is None else {"colors_precomp": colors})
+    out = _C.rasterize_gaussians(*args, return_maps=maps, debug_out=dbg, **_kw(prune, quant))
+    return args, out
+
+
+def _backward(args, out, dL, prune, quant, **extra):
+    (bg, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
+    R, color, radii, geom, binning, img = out[:6]
+    return _C.rasterize_gaussians_backward(bg, means3D, radii, colors, scales, rotations, mod, cov, view, proj, tx, ty, dL.to(DEV), sh,
+                                           degrees, campos, geom, R, binning, img, 0.0, False, **_kw(prune, quant), **extra)
+
+
+def _bits(t):
+    return t.contiguous().view(torch.int32) if t.dtype == torch.float32 else t
+
+
+def _same(a, b):
+    return a.shape == b.shape and torch.equal(_bits(a), _bits(b))
+
+
+# Outputs the preprocess backward copies or scales from the accumulator are bit-identical with the camera gradients on.  The ones
+# it computes through the covariance / SH chains come from a separately compiled kernel (CAM = true), whose multiply-adds the
+# compiler may fuse differently: they agree to fp32 rounding.
+_BITWISE = ("dL_dmeans2D", "dL_dcolors", "dL_dopacity", "dL_dconic")
+
+
+def _close(a, b):
+    return a.shape == b.shape and float((a - b).abs().max()) <= 1e-6 * float(a.abs().max()) + 1e-30
+
+
+# ---- 1. nothing else moves ---------------------------------------------------------------------------------------------------
+# The render backward adds each Gaussian's per-warp sums (one warp = an 8x4 pixel block) into its accumulator with float
+# reductions, in whatever order the warps finish: two backward calls over a larger image agree only to rounding, with or without
+# the camera gradients.  An 8x4 image is one warp block, so there every accumulator receives one addition and two calls must
+# agree bit for bit; with the default 50 degree field of view every Gaussian in the frustum still lands in it.
+
+def _small(name):
+    scene, _, prune, quant = _config({"maps": "mixed", "accumulate": "mixed"}.get(name, name))
+    return scene, _yaw_cam(8, 4, 2.0, dev="cpu"), prune, quant
+
+
+@pytest.mark.parametrize("name", ["c1", "quant", "pruned", "maps", "accumulate"])
+def test_camera_grads_change_nothing_else(name):
+    scene, cam, prune, quant = _small(name)
+    cam = cam.to(DEV)
+    H, W = cam.image_height, cam.image_width
+    g = torch.Generator().manual_seed(170)
+    dL = torch.randn(3, H, W, generator=g).to(DEV)
+    extra = dict(want_conic=True)
+    if name == "maps":
+        extra.update(dL_dinvdepth=torch.randn(1, H, W, generator=g).to(DEV), dL_dalpha=torch.randn(1, H, W, generator=g).to(DEV))
+    bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
+    args, out = _forward(scene, cam, bg, prune, quant, maps=(name == "maps"))
+    assert int((out[2] > 0).sum()) > 1000
+    if name == "accumulate":
+        # two views into one set of buffers; the second call also exports its own dL_dmeans2D
+        args0, out0 = _forward(scene, _yaw_cam(W, H, 3.0), bg, prune, quant)
+        base = _backward(args0, out0, dL, prune, quant)
+        acc_a, acc_b = tuple(t.clone() for t in base), tuple(t.clone() for t in base)
+        v_a, v_b = torch.empty(scene.P, 3, device=DEV), torch.empty(scene.P, 3, device=DEV)
+        plain = _backward(args, out, dL, prune, quant, accumulate_into=acc_a, view_means2D=v_a, **extra)
+        cam1 = _backward(args, out, dL, prune, quant, accumulate_into=acc_b, view_means2D=v_b, camera_grads=True, **extra)
+        assert _same(v_a, v_b)
+        for n, a, b in zip(O.GRAD_NAMES, acc_a, acc_b):
+            assert _same(a, b) if n in _BITWISE else _close(a, b), n
+    else:
+        plain = _backward(args, out, dL, prune, quant, **extra)
+        cam1 = _backward(args, out, dL, prune, quant, camera_grads=True, **extra)
+    assert len(plain) == 9 and len(cam1) == 12
+    for n, a, b in zip(O.GRAD_NAMES + ["dL_dconic"], plain, cam1[:9]):
+        assert _same(a, b) if n in _BITWISE else _close(a, b), n
+    dview, dproj, dcampos = cam1[9:]
+    assert dview.shape == (4, 4) and dproj.shape == (4, 4) and dcampos.shape == (3,)
+    assert torch.isfinite(dview).all() and torch.isfinite(dproj).all() and torch.isfinite(dcampos).all()
+    # entries the preprocess never reads are exactly zero, the others are not
+    assert float(dview[:, 3].abs().max()) == 0.0 and float(dproj[:, 2].abs().max()) == 0.0
+    assert float(dview[:, :3].abs().min()) > 0 and float(dproj[:, [0, 1, 3]].abs().min()) > 0
+    if name == "accumulate":
+        # the camera outputs are this view's: equal to an overwrite-mode call of the same view
+        ref = _backward(args, out, dL, prune, quant, camera_grads=True, **extra)
+        assert all(_same(a, b) for a, b in zip(ref[9:], cam1[9:]))
+        return
+    # the same bytes on a second run and on a non-default stream
+    again = _backward(args, out, dL, prune, quant, camera_grads=True, **extra)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        other = _backward(args, out, dL, prune, quant, camera_grads=True, **extra)
+    torch.cuda.current_stream().wait_stream(s)
+    torch.cuda.synchronize()
+    for a, b, c in zip(cam1[9:], again[9:], other[9:]):
+        assert _same(a, b) and _same(a, c)
+
+
+def test_quant_grads_unchanged_by_a_learnable_camera():
+    from gaussian_renderer import render
+    scene, cam, _, quant = _small("quant")                                   # one warp block: see above
+    cam = cam.to(DEV)
+    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
+    bg = torch.tensor([0.1, 0.2, 0.3], device=DEV)
+    G = synth.grad_image(cam.image_width, cam.image_height, 171).to(DEV)
+    res = []
+    for learn in (False, True):
+        pc = GaussianModelView(scene, DEV, quant=quant)
+        c = SimpleNamespace(**vars(cam))
+        if learn:
+            c.world_view_transform = cam.world_view_transform.clone().requires_grad_(True)
+            c.full_proj_transform = cam.full_proj_transform.clone().requires_grad_(True)
+            c.camera_center = cam.camera_center.clone().requires_grad_(True)
+        pkg = render(c, pc, pipe, bg)
+        (pkg["render"] * G).sum().backward()
+        res.append((pc, pkg, c))
+    (pa, ka, _), (pb, kb, cb) = res
+    assert _same(pa.quant.grads["opacity"], pb.quant.grads["opacity"])
+    for k in ("sh", "scales", "rotations"):
+        assert _close(pa.quant.grads[k], pb.quant.grads[k]), k
+    assert _close(pa._xyz.grad, pb._xyz.grad) and _same(ka["viewspace_points"].grad, kb["viewspace_points"].grad)
+    for t in (cb.world_view_transform, cb.full_proj_transform, cb.camera_center):
+        assert t.grad is not None and t.grad.shape == t.shape and float(t.grad.abs().max()) > 0
+
+
+def test_camera_grads_of_empty_and_fully_culled_scenes():
+    W, H = 100, 60
+    cam = synth.make_camera(W, H).to(DEV)
+    bg = torch.tensor([0.25, 0.5, 0.75], device=DEV)
+    empty = synth.Scene(torch.zeros(0, 3), torch.zeros(0, 1), torch.zeros(0, 3), torch.zeros(0, 4), torch.zeros(0, 1, 3),
+                        torch.zeros(0, 1, dtype=torch.int32))
+    P = 33
+    means = torch.zeros(P, 3)
+    means[:, 2] = -9.0                                                       # behind the camera: every Gaussian is culled, R = 0
+    culled = synth.Scene(means, torch.zeros(P, 1), torch.full((P, 3), 0.1), torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1),
+                         torch.zeros(P, 1, 3), torch.zeros(P, 1, dtype=torch.int32))
+    for scene in (empty, culled):
+        args, out = _forward(scene, cam, bg, None, None)
+        assert out[0] == 0
+        for acc in (False, True):
+            extra = dict(camera_grads=True)
+            if acc:
+                extra["accumulate_into"] = tuple(t.clone() for t in _backward(args, out, torch.ones(3, H, W), None, None))
+            g = _backward(args, out, torch.ones(3, H, W), None, None, **extra)
+            # poison-free check: the camera outputs are written (not left as whatever the allocation held)
+            assert all(float(t.abs().max()) == 0.0 for t in g[8:]), (scene.P, acc)
+            assert [tuple(t.shape) for t in g[8:]] == [(4, 4), (4, 4), (3,)]
+
+
+# ---- 2./3. chain check in float64 --------------------------------------------------------------------------------------------
+
+_C0 = 0.28209479177387814
+_C1 = 0.4886025119029199
+_C2 = [1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396]
+_C3 = [-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658, 1.445305721320277,
+       -0.5900435899266435]
+
+
+def _sh_colour(sh, deg, d):
+    """SH colour + 0.5 of degree deg[i] (forward.cu:20-71), [P,3]; sh [P,M,3], d [P,3] unit directions."""
+    x, y, z = d[:, 0:1], d[:, 1:2], d[:, 2:3]
+    deg = deg.view(-1, 1)
+    M = sh.shape[1]
+    r = _C0 * sh[:, 0]
+    if M > 1:
+        r = r + (deg > 0) * (-_C1 * y * sh[:, 1] + _C1 * z * sh[:, 2] - _C1 * x * sh[:, 3])
+    if M > 4:
+        xx, yy, zz, xy, yz, xz = x * x, y * y, z * z, x * y, y * z, x * z
+        r = r + (deg > 1) * (_C2[0] * xy * sh[:, 4] + _C2[1] * yz * sh[:, 5] + _C2[2] * (2 * zz - xx - yy) * sh[:, 6] +
+                             _C2[3] * xz * sh[:, 7] + _C2[4] * (xx - yy) * sh[:, 8])
+    if M > 9:
+        r = r + (deg > 2) * (_C3[0] * y * (3 * xx - yy) * sh[:, 9] + _C3[1] * xy * z * sh[:, 10] + _C3[2] * y * (4 * zz - xx - yy) * sh[:, 11] +
+                             _C3[3] * z * (2 * zz - 3 * xx - 3 * yy) * sh[:, 12] + _C3[4] * x * (4 * zz - xx - yy) * sh[:, 13] +
+                             _C3[5] * z * (xx - yy) * sh[:, 14] + _C3[6] * x * (xx - 3 * yy) * sh[:, 15])
+    return r + 0.5
+
+
+def _chain(view, proj, campos, W, H, tanx, tany, means, cov3D, sh, deg, clamped, vis, g_m2, g_con, g_col):
+    """Per-Gaussian camera gradients (float64): the screen-space gradients contracted with a torch restatement of the preprocess
+    (t, clamped t, J, T, cov2D + 0.3, conic, ndc, SH colour).  view / proj / campos are independent.  -> ([P,4,4], [P,4,4], [P,3])
+    per visible Gaussian, whose sums are the camera gradients and whose absolute sums are the scales of the bars."""
+    idx = torch.nonzero(vis).view(-1)
+    P = idx.numel()
+    f = lambda t: t.to(device=DEV, dtype=F64)[idx]
+    m, cov, gm, gc = f(means), f(cov3D), f(g_m2), f(g_con)
+    V = view.to(DEV, F64).detach().expand(P, 4, 4).clone().requires_grad_(True)
+    Pm = proj.to(DEV, F64).detach().expand(P, 4, 4).clone().requires_grad_(True)
+    cp = campos.to(DEV, F64).detach().expand(P, 3).clone().requires_grad_(True)
+    mh = torch.cat([m, torch.ones(P, 1, dtype=F64, device=DEV)], 1)
+    t = torch.einsum("pr,prc->pc", mh, V)
+    tx, ty, tz = t[:, 0], t[:, 1], t[:, 2]
+    limx, limy = 1.3 * tanx, 1.3 * tany
+    rx, ry = tx / tz, ty / tz
+    # outside the clamp the backward holds the clamped t constant (its derivative is masked, d/dtz of the clamp is not taken)
+    txc = torch.where((rx >= -limx) & (rx <= limx), tx, (rx.clamp(-limx, limx) * tz).detach())
+    tyc = torch.where((ry >= -limy) & (ry <= limy), ty, (ry.clamp(-limy, limy) * tz).detach())
+    fx, fy = W / (2.0 * tanx), H / (2.0 * tany)
+    J00, J02, J11, J12 = fx / tz, -fx * txc / (tz * tz), fy / tz, -fy * tyc / (tz * tz)
+    Wm = V[:, :3, :3]                                                        # Wm[p, r, k] = view[4r+k]
+    T0 = Wm[:, :, 0] * J00[:, None] + Wm[:, :, 2] * J02[:, None]
+    T1 = Wm[:, :, 1] * J11[:, None] + Wm[:, :, 2] * J12[:, None]
+    S = torch.stack([cov[:, 0], cov[:, 1], cov[:, 2], cov[:, 1], cov[:, 3], cov[:, 4], cov[:, 2], cov[:, 4], cov[:, 5]], 1).view(P, 3, 3)
+    a = torch.einsum("pi,pij,pj->p", T0, S, T0) + 0.3
+    b = torch.einsum("pi,pij,pj->p", T0, S, T1)
+    c = torch.einsum("pi,pij,pj->p", T1, S, T1) + 0.3
+    det = a * c - b * b
+    loss = gc[:, 0] * (c / det) + 2.0 * gc[:, 1] * (-b / det) + gc[:, 3] * (a / det)
+    hom = torch.einsum("pr,prc->pc", mh, Pm)
+    m_w = 1.0 / (hom[:, 3] + 1e-7)
+    loss = loss + gm[:, 0] * hom[:, 0] * m_w + gm[:, 1] * hom[:, 1] * m_w
+    if sh is not None:
+        d = m - cp
+        d = d / d.norm(dim=1, keepdim=True)
+        col = _sh_colour(f(sh), deg.to(DEV)[idx], d)
+        loss = loss + (f(g_col) * col * (1.0 - f(clamped.float()))).sum(1)
+    loss.sum().backward()
+    return V.grad, Pm.grad, cp.grad
+
+
+def _check(got, per, bar, label):
+    """got: kernel (view, proj, campos); per: per-Gaussian contributions.  |got - sum| <= bar * sum |c_i| per entry -> max ratio."""
+    worst = 0.0
+    for n, k, p in zip(("view", "proj", "campos"), got, per):
+        k = k.to(F64).reshape(-1)
+        if p is None:
+            continue
+        p = p.reshape(p.shape[0], -1)
+        tot, scale = p.sum(0), p.abs().sum(0)
+        zero = scale == 0
+        assert float(k[zero].abs().max()) == 0.0 if bool(zero.any()) else True, (label, n)
+        r = ((k - tot).abs() / torch.where(zero, torch.ones_like(scale), scale))[~zero]
+        worst = max(worst, float(r.max()))
+        assert float(r.max()) <= bar, (label, n, float(r.max()), k.tolist(), tot.tolist())
+    print(f"\n[camera chain] {label}: max |kernel - chain| / sum|c_i| = {worst:.3e} (bar {bar:g})")
+    return worst
+
+
+def _kernel_and_chain(name):
+    scene, cam, prune, quant = _config(name)
+    cam = cam.to(DEV)
+    H, W = cam.image_height, cam.image_width
+    bg = torch.tensor([0.2, 0.1, 0.3], device=DEV)
+    dL = synth.grad_image(W, H, 172).to(DEV)
+    dbg = {}
+    args, out = _forward(scene, cam, bg, prune, quant, dbg=dbg)
+    g = _backward(args, out, dL, prune, quant, want_conic=True, camera_grads=True)
+    vis = out[2] > 0
+    sh = scene.sh if scene.sh.shape[1] > 0 else None
+    per = _chain(cam.world_view_transform, cam.full_proj_transform, cam.camera_center, W, H, math.tan(cam.FoVx * 0.5),
+                 math.tan(cam.FoVy * 0.5), scene.means3D, dbg["cov3D"], sh, scene.degrees, dbg["clamped"], vis, g[0], g[8], g[1])
+    return scene, cam, dbg, out, g, per
+
+
+@pytest.mark.parametrize("name", ["c1", "sh3", "mixed", "pruned"])
+def test_camera_grads_are_the_chain_of_the_screen_space_gradients(name):
+    _, _, _, out, g, per = _kernel_and_chain(name)
+    assert int((out[2] > 0).sum()) > 1000
+    _check(g[9:], per, 1e-5, name)
+
+
+def test_camera_grads_against_the_fp64_oracle():
+    import gs_oracle
+    scene, cam = synth.config_scene("C1"), synth.make_camera(*synth.config_image("C1"))
+    H, W = cam.image_height, cam.image_width
+    bg = torch.tensor([0.2, 0.1, 0.3])
+    dL = synth.grad_image(W, H, 173)
+    kw = dict(viewmatrix=cam.world_view_transform, projmatrix=cam.full_proj_transform, campos=cam.camera_center, W=W, H=H,
+              tan_fovx=math.tan(cam.FoVx * 0.5), tan_fovy=math.tan(cam.FoVy * 0.5))
+    o = gs_oracle.forward(scene.means3D, scene.opacity, scene.scales, scene.rotations, scene.sh, scene.degrees, bg=bg, **kw)
+    ob = gs_oracle.backward(o, dL, scene.means3D, scene.scales, scene.rotations, scene.sh, scene.degrees, bg=bg, f64=True, **kw)
+    dbg = {}
+    args, out = _forward(scene, cam.to(DEV), bg.to(DEV), None, None, dbg=dbg)
+    assert np.array_equal(out[2].cpu().numpy(), o["radii"])
+    g = _backward(args, out, dL, None, None, camera_grads=True)
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a))
+    per = _chain(cam.world_view_transform, cam.full_proj_transform, cam.camera_center, W, H, kw["tan_fovx"], kw["tan_fovy"],
+                 scene.means3D, t(o["cov3D"]), scene.sh, scene.degrees, t(o["clamped"]), out[2] > 0, t(ob["dL_dmeans2D"]),
+                 t(ob["dL_dconic"]), t(ob["dL_dcolors"]))
+    _check(g[8:], per, 2e-4, "C1 vs fp64 oracle")
+
+
+# ---- 4. invariance identities ------------------------------------------------------------------------------------------------
+
+def _skew(v):
+    x, y, z = v.tolist()
+    return torch.tensor([[0.0, -z, y], [z, 0.0, -x], [-y, x, 0.0]], dtype=F64, device=DEV)
+
+
+def _qmul(a, b):
+    aw, ax, ay, az = a.unbind(-1)
+    bw, bx, by, bz = b.unbind(-1)
+    return torch.stack([aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
+                        aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw], -1)
+
+
+@pytest.mark.parametrize("name", ["c1", "mixed", "quant"])
+def test_translating_the_world_and_the_camera_together_changes_nothing(name):
+    scene, cam, prune, quant = _config(name)
+    cam = cam.to(DEV)
+    H, W = cam.image_height, cam.image_width
+    args, out = _forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), prune, quant)
+    g = _backward(args, out, synth.grad_image(W, H, 174).to(DEV), prune, quant, camera_grads=True)
+    gm = g[3].to(F64)
+    gv, gp, gc = g[8].to(F64), g[9].to(F64), g[10].to(F64)
+    V, Pf = cam.world_view_transform.to(DEV, F64), cam.full_proj_transform.to(DEV, F64)
+    # means += tau, campos += tau, view[3,:] -= tau . view[:3,:], full_proj[3,:] -= tau . full_proj[:3,:] keep every t and ndc
+    worst = 0.0
+    for k in range(3):
+        terms = [gm[:, k], gc[k:k + 1], -gv[3, :] * V[k, :], -gp[3, :] * Pf[k, :]]
+        s = sum(float(x.sum()) for x in terms)
+        scale = sum(float(x.abs().sum()) for x in terms)
+        worst = max(worst, abs(s) / scale)
+        assert abs(s) <= 1e-5 * scale, (name, k, s, scale)
+    print(f"\n[camera invariance] translation {name}: max |sum| / sum|terms| = {worst:.3e}")
+
+
+def test_rotating_the_world_and_the_camera_together_changes_nothing():
+    scene, cam, _, _ = _config("mixed")
+    cam = cam.to(DEV)
+    H, W = cam.image_height, cam.image_width
+    col = torch.rand(scene.P, 3, generator=torch.Generator().manual_seed(175))
+    args, out = _forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), None, None, colors=col)
+    g = _backward(args, out, synth.grad_image(W, H, 176).to(DEV), None, None, camera_grads=True)
+    gm, gq = g[3].to(F64), g[7].to(F64)
+    gv, gp = g[8].to(F64), g[9].to(F64)
+    m, q = scene.means3D.to(DEV, F64), scene.rotations.to(DEV, F64)
+    V, Pf = cam.world_view_transform.to(DEV, F64), cam.full_proj_transform.to(DEV, F64)
+    # column-vector world rotation R = exp([w]x): means -> R m, quaternions -> q_R (x) q (Sigma -> R Sigma R^T), the first three
+    # rows of both transposed matrices -> R rows (t and ndc unchanged); the derivative at w = 0 along e_k:
+    worst = 0.0
+    for k in range(3):
+        e = torch.zeros(3, dtype=F64, device=DEV)
+        e[k] = 1.0
+        S = _skew(e)
+        dm = m @ S.T                                                         # e_k x m
+        dq = _qmul(torch.cat([torch.zeros(1, dtype=F64, device=DEV), 0.5 * e]).expand_as(q), q)
+        terms = [(gm * dm).sum(1), (gq * dq).sum(1), (gv[:3, :] * (S @ V[:3, :])).reshape(-1), (gp[:3, :] * (S @ Pf[:3, :])).reshape(-1)]
+        s = sum(float(x.sum()) for x in terms)
+        scale = sum(float(x.abs().sum()) for x in terms)
+        worst = max(worst, abs(s) / scale)
+        assert abs(s) <= 1e-5 * scale, (k, s, scale)
+    print(f"\n[camera invariance] rotation: max |sum| / sum|terms| = {worst:.3e}")
+
+
+# ---- 5. maps ------------------------------------------------------------------------------------------------------------------
+
+def test_camera_grads_of_the_maps_equal_those_of_the_colour_emulation():
+    scene, cam, _, _ = _config("mixed")
+    cam = cam.to(DEV)
+    H, W = cam.image_height, cam.image_width
+    g = torch.Generator().manual_seed(177)
+    Gd, Ga = torch.randn(1, H, W, generator=g).to(DEV), torch.randn(1, H, W, generator=g).to(DEV)
+    zero3 = torch.zeros(3, H, W, device=DEV)
+    dbg = {}
+    args, out = _forward(scene, cam, torch.tensor([0.3, 0.1, 0.2], device=DEV), None, None, maps=True, dbg=dbg)
+    vis = out[2] > 0
+    z = dbg["depths"]
+    got_d = _backward(args, out, zero3, None, None, dL_dinvdepth=Gd, camera_grads=True)
+    got_a = _backward(args, out, zero3, None, None, dL_dalpha=Ga, camera_grads=True)
+    # invdepth: colour (1/z, 0, 0) without background, plus the direct term d(1/z_i)/dview[4r+2] = -m_r / z_i^2
+    col = torch.zeros(scene.P, 3)
+    col[:, 0] = torch.where(vis.cpu(), 1.0 / torch.where(vis, z, torch.ones_like(z)).cpu(), torch.zeros(scene.P))
+    ab, ob = _forward(scene, cam, torch.zeros(3, device=DEV), None, None, colors=col)
+    dLb = torch.zeros(3, H, W, device=DEV)
+    dLb[0] = Gd[0]
+    gb = _backward(ab, ob, dLb, None, None, camera_grads=True)
+    m = scene.means3D.to(DEV, F64)[vis]
+    w = (-gb[1][:, 0].to(F64)[vis] / (z.to(F64)[vis] ** 2))
+    direct = torch.zeros(4, 4, dtype=F64, device=DEV)
+    direct[:3, 2] = (w[:, None] * m).sum(0)
+    direct[3, 2] = w.sum()
+    exp_d = (gb[8].to(F64) + direct, gb[9].to(F64), gb[10].to(F64))
+    # alpha: colour 0 with background (-1, 0, 0)
+    ac, oc = _forward(scene, cam, torch.tensor([-1.0, 0.0, 0.0], device=DEV), None, None, colors=torch.zeros(scene.P, 3))
+    dLc = torch.zeros(3, H, W, device=DEV)
+    dLc[0] = Ga[0]
+    gc = _backward(ac, oc, dLc, None, None, camera_grads=True)
+    exp_a = (gc[8].to(F64), gc[9].to(F64), gc[10].to(F64))
+    scale_d = (w.abs()[:, None] * torch.cat([m.abs(), torch.ones_like(w)[:, None]], 1)).sum()
+    for label, got, exp in (("invdepth", got_d[8:], exp_d), ("alpha", got_a[8:], exp_a)):
+        for n, a, e in zip(("view", "proj", "campos"), got, exp):
+            tol = 1e-4 * (float(e.abs().max()) + (float(scale_d) if label == "invdepth" and n == "view" else 0.0)) + 1e-30
+            assert float((a.to(F64) - e).abs().max()) <= tol, (label, n, a.tolist(), e.tolist())
+    assert float(got_d[8][:3, 2].abs().max()) > 0 and float(got_a[8][:3, :3].abs().max()) > 0
+    assert float(got_d[10].abs().max()) == 0.0 and float(got_a[10].abs().max()) == 0.0   # the maps do not depend on the view direction
+
+
+# ---- 6. end to end: pose refinement through render() -------------------------------------------------------------------------
+
+def _pose_camera(xi, W, H, proj_T, fovx, fovy):
+    """Camera from a 6-vector (axis-angle, translation) applied to the default camera (R = I, T = (0, 0, 4)), built in torch the
+    way scene/cameras.py builds it: world_view_transform = [R | T]^T, full = view @ proj, campos = inverse(view)[3, :3]."""
+    w, dt = xi[:3], xi[3:]
+    K = torch.zeros(3, 3, dtype=xi.dtype, device=xi.device)
+    K[0, 1], K[0, 2], K[1, 0], K[1, 2], K[2, 0], K[2, 1] = -w[2], w[1], w[2], -w[0], -w[1], w[0]
+    Rwc = torch.linalg.matrix_exp(K)                                         # world -> camera rotation
+    T = torch.tensor([0.0, 0.0, 4.0], dtype=xi.dtype, device=xi.device) + dt
+    top = torch.cat([Rwc, T[:, None]], 1)
+    Mwc = torch.cat([top, torch.tensor([[0.0, 0.0, 0.0, 1.0]], dtype=xi.dtype, device=xi.device)], 0)
+    view = Mwc.transpose(0, 1)
+    full = view @ proj_T
+    campos = torch.inverse(view)[3, :3]
+    return SimpleNamespace(FoVx=fovx, FoVy=fovy, image_height=H, image_width=W, world_view_transform=view,
+                           full_proj_transform=full, camera_center=campos)
+
+
+def test_pose_refinement_through_render_recovers_the_camera():
+    from gaussian_renderer import render
+    W, H = 256, 192
+    scene = synth.make_scene(8_000, 178, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.05), M=16)
+    base = synth.make_camera(W, H)
+    proj_T = synth._projection(base.znear, base.zfar, base.FoVx, base.FoVy).transpose(0, 1).to(DEV)
+    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
+    bg = torch.zeros(3, device=DEV)
+    pc = GaussianModelView(scene, DEV, requires_grad=False)
+    with torch.no_grad():
+        cam0 = _pose_camera(torch.zeros(6, device=DEV), W, H, proj_T, base.FoVx, base.FoVy)
+        assert torch.allclose(cam0.world_view_transform.cpu(), base.world_view_transform, atol=1e-6)
+        gt = render(cam0, pc, pipe, bg)["render"].clone()
+    # about 1 degree and 3 cm off
+    xi0 = torch.tensor([0.01, -0.012, 0.008, 0.02, -0.015, 0.02], device=DEV)
+    xi = xi0.clone().requires_grad_(True)
+    opt = torch.optim.Adam([xi], lr=2e-3)
+    sched = torch.optim.lr_scheduler.ExponentialLR(opt, gamma=0.985)
+    losses = []
+    for _ in range(200):
+        opt.zero_grad(set_to_none=True)
+        img = render(_pose_camera(xi, W, H, proj_T, base.FoVx, base.FoVy), pc, pipe, bg)["render"]
+        loss = (img - gt).abs().mean()
+        loss.backward()
+        assert xi.grad is not None and torch.isfinite(xi.grad).all() and float(xi.grad.abs().max()) > 0
+        opt.step()
+        sched.step()
+        losses.append(float(loss.detach()))
+    err0, err1 = float(xi0.norm()), float(xi.detach().norm())
+    first, last = sum(losses[:3]) / 3, sum(losses[-3:]) / 3
+    print(f"\n[camera pose] pose error {err0:.4f} -> {err1:.5f}, L1 {first:.5f} -> {last:.6f}")
+    assert err1 < err0 / 5 and last < first / 5, (err0, err1, first, last)
