@@ -210,6 +210,34 @@ GSB_API int gsb_backward_camera(const GsbScene* scene, const GsbCamera* cam, int
                  float lambda_sh_sparsity, float* dL_dviewmatrix /* [16] */, float* dL_dprojmatrix /* [16] */,
                  float* dL_dcampos /* [3] */, char* workspace, void* stream);
 
+/* Anti-aliased rendering (the `antialiasing` option of upstream 3DGS: the Mip-Splatting 2D filter).  The 0.3 px^2 dilation of
+ * cov2D stays; each visible Gaussian's opacity is scaled by s = sqrt(max(2.5e-5, det0 / det1)), det0 = a c - b^2 of the UNDILATED
+ * screen covariance and det1 = (a + 0.3)(c + 0.3) - b^2 of the dilated one, so that its integral no longer grows by
+ * (sigma^2 + 0.3) / sigma^2 when it is smaller than a pixel.  The scaled opacity o^ = sigmoid(logit) * s is what the record, the
+ * 1/255 cull threshold, every pair's alpha and GsbDebug.conic_opacity[:,3] hold.  Radii, tiles, depths, means2D, conic, cov3D, rgb,
+ * clamped, R and the binning are bit-identical to the same call without anti-aliasing; n_contrib, final_T, the colour and the maps
+ * may differ.
+ *   gsb_forward_antialiased:  the arguments of gsb_forward_maps; out_invdepth / out_alpha are optional (both or neither).
+ *   gsb_backward_antialiased: the arguments of gsb_backward_camera, with the map gradients, the camera outputs and the workspace
+ *                             optional as there.  dL_dopacity stays the gradient w.r.t. the raw logit; dL/do^ also reaches cov2D
+ *                             through s, and from there dL_dcov3D, dL_dscales, dL_drotations, dL_dmeans3D and the camera.
+ * The blobs of gsb_forward_antialiased must go to gsb_backward_antialiased, and those of the other forwards to the other backwards:
+ * the blobs do not record the flag (checking it would need a host synchronisation), and a mismatched pair gives wrong gradients
+ * without an error.  P == 0 and R == 0 behave as in gsb_forward_maps / gsb_backward_camera.  gsb_forward_statistics has no
+ * anti-aliased form: the SH-culling statistics keep the reference's definition. */
+GSB_API int gsb_forward_antialiased(const GsbScene* scene, const GsbCamera* cam,
+                gsb_alloc_fn geom_alloc, void* geom_user,
+                gsb_alloc_fn binning_alloc, void* binning_user,
+                gsb_alloc_fn image_alloc, void* image_user,
+                float* out_color, int32_t* radii, int64_t* num_rendered,
+                const GsbDebug* debug, float* out_invdepth /* or NULL */, float* out_alpha /* or NULL */, void* stream);
+GSB_API int gsb_backward_antialiased(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
+                 const char* geom_blob, const char* binning_blob, const char* image_blob,
+                 const float* dL_dout_color /* [3,H,W] */, const GsbGrads* grads,
+                 const float* dL_dinvdepth /* [1,H,W] or NULL */, const float* dL_dalpha /* [1,H,W] or NULL */,
+                 float lambda_sh_sparsity, float* dL_dviewmatrix /* [16] or NULL */, float* dL_dprojmatrix /* [16] or NULL */,
+                 float* dL_dcampos /* [3] or NULL */, char* workspace, void* stream);
+
 /* present[i] = view-space z of means3D[i] > 0.2 (auxiliary.h:139-159). */
 GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);

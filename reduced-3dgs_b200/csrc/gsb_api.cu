@@ -94,7 +94,8 @@ static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter
 	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
-int launch_preprocess(const GsbScene*, const GsbCamera*, const GeomState&, const ImageState&, const BinPlan&, int32_t*, const GsbDebug*, cudaStream_t);
+int launch_preprocess(const GsbScene*, const GsbCamera*, const GeomState&, const ImageState&, const BinPlan&, int32_t*, const GsbDebug*, bool,
+	cudaStream_t);
 int launch_mark_visible(int, const float*, const float*, uint8_t*, cudaStream_t);
 int launch_tile_scan(const ImageState&, const GeomState&, const BinPlan&, int, int, cudaStream_t);
 int launch_scatter_sort(const GeomState&, const BinningState&, const ImageState&, const BinPlan&, int, long long, int, int, cudaStream_t);
@@ -116,7 +117,7 @@ int launch_knn(const float*, long long, int, const int32_t*, long long, const in
 int launch_render_backward(const ImageState&, const BinningState&, const GeomState&, int, int, int, const float*, const float*, const float*,
 	const float*, float*, cudaStream_t);
 int launch_preprocess_backward(const GsbScene*, const GsbCamera*, const GeomState&, const int32_t*, const float*, const GsbGrads*, bool, float,
-	float*, cudaStream_t);
+	float*, bool, cudaStream_t);
 size_t camera_grad_workspace_bytes(int);
 int launch_camera_grad_finish(int, const float*, float*, float*, float*, cudaStream_t);
 
@@ -218,7 +219,7 @@ static thread_local std::map<int, HostSide> t_host;
 static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
 	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
 	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, int32_t* touched_pixels, float* transmittance,
-	float* out_invdepth, float* out_alpha, void* stream_)
+	float* out_invdepth, float* out_alpha, bool aa, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (int e = check_scene(scene, cam)) return e;
@@ -242,7 +243,7 @@ static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_f
 	ImageState img = ImageState::carve(img_blob, W, H, nullptr, plan.priv ? plan.ctas : 0);
 	GSB_CUDA_OK(cudaMemsetAsync(g.counters, 0, 16 * sizeof(uint32_t), stream));
 	if (!plan.priv) GSB_CUDA_OK(cudaMemsetAsync(img.tile_count, 0, ImageState::tiles(W, H) * sizeof(uint32_t), stream));
-	if (int e = launch_preprocess(scene, cam, g, img, plan, radii, debug, stream)) return e;
+	if (int e = launch_preprocess(scene, cam, g, img, plan, radii, debug, aa, stream)) return e;
 	if (int e = launch_tile_scan(img, g, plan, W, H, stream)) return e;
 
 	// The instance count R sizes the binning blob (rasterizer_impl.cu:445-450 reads it back and stalls the device meanwhile).
@@ -292,7 +293,18 @@ int gsb_forward(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_a
 	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, void* stream)
 {
 	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, debug, nullptr, nullptr, nullptr, nullptr, stream);
+		num_rendered, debug, nullptr, nullptr, nullptr, nullptr, false, stream);
+}
+
+int gsb_forward_antialiased(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
+	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
+	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, float* out_invdepth, float* out_alpha, void* stream)
+{
+	if (!scene || scene->P < 0) { set_error("forward_antialiased: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if ((out_invdepth == nullptr) != (out_alpha == nullptr))
+	{ set_error("forward_antialiased: give both map outputs (invdepth and alpha) or neither"); return GSB_EINVAL; }
+	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
+		num_rendered, debug, nullptr, nullptr, out_invdepth, out_alpha, true, stream);
 }
 
 int gsb_forward_maps(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
@@ -302,7 +314,7 @@ int gsb_forward_maps(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn g
 	if (!scene || scene->P < 0) { set_error("forward_maps: scene is NULL or P < 0"); return GSB_EINVAL; }
 	if (!out_invdepth || !out_alpha) { set_error("forward_maps: map output pointers missing"); return GSB_EINVAL; }
 	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, debug, nullptr, nullptr, out_invdepth, out_alpha, stream);
+		num_rendered, debug, nullptr, nullptr, out_invdepth, out_alpha, false, stream);
 }
 
 int gsb_forward_statistics(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
@@ -318,7 +330,7 @@ int gsb_forward_statistics(const GsbScene* scene, const GsbCamera* cam, gsb_allo
 		GSB_CUDA_OK(cudaMemsetAsync(transmittance_sum, 0, size_t(scene->P) * sizeof(float), (cudaStream_t)stream));
 	}
 	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, nullptr, touched_pixels, transmittance_sum, nullptr, nullptr, stream);
+		num_rendered, nullptr, touched_pixels, transmittance_sum, nullptr, nullptr, false, stream);
 }
 
 int gsb_sh_statistics_update(int32_t P, int32_t M, const int32_t* degrees, const float* means3D, const float* campos, const float* shs,
@@ -414,7 +426,7 @@ int gsb_min_redundancy_value(int32_t P, const int32_t* redundancy_values, const 
 static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
 	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
 	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dview, float* dL_dproj, float* dL_dcampos, char* cam_workspace, void* stream_)
+	float* dL_dview, float* dL_dproj, float* dL_dcampos, char* cam_workspace, bool aa, void* stream_)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (int e = check_scene(scene, cam)) return e;
@@ -439,7 +451,7 @@ static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R,
 	float* acc = reinterpret_cast<float*>(const_cast<char*>(geom_blob) + geom_state_bytes(P));
 	if (int e = launch_render_backward(img, b, g, P, W, H, cam->background, dL_dout_color, dL_dinvdepth, dL_dalpha, acc, stream)) return e;
 	float* cam_rows = want_cam ? reinterpret_cast<float*>(cam_workspace) : nullptr;
-	if (int e = launch_preprocess_backward(scene, cam, g, radii, acc, grads, dL_dinvdepth != nullptr, lambda_sh_sparsity, cam_rows, stream))
+	if (int e = launch_preprocess_backward(scene, cam, g, radii, acc, grads, dL_dinvdepth != nullptr, lambda_sh_sparsity, cam_rows, aa, stream))
 		return e;
 	if (want_cam) if (int e = launch_camera_grad_finish(P, cam_rows, dL_dview, dL_dproj, dL_dcampos, stream)) return e;
 	return GSB_OK;
@@ -450,7 +462,7 @@ int gsb_backward(const GsbScene* scene, const GsbCamera* cam, int64_t R, const i
 	const GsbGrads* grads, float lambda_sh_sparsity, void* stream)
 {
 	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, nullptr, nullptr,
-		lambda_sh_sparsity, nullptr, nullptr, nullptr, nullptr, stream);
+		lambda_sh_sparsity, nullptr, nullptr, nullptr, nullptr, false, stream);
 }
 
 size_t gsb_camera_grad_workspace_bytes(int32_t P) { return camera_grad_workspace_bytes(P); }
@@ -464,7 +476,19 @@ int gsb_backward_camera(const GsbScene* scene, const GsbCamera* cam, int64_t R, 
 	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
 	{ set_error("backward_camera: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
 	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, stream);
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, false, stream);
+}
+
+int gsb_backward_antialiased(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
+	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
+	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
+	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, void* stream)
+{
+	if (!scene || scene->P < 0) { set_error("backward_antialiased: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
+	{ set_error("backward_antialiased: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
+	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, true, stream);
 }
 
 int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
@@ -473,7 +497,7 @@ int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t R, co
 {
 	if (!scene || scene->P < 0) { set_error("backward_maps: scene is NULL or P < 0"); return GSB_EINVAL; }
 	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, nullptr, nullptr, nullptr, nullptr, stream);
+		lambda_sh_sparsity, nullptr, nullptr, nullptr, nullptr, false, stream);
 }
 
 int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present, void* stream)

@@ -63,7 +63,9 @@ __device__ __forceinline__ void warp_store(float* __restrict__ dst, long long ba
 // needs (dL/dt, dL/dT, J, the projection terms, the SH direction term of dmean); after the write-back the warp forms the 27 products
 // one at a time and reduces each with an xor butterfly (every lane ends with the same bits), and lane k adds slot k to its running
 // sum.  At the end the CTA sums its 8 warps in warp order into its row of a.cam_rows: no atomics, the same bytes on every run.
-template <bool QUANT, bool ACC, bool MAPS, bool CAM>
+// AA: the forward scaled the opacity by s(cov2D) (DESIGN.md §5e); dL/do^ (accumulator slot 3) also reaches the cov2D through s,
+// before dcov and dL/dT are formed, and from there the 3D covariance, the means through J and, with CAM, the camera.
+template <bool QUANT, bool ACC, bool MAPS, bool CAM, bool AA>
 __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs a)
 {
 	extern __shared__ float s_dyn[];
@@ -177,6 +179,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 			else if (a.cov3D_precomp) { for (int k = 0; k < 6; k++) cov3D[k] = a.cov3D_precomp[6 * idx + k]; }
 			else compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);   // the forward computed exactly this; recomputing is bit-identical
 			float dmean[3], dcov[6];
+			float aa_s = 1.f;                                                 // AA: the opacity factor s, recomputed from cov2D
 			// ---------------- computeCov2DCUDA, backward.cu:177-307 ----------------
 			{
 				const float* v = a.view;
@@ -216,6 +219,31 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 					dcov[4] = 2 * T0[2] * T0[1] * dL_da + (T0[1] * T1[2] + T0[2] * T1[1]) * dL_db + 2 * T1[1] * T1[2] * dL_dc;
 				}
 				else { for (int i = 0; i < 6; i++) dcov[i] = 0; }
+				// AA (the code above stays as it was so that AA = false compiles to the same SASS):  o^ = sigmoid * s, s = sqrt(q),
+				// q = det0 / det1, clamped below at 2.5e-5 (no gradient through q there).  With h = 0.3 and (a, b, c) the UNDILATED
+				// cov2D (b the single off-diagonal parameter): dq/da = h (c^2 + h c + b^2) / det1^2, dq/dc = h (a^2 + h a + b^2) / det1^2,
+				// dq/db = -2 b h (a + c + h) / det1^2, and dL/dq = dL/do^ * sigmoid / (2 s) with sigmoid = o^ / s.  The terms are added
+				// whether or not the conic branch above was taken, and dcov (linear in dL/da, dL/db, dL/dc) is formed again from the sums.
+				if constexpr (AA)
+				{
+					const float ua = TV0[0] * T0[0] + TV0[1] * T0[1] + TV0[2] * T0[2];
+					const float uc = TV1[0] * T1[0] + TV1[1] * T1[1] + TV1[2] * T1[2];
+					const float q = (ua * uc - cb * cb) / denom;
+					aa_s = sqrtf(fmaxf(GSB_AA_MIN_RATIO, q));
+					if (q > GSB_AA_MIN_RATIO)
+					{
+						const float k = acc0.w * (opac / aa_s) * 0.3f / (2.f * aa_s * denom * denom);
+						dL_da += k * (uc * uc + 0.3f * uc + cb * cb);
+						dL_dc += k * (ua * ua + 0.3f * ua + cb * cb);
+						dL_db -= 2.f * cb * k * (ua + uc + 0.3f);
+					}
+					dcov[0] = (T0[0] * T0[0] * dL_da + T0[0] * T1[0] * dL_db + T1[0] * T1[0] * dL_dc);
+					dcov[3] = (T0[1] * T0[1] * dL_da + T0[1] * T1[1] * dL_db + T1[1] * T1[1] * dL_dc);
+					dcov[5] = (T0[2] * T0[2] * dL_da + T0[2] * T1[2] * dL_db + T1[2] * T1[2] * dL_dc);
+					dcov[1] = 2 * T0[0] * T0[1] * dL_da + (T0[0] * T1[1] + T0[1] * T1[0]) * dL_db + 2 * T1[0] * T1[1] * dL_dc;
+					dcov[2] = 2 * T0[0] * T0[2] * dL_da + (T0[0] * T1[2] + T0[2] * T1[0]) * dL_db + 2 * T1[0] * T1[2] * dL_dc;
+					dcov[4] = 2 * T0[2] * T0[1] * dL_da + (T0[1] * T1[2] + T0[2] * T1[1]) * dL_db + 2 * T1[1] * T1[2] * dL_dc;
+				}
 				const float dL_dT00 = 2 * TV0[0] * dL_da + TV1[0] * dL_db, dL_dT01 = 2 * TV0[1] * dL_da + TV1[1] * dL_db, dL_dT02 = 2 * TV0[2] * dL_da + TV1[2] * dL_db;
 				const float dL_dT10 = 2 * TV1[0] * dL_dc + TV0[0] * dL_db, dL_dT11 = 2 * TV1[1] * dL_dc + TV0[1] * dL_db, dL_dT12 = 2 * TV1[2] * dL_dc + TV0[2] * dL_db;
 				// W[c][r] = view[4r + c]
@@ -353,6 +381,8 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 			o_m2[0] = g2x; o_m2[1] = g2y;
 			o_col[0] = acc0.x; o_col[1] = acc0.y; o_col[2] = acc0.z;
 			o_op[0] = acc0.w * (opac * (1.0f - opac));                                    // backward.cu:433
+			// AA: the record holds o^ = sigmoid * s, so dL/dlogit = dL/do^ * s * sigmoid (1 - sigmoid) = dL/do^ * o^ (1 - o^ / s)
+			if constexpr (AA) o_op[0] = acc0.w * (opac * (1.0f - opac / aa_s));
 			for (int k = 0; k < 3; k++) o_m3[k] = dmean[k];
 			for (int k = 0; k < 6; k++) o_cov[k] = dcov[k];
 			o_con[0] = dconx; o_con[1] = dcony; o_con[3] = dconz;
@@ -485,7 +515,7 @@ int launch_camera_grad_finish(int P, const float* rows, float* dview, float* dpr
 }
 
 int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const int32_t* radii, const float* acc,
-	const GsbGrads* grads, bool maps, float lambda, float* cam_rows, cudaStream_t stream)
+	const GsbGrads* grads, bool maps, float lambda, float* cam_rows, bool aa, cudaStream_t stream)
 {
 	BwdArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
@@ -500,18 +530,23 @@ int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const Ge
 	const int grid = preprocess_backward_grid(s->P);
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * s->M + 1) + 32 * 6) * sizeof(float);
 	ProfScope prof(K_PREPROCESS_BWD, stream);
-#define GSB_LAUNCH_PB(Q, A, MP, CM)                                                                                   \
+#define GSB_LAUNCH_PB(Q, A, MP, CM, AA)                                                                               \
 	do {                                                                                                             \
-		if (int e = ensure_dyn_smem((const void*)preprocess_backward_kernel<Q, A, MP, CM>, 160 * 1024)) return e;      \
-		preprocess_backward_kernel<Q, A, MP, CM><<<grid, 256, smem, stream>>>(a);                                    \
+		if (int e = ensure_dyn_smem((const void*)preprocess_backward_kernel<Q, A, MP, CM, AA>, 160 * 1024)) return e;  \
+		preprocess_backward_kernel<Q, A, MP, CM, AA><<<grid, 256, smem, stream>>>(a);                                \
 	} while (0)
-#define GSB_LAUNCH_PB_QA(MP, CM)                                                                                     \
+#define GSB_LAUNCH_PB_QA(MP, CM, AA)                                                                                 \
 	do {                                                                                                             \
-		if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(true, true, MP, CM); else GSB_LAUNCH_PB(true, false, MP, CM); }  \
-		else { if (grads->accumulate) GSB_LAUNCH_PB(false, true, MP, CM); else GSB_LAUNCH_PB(false, false, MP, CM); }        \
+		if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(true, true, MP, CM, AA); else GSB_LAUNCH_PB(true, false, MP, CM, AA); }  \
+		else { if (grads->accumulate) GSB_LAUNCH_PB(false, true, MP, CM, AA); else GSB_LAUNCH_PB(false, false, MP, CM, AA); }        \
 	} while (0)
-	if (cam_rows) { if (maps) GSB_LAUNCH_PB_QA(true, true); else GSB_LAUNCH_PB_QA(false, true); }
-	else { if (maps) GSB_LAUNCH_PB_QA(true, false); else GSB_LAUNCH_PB_QA(false, false); }
+#define GSB_LAUNCH_PB_MC(AA)                                                                                         \
+	do {                                                                                                             \
+		if (cam_rows) { if (maps) GSB_LAUNCH_PB_QA(true, true, AA); else GSB_LAUNCH_PB_QA(false, true, AA); }        \
+		else { if (maps) GSB_LAUNCH_PB_QA(true, false, AA); else GSB_LAUNCH_PB_QA(false, false, AA); }              \
+	} while (0)
+	if (aa) GSB_LAUNCH_PB_MC(true); else GSB_LAUNCH_PB_MC(false);
+#undef GSB_LAUNCH_PB_MC
 #undef GSB_LAUNCH_PB_QA
 #undef GSB_LAUNCH_PB
 	GSB_LAUNCHED();

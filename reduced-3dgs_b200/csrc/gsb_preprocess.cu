@@ -96,7 +96,10 @@ __device__ __forceinline__ void sh_to_rgb(int deg, float x, float y, float z, SH
 #define IDS_REST_ROW 45
 static_assert(32 * IDS_REST_ROW == GSB_IDS_STAGE_BYTES_PER_WARP, "staging buffer size");
 
-template <bool QUANT>
+// AA (anti-aliasing, DESIGN.md §5e): the opacity is scaled by aa_opacity_factor() of the undilated and dilated cov2D, everywhere
+// the forward uses it (record r1.z, the cull threshold pth, the debug export).  Nothing else in the record, radii, rects or depths
+// changes, so binning is the same as without it.
+template <bool QUANT, bool AA>
 __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 {
 	extern __shared__ __align__(16) float s_cb[];   // QUANT: [20][256] centres; scaling row holds exp(centre)
@@ -195,9 +198,11 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 				}
 				opacity = sigmoid_ref(opac_raw);
 				const float tx = xform_row(a.view, 0, px, py, pz), ty = xform_row(a.view, 1, px, py, pz);
-				const float3 cov = compute_cov2D(tx, ty, tz, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, cov3D, a.view);
+				const float3 cov_u = compute_cov2D_undilated(tx, ty, tz, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, cov3D, a.view);
+				const float3 cov = dilate_cov2D(cov_u);
 				const float det = __fmaf_rn(cov.x, cov.z, -__fmul_rn(cov.y, cov.y));   // forward.cu:419
 				if (det == 0.0f) break;
+				if (AA) opacity = __fmul_rn(opacity, aa_opacity_factor(cov_u, det));
 				const float det_inv = __frcp_rn(det);
 				conx = __fmul_rn(cov.z, det_inv); cony = __fmul_rn(-cov.y, det_inv); conz = __fmul_rn(cov.x, det_inv);
 				const float mid = __fmul_rn(0.5f, __fadd_rn(cov.x, cov.z));
@@ -395,7 +400,8 @@ int launch_debug_dequant(const GsbQuant* q, int P, float* scales, float* rots, c
 	return GSB_OK;
 }
 
-int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const ImageState& img, const BinPlan& plan, int32_t* radii, const GsbDebug* dbg, cudaStream_t stream)
+int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const ImageState& img, const BinPlan& plan, int32_t* radii, const GsbDebug* dbg,
+	bool aa, cudaStream_t stream)
 {
 	PreArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
@@ -433,12 +439,14 @@ int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& 
 	const size_t hist_words = plan.priv ? (plan.hist_bytes / 4 + 3) / 4 * 4 : 0;
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE * sizeof(float) : 0) + hist_words * 4 +
 		(a.quant ? size_t(threads / 32) * 32 * IDS_REST_ROW : 0);
-	if (int e = ensure_dyn_smem(a.quant ? (const void*)preprocess_kernel<true> : (const void*)preprocess_kernel<false>, 220 * 1024)) return e;
+	const void* kernel = a.quant ? (aa ? (const void*)preprocess_kernel<true, true> : (const void*)preprocess_kernel<true, false>)
+	                             : (aa ? (const void*)preprocess_kernel<false, true> : (const void*)preprocess_kernel<false, false>);
+	if (int e = ensure_dyn_smem(kernel, 220 * 1024)) return e;
 	ProfScope prof(K_PREPROCESS, stream);
 	int grid = plan.priv ? plan.ctas : blocks_needed;
 	if (!plan.priv && a.quant && grid > GSB_NUM_SMS * 8) grid = GSB_NUM_SMS * 8;                         // persistent: amortise the table load
-	if (a.quant) preprocess_kernel<true><<<grid, threads, smem, stream>>>(a);
-	else preprocess_kernel<false><<<grid, threads, smem, stream>>>(a);
+	if (a.quant) { if (aa) preprocess_kernel<true, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<true, false><<<grid, threads, smem, stream>>>(a); }
+	else { if (aa) preprocess_kernel<false, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<false, false><<<grid, threads, smem, stream>>>(a); }
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;

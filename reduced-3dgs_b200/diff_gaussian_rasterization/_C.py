@@ -7,7 +7,8 @@ Build-defined extensions (keyword-only, SURVEY §8(b)): `prune_mask` (u8/bool [P
 receives the forward intermediates in the reference's GeometryState layouts).  `return_maps` (forward) also renders the
 inverse-depth and alpha maps in the same pass; `dL_dinvdepth` / `dL_dalpha` (backward) take their gradients (gs_b200.h
 gsb_forward_maps / gsb_backward_maps).  `camera_grads` (backward) also returns the gradients w.r.t. viewmatrix, projmatrix and
-campos (gsb_backward_camera).
+campos (gsb_backward_camera).  `antialiasing` (forward and backward, the same value for both) scales each Gaussian's opacity so
+that the 0.3 px^2 dilation no longer inflates sub-pixel splats (gsb_forward_antialiased / gsb_backward_antialiased).
 """
 from __future__ import annotations
 
@@ -96,7 +97,7 @@ def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, 
 
 def _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
              tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug, packed_counts=None,
-             prune_mask=None, quant=None, debug_out=None, statistics=None, return_maps=False):
+             prune_mask=None, quant=None, debug_out=None, statistics=None, return_maps=False, antialiasing=False):
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")          # rasterize_points.cu:158-161
     device = _device_of(means3D)
@@ -128,6 +129,11 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
             st = L.gsb_forward_statistics(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
                                           out_color.data_ptr(), ptr(radii), C.byref(R), ptr(statistics[0]), ptr(statistics[1]),
                                           _lib.current_stream(device))
+        elif antialiasing:
+            st = L.gsb_forward_antialiased(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
+                                           out_color.data_ptr(), ptr(radii), C.byref(R), dbg_ptr,
+                                           maps[0].data_ptr() if maps else None, maps[1].data_ptr() if maps else None,
+                                           _lib.current_stream(device))
         elif maps is not None:
             st = L.gsb_forward_maps(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
                                     out_color.data_ptr(), ptr(radii), C.byref(R), dbg_ptr, maps[0].data_ptr(), maps[1].data_ptr(),
@@ -146,40 +152,42 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
 
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                         projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                        *, prune_mask=None, quant=None, debug_out=None, return_maps=False):
+                        *, prune_mask=None, quant=None, debug_out=None, return_maps=False, antialiasing=False):
     """rasterize_points.h:43-63 RasterizeGaussiansCUDA -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer).
     `return_maps`: -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer, invdepth [1,H,W], alpha [1,H,W]) with
-    invdepth = sum (1/depth) * alpha * T over the pairs that composite the colour and alpha = 1 - final_T (gsb_forward_maps)."""
+    invdepth = sum (1/depth) * alpha * T over the pairs that composite the colour and alpha = 1 - final_T (gsb_forward_maps).
+    `antialiasing`: opacity-compensated 2D filter (gsb_forward_antialiased); its buffers need the backward's `antialiasing=True`."""
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                     projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                    None, prune_mask, quant, debug_out, return_maps=return_maps)
+                    None, prune_mask, quant, debug_out, return_maps=return_maps, antialiasing=antialiasing)
 
 
 def rasterize_gaussians_variableSH_bands(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                                          viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh,
                                          perBandPrimitiveCount, cumSumPrimitiveCount, coeffsNum, degrees, campos, prefiltered,
-                                         debug, *, prune_mask=None, debug_out=None, return_maps=False):
+                                         debug, *, prune_mask=None, debug_out=None, return_maps=False, antialiasing=False):
     """rasterize_points.h:18-41 RasterizeGaussiansVariableSHBandsCUDA (inference, packed per-degree SH groups).
     cumSumPrimitiveCount / coeffsNum are implied by perBandPrimitiveCount ([1,4,9,16] per gaussian_renderer:90-92).
-    `return_maps` as in rasterize_gaussians."""
+    `return_maps` and `antialiasing` as in rasterize_gaussians."""
     counts = [int(v) for v in perBandPrimitiveCount.detach().cpu().tolist()]
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                     projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                    counts, prune_mask, None, debug_out, return_maps=return_maps)
+                    counts, prune_mask, None, debug_out, return_maps=return_maps, antialiasing=antialiasing)
 
 
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                                  projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R,
                                  binningBuffer, imageBuffer, lambda_sh_sparsity, debug, *, prune_mask=None, quant=None,
                                  accumulate_into=None, want_conic=False, view_means2D=None, dL_dinvdepth=None, dL_dalpha=None,
-                                 camera_grads=False):
+                                 camera_grads=False, antialiasing=False):
     """rasterize_points.h:65-88 RasterizeGaussiansBackwardCUDA ->
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     `accumulate_into`: the same 8-tuple from a previous call; gradients are added in place (view-batch accumulation);
     `view_means2D` ([P,3], accumulate mode): receives THIS view's dL_dmeans2D on its own (per-view densification statistics);
     `dL_dinvdepth` / `dL_dalpha` ([1,H,W] each, None = zero): gradients of the maps of `return_maps` (gsb_backward_maps);
     `camera_grads`: the tuple (after dL_dconic when `want_conic`) ends with (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4],
-    dL_dcampos [3]) in the layouts of the inputs (gsb_backward_camera); they are this view's gradients, also with `accumulate_into`."""
+    dL_dcampos [3]) in the layouts of the inputs (gsb_backward_camera); they are this view's gradients, also with `accumulate_into`;
+    `antialiasing`: the backward of a forward with `antialiasing=True` (gsb_backward_antialiased); it must match the forward's flag."""
     device = _device_of(means3D)
     L = _lib.lib()
     keep = []
@@ -204,14 +212,22 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         else:
             outs = _carve_f32(device, [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)] + cam_shapes)
             outs, cam_out = outs[:8], outs[8:]
-        conic = torch.empty((P, 4), dtype=torch.float32, device=device) if want_conic else None
+        # accumulate mode ADDS into every output, this fresh one included: it must start from zero
+        conic = None
+        if want_conic:
+            conic = (torch.zeros if accumulate_into is not None else torch.empty)((P, 4), dtype=torch.float32, device=device)
         if view_means2D is not None and (accumulate_into is None or tuple(view_means2D.shape) != (P, 3) or
                                          view_means2D.dtype != torch.float32 or not view_means2D.is_contiguous()):
             raise RuntimeError("view_means2D needs accumulate_into and a contiguous fp32 [P,3] tensor")
         g = GsbGrads(ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), ptr(outs[4]), ptr(outs[5]), ptr(outs[6]), ptr(outs[7]),
                      ptr(conic), 1 if accumulate_into is not None else 0, ptr(view_means2D))
         radii = radii.to(device=device, dtype=torch.int32).contiguous()
-        if camera_grads:
+        if antialiasing:
+            st = L.gsb_backward_antialiased(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
+                                            ptr(imageBuffer), ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]),
+                                            float(lambda_sh_sparsity), *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4),
+                                            _lib.current_stream(device))
+        elif camera_grads:
             st = L.gsb_backward_camera(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
                                        ptr(imageBuffer), ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
                                        cam_out[0].data_ptr(), cam_out[1].data_ptr(), cam_out[2].data_ptr(), cam_out[3].data_ptr(),

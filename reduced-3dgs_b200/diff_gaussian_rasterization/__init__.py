@@ -7,7 +7,9 @@ Differences, all additive: GaussianRasterizer.forward takes keyword-only `prune_
 (fused resolution-aware prune mask / codebook de-quantisation, SURVEY §8(b)) and `return_maps` (differentiable inverse-depth
 and alpha maps from the same pass: (color, radii, invdepth, alpha)); a raster_settings.viewmatrix / projmatrix / campos
 that requires grad receives its gradient (gsb_backward_camera), where the reference silently treats the camera as a
-constant; the forward no longer forces
+constant; GaussianRasterizationSettings takes upstream 3DGS's trailing `antialiasing` argument (default False; the tuple keeps the
+reference's 12 fields), which turns on the opacity-compensated 2D filter in the forward and the backward; the
+forward no longer forces
 debug=True (reference :85 hard-wires a device sync after every stage); gradients are allocated uninitialised
 because the kernels write every element.
 """
@@ -46,16 +48,17 @@ class _RasterizeGaussians(torch.autograd.Function):
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, raster_settings.image_height, raster_settings.image_width, sh, degrees,
                 raster_settings.campos, raster_settings.prefiltered, raster_settings.debug)
+        fw = dict(prune_mask=prune_mask, quant=quant, return_maps=return_maps, antialiasing=raster_settings.antialiasing)
         if raster_settings.debug:
             cpu_args = cpu_deep_copy_tuple(args)   # Copy them before they can be corrupted (reference :90-97)
             try:
-                out = _C.rasterize_gaussians(*args, prune_mask=prune_mask, quant=quant, return_maps=return_maps)
+                out = _C.rasterize_gaussians(*args, **fw)
             except Exception as ex:
                 torch.save(cpu_args, "snapshot_fw.dump")
                 print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
                 raise ex
         else:
-            out = _C.rasterize_gaussians(*args, prune_mask=prune_mask, quant=quant, return_maps=return_maps)
+            out = _C.rasterize_gaussians(*args, **fw)
         num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = out[:6]
         ctx.raster_settings = raster_settings
         ctx.num_rendered = num_rendered
@@ -82,7 +85,8 @@ class _RasterizeGaussians(torch.autograd.Function):
                                          device=means3D.device)
         need = ctx.needs_input_grad
         camera_need = need[14:17] if ctx.camera_meta is not None else (False, False, False)
-        maps = dict(dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need))
+        maps = dict(dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need),
+                    antialiasing=raster_settings.antialiasing)
         args = (raster_settings.bg, means3D, radii, colors_precomp, scales, rotations, raster_settings.scale_modifier,
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, grad_out_color, sh, degrees, raster_settings.campos, geomBuffer, num_rendered,
@@ -120,7 +124,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         return grads
 
 
-class GaussianRasterizationSettings(NamedTuple):
+class _ReferenceSettings(NamedTuple):
     image_height: int
     image_width: int
     tanfovx: float
@@ -133,6 +137,23 @@ class GaussianRasterizationSettings(NamedTuple):
     campos: torch.Tensor
     prefiltered: bool
     debug: bool
+
+
+class GaussianRasterizationSettings(_ReferenceSettings):
+    """The reference's 12-field settings tuple (its `_fields`, length and positional layout are unchanged) plus upstream 3DGS's
+    trailing `antialiasing` flag, given as a keyword or as a 13th positional argument; default False."""
+    antialiasing = False
+
+    def __new__(cls, *args, antialiasing=False, **kwargs):
+        if len(args) == len(_ReferenceSettings._fields) + 1:
+            *args, antialiasing = args
+        self = super().__new__(cls, *args, **kwargs)
+        self.antialiasing = bool(antialiasing)
+        return self
+
+    def _replace(self, **kwargs):
+        antialiasing = kwargs.pop("antialiasing", self.antialiasing)
+        return type(self)(*super()._replace(**kwargs), antialiasing=antialiasing)
 
 
 class GaussianRasterizer(nn.Module):

@@ -6,7 +6,8 @@ full_proj_transform, camera_center).
 
 Build-defined extras: `pc.prune_mask` (optional tensor) and `pc.quant` (optional QuantScene) are forwarded to the
 fused kernels when present; `return_maps=True` adds the inverse-depth and alpha maps of the same pass to the dict
-("invdepth", "alpha", [1,H,W] each; differentiable except on the variable-SH inference path).
+("invdepth", "alpha", [1,H,W] each; differentiable except on the variable-SH inference path).  `pipe.antialiasing` (upstream
+3DGS's PipelineParams flag; absent = off, as in reduced-3dgs) renders with the opacity-compensated 2D filter, on every path.
 
 A learnable camera needs no argument: when world_view_transform, full_proj_transform or camera_center requires grad, the
 rasterizer returns their gradients (the variable-SH inference path stays non-differentiable).  The rasterizer takes
@@ -68,7 +69,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         image_height=int(viewpoint_camera.image_height), image_width=int(viewpoint_camera.image_width),
         tanfovx=tanfovx, tanfovy=tanfovy, bg=bg_color, scale_modifier=scaling_modifier,
         viewmatrix=viewpoint_camera.world_view_transform, projmatrix=viewpoint_camera.full_proj_transform,
-        sh_degree=pc.active_sh_degree, campos=viewpoint_camera.camera_center, prefiltered=False, debug=pipe.debug)
+        sh_degree=pc.active_sh_degree, campos=viewpoint_camera.camera_center, prefiltered=False, debug=pipe.debug,
+        antialiasing=getattr(pipe, "antialiasing", False))
     rasterizer = GaussianRasterizer(raster_settings=raster_settings)
 
     means3D = pc.get_xyz
@@ -123,7 +125,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
             raster_settings.image_height, raster_settings.image_width, shs, per_band_count, cumsum_count, coeffs_num,
             degrees, raster_settings.campos, raster_settings.prefiltered, raster_settings.debug, prune_mask=prune_mask,
-            return_maps=return_maps)
+            return_maps=return_maps, antialiasing=raster_settings.antialiasing)
         rendered_image, radii = out[1], out[2]
         maps = out[6:]
     else:

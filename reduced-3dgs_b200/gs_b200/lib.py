@@ -140,6 +140,10 @@ def lib():
         L.gsb_backward_camera.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.POINTER(GsbGrads), C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
                                           C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gsb_forward_antialiased.restype = C.c_int
+        L.gsb_forward_antialiased.argtypes = L.gsb_forward_maps.argtypes
+        L.gsb_backward_antialiased.restype = C.c_int
+        L.gsb_backward_antialiased.argtypes = L.gsb_backward_camera.argtypes
         L.gsb_mark_visible.restype = C.c_int
         L.gsb_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_export_binning.restype = C.c_int
@@ -177,7 +181,8 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_sh_statistics_update", "gsb_min_projected_pixel_size", "gsb_sphere_ellipsoid_intersection",
                     "gsb_min_redundancy_value", "gsb_kmeans_workspace_bytes", "gsb_kmeans", "gsb_l1_ssim_blocks",
                     "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn",
-                    "gsb_forward_maps", "gsb_backward_maps", "gsb_camera_grad_workspace_bytes", "gsb_backward_camera"]
+                    "gsb_forward_maps", "gsb_backward_maps", "gsb_camera_grad_workspace_bytes", "gsb_backward_camera",
+                    "gsb_forward_antialiased", "gsb_backward_antialiased"]
 
 
 def check(status: int):

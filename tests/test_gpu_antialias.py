@@ -1,0 +1,614 @@
+"""GPU: anti-aliased rendering (`antialiasing=True`, gsb_forward_antialiased / gsb_backward_antialiased, DESIGN.md §5e).
+  1. nothing else moves: radii, tiles, depths, means2D, conic, cov3D, rgb, clamped, R, sorted keys and point_list are bit-identical
+     with and without anti-aliasing, and without it conic_opacity[:,3] is the plain sigmoid;
+  2. the effective opacity is sigmoid * s, s = sqrt(max(2.5e-5, det0 / det1)), against float64;
+  3. a float64 torch restatement of the whole pipeline (AA preprocess, front-to-back compositing with the reference's skip,
+     saturate and stop rules, the maps) gives the colour, the maps and every gradient, camera included;
+  4. resolution invariance, the point of the feature: one small Gaussian keeps its total alpha across a 4x zoom only with AA;
+  5. equivalences: quantised == de-quantised, pruned == compacted, accumulate == sum of calls, quant.grads accumulates;
+  6. translating / rotating the world together with the camera cancels against the camera gradients;
+  7. the same bytes on every run and stream, P = 0 and R = 0, a second device;
+  8. 90 Adam steps through render() with pipe.antialiasing reduce the loss.
+Observed maxima are printed (pytest -s)."""
+import math
+from types import SimpleNamespace
+
+import numpy as np
+import pytest
+import torch
+
+import ours as O
+from diff_gaussian_rasterization import _C
+from gs_b200 import synth
+from gs_b200.model import GaussianModelView
+
+pytestmark = pytest.mark.gpu
+
+DEV = "cuda"
+F64 = torch.float64
+EMPTY = torch.Tensor([])
+H_DIL = 0.3
+
+
+def _yaw_cam(W, H, deg, dev=DEV):
+    th = math.radians(deg)
+    Rc2w = np.array([[math.cos(th), 0, math.sin(th)], [0, 1, 0], [-math.sin(th), 0, math.cos(th)]])
+    C = Rc2w @ np.array([0.0, 0.0, -4.0])
+    return synth.make_camera(W, H, Rc2w, -Rc2w.T @ C).to(dev)
+
+
+def _config(name):
+    """-> (scene, cam on DEV, prune_mask or None, quant or None)."""
+    if name == "c1":
+        W, H = synth.config_image("C1")
+        return synth.config_scene("C1"), synth.make_camera(W, H).to(DEV), None, None
+    W, H = 320, 200
+    box, ls = (1.9 * W / H, 1.9, 1.0), math.log(0.02)
+    if name == "mixed":
+        return synth.make_scene(20_000, 201, mixed_degrees=True, box=box, log_scale_mean=ls), _yaw_cam(W, H, -5.0), None, None
+    if name == "quant":
+        scene = synth.make_scene(20_000, 202, mixed_degrees=True, box=box, log_scale_mean=ls)
+        return scene, _yaw_cam(W, H, 4.0), None, synth.quantise_scene(scene)
+    if name == "pruned":
+        scene = synth.make_scene(20_000, 203, sh_degree=2, box=box, log_scale_mean=ls)
+        return scene, _yaw_cam(W, H, -3.0), synth.prune_mask(scene.P, 204), None
+    raise ValueError(name)
+
+
+def _kw(prune, quant):
+    return dict(prune_mask=None if prune is None else prune.to(DEV), quant=None if quant is None else quant.to(DEV))
+
+
+def _forward(scene, cam, bg, prune=None, quant=None, aa=True, extra=None, maps=False, dbg=None):
+    args = O.forward_args(scene, cam, bg, extra)
+    return args, _C.rasterize_gaussians(*args, return_maps=maps, debug_out=dbg, antialiasing=aa, **_kw(prune, quant))
+
+
+def _backward(args, out, dL, prune=None, quant=None, aa=True, **extra):
+    (bg, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
+    R, color, radii, geom, binning, img = out[:6]
+    return _C.rasterize_gaussians_backward(bg, means3D, radii, colors, scales, rotations, mod, cov, view, proj, tx, ty, dL.to(DEV), sh,
+                                           degrees, campos, geom, R, binning, img, 0.0, False, antialiasing=aa, **_kw(prune, quant),
+                                           **extra)
+
+
+def _state(out, cam, P):
+    st = _C.export_state(out[3], out[4], out[5], out[0], cam.image_width, cam.image_height, P=P)
+    torch.cuda.synchronize()
+    return st
+
+
+def _bits(t):
+    return t.contiguous().view(torch.int32) if t.dtype == torch.float32 else t
+
+
+def _same(a, b):
+    return a.shape == b.shape and torch.equal(_bits(a), _bits(b))
+
+
+def _rel(a, b):
+    """max |a - b| / max |b|."""
+    a, b = a.to(F64), b.to(F64)
+    return float((a - b).abs().max()) / (float(b.abs().max()) + 1e-30)
+
+
+# ---- 1./2. nothing else moves; the effective opacity --------------------------------------------------------------------------
+
+def _cov2D64(means, cov3D, cam):
+    """Undilated screen covariance (a, b, c) in float64 from the kernel's own cov3D, following computeCov2D."""
+    V = cam.world_view_transform.to(DEV, F64)
+    m = means.to(DEV, F64)
+    t = torch.cat([m, torch.ones(m.shape[0], 1, dtype=F64, device=DEV)], 1) @ V
+    tanx, tany = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
+    fx, fy = cam.image_width / (2.0 * tanx), cam.image_height / (2.0 * tany)
+    tz = t[:, 2]
+    tx = (t[:, 0] / tz).clamp(-1.3 * tanx, 1.3 * tanx) * tz
+    ty = (t[:, 1] / tz).clamp(-1.3 * tany, 1.3 * tany) * tz
+    J00, J02, J11, J12 = fx / tz, -fx * tx / (tz * tz), fy / tz, -fy * ty / (tz * tz)
+    Wm = V[:3, :3]
+    T0 = Wm[None, :, 0] * J00[:, None] + Wm[None, :, 2] * J02[:, None]
+    T1 = Wm[None, :, 1] * J11[:, None] + Wm[None, :, 2] * J12[:, None]
+    c = cov3D.to(DEV, F64)
+    S = torch.stack([c[:, 0], c[:, 1], c[:, 2], c[:, 1], c[:, 3], c[:, 4], c[:, 2], c[:, 4], c[:, 5]], 1).view(-1, 3, 3)
+    return (torch.einsum("pi,pij,pj->p", T0, S, T0), torch.einsum("pi,pij,pj->p", T0, S, T1), torch.einsum("pi,pij,pj->p", T1, S, T1))
+
+
+@pytest.mark.parametrize("name", ["c1", "quant", "pruned"])
+def test_antialiasing_moves_nothing_but_the_opacity(name):
+    scene, cam, prune, quant = _config(name)
+    bg = torch.tensor([0.2, 0.4, 0.6], device=DEV)
+    d0, d1 = {}, {}
+    _, plain = _forward(scene, cam, bg, prune, quant, aa=False, dbg=d0)
+    _, aa = _forward(scene, cam, bg, prune, quant, aa=True, dbg=d1)
+    assert plain[0] == aa[0] and plain[0] > 0 and _same(plain[2], aa[2])
+    for k in ("depths", "means2D", "cov3D", "rgb", "tiles_touched", "clamped"):
+        assert _same(d0[k], d1[k]), k
+    assert _same(d0["conic_opacity"][:, :3], d1["conic_opacity"][:, :3])
+    st0, st1 = _state(plain, cam, scene.P), _state(aa, cam, scene.P)
+    for k in ("keys", "point_list", "ranges"):
+        assert torch.equal(st0[k], st1[k]), k
+    vis = plain[2] > 0
+    logit = (quant.dequantise().opacity if quant is not None else scene.opacity).to(DEV).view(-1)
+    sig = torch.sigmoid(logit.to(F64))
+    # without AA: the plain sigmoid (the kernel's expf sequence is within 2 ulp of it)
+    assert float((d0["conic_opacity"][vis, 3].to(F64) - sig[vis]).abs().max()) <= 3e-7
+    # with AA: sigmoid * s in float64, from the undilated cov2D of the kernel's cov3D
+    a, b, c = _cov2D64(scene.means3D, d1["cov3D"], cam)
+    det0, det1 = a * c - b * b, (a + H_DIL) * (c + H_DIL) - b * b
+    s = torch.sqrt(torch.clamp_min(det0 / det1, 2.5e-5))
+    err = float((d1["conic_opacity"][vis, 3].to(F64) - (sig * s)[vis]).abs().max())
+    print(f"\n[antialias] {name}: max |o^ - sigmoid * s| = {err:.3e} (bar 1e-5); s in [{float(s[vis].min()):.4f}, {float(s[vis].max()):.4f}]")
+    assert err <= 1e-5
+    assert float(s[vis].min()) < 0.5                                           # the scene has sub-pixel splats
+    # lower opacities let more light through on the whole (not at every pixel: near saturation the early stop comes later)
+    assert not torch.equal(plain[1], aa[1]) and float(st1["final_T"].mean()) > float(st0["final_T"].mean())
+
+
+# ---- 3. float64 restatement of the pipeline ----------------------------------------------------------------------------------
+
+_C0 = 0.28209479177387814
+_C1 = 0.4886025119029199
+_C2 = [1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396]
+_C3 = [-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658, 1.445305721320277,
+       -0.5900435899266435]
+
+
+def _sh_colour(sh, deg, d):
+    x, y, z = d[:, 0:1], d[:, 1:2], d[:, 2:3]
+    deg = deg.view(-1, 1)
+    r = _C0 * sh[:, 0]
+    r = r + (deg > 0) * (-_C1 * y * sh[:, 1] + _C1 * z * sh[:, 2] - _C1 * x * sh[:, 3])
+    xx, yy, zz, xy, yz, xz = x * x, y * y, z * z, x * y, y * z, x * z
+    r = r + (deg > 1) * (_C2[0] * xy * sh[:, 4] + _C2[1] * yz * sh[:, 5] + _C2[2] * (2 * zz - xx - yy) * sh[:, 6] +
+                         _C2[3] * xz * sh[:, 7] + _C2[4] * (xx - yy) * sh[:, 8])
+    r = r + (deg > 2) * (_C3[0] * y * (3 * xx - yy) * sh[:, 9] + _C3[1] * xy * z * sh[:, 10] + _C3[2] * y * (4 * zz - xx - yy) * sh[:, 11] +
+                         _C3[3] * z * (2 * zz - 3 * xx - 3 * yy) * sh[:, 12] + _C3[4] * x * (4 * zz - xx - yy) * sh[:, 13] +
+                         _C3[5] * z * (xx - yy) * sh[:, 14] + _C3[6] * x * (xx - 3 * yy) * sh[:, 15])
+    return r + 0.5
+
+
+def _cov3D_from(scales, rots):
+    r, x, y, z = rots.unbind(1)
+    R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y),
+                     2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x),
+                     2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], 1).view(-1, 3, 3)
+    M = R * scales[:, None, :]
+    S = M @ M.transpose(1, 2)
+    return torch.stack([S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1], S[:, 1, 2], S[:, 2, 2]], 1)
+
+
+def _render64(x, cam, bg, vis, tiles):
+    """float64 AA forward of the visible Gaussians.  x: dict of float64 leaves (means, logit, view, proj, campos, and scales + rots or
+    cov3D, sh + deg or colors).  tiles: per 16x16 tile the kernel's depth-sorted Gaussian ids.  -> (colour, invdepth, alpha, n_contrib,
+    intermediates, margins)."""
+    W, H = cam.image_width, cam.image_height
+    tanx, tany = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
+    P = x["means"].shape[0]
+    m = x["means"]
+    mh = torch.cat([m, torch.ones(P, 1, dtype=F64, device=DEV)], 1)
+    t = mh @ x["view"]
+    tx, ty, tz = t[:, 0], t[:, 1], t[:, 2]
+    limx, limy = 1.3 * tanx, 1.3 * tany
+    rx, ry = tx / tz, ty / tz
+    txc = torch.where((rx >= -limx) & (rx <= limx), tx, (rx.clamp(-limx, limx) * tz).detach())
+    tyc = torch.where((ry >= -limy) & (ry <= limy), ty, (ry.clamp(-limy, limy) * tz).detach())
+    fx, fy = W / (2.0 * tanx), H / (2.0 * tany)
+    J00, J02, J11, J12 = fx / tz, -fx * txc / (tz * tz), fy / tz, -fy * tyc / (tz * tz)
+    Wm = x["view"][:3, :3]
+    T0 = Wm[None, :, 0] * J00[:, None] + Wm[None, :, 2] * J02[:, None]
+    T1 = Wm[None, :, 1] * J11[:, None] + Wm[None, :, 2] * J12[:, None]
+    cov = x["cov3D"] if "cov3D" in x else _cov3D_from(x["scales"], x["rots"])
+    S = torch.stack([cov[:, 0], cov[:, 1], cov[:, 2], cov[:, 1], cov[:, 3], cov[:, 4], cov[:, 2], cov[:, 4], cov[:, 5]], 1).view(P, 3, 3)
+    a = torch.einsum("pi,pij,pj->p", T0, S, T0)
+    b = torch.einsum("pi,pij,pj->p", T0, S, T1)
+    c = torch.einsum("pi,pij,pj->p", T1, S, T1)
+    det0 = a * c - b * b
+    A, C = a + H_DIL, c + H_DIL
+    det1 = A * C - b * b
+    con = torch.stack([C / det1, -b / det1, A / det1], 1)
+    o_hat = torch.sigmoid(x["logit"].view(-1)) * torch.sqrt(torch.clamp_min(det0 / det1, 2.5e-5))
+    hom = mh @ x["proj"]
+    m_w = 1.0 / (hom[:, 3] + 1e-7)
+    ndc = hom[:, :2] * m_w[:, None]
+    ndc.retain_grad()
+    pix = torch.stack([((ndc[:, 0] + 1.0) * W - 1.0) * 0.5, ((ndc[:, 1] + 1.0) * H - 1.0) * 0.5], 1)
+    if "colors" in x:
+        rgb = x["colors"]
+    else:
+        d = m - x["campos"]
+        d = d / d.norm(dim=1, keepdim=True)
+        rgb = torch.clamp_min(_sh_colour(x["sh"], x["deg"], d), 0.0)
+        rgb.retain_grad()
+    invd = 1.0 / tz
+    colour = torch.zeros(3, H, W, dtype=F64, device=DEV)
+    invdepth = torch.zeros(H, W, dtype=F64, device=DEV)
+    alpha_map = torch.zeros(H, W, dtype=F64, device=DEV)
+    n_contrib = torch.zeros(H, W, dtype=torch.int64, device=DEV)
+    margin_a, margin_t = math.inf, math.inf
+    gx = (W + 15) // 16
+    for tile, ids in enumerate(tiles):
+        x0, y0 = (tile % gx) * 16, (tile // gx) * 16
+        ys, xs = torch.meshgrid(torch.arange(y0, min(y0 + 16, H), device=DEV), torch.arange(x0, min(x0 + 16, W), device=DEV), indexing="ij")
+        ys, xs = ys.reshape(-1), xs.reshape(-1)
+        if ids.numel() == 0:
+            colour[:, ys, xs] = bg.to(F64)[:, None]
+            continue
+        assert bool(vis[ids].all())
+        dx = pix[ids, 0][None, :] - xs[:, None].to(F64)
+        dy = pix[ids, 1][None, :] - ys[:, None].to(F64)
+        cc = con[ids]
+        power = -0.5 * (cc[:, 0] * dx * dx + cc[:, 2] * dy * dy) - cc[:, 1] * dx * dy
+        raw = o_hat[ids][None, :] * torch.exp(power)
+        # the reference's backward differentiates alpha = o G through the 0.99 clamp
+        alpha = raw + (torch.clamp_max(raw, 0.99) - raw).detach()
+        with torch.no_grad():
+            keep = (power <= 0) & (alpha >= 1.0 / 255.0)
+            margin_a = min(margin_a, float((alpha - 1.0 / 255.0).abs()[power <= 0].min()))
+            a_eff = torch.where(keep, alpha, torch.zeros_like(alpha))
+            test_T = torch.cumprod(1.0 - a_eff, 1)
+            stop = keep & (test_T < 1e-4)
+            done = torch.cumsum(stop.int(), 1) > 0
+            use = keep & ~done
+            margin_t = min(margin_t, float((test_T - 1e-4).abs()[keep].min()))
+            pos = torch.arange(1, ids.numel() + 1, device=DEV)[None, :]
+            n_contrib[ys, xs] = (use * pos).max(1).values
+        a_use = torch.where(use, alpha, torch.zeros_like(alpha))
+        T_after = torch.cumprod(1.0 - a_use, 1)
+        T_before = torch.cat([torch.ones_like(T_after[:, :1]), T_after[:, :-1]], 1)
+        w = a_use * T_before
+        T_final = T_after[:, -1]
+        colour[:, ys, xs] = (w @ rgb[ids]).T + T_final[None, :] * bg.to(F64)[:, None]
+        invdepth[ys, xs] = w @ invd[ids]
+        alpha_map[ys, xs] = 1.0 - T_final
+    return colour, invdepth[None], alpha_map[None], n_contrib, dict(ndc=ndc, rgb=rgb, cov=cov), (margin_a, margin_t)
+
+
+def _tiny_scene(seed, P=48):
+    return synth.make_scene(P, seed, mixed_degrees=True, box=(1.3, 1.3, 0.8), log_scale_mean=math.log(0.05), M=16, near_frac=0.0)
+
+
+@pytest.mark.parametrize("case", ["sh", "colors_precomp", "cov3D_precomp", "maps_only"])
+def test_antialiasing_against_a_float64_restatement(case):
+    W = H = 32
+    scene = _tiny_scene({"sh": 211, "colors_precomp": 212, "cov3D_precomp": 213, "maps_only": 214}[case])
+    cam = _yaw_cam(W, H, 3.0)
+    bg = torch.tensor([0.3, 0.2, 0.1], device=DEV)
+    gen = torch.Generator().manual_seed(215)
+    extra = {}
+    if case == "colors_precomp":
+        extra["colors_precomp"] = torch.rand(scene.P, 3, generator=gen)
+    if case == "cov3D_precomp":
+        extra["cov3D_precomp"] = _cov3D_from(scene.scales.to(F64), scene.rotations.to(F64)).float()
+    dbg = {}
+    args, out = _forward(scene, cam, bg, extra=extra, maps=True, dbg=dbg)
+    Gc = torch.zeros(3, H, W) if case == "maps_only" else torch.randn(3, H, W, generator=gen)
+    Gd, Ga = torch.randn(1, H, W, generator=gen), torch.randn(1, H, W, generator=gen)
+    g = _backward(args, out, Gc, dL_dinvdepth=Gd.to(DEV), dL_dalpha=Ga.to(DEV), camera_grads=True)
+    st = _state(out, cam, scene.P)
+    vis = out[2] > 0
+    assert int(vis.sum()) >= 30
+    tiles = [st["point_list"][int(r0):int(r1)].long() for r0, r1 in st["ranges"].tolist()]
+    leaf = lambda v: v.to(DEV, F64).detach().clone().requires_grad_(True)
+    x = dict(means=leaf(scene.means3D), logit=leaf(scene.opacity), view=leaf(cam.world_view_transform),
+             proj=leaf(cam.full_proj_transform), campos=leaf(cam.camera_center))
+    if "cov3D_precomp" in extra:
+        x["cov3D"] = leaf(extra["cov3D_precomp"])
+    else:
+        x["scales"], x["rots"] = leaf(scene.scales), leaf(scene.rotations)
+    if "colors_precomp" in extra:
+        x["colors"] = leaf(extra["colors_precomp"])
+    else:
+        x["sh"], x["deg"] = leaf(scene.sh), scene.degrees.to(DEV)
+    col, invd, alpha, nc, mid, (margin_a, margin_t) = _render64(x, cam, bg, vis, tiles)
+    # the restatement took the kernel's decisions: the same last contributor everywhere, and no pair near a threshold
+    assert torch.equal(nc, st["n_contrib"].long()), "compositing decisions differ from the kernel's"
+    assert margin_a > 1e-7 and margin_t > 1e-9, (margin_a, margin_t)
+    e_img = max(float((out[1].to(F64) - col.detach()).abs().max()), float((out[6].to(F64) - invd.detach()).abs().max()),
+                float((out[7].to(F64) - alpha.detach()).abs().max()))
+    loss = (col * Gc.to(DEV, F64)).sum() + (invd * Gd.to(DEV, F64)).sum() + (alpha * Ga.to(DEV, F64)).sum()
+    loss.backward()
+    ref = dict(dL_dmeans2D=mid["ndc"].grad, dL_dopacity=x["logit"].grad, dL_dmeans3D=x["means"].grad,
+               view=x["view"].grad, proj=x["proj"].grad, campos=x["campos"].grad)
+    got = dict(dL_dmeans2D=g[0][:, :2], dL_dopacity=g[2], dL_dmeans3D=g[3], view=g[8], proj=g[9], campos=g[10])
+    if "colors" in x:
+        ref["dL_dcolors"], got["dL_dcolors"] = x["colors"].grad, g[1]
+    else:
+        ref["dL_dcolors"], got["dL_dcolors"] = mid["rgb"].grad, g[1]
+        ref["dL_dsh"], got["dL_dsh"] = x["sh"].grad, g[5]
+    if "cov3D" in x:
+        ref["dL_dcov3D"], got["dL_dcov3D"] = x["cov3D"].grad, g[4]
+    else:
+        ref["dL_dscales"], got["dL_dscales"] = x["scales"].grad, g[6]
+        ref["dL_drotations"], got["dL_drotations"] = x["rots"].grad, g[7]
+    # an input the loss does not depend on (campos without SH colours, the colours under a loss on the maps alone) must get zeros
+    zero = [k for k in ref if ref[k] is None or float(ref[k].abs().max()) == 0]
+    for k in zero:
+        assert float(got[k].abs().max()) == 0.0, k
+    errs = {k: _rel(got[k].reshape(ref[k].shape), ref[k]) for k in ref if k not in zero}
+    worst = max(errs.items(), key=lambda kv: kv[1])
+    print(f"\n[antialias fp64] {case}: image/maps max |diff| = {e_img:.3e} (bar 1e-5); worst gradient {worst[0]} {worst[1]:.3e} "
+          f"(bar 2e-4); margins alpha {margin_a:.2e} T {margin_t:.2e}; exactly zero: {zero}")
+    assert e_img <= 1e-5
+    assert len(errs) >= 6
+    for k, e in errs.items():
+        assert e <= 2e-4, (k, e)
+
+
+# ---- 4. resolution invariance -------------------------------------------------------------------------------------------------
+
+def test_total_alpha_of_a_small_gaussian_is_resolution_invariant_only_with_aa():
+    Wh = 256
+    cam_hi, cam_lo = synth.make_camera(Wh, Wh).to(DEV), synth.make_camera(Wh // 4, Wh // 4).to(DEV)
+    focal = Wh / (2.0 * math.tan(cam_hi.FoVx * 0.5))
+    sigma = 2.0 * 4.0 / focal                                                  # 2 px at W, 0.5 px at W / 4 (depth 4)
+    scene = synth.Scene(torch.tensor([[0.0013, -0.0021, 0.0]]), torch.tensor([[math.log(0.9 / 0.1)]]), torch.full((1, 3), sigma),
+                        torch.tensor([[1.0, 0.0, 0.0, 0.0]]), torch.zeros(1, 1, 3), torch.zeros(1, 1, dtype=torch.int32))
+    bg = torch.zeros(3, device=DEV)
+    total = {}
+    for aa in (False, True):
+        for label, cam in (("hi", cam_hi), ("lo", cam_lo)):
+            dbg = {}
+            _, out = _forward(scene, cam, bg, aa=aa, maps=True, dbg=dbg)
+            a = out[7][0].to(F64)
+            # per pixel: min(0.99, o^ exp(power)), cut below 1/255, from the kernel's own conic / means2D / o^ in float64
+            co, mu = dbg["conic_opacity"][0].to(F64), dbg["means2D"][0].to(F64)
+            ys, xs = torch.meshgrid(torch.arange(cam.image_height, device=DEV, dtype=F64),
+                                    torch.arange(cam.image_width, device=DEV, dtype=F64), indexing="ij")
+            dx, dy = mu[0] - xs, mu[1] - ys
+            raw = co[3] * torch.exp(-0.5 * (co[0] * dx * dx + co[2] * dy * dy) - co[1] * dx * dy)
+            exp = torch.where(raw >= 1.0 / 255.0, torch.clamp_max(raw, 0.99), torch.zeros_like(raw))
+            near_cut = (raw - 1.0 / 255.0).abs() < 1e-5
+            assert float((a - exp).abs()[~near_cut].max()) <= 2e-6, (aa, label)
+            total[(aa, label)] = float(a.sum())
+    r_aa = 16.0 * total[(True, "lo")] / total[(True, "hi")]
+    r_plain = 16.0 * total[(False, "lo")] / total[(False, "hi")]
+    print(f"\n[antialias] 16 sum(alpha_lo) / sum(alpha_hi): with AA {r_aa:.4f}, without {r_plain:.4f}")
+    assert abs(r_aa - 1.0) <= 0.03
+    assert r_plain > 1.5
+
+
+# ---- 5. equivalences ----------------------------------------------------------------------------------------------------------
+# Backward comparisons use an 8x4 image: one warp block, where the render backward's accumulator receives one addition per
+# Gaussian, so two calls agree bit for bit and only the kernels' own arithmetic can differ (see test_gpu_camera.py).
+
+def _small(name):
+    scene, _, prune, quant = _config(name)
+    return scene, _yaw_cam(8, 4, 2.0), prune, quant
+
+
+def _grads_close(a, b, bar=1e-6):
+    return all(_rel(x, y) <= bar if float(y.abs().max()) > 0 else float(x.abs().max()) == 0 for x, y in zip(a, b))
+
+
+def test_quantised_aa_equals_dequantised_aa():
+    scene, cam, _, quant = _small("quant")
+    dense = quant.to(DEV).dequantise()                       # on the GPU, as the reference flow does (load_ply)
+    bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
+    G = torch.randn(3, 4, 8, generator=torch.Generator().manual_seed(221))
+    Gd = torch.randn(1, 4, 8, generator=torch.Generator().manual_seed(222)).to(DEV)
+    aq, oq = _forward(scene, cam, bg, quant=quant, maps=True)
+    ad, od = _forward(dense, cam, bg, maps=True)
+    assert int((oq[2] > 0).sum()) > 1000
+    for i in (0, 1, 2, 6, 7):
+        assert oq[i] == od[i] if i == 0 else _same(oq[i], od[i]), i
+    gq = _backward(aq, oq, G, quant=quant, dL_dinvdepth=Gd)
+    gd = _backward(ad, od, G, dL_dinvdepth=Gd)
+    assert _grads_close(gq, gd)
+
+
+def test_pruned_aa_equals_compacted_aa():
+    scene, cam, prune, _ = _small("pruned")
+    keep = prune == 0
+    bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
+    G = torch.randn(3, 4, 8, generator=torch.Generator().manual_seed(223))
+    ap, op = _forward(scene, cam, bg, prune=prune, maps=True)
+    ac, oc = _forward(scene.compact(keep), cam, bg, maps=True)
+    assert op[0] == oc[0] and op[0] > 0
+    for i in (1, 6, 7):
+        assert _same(op[i], oc[i]), i
+    gp = _backward(ap, op, G, prune=prune)
+    gc = _backward(ac, oc, G)
+    kd = keep.to(DEV)
+    assert _grads_close([t[kd] for t in gp], gc)
+    assert all(float(t[~kd].abs().max()) == 0 for t in gp if t.numel())
+
+
+def test_aa_accumulate_equals_the_sum_of_two_calls_and_quant_grads_accumulate():
+    scene, cam, _, _ = _small("mixed")
+    cam2 = _yaw_cam(8, 4, 3.5)
+    bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
+    G = torch.randn(3, 4, 8, generator=torch.Generator().manual_seed(224))
+    a1, o1 = _forward(scene, cam, bg)
+    a2, o2 = _forward(scene, cam2, bg)
+    g1, g2 = _backward(a1, o1, G), _backward(a2, o2, G)
+    acc = tuple(t.clone() for t in g1)
+    _backward(a2, o2, G, accumulate_into=acc)
+    assert _grads_close(acc, [x + y for x, y in zip(g1, g2)])
+    # quant.grads accumulate over backward calls through render() with pipe.antialiasing
+    from gaussian_renderer import render
+    qscene, qcam, _, quant = _small("quant")
+    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False, antialiasing=True)
+    pc = GaussianModelView(qscene, DEV, quant=quant)
+    Gq = G.to(DEV)
+    (render(qcam, pc, pipe, bg)["render"] * Gq).sum().backward()
+    first = {k: v.clone() for k, v in pc.quant.grads.items()}
+    (render(qcam, pc, pipe, bg)["render"] * Gq).sum().backward()
+    for k, v in pc.quant.grads.items():
+        assert float(first[k].abs().max()) > 0 and _rel(v, 2 * first[k]) <= 1e-6, k
+    # and they are the AA gradients: they equal the raw entry point's
+    aq, oq = _forward(qscene, qcam, bg, quant=quant)
+    gq = _backward(aq, oq, G, quant=quant)
+    assert _rel(first["opacity"], gq[2]) <= 1e-6 and _rel(first["scales"], gq[6]) <= 1e-6
+
+
+# ---- 6. camera through AA -----------------------------------------------------------------------------------------------------
+
+@pytest.mark.parametrize("name", ["c1", "quant"])
+def test_aa_translation_invariance_with_the_camera(name):
+    scene, cam, prune, quant = _config(name)
+    H, W = cam.image_height, cam.image_width
+    args, out = _forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), prune, quant)
+    g = _backward(args, out, synth.grad_image(W, H, 225).to(DEV), prune, quant, camera_grads=True)
+    gm, gv, gp, gc = g[3].to(F64), g[8].to(F64), g[9].to(F64), g[10].to(F64)
+    V, Pf = cam.world_view_transform.to(DEV, F64), cam.full_proj_transform.to(DEV, F64)
+    worst = 0.0
+    for k in range(3):
+        terms = [gm[:, k], gc[k:k + 1], -gv[3, :] * V[k, :], -gp[3, :] * Pf[k, :]]
+        s, scale = sum(float(x.sum()) for x in terms), sum(float(x.abs().sum()) for x in terms)
+        worst = max(worst, abs(s) / scale)
+        assert abs(s) <= 1e-5 * scale, (name, k, s, scale)
+    print(f"\n[antialias camera] translation {name}: max |sum| / sum|terms| = {worst:.3e}")
+
+
+def _skew(v):
+    x, y, z = v.tolist()
+    return torch.tensor([[0.0, -z, y], [z, 0.0, -x], [-y, x, 0.0]], dtype=F64, device=DEV)
+
+
+def _qmul(a, b):
+    aw, ax, ay, az = a.unbind(-1)
+    bw, bx, by, bz = b.unbind(-1)
+    return torch.stack([aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
+                        aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw], -1)
+
+
+def test_aa_rotation_invariance_with_the_camera():
+    scene, cam, _, _ = _config("mixed")
+    H, W = cam.image_height, cam.image_width
+    col = torch.rand(scene.P, 3, generator=torch.Generator().manual_seed(226))
+    args, out = _forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), extra={"colors_precomp": col})
+    g = _backward(args, out, synth.grad_image(W, H, 227).to(DEV), camera_grads=True)
+    gm, gq, gv, gp = g[3].to(F64), g[7].to(F64), g[8].to(F64), g[9].to(F64)
+    m, q = scene.means3D.to(DEV, F64), scene.rotations.to(DEV, F64)
+    V, Pf = cam.world_view_transform.to(DEV, F64), cam.full_proj_transform.to(DEV, F64)
+    worst = 0.0
+    for k in range(3):
+        e = torch.zeros(3, dtype=F64, device=DEV)
+        e[k] = 1.0
+        S = _skew(e)
+        dq = _qmul(torch.cat([torch.zeros(1, dtype=F64, device=DEV), 0.5 * e]).expand_as(q), q)
+        terms = [(gm * (m @ S.T)).sum(1), (gq * dq).sum(1), (gv[:3, :] * (S @ V[:3, :])).reshape(-1), (gp[:3, :] * (S @ Pf[:3, :])).reshape(-1)]
+        s, scale = sum(float(x.sum()) for x in terms), sum(float(x.abs().sum()) for x in terms)
+        worst = max(worst, abs(s) / scale)
+        assert abs(s) <= 1e-5 * scale, (k, s, scale)
+    print(f"\n[antialias camera] rotation: max |sum| / sum|terms| = {worst:.3e}")
+
+
+# ---- 7. determinism and edges -------------------------------------------------------------------------------------------------
+
+def test_aa_is_deterministic_on_any_stream():
+    scene, _, _, _ = _config("mixed")
+    bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
+    big = _yaw_cam(320, 200, 1.0)
+    _, f1 = _forward(scene, big, bg, maps=True)
+    _, f2 = _forward(scene, big, bg, maps=True)
+    assert all(_same(f1[i], f2[i]) for i in (1, 2, 6, 7))
+    cam = _yaw_cam(8, 4, 2.0)
+    G = torch.randn(3, 4, 8, generator=torch.Generator().manual_seed(228)).to(DEV)
+    args, out = _forward(scene, cam, bg, maps=True)
+    kw = dict(dL_dalpha=torch.ones(1, 4, 8, device=DEV), camera_grads=True)
+    first = _backward(args, out, G, **kw)
+    again = _backward(args, out, G, **kw)
+    s = torch.cuda.Stream()
+    s.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(s):
+        a3, o3 = _forward(scene, cam, bg, maps=True)
+        other = _backward(a3, o3, G, **kw)
+    torch.cuda.current_stream().wait_stream(s)
+    torch.cuda.synchronize()
+    assert _same(o3[1], out[1]) and _same(o3[7], out[7])
+    for a, b, c in zip(first, again, other):
+        assert _same(a, b) and _same(a, c)
+
+
+def test_aa_empty_and_fully_culled_scenes_give_zeros():
+    W, H = 100, 60
+    cam = synth.make_camera(W, H).to(DEV)
+    bg = torch.tensor([0.25, 0.5, 0.75], device=DEV)
+    empty = synth.Scene(torch.zeros(0, 3), torch.zeros(0, 1), torch.zeros(0, 3), torch.zeros(0, 4), torch.zeros(0, 1, 3),
+                        torch.zeros(0, 1, dtype=torch.int32))
+    P = 33
+    means = torch.zeros(P, 3)
+    means[:, 2] = -9.0                                                          # behind the camera: R = 0
+    culled = synth.Scene(means, torch.zeros(P, 1), torch.full((P, 3), 0.1), torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1),
+                         torch.zeros(P, 1, 3), torch.zeros(P, 1, dtype=torch.int32))
+    for scene in (empty, culled):
+        args, out = _forward(scene, cam, bg, maps=True)
+        assert out[0] == 0 and float(out[6].abs().max()) == 0.0 and float(out[7].abs().max()) == 0.0
+        g = _backward(args, out, torch.ones(3, H, W), camera_grads=True, dL_dalpha=torch.ones(1, H, W, device=DEV))
+        assert all(float(t.abs().max()) == 0.0 for t in g if t.numel()), scene.P
+
+
+@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs a second GPU")
+def test_aa_on_a_second_device():
+    scene, _, _, _ = _small("mixed")
+    bg = torch.tensor([0.1, 0.3, 0.2])
+    outs = []
+    for dev in ("cuda:0", "cuda:1"):
+        cam = _yaw_cam(8, 4, 2.0, dev=dev)
+        args = O.forward_args(scene, cam, bg, dev=dev)
+        out = _C.rasterize_gaussians(*args, antialiasing=True)
+        (bgd, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
+        g = _C.rasterize_gaussians_backward(bgd, means3D, out[2], colors, scales, rotations, mod, cov, view, proj, tx, ty,
+                                            torch.ones(3, H, W, device=dev), sh, degrees, campos, out[3], out[0], out[4], out[5], 0.0,
+                                            False, antialiasing=True)
+        outs.append((out[1].cpu(), [t.cpu() for t in g]))
+    assert _same(outs[0][0], outs[1][0])
+    assert all(_same(a, b) for a, b in zip(outs[0][1], outs[1][1]))
+
+
+# ---- 8. training --------------------------------------------------------------------------------------------------------------
+
+class _Model:
+    def __init__(self, scene, dev):
+        self._xyz = scene.means3D.to(dev).clone().requires_grad_(True)
+        self._opacity = scene.opacity.to(dev).clone().requires_grad_(True)
+        self._log_scaling = torch.log(scene.scales.to(dev)).requires_grad_(True)
+        self._rotation = scene.rotations.to(dev).clone().requires_grad_(True)
+        self._features = scene.sh.to(dev).clone().requires_grad_(True)
+        self._degrees = scene.degrees.to(dev)
+        self.active_sh_degree = self.max_sh_degree = 3
+        self.per_band_count = [int((scene.degrees == d).sum()) for d in range(4)]
+
+    get_xyz = property(lambda s: s._xyz)
+    get_scaling = property(lambda s: torch.exp(s._log_scaling))
+    get_rotation = property(lambda s: torch.nn.functional.normalize(s._rotation))
+    get_features = property(lambda s: s._features)
+
+    def params(self):
+        return [self._xyz, self._opacity, self._log_scaling, self._rotation, self._features]
+
+
+def test_adam_steps_with_antialiasing_reduce_the_loss():
+    from gaussian_renderer import render
+    from utils.loss_utils import l1_ssim_loss
+    W, H = 256, 192
+    target = synth.make_scene(6_000, 231, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.02), M=16)
+    cams = [_yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
+    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False, antialiasing=True)
+    bg = torch.tensor([0.1, 0.1, 0.1], device=DEV)
+    with torch.no_grad():
+        gts = [render(c, _Model(target, DEV), pipe, bg)["render"].clone() for c in cams]
+    g = torch.Generator().manual_seed(232)
+    start = synth.Scene(target.means3D + 0.01 * torch.randn(target.means3D.shape, generator=g),
+                        target.opacity + 0.5 * torch.randn(target.opacity.shape, generator=g),
+                        target.scales * torch.exp(0.2 * torch.randn(target.scales.shape, generator=g)),
+                        torch.nn.functional.normalize(target.rotations + 0.1 * torch.randn(target.rotations.shape, generator=g)),
+                        target.sh + 0.1 * torch.randn(target.sh.shape, generator=g), target.degrees)
+    model = _Model(start, DEV)
+    opt = torch.optim.Adam([{"params": [model._xyz], "lr": 2e-4}, {"params": [model._opacity], "lr": 5e-2},
+                            {"params": [model._log_scaling], "lr": 5e-3}, {"params": [model._rotation], "lr": 1e-3},
+                            {"params": [model._features], "lr": 1e-2}])
+    losses = []
+    for it in range(90):
+        k = it % len(cams)
+        opt.zero_grad(set_to_none=True)
+        loss = l1_ssim_loss(render(cams[k], model, pipe, bg)["render"], gts[k], 0.2)
+        loss.backward()
+        for p in model.params():
+            assert p.grad is not None and torch.isfinite(p.grad).all()
+        opt.step()
+        losses.append(float(loss.detach()))
+    first, last = sum(losses[:3]) / 3, sum(losses[-3:]) / 3
+    print(f"\n[antialias training] loss {first:.4f} -> {last:.4f}")
+    assert last < 0.8 * first, (first, last)
