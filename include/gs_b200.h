@@ -323,6 +323,37 @@ GSB_API int gsb_l1_ssim_backward(const float* image, const float* gt, int32_t ch
                 const float* maps, float coef_l1, const float* upstream_l1, float coef_ssim, const float* upstream_ssim,
                 float* dL_dimage, void* stream);
 
+/* ---- optimizer step (gs_b200.optim.GaussianAdam) ----
+ *
+ * One Adam step over a table of fp32 tensors, with the arithmetic of torch.optim.Adam's default (foreach) CUDA path, so that
+ * param / exp_avg / exp_avg_sq are bit-identical to it (DESIGN.md §5f).  Per entry (scalars are the fp32 casts of the values
+ * torch computes in double on the host: one_minus_beta1 = 1 - beta1, one_minus_beta2 = 1 - beta2,
+ * bc2_sqrt = (1 - beta2^step)^0.5, step_size = -(lr / (1 - beta1^step))):
+ *   m = lerp(m, g, one_minus_beta1);  v = v * beta2;  v = v + one_minus_beta2 * (g * g);
+ *   p = p + step_size * (m / (sqrt(v) / bc2_sqrt + eps)).
+ * Sparse modes.  With visibility [P] (u8, nonzero = update) and / or degrees [P] (int32, clamped to 0..3) every tensor is a
+ * [P, row_width] matrix (numel == P * row_width) and element (i, c) is updated only if visibility[i] and, for an entry with
+ * sh_offset = k >= 0 (an [P, C, 3] SH tensor whose column c / 3 is SH coefficient k + c / 3), only if k + c / 3 < (degrees[i] + 1)^2.
+ * Skipped elements are neither read nor written.  Both NULL = dense: every element is updated and P is not read.
+ * Any contiguous fp32 storage works (128-bit accesses where param, grad and both moments share their 16-byte alignment).
+ * All tensors of one call take one kernel launch; none when no element exists.  No host synchronisation; deterministic.
+ * Errors (GSB_EINVAL, nothing launched): tensors NULL with n > 0, n outside 0..GSB_ADAM_MAX_TENSORS, P < 0, numel < 0, a NULL
+ * pointer of a non-empty entry, sh_offset < -1, sh_offset >= 0 with row_width not a positive multiple of 3, and in a sparse
+ * mode row_width <= 0 or numel != P * row_width. */
+#define GSB_ADAM_MAX_TENSORS 16
+typedef struct GsbAdamTensor {
+	float* param;
+	const float* grad;
+	float* exp_avg;
+	float* exp_avg_sq;
+	int64_t numel;
+	int32_t row_width;        /* elements per row (numel / P); used in the sparse modes                                    */
+	int32_t sh_offset;        /* -1: not banded; k >= 0: SH coefficient of column 0 (the reference's f_rest: 1, f_dc: 0)    */
+	float one_minus_beta1, beta2, one_minus_beta2, eps, bc2_sqrt, step_size;
+} GsbAdamTensor;
+GSB_API int gsb_adam_step(const GsbAdamTensor* tensors, int32_t n, int32_t P, const uint8_t* visibility /* NULL = all */,
+                const int32_t* degrees /* NULL = all bands */, void* stream);
+
 /* Number of kernels this library has launched since load (bench.py reports it as gpu_launches). */
 GSB_API uint64_t gsb_launch_count(void);
 

@@ -50,6 +50,16 @@ class GsbGrads(C.Structure):
                 ("accumulate", C.c_int32), ("dL_dmeans2D_view", C.c_void_p)]
 
 
+class GsbAdamTensor(C.Structure):
+    _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
+                ("numel", C.c_int64), ("row_width", C.c_int32), ("sh_offset", C.c_int32), ("one_minus_beta1", C.c_float),
+                ("beta2", C.c_float), ("one_minus_beta2", C.c_float), ("eps", C.c_float), ("bc2_sqrt", C.c_float),
+                ("step_size", C.c_float)]
+
+
+ADAM_MAX_TENSORS = 16          # GSB_ADAM_MAX_TENSORS
+
+
 _lib = None
 
 
@@ -153,6 +163,8 @@ def lib():
         L.gsb_export_image.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_debug_dequant.restype = C.c_int
         L.gsb_debug_dequant.argtypes = [C.POINTER(GsbQuant), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gsb_adam_step.restype = C.c_int
+        L.gsb_adam_step.argtypes = [C.POINTER(GsbAdamTensor), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_profile_enable.restype = None
         L.gsb_profile_enable.argtypes = [C.c_int]
         L.gsb_profile_read.restype = C.c_int
@@ -182,7 +194,7 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_min_redundancy_value", "gsb_kmeans_workspace_bytes", "gsb_kmeans", "gsb_l1_ssim_blocks",
                     "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn",
                     "gsb_forward_maps", "gsb_backward_maps", "gsb_camera_grad_workspace_bytes", "gsb_backward_camera",
-                    "gsb_forward_antialiased", "gsb_backward_antialiased"]
+                    "gsb_forward_antialiased", "gsb_backward_antialiased", "gsb_adam_step"]
 
 
 def check(status: int):
