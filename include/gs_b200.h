@@ -354,6 +354,76 @@ typedef struct GsbAdamTensor {
 GSB_API int gsb_adam_step(const GsbAdamTensor* tensors, int32_t n, int32_t P, const uint8_t* visibility /* NULL = all */,
                 const int32_t* degrees /* NULL = all bands */, void* stream);
 
+/* ---- densification (gs_b200.densify) ----
+ *
+ * The reference's GaussianModel.add_densification_stats / densify_and_prune / prune / prune_points (gaussian_model.py:553-695)
+ * as three calls, with the reference's arithmetic and row order (DESIGN.md §5g).  Every pointer is device memory; nothing
+ * synchronises with the host; the work runs on `stream`.  All thresholds are the fp32 casts of the Python doubles the reference
+ * forms (torch compares an fp32 tensor with a Python number in fp32).
+ *
+ * gsb_densify_stats: per iteration, for i < P (viewspace_grad is [P, grad_row_stride], its first two columns are read):
+ *   xyz_gradient_accum[i] += sqrt(g0*g0 + g1*g1);  denom[i] += visibility[i] != 0;
+ *   with radii (may be NULL): if visibility[i], max_radii2D[i] = max(max_radii2D[i], (float)radii[i]).
+ * Errors (GSB_EINVAL): P < 0, grad_row_stride < 2, a NULL pointer other than radii / max_radii2D when P > 0, radii without
+ * max_radii2D. */
+GSB_API int gsb_densify_stats(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const uint8_t* visibility,
+                const int32_t* radii, float* xyz_gradient_accum, float* denom, float* max_radii2D, void* stream);
+
+/* gsb_densify_plan: decides every row of the output and counts them into counts[GSB_DENSIFY_COUNTS] (device int64), which the
+ * caller reads back once to size the outputs.  Modes:
+ *   GSB_DENSIFY_CLONE_SPLIT  densify_and_prune: grads = accum / denom (NaN -> 0); clone if grads >= max_grad and
+ *                            max(exp(scaling)) <= clone_max_scale; split if grads >= max_grad and max(exp(scaling)) > clone_max_scale;
+ *                            then prune() over the result with max_radii2D = 0 (the reference has reset it by then).
+ *   GSB_DENSIFY_PRUNE        prune(): drop sigmoid(opacity) < min_opacity, or with screen_test, max_radii2D > max_screen_size or
+ *                            max(exp(scaling)) > big_scale.
+ *   GSB_DENSIFY_PRUNE_MASK   prune_points(mask): drop the rows where prune_mask (u8 [P]) is nonzero.
+ * Output order: [kept originals][kept clones][kept first children][kept second children].  A split child has the parent's
+ * scaling times split_scale_factor (the fp32 reciprocal of 0.8 * N that torch multiplies by) before the log, and is pruned on
+ * its own reduced scaling.  The workspace (gsb_densify_workspace_bytes(P) bytes) keeps the plan for gsb_densify_emit and holds
+ * exp(scaling) of the split parents, [n_split, 3] fp32 at byte offset gsb_densify_split_std_offset(P), for the caller's draw.
+ * Errors (GSB_EINVAL): P < 0 or P >= 2^30, an unknown mode, NULL workspace / counts, NULL inputs the mode reads (P > 0). */
+#define GSB_DENSIFY_CLONE_SPLIT 0
+#define GSB_DENSIFY_PRUNE 1
+#define GSB_DENSIFY_PRUNE_MASK 2
+#define GSB_DENSIFY_COUNTS 8      /* kept originals, clones, kept clones, split parents, kept children per copy, P', pruned, 0 */
+GSB_API size_t gsb_densify_workspace_bytes(int32_t P);
+GSB_API size_t gsb_densify_split_std_offset(int32_t P);
+GSB_API int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* denom, const float* scaling,
+                const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad, float clone_max_scale,
+                float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
+                void* workspace, int64_t* counts, void* stream);
+
+/* gsb_densify_emit: writes every output row of every table entry in one launch, from the plan in `workspace` and the counts
+ * read back.  Per entry: the [P, row_width] source rows of 4-byte elements (param, and optionally both moments and the grad)
+ * go to [P', row_width] destinations.  Kept rows and clones are copies; new rows (clones and children) get zero moments and
+ * grads.  Split children copy the parent except for kind GSB_DENSIFY_XYZ (rotation(parent) @ samples[j] + xyz, with
+ * samples [2 * n_split, 3] and j = the parent's split rank, + n_split for the second child) and GSB_DENSIFY_SCALING
+ * (log(exp(scaling) * split_scale_factor)); XYZ needs rotation [P, 4].  A moment pair or the grad pair is
+ * either both NULL (absent) or both set.
+ * Errors (GSB_EINVAL, nothing launched): tensors NULL with n > 0, n outside 0..GSB_DENSIFY_MAX_TENSORS, P outside 0..2^30,
+ * negative counts, NULL workspace, row_width <= 0, an unknown kind or an XYZ / SCALING entry whose row_width is not 3, a
+ * pointer not 4-byte aligned, and when the output has rows (n_kept + n_clones_kept + n_children_kept > 0), a NULL src / dst,
+ * a half-given pair or, with children, NULL rotation / samples.  A call without output rows writes nothing. */
+#define GSB_DENSIFY_MAX_TENSORS 16
+#define GSB_DENSIFY_COPY 0
+#define GSB_DENSIFY_XYZ 1
+#define GSB_DENSIFY_SCALING 2
+typedef struct GsbDensifyTensor {
+	const void* src;              /* [P, row_width] 4-byte elements (fp32 params and statistics, int32 degrees)  */
+	void* dst;                    /* [P', row_width]                                                             */
+	const float* exp_avg_src;     /* moments: NULL pairs = none                                                  */
+	float* exp_avg_dst;
+	const float* exp_avg_sq_src;
+	float* exp_avg_sq_dst;
+	const float* grad_src;        /* grad: NULL pair = none                                                      */
+	float* grad_dst;
+	int32_t row_width;
+	int32_t kind;                 /* GSB_DENSIFY_COPY / _XYZ / _SCALING                                          */
+} GsbDensifyTensor;
+GSB_API int gsb_densify_emit(const GsbDensifyTensor* tensors, int32_t n, int32_t P, const void* workspace, int64_t n_kept,
+                int64_t n_clones_kept, int64_t n_split, int64_t n_children_kept, const float* rotation, const float* samples,
+                float split_scale_factor, void* stream);
+
 /* Number of kernels this library has launched since load (bench.py reports it as gpu_launches). */
 GSB_API uint64_t gsb_launch_count(void);
 

@@ -44,16 +44,6 @@ __device__ __forceinline__ void adam_update(float& p, float g, float& m, float& 
 	p = __fmaf_rn(k.step_size, __fdiv_rn(m, d), p);
 }
 
-// Row and column of flat element e of a [P, w] tensor.  (double)e * (1/w) is within one of the row for e < 2^53.
-__device__ __forceinline__ void row_col(long long e, int w, double inv_w, long long& r, int& c)
-{
-	r = (long long)((double)e * inv_w);
-	long long cc = e - r * w;
-	if (cc < 0) { r--; cc += w; }
-	else if (cc >= w) { r++; cc -= w; }
-	c = (int)cc;
-}
-
 template <bool VIS, bool DEG>
 __global__ void __launch_bounds__(ADAM_THREADS, ADAM_CTAS_PER_SM) adam_step_kernel(const __grid_constant__ AdamTable tab,
 	const uint8_t* __restrict__ visibility, const int32_t* __restrict__ degrees)

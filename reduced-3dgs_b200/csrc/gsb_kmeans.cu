@@ -101,11 +101,8 @@ __global__ void __launch_bounds__(256) km_sort_plan_kernel(const uint32_t* __res
 	}
 }
 
-#define KM_LB_AGG 0x40000000u
-#define KM_LB_INC 0x80000000u
-#define KM_LB_VAL 0x3fffffffu
 // One onesweep pass: tile = 4096 consecutive keys; warp w ranks keys [512 w, 512 (w+1)) in 16 warp-wide steps with match.any
-// (stable), digit counts are chained across tiles with decoupled look-back.  PAIRS: a 32-bit value travels with each key
+// (stable), digit counts are chained across tiles with decoupled look-back (lookback_exclusive).  PAIRS: a 32-bit value travels with each key
 // (the kNN's (Morton code, point index) sort); the k-means sorts keys only.
 template <bool PAIRS>
 __global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint32_t* keys1, uint32_t* vals0, uint32_t* vals1, long long n,
@@ -162,22 +159,7 @@ __global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint
 	uint32_t total = 0;
 #pragma unroll
 	for (int w = 0; w < 8; w++) { const uint32_t c = s_whist[w][tid]; s_whist[w][tid] = total; total += c; }
-	uint32_t excl = 0;
-	if (tile == 0) atomicExch(&lookback[tid], KM_LB_INC | total);
-	else
-	{
-		atomicExch(&lookback[(size_t)tile * 256 + tid], KM_LB_AGG | total);
-		long long j = (long long)tile - 1;
-		while (true)
-		{
-			uint32_t c;
-			do { c = *reinterpret_cast<volatile uint32_t*>(&lookback[(size_t)j * 256 + tid]); } while (c == 0);
-			excl += c & KM_LB_VAL;
-			if (c & KM_LB_INC) break;
-			j--;
-		}
-		atomicExch(&lookback[(size_t)tile * 256 + tid], KM_LB_INC | (excl + total));
-	}
+	const uint32_t excl = lookback_exclusive(lookback, tile, 256, tid, total);
 	s_dstart[tid] = total;
 	__syncthreads();
 	for (int o = 1; o < 256; o <<= 1)

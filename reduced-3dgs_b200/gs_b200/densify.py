@@ -1,0 +1,238 @@
+"""Native densification: the reference's GaussianModel.densify_and_prune / prune / prune_points / add_densification_stats
+(scene/gaussian_model.py:553-695) on the model and its optimizer state, row for row (DESIGN.md §5g).
+
+    from gs_b200 import densify
+    GaussianModel.densify_and_prune = densify.densify_and_prune      # INTEGRATION.md section D
+    GaussianModel.prune = densify.prune
+    GaussianModel.prune_points = densify.prune_points
+    GaussianModel.add_densification_stats = densify.add_densification_stats
+
+The signatures are the reference's methods with `self` -> `model`.  The results are the reference's: the same rows in the same
+order ([kept originals][kept clones][kept first children][kept second children]), the same values, the same optimizer state
+dicts (their `step` tensors included) moved to the new nn.Parameters, the same statistics and dictionary entries, and the same
+CUDA generator state (torch.normal is called once, with the reference's [2 S, 3] shape, also for S = 0).  The split children's
+xyz goes through rotation @ sample, whose torch.bmm rounding depends on cuBLAS's kernel choice; those values agree to rounding.
+
+densify_and_prune, prune and prune_points each read the host once (the counts that size the outputs), where the reference
+synchronises about ten times; add_densification_stats never does.  torch.cuda.empty_cache() is not called.
+
+Model contract (duck-typed on the reference's attribute names): the optimizer is torch.optim.Adam or GaussianAdam with exactly
+the six groups "xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation", one fp32 contiguous CUDA param each (f_rest a dense
+[P, C, 3] tensor); `_degrees` int32 [P, 1]; `xyz_gradient_accum`, `denom` fp32 [P, 1]; `max_radii2D` fp32 [P];
+`percent_dense`.  Anything else is refused before the model or the optimizer changes.
+"""
+from __future__ import annotations
+
+import numpy as np
+import torch
+from torch import nn
+
+from . import lib as gsl
+
+GROUPS = ("xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation")
+ATTR = {"xyz": "_xyz", "f_dc": "_features_dc", "f_rest": "_features_rest", "opacity": "_opacity", "scaling": "_scaling",
+        "rotation": "_rotation"}
+ROW_SHAPE = {"xyz": (3,), "opacity": (1,), "scaling": (3,), "rotation": (4,)}
+SPLIT_N = 2
+
+
+def split_scale_factor(n=SPLIT_N):
+    """torch's CUDA division of an fp32 tensor by the Python number 0.8 * N multiplies by the fp32 reciprocal of its fp32 cast
+    (tools/probe_torch_densify.py)."""
+    return float(np.float32(1) / np.float32(0.8 * n))
+
+
+def add_densification_stats(model, viewspace_point_tensor, update_filter, radii=None):
+    """xyz_gradient_accum += |grad[:, :2]|; denom += update_filter; with radii, also train.py:134's
+    max_radii2D[update_filter] = max(max_radii2D[update_filter], radii[update_filter]).  One launch, no host synchronisation."""
+    g = viewspace_point_tensor.grad
+    accum, denom = model.xyz_gradient_accum, model.denom
+    P = accum.shape[0] if accum.dim() > 0 else -1
+    if g is None:
+        raise RuntimeError("densify: viewspace_point_tensor has no gradient")
+    dev = g.device
+    if (not g.is_cuda or g.dtype != torch.float32 or g.dim() != 2 or g.shape[0] != P or g.shape[1] < 2 or g.stride(1) != 1
+            or (P > 1 and g.stride(0) < 2)):
+        raise RuntimeError("densify: the view-space gradient must be an fp32 CUDA [P, >= 2] tensor with unit column stride")
+    _check_f32(accum, (P, 1), dev, "xyz_gradient_accum")
+    _check_f32(denom, (P, 1), dev, "denom")
+    if (update_filter.dtype != torch.bool or update_filter.shape != (P,) or update_filter.device != dev
+            or not update_filter.is_contiguous()):
+        raise RuntimeError(f"densify: update_filter must be a contiguous bool tensor [{P}] on {dev}")
+    mr = None
+    if radii is not None:
+        if radii.dtype != torch.int32 or radii.shape != (P,) or radii.device != dev or not radii.is_contiguous():
+            raise RuntimeError(f"densify: radii must be a contiguous int32 tensor [{P}] on {dev}")
+        mr = model.max_radii2D
+        _check_f32(mr, (P,), dev, "max_radii2D")
+    if P == 0:
+        return
+    with gsl.on_device(dev):
+        gsl.check(gsl.lib().gsb_densify_stats(P, g.data_ptr(), g.stride(0), update_filter.data_ptr(),
+                                               None if radii is None else radii.data_ptr(), accum.data_ptr(), denom.data_ptr(),
+                                               None if mr is None else mr.data_ptr(), gsl.current_stream(dev)))
+
+
+def densify_and_prune(model, max_grad, min_opacity, extent, max_screen_size, densification_statistics_dict, store_grads=False):
+    """densify_and_clone + densify_and_split + prune of the reference, in one plan and one emit."""
+    groups, P, dev = _validate(model, store_grads, grads_everywhere=store_grads)
+    counts, ws, dcounts = _plan(model, groups, P, dev, gsl.DENSIFY_CLONE_SPLIT, max_grad=max_grad, percent_dense=model.percent_dense,
+                       min_opacity=min_opacity, extent=extent, max_screen_size=max_screen_size)
+    n_kept, C, n_clones_kept, S, n_children, P_out = counts[:6]
+    # the reference's draw (gaussian_model.py:633-635): std = exp(scaling) of the split parents, repeated N times
+    off = gsl.lib().gsb_densify_split_std_offset(P)
+    stds = ws[off:off + 12 * S].view(torch.float32).view(S, 3).repeat(SPLIT_N, 1)
+    means = torch.zeros((stds.size(0), 3), device=dev)
+    samples = torch.normal(mean=means, std=stds)
+    _emit(model, groups, P, dev, ws, counts, store_grads, gather_stats=False, samples=samples)
+    model.xyz_gradient_accum = torch.zeros((P_out, 1), device=dev)
+    # densification_postfix creates density_gradient_accum after the split's concatenation; the prunes that follow do not index it
+    model.density_gradient_accum = torch.zeros((P + C + SPLIT_N * S, 1), device=dev)
+    model.denom = torch.zeros((P_out, 1), device=dev)
+    model.max_radii2D = torch.zeros((P_out), device=dev)
+    densification_statistics_dict["n_points_pruned"] = _pruned(dcounts)
+    densification_statistics_dict["n_points_cloned"] = C
+    densification_statistics_dict["n_points_split"] = S
+
+
+def prune(model, min_opacity, extent, max_screen_size, densification_statistics_dict, store_grads=False):
+    """The reference's prune(): drop sigmoid(opacity) < min_opacity and, if max_screen_size, the rows too large on screen or in
+    the world."""
+    groups, P, dev = _validate(model, store_grads)
+    counts, ws, dcounts = _plan(model, groups, P, dev, gsl.DENSIFY_PRUNE, min_opacity=min_opacity, extent=extent,
+                       max_screen_size=max_screen_size)
+    densification_statistics_dict["n_points_pruned"] = _pruned(dcounts)
+    _emit(model, groups, P, dev, ws, counts, store_grads, gather_stats=True)
+
+
+def prune_points(model, mask, store_grads=False):
+    """The reference's prune_points(mask): drop the rows where mask (bool [P], e.g. from mercy_points) is True."""
+    groups, P, dev = _validate(model, store_grads)
+    if not torch.is_tensor(mask) or mask.dtype != torch.bool or mask.shape != (P,) or mask.device != dev:
+        raise RuntimeError(f"densify: the prune mask must be a bool tensor [{P}] on {dev}")
+    counts, ws, _ = _plan(model, groups, P, dev, gsl.DENSIFY_PRUNE_MASK, mask=mask.contiguous())
+    _emit(model, groups, P, dev, ws, counts, store_grads, gather_stats=True)
+
+
+# ------------------------------------------------------------------------------------------------ internals
+def _check_f32(t, shape, dev, name):
+    if not torch.is_tensor(t) or t.dtype != torch.float32 or tuple(t.shape) != tuple(shape) or t.device != dev or not t.is_contiguous():
+        raise RuntimeError(f"densify: {name} must be a contiguous fp32 tensor {list(shape)} on {dev}")
+
+
+def _validate(model, store_grads, grads_everywhere=False):
+    """[(name, group, param, state or None)] in group order, P, device; raises before anything changes."""
+    if getattr(model, "_codebook_dict", None) is not None:
+        raise RuntimeError("densify: a quantised model (codebooks) cannot be densified")
+    if isinstance(getattr(model, "_features_rest", None), (list, tuple)):
+        raise RuntimeError("densify: variable-SH-band models (a list-valued _features_rest) are not supported")
+    opt = getattr(model, "optimizer", None)
+    if not isinstance(opt, torch.optim.Adam):
+        raise RuntimeError("densify: the model's optimizer must be torch.optim.Adam or GaussianAdam")
+    names = [g.get("name") for g in opt.param_groups]
+    if sorted(names) != sorted(GROUPS) or any(len(g["params"]) != 1 for g in opt.param_groups):
+        raise RuntimeError(f"densify: the optimizer needs exactly the groups {GROUPS}, one param each; it has {names}")
+    p0 = next(g["params"][0] for g in opt.param_groups if g["name"] == "xyz")
+    P, dev = p0.shape[0] if p0.dim() > 0 else -1, p0.device
+    if not p0.is_cuda:
+        raise RuntimeError("densify: the model's params must be CUDA tensors (there is no CPU path)")
+    groups = []
+    for g in opt.param_groups:
+        name, p = g["name"], g["params"][0]
+        want = (P,) + ROW_SHAPE[name] if name in ROW_SHAPE else None
+        if p.dtype != torch.float32 or not p.is_contiguous() or p.device != dev or p.dim() < 2 or p.shape[0] != P \
+                or (want is not None and tuple(p.shape) != want) or (name == "f_rest" and (p.dim() != 3 or p.shape[2] != 3)):
+            raise RuntimeError(f"densify: param '{name}' must be a contiguous fp32 tensor of {P} rows on {dev} "
+                               f"({'x'.join(map(str, want)) if want else '[P, C, 3]'}), got {tuple(p.shape)} {p.dtype} on {p.device}")
+        state = opt.state.get(p, None)
+        if state is not None:
+            for k in ("exp_avg", "exp_avg_sq"):
+                s = state.get(k)
+                if not torch.is_tensor(s) or s.shape != p.shape or s.dtype != torch.float32 or s.device != dev or not s.is_contiguous():
+                    raise RuntimeError(f"densify: state['{k}'] of '{name}' must be a contiguous fp32 tensor of the param's shape")
+        if store_grads and (state is not None or grads_everywhere):
+            gr = p.grad
+            if gr is None or gr.shape != p.shape or gr.dtype != torch.float32 or gr.device != dev or not gr.is_contiguous():
+                raise RuntimeError(f"densify: store_grads needs a contiguous fp32 gradient of '{name}' (the reference carries it)")
+        groups.append((name, g, p, state))
+    deg = getattr(model, "_degrees", None)
+    if not torch.is_tensor(deg) or deg.dtype != torch.int32 or tuple(deg.shape) != (P, 1) or deg.device != dev or not deg.is_contiguous():
+        raise RuntimeError(f"densify: _degrees must be a contiguous int32 tensor [{P}, 1] on {dev}")
+    _check_f32(getattr(model, "xyz_gradient_accum", None), (P, 1), dev, "xyz_gradient_accum")
+    _check_f32(getattr(model, "denom", None), (P, 1), dev, "denom")
+    _check_f32(getattr(model, "max_radii2D", None), (P,), dev, "max_radii2D")
+    return groups, P, dev
+
+
+def _plan(model, groups, P, dev, mode, max_grad=0.0, percent_dense=0.0, min_opacity=0.0, extent=0.0, max_screen_size=None, mask=None):
+    """Runs the plan and reads its counts back (the one host synchronisation).  The thresholds are the reference's Python
+    doubles (percent_dense*extent, 0.1*extent), cast to fp32 by ctypes as torch casts a Python number it compares with."""
+    param = {name: p for name, _, p, _ in groups}
+    ws = torch.empty(gsl.lib().gsb_densify_workspace_bytes(P), dtype=torch.uint8, device=dev)
+    counts = torch.empty(gsl.DENSIFY_COUNTS, dtype=torch.int64, device=dev)
+    screen = bool(max_screen_size)
+    with gsl.on_device(dev):
+        gsl.check(gsl.lib().gsb_densify_plan(
+            P, mode, model.xyz_gradient_accum.data_ptr(), model.denom.data_ptr(), param["scaling"].data_ptr(),
+            param["opacity"].data_ptr(), model.max_radii2D.data_ptr(), None if mask is None else mask.data_ptr(),
+            max_grad, percent_dense * extent, min_opacity, 1 if screen else 0, max_screen_size if screen else 0.0, 0.1 * extent,
+            split_scale_factor(), ws.data_ptr(), counts.data_ptr(), gsl.current_stream(dev)))
+    return [int(v) for v in counts.tolist()], ws, counts
+
+
+def _pruned(counts):
+    """n_points_pruned: a 0-dim int64 device tensor, as the reference's prune_mask.sum() is; copied on the device."""
+    return counts[6].clone()
+
+
+def _emit(model, groups, P, dev, ws, counts, store_grads, gather_stats, samples=None):
+    n_kept, _, n_clones_kept, S, n_children, P_out = counts[:6]
+    entries, new = [], []
+    for name, g, p, state in groups:
+        dst = torch.empty((P_out,) + tuple(p.shape[1:]), dtype=torch.float32, device=dev)
+        e = gsl.GsbDensifyTensor()
+        e.src, e.dst = p.data_ptr(), dst.data_ptr()
+        e.row_width = p.shape[1:].numel()
+        e.kind = {"xyz": gsl.DENSIFY_XYZ, "scaling": gsl.DENSIFY_SCALING}.get(name, gsl.DENSIFY_COPY)
+        m = v = gr = None
+        if state is not None:
+            m, v = torch.empty_like(dst), torch.empty_like(dst)
+            e.exp_avg_src, e.exp_avg_dst = state["exp_avg"].data_ptr(), m.data_ptr()
+            e.exp_avg_sq_src, e.exp_avg_sq_dst = state["exp_avg_sq"].data_ptr(), v.data_ptr()
+            if store_grads:
+                gr = torch.empty_like(dst)
+                e.grad_src, e.grad_dst = p.grad.data_ptr(), gr.data_ptr()
+        entries.append(e)
+        new.append((name, g, p, state, dst, m, v, gr))
+    stats = [("_degrees", torch.int32, (1,))]
+    if gather_stats:
+        stats += [("xyz_gradient_accum", torch.float32, (1,)), ("denom", torch.float32, (1,)), ("max_radii2D", torch.float32, ())]
+    out_stats = {}
+    for attr, dtype, row in stats:
+        src = getattr(model, attr)
+        dst = torch.empty((P_out,) + row, dtype=dtype, device=dev)
+        e = gsl.GsbDensifyTensor()
+        e.src, e.dst, e.row_width, e.kind = src.data_ptr(), dst.data_ptr(), 1, gsl.DENSIFY_COPY
+        entries.append(e)
+        out_stats[attr] = dst
+    rot = next(p for name, _, p, _ in groups if name == "rotation")
+    table = (gsl.GsbDensifyTensor * len(entries))(*entries)
+    with gsl.on_device(dev):
+        gsl.check(gsl.lib().gsb_densify_emit(table, len(entries), P, ws.data_ptr(), n_kept, n_clones_kept, S, n_children,
+                                              rot.data_ptr(), None if samples is None or samples.numel() == 0 else samples.data_ptr(),
+                                              split_scale_factor(), gsl.current_stream(dev)))
+    # the reference's optimizer surgery (_prune_optimizer / cat_tensors_to_optimizer): the state dict object moves to the new
+    # Parameter with the new moments; a group without state only gets its param; .grad travels only with state and store_grads
+    opt = model.optimizer
+    for name, g, p, state, dst, m, v, gr in new:
+        param = nn.Parameter(dst.requires_grad_(True))
+        if state is not None:
+            state["exp_avg"], state["exp_avg_sq"] = m, v
+            del opt.state[p]
+            if gr is not None:
+                param.grad = gr
+            opt.state[param] = state
+        g["params"][0] = param
+        setattr(model, ATTR[name], param)
+    for attr, t in out_stats.items():
+        setattr(model, attr, t)

@@ -60,6 +60,18 @@ class GsbAdamTensor(C.Structure):
 ADAM_MAX_TENSORS = 16          # GSB_ADAM_MAX_TENSORS
 
 
+class GsbDensifyTensor(C.Structure):
+    _fields_ = [("src", C.c_void_p), ("dst", C.c_void_p), ("exp_avg_src", C.c_void_p), ("exp_avg_dst", C.c_void_p),
+                ("exp_avg_sq_src", C.c_void_p), ("exp_avg_sq_dst", C.c_void_p), ("grad_src", C.c_void_p), ("grad_dst", C.c_void_p),
+                ("row_width", C.c_int32), ("kind", C.c_int32)]
+
+
+DENSIFY_MAX_TENSORS = 16       # GSB_DENSIFY_MAX_TENSORS
+DENSIFY_COUNTS = 8             # GSB_DENSIFY_COUNTS
+DENSIFY_CLONE_SPLIT, DENSIFY_PRUNE, DENSIFY_PRUNE_MASK = 0, 1, 2
+DENSIFY_COPY, DENSIFY_XYZ, DENSIFY_SCALING = 0, 1, 2
+
+
 _lib = None
 
 
@@ -165,6 +177,19 @@ def lib():
         L.gsb_debug_dequant.argtypes = [C.POINTER(GsbQuant), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_adam_step.restype = C.c_int
         L.gsb_adam_step.argtypes = [C.POINTER(GsbAdamTensor), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gsb_densify_stats.restype = C.c_int
+        L.gsb_densify_stats.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p]
+        L.gsb_densify_workspace_bytes.restype = C.c_size_t
+        L.gsb_densify_workspace_bytes.argtypes = [C.c_int32]
+        L.gsb_densify_split_std_offset.restype = C.c_size_t
+        L.gsb_densify_split_std_offset.argtypes = [C.c_int32]
+        L.gsb_densify_plan.restype = C.c_int
+        L.gsb_densify_plan.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.c_float] * 3 + [C.c_int32] + [C.c_float] * 3 + \
+            [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gsb_densify_emit.restype = C.c_int
+        L.gsb_densify_emit.argtypes = [C.POINTER(GsbDensifyTensor), C.c_int32, C.c_int32, C.c_void_p] + [C.c_int64] * 4 + \
+            [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
         L.gsb_profile_enable.restype = None
         L.gsb_profile_enable.argtypes = [C.c_int]
         L.gsb_profile_read.restype = C.c_int
@@ -194,7 +219,8 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_min_redundancy_value", "gsb_kmeans_workspace_bytes", "gsb_kmeans", "gsb_l1_ssim_blocks",
                     "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn",
                     "gsb_forward_maps", "gsb_backward_maps", "gsb_camera_grad_workspace_bytes", "gsb_backward_camera",
-                    "gsb_forward_antialiased", "gsb_backward_antialiased", "gsb_adam_step"]
+                    "gsb_forward_antialiased", "gsb_backward_antialiased", "gsb_adam_step", "gsb_densify_stats",
+                    "gsb_densify_workspace_bytes", "gsb_densify_split_std_offset", "gsb_densify_plan", "gsb_densify_emit"]
 
 
 def check(status: int):
