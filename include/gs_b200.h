@@ -238,6 +238,55 @@ GSB_API int gsb_backward_antialiased(const GsbScene* scene, const GsbCamera* cam
                  float lambda_sh_sparsity, float* dL_dviewmatrix /* [16] or NULL */, float* dL_dprojmatrix /* [16] or NULL */,
                  float* dL_dcampos /* [3] or NULL */, char* workspace, void* stream);
 
+/* Rendering from the model's raw parameters (`pipe.fused_activations`, DESIGN.md §5h): the leaf tensors of the reference's
+ * GaussianModel as they are, with get_scaling = exp(_scaling), get_rotation = F.normalize(_rotation) and
+ * get_features = cat(_features_dc, _features_rest) applied inside the kernels (exp and the norm in torch's CUDA roundings), so no
+ * elementwise pass and no [P,16,3] copy runs in between.  All tensors fp32, contiguous, device memory. */
+typedef struct GsbRawParams {
+	const float* features_dc;    /* [P,1,3]  SH coefficient 0; NULL when the scene has colors_precomp                    */
+	const float* features_rest;  /* [P,C,3]  SH coefficients 1..C; NULL when C == 0 or with colors_precomp               */
+	int32_t C;                   /* rest coefficients per Gaussian: 0, 3, 8 or 15 (max SH degree 0..3)                   */
+	const float* scaling;        /* [P,3]    log-scales (_scaling)                                                       */
+	const float* rotation;       /* [P,4]    unnormalised quaternions (r,x,y,z) (_rotation)                              */
+} GsbRawParams;
+
+/* Gradients w.r.t. the four raw tensors, overwritten (or added to, with GsbGrads.accumulate).  dL_dfeatures_dc / _rest are the
+ * SH gradient split at coefficient 1 (zeros outside each Gaussian's active bands; the sparsity sign term on the rest), and may be
+ * NULL (then not written; they must be NULL with colors_precomp).  dL_dscaling = dL/ds * s (ExpBackward0's single multiply);
+ * dL_drotation is autograd's chain through F.normalize in torch's CUDA roundings (tools/probe_torch_activations.py). */
+typedef struct GsbRawGrads {
+	float* dL_dfeatures_dc;      /* [P,1,3] or NULL */
+	float* dL_dfeatures_rest;    /* [P,C,3] or NULL (NULL when C == 0) */
+	float* dL_dscaling;          /* [P,3]           */
+	float* dL_drotation;         /* [P,4]           */
+} GsbRawGrads;
+
+/* gsb_forward_raw:  the arguments of gsb_forward_antialiased plus the raw parameters and the anti-aliasing flag.  The scene keeps
+ *                   P, means3D, opacities, degrees, prune_mask, colors_precomp and scale_modifier; its scales, rotations, shs,
+ *                   cov3D_precomp and quant must be NULL, sh_packed 0, and M is ignored.  Colour, radii, R, the maps, the blobs
+ *                   and every GsbDebug export are bit-identical to the activated call on exp(scaling), F.normalize(rotation) and
+ *                   cat(features_dc, features_rest).
+ * gsb_backward_raw: the arguments of gsb_backward_antialiased plus the raw parameters, their gradients and the flag (the same
+ *                   values as the forward's).  grads->dL_dsh, dL_dscales and dL_drotations must be NULL (raw_grads replaces them);
+ *                   grads->dL_dcov3D and dL_dcolors may be NULL (not written).  Everything else as gsb_backward_antialiased /
+ *                   gsb_backward_camera; per-Gaussian outputs other than the four raw gradients are those of the activated call.
+ * Errors (GSB_EINVAL, nothing launched): raw NULL, C not in {0, 3, 8, 15}, a scene field above that must be NULL, and with P > 0
+ * NULL scaling / rotation / degrees, or SH pointers that do not match colors_precomp and C. */
+GSB_API int gsb_forward_raw(const GsbScene* scene, const GsbCamera* cam,
+                gsb_alloc_fn geom_alloc, void* geom_user,
+                gsb_alloc_fn binning_alloc, void* binning_user,
+                gsb_alloc_fn image_alloc, void* image_user,
+                float* out_color, int32_t* radii, int64_t* num_rendered,
+                const GsbDebug* debug, float* out_invdepth /* or NULL */, float* out_alpha /* or NULL */,
+                const GsbRawParams* raw, int32_t antialiasing, void* stream);
+GSB_API int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
+                 const char* geom_blob, const char* binning_blob, const char* image_blob,
+                 const float* dL_dout_color /* [3,H,W] */, const GsbGrads* grads,
+                 const float* dL_dinvdepth /* [1,H,W] or NULL */, const float* dL_dalpha /* [1,H,W] or NULL */,
+                 float lambda_sh_sparsity, float* dL_dviewmatrix /* [16] or NULL */, float* dL_dprojmatrix /* [16] or NULL */,
+                 float* dL_dcampos /* [3] or NULL */, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
+                 int32_t antialiasing, void* stream);
+
 /* present[i] = view-space z of means3D[i] > 0.2 (auxiliary.h:139-159). */
 GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);

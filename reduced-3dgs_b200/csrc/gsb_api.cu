@@ -95,7 +95,7 @@ static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
 int launch_preprocess(const GsbScene*, const GsbCamera*, const GeomState&, const ImageState&, const BinPlan&, int32_t*, const GsbDebug*, bool,
-	cudaStream_t);
+	const GsbRawParams*, cudaStream_t);
 int launch_mark_visible(int, const float*, const float*, uint8_t*, cudaStream_t);
 int launch_tile_scan(const ImageState&, const GeomState&, const BinPlan&, int, int, cudaStream_t);
 int launch_scatter_sort(const GeomState&, const BinningState&, const ImageState&, const BinPlan&, int, long long, int, int, cudaStream_t);
@@ -117,14 +117,33 @@ int launch_knn(const float*, long long, int, const int32_t*, long long, const in
 int launch_render_backward(const ImageState&, const BinningState&, const GeomState&, int, int, int, const float*, const float*, const float*,
 	const float*, float*, cudaStream_t);
 int launch_preprocess_backward(const GsbScene*, const GsbCamera*, const GeomState&, const int32_t*, const float*, const GsbGrads*, bool, float,
-	float*, bool, cudaStream_t);
+	float*, bool, const GsbRawParams*, const GsbRawGrads*, cudaStream_t);
 size_t camera_grad_workspace_bytes(int);
 int launch_camera_grad_finish(int, const float*, float*, float*, float*, cudaStream_t);
 
 // geometry blob = GeomState followed by the backward's gradient accumulator (12 floats per Gaussian)
 static size_t geom_state_bytes(int P) { size_t b; GeomState::carve(nullptr, P, &b); return (b + 255) & ~size_t(255); }
 
-static int check_scene(const GsbScene* s, const GsbCamera* c)
+// The raw-parameter entry points (gsb_forward_raw / gsb_backward_raw): what the scene and the raw struct must hold.
+static int check_raw(const GsbScene* s, const GsbRawParams* raw)
+{
+	if (!raw) { set_error("raw parameters are NULL"); return GSB_EINVAL; }
+	if (raw->C != 0 && raw->C != 3 && raw->C != 8 && raw->C != 15)
+	{ set_error("raw parameters: C = %d rest coefficients; only 0, 3, 8 or 15 (max SH degree 0..3) exist", raw->C); return GSB_EINVAL; }
+	if (s->scales || s->rotations || s->shs || s->cov3D_precomp || s->quant || s->sh_packed)
+	{ set_error("raw parameters: the scene's scales, rotations, shs, cov3D_precomp and quant must be NULL and sh_packed 0"); return GSB_EINVAL; }
+	if (s->P == 0) return GSB_OK;
+	if (!raw->scaling || !raw->rotation) { set_error("raw parameters: scaling / rotation missing"); return GSB_EINVAL; }
+	if (s->colors_precomp)
+	{
+		if (raw->features_dc || raw->features_rest) { set_error("raw parameters: SH given together with colors_precomp"); return GSB_EINVAL; }
+	}
+	else if (!raw->features_dc || !s->degrees || (raw->features_rest == nullptr) != (raw->C == 0))
+	{ set_error("raw parameters: features_dc, degrees and (for C > 0) features_rest are required without colors_precomp"); return GSB_EINVAL; }
+	return GSB_OK;
+}
+
+static int check_scene(const GsbScene* s, const GsbCamera* c, const GsbRawParams* raw = nullptr)
 {
 	if (!s || !c) { set_error("scene / camera is NULL"); return GSB_EINVAL; }
 	if (s->P < 0) { set_error("P < 0"); return GSB_EINVAL; }
@@ -141,6 +160,7 @@ static int check_scene(const GsbScene* s, const GsbCamera* c)
 		return GSB_OK;
 	}
 	if (!s->opacities) { set_error("opacities missing"); return GSB_EINVAL; }
+	if (raw) return check_raw(s, raw);
 	// diff_gaussian_rasterization/__init__.py:203-207
 	if ((s->shs == nullptr) == (s->colors_precomp == nullptr)) { set_error("Please provide excatly one of either SHs or precomputed colors!"); return GSB_EINVAL; }
 	const bool sr = s->scales != nullptr && s->rotations != nullptr;
@@ -219,10 +239,10 @@ static thread_local std::map<int, HostSide> t_host;
 static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
 	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
 	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, int32_t* touched_pixels, float* transmittance,
-	float* out_invdepth, float* out_alpha, bool aa, void* stream_)
+	float* out_invdepth, float* out_alpha, bool aa, void* stream_, const GsbRawParams* raw = nullptr)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
-	if (int e = check_scene(scene, cam)) return e;
+	if (int e = check_scene(scene, cam, raw)) return e;
 	if (!out_color || !num_rendered || (scene->P > 0 && !radii)) { set_error("output pointers missing"); return GSB_EINVAL; }
 	*num_rendered = 0;
 	const int P = scene->P, W = cam->width, H = cam->height;
@@ -243,7 +263,7 @@ static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_f
 	ImageState img = ImageState::carve(img_blob, W, H, nullptr, plan.priv ? plan.ctas : 0);
 	GSB_CUDA_OK(cudaMemsetAsync(g.counters, 0, 16 * sizeof(uint32_t), stream));
 	if (!plan.priv) GSB_CUDA_OK(cudaMemsetAsync(img.tile_count, 0, ImageState::tiles(W, H) * sizeof(uint32_t), stream));
-	if (int e = launch_preprocess(scene, cam, g, img, plan, radii, debug, aa, stream)) return e;
+	if (int e = launch_preprocess(scene, cam, g, img, plan, radii, debug, aa, raw, stream)) return e;
 	if (int e = launch_tile_scan(img, g, plan, W, H, stream)) return e;
 
 	// The instance count R sizes the binning blob (rasterizer_impl.cu:445-450 reads it back and stalls the device meanwhile).
@@ -426,10 +446,11 @@ int gsb_min_redundancy_value(int32_t P, const int32_t* redundancy_values, const 
 static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
 	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
 	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dview, float* dL_dproj, float* dL_dcampos, char* cam_workspace, bool aa, void* stream_)
+	float* dL_dview, float* dL_dproj, float* dL_dcampos, char* cam_workspace, bool aa, void* stream_,
+	const GsbRawParams* raw = nullptr, const GsbRawGrads* raw_grads = nullptr)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
-	if (int e = check_scene(scene, cam)) return e;
+	if (int e = check_scene(scene, cam, raw)) return e;
 	if (!grads) { set_error("grads is NULL"); return GSB_EINVAL; }
 	const int P = scene->P, W = cam->width, H = cam->height;
 	const bool want_cam = dL_dview || dL_dproj || dL_dcampos;
@@ -442,7 +463,12 @@ static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R,
 		return GSB_OK;
 	}
 	if (!geom_blob || !binning_blob || !image_blob || !dL_dout_color || !radii) { set_error("backward inputs missing"); return GSB_EINVAL; }
-	if (!grads->dL_dmeans2D || !grads->dL_dcolors || !grads->dL_dopacity || !grads->dL_dmeans3D || !grads->dL_dcov3D ||
+	if (raw)
+	{
+		if (!grads->dL_dmeans2D || !grads->dL_dopacity || !grads->dL_dmeans3D || !raw_grads->dL_dscaling || !raw_grads->dL_drotation)
+		{ set_error("gradient output pointers missing"); return GSB_EINVAL; }
+	}
+	else if (!grads->dL_dmeans2D || !grads->dL_dcolors || !grads->dL_dopacity || !grads->dL_dmeans3D || !grads->dL_dcov3D ||
 		!grads->dL_dscales || !grads->dL_drotations || (scene->M > 0 && !grads->dL_dsh))
 	{ set_error("gradient output pointers missing"); return GSB_EINVAL; }
 	GeomState g = GeomState::carve(const_cast<char*>(geom_blob), P);
@@ -451,7 +477,8 @@ static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R,
 	float* acc = reinterpret_cast<float*>(const_cast<char*>(geom_blob) + geom_state_bytes(P));
 	if (int e = launch_render_backward(img, b, g, P, W, H, cam->background, dL_dout_color, dL_dinvdepth, dL_dalpha, acc, stream)) return e;
 	float* cam_rows = want_cam ? reinterpret_cast<float*>(cam_workspace) : nullptr;
-	if (int e = launch_preprocess_backward(scene, cam, g, radii, acc, grads, dL_dinvdepth != nullptr, lambda_sh_sparsity, cam_rows, aa, stream))
+	if (int e = launch_preprocess_backward(scene, cam, g, radii, acc, grads, dL_dinvdepth != nullptr, lambda_sh_sparsity, cam_rows, aa, raw,
+		raw_grads, stream))
 		return e;
 	if (want_cam) if (int e = launch_camera_grad_finish(P, cam_rows, dL_dview, dL_dproj, dL_dcampos, stream)) return e;
 	return GSB_OK;
@@ -489,6 +516,39 @@ int gsb_backward_antialiased(const GsbScene* scene, const GsbCamera* cam, int64_
 	{ set_error("backward_antialiased: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
 	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
 		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, true, stream);
+}
+
+int gsb_forward_raw(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
+	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
+	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, float* out_invdepth, float* out_alpha,
+	const GsbRawParams* raw, int32_t antialiasing, void* stream)
+{
+	if (!scene || scene->P < 0) { set_error("forward_raw: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if ((out_invdepth == nullptr) != (out_alpha == nullptr))
+	{ set_error("forward_raw: give both map outputs (invdepth and alpha) or neither"); return GSB_EINVAL; }
+	if (int e = check_raw(scene, raw)) return e;
+	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
+		num_rendered, debug, nullptr, nullptr, out_invdepth, out_alpha, antialiasing != 0, stream, raw);
+}
+
+int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
+	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
+	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
+	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
+	int32_t antialiasing, void* stream)
+{
+	if (!scene || scene->P < 0) { set_error("backward_raw: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
+	{ set_error("backward_raw: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
+	if (int e = check_raw(scene, raw)) return e;
+	if (!raw_grads || !grads) { set_error("backward_raw: grads / raw_grads are NULL"); return GSB_EINVAL; }
+	if (grads->dL_dsh || grads->dL_dscales || grads->dL_drotations)
+	{ set_error("backward_raw: grads->dL_dsh, dL_dscales and dL_drotations must be NULL (raw_grads replaces them)"); return GSB_EINVAL; }
+	if (scene->colors_precomp && (raw_grads->dL_dfeatures_dc || raw_grads->dL_dfeatures_rest))
+	{ set_error("backward_raw: SH gradients requested together with colors_precomp"); return GSB_EINVAL; }
+	if (raw->C == 0 && raw_grads->dL_dfeatures_rest) { set_error("backward_raw: dL_dfeatures_rest given with C == 0"); return GSB_EINVAL; }
+	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, antialiasing != 0, stream, raw, raw_grads);
 }
 
 int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,

@@ -20,6 +20,10 @@ struct BwdArgs {
 	GeomState g; const float* acc;
 	GsbGrads out;
 	float* cam_rows;          // CAM: one row of GSB_CAM_SLOTS partial sums per CTA (the caller's workspace)
+	// IN_RAW (appended: the other modes' parameter offsets stay as they were).  scales / rotations above point at _scaling /
+	// _rotation and out.dL_dscales / dL_drotations receive their gradients; the SH rows come from _features_dc / _features_rest
+	// and their gradients go to dL_ddc / dL_drest (either may be NULL: not written); raw_vec4: every SH pointer is 16-byte aligned
+	const float* sh_dc; const float* sh_rest; float* dL_ddc; float* dL_drest; int n_rest; int raw_vec4;
 };
 
 // Camera gradient slots (CAM): 0..11 view[4r+c] (r = 0..3, c = 0..2) at 3r+c; 12..23 proj[4r+j] (j = 0, 1, 3) at 12+3r+{0,1,2};
@@ -55,6 +59,62 @@ __device__ __forceinline__ void warp_store(float* __restrict__ dst, long long ba
 	__syncwarp();
 }
 
+// RAW: moves the warp's SH rows between the padded shared-memory rows (row r: coefficient 0 in columns 0..2, coefficients 1..C in
+// columns 3..3C+2) and the two tensors, whose 32-row blocks are contiguous: [base, base + n) rows of _features_dc (3 floats each)
+// and of _features_rest (3C floats each).  STORE = false stages the values; STORE = true writes the gradients (zeros when !have)
+// to dL_ddc / dL_drest, whichever is non-NULL, adding them in accumulate mode.  Full warps of 16-byte aligned tensors move float4.
+template <bool STORE, bool ACC>
+__device__ __forceinline__ void raw_block(const float* src, float* dst, int width, int col0, long long base, int n_valid, float* s_row,
+	int RS, int lane, bool have, bool vec4)
+{
+	if (vec4 && n_valid == 32)
+	{
+		const int n4 = 8 * width;                                        // 32 rows * width floats / 4
+		for (int i = lane; i < n4; i += 32)
+		{
+			const int f = 4 * i;
+			int row = f / width, col = f - row * width;
+			if (!STORE)
+			{
+				const float4 v = reinterpret_cast<const float4*>(src + base * width)[i];
+				const float e[4] = { v.x, v.y, v.z, v.w };
+#pragma unroll
+				for (int j = 0; j < 4; j++)
+				{
+					s_row[row * RS + col0 + col] = e[j];
+					if (++col == width) { col = 0; row++; }
+				}
+			}
+			else
+			{
+				float e[4];
+#pragma unroll
+				for (int j = 0; j < 4; j++)
+				{
+					e[j] = have ? s_row[row * RS + col0 + col] : 0.f;
+					if (++col == width) { col = 0; row++; }
+				}
+				float* p = dst + base * width + f;
+				if (ACC)
+				{
+					if (e[0] != 0.f || e[1] != 0.f || e[2] != 0.f || e[3] != 0.f) red_add_f32x4(p, e[0], e[1], e[2], e[3]);
+				}
+				else *reinterpret_cast<float4*>(p) = make_float4(e[0], e[1], e[2], e[3]);
+			}
+		}
+		return;
+	}
+	int row = 0, col = lane;
+	while (col >= width) { col -= width; row++; }
+	for (int f = lane; f < n_valid * width; f += 32)
+	{
+		if (!STORE) s_row[row * RS + col0 + col] = src[base * width + f];
+		else put<ACC>(dst + base * width + f, have ? s_row[row * RS + col0 + col] : 0.f);
+		col += 32;
+		while (col >= width) { col -= width; row++; }
+	}
+}
+
 // One warp per 32 consecutive Gaussians (lane = Gaussian).  The SH rows of the warp (32 x 3M floats, contiguous in HBM) are
 // staged through shared memory with unit-stride loads, overwritten in place by the SH gradients and written back with
 // unit-stride stores; the seven small outputs go through warp_store.  Every output element is written exactly once.
@@ -65,9 +125,15 @@ __device__ __forceinline__ void warp_store(float* __restrict__ dst, long long ba
 // sum.  At the end the CTA sums its 8 warps in warp order into its row of a.cam_rows: no atomics, the same bytes on every run.
 // AA: the forward scaled the opacity by s(cov2D) (DESIGN.md §5e); dL/do^ (accumulator slot 3) also reaches the cov2D through s,
 // before dcov and dL/dT are formed, and from there the 3D covariance, the means through J and, with CAM, the camera.
-template <bool QUANT, bool ACC, bool MAPS, bool CAM, bool AA>
+// RAW (IN == IN_RAW, DESIGN.md §5h): the inputs are the model's leaf parameters.  Their activations are recomputed exactly as the
+// forward applied them, and the gradients are chained back through them in torch's CUDA roundings: dL/d_scaling = dL/ds * s
+// (ExpBackward0), dL/d_rotation = autograd's F.normalize chain (tools/probe_torch_activations.py), the SH gradient row split
+// into its dc and rest parts.  A warp's 32 dc rows (96 floats) and 32 rest rows (96 C floats) are each contiguous and a multiple
+// of 16 bytes: they are staged into the padded rows and written back with 128-bit accesses.
+template <int IN, bool ACC, bool MAPS, bool CAM, bool AA>
 __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs a)
 {
+	constexpr bool QUANT = IN == IN_QUANT, RAW = IN == IN_RAW;
 	extern __shared__ float s_dyn[];
 	float* s_cb = s_dyn;                                                  // QUANT: [20][256]
 	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -87,7 +153,8 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 	// rasterizer_impl.cu:549-571: sh_sparsity_multiplier = lambda / (n_visible * 15 * 3)
 	const float mult = a.lambda != 0.0f ? a.lambda / (float)((int)a.g.counters[1] * 15 * 3) : 0.0f;
 	// colours given by the caller (override_color): the SH coefficients were not used by the forward, their gradient is zero
-	const bool have_sh = (QUANT || a.shs != nullptr) && a.out.dL_dsh != nullptr && a.colors_precomp == nullptr;
+	const bool have_sh = RAW ? (a.sh_dc != nullptr && a.colors_precomp == nullptr)
+	                         : ((QUANT || a.shs != nullptr) && a.out.dL_dsh != nullptr && a.colors_precomp == nullptr);
 	const bool have_scales = QUANT || a.scales != nullptr;
 	float cam_sum = 0.f;                                                  // CAM: this warp's running sum of slot `lane`
 	for (long long base = ((long long)blockIdx.x * 8 + warp) * 32; base < a.P; base += (long long)gridDim.x * 8 * 32)
@@ -97,7 +164,15 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 		const bool valid = lane < n_valid;
 		const bool vis = valid && a.radii[idx] > 0;
 		// ---- stage the warp's SH rows -------------------------------------------------------------
-		if (have_sh && !QUANT && RL == 48 && n_valid == 32)
+		if (RAW)
+		{
+			if (have_sh)
+			{
+				raw_block<false, ACC>(a.sh_dc, nullptr, 3, 0, base, n_valid, s_row, RS, lane, true, a.raw_vec4);
+				if (a.n_rest) raw_block<false, ACC>(a.sh_rest, nullptr, 3 * a.n_rest, 3, base, n_valid, s_row, RS, lane, true, a.raw_vec4);
+			}
+		}
+		else if (have_sh && !QUANT && RL == 48 && n_valid == 32)
 		{
 			// M == 16 fast path: 12 independent 128-bit loads per lane (6 KB contiguous per warp), then scatter to padded rows
 			const float4* src4 = reinterpret_cast<const float4*>(a.shs + base * 48);
@@ -175,6 +250,12 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				qr = s_cb[18 * 256 + (irw & 0xffu)]; qx = s_cb[19 * 256 + ((irw >> 8) & 0xffu)]; qy = s_cb[19 * 256 + ((irw >> 16) & 0xffu)]; qz = s_cb[19 * 256 + (irw >> 24)];
 				normalize_quat(qr, qx, qy, qz);
 				compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);
+			}
+			else if (RAW)
+			{
+				normalize_quat(qr, qx, qy, qz);
+				for (int k = 0; k < 3; k++) sc[k] = exp_ref(sc[k]);
+				compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);      // bit-identical to the forward's
 			}
 			else if (a.cov3D_precomp) { for (int k = 0; k < 6; k++) cov3D[k] = a.cov3D_precomp[6 * idx + k]; }
 			else compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);   // the forward computed exactly this; recomputing is bit-identical
@@ -377,6 +458,26 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				o_rot[1] = 2 * y * (dMt[1][0] + dMt[0][1]) + 2 * z * (dMt[2][0] + dMt[0][2]) + 2 * r * (dMt[1][2] - dMt[2][1]) - 4 * x * (dMt[2][2] + dMt[1][1]);
 				o_rot[2] = 2 * x * (dMt[1][0] + dMt[0][1]) + 2 * r * (dMt[2][0] - dMt[0][2]) + 2 * z * (dMt[1][2] + dMt[2][1]) - 4 * y * (dMt[2][2] + dMt[0][0]);
 				o_rot[3] = 2 * r * (dMt[0][1] - dMt[1][0]) + 2 * x * (dMt[2][0] + dMt[0][2]) + 2 * y * (dMt[1][2] + dMt[2][1]) - 4 * z * (dMt[1][1] + dMt[0][0]);
+				if (RAW)
+				{
+					// ExpBackward0: grad * result
+					for (int k = 0; k < 3; k++) o_sc[k] = __fmul_rn(o_sc[k], sc[k]);
+					// F.normalize = q / expand(clamp_min(norm(q), 1e-12)).  DivBackward0: g / d and -g * ((q / d) / d), where q / d is
+					// the normalised (r, x, y, z) above; ExpandBackward0 sums the four as (0 + 2) + (1 + 3); ClampMinBackward0 passes
+					// it where norm >= 1e-12; LinalgVectorNormBackward0: gn * (q / norm), 0 where norm == 0
+					// the unnormalised rotation is read again here (an L1 / L2 hit) rather than kept live through the covariance
+					const float4 q4 = reinterpret_cast<const float4*>(a.rotations)[idx];
+					const float rq[4] = { q4.x, q4.y, q4.z, q4.w };
+					const float rq_n = quat_norm(q4.x, q4.y, q4.z, q4.w);
+					const float d = fmaxf(rq_n, 1e-12f);
+					const float qn[4] = { r, x, y, z };
+					float go[4];
+					for (int k = 0; k < 4; k++) go[k] = __fmul_rn(-o_rot[k], __fdiv_rn(qn[k], d));
+					const float gsum = __fadd_rn(__fadd_rn(go[0], go[2]), __fadd_rn(go[1], go[3]));
+					const float gn = rq_n >= 1e-12f ? gsum : 0.f;
+					for (int k = 0; k < 4; k++)
+						o_rot[k] = __fadd_rn(__fdiv_rn(o_rot[k], d), rq_n == 0.f ? 0.f : __fmul_rn(gn, __fdiv_rn(rq[k], rq_n)));
+				}
 			}
 			o_m2[0] = g2x; o_m2[1] = g2y;
 			o_col[0] = acc0.x; o_col[1] = acc0.y; o_col[2] = acc0.z;
@@ -389,7 +490,13 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 		}
 		__syncwarp();
 		// ---- unit-stride write-back ------------------------------------------------------------------
-		if (a.out.dL_dsh && RL == 48 && n_valid == 32)
+		if (RAW)
+		{
+			if (a.dL_ddc) raw_block<true, ACC>(nullptr, a.dL_ddc, 3, 0, base, n_valid, s_row, RS, lane, have_sh, a.raw_vec4);
+			if (a.dL_drest && a.n_rest)
+				raw_block<true, ACC>(nullptr, a.dL_drest, 3 * a.n_rest, 3, base, n_valid, s_row, RS, lane, have_sh, a.raw_vec4);
+		}
+		else if (a.out.dL_dsh && RL == 48 && n_valid == 32)
 		{
 			float4* dst4 = reinterpret_cast<float4*>(a.out.dL_dsh + base * 48);
 #pragma unroll
@@ -420,10 +527,10 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 		warp_store<3, ACC>(a.out.dL_dmeans2D, base, n_valid, o_m2, s_tmp, lane);
 		// accumulate mode: THIS view's screen-space gradient on its own (densification statistics are ||.|| per view, gaussian_model.py:693-695)
 		if (ACC && a.out.dL_dmeans2D_view) warp_store<3, false>(a.out.dL_dmeans2D_view, base, n_valid, o_m2, s_tmp, lane);
-		warp_store<3, ACC>(a.out.dL_dcolors, base, n_valid, o_col, s_tmp, lane);
+		if (!RAW || a.out.dL_dcolors) warp_store<3, ACC>(a.out.dL_dcolors, base, n_valid, o_col, s_tmp, lane);
 		warp_store<1, ACC>(a.out.dL_dopacity, base, n_valid, o_op, s_tmp, lane);
 		warp_store<3, ACC>(a.out.dL_dmeans3D, base, n_valid, o_m3, s_tmp, lane);
-		warp_store<6, ACC>(a.out.dL_dcov3D, base, n_valid, o_cov, s_tmp, lane);
+		if (!RAW || a.out.dL_dcov3D) warp_store<6, ACC>(a.out.dL_dcov3D, base, n_valid, o_cov, s_tmp, lane);
 		warp_store<3, ACC>(a.out.dL_dscales, base, n_valid, o_sc, s_tmp, lane);
 		warp_store<4, ACC>(a.out.dL_drotations, base, n_valid, o_rot, s_tmp, lane);
 		if (a.out.dL_dconic) warp_store<4, ACC>(a.out.dL_dconic, base, n_valid, o_con, s_tmp, lane);
@@ -515,7 +622,8 @@ int launch_camera_grad_finish(int P, const float* rows, float* dview, float* dpr
 }
 
 int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const int32_t* radii, const float* acc,
-	const GsbGrads* grads, bool maps, float lambda, float* cam_rows, bool aa, cudaStream_t stream)
+	const GsbGrads* grads, bool maps, float lambda, float* cam_rows, bool aa, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
+	cudaStream_t stream)
 {
 	BwdArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
@@ -527,8 +635,18 @@ int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const Ge
 	a.view = cam->viewmatrix; a.proj = cam->projmatrix; a.campos = cam->campos;
 	a.quant = s->quant != nullptr; if (s->quant) a.q = *s->quant;
 	a.g = g; a.acc = acc; a.out = *grads; a.cam_rows = cam_rows;
+	if (raw)
+	{
+		a.M = raw->features_dc && !s->colors_precomp ? 1 + raw->C : 0;
+		a.scales = raw->scaling; a.rotations = raw->rotation;
+		a.sh_dc = s->colors_precomp ? nullptr : raw->features_dc; a.sh_rest = raw->features_rest; a.n_rest = raw->C;
+		a.out.dL_dscales = raw_grads->dL_dscaling; a.out.dL_drotations = raw_grads->dL_drotation;
+		a.dL_ddc = raw_grads->dL_dfeatures_dc; a.dL_drest = raw_grads->dL_dfeatures_rest;
+		auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
+		a.raw_vec4 = al(a.sh_dc) && al(a.sh_rest) && al(a.dL_ddc) && al(a.dL_drest);
+	}
 	const int grid = preprocess_backward_grid(s->P);
-	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * s->M + 1) + 32 * 6) * sizeof(float);
+	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * a.M + 1) + 32 * 6) * sizeof(float);
 	ProfScope prof(K_PREPROCESS_BWD, stream);
 #define GSB_LAUNCH_PB(Q, A, MP, CM, AA)                                                                               \
 	do {                                                                                                             \
@@ -537,8 +655,9 @@ int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const Ge
 	} while (0)
 #define GSB_LAUNCH_PB_QA(MP, CM, AA)                                                                                 \
 	do {                                                                                                             \
-		if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(true, true, MP, CM, AA); else GSB_LAUNCH_PB(true, false, MP, CM, AA); }  \
-		else { if (grads->accumulate) GSB_LAUNCH_PB(false, true, MP, CM, AA); else GSB_LAUNCH_PB(false, false, MP, CM, AA); }        \
+		if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(IN_QUANT, true, MP, CM, AA); else GSB_LAUNCH_PB(IN_QUANT, false, MP, CM, AA); }  \
+		else if (raw) { if (grads->accumulate) GSB_LAUNCH_PB(IN_RAW, true, MP, CM, AA); else GSB_LAUNCH_PB(IN_RAW, false, MP, CM, AA); }    \
+		else { if (grads->accumulate) GSB_LAUNCH_PB(IN_ACTIVATED, true, MP, CM, AA); else GSB_LAUNCH_PB(IN_ACTIVATED, false, MP, CM, AA); }  \
 	} while (0)
 #define GSB_LAUNCH_PB_MC(AA)                                                                                         \
 	do {                                                                                                             \

@@ -23,6 +23,9 @@ struct PreArgs {
 	int sh_vec4;                                       // dense fp32 SH rows can be read as 12 float4 (M == 16, 16-byte aligned)
 	int rest_aligned;                                  // QUANT: ids_rest is 16-byte aligned (warp-cooperative staging allowed)
 	GsbDebug dbg; int prefiltered;
+	// IN_RAW (appended so that the other modes' parameter offsets, and with them their SASS, stay as they were): scales /
+	// rotations above then point at _scaling / _rotation, the SH rows at _features_dc [P,1,3] and _features_rest [P,n_rest,3]
+	const float* sh_dc; const float* sh_rest; int n_rest;
 };
 
 // forward.cu:105-159 computeColorFromSH with the accumulation order of the reference build
@@ -99,9 +102,12 @@ static_assert(32 * IDS_REST_ROW == GSB_IDS_STAGE_BYTES_PER_WARP, "staging buffer
 // AA (anti-aliasing, DESIGN.md §5e): the opacity is scaled by aa_opacity_factor() of the undilated and dilated cov2D, everywhere
 // the forward uses it (record r1.z, the cull threshold pth, the debug export).  Nothing else in the record, radii, rects or depths
 // changes, so binning is the same as without it.
-template <bool QUANT, bool AA>
+// IN (gsb_common.cuh InputMode): IN_RAW applies exp to the log-scales and normalize_quat to the rotation on load, and reads SH
+// coefficient k from _features_dc (k == 0) or _features_rest (k >= 1): the same values as the activated tensors, bit for bit.
+template <int IN, bool AA>
 __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 {
+	constexpr bool QUANT = IN == IN_QUANT, RAW = IN == IN_RAW;
 	extern __shared__ __align__(16) float s_cb[];   // QUANT: [20][256] centres; scaling row holds exp(centre)
 	if (QUANT)
 	{
@@ -193,6 +199,12 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 #pragma unroll
 						for (int k = 0; k < 6; k++) cov3D[k] = a.cov3D_precomp[6 * idx + k];
 					}
+					else if (RAW)
+					{
+						float r = qrot.x, x = qrot.y, y = qrot.z, z = qrot.w;
+						normalize_quat(r, x, y, z);                                       // get_rotation, gaussian_model.py:145-146
+						compute_cov3D(exp_ref(sc0), exp_ref(sc1), exp_ref(sc2), a.mod, r, x, y, z, cov3D);   // get_scaling, :141-142
+					}
 					else compute_cov3D(sc0, sc1, sc2, a.mod, qrot.x, qrot.y, qrot.z, qrot.w, cov3D);
 					opac_raw = opac_in;
 				}
@@ -281,6 +293,13 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 						sh_to_rgb(deg, dx, dy, dz, [&](int k, int c) {
 							return k == 0 ? dc[c] : s_cb[k * 256 + irest[3 * (k - 1) + c]]; }, res);
 					}
+				}
+				else if (RAW)
+				{
+					// get_features = cat(_features_dc, _features_rest), gaussian_model.py:153-156, without the copy
+					const float* dc = a.sh_dc + 3 * idx;
+					const float* rest = a.sh_rest + 3 * (long long)a.n_rest * idx;
+					sh_to_rgb(deg, dx, dy, dz, [&](int k, int c) { return k == 0 ? dc[c] : rest[3 * (k - 1) + c]; }, res);
 				}
 				else if (a.packed)
 				{
@@ -379,7 +398,7 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D, co
 }
 
 // Debug/test export of the fused de-quantisation: activated scales [P,3] and normalised rotations [P,4] exactly as
-// preprocess_kernel<true> computes them (compared bit-for-bit with torch.exp / F.normalize in the tests).
+// preprocess_kernel<IN_QUANT> computes them (compared bit-for-bit with torch.exp / F.normalize in the tests).
 __global__ void debug_dequant_kernel(int P, GsbQuant q, float* __restrict__ scales, float* __restrict__ rots)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -401,7 +420,7 @@ int launch_debug_dequant(const GsbQuant* q, int P, float* scales, float* rots, c
 }
 
 int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const ImageState& img, const BinPlan& plan, int32_t* radii, const GsbDebug* dbg,
-	bool aa, cudaStream_t stream)
+	bool aa, const GsbRawParams* raw, cudaStream_t stream)
 {
 	PreArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
@@ -431,6 +450,11 @@ int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& 
 	a.hist_priv = plan.priv; a.chunk = plan.chunk; a.T = a.gx * a.gy; a.cta_count = img.cta_count;
 	if (dbg) a.dbg = *dbg;
 	a.prefiltered = cam->prefiltered;
+	if (raw)
+	{
+		a.scales = raw->scaling; a.rotations = raw->rotation;
+		a.sh_dc = raw->features_dc; a.sh_rest = raw->features_rest; a.n_rest = raw->C;
+	}
 	a.sh_vec4 = !a.quant && !a.packed && a.shs && a.M == 16 && (reinterpret_cast<uintptr_t>(a.shs) & 15) == 0;
 	a.rest_aligned = a.quant && (reinterpret_cast<uintptr_t>(a.q.ids_rest) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.q.ids_rot) & 3) == 0;
 	if (a.quant && (reinterpret_cast<uintptr_t>(a.q.ids_rot) & 3) != 0) { set_error("quantised scene: ids_rot must be 4-byte aligned"); return GSB_EINVAL; }
@@ -439,14 +463,17 @@ int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& 
 	const size_t hist_words = plan.priv ? (plan.hist_bytes / 4 + 3) / 4 * 4 : 0;
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE * sizeof(float) : 0) + hist_words * 4 +
 		(a.quant ? size_t(threads / 32) * 32 * IDS_REST_ROW : 0);
-	const void* kernel = a.quant ? (aa ? (const void*)preprocess_kernel<true, true> : (const void*)preprocess_kernel<true, false>)
-	                             : (aa ? (const void*)preprocess_kernel<false, true> : (const void*)preprocess_kernel<false, false>);
+	const int mode = a.quant ? IN_QUANT : (raw ? IN_RAW : IN_ACTIVATED);
+	const void* kernel = mode == IN_QUANT ? (aa ? (const void*)preprocess_kernel<IN_QUANT, true> : (const void*)preprocess_kernel<IN_QUANT, false>)
+	                   : mode == IN_RAW   ? (aa ? (const void*)preprocess_kernel<IN_RAW, true> : (const void*)preprocess_kernel<IN_RAW, false>)
+	                                      : (aa ? (const void*)preprocess_kernel<IN_ACTIVATED, true> : (const void*)preprocess_kernel<IN_ACTIVATED, false>);
 	if (int e = ensure_dyn_smem(kernel, 220 * 1024)) return e;
 	ProfScope prof(K_PREPROCESS, stream);
 	int grid = plan.priv ? plan.ctas : blocks_needed;
 	if (!plan.priv && a.quant && grid > GSB_NUM_SMS * 8) grid = GSB_NUM_SMS * 8;                         // persistent: amortise the table load
-	if (a.quant) { if (aa) preprocess_kernel<true, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<true, false><<<grid, threads, smem, stream>>>(a); }
-	else { if (aa) preprocess_kernel<false, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<false, false><<<grid, threads, smem, stream>>>(a); }
+	if (mode == IN_QUANT) { if (aa) preprocess_kernel<IN_QUANT, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<IN_QUANT, false><<<grid, threads, smem, stream>>>(a); }
+	else if (mode == IN_RAW) { if (aa) preprocess_kernel<IN_RAW, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<IN_RAW, false><<<grid, threads, smem, stream>>>(a); }
+	else { if (aa) preprocess_kernel<IN_ACTIVATED, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<IN_ACTIVATED, false><<<grid, threads, smem, stream>>>(a); }
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;

@@ -8,7 +8,9 @@ receives the forward intermediates in the reference's GeometryState layouts).  `
 inverse-depth and alpha maps in the same pass; `dL_dinvdepth` / `dL_dalpha` (backward) take their gradients (gs_b200.h
 gsb_forward_maps / gsb_backward_maps).  `camera_grads` (backward) also returns the gradients w.r.t. viewmatrix, projmatrix and
 campos (gsb_backward_camera).  `antialiasing` (forward and backward, the same value for both) scales each Gaussian's opacity so
-that the 0.3 px^2 dilation no longer inflates sub-pixel splats (gsb_forward_antialiased / gsb_backward_antialiased).
+that the 0.3 px^2 dilation no longer inflates sub-pixel splats (gsb_forward_antialiased / gsb_backward_antialiased).  `raw`
+(forward and backward) takes the model's leaf parameters (features_dc, features_rest, scaling, rotation) in place of sh, scales
+and rotations, and applies exp / F.normalize / the SH concatenation inside the kernels (gsb_forward_raw / gsb_backward_raw).
 """
 from __future__ import annotations
 
@@ -18,7 +20,10 @@ import math
 import torch
 
 from gs_b200 import lib as _lib
-from gs_b200.lib import GsbCamera, GsbDebug, GsbGrads, GsbQuant, GsbScene, BlobAllocator, f32, on_device, ptr
+from gs_b200.lib import (GsbCamera, GsbDebug, GsbGrads, GsbQuant, GsbRawGrads, GsbRawParams, GsbScene, BlobAllocator, f32, on_device,
+                         ptr)
+
+RAW_REST_COEFFS = (0, 3, 8, 15)     # _features_rest widths of max SH degree 0..3
 
 
 def _carve_f32(device, shapes):
@@ -62,6 +67,58 @@ def _quant_struct(quant, device, keep):
     return C.pointer(q)
 
 
+def _present(t):
+    return t is not None and not (isinstance(t, torch.Tensor) and t.numel() == 0)
+
+
+def _raw_struct(raw, device, P, want_sh, sh, scales, rotations, cov3D_precomp, quant):
+    """raw = (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]): the model's leaf tensors, passed by
+    pointer as they are (no copy, no cast), so each must already be a contiguous fp32 tensor on the device.  Everything is
+    checked before anything is launched.  -> (GsbRawParams, C)."""
+    if quant is not None:
+        raise RuntimeError("raw parameters: a quantised model has no raw fp32 parameters (its kernels activate the codebooks already)")
+    if any(_present(t) for t in (sh, scales, rotations, cov3D_precomp)):
+        raise RuntimeError("raw parameters replace sh, scales and rotations; give those (and cov3D_precomp) empty")
+    if not isinstance(raw, (tuple, list)) or len(raw) != 4:
+        raise RuntimeError("raw parameters: expected (features_dc, features_rest, scaling, rotation)")
+    dc, rest, scaling, rotation = raw
+    if isinstance(rest, (list, tuple)) or isinstance(dc, (list, tuple)):
+        raise RuntimeError("raw parameters: the packed variable-SH layout (a list of per-degree tensors) is not supported")
+
+    checked = []
+
+    def check(name, t, shape):
+        if not isinstance(t, torch.Tensor):
+            raise RuntimeError(f"raw parameters: {name} must be a tensor, got {type(t).__name__}")
+        if t.dtype != torch.float32:
+            raise RuntimeError(f"raw parameters: {name} must be float32, got {t.dtype}")
+        if not t.is_contiguous():
+            raise RuntimeError(f"raw parameters: {name} must be contiguous (it is read in place)")
+        if tuple(t.shape) != tuple(shape):
+            raise RuntimeError(f"raw parameters: {name} must have shape {tuple(shape)}, got {tuple(t.shape)}")
+        checked.append((name, t))
+
+    check("scaling", scaling, (P, 3))
+    check("rotation", rotation, (P, 4))
+    C_rest = 0
+    if want_sh:
+        check("features_dc", dc, (P, 1, 3))
+        if not isinstance(rest, torch.Tensor) or rest.dim() != 3 or rest.shape[2] != 3:
+            raise RuntimeError("raw parameters: features_rest must be a [P, C, 3] tensor")
+        C_rest = int(rest.shape[1])
+        if C_rest not in RAW_REST_COEFFS:
+            raise RuntimeError(f"raw parameters: features_rest has C = {C_rest} coefficients; only {RAW_REST_COEFFS} exist")
+        if int(rest.shape[0]) != P:
+            raise RuntimeError(f"raw parameters: features_dc has {P} rows but features_rest {int(rest.shape[0])}")
+        check("features_rest", rest, (P, C_rest, 3))
+    elif _present(dc) or _present(rest):
+        raise RuntimeError("raw parameters: SH features given together with colors_precomp")
+    for name, t in checked:
+        if not t.is_cuda or t.device != device:
+            raise RuntimeError(f"raw parameters: {name} must live on {device}, got {t.device}")
+    return GsbRawParams(ptr(dc) if want_sh else None, ptr(rest) if want_sh else None, C_rest, ptr(scaling), ptr(rotation)), C_rest
+
+
 def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, sh, degrees, keep,
            packed_counts=None, prune_mask=None, quant=None):
     means3D = f32(means3D, device)
@@ -97,10 +154,15 @@ def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, 
 
 def _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
              tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug, packed_counts=None,
-             prune_mask=None, quant=None, debug_out=None, statistics=None, return_maps=False, antialiasing=False):
+             prune_mask=None, quant=None, debug_out=None, statistics=None, return_maps=False, antialiasing=False, raw=None):
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")          # rasterize_points.cu:158-161
     device = _device_of(means3D)
+    raw_s = None
+    if raw is not None:
+        if packed_counts is not None or statistics is not None:
+            raise RuntimeError("raw parameters: the packed variable-SH and statistics forwards have no raw form")
+        raw_s, _ = _raw_struct(raw, device, int(means3D.shape[0]), not _present(colors), sh, scales, rotations, cov3D_precomp, quant)
     L = _lib.lib()
     keep = []
     H, W = int(image_height), int(image_width)
@@ -125,7 +187,12 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
             dbg = GsbDebug(*[ptr(d[k]) for k in ("depths", "means2D", "cov3D", "conic_opacity", "rgb", "tiles_touched", "clamped")])
             dbg_ptr = C.pointer(dbg)
         R = C.c_int64(0)
-        if statistics is not None:                               # (touched_pixels int32 [P,1], transmittance_sum f32 [P,1]) to fill
+        if raw_s is not None:
+            st = L.gsb_forward_raw(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
+                                   out_color.data_ptr(), ptr(radii), C.byref(R), dbg_ptr, maps[0].data_ptr() if maps else None,
+                                   maps[1].data_ptr() if maps else None, C.byref(raw_s), int(bool(antialiasing)),
+                                   _lib.current_stream(device))
+        elif statistics is not None:                             # (touched_pixels int32 [P,1], transmittance_sum f32 [P,1]) to fill
             st = L.gsb_forward_statistics(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
                                           out_color.data_ptr(), ptr(radii), C.byref(R), ptr(statistics[0]), ptr(statistics[1]),
                                           _lib.current_stream(device))
@@ -152,14 +219,17 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
 
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                         projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                        *, prune_mask=None, quant=None, debug_out=None, return_maps=False, antialiasing=False):
+                        *, prune_mask=None, quant=None, debug_out=None, return_maps=False, antialiasing=False, raw=None):
     """rasterize_points.h:43-63 RasterizeGaussiansCUDA -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer).
     `return_maps`: -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer, invdepth [1,H,W], alpha [1,H,W]) with
     invdepth = sum (1/depth) * alpha * T over the pairs that composite the colour and alpha = 1 - final_T (gsb_forward_maps).
-    `antialiasing`: opacity-compensated 2D filter (gsb_forward_antialiased); its buffers need the backward's `antialiasing=True`."""
+    `antialiasing`: opacity-compensated 2D filter (gsb_forward_antialiased); its buffers need the backward's `antialiasing=True`.
+    `raw`: (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]), the model's leaf parameters, with sh, scales
+    and rotations empty; the kernels read them in place and activate them (gsb_forward_raw).  With colors, features_dc and
+    features_rest are None.  The same output bits as the activated call on cat(dc, rest), exp(scaling), F.normalize(rotation)."""
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                     projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                    None, prune_mask, quant, debug_out, return_maps=return_maps, antialiasing=antialiasing)
+                    None, prune_mask, quant, debug_out, return_maps=return_maps, antialiasing=antialiasing, raw=raw)
 
 
 def rasterize_gaussians_variableSH_bands(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
@@ -179,7 +249,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R,
                                  binningBuffer, imageBuffer, lambda_sh_sparsity, debug, *, prune_mask=None, quant=None,
                                  accumulate_into=None, want_conic=False, view_means2D=None, dL_dinvdepth=None, dL_dalpha=None,
-                                 camera_grads=False, antialiasing=False):
+                                 camera_grads=False, antialiasing=False, raw=None):
     """rasterize_points.h:65-88 RasterizeGaussiansBackwardCUDA ->
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     `accumulate_into`: the same 8-tuple from a previous call; gradients are added in place (view-batch accumulation);
@@ -187,8 +257,17 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     `dL_dinvdepth` / `dL_dalpha` ([1,H,W] each, None = zero): gradients of the maps of `return_maps` (gsb_backward_maps);
     `camera_grads`: the tuple (after dL_dconic when `want_conic`) ends with (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4],
     dL_dcampos [3]) in the layouts of the inputs (gsb_backward_camera); they are this view's gradients, also with `accumulate_into`;
-    `antialiasing`: the backward of a forward with `antialiasing=True` (gsb_backward_antialiased); it must match the forward's flag."""
+    `antialiasing`: the backward of a forward with `antialiasing=True` (gsb_backward_antialiased); it must match the forward's flag.
+    `raw`: the backward of a forward with the same `raw` (gsb_backward_raw).  The 8-tuple then becomes the 9-tuple
+    (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, None, dL_dfeatures_dc, dL_dfeatures_rest, dL_dscaling, dL_drotation):
+    the SH gradient split at coefficient 1, scaling / rotation chained through exp / F.normalize; dL_dcolors only with colors
+    (else None), the SH gradients None with colors, and no dL_dcov3D.  `accumulate_into` takes that 9-tuple."""
     device = _device_of(means3D)
+    if raw is not None:
+        return _backward_raw(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
+                             projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R, binningBuffer,
+                             imageBuffer, lambda_sh_sparsity, debug, prune_mask, quant, accumulate_into, want_conic, view_means2D,
+                             dL_dinvdepth, dL_dalpha, camera_grads, antialiasing, raw, device)
     L = _lib.lib()
     keep = []
     H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
@@ -239,6 +318,63 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             st = L.gsb_backward_maps(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
                                      ptr(imageBuffer), ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
                                      _lib.current_stream(device))
+        _lib.check(st)
+        if debug:
+            torch.cuda.synchronize(device)
+    res = tuple(outs) + ((conic,) if want_conic else ())
+    return res + tuple(cam_out[:3]) if camera_grads else res
+
+
+def _backward_raw(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
+                  tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R, binningBuffer, imageBuffer, lambda_sh_sparsity,
+                  debug, prune_mask, quant, accumulate_into, want_conic, view_means2D, dL_dinvdepth, dL_dalpha, camera_grads,
+                  antialiasing, raw, device):
+    """rasterize_gaussians_backward with `raw` (gsb_backward_raw): the gradients of the raw parameters are the kernel's own outputs."""
+    L = _lib.lib()
+    keep = []
+    P = int(means3D.shape[0])
+    H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
+    want_sh = not _present(colors)
+    raw_s, C_rest = _raw_struct(raw, device, P, want_sh, sh, scales, rotations, cov3D_precomp, quant)
+    with on_device(device):
+        scene, _, _ = _scene(device, means3D, colors, None, None, None, scale_modifier, None, None, degrees, keep, None, prune_mask, None)
+        scene.opacities = means3D.data_ptr() if P > 0 else None          # not read by the backward; keeps the scene check satisfied
+        cam = _camera(device, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, H, W, False, keep)
+        dL = f32(dL_dout_color, device)
+        dmaps = [f32(m, device) for m in (dL_dinvdepth, dL_dalpha)]
+        for m in dmaps:
+            if m is not None and m.numel() != H * W:
+                raise RuntimeError(f"dL_dinvdepth / dL_dalpha must have H*W = {H * W} elements, got {m.numel()}")
+        keep += dmaps
+        cam_shapes = [(4, 4), (4, 4), (3,), ((int(L.gsb_camera_grad_workspace_bytes(P)) + 3) // 4,)] if camera_grads else []
+        # slots: means2D, colors, opacity, means3D, (cov3D: none), features_dc, features_rest, scaling, rotation
+        shapes = [(P, 3), (P, 3) if not want_sh else None, (P, 1), (P, 3), None, (P, 1, 3) if want_sh else None,
+                  (P, C_rest, 3) if want_sh else None, (P, 3), (P, 4)]
+        if accumulate_into is not None:
+            outs = list(accumulate_into)
+            if len(outs) != 9:
+                raise RuntimeError("accumulate_into: the raw backward's 9-tuple is expected")
+            cam_out = _carve_f32(device, cam_shapes) if camera_grads else []
+        else:
+            live = [sh_ for sh_ in shapes if sh_ is not None]
+            carved = _carve_f32(device, live + cam_shapes)
+            it = iter(carved[:len(live)])
+            outs = [next(it) if sh_ is not None else None for sh_ in shapes]
+            cam_out = carved[len(live):]
+        conic = None
+        if want_conic:
+            conic = (torch.zeros if accumulate_into is not None else torch.empty)((P, 4), dtype=torch.float32, device=device)
+        if view_means2D is not None and (accumulate_into is None or tuple(view_means2D.shape) != (P, 3) or
+                                         view_means2D.dtype != torch.float32 or not view_means2D.is_contiguous()):
+            raise RuntimeError("view_means2D needs accumulate_into and a contiguous fp32 [P,3] tensor")
+        g = GsbGrads(ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), None, None, None, None, ptr(conic),
+                     1 if accumulate_into is not None else 0, ptr(view_means2D))
+        rg = GsbRawGrads(ptr(outs[5]), ptr(outs[6]), ptr(outs[7]), ptr(outs[8]))
+        radii = radii.to(device=device, dtype=torch.int32).contiguous()
+        st = L.gsb_backward_raw(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer), ptr(imageBuffer),
+                                ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
+                                *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4), C.byref(raw_s), C.byref(rg),
+                                int(bool(antialiasing)), _lib.current_stream(device))
         _lib.check(st)
         if debug:
             torch.cuda.synchronize(device)

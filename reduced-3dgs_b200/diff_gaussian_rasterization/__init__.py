@@ -11,7 +11,10 @@ constant; GaussianRasterizationSettings takes upstream 3DGS's trailing `antialia
 reference's 12 fields), which turns on the opacity-compensated 2D filter in the forward and the backward; the
 forward no longer forces
 debug=True (reference :85 hard-wires a device sync after every stage); gradients are allocated uninitialised
-because the kernels write every element.
+because the kernels write every element.  GaussianRasterizer.forward also takes keyword-only `raw_params`, the model's leaf
+tensors (features_dc, features_rest, scaling, rotation) in place of shs / scales / rotations: exp, F.normalize and the SH
+concatenation then run inside the kernels, and the gradients of the four tensors are the kernels' own outputs
+(_RasterizeGaussiansRaw).
 """
 from typing import NamedTuple
 
@@ -124,6 +127,90 @@ class _RasterizeGaussians(torch.autograd.Function):
         return grads
 
 
+def _call(fn, args, kw, dump, what):
+    """fn(*args, **kw); in debug mode, a failure first saves a CPU copy of the arguments (reference :90-97)."""
+    if not args[-1]:                                               # raster_settings.debug
+        return fn(*args, **kw)
+    cpu_args = cpu_deep_copy_tuple(args)
+    try:
+        return fn(*args, **kw)
+    except Exception as ex:
+        torch.save(cpu_args, dump)
+        print(f"\nAn error occured in {what}. Please forward {dump} for debugging.")
+        raise ex
+
+
+def rasterize_gaussians_raw(means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
+                            raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False):
+    """rasterize_gaussians on the model's raw parameters (see _RasterizeGaussiansRaw)."""
+    args = (means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation, raster_settings,
+            lambda_sh_sparsity, prune_mask, return_maps)
+    camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
+    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera):
+        return _RasterizeGaussiansRaw.apply(*args, *camera)
+    return _RasterizeGaussiansRaw.apply(*args)
+
+
+class _RasterizeGaussiansRaw(torch.autograd.Function):
+    """_RasterizeGaussians with the model's leaf tensors as inputs: features_dc [P,1,3], features_rest [P,C,3] (empty with
+    colors_precomp), scaling [P,3] (log-scales), rotation [P,4] (unnormalised).  The kernels apply get_features / get_scaling /
+    get_rotation themselves and return the gradients of these four tensors directly, so the graph holds no Cat / Exp / Div node
+    and no [P,16,3] copy or gradient exists.  Outputs, camera handling and `return_maps` as in _RasterizeGaussians."""
+
+    @staticmethod
+    def forward(ctx, means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
+                raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None):
+        ctx.camera_meta = None if viewmatrix is None else [(t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos)]
+        empty = torch.Tensor([])
+        with_colors = colors_precomp.numel() > 0
+        raw = (None, None, scaling, rotation) if with_colors else (features_dc, features_rest, scaling, rotation)
+        args = (raster_settings.bg, means3D, colors_precomp, opacities, empty, empty, raster_settings.scale_modifier, empty,
+                raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
+                raster_settings.image_height, raster_settings.image_width, empty, degrees, raster_settings.campos,
+                raster_settings.prefiltered, raster_settings.debug)
+        out = _call(_C.rasterize_gaussians, args, dict(prune_mask=prune_mask, return_maps=return_maps,
+                                                        antialiasing=raster_settings.antialiasing, raw=raw), "snapshot_fw.dump", "forward")
+        num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = out[:6]
+        ctx.raster_settings = raster_settings
+        ctx.num_rendered = num_rendered
+        ctx.lambda_sh_sparsity = lambda_sh_sparsity
+        ctx.prune_mask = prune_mask
+        ctx.with_colors = with_colors
+        ctx.save_for_backward(colors_precomp, means3D, features_dc, features_rest, scaling, rotation, radii, geomBuffer, binningBuffer,
+                              imgBuffer, degrees)
+        ctx.mark_non_differentiable(radii)
+        if return_maps:
+            ctx.set_materialize_grads(False)
+            return color, radii, out[6], out[7]
+        return color, radii
+
+    @staticmethod
+    def backward(ctx, grad_out_color, _, grad_invdepth=None, grad_alpha=None):
+        rs = ctx.raster_settings
+        (colors_precomp, means3D, features_dc, features_rest, scaling, rotation, radii, geomBuffer, binningBuffer, imgBuffer,
+         degrees) = ctx.saved_tensors
+        if grad_out_color is None:
+            grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
+        need = ctx.needs_input_grad
+        camera_need = need[13:16] if ctx.camera_meta is not None else (False, False, False)
+        empty = torch.Tensor([])
+        raw = (None, None, scaling, rotation) if ctx.with_colors else (features_dc, features_rest, scaling, rotation)
+        args = (rs.bg, means3D, radii, colors_precomp, empty, empty, rs.scale_modifier, empty, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
+                rs.tanfovy, grad_out_color, empty, degrees, rs.campos, geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer,
+                ctx.lambda_sh_sparsity, rs.debug)
+        kw = dict(prune_mask=ctx.prune_mask, dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need),
+                  antialiasing=rs.antialiasing, raw=raw)
+        g = _call(_C.rasterize_gaussians_backward, args, kw, "snapshot_bw.dump", "backward")
+        (grad_means2D, grad_colors, grad_opacities, grad_means3D, _, grad_dc, grad_rest, grad_scaling, grad_rotation) = g[:9]
+        grads = (grad_means3D, grad_means2D, grad_dc if need[2] else None, grad_rest if need[3] else None, None,
+                 grad_colors if need[5] else None, grad_opacities if need[6] else None, grad_scaling if need[7] else None,
+                 grad_rotation if need[8] else None, None, None, None, None)
+        if ctx.camera_meta is not None:
+            grads += tuple(gc.reshape(shape).to(dtype) if n else None
+                           for gc, n, (shape, dtype) in zip(g[9:12] if any(camera_need) else (None,) * 3, camera_need, ctx.camera_meta))
+        return grads
+
+
 class _ReferenceSettings(NamedTuple):
     image_height: int
     image_width: int
@@ -169,9 +256,29 @@ class GaussianRasterizer(nn.Module):
         return visible
 
     def forward(self, means3D, means2D, opacities, shs=None, degrees=None, colors_precomp=None, scales=None,
-                rotations=None, cov3D_precomp=None, lambda_sh_sparsity=0., *, prune_mask=None, quant=None, return_maps=False):
-        """-> (color, radii); with return_maps, (color, radii, invdepth [1,H,W], alpha [1,H,W]), all three differentiable."""
+                rotations=None, cov3D_precomp=None, lambda_sh_sparsity=0., *, prune_mask=None, quant=None, return_maps=False,
+                raw_params=None):
+        """-> (color, radii); with return_maps, (color, radii, invdepth [1,H,W], alpha [1,H,W]), all three differentiable.
+        `raw_params`: (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]), the model's leaf tensors, in place
+        of shs / scales / rotations (which must then be None, as must cov3D_precomp and quant); with colors_precomp the two
+        feature tensors are None.  The kernels apply exp / F.normalize / the concatenation and return the four gradients."""
         raster_settings = self.raster_settings
+        if raw_params is not None:
+            if quant is not None or any(t is not None for t in (shs, scales, rotations, cov3D_precomp)):
+                raise Exception('raw_params replace shs, scales and rotations; leave those, cov3D_precomp and quant None')
+            features_dc, features_rest, scaling, rotation = raw_params
+            empty = torch.Tensor([])
+            if colors_precomp is None:
+                colors_precomp = empty
+            if colors_precomp.numel() > 0:
+                if features_dc is not None or features_rest is not None:
+                    raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+                features_dc = features_rest = empty
+            elif features_dc is None or features_rest is None:
+                raise Exception('Please provide excatly one of either SHs or precomputed colors!')
+            return rasterize_gaussians_raw(means3D, means2D, features_dc, features_rest, degrees, colors_precomp,
+                                           empty if opacities is None else opacities, scaling, rotation, raster_settings,
+                                           lambda_sh_sparsity, prune_mask, return_maps)
         if quant is None:
             if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
                 raise Exception('Please provide excatly one of either SHs or precomputed colors!')

@@ -8,6 +8,10 @@ Build-defined extras: `pc.prune_mask` (optional tensor) and `pc.quant` (optional
 fused kernels when present; `return_maps=True` adds the inverse-depth and alpha maps of the same pass to the dict
 ("invdepth", "alpha", [1,H,W] each; differentiable except on the variable-SH inference path).  `pipe.antialiasing` (upstream
 3DGS's PipelineParams flag; absent = off, as in reduced-3dgs) renders with the opacity-compensated 2D filter, on every path.
+`pipe.fused_activations` (absent = off) renders from the model's raw parameters `_features_dc`, `_features_rest`, `_scaling` and
+`_rotation`: exp, F.normalize and the SH concatenation run inside the kernels, which write the four gradients directly
+(DESIGN.md §5h).  It needs a GaussianModel-like `pc` whose scaling_activation is torch.exp and rotation_activation
+torch.nn.functional.normalize; the variable-SH inference path ignores it.
 
 A learnable camera needs no argument: when world_view_transform, full_proj_transform or camera_center requires grad, the
 rasterizer returns their gradients (the variable-SH inference path stays non-differentiable).  The rasterizer takes
@@ -18,6 +22,7 @@ import math
 import pkgutil
 
 import torch
+import torch.nn.functional as F
 
 # When this package shadows the reference's `gaussian_renderer` on sys.path, its sibling modules (network_gui, imported by
 # train.py next to `render`) must stay importable: let submodule lookups continue into same-named packages further down the path.
@@ -51,6 +56,27 @@ def eval_sh(deg, sh, dirs):
     return result
 
 
+def _raw_params(pc, pipe, override_color):
+    """pipe.fused_activations: the leaf tensors of `pc` for GaussianRasterizer(raw_params=...), after the refusals (nothing runs
+    before they are checked)."""
+    if getattr(pc, "quant", None) is not None:
+        raise RuntimeError("gaussian_renderer.render: pipe.fused_activations needs fp32 parameters; a quantised model is fused already")
+    if pipe.compute_cov3D_python or pipe.convert_SHs_python:
+        raise RuntimeError("gaussian_renderer.render: pipe.fused_activations replaces pipe.compute_cov3D_python / convert_SHs_python; "
+                           "turn those off")
+    if getattr(pc, "scaling_activation", None) is not torch.exp:
+        raise RuntimeError("gaussian_renderer.render: pipe.fused_activations applies exp to pc._scaling; this model's "
+                           "scaling_activation is not torch.exp")
+    if getattr(pc, "rotation_activation", None) is not F.normalize:
+        raise RuntimeError("gaussian_renderer.render: pipe.fused_activations applies F.normalize to pc._rotation; this model's "
+                           "rotation_activation is not torch.nn.functional.normalize")
+    if isinstance(pc._features_rest, (list, tuple)) or isinstance(pc._features_dc, (list, tuple)):
+        raise RuntimeError("gaussian_renderer.render: pipe.fused_activations does not take the packed variable-SH layout")
+    if override_color is not None:
+        return (None, None, pc._scaling, pc._rotation)
+    return (pc._features_dc, pc._features_rest, pc._scaling, pc._rotation)
+
+
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
            lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False, return_maps=False):
     """
@@ -61,6 +87,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     # Create zero tensor. We will use it to make pytorch return gradients of the 2D (screen-space) means.
     # (The reference adds 0 to make it a non-leaf and then calls retain_grad(), GR:27-31; a leaf keeps its .grad by itself and
     # saves an elementwise pass over [P,3].)
+    fused = bool(getattr(pipe, "fused_activations", False)) and not variable_sh_bands
+    raw_params = _raw_params(pc, pipe, override_color) if fused else None
     screenspace_points = torch.zeros_like(pc.get_xyz, dtype=pc.get_xyz.dtype, requires_grad=True, device=pc.get_xyz.device)
 
     tanfovx = math.tan(viewpoint_camera.FoVx * 0.5)
@@ -82,7 +110,9 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
 
     scales = rotations = cov3D_precomp = None
     shs = colors_precomp = None
-    if quant is None:
+    if raw_params is not None:
+        colors_precomp = override_color
+    elif quant is None:
         if pipe.compute_cov3D_python:
             cov3D_precomp = pc.get_covariance(scaling_modifier)
         else:
@@ -132,7 +162,7 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         out = rasterizer(
             means3D=means3D, means2D=means2D, shs=shs, degrees=degrees, colors_precomp=colors_precomp, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, lambda_sh_sparsity=lambda_sh_sparsity,
-            prune_mask=prune_mask, quant=quant, return_maps=return_maps)
+            prune_mask=prune_mask, quant=quant, return_maps=return_maps, raw_params=raw_params)
         rendered_image, radii = out[0], out[1]
         maps = out[2:]
     if measure_fps:

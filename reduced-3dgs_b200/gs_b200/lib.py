@@ -50,6 +50,16 @@ class GsbGrads(C.Structure):
                 ("accumulate", C.c_int32), ("dL_dmeans2D_view", C.c_void_p)]
 
 
+class GsbRawParams(C.Structure):
+    _fields_ = [("features_dc", C.c_void_p), ("features_rest", C.c_void_p), ("C", C.c_int32), ("scaling", C.c_void_p),
+                ("rotation", C.c_void_p)]
+
+
+class GsbRawGrads(C.Structure):
+    _fields_ = [("dL_dfeatures_dc", C.c_void_p), ("dL_dfeatures_rest", C.c_void_p), ("dL_dscaling", C.c_void_p),
+                ("dL_drotation", C.c_void_p)]
+
+
 class GsbAdamTensor(C.Structure):
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
                 ("numel", C.c_int64), ("row_width", C.c_int32), ("sh_offset", C.c_int32), ("one_minus_beta1", C.c_float),
@@ -166,6 +176,11 @@ def lib():
         L.gsb_forward_antialiased.argtypes = L.gsb_forward_maps.argtypes
         L.gsb_backward_antialiased.restype = C.c_int
         L.gsb_backward_antialiased.argtypes = L.gsb_backward_camera.argtypes
+        L.gsb_forward_raw.restype = C.c_int
+        L.gsb_forward_raw.argtypes = L.gsb_forward_maps.argtypes[:-1] + [C.POINTER(GsbRawParams), C.c_int32, C.c_void_p]
+        L.gsb_backward_raw.restype = C.c_int
+        L.gsb_backward_raw.argtypes = L.gsb_backward_camera.argtypes[:-1] + [C.POINTER(GsbRawParams), C.POINTER(GsbRawGrads), C.c_int32,
+                                                                             C.c_void_p]
         L.gsb_mark_visible.restype = C.c_int
         L.gsb_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_export_binning.restype = C.c_int
@@ -220,7 +235,8 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn",
                     "gsb_forward_maps", "gsb_backward_maps", "gsb_camera_grad_workspace_bytes", "gsb_backward_camera",
                     "gsb_forward_antialiased", "gsb_backward_antialiased", "gsb_adam_step", "gsb_densify_stats",
-                    "gsb_densify_workspace_bytes", "gsb_densify_split_std_offset", "gsb_densify_plan", "gsb_densify_emit"]
+                    "gsb_densify_workspace_bytes", "gsb_densify_split_std_offset", "gsb_densify_plan", "gsb_densify_emit",
+                    "gsb_forward_raw", "gsb_backward_raw"]
 
 
 def check(status: int):

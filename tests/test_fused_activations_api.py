@@ -1,0 +1,358 @@
+"""CPU: rendering from the model's raw parameters (`pipe.fused_activations`, gsb_forward_raw / gsb_backward_raw, DESIGN.md §5h):
+the symbols and struct layouts, the GSB_EINVAL cases of the C entry points (all raised before any CUDA call), every refusal of the
+Python layers (raised before anything runs, parameters untouched), and, against a stub of `_C`, that render() hands the
+parameters' own storage to the rasterizer, that the flag reaches the backward, and that the `.grad` tensors are the rasterizer's
+own outputs with no Cat / Exp / Div node in the graph."""
+import ctypes as C
+import os
+import shutil
+import subprocess
+import tempfile
+from types import SimpleNamespace
+
+import pytest
+import torch
+import torch.nn.functional as F
+
+from gs_b200 import lib
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def test_raw_symbols_are_exported():
+    L = lib.lib()
+    for sym in ("gsb_forward_raw", "gsb_backward_raw"):
+        assert sym in lib.EXPORTED_SYMBOLS
+        getattr(L, sym)
+
+
+def test_raw_struct_layouts_match_header():
+    assert C.sizeof(lib.GsbRawParams) == 40
+    assert [getattr(lib.GsbRawParams, f).offset for f in ("features_dc", "features_rest", "C", "scaling", "rotation")] == [0, 8, 16, 24, 32]
+    assert C.sizeof(lib.GsbRawGrads) == 32
+    assert [getattr(lib.GsbRawGrads, f).offset for f in ("dL_dfeatures_dc", "dL_dfeatures_rest", "dL_dscaling", "dL_drotation")] == \
+        [0, 8, 16, 24]
+    cc = shutil.which("cc") or shutil.which("gcc")
+    if cc is None:
+        pytest.skip("no C compiler to read the header's own offsets")
+    src = ('#include <stdio.h>\n#include <stddef.h>\n#include "gs_b200.h"\nint main(void){printf("%zu %zu %zu %zu %zu %zu %zu\\n",'
+           'sizeof(GsbRawParams), offsetof(GsbRawParams, C), offsetof(GsbRawParams, scaling), offsetof(GsbRawParams, rotation),'
+           'sizeof(GsbRawGrads), offsetof(GsbRawGrads, dL_dscaling), offsetof(GsbRawGrads, dL_drotation)); return 0;}\n')
+    with tempfile.TemporaryDirectory() as d:
+        with open(os.path.join(d, "t.c"), "w") as f:
+            f.write(src)
+        subprocess.run([cc, "-I", os.path.join(ROOT, "include"), "-o", os.path.join(d, "t"), os.path.join(d, "t.c")], check=True)
+        got = subprocess.run([os.path.join(d, "t")], check=True, capture_output=True, text=True).stdout.split()
+    assert [int(v) for v in got] == [40, 16, 24, 32, 32, 16, 24]
+
+
+# ---- GSB_EINVAL: nothing below is dereferenced, the checks come before any CUDA call ------------------------------------------
+
+_BUF = (C.c_float * 64)()
+_A = C.addressof(_BUF)
+
+
+def _scene(P=10, **kw):
+    s = lib.GsbScene(P=P)
+    s.means3D = s.opacities = _A
+    s.degrees = _A
+    for k, v in kw.items():
+        setattr(s, k, v)
+    return s
+
+
+def _raw(Cn=15, dc=_A, rest=_A, scaling=_A, rotation=_A):
+    return lib.GsbRawParams(dc, rest if Cn else None, Cn, scaling, rotation)
+
+
+def _fwd(scene, raw, invdepth=None, alpha=None):
+    L = lib.lib()
+    R = C.c_int64(0)
+    cam = lib.GsbCamera()
+    return L.gsb_forward_raw(C.byref(scene) if scene is not None else None, C.byref(cam), lib.ALLOC_FN(0), None, lib.ALLOC_FN(0), None,
+                             lib.ALLOC_FN(0), None, None, None, C.byref(R), None, invdepth, alpha,
+                             C.byref(raw) if raw is not None else None, 0, None)
+
+
+def _bwd(scene, raw, grads=None, raw_grads=None):
+    L = lib.lib()
+    cam = lib.GsbCamera()
+    g = grads if grads is not None else lib.GsbGrads()
+    rg = raw_grads if raw_grads is not None else lib.GsbRawGrads(_A, _A, _A, _A)
+    return L.gsb_backward_raw(C.byref(scene), C.byref(cam), 0, None, None, None, None, None, C.byref(g), None, None, 0.0, None, None, None,
+                              None, C.byref(raw) if raw is not None else None, C.byref(rg), 0, None)
+
+
+@pytest.mark.parametrize("case, msg", [
+    ("no_raw", b"raw parameters are NULL"),
+    ("C5", b"C = 5"),
+    ("scales_set", b"must be NULL"),
+    ("shs_set", b"must be NULL"),
+    ("cov3D_set", b"must be NULL"),
+    ("quant_set", b"must be NULL"),
+    ("packed", b"must be NULL"),
+    ("no_scaling", b"scaling / rotation missing"),
+    ("no_rotation", b"scaling / rotation missing"),
+    ("no_dc", b"features_dc"),
+    ("no_rest", b"features_rest"),
+    ("rest_with_C0", b"features_rest"),
+    ("sh_and_colors", b"colors_precomp"),
+])
+def test_raw_entry_points_refuse(case, msg):
+    scene, raw = _scene(), _raw()
+    if case == "no_raw":
+        raw = None
+    elif case == "C5":
+        raw = _raw(Cn=5)
+    elif case == "scales_set":
+        scene.scales = _A
+    elif case == "shs_set":
+        scene.shs = _A
+    elif case == "cov3D_set":
+        scene.cov3D_precomp = _A
+    elif case == "quant_set":
+        q = lib.GsbQuant()
+        scene.quant = C.pointer(q)
+    elif case == "packed":
+        scene.sh_packed = 1
+    elif case == "no_scaling":
+        raw.scaling = None
+    elif case == "no_rotation":
+        raw.rotation = None
+    elif case == "no_dc":
+        raw.features_dc = None
+    elif case == "no_rest":
+        raw.features_rest = None
+    elif case == "rest_with_C0":
+        raw = _raw(Cn=0)
+        raw.features_rest = _A
+    elif case == "sh_and_colors":
+        scene.colors_precomp = _A
+    L = lib.lib()
+    assert _fwd(scene, raw) == -1 and msg in L.gsb_last_error()
+    assert _bwd(scene, raw) == -1 and msg in L.gsb_last_error()
+
+
+def test_raw_entry_points_refuse_bad_outputs():
+    L = lib.lib()
+    assert _fwd(None, _raw()) == -1 and b"P < 0" in L.gsb_last_error()
+    assert _fwd(_scene(), _raw(), invdepth=_A) == -1 and b"both map outputs" in L.gsb_last_error()
+    for field in ("dL_dsh", "dL_dscales", "dL_drotations"):
+        g = lib.GsbGrads()
+        setattr(g, field, _A)
+        assert _bwd(_scene(), _raw(), grads=g) == -1 and b"must be NULL" in L.gsb_last_error()
+    scene = _scene(colors_precomp=_A)
+    raw = _raw(dc=None, rest=None)
+    assert _bwd(scene, raw, raw_grads=lib.GsbRawGrads(_A, None, _A, _A)) == -1 and b"colors_precomp" in L.gsb_last_error()
+    assert _bwd(_scene(), _raw(Cn=0), raw_grads=lib.GsbRawGrads(_A, _A, _A, _A)) == -1 and b"C == 0" in L.gsb_last_error()
+    # P == 0 needs no tensor at all: the checks pass and the call reaches the scene / camera checks (here: an empty camera)
+    assert _fwd(_scene(P=0), _raw(dc=None, rest=None, scaling=None, rotation=None)) == -1
+    assert b"raw" not in L.gsb_last_error()
+
+
+# ---- Python-side refusals -----------------------------------------------------------------------------------------------------
+
+def _leaves(P=6, Cn=15, device="cpu"):
+    g = torch.Generator().manual_seed(3)
+    return (torch.randn(P, 1, 3, generator=g).to(device), torch.randn(P, Cn, 3, generator=g).to(device),
+            torch.randn(P, 3, generator=g).to(device), torch.randn(P, 4, generator=g).to(device))
+
+
+@pytest.mark.parametrize("case, msg", [
+    ("f64", "float32"), ("noncontig", "contiguous"), ("C5", "C = 5"), ("P_differ", "rows"), ("dc_shape", "shape"),
+    ("rot_shape", "shape"), ("list_rest", "packed"), ("cpu", "must live on"),
+])
+def test_raw_struct_refusals(case, msg):
+    from diff_gaussian_rasterization import _C
+    dc, rest, sc, rot = _leaves()
+    if case == "f64":
+        sc = sc.double()
+    elif case == "noncontig":
+        rot = torch.randn(4, 6).t()
+    elif case == "C5":
+        rest = torch.zeros(6, 5, 3)
+    elif case == "P_differ":
+        rest = torch.zeros(7, 15, 3)
+    elif case == "dc_shape":
+        dc = torch.zeros(6, 3)
+    elif case == "rot_shape":
+        rot = torch.zeros(6, 3)
+    elif case == "list_rest":
+        rest = [torch.zeros(3, 3, 3), torch.zeros(3, 8, 3)]
+    with pytest.raises(RuntimeError, match=msg):
+        _C._raw_struct((dc, rest, sc, rot), torch.device("cpu"), 6, True, None, None, None, None, None)
+
+
+def test_raw_keyword_refuses_activated_inputs_and_cpu():
+    from diff_gaussian_rasterization import _C
+    dc, rest, sc, rot = _leaves()
+    z = torch.zeros(6, 3)
+    with pytest.raises(RuntimeError, match="replace"):
+        _C._raw_struct((dc, rest, sc, rot), torch.device("cpu"), 6, True, torch.zeros(6, 16, 3), None, None, None, None)
+    with pytest.raises(RuntimeError, match="quantised"):
+        _C._raw_struct((dc, rest, sc, rot), torch.device("cpu"), 6, True, None, None, None, None, object())
+    with pytest.raises(RuntimeError):              # CPU means3D: refused before anything else
+        _C.rasterize_gaussians(torch.zeros(3), z, torch.empty(0), torch.zeros(6, 1), torch.empty(0), torch.empty(0), 1.0, torch.empty(0),
+                               torch.eye(4), torch.eye(4), 1.0, 1.0, 8, 8, torch.empty(0), torch.zeros(6, 1, dtype=torch.int32),
+                               torch.zeros(3), False, False, raw=(dc, rest, sc, rot))
+
+
+class _Model:
+    """The reference GaussianModel's attribute names and activations (scene/gaussian_model.py:32-47, 140-163)."""
+
+    def __init__(self, P=6, Cn=15):
+        dc, rest, sc, rot = _leaves(P, Cn)
+        self._xyz = torch.randn(P, 3).requires_grad_()
+        self._features_dc = dc.requires_grad_()
+        self._features_rest = rest.requires_grad_()
+        self._scaling = sc.requires_grad_()
+        self._rotation = rot.requires_grad_()
+        self._opacity = torch.randn(P, 1).requires_grad_()
+        self._degrees = torch.full((P, 1), 3 if Cn == 15 else 0, dtype=torch.int32)
+        self.scaling_activation = torch.exp
+        self.rotation_activation = F.normalize
+        self.active_sh_degree = self.max_sh_degree = {0: 0, 3: 1, 8: 2, 15: 3}[Cn]
+        self.per_band_count = [P, 0, 0, 0]
+
+    get_xyz = property(lambda s: s._xyz)
+    get_scaling = property(lambda s: s.scaling_activation(s._scaling))
+    get_rotation = property(lambda s: s.rotation_activation(s._rotation))
+    get_features = property(lambda s: torch.cat((s._features_dc, s._features_rest), dim=1))
+
+    def leaves(self):
+        return [self._xyz, self._features_dc, self._features_rest, self._scaling, self._rotation, self._opacity]
+
+
+def _camera():
+    return SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=8, image_width=8, world_view_transform=torch.eye(4),
+                           full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
+
+
+def _pipe(**kw):
+    return SimpleNamespace(**{**dict(debug=False, convert_SHs_python=False, compute_cov3D_python=False, fused_activations=True), **kw})
+
+
+@pytest.mark.parametrize("case, msg", [
+    ("quant", "quantised"), ("cov3D_python", "compute_cov3D_python"), ("shs_python", "convert_SHs_python"),
+    ("scaling_act", "scaling_activation"), ("rotation_act", "rotation_activation"), ("no_act", "scaling_activation"),
+    ("packed", "packed"),
+])
+def test_render_refusals_leave_the_model_untouched(monkeypatch, case, msg):
+    import diff_gaussian_rasterization as dgr
+    import gaussian_renderer
+    calls = []
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians", lambda *a, **k: calls.append(1))
+    pc, pipe = _Model(), _pipe()
+    if case == "quant":
+        pc.quant = object()
+    elif case == "cov3D_python":
+        pipe.compute_cov3D_python = True
+    elif case == "shs_python":
+        pipe.convert_SHs_python = True
+    elif case == "scaling_act":
+        pc.scaling_activation = torch.nn.functional.softplus
+    elif case == "rotation_act":
+        pc.rotation_activation = lambda q: q
+    elif case == "no_act":
+        del pc.scaling_activation
+    elif case == "packed":
+        pc._features_rest = [torch.zeros(3, 3, 3), torch.zeros(3, 8, 3)]
+    before = [t.detach().clone() for t in pc.leaves() if isinstance(t, torch.Tensor)]
+    with pytest.raises(RuntimeError, match=msg):
+        gaussian_renderer.render(_camera(), pc, pipe, torch.zeros(3))
+    after = [t for t in pc.leaves() if isinstance(t, torch.Tensor)]
+    assert not calls
+    assert all(torch.equal(a.detach(), b) and a.grad is None for a, b in zip(after, before))
+
+
+# ---- plumbing against a stub _C ------------------------------------------------------------------------------------------------
+
+class _StubC:
+    def __init__(self):
+        self.fw = []
+        self.bw = []
+        self.out_ptrs = None
+
+    def rasterize_gaussians(self, *args, raw=None, antialiasing=False, return_maps=False, **kw):
+        self.fw.append(dict(raw=raw, sh=args[14], scales=args[4], rotations=args[5], colors=args[2], aa=antialiasing))
+        H, W, P = args[12], args[13], args[1].shape[0]
+        out = (1, torch.ones(3, H, W), torch.ones(P, dtype=torch.int32), torch.zeros(8, dtype=torch.uint8),
+               torch.zeros(8, dtype=torch.uint8), torch.zeros(8, dtype=torch.uint8))
+        return out + ((torch.zeros(1, H, W), torch.zeros(1, H, W)) if return_maps else ())
+
+    def rasterize_gaussians_backward(self, *args, raw=None, **kw):
+        self.bw.append(dict(raw=None if raw is None else [None if t is None else t.data_ptr() for t in raw], kw=kw))
+        P = args[1].shape[0]
+        colors = raw is not None and raw[0] is None
+        Cn = 0 if colors else raw[1].shape[1]
+        outs = [torch.full((P, 3), 0.5), torch.full((P, 3), 0.5) if colors else None, torch.full((P, 1), 0.5), torch.full((P, 3), 0.5),
+                None, None if colors else torch.full((P, 1, 3), 0.25), None if colors else torch.full((P, Cn, 3), 0.125),
+                torch.full((P, 3), 0.75), torch.full((P, 4), 1.5)]
+        self.out_ptrs = [None if t is None else t.data_ptr() for t in outs]
+        return tuple(outs)
+
+
+def _graph_names(root):
+    seen, stack, names = set(), [root], []
+    while stack:
+        fn = stack.pop()
+        if fn is None or fn in seen:
+            continue
+        seen.add(fn)
+        names.append(type(fn).__name__)
+        stack.extend(f for f, _ in fn.next_functions)
+    return names
+
+
+@pytest.mark.parametrize("Cn", [0, 3, 8, 15])
+def test_render_passes_the_parameters_own_storage_and_grads(monkeypatch, Cn):
+    import diff_gaussian_rasterization as dgr
+    import gaussian_renderer
+    stub = _StubC()
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
+    pc = _Model(Cn=Cn)
+    pkg = gaussian_renderer.render(_camera(), pc, _pipe(antialiasing=True), torch.zeros(3))
+    f = stub.fw[0]
+    assert f["aa"] is True
+    assert [t.data_ptr() for t in f["raw"]] == [pc._features_dc.data_ptr(), pc._features_rest.data_ptr(), pc._scaling.data_ptr(),
+                                               pc._rotation.data_ptr()]
+    assert all(not (isinstance(t, torch.Tensor) and t.numel()) for t in (f["sh"], f["scales"], f["rotations"]))
+    names = _graph_names(pkg["render"].grad_fn)
+    assert not [n for n in names if any(k in n for k in ("Cat", "Exp", "Div", "Norm", "Clamp", "Expand"))], names
+    assert names.count("AccumulateGrad") == 7                 # xyz, screen-space points, dc, rest, opacity, scaling, rotation
+    pkg["render"].sum().backward()
+    assert stub.bw[0]["raw"] == [t.data_ptr() for t in (pc._features_dc, pc._features_rest, pc._scaling, pc._rotation)]
+    assert stub.bw[0]["kw"]["antialiasing"] is True
+    # the rasterizer's own outputs became .grad: no clone
+    got = [pc._features_dc.grad, pc._features_rest.grad, pc._scaling.grad, pc._rotation.grad]
+    assert [g.data_ptr() for g in got[:1] + got[2:]] == [stub.out_ptrs[5], stub.out_ptrs[7], stub.out_ptrs[8]]
+    assert all(g.is_contiguous() for g in got) and tuple(got[1].shape) == (6, Cn, 3)
+
+
+def test_render_override_color_reads_no_sh(monkeypatch):
+    import diff_gaussian_rasterization as dgr
+    import gaussian_renderer
+    stub = _StubC()
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
+    pc = _Model()
+    colors = torch.rand(6, 3, requires_grad=True)
+    pkg = gaussian_renderer.render(_camera(), pc, _pipe(), torch.zeros(3), override_color=colors)
+    assert stub.fw[0]["raw"][:2] == (None, None) and stub.fw[0]["colors"] is colors
+    pkg["render"].sum().backward()
+    assert stub.bw[0]["raw"][:2] == [None, None]
+    assert pc._features_dc.grad is None and pc._features_rest.grad is None
+    assert colors.grad is not None and pc._scaling.grad is not None
+
+
+def test_flag_off_changes_nothing(monkeypatch):
+    import diff_gaussian_rasterization as dgr
+    import gaussian_renderer
+    stub = _StubC()
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
+    pc = _Model()
+    for pipe in (_pipe(fused_activations=False), SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)):
+        gaussian_renderer.render(_camera(), pc, pipe, torch.zeros(3))
+    assert [f["raw"] for f in stub.fw] == [None, None]
+    assert all(tuple(f["sh"].shape) == (6, 16, 3) and f["scales"].numel() == 18 for f in stub.fw)
