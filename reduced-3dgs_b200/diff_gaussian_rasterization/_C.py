@@ -187,27 +187,18 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
             dbg = GsbDebug(*[ptr(d[k]) for k in ("depths", "means2D", "cov3D", "conic_opacity", "rgb", "tiles_touched", "clamped")])
             dbg_ptr = C.pointer(dbg)
         R = C.c_int64(0)
+        head = (C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None, out_color.data_ptr(),
+                ptr(radii), C.byref(R))
+        map_ptrs = (maps[0].data_ptr(), maps[1].data_ptr()) if maps else (None, None)
+        stream = _lib.current_stream(device)
         if raw_s is not None:
-            st = L.gsb_forward_raw(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
-                                   out_color.data_ptr(), ptr(radii), C.byref(R), dbg_ptr, maps[0].data_ptr() if maps else None,
-                                   maps[1].data_ptr() if maps else None, C.byref(raw_s), int(bool(antialiasing)),
-                                   _lib.current_stream(device))
+            st = L.gsb_forward_raw(*head, dbg_ptr, *map_ptrs, C.byref(raw_s), int(bool(antialiasing)), stream)
         elif statistics is not None:                             # (touched_pixels int32 [P,1], transmittance_sum f32 [P,1]) to fill
-            st = L.gsb_forward_statistics(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
-                                          out_color.data_ptr(), ptr(radii), C.byref(R), ptr(statistics[0]), ptr(statistics[1]),
-                                          _lib.current_stream(device))
-        elif antialiasing:
-            st = L.gsb_forward_antialiased(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
-                                           out_color.data_ptr(), ptr(radii), C.byref(R), dbg_ptr,
-                                           maps[0].data_ptr() if maps else None, maps[1].data_ptr() if maps else None,
-                                           _lib.current_stream(device))
-        elif maps is not None:
-            st = L.gsb_forward_maps(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
-                                    out_color.data_ptr(), ptr(radii), C.byref(R), dbg_ptr, maps[0].data_ptr(), maps[1].data_ptr(),
-                                    _lib.current_stream(device))
+            st = L.gsb_forward_statistics(*head, ptr(statistics[0]), ptr(statistics[1]), stream)
+        elif antialiasing or maps is not None:
+            st = (L.gsb_forward_antialiased if antialiasing else L.gsb_forward_maps)(*head, dbg_ptr, *map_ptrs, stream)
         else:
-            st = L.gsb_forward(C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None,
-                               out_color.data_ptr(), ptr(radii), C.byref(R), dbg_ptr, _lib.current_stream(device))
+            st = L.gsb_forward(*head, dbg_ptr, stream)
         geomB, binB, imgB = blobs.take("geom"), blobs.take("binning"), blobs.take("image")
         _lib.check(st)
         if debug:
@@ -264,10 +255,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     (else None), the SH gradients None with colors, and no dL_dcov3D.  `accumulate_into` takes that 9-tuple."""
     device = _device_of(means3D)
     if raw is not None:
-        return _backward_raw(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
-                             projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R, binningBuffer,
-                             imageBuffer, lambda_sh_sparsity, debug, prune_mask, quant, accumulate_into, want_conic, view_means2D,
-                             dL_dinvdepth, dL_dalpha, camera_grads, antialiasing, raw, device)
+        want_sh = not _present(colors)
+        raw_s, C_rest = _raw_struct(raw, device, int(means3D.shape[0]), want_sh, sh, scales, rotations, cov3D_precomp, quant)
     L = _lib.lib()
     keep = []
     H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
@@ -283,14 +272,25 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             if m is not None and m.numel() != H * W:
                 raise RuntimeError(f"dL_dinvdepth / dL_dalpha must have H*W = {H * W} elements, got {m.numel()}")
         keep += dmaps
+        if raw is None:
+            shapes = [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)]
+        else:
+            # slots: means2D, colors, opacity, means3D, (cov3D: none), features_dc, features_rest, scaling, rotation
+            shapes = [(P, 3), (P, 3) if not want_sh else None, (P, 1), (P, 3), None, (P, 1, 3) if want_sh else None,
+                      (P, C_rest, 3) if want_sh else None, (P, 3), (P, 4)]
         # camera gradients and their workspace ride in the same single allocation as the per-Gaussian outputs
         cam_shapes = [(4, 4), (4, 4), (3,), ((int(L.gsb_camera_grad_workspace_bytes(P)) + 3) // 4,)] if camera_grads else []
         if accumulate_into is not None:
             outs = list(accumulate_into)
+            if raw is not None and len(outs) != 9:
+                raise RuntimeError("accumulate_into: the raw backward's 9-tuple is expected")
             cam_out = _carve_f32(device, cam_shapes) if camera_grads else []
         else:
-            outs = _carve_f32(device, [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)] + cam_shapes)
-            outs, cam_out = outs[:8], outs[8:]
+            live = [s for s in shapes if s is not None]
+            carved = _carve_f32(device, live + cam_shapes)
+            it = iter(carved)
+            outs = [next(it) if s is not None else None for s in shapes]
+            cam_out = carved[len(live):]
         # accumulate mode ADDS into every output, this fresh one included: it must start from zero
         conic = None
         if want_conic:
@@ -298,83 +298,20 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         if view_means2D is not None and (accumulate_into is None or tuple(view_means2D.shape) != (P, 3) or
                                          view_means2D.dtype != torch.float32 or not view_means2D.is_contiguous()):
             raise RuntimeError("view_means2D needs accumulate_into and a contiguous fp32 [P,3] tensor")
-        g = GsbGrads(ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), ptr(outs[4]), ptr(outs[5]), ptr(outs[6]), ptr(outs[7]),
-                     ptr(conic), 1 if accumulate_into is not None else 0, ptr(view_means2D))
-        radii = radii.to(device=device, dtype=torch.int32).contiguous()
-        if antialiasing:
-            st = L.gsb_backward_antialiased(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
-                                            ptr(imageBuffer), ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]),
-                                            float(lambda_sh_sparsity), *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4),
-                                            _lib.current_stream(device))
-        elif camera_grads:
-            st = L.gsb_backward_camera(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
-                                       ptr(imageBuffer), ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
-                                       cam_out[0].data_ptr(), cam_out[1].data_ptr(), cam_out[2].data_ptr(), cam_out[3].data_ptr(),
-                                       _lib.current_stream(device))
-        elif dmaps[0] is None and dmaps[1] is None:
-            st = L.gsb_backward(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
-                                ptr(imageBuffer), ptr(dL), C.byref(g), float(lambda_sh_sparsity), _lib.current_stream(device))
-        else:
-            st = L.gsb_backward_maps(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer),
-                                     ptr(imageBuffer), ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
-                                     _lib.current_stream(device))
-        _lib.check(st)
-        if debug:
-            torch.cuda.synchronize(device)
-    res = tuple(outs) + ((conic,) if want_conic else ())
-    return res + tuple(cam_out[:3]) if camera_grads else res
-
-
-def _backward_raw(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
-                  tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R, binningBuffer, imageBuffer, lambda_sh_sparsity,
-                  debug, prune_mask, quant, accumulate_into, want_conic, view_means2D, dL_dinvdepth, dL_dalpha, camera_grads,
-                  antialiasing, raw, device):
-    """rasterize_gaussians_backward with `raw` (gsb_backward_raw): the gradients of the raw parameters are the kernel's own outputs."""
-    L = _lib.lib()
-    keep = []
-    P = int(means3D.shape[0])
-    H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
-    want_sh = not _present(colors)
-    raw_s, C_rest = _raw_struct(raw, device, P, want_sh, sh, scales, rotations, cov3D_precomp, quant)
-    with on_device(device):
-        scene, _, _ = _scene(device, means3D, colors, None, None, None, scale_modifier, None, None, degrees, keep, None, prune_mask, None)
-        scene.opacities = means3D.data_ptr() if P > 0 else None          # not read by the backward; keeps the scene check satisfied
-        cam = _camera(device, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, H, W, False, keep)
-        dL = f32(dL_dout_color, device)
-        dmaps = [f32(m, device) for m in (dL_dinvdepth, dL_dalpha)]
-        for m in dmaps:
-            if m is not None and m.numel() != H * W:
-                raise RuntimeError(f"dL_dinvdepth / dL_dalpha must have H*W = {H * W} elements, got {m.numel()}")
-        keep += dmaps
-        cam_shapes = [(4, 4), (4, 4), (3,), ((int(L.gsb_camera_grad_workspace_bytes(P)) + 3) // 4,)] if camera_grads else []
-        # slots: means2D, colors, opacity, means3D, (cov3D: none), features_dc, features_rest, scaling, rotation
-        shapes = [(P, 3), (P, 3) if not want_sh else None, (P, 1), (P, 3), None, (P, 1, 3) if want_sh else None,
-                  (P, C_rest, 3) if want_sh else None, (P, 3), (P, 4)]
-        if accumulate_into is not None:
-            outs = list(accumulate_into)
-            if len(outs) != 9:
-                raise RuntimeError("accumulate_into: the raw backward's 9-tuple is expected")
-            cam_out = _carve_f32(device, cam_shapes) if camera_grads else []
-        else:
-            live = [sh_ for sh_ in shapes if sh_ is not None]
-            carved = _carve_f32(device, live + cam_shapes)
-            it = iter(carved[:len(live)])
-            outs = [next(it) if sh_ is not None else None for sh_ in shapes]
-            cam_out = carved[len(live):]
-        conic = None
-        if want_conic:
-            conic = (torch.zeros if accumulate_into is not None else torch.empty)((P, 4), dtype=torch.float32, device=device)
-        if view_means2D is not None and (accumulate_into is None or tuple(view_means2D.shape) != (P, 3) or
-                                         view_means2D.dtype != torch.float32 or not view_means2D.is_contiguous()):
-            raise RuntimeError("view_means2D needs accumulate_into and a contiguous fp32 [P,3] tensor")
-        g = GsbGrads(ptr(outs[0]), ptr(outs[1]), ptr(outs[2]), ptr(outs[3]), None, None, None, None, ptr(conic),
+        # raw mode: GsbRawGrads takes the SH, scaling and rotation slots, and GsbGrads leaves its own NULL
+        g = GsbGrads(*[ptr(t) for t in (outs[:8] if raw is None else outs[:4] + [None] * 4)], ptr(conic),
                      1 if accumulate_into is not None else 0, ptr(view_means2D))
-        rg = GsbRawGrads(ptr(outs[5]), ptr(outs[6]), ptr(outs[7]), ptr(outs[8]))
         radii = radii.to(device=device, dtype=torch.int32).contiguous()
-        st = L.gsb_backward_raw(C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer), ptr(imageBuffer),
-                                ptr(dL), C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
-                                *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4), C.byref(raw_s), C.byref(rg),
-                                int(bool(antialiasing)), _lib.current_stream(device))
+        head = (C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer), ptr(imageBuffer), ptr(dL),
+                C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
+                *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4))
+        stream = _lib.current_stream(device)
+        if raw is not None:
+            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]])
+            st = L.gsb_backward_raw(*head, C.byref(raw_s), C.byref(rg), int(bool(antialiasing)), stream)
+        else:
+            # with NULL map and camera pointers this is exactly gsb_backward / gsb_backward_maps
+            st = (L.gsb_backward_antialiased if antialiasing else L.gsb_backward_camera)(*head, stream)
         _lib.check(st)
         if debug:
             torch.cuda.synchronize(device)

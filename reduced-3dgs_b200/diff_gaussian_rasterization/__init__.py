@@ -29,15 +29,74 @@ def cpu_deep_copy_tuple(input_tuple):
     return tuple(copied_tensors)
 
 
-def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False):
-    args = (means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
-            lambda_sh_sparsity, prune_mask, quant, return_maps)
+def _call(fn, args, kw, dump, message):
+    """fn(*args, **kw); in debug mode, a failure first saves a CPU copy of the arguments to `dump` (reference :90-97, 142-149)."""
+    if not args[-1]:                                               # raster_settings.debug
+        return fn(*args, **kw)
+    cpu_args = cpu_deep_copy_tuple(args)   # Copy them before they can be corrupted
+    try:
+        return fn(*args, **kw)
+    except Exception as ex:
+        torch.save(cpu_args, dump)
+        print(message)
+        raise ex
+
+
+def _apply(op, raster_settings, *args):
     camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
     if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera):
         # a learnable camera: the three tensors become inputs of the autograd op so that their gradients have a destination
-        return _RasterizeGaussians.apply(*args, *camera)
-    return _RasterizeGaussians.apply(*args)
+        return op.apply(*args, *camera)
+    return op.apply(*args)
+
+
+def _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, camera, **kw):
+    """The forward both ops share: the _C call and the ctx state their backwards read.  `camera` is (viewmatrix, projmatrix,
+    campos), raster_settings' own tensors, passed again as inputs only when the camera is learnable, else (None, None, None).
+    -> (_C.rasterize_gaussians' tuple, the op's outputs: (color, radii) or, with return_maps, (color, radii, invdepth, alpha))."""
+    ctx.camera_meta = None if camera[0] is None else [(t.shape, t.dtype) for t in camera]
+    kw.update(prune_mask=prune_mask, return_maps=return_maps, antialiasing=raster_settings.antialiasing)
+    out = _call(_C.rasterize_gaussians, args, kw,
+                "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
+    ctx.raster_settings = raster_settings
+    ctx.num_rendered = out[0]
+    ctx.lambda_sh_sparsity = lambda_sh_sparsity
+    ctx.prune_mask = prune_mask
+    ctx.mark_non_differentiable(out[2])
+    if return_maps:
+        # a loss on some outputs only: the others' gradients arrive as None and reach the kernels as NULL (zero)
+        ctx.set_materialize_grads(False)
+        return out, (out[1], out[2], out[6], out[7])
+    return out, (out[1], out[2])
+
+
+def _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp,
+              sh, degrees, geomBuffer, binningBuffer, imgBuffer, **kw):
+    """The backward both ops share: the _C call from the saved state.  -> (its gradient tuple, the gradients of the camera
+    inputs: () for a constant camera, else one per tensor, None where not needed)."""
+    rs = ctx.raster_settings
+    if grad_out_color is None:
+        grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
+    # the camera tensors are the op's last three inputs when it has them
+    camera_need = ctx.needs_input_grad[-3:] if ctx.camera_meta is not None else (False, False, False)
+    args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
+            rs.tanfovx, rs.tanfovy, grad_out_color, sh, degrees, rs.campos, geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer,
+            ctx.lambda_sh_sparsity, rs.debug)
+    kw.update(prune_mask=ctx.prune_mask, dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need),
+              antialiasing=rs.antialiasing)
+    g = _call(_C.rasterize_gaussians_backward, args, kw,
+              "snapshot_bw.dump", "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
+    if ctx.camera_meta is None:
+        return g, ()
+    # with camera_grads the tuple ends with (dL_dviewmatrix, dL_dprojmatrix, dL_dcampos)
+    return g, tuple(gc.reshape(shape).to(dtype) if n else None
+                    for gc, n, (shape, dtype) in zip(g[-3:] if any(camera_need) else (None,) * 3, camera_need, ctx.camera_meta))
+
+
+def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                        raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False):
+    return _apply(_RasterizeGaussians, raster_settings, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations,
+                  cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -45,110 +104,46 @@ class _RasterizeGaussians(torch.autograd.Function):
     def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, viewmatrix=None,
                 projmatrix=None, campos=None):
-        # viewmatrix / projmatrix / campos are raster_settings' own tensors, passed again only when the camera is learnable
-        ctx.camera_meta = None if viewmatrix is None else [(t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos)]
         args = (raster_settings.bg, means3D, colors_precomp, opacities, scales, rotations, raster_settings.scale_modifier,
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, raster_settings.image_height, raster_settings.image_width, sh, degrees,
                 raster_settings.campos, raster_settings.prefiltered, raster_settings.debug)
-        fw = dict(prune_mask=prune_mask, quant=quant, return_maps=return_maps, antialiasing=raster_settings.antialiasing)
-        if raster_settings.debug:
-            cpu_args = cpu_deep_copy_tuple(args)   # Copy them before they can be corrupted (reference :90-97)
-            try:
-                out = _C.rasterize_gaussians(*args, **fw)
-            except Exception as ex:
-                torch.save(cpu_args, "snapshot_fw.dump")
-                print("\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
-                raise ex
-        else:
-            out = _C.rasterize_gaussians(*args, **fw)
-        num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = out[:6]
-        ctx.raster_settings = raster_settings
-        ctx.num_rendered = num_rendered
-        ctx.lambda_sh_sparsity = lambda_sh_sparsity
-        ctx.prune_mask = prune_mask
+        out, outputs = _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, (viewmatrix, projmatrix, campos),
+                                quant=quant)
         ctx.quant = quant
-        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer,
-                              binningBuffer, imgBuffer, degrees)
-        ctx.mark_non_differentiable(radii)
-        if return_maps:
-            # a loss on some outputs only: the others' gradients arrive as None and reach the kernels as NULL (zero)
-            ctx.set_materialize_grads(False)
-            return color, radii, out[6], out[7]
-        return color, radii
+        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, out[2], sh, out[3], out[4], out[5], degrees)
+        return outputs
 
     @staticmethod
     def backward(ctx, grad_out_color, _, grad_invdepth=None, grad_alpha=None):
-        num_rendered = ctx.num_rendered
-        raster_settings = ctx.raster_settings
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer,
          degrees) = ctx.saved_tensors
-        if grad_out_color is None:
-            grad_out_color = torch.zeros((3, raster_settings.image_height, raster_settings.image_width), dtype=torch.float32,
-                                         device=means3D.device)
-        need = ctx.needs_input_grad
-        camera_need = need[14:17] if ctx.camera_meta is not None else (False, False, False)
-        maps = dict(dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need),
-                    antialiasing=raster_settings.antialiasing)
-        args = (raster_settings.bg, means3D, radii, colors_precomp, scales, rotations, raster_settings.scale_modifier,
-                cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
-                raster_settings.tanfovy, grad_out_color, sh, degrees, raster_settings.campos, geomBuffer, num_rendered,
-                binningBuffer, imgBuffer, ctx.lambda_sh_sparsity, raster_settings.debug)
-        if raster_settings.debug:
-            cpu_args = cpu_deep_copy_tuple(args)
-            try:
-                grads8 = _C.rasterize_gaussians_backward(*args, prune_mask=ctx.prune_mask, quant=ctx.quant, **maps)
-            except Exception as ex:
-                torch.save(cpu_args, "snapshot_bw.dump")
-                print("\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
-                raise ex
-        else:
-            grads8 = _C.rasterize_gaussians_backward(*args, prune_mask=ctx.prune_mask, quant=ctx.quant, **maps)
+        g, grad_camera = _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, scales, rotations,
+                                   cov3Ds_precomp, sh, degrees, geomBuffer, binningBuffer, imgBuffer, quant=ctx.quant)
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
-         grad_rotations) = grads8[:8]
+         grad_rotations) = g[:8]
         if ctx.quant is not None:
             # inputs were id planes: the per-Gaussian attribute gradients have no autograd destination; expose them with the
             # semantics of `.grad`: they accumulate over backward calls until the caller resets `quant.grads = None`
             new = dict(sh=grad_sh, opacity=grad_opacities, scales=grad_scales, rotations=grad_rotations)
             old = getattr(ctx.quant, "grads", None)
             if old:
-                for k, g in new.items():
-                    old[k].add_(g)
+                for k, t in new.items():
+                    old[k].add_(t)
             else:
                 ctx.quant.grads = new
-        grads = (grad_means3D, grad_means2D, grad_sh if need[2] else None, None,
-                 grad_colors_precomp if need[4] else None, grad_opacities if need[5] else None,
-                 grad_scales if need[6] else None, grad_rotations if need[7] else None,
-                 grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None)
-        if ctx.camera_meta is not None:
-            grads += tuple(g.reshape(shape).to(dtype) if n else None
-                           for g, n, (shape, dtype) in zip(grads8[8:11] if any(camera_need) else (None,) * 3, camera_need,
-                                                           ctx.camera_meta))
-        return grads
-
-
-def _call(fn, args, kw, dump, what):
-    """fn(*args, **kw); in debug mode, a failure first saves a CPU copy of the arguments (reference :90-97)."""
-    if not args[-1]:                                               # raster_settings.debug
-        return fn(*args, **kw)
-    cpu_args = cpu_deep_copy_tuple(args)
-    try:
-        return fn(*args, **kw)
-    except Exception as ex:
-        torch.save(cpu_args, dump)
-        print(f"\nAn error occured in {what}. Please forward {dump} for debugging.")
-        raise ex
+        need = ctx.needs_input_grad
+        return (grad_means3D, grad_means2D, grad_sh if need[2] else None, None,
+                grad_colors_precomp if need[4] else None, grad_opacities if need[5] else None,
+                grad_scales if need[6] else None, grad_rotations if need[7] else None,
+                grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None) + grad_camera
 
 
 def rasterize_gaussians_raw(means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
                             raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False):
     """rasterize_gaussians on the model's raw parameters (see _RasterizeGaussiansRaw)."""
-    args = (means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation, raster_settings,
-            lambda_sh_sparsity, prune_mask, return_maps)
-    camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
-    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera):
-        return _RasterizeGaussiansRaw.apply(*args, *camera)
-    return _RasterizeGaussiansRaw.apply(*args)
+    return _apply(_RasterizeGaussiansRaw, raster_settings, means3D, means2D, features_dc, features_rest, degrees, colors_precomp,
+                  opacities, scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps)
 
 
 class _RasterizeGaussiansRaw(torch.autograd.Function):
@@ -160,7 +155,6 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
                 raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None):
-        ctx.camera_meta = None if viewmatrix is None else [(t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos)]
         empty = torch.Tensor([])
         with_colors = colors_precomp.numel() > 0
         raw = (None, None, scaling, rotation) if with_colors else (features_dc, features_rest, scaling, rotation)
@@ -168,47 +162,26 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                 raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
                 raster_settings.image_height, raster_settings.image_width, empty, degrees, raster_settings.campos,
                 raster_settings.prefiltered, raster_settings.debug)
-        out = _call(_C.rasterize_gaussians, args, dict(prune_mask=prune_mask, return_maps=return_maps,
-                                                        antialiasing=raster_settings.antialiasing, raw=raw), "snapshot_fw.dump", "forward")
-        num_rendered, color, radii, geomBuffer, binningBuffer, imgBuffer = out[:6]
-        ctx.raster_settings = raster_settings
-        ctx.num_rendered = num_rendered
-        ctx.lambda_sh_sparsity = lambda_sh_sparsity
-        ctx.prune_mask = prune_mask
+        out, outputs = _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, (viewmatrix, projmatrix, campos),
+                                raw=raw)
         ctx.with_colors = with_colors
-        ctx.save_for_backward(colors_precomp, means3D, features_dc, features_rest, scaling, rotation, radii, geomBuffer, binningBuffer,
-                              imgBuffer, degrees)
-        ctx.mark_non_differentiable(radii)
-        if return_maps:
-            ctx.set_materialize_grads(False)
-            return color, radii, out[6], out[7]
-        return color, radii
+        ctx.save_for_backward(colors_precomp, means3D, features_dc, features_rest, scaling, rotation, out[2], out[3], out[4], out[5],
+                              degrees)
+        return outputs
 
     @staticmethod
     def backward(ctx, grad_out_color, _, grad_invdepth=None, grad_alpha=None):
-        rs = ctx.raster_settings
         (colors_precomp, means3D, features_dc, features_rest, scaling, rotation, radii, geomBuffer, binningBuffer, imgBuffer,
          degrees) = ctx.saved_tensors
-        if grad_out_color is None:
-            grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
-        need = ctx.needs_input_grad
-        camera_need = need[13:16] if ctx.camera_meta is not None else (False, False, False)
         empty = torch.Tensor([])
         raw = (None, None, scaling, rotation) if ctx.with_colors else (features_dc, features_rest, scaling, rotation)
-        args = (rs.bg, means3D, radii, colors_precomp, empty, empty, rs.scale_modifier, empty, rs.viewmatrix, rs.projmatrix, rs.tanfovx,
-                rs.tanfovy, grad_out_color, empty, degrees, rs.campos, geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer,
-                ctx.lambda_sh_sparsity, rs.debug)
-        kw = dict(prune_mask=ctx.prune_mask, dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need),
-                  antialiasing=rs.antialiasing, raw=raw)
-        g = _call(_C.rasterize_gaussians_backward, args, kw, "snapshot_bw.dump", "backward")
+        g, grad_camera = _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, empty, empty, empty,
+                                   empty, degrees, geomBuffer, binningBuffer, imgBuffer, raw=raw)
         (grad_means2D, grad_colors, grad_opacities, grad_means3D, _, grad_dc, grad_rest, grad_scaling, grad_rotation) = g[:9]
-        grads = (grad_means3D, grad_means2D, grad_dc if need[2] else None, grad_rest if need[3] else None, None,
-                 grad_colors if need[5] else None, grad_opacities if need[6] else None, grad_scaling if need[7] else None,
-                 grad_rotation if need[8] else None, None, None, None, None)
-        if ctx.camera_meta is not None:
-            grads += tuple(gc.reshape(shape).to(dtype) if n else None
-                           for gc, n, (shape, dtype) in zip(g[9:12] if any(camera_need) else (None,) * 3, camera_need, ctx.camera_meta))
-        return grads
+        need = ctx.needs_input_grad
+        return (grad_means3D, grad_means2D, grad_dc if need[2] else None, grad_rest if need[3] else None, None,
+                grad_colors if need[5] else None, grad_opacities if need[6] else None, grad_scaling if need[7] else None,
+                grad_rotation if need[8] else None, None, None, None, None) + grad_camera
 
 
 class _ReferenceSettings(NamedTuple):
@@ -267,36 +240,20 @@ class GaussianRasterizer(nn.Module):
             if quant is not None or any(t is not None for t in (shs, scales, rotations, cov3D_precomp)):
                 raise Exception('raw_params replace shs, scales and rotations; leave those, cov3D_precomp and quant None')
             features_dc, features_rest, scaling, rotation = raw_params
-            empty = torch.Tensor([])
-            if colors_precomp is None:
-                colors_precomp = empty
-            if colors_precomp.numel() > 0:
-                if features_dc is not None or features_rest is not None:
-                    raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-                features_dc = features_rest = empty
-            elif features_dc is None or features_rest is None:
-                raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-            return rasterize_gaussians_raw(means3D, means2D, features_dc, features_rest, degrees, colors_precomp,
-                                           empty if opacities is None else opacities, scaling, rotation, raster_settings,
-                                           lambda_sh_sparsity, prune_mask, return_maps)
+            # the SHs are the two feature tensors, and an empty colors_precomp counts as none (the raw op reads it so)
+            sh, with_colors = (features_dc, features_rest), colors_precomp is not None and colors_precomp.numel() > 0
+        else:
+            sh, with_colors = (shs,), colors_precomp is not None
         if quant is None:
-            if (shs is None and colors_precomp is None) or (shs is not None and colors_precomp is not None):
+            if any(t is not None for t in sh) if with_colors else any(t is None for t in sh):
                 raise Exception('Please provide excatly one of either SHs or precomputed colors!')
-            if ((scales is None or rotations is None) and cov3D_precomp is None) or \
-                    ((scales is not None or rotations is not None) and cov3D_precomp is not None):
+            if raw_params is None and (((scales is None or rotations is None) and cov3D_precomp is None) or
+                                       ((scales is not None or rotations is not None) and cov3D_precomp is not None)):
                 raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
         empty = torch.Tensor([])
-        if shs is None:
-            shs = empty
-        if colors_precomp is None:
-            colors_precomp = empty
-        if scales is None:
-            scales = empty
-        if rotations is None:
-            rotations = empty
-        if cov3D_precomp is None:
-            cov3D_precomp = empty
-        if opacities is None:
-            opacities = empty
-        return rasterize_gaussians(means3D, means2D, shs, degrees, colors_precomp, opacities, scales, rotations,
-                                   cov3D_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps)
+        e = lambda t: empty if t is None else t                                  # absent inputs travel as empty tensors
+        if raw_params is not None:
+            return rasterize_gaussians_raw(means3D, means2D, e(features_dc), e(features_rest), degrees, e(colors_precomp), e(opacities),
+                                           scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps)
+        return rasterize_gaussians(means3D, means2D, e(shs), degrees, e(colors_precomp), e(opacities), e(scales), e(rotations),
+                                   e(cov3D_precomp), raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps)

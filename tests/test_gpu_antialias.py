@@ -11,9 +11,9 @@
   8. 90 Adam steps through render() with pipe.antialiasing reduce the loss.
 Observed maxima are printed (pytest -s)."""
 import math
+from functools import partial
 from types import SimpleNamespace
 
-import numpy as np
 import pytest
 import torch
 
@@ -30,13 +30,6 @@ EMPTY = torch.Tensor([])
 H_DIL = 0.3
 
 
-def _yaw_cam(W, H, deg, dev=DEV):
-    th = math.radians(deg)
-    Rc2w = np.array([[math.cos(th), 0, math.sin(th)], [0, 1, 0], [-math.sin(th), 0, math.cos(th)]])
-    C = Rc2w @ np.array([0.0, 0.0, -4.0])
-    return synth.make_camera(W, H, Rc2w, -Rc2w.T @ C).to(dev)
-
-
 def _config(name):
     """-> (scene, cam on DEV, prune_mask or None, quant or None)."""
     if name == "c1":
@@ -45,45 +38,19 @@ def _config(name):
     W, H = 320, 200
     box, ls = (1.9 * W / H, 1.9, 1.0), math.log(0.02)
     if name == "mixed":
-        return synth.make_scene(20_000, 201, mixed_degrees=True, box=box, log_scale_mean=ls), _yaw_cam(W, H, -5.0), None, None
+        return synth.make_scene(20_000, 201, mixed_degrees=True, box=box, log_scale_mean=ls), O.yaw_cam(W, H, -5.0), None, None
     if name == "quant":
         scene = synth.make_scene(20_000, 202, mixed_degrees=True, box=box, log_scale_mean=ls)
-        return scene, _yaw_cam(W, H, 4.0), None, synth.quantise_scene(scene)
+        return scene, O.yaw_cam(W, H, 4.0), None, synth.quantise_scene(scene)
     if name == "pruned":
         scene = synth.make_scene(20_000, 203, sh_degree=2, box=box, log_scale_mean=ls)
-        return scene, _yaw_cam(W, H, -3.0), synth.prune_mask(scene.P, 204), None
+        return scene, O.yaw_cam(W, H, -3.0), synth.prune_mask(scene.P, 204), None
     raise ValueError(name)
 
 
-def _kw(prune, quant):
-    return dict(prune_mask=None if prune is None else prune.to(DEV), quant=None if quant is None else quant.to(DEV))
-
-
-def _forward(scene, cam, bg, prune=None, quant=None, aa=True, extra=None, maps=False, dbg=None):
-    args = O.forward_args(scene, cam, bg, extra)
-    return args, _C.rasterize_gaussians(*args, return_maps=maps, debug_out=dbg, antialiasing=aa, **_kw(prune, quant))
-
-
-def _backward(args, out, dL, prune=None, quant=None, aa=True, **extra):
-    (bg, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
-    R, color, radii, geom, binning, img = out[:6]
-    return _C.rasterize_gaussians_backward(bg, means3D, radii, colors, scales, rotations, mod, cov, view, proj, tx, ty, dL.to(DEV), sh,
-                                           degrees, campos, geom, R, binning, img, 0.0, False, antialiasing=aa, **_kw(prune, quant),
-                                           **extra)
-
-
-def _state(out, cam, P):
-    st = _C.export_state(out[3], out[4], out[5], out[0], cam.image_width, cam.image_height, P=P)
-    torch.cuda.synchronize()
-    return st
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _same(a, b):
-    return a.shape == b.shape and torch.equal(_bits(a), _bits(b))
+# every call here is anti-aliased unless it passes aa=False
+_forward = partial(O.forward, aa=True)
+_backward = partial(O.backward, aa=True)
 
 
 def _rel(a, b):
@@ -120,11 +87,11 @@ def test_antialiasing_moves_nothing_but_the_opacity(name):
     d0, d1 = {}, {}
     _, plain = _forward(scene, cam, bg, prune, quant, aa=False, dbg=d0)
     _, aa = _forward(scene, cam, bg, prune, quant, aa=True, dbg=d1)
-    assert plain[0] == aa[0] and plain[0] > 0 and _same(plain[2], aa[2])
+    assert plain[0] == aa[0] and plain[0] > 0 and O.same(plain[2], aa[2])
     for k in ("depths", "means2D", "cov3D", "rgb", "tiles_touched", "clamped"):
-        assert _same(d0[k], d1[k]), k
-    assert _same(d0["conic_opacity"][:, :3], d1["conic_opacity"][:, :3])
-    st0, st1 = _state(plain, cam, scene.P), _state(aa, cam, scene.P)
+        assert O.same(d0[k], d1[k]), k
+    assert O.same(d0["conic_opacity"][:, :3], d1["conic_opacity"][:, :3])
+    st0, st1 = O.state(plain, cam, scene.P), O.state(aa, cam, scene.P)
     for k in ("keys", "point_list", "ranges"):
         assert torch.equal(st0[k], st1[k]), k
     vis = plain[2] > 0
@@ -271,7 +238,7 @@ def _tiny_scene(seed, P=48):
 def test_antialiasing_against_a_float64_restatement(case):
     W = H = 32
     scene = _tiny_scene({"sh": 211, "colors_precomp": 212, "cov3D_precomp": 213, "maps_only": 214}[case])
-    cam = _yaw_cam(W, H, 3.0)
+    cam = O.yaw_cam(W, H, 3.0)
     bg = torch.tensor([0.3, 0.2, 0.1], device=DEV)
     gen = torch.Generator().manual_seed(215)
     extra = {}
@@ -284,7 +251,7 @@ def test_antialiasing_against_a_float64_restatement(case):
     Gc = torch.zeros(3, H, W) if case == "maps_only" else torch.randn(3, H, W, generator=gen)
     Gd, Ga = torch.randn(1, H, W, generator=gen), torch.randn(1, H, W, generator=gen)
     g = _backward(args, out, Gc, dL_dinvdepth=Gd.to(DEV), dL_dalpha=Ga.to(DEV), camera_grads=True)
-    st = _state(out, cam, scene.P)
+    st = O.state(out, cam, scene.P)
     vis = out[2] > 0
     assert int(vis.sum()) >= 30
     tiles = [st["point_list"][int(r0):int(r1)].long() for r0, r1 in st["ranges"].tolist()]
@@ -373,7 +340,7 @@ def test_total_alpha_of_a_small_gaussian_is_resolution_invariant_only_with_aa():
 
 def _small(name):
     scene, _, prune, quant = _config(name)
-    return scene, _yaw_cam(8, 4, 2.0), prune, quant
+    return scene, O.yaw_cam(8, 4, 2.0), prune, quant
 
 
 def _grads_close(a, b, bar=1e-6):
@@ -390,7 +357,7 @@ def test_quantised_aa_equals_dequantised_aa():
     ad, od = _forward(dense, cam, bg, maps=True)
     assert int((oq[2] > 0).sum()) > 1000
     for i in (0, 1, 2, 6, 7):
-        assert oq[i] == od[i] if i == 0 else _same(oq[i], od[i]), i
+        assert oq[i] == od[i] if i == 0 else O.same(oq[i], od[i]), i
     gq = _backward(aq, oq, G, quant=quant, dL_dinvdepth=Gd)
     gd = _backward(ad, od, G, dL_dinvdepth=Gd)
     assert _grads_close(gq, gd)
@@ -405,7 +372,7 @@ def test_pruned_aa_equals_compacted_aa():
     ac, oc = _forward(scene.compact(keep), cam, bg, maps=True)
     assert op[0] == oc[0] and op[0] > 0
     for i in (1, 6, 7):
-        assert _same(op[i], oc[i]), i
+        assert O.same(op[i], oc[i]), i
     gp = _backward(ap, op, G, prune=prune)
     gc = _backward(ac, oc, G)
     kd = keep.to(DEV)
@@ -415,7 +382,7 @@ def test_pruned_aa_equals_compacted_aa():
 
 def test_aa_accumulate_equals_the_sum_of_two_calls_and_quant_grads_accumulate():
     scene, cam, _, _ = _small("mixed")
-    cam2 = _yaw_cam(8, 4, 3.5)
+    cam2 = O.yaw_cam(8, 4, 3.5)
     bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
     G = torch.randn(3, 4, 8, generator=torch.Generator().manual_seed(224))
     a1, o1 = _forward(scene, cam, bg)
@@ -499,11 +466,11 @@ def test_aa_rotation_invariance_with_the_camera():
 def test_aa_is_deterministic_on_any_stream():
     scene, _, _, _ = _config("mixed")
     bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
-    big = _yaw_cam(320, 200, 1.0)
+    big = O.yaw_cam(320, 200, 1.0)
     _, f1 = _forward(scene, big, bg, maps=True)
     _, f2 = _forward(scene, big, bg, maps=True)
-    assert all(_same(f1[i], f2[i]) for i in (1, 2, 6, 7))
-    cam = _yaw_cam(8, 4, 2.0)
+    assert all(O.same(f1[i], f2[i]) for i in (1, 2, 6, 7))
+    cam = O.yaw_cam(8, 4, 2.0)
     G = torch.randn(3, 4, 8, generator=torch.Generator().manual_seed(228)).to(DEV)
     args, out = _forward(scene, cam, bg, maps=True)
     kw = dict(dL_dalpha=torch.ones(1, 4, 8, device=DEV), camera_grads=True)
@@ -516,9 +483,9 @@ def test_aa_is_deterministic_on_any_stream():
         other = _backward(a3, o3, G, **kw)
     torch.cuda.current_stream().wait_stream(s)
     torch.cuda.synchronize()
-    assert _same(o3[1], out[1]) and _same(o3[7], out[7])
+    assert O.same(o3[1], out[1]) and O.same(o3[7], out[7])
     for a, b, c in zip(first, again, other):
-        assert _same(a, b) and _same(a, c)
+        assert O.same(a, b) and O.same(a, c)
 
 
 def test_aa_empty_and_fully_culled_scenes_give_zeros():
@@ -545,7 +512,7 @@ def test_aa_on_a_second_device():
     bg = torch.tensor([0.1, 0.3, 0.2])
     outs = []
     for dev in ("cuda:0", "cuda:1"):
-        cam = _yaw_cam(8, 4, 2.0, dev=dev)
+        cam = O.yaw_cam(8, 4, 2.0, dev=dev)
         args = O.forward_args(scene, cam, bg, dev=dev)
         out = _C.rasterize_gaussians(*args, antialiasing=True)
         (bgd, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
@@ -553,8 +520,8 @@ def test_aa_on_a_second_device():
                                             torch.ones(3, H, W, device=dev), sh, degrees, campos, out[3], out[0], out[4], out[5], 0.0,
                                             False, antialiasing=True)
         outs.append((out[1].cpu(), [t.cpu() for t in g]))
-    assert _same(outs[0][0], outs[1][0])
-    assert all(_same(a, b) for a, b in zip(outs[0][1], outs[1][1]))
+    assert O.same(outs[0][0], outs[1][0])
+    assert all(O.same(a, b) for a, b in zip(outs[0][1], outs[1][1]))
 
 
 # ---- 8. training --------------------------------------------------------------------------------------------------------------
@@ -584,7 +551,7 @@ def test_adam_steps_with_antialiasing_reduce_the_loss():
     from utils.loss_utils import l1_ssim_loss
     W, H = 256, 192
     target = synth.make_scene(6_000, 231, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.02), M=16)
-    cams = [_yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
+    cams = [O.yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
     pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False, antialiasing=True)
     bg = torch.tensor([0.1, 0.1, 0.1], device=DEV)
     with torch.no_grad():

@@ -17,7 +17,6 @@ import pytest
 import torch
 
 import ours as O
-from diff_gaussian_rasterization import _C
 from gs_b200 import synth
 from gs_b200.model import GaussianModelView
 
@@ -35,48 +34,16 @@ def _config(name):
     W, H = 320, 200
     box, ls = (1.9 * W / H, 1.9, 1.0), math.log(0.03)
     if name == "sh3":
-        return synth.make_scene(20_000, 181, sh_degree=3, box=box, log_scale_mean=ls), _yaw_cam(W, H, 8.0, dev="cpu"), None, None
+        return synth.make_scene(20_000, 181, sh_degree=3, box=box, log_scale_mean=ls), O.yaw_cam(W, H, 8.0, dev="cpu"), None, None
     if name == "mixed":
-        return synth.make_scene(20_000, 182, mixed_degrees=True, box=box, log_scale_mean=ls), _yaw_cam(W, H, -5.0, dev="cpu"), None, None
+        return synth.make_scene(20_000, 182, mixed_degrees=True, box=box, log_scale_mean=ls), O.yaw_cam(W, H, -5.0, dev="cpu"), None, None
     if name == "quant":
         scene = synth.make_scene(20_000, 183, mixed_degrees=True, box=box, log_scale_mean=ls)
-        return scene, _yaw_cam(W, H, 4.0, dev="cpu"), None, synth.quantise_scene(scene)
+        return scene, O.yaw_cam(W, H, 4.0, dev="cpu"), None, synth.quantise_scene(scene)
     if name == "pruned":
         scene = synth.make_scene(20_000, 184, sh_degree=2, box=box, log_scale_mean=ls)
-        return scene, _yaw_cam(W, H, -3.0, dev="cpu"), synth.prune_mask(scene.P, 185), None
+        return scene, O.yaw_cam(W, H, -3.0, dev="cpu"), synth.prune_mask(scene.P, 185), None
     raise ValueError(name)
-
-
-def _yaw_cam(W, H, deg, dev=DEV):
-    th = math.radians(deg)
-    Rc2w = np.array([[math.cos(th), 0, math.sin(th)], [0, 1, 0], [-math.sin(th), 0, math.cos(th)]])
-    C = Rc2w @ np.array([0.0, 0.0, -4.0])
-    return synth.make_camera(W, H, Rc2w, -Rc2w.T @ C).to(dev)
-
-
-def _kw(prune, quant):
-    return dict(prune_mask=None if prune is None else prune.to(DEV), quant=None if quant is None else quant.to(DEV))
-
-
-def _forward(scene, cam, bg, prune, quant, colors=None, maps=False, dbg=None):
-    args = O.forward_args(scene, cam, bg, None if colors is None else {"colors_precomp": colors})
-    out = _C.rasterize_gaussians(*args, return_maps=maps, debug_out=dbg, **_kw(prune, quant))
-    return args, out
-
-
-def _backward(args, out, dL, prune, quant, **extra):
-    (bg, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
-    R, color, radii, geom, binning, img = out[:6]
-    return _C.rasterize_gaussians_backward(bg, means3D, radii, colors, scales, rotations, mod, cov, view, proj, tx, ty, dL.to(DEV), sh,
-                                           degrees, campos, geom, R, binning, img, 0.0, False, **_kw(prune, quant), **extra)
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _same(a, b):
-    return a.shape == b.shape and torch.equal(_bits(a), _bits(b))
 
 
 # Outputs the preprocess backward copies or scales from the accumulator are bit-identical with the camera gradients on.  The ones
@@ -97,7 +64,7 @@ def _close(a, b):
 
 def _small(name):
     scene, _, prune, quant = _config({"maps": "mixed", "accumulate": "mixed"}.get(name, name))
-    return scene, _yaw_cam(8, 4, 2.0, dev="cpu"), prune, quant
+    return scene, O.yaw_cam(8, 4, 2.0, dev="cpu"), prune, quant
 
 
 @pytest.mark.parametrize("name", ["c1", "quant", "pruned", "maps", "accumulate"])
@@ -111,25 +78,25 @@ def test_camera_grads_change_nothing_else(name):
     if name == "maps":
         extra.update(dL_dinvdepth=torch.randn(1, H, W, generator=g).to(DEV), dL_dalpha=torch.randn(1, H, W, generator=g).to(DEV))
     bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
-    args, out = _forward(scene, cam, bg, prune, quant, maps=(name == "maps"))
+    args, out = O.forward(scene, cam, bg, prune, quant, maps=(name == "maps"))
     assert int((out[2] > 0).sum()) > 1000
     if name == "accumulate":
         # two views into one set of buffers; the second call also exports its own dL_dmeans2D
-        args0, out0 = _forward(scene, _yaw_cam(W, H, 3.0), bg, prune, quant)
-        base = _backward(args0, out0, dL, prune, quant)
+        args0, out0 = O.forward(scene, O.yaw_cam(W, H, 3.0), bg, prune, quant)
+        base = O.backward(args0, out0, dL, prune, quant)
         acc_a, acc_b = tuple(t.clone() for t in base), tuple(t.clone() for t in base)
         v_a, v_b = torch.empty(scene.P, 3, device=DEV), torch.empty(scene.P, 3, device=DEV)
-        plain = _backward(args, out, dL, prune, quant, accumulate_into=acc_a, view_means2D=v_a, **extra)
-        cam1 = _backward(args, out, dL, prune, quant, accumulate_into=acc_b, view_means2D=v_b, camera_grads=True, **extra)
-        assert _same(v_a, v_b)
+        plain = O.backward(args, out, dL, prune, quant, accumulate_into=acc_a, view_means2D=v_a, **extra)
+        cam1 = O.backward(args, out, dL, prune, quant, accumulate_into=acc_b, view_means2D=v_b, camera_grads=True, **extra)
+        assert O.same(v_a, v_b)
         for n, a, b in zip(O.GRAD_NAMES, acc_a, acc_b):
-            assert _same(a, b) if n in _BITWISE else _close(a, b), n
+            assert O.same(a, b) if n in _BITWISE else _close(a, b), n
     else:
-        plain = _backward(args, out, dL, prune, quant, **extra)
-        cam1 = _backward(args, out, dL, prune, quant, camera_grads=True, **extra)
+        plain = O.backward(args, out, dL, prune, quant, **extra)
+        cam1 = O.backward(args, out, dL, prune, quant, camera_grads=True, **extra)
     assert len(plain) == 9 and len(cam1) == 12
     for n, a, b in zip(O.GRAD_NAMES + ["dL_dconic"], plain, cam1[:9]):
-        assert _same(a, b) if n in _BITWISE else _close(a, b), n
+        assert O.same(a, b) if n in _BITWISE else _close(a, b), n
     dview, dproj, dcampos = cam1[9:]
     assert dview.shape == (4, 4) and dproj.shape == (4, 4) and dcampos.shape == (3,)
     assert torch.isfinite(dview).all() and torch.isfinite(dproj).all() and torch.isfinite(dcampos).all()
@@ -138,19 +105,19 @@ def test_camera_grads_change_nothing_else(name):
     assert float(dview[:, :3].abs().min()) > 0 and float(dproj[:, [0, 1, 3]].abs().min()) > 0
     if name == "accumulate":
         # the camera outputs are this view's: equal to an overwrite-mode call of the same view
-        ref = _backward(args, out, dL, prune, quant, camera_grads=True, **extra)
-        assert all(_same(a, b) for a, b in zip(ref[9:], cam1[9:]))
+        ref = O.backward(args, out, dL, prune, quant, camera_grads=True, **extra)
+        assert all(O.same(a, b) for a, b in zip(ref[9:], cam1[9:]))
         return
     # the same bytes on a second run and on a non-default stream
-    again = _backward(args, out, dL, prune, quant, camera_grads=True, **extra)
+    again = O.backward(args, out, dL, prune, quant, camera_grads=True, **extra)
     s = torch.cuda.Stream()
     s.wait_stream(torch.cuda.current_stream())
     with torch.cuda.stream(s):
-        other = _backward(args, out, dL, prune, quant, camera_grads=True, **extra)
+        other = O.backward(args, out, dL, prune, quant, camera_grads=True, **extra)
     torch.cuda.current_stream().wait_stream(s)
     torch.cuda.synchronize()
     for a, b, c in zip(cam1[9:], again[9:], other[9:]):
-        assert _same(a, b) and _same(a, c)
+        assert O.same(a, b) and O.same(a, c)
 
 
 def test_quant_grads_unchanged_by_a_learnable_camera():
@@ -172,10 +139,10 @@ def test_quant_grads_unchanged_by_a_learnable_camera():
         (pkg["render"] * G).sum().backward()
         res.append((pc, pkg, c))
     (pa, ka, _), (pb, kb, cb) = res
-    assert _same(pa.quant.grads["opacity"], pb.quant.grads["opacity"])
+    assert O.same(pa.quant.grads["opacity"], pb.quant.grads["opacity"])
     for k in ("sh", "scales", "rotations"):
         assert _close(pa.quant.grads[k], pb.quant.grads[k]), k
-    assert _close(pa._xyz.grad, pb._xyz.grad) and _same(ka["viewspace_points"].grad, kb["viewspace_points"].grad)
+    assert _close(pa._xyz.grad, pb._xyz.grad) and O.same(ka["viewspace_points"].grad, kb["viewspace_points"].grad)
     for t in (cb.world_view_transform, cb.full_proj_transform, cb.camera_center):
         assert t.grad is not None and t.grad.shape == t.shape and float(t.grad.abs().max()) > 0
 
@@ -192,13 +159,13 @@ def test_camera_grads_of_empty_and_fully_culled_scenes():
     culled = synth.Scene(means, torch.zeros(P, 1), torch.full((P, 3), 0.1), torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1),
                          torch.zeros(P, 1, 3), torch.zeros(P, 1, dtype=torch.int32))
     for scene in (empty, culled):
-        args, out = _forward(scene, cam, bg, None, None)
+        args, out = O.forward(scene, cam, bg, None, None)
         assert out[0] == 0
         for acc in (False, True):
             extra = dict(camera_grads=True)
             if acc:
-                extra["accumulate_into"] = tuple(t.clone() for t in _backward(args, out, torch.ones(3, H, W), None, None))
-            g = _backward(args, out, torch.ones(3, H, W), None, None, **extra)
+                extra["accumulate_into"] = tuple(t.clone() for t in O.backward(args, out, torch.ones(3, H, W), None, None))
+            g = O.backward(args, out, torch.ones(3, H, W), None, None, **extra)
             # poison-free check: the camera outputs are written (not left as whatever the allocation held)
             assert all(float(t.abs().max()) == 0.0 for t in g[8:]), (scene.P, acc)
             assert [tuple(t.shape) for t in g[8:]] == [(4, 4), (4, 4), (3,)]
@@ -299,8 +266,8 @@ def _kernel_and_chain(name):
     bg = torch.tensor([0.2, 0.1, 0.3], device=DEV)
     dL = synth.grad_image(W, H, 172).to(DEV)
     dbg = {}
-    args, out = _forward(scene, cam, bg, prune, quant, dbg=dbg)
-    g = _backward(args, out, dL, prune, quant, want_conic=True, camera_grads=True)
+    args, out = O.forward(scene, cam, bg, prune, quant, dbg=dbg)
+    g = O.backward(args, out, dL, prune, quant, want_conic=True, camera_grads=True)
     vis = out[2] > 0
     sh = scene.sh if scene.sh.shape[1] > 0 else None
     per = _chain(cam.world_view_transform, cam.full_proj_transform, cam.camera_center, W, H, math.tan(cam.FoVx * 0.5),
@@ -326,9 +293,9 @@ def test_camera_grads_against_the_fp64_oracle():
     o = gs_oracle.forward(scene.means3D, scene.opacity, scene.scales, scene.rotations, scene.sh, scene.degrees, bg=bg, **kw)
     ob = gs_oracle.backward(o, dL, scene.means3D, scene.scales, scene.rotations, scene.sh, scene.degrees, bg=bg, f64=True, **kw)
     dbg = {}
-    args, out = _forward(scene, cam.to(DEV), bg.to(DEV), None, None, dbg=dbg)
+    args, out = O.forward(scene, cam.to(DEV), bg.to(DEV), None, None, dbg=dbg)
     assert np.array_equal(out[2].cpu().numpy(), o["radii"])
-    g = _backward(args, out, dL, None, None, camera_grads=True)
+    g = O.backward(args, out, dL, None, None, camera_grads=True)
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a))
     per = _chain(cam.world_view_transform, cam.full_proj_transform, cam.camera_center, W, H, kw["tan_fovx"], kw["tan_fovy"],
                  scene.means3D, t(o["cov3D"]), scene.sh, scene.degrees, t(o["clamped"]), out[2] > 0, t(ob["dL_dmeans2D"]),
@@ -355,8 +322,8 @@ def test_translating_the_world_and_the_camera_together_changes_nothing(name):
     scene, cam, prune, quant = _config(name)
     cam = cam.to(DEV)
     H, W = cam.image_height, cam.image_width
-    args, out = _forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), prune, quant)
-    g = _backward(args, out, synth.grad_image(W, H, 174).to(DEV), prune, quant, camera_grads=True)
+    args, out = O.forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), prune, quant)
+    g = O.backward(args, out, synth.grad_image(W, H, 174).to(DEV), prune, quant, camera_grads=True)
     gm = g[3].to(F64)
     gv, gp, gc = g[8].to(F64), g[9].to(F64), g[10].to(F64)
     V, Pf = cam.world_view_transform.to(DEV, F64), cam.full_proj_transform.to(DEV, F64)
@@ -376,8 +343,8 @@ def test_rotating_the_world_and_the_camera_together_changes_nothing():
     cam = cam.to(DEV)
     H, W = cam.image_height, cam.image_width
     col = torch.rand(scene.P, 3, generator=torch.Generator().manual_seed(175))
-    args, out = _forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), None, None, colors=col)
-    g = _backward(args, out, synth.grad_image(W, H, 176).to(DEV), None, None, camera_grads=True)
+    args, out = O.forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), None, None, colors=col)
+    g = O.backward(args, out, synth.grad_image(W, H, 176).to(DEV), None, None, camera_grads=True)
     gm, gq = g[3].to(F64), g[7].to(F64)
     gv, gp = g[8].to(F64), g[9].to(F64)
     m, q = scene.means3D.to(DEV, F64), scene.rotations.to(DEV, F64)
@@ -409,18 +376,18 @@ def test_camera_grads_of_the_maps_equal_those_of_the_colour_emulation():
     Gd, Ga = torch.randn(1, H, W, generator=g).to(DEV), torch.randn(1, H, W, generator=g).to(DEV)
     zero3 = torch.zeros(3, H, W, device=DEV)
     dbg = {}
-    args, out = _forward(scene, cam, torch.tensor([0.3, 0.1, 0.2], device=DEV), None, None, maps=True, dbg=dbg)
+    args, out = O.forward(scene, cam, torch.tensor([0.3, 0.1, 0.2], device=DEV), None, None, maps=True, dbg=dbg)
     vis = out[2] > 0
     z = dbg["depths"]
-    got_d = _backward(args, out, zero3, None, None, dL_dinvdepth=Gd, camera_grads=True)
-    got_a = _backward(args, out, zero3, None, None, dL_dalpha=Ga, camera_grads=True)
+    got_d = O.backward(args, out, zero3, None, None, dL_dinvdepth=Gd, camera_grads=True)
+    got_a = O.backward(args, out, zero3, None, None, dL_dalpha=Ga, camera_grads=True)
     # invdepth: colour (1/z, 0, 0) without background, plus the direct term d(1/z_i)/dview[4r+2] = -m_r / z_i^2
     col = torch.zeros(scene.P, 3)
     col[:, 0] = torch.where(vis.cpu(), 1.0 / torch.where(vis, z, torch.ones_like(z)).cpu(), torch.zeros(scene.P))
-    ab, ob = _forward(scene, cam, torch.zeros(3, device=DEV), None, None, colors=col)
+    ab, ob = O.forward(scene, cam, torch.zeros(3, device=DEV), None, None, colors=col)
     dLb = torch.zeros(3, H, W, device=DEV)
     dLb[0] = Gd[0]
-    gb = _backward(ab, ob, dLb, None, None, camera_grads=True)
+    gb = O.backward(ab, ob, dLb, None, None, camera_grads=True)
     m = scene.means3D.to(DEV, F64)[vis]
     w = (-gb[1][:, 0].to(F64)[vis] / (z.to(F64)[vis] ** 2))
     direct = torch.zeros(4, 4, dtype=F64, device=DEV)
@@ -428,10 +395,10 @@ def test_camera_grads_of_the_maps_equal_those_of_the_colour_emulation():
     direct[3, 2] = w.sum()
     exp_d = (gb[8].to(F64) + direct, gb[9].to(F64), gb[10].to(F64))
     # alpha: colour 0 with background (-1, 0, 0)
-    ac, oc = _forward(scene, cam, torch.tensor([-1.0, 0.0, 0.0], device=DEV), None, None, colors=torch.zeros(scene.P, 3))
+    ac, oc = O.forward(scene, cam, torch.tensor([-1.0, 0.0, 0.0], device=DEV), None, None, colors=torch.zeros(scene.P, 3))
     dLc = torch.zeros(3, H, W, device=DEV)
     dLc[0] = Ga[0]
-    gc = _backward(ac, oc, dLc, None, None, camera_grads=True)
+    gc = O.backward(ac, oc, dLc, None, None, camera_grads=True)
     exp_a = (gc[8].to(F64), gc[9].to(F64), gc[10].to(F64))
     scale_d = (w.abs()[:, None] * torch.cat([m.abs(), torch.ones_like(w)[:, None]], 1)).sum()
     for label, got, exp in (("invdepth", got_d[8:], exp_d), ("alpha", got_a[8:], exp_a)):

@@ -42,36 +42,6 @@ def _config(name):
     raise ValueError(name)
 
 
-def _yaw_cam(W, H, deg):
-    th = math.radians(deg)
-    Rc2w = np.array([[math.cos(th), 0, math.sin(th)], [0, 1, 0], [-math.sin(th), 0, math.cos(th)]])
-    C = Rc2w @ np.array([0.0, 0.0, -4.0])
-    return synth.make_camera(W, H, Rc2w, -Rc2w.T @ C).to(DEV)
-
-
-def _kw(prune, quant):
-    return dict(prune_mask=None if prune is None else prune.to(DEV), quant=None if quant is None else quant.to(DEV))
-
-
-def _forward(scene, cam, bg, prune, quant, colors=None, maps=False, dbg=None):
-    args = O.forward_args(scene, cam, bg, None if colors is None else {"colors_precomp": colors})
-    out = _C.rasterize_gaussians(*args, return_maps=maps, debug_out=dbg, **_kw(prune, quant))
-    return args, out
-
-
-def _state(out, cam, P):
-    st = _C.export_state(out[3], out[4], out[5], out[0], cam.image_width, cam.image_height, P=P)
-    torch.cuda.synchronize()
-    return st
-
-
-def _backward(args, out, dL, prune, quant, **extra):
-    (bg, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
-    R, color, radii, geom, binning, img = out[:6]
-    return _C.rasterize_gaussians_backward(bg, means3D, radii, colors, scales, rotations, mod, cov, view, proj, tx, ty, dL.to(DEV), sh,
-                                           degrees, campos, geom, R, binning, img, 0.0, False, **_kw(prune, quant), **extra)
-
-
 def _invdepth_colours(radii, depths):
     """(1/depth, 0, 0) per Gaussian (IEEE division on the host), 0 for culled ones."""
     d = depths.cpu().numpy()
@@ -88,11 +58,11 @@ def test_maps_change_nothing_else_and_match_the_colour_path(name):
     scene, cam, prune, quant = _config(name)
     cam = cam.to(DEV)
     bg = torch.tensor([0.2, 0.4, 0.6], device=DEV)
-    _, plain = _forward(scene, cam, bg, prune, quant)
+    _, plain = O.forward(scene, cam, bg, prune, quant)
     dbg = {}
-    _, mapped = _forward(scene, cam, bg, prune, quant, maps=True, dbg=dbg)
+    _, mapped = O.forward(scene, cam, bg, prune, quant, maps=True, dbg=dbg)
     assert len(plain) == 6 and len(mapped) == 8
-    st0, st1 = _state(plain, cam, scene.P), _state(mapped, cam, scene.P)
+    st0, st1 = O.state(plain, cam, scene.P), O.state(mapped, cam, scene.P)
     assert mapped[0] == plain[0] and plain[0] > 0
     assert torch.equal(mapped[1], plain[1]) and torch.equal(mapped[2], plain[2])
     for k in ("final_T", "n_contrib", "point_list", "ranges"):
@@ -104,12 +74,12 @@ def test_maps_change_nothing_else_and_match_the_colour_path(name):
     assert torch.equal(alpha[0], 1.0 - st1["final_T"])
     # invdepth == channel 0 of the colour render with colour (1/depth, 0, 0) and no background, bitwise
     col = _invdepth_colours(mapped[2], dbg["depths"])
-    _, ref = _forward(scene, cam, torch.zeros(3, device=DEV), prune, quant, colors=col)
+    _, ref = O.forward(scene, cam, torch.zeros(3, device=DEV), prune, quant, colors=col)
     assert torch.equal(ref[2], mapped[2])
     assert torch.equal(invdepth[0], ref[1][0])
     assert float(invdepth.max()) > 0 and float(alpha.max()) > 0.5
     # the maps are a deterministic function of the inputs
-    _, again = _forward(scene, cam, bg, prune, quant, maps=True)
+    _, again = O.forward(scene, cam, bg, prune, quant, maps=True)
     assert torch.equal(again[6].view(torch.int32), invdepth.view(torch.int32))
     assert torch.equal(again[7].view(torch.int32), alpha.view(torch.int32))
 
@@ -128,12 +98,12 @@ def test_maps_of_the_variable_sh_entry_point():
     plain, mapped = packed(False), packed(True)
     assert len(plain) == 6 and len(mapped) == 8
     assert mapped[0] == plain[0] and torch.equal(mapped[1], plain[1]) and torch.equal(mapped[2], plain[2])
-    st0, st1 = _state(plain, cam, scene.P), _state(mapped, cam, scene.P)
+    st0, st1 = O.state(plain, cam, scene.P), O.state(mapped, cam, scene.P)
     for k in ("final_T", "n_contrib", "point_list"):
         assert torch.equal(st0[k], st1[k]), k
     assert torch.equal(mapped[7][0], 1.0 - st1["final_T"])
     # the geometry is the dense path's: so are the maps
-    _, dense = _forward(scene, cam, bg, None, None, maps=True)
+    _, dense = O.forward(scene, cam, bg, None, None, maps=True)
     assert torch.equal(mapped[6], dense[6]) and torch.equal(mapped[7], dense[7])
 
 
@@ -143,7 +113,7 @@ def test_maps_of_empty_and_fully_culled_scenes():
     bg = torch.tensor([0.25, 0.5, 0.75], device=DEV)
     empty = synth.Scene(torch.zeros(0, 3), torch.zeros(0, 1), torch.zeros(0, 3), torch.zeros(0, 4), torch.zeros(0, 1, 3),
                         torch.zeros(0, 1, dtype=torch.int32))
-    _, out = _forward(empty, cam, bg, None, None, maps=True)
+    _, out = O.forward(empty, cam, bg, None, None, maps=True)
     assert out[0] == 0 and out[6].shape == (1, H, W) and out[7].shape == (1, H, W)
     assert float(out[6].abs().max()) == 0.0 and float(out[7].abs().max()) == 0.0
     P = 33
@@ -151,10 +121,10 @@ def test_maps_of_empty_and_fully_culled_scenes():
     means[:, 2] = -9.0                                                       # behind the camera: every Gaussian is culled
     culled = synth.Scene(means, torch.zeros(P, 1), torch.full((P, 3), 0.1), torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1),
                          torch.zeros(P, 1, 3), torch.zeros(P, 1, dtype=torch.int32))
-    args, out = _forward(culled, cam, bg, None, None, maps=True)
+    args, out = O.forward(culled, cam, bg, None, None, maps=True)
     assert out[0] == 0 and int((out[2] > 0).sum()) == 0
     assert float(out[6].abs().max()) == 0.0 and float(out[7].abs().max()) == 0.0
-    g = _backward(args, out, torch.ones(3, H, W), None, None, dL_dinvdepth=torch.ones(1, H, W, device=DEV),
+    g = O.backward(args, out, torch.ones(3, H, W), None, None, dL_dinvdepth=torch.ones(1, H, W, device=DEV),
                   dL_dalpha=torch.ones(1, H, W, device=DEV))
     assert all(float(t.abs().max()) == 0.0 for t in g if t.numel())
 
@@ -163,22 +133,22 @@ def _expected_grads(scene, cam, prune, quant, Gc, Gd, Ga):
     """Sum of three existing backwards (see the module docstring) -> (maps backward, expected, radii)."""
     bg = torch.tensor([0.3, 0.1, 0.2], device=DEV)
     dbg = {}
-    args, out = _forward(scene, cam, bg, prune, quant, maps=True, dbg=dbg)
-    got = _backward(args, out, Gc, prune, quant, dL_dinvdepth=Gd, dL_dalpha=Ga)
+    args, out = O.forward(scene, cam, bg, prune, quant, maps=True, dbg=dbg)
+    got = O.backward(args, out, Gc, prune, quant, dL_dinvdepth=Gd, dL_dalpha=Ga)
     # (a) the colour backward
-    ga = _backward(args, out, Gc, prune, quant)
+    ga = O.backward(args, out, Gc, prune, quant)
     # (b) colour (1/depth, 0, 0), no background, dL/dpixel (Gd, 0, 0); dL/dcolour[:,0] chained through d(1/z)/dmeans3D
     zero3 = torch.zeros(3, device=DEV)
     col = _invdepth_colours(out[2], dbg["depths"])
-    argsb, outb = _forward(scene, cam, zero3, prune, quant, colors=col)
+    argsb, outb = O.forward(scene, cam, zero3, prune, quant, colors=col)
     dLb = torch.zeros(3, cam.image_height, cam.image_width, device=DEV)
     dLb[0] = Gd[0]
-    gb = _backward(argsb, outb, dLb, prune, quant)
+    gb = O.backward(argsb, outb, dLb, prune, quant)
     # (c) colour 0, background (-1, 0, 0), dL/dpixel (Ga, 0, 0)
-    argsc, outc = _forward(scene, cam, torch.tensor([-1.0, 0.0, 0.0], device=DEV), prune, quant, colors=torch.zeros(scene.P, 3))
+    argsc, outc = O.forward(scene, cam, torch.tensor([-1.0, 0.0, 0.0], device=DEV), prune, quant, colors=torch.zeros(scene.P, 3))
     dLc = torch.zeros_like(dLb)
     dLc[0] = Ga[0]
-    gc = _backward(argsc, outc, dLc, prune, quant)
+    gc = O.backward(argsc, outc, dLc, prune, quant)
     # dL_dcolors and dL_dsh are the colour path's alone (the override renders have no SH: their dL_dsh is empty)
     exp = [a if i in (1, 5) else a + b + c for i, (a, b, c) in enumerate(zip(ga, gb, gc))]
     z = dbg["depths"]
@@ -218,7 +188,7 @@ def test_map_gradients_through_autograd_and_accumulation():
     from gaussian_renderer import render
     W, H = 256, 160
     scene = synth.make_scene(8000, 91, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.04))
-    cams = [_yaw_cam(W, H, 0.0), _yaw_cam(W, H, 6.0)]
+    cams = [O.yaw_cam(W, H, 0.0), O.yaw_cam(W, H, 6.0)]
     bg = torch.tensor([0.0, 0.3, 0.0], device=DEV)
     g = torch.Generator().manual_seed(92)
     Gd, Ga = torch.randn(1, H, W, generator=g).to(DEV), torch.randn(1, H, W, generator=g).to(DEV)
@@ -228,9 +198,9 @@ def test_map_gradients_through_autograd_and_accumulation():
     pkg = render(cams[0], pc, pipe, bg, return_maps=True)
     assert pkg["invdepth"].shape == (1, H, W) and pkg["alpha"].shape == (1, H, W)
     ((pkg["invdepth"] * Gd).sum() + (pkg["alpha"] * Ga).sum()).backward()
-    args, out = _forward(scene, cams[0], bg, None, None, maps=True)
+    args, out = O.forward(scene, cams[0], bg, None, None, maps=True)
     assert torch.equal(out[1], pkg["render"].detach()) and torch.equal(out[6], pkg["invdepth"].detach())
-    ref = _backward(args, out, torch.zeros(3, H, W), None, None, dL_dinvdepth=Gd, dL_dalpha=Ga)
+    ref = O.backward(args, out, torch.zeros(3, H, W), None, None, dL_dinvdepth=Gd, dL_dalpha=Ga)
 
     def close(t, r):
         r = r.reshape(t.shape)
@@ -241,10 +211,10 @@ def test_map_gradients_through_autograd_and_accumulation():
     assert float(pkg["viewspace_points"].grad[:, :2].norm(dim=1).max()) > 0  # the densification statistic sees the maps
     # accumulate_into over two views == the sum of two separate calls
     Gc = torch.randn(3, H, W, generator=g).to(DEV)
-    runs = [_forward(scene, c, bg, None, None, maps=True) for c in cams]
-    sep = [_backward(a, o, Gc, None, None, dL_dinvdepth=Gd, dL_dalpha=Ga) for a, o in runs]
+    runs = [O.forward(scene, c, bg, None, None, maps=True) for c in cams]
+    sep = [O.backward(a, o, Gc, None, None, dL_dinvdepth=Gd, dL_dalpha=Ga) for a, o in runs]
     acc = tuple(t.clone() for t in sep[0])
-    _backward(*runs[1], Gc, None, None, dL_dinvdepth=Gd, dL_dalpha=Ga, accumulate_into=acc)
+    O.backward(*runs[1], Gc, None, None, dL_dinvdepth=Gd, dL_dalpha=Ga, accumulate_into=acc)
     for a, s0, s1 in zip(acc, *sep):
         s = s0 + s1
         assert float((a - s).abs().max()) <= 2e-4 * (float(s.abs().max()) + 1e-12)
@@ -262,8 +232,8 @@ def test_quantised_map_gradients_reach_quant_grads():
     pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
     pkg = render(cam, pc, pipe, bg, return_maps=True)
     ((pkg["invdepth"] * Gd).sum() + (pkg["alpha"] * Ga).sum()).backward()
-    args, out = _forward(scene, cam, bg, None, quant, maps=True)
-    ref = _backward(args, out, torch.zeros(3, H, W), None, quant, dL_dinvdepth=Gd, dL_dalpha=Ga)
+    args, out = O.forward(scene, cam, bg, None, quant, maps=True)
+    ref = O.backward(args, out, torch.zeros(3, H, W), None, quant, dL_dinvdepth=Gd, dL_dalpha=Ga)
     for k, i in (("opacity", 2), ("scales", 6), ("rotations", 7)):
         r = ref[i]
         assert float((pc.quant.grads[k].reshape(r.shape) - r).abs().max()) <= 1e-4 * float(r.abs().max()), k
@@ -275,7 +245,7 @@ def test_invdepth_loss_alone_pulls_the_means_back():
     from gaussian_renderer import render
     W, H = 256, 192
     target = synth.make_scene(6_000, 94, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.04), M=16)
-    cams = [_yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
+    cams = [O.yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
     pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
     bg = torch.zeros(3, device=DEV)
     with torch.no_grad():
