@@ -12,6 +12,7 @@ import numpy as np
 import pytest
 import torch
 
+import backward_edges as BE
 import ours as O
 from diff_gaussian_rasterization import _C
 from gs_b200 import synth
@@ -32,6 +33,9 @@ def _config(name):
         W, H = 1920, 1080
         scene = synth.make_scene(300_000, 81, mixed_degrees=True)
         return scene, synth.make_camera(W, H), None, None
+    if name == "staircase" or name.startswith("odd_"):
+        case = BE.build(name)                       # the per-element backward's boundary scenes (tests/backward_edges.py)
+        return case.scene, case.cam, None, None
     W, H = 320, 200
     if name == "quant":
         scene = synth.make_scene(20_000, 82, mixed_degrees=True, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.03))
@@ -172,7 +176,7 @@ def _assert_close(got, exp, radii):
             assert float(g[off].abs().max()) == 0.0, n
 
 
-@pytest.mark.parametrize("name", ["c1", "quant", "pruned"])
+@pytest.mark.parametrize("name", ["c1", "quant", "pruned", "staircase"] + ["odd_%dx%d" % s for s in BE.ODD_SIZES])
 def test_map_gradients_equal_the_sum_of_colour_backwards(name):
     scene, cam, prune, quant = _config(name)
     cam = cam.to(DEV)

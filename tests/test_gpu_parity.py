@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 import torch
 
+import backward_edges
 import cases
 import gs_oracle
 import make_golden
@@ -170,35 +171,10 @@ def test_sort_paths_ties_and_dense_tiles(kind):
     sort leaves them), clustered depths (distribution-sort fallback), and tiles with > 2048 / > 8192 instances
     (persistent shared-memory class and the global-memory fallback).  Integers must equal the oracle exactly."""
     ours = _ours()
-    g = torch.Generator().manual_seed(7)
-    if kind == "ties":
-        P, W, H = 30_000, 128, 128
-        xyz = torch.rand(P, 3, generator=g) * 2 - 1
-        xyz[:, 2] = 0.0                                  # one plane facing the camera: identical view-space depth
-        xyz[::3, 2] = 0.25                               # ... and a second plane
-        scale = 0.02
-    elif kind == "dense_ties":
-        # tiles of 2049..8192 instances whose depths are all identical: the 8192-bin distribution sort of that class must hand
-        # them to the radix fallback (a bin holds more than 32 entries), and ties must come out in ascending Gaussian id
-        P, W, H = 8_000, 64, 48
-        xyz = (torch.rand(P, 3, generator=g) * 2 - 1) * torch.tensor([0.5, 0.4, 1.0])
-        xyz[:, 2] = 0.0
-        scale = 0.01
-    else:
-        P = {"dense_4k": 12_000, "dense_12k": 40_000, "dense_40k": 120_000}[kind]
-        W, H = 64, 48
-        xyz = (torch.rand(P, 3, generator=g) * 2 - 1) * torch.tensor([0.5, 0.4, 1.0])
-        scale = 0.01
-    scales = torch.full((P, 3), scale) * (0.5 + torch.rand(P, 3, generator=g))
-    q = torch.nn.functional.normalize(torch.randn(P, 4, generator=g))
-    op = torch.randn(P, 1, generator=g) - 2.0
-    sh = torch.randn(P, 1, 3, generator=g)
-    deg = torch.zeros(P, 1, dtype=torch.int32)
-    scene = synth.Scene(xyz.contiguous(), op, scales.contiguous(), q.contiguous(), sh, deg)
-    cam = synth.make_camera(W, H)
-    bg = torch.zeros(3)
+    scene, cam, bg = backward_edges.dense_scene(kind)      # shared with test_gpu_backward_edges, which runs their backward
+    W, H = cam.image_width, cam.image_height
     args, out, fwd = ours.run_forward(scene, cam, bg)
-    o = gs_oracle.forward(xyz, op, scales, q, sh, deg, bg=bg, **cam_kw(cam, W, H))
+    o = gs_oracle.forward(scene.means3D, scene.opacity, scene.scales, scene.rotations, scene.sh, scene.degrees, bg=bg, **cam_kw(cam, W, H))
     assert fwd["num_rendered"] == o["num_rendered"]
     counts = (o["ranges"][:, 1] - o["ranges"][:, 0]).astype(np.int64)
     if kind == "dense_4k":
