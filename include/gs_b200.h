@@ -287,6 +287,29 @@ GSB_API int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_
                  float* dL_dcampos /* [3] or NULL */, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
                  int32_t antialiasing, void* stream);
 
+/* Deterministic backward (DESIGN.md §5i): the same gradients as the default backward, summed in a fixed order, so the same inputs
+ * give the same bytes on every run, on any stream and device.  The render backward stores one partial per (Gaussian, tile)
+ * instance instead of adding into the per-Gaussian accumulator with float atomics; a gather adds each Gaussian's partials in
+ * row-major tile order.
+ * gsb_deterministic_workspace_bytes: the det_workspace size for P Gaussians and num_rendered instances (slot offsets, scan scratch
+ *                   and 40 bytes per instance).
+ * gsb_backward_deterministic: the arguments of gsb_backward_raw plus det_workspace.  raw / raw_grads may be NULL: then the activated
+ *                   or quantised backward of the scene, exactly as gsb_backward / gsb_backward_maps / gsb_backward_camera /
+ *                   gsb_backward_antialiased dispatch it.  It pairs with the blobs of any forward with the same anti-aliasing flag.
+ *                   No host synchronisation.  A num_rendered > 0 other than the blobs' instance count makes every accumulated
+ *                   gradient NaN (and no slot beyond num_rendered is written); num_rendered = 0 means nothing was rendered.
+ * Errors (GSB_EINVAL, nothing launched): scene NULL, P < 0, num_rendered < 0, det_workspace NULL with P > 0 and num_rendered > 0,
+ * a camera gradient without workspace, raw_grads without raw, and with raw the checks of gsb_backward_raw.
+ * GSB_ERANGE: num_rendered >= 2^30. */
+GSB_API size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered);
+GSB_API int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
+                 const char* geom_blob, const char* binning_blob, const char* image_blob,
+                 const float* dL_dout_color /* [3,H,W] */, const GsbGrads* grads,
+                 const float* dL_dinvdepth /* [1,H,W] or NULL */, const float* dL_dalpha /* [1,H,W] or NULL */,
+                 float lambda_sh_sparsity, float* dL_dviewmatrix /* [16] or NULL */, float* dL_dprojmatrix /* [16] or NULL */,
+                 float* dL_dcampos /* [3] or NULL */, char* workspace, const GsbRawParams* raw /* or NULL */,
+                 const GsbRawGrads* raw_grads /* or NULL */, int32_t antialiasing, char* det_workspace, void* stream);
+
 /* present[i] = view-space z of means3D[i] > 0.2 (auxiliary.h:139-159). */
 GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);

@@ -91,7 +91,8 @@ void prof_end(int kid, cudaStream_t stream)
 	t_prof_cur = nullptr;
 }
 static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter", "tile_sort_large", "unused4", "tile_sort", "unused6",
-	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad" };
+	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad", "det_scan",
+	"det_gather", "det_clear" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
 int launch_preprocess(const GsbScene*, const GsbCamera*, const GeomState&, const ImageState&, const BinPlan&, int32_t*, const GsbDebug*, bool,
@@ -118,6 +119,9 @@ int launch_render_backward(const ImageState&, const BinningState&, const GeomSta
 	const float*, float*, cudaStream_t);
 int launch_preprocess_backward(const GsbScene*, const GsbCamera*, const GeomState&, const int32_t*, const float*, const GsbGrads*, bool, float,
 	float*, bool, const GsbRawParams*, const GsbRawGrads*, cudaStream_t);
+size_t det_workspace_bytes(int, long long);
+int launch_render_backward_deterministic(const ImageState&, const BinningState&, const GeomState&, int, long long, int, int, const float*,
+	const float*, const float*, const float*, float*, char*, cudaStream_t);
 size_t camera_grad_workspace_bytes(int);
 int launch_camera_grad_finish(int, const float*, float*, float*, float*, cudaStream_t);
 
@@ -140,6 +144,19 @@ static int check_raw(const GsbScene* s, const GsbRawParams* raw)
 	}
 	else if (!raw->features_dc || !s->degrees || (raw->features_rest == nullptr) != (raw->C == 0))
 	{ set_error("raw parameters: features_dc, degrees and (for C > 0) features_rest are required without colors_precomp"); return GSB_EINVAL; }
+	return GSB_OK;
+}
+
+// What gsb_backward_raw (and gsb_backward_deterministic with raw parameters) requires of the gradient outputs.
+static int check_backward_raw(const GsbScene* scene, const GsbGrads* grads, const GsbRawParams* raw, const GsbRawGrads* raw_grads)
+{
+	if (int e = check_raw(scene, raw)) return e;
+	if (!raw_grads || !grads) { set_error("backward_raw: grads / raw_grads are NULL"); return GSB_EINVAL; }
+	if (grads->dL_dsh || grads->dL_dscales || grads->dL_drotations)
+	{ set_error("backward_raw: grads->dL_dsh, dL_dscales and dL_drotations must be NULL (raw_grads replaces them)"); return GSB_EINVAL; }
+	if (scene->colors_precomp && (raw_grads->dL_dfeatures_dc || raw_grads->dL_dfeatures_rest))
+	{ set_error("backward_raw: SH gradients requested together with colors_precomp"); return GSB_EINVAL; }
+	if (raw->C == 0 && raw_grads->dL_dfeatures_rest) { set_error("backward_raw: dL_dfeatures_rest given with C == 0"); return GSB_EINVAL; }
 	return GSB_OK;
 }
 
@@ -447,7 +464,7 @@ static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R,
 	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
 	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
 	float* dL_dview, float* dL_dproj, float* dL_dcampos, char* cam_workspace, bool aa, void* stream_,
-	const GsbRawParams* raw = nullptr, const GsbRawGrads* raw_grads = nullptr)
+	const GsbRawParams* raw = nullptr, const GsbRawGrads* raw_grads = nullptr, bool det = false, char* det_workspace = nullptr)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (int e = check_scene(scene, cam, raw)) return e;
@@ -475,7 +492,10 @@ static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R,
 	ImageState img = ImageState::carve(const_cast<char*>(image_blob), W, H);
 	BinningState b = BinningState::carve(const_cast<char*>(binning_blob), R);
 	float* acc = reinterpret_cast<float*>(const_cast<char*>(geom_blob) + geom_state_bytes(P));
-	if (int e = launch_render_backward(img, b, g, P, W, H, cam->background, dL_dout_color, dL_dinvdepth, dL_dalpha, acc, stream)) return e;
+	if (int e = det ? launch_render_backward_deterministic(img, b, g, P, R, W, H, cam->background, dL_dout_color, dL_dinvdepth, dL_dalpha,
+			acc, det_workspace, stream)
+		: launch_render_backward(img, b, g, P, W, H, cam->background, dL_dout_color, dL_dinvdepth, dL_dalpha, acc, stream))
+		return e;
 	float* cam_rows = want_cam ? reinterpret_cast<float*>(cam_workspace) : nullptr;
 	if (int e = launch_preprocess_backward(scene, cam, g, radii, acc, grads, dL_dinvdepth != nullptr, lambda_sh_sparsity, cam_rows, aa, raw,
 		raw_grads, stream))
@@ -540,15 +560,31 @@ int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_t R, con
 	if (!scene || scene->P < 0) { set_error("backward_raw: scene is NULL or P < 0"); return GSB_EINVAL; }
 	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
 	{ set_error("backward_raw: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
-	if (int e = check_raw(scene, raw)) return e;
-	if (!raw_grads || !grads) { set_error("backward_raw: grads / raw_grads are NULL"); return GSB_EINVAL; }
-	if (grads->dL_dsh || grads->dL_dscales || grads->dL_drotations)
-	{ set_error("backward_raw: grads->dL_dsh, dL_dscales and dL_drotations must be NULL (raw_grads replaces them)"); return GSB_EINVAL; }
-	if (scene->colors_precomp && (raw_grads->dL_dfeatures_dc || raw_grads->dL_dfeatures_rest))
-	{ set_error("backward_raw: SH gradients requested together with colors_precomp"); return GSB_EINVAL; }
-	if (raw->C == 0 && raw_grads->dL_dfeatures_rest) { set_error("backward_raw: dL_dfeatures_rest given with C == 0"); return GSB_EINVAL; }
+	if (int e = check_backward_raw(scene, grads, raw, raw_grads)) return e;
 	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
 		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, antialiasing != 0, stream, raw, raw_grads);
+}
+
+size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered); }
+
+int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
+	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
+	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
+	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
+	int32_t antialiasing, char* det_workspace, void* stream)
+{
+	if (!scene || scene->P < 0) { set_error("backward_deterministic: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if (R < 0) { set_error("backward_deterministic: num_rendered < 0"); return GSB_EINVAL; }
+	if (R >= (1ll << 30))
+	{ set_error("backward_deterministic: 2^30 or more instances (the slot scan's look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
+	if (scene->P > 0 && R > 0 && !det_workspace) { set_error("backward_deterministic: det_workspace is NULL"); return GSB_EINVAL; }
+	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
+	{ set_error("backward_deterministic: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
+	if (raw_grads && !raw) { set_error("backward_deterministic: raw_grads given without raw"); return GSB_EINVAL; }
+	if (raw) if (int e = check_backward_raw(scene, grads, raw, raw_grads)) return e;
+	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, antialiasing != 0, stream, raw, raw_grads, true,
+		det_workspace);
 }
 
 int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,

@@ -265,16 +265,28 @@ __device__ __forceinline__ void red_add_v2(float* addr, float a, float b)
 //    dL/dinvdepth fills the B column of the u product that is zero padding otherwise, and sum_p u_p * dL/dinvdepth(p) lands in
 //    slot 9 of the accumulator, next to cyy (one vector reduction instead of the scalar one).
 // 1/depth is the MUFU reciprocal here (the forward's IEEE value to 1 ulp; the result is a tolerance-compared gradient).
-template <bool MAPS>
-__global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __restrict__ ranges,
+//
+// DET = true is the deterministic variant (DESIGN.md §5i).  The pair arithmetic and the MMA pixel sums are the same; only the
+// summation across warps and tiles changes.  A staged batch is processed in lockstep: every warp flushes its stash at the end of
+// the batch and writes each row's 9 (10 with MAPS) values to its own shared-memory row of the batch entry (ebuf, zero for entries
+// it culled); after a CTA barrier the threads add the 8 warps' rows in warp order 0..7 and STORE the sum to the instance's slot
+// offset[g] + (ty - miny) * w + (tx - minx) of `parts` (no atomics).  det_gather_kernel then adds each Gaussian's slots in
+// row-major tile order.  The stash rows keep their batch entry index instead of the Gaussian id: the records are still staged.
+#define DET_NS(MAPS) ((MAPS) ? 10 : 9)       // floats per slot: the accumulator's [dcol0 dcol1 dcol2 dop sx sy cxx cxy cyy (dinvd)]
+template <bool MAPS, bool DET = false>
+__global__ void __launch_bounds__(256, DET ? 3 : 4) render_backward_kernel(const uint2* __restrict__ ranges,
 	const uint32_t* __restrict__ point_list,
 	int W, int H, const float4* __restrict__ rec, const float* __restrict__ bg,
 	const float* __restrict__ final_Ts, const uint32_t* __restrict__ n_contrib, const uint32_t* __restrict__ tile_max,
-	const float* __restrict__ dL_dpixels, float* __restrict__ acc, const float* __restrict__ dL_dinvdepth, const float* __restrict__ dL_dalpha)
+	const float* __restrict__ dL_dpixels, float* __restrict__ acc, const float* __restrict__ dL_dinvdepth, const float* __restrict__ dL_dalpha,
+	float* __restrict__ parts = nullptr, const uint32_t* __restrict__ slot_offset = nullptr, const uint2* __restrict__ rect = nullptr,
+	unsigned long long num_slots = 0)
 {
 	constexpr int NCH = MAPS ? 4 : 3;
+	constexpr int NS = DET_NS(MAPS);
 	extern __shared__ __align__(16) unsigned char s_dyn_raw[];
 	BwdSmem<NCH>& S = *reinterpret_cast<BwdSmem<NCH>*>(s_dyn_raw);
+	float* const ebuf = reinterpret_cast<float*>(s_dyn_raw + sizeof(BwdSmem<NCH>));     // DET: [8 warps][BWD_BATCH entries][NS]
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const int tile = blockIdx.y * gridDim.x + blockIdx.x;
 	const uint32_t hi = tile_max[tile];
@@ -332,6 +344,7 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 	Wp.dlp[lane] = dLp0; Wp.dlp[32 + lane] = dLp1; Wp.dlp[64 + lane] = dLp2;
 	if (MAPS) Wp.dlp[96 + lane] = dLd;
 	const float cxw = rx0 + 3.5f, cyw = ry0 + 1.5f;                                // centre of the warp's 8x4 pixel block
+	if (DET) for (int i = tid; i < 8 * BWD_BATCH * NS; i += 256) ebuf[i] = 0.0f;
 	__syncthreads();
 
 	// Pixel sums of the stashed rows on the tensor cores; lane (g, t = 0) then owns rows g and g + 8: it converts the moments
@@ -341,7 +354,7 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 		if (nrows == 0) return;
 		for (uint32_t r = nrows; r < 16; r++) { sw[r * STASH_LD + lane] = 0.f; su[r * STASH_LD + lane] = 0.f; }
 		__syncwarp();
-		if (ft == 0)                                                                 // the epilogue re-reads the rows' records: pull them into L1 behind the MMAs
+		if (!DET && ft == 0)                                                         // the epilogue re-reads the rows' records: pull them into L1 behind the MMAs
 		{
 			if (fg < nrows) asm volatile("prefetch.global.L1 [%0];" ::"l"(rec + 3 * (size_t)Wp.rowid[fg]));
 			if (fg + 8 < nrows) asm volatile("prefetch.global.L1 [%0];" ::"l"(rec + 3 * (size_t)Wp.rowid[fg + 8]));
@@ -383,13 +396,29 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 			if (ft == 0 && row < nrows)
 			{
 				const uint32_t gid = Wp.rowid[row];
-				const float4 r0 = __ldg(rec + 3 * (size_t)gid), r1 = __ldg(rec + 3 * (size_t)gid + 1);      // L2-resident: staged moments ago
+				float4 r0, r1;
+				if (DET)
+				{
+					// gid is the row's batch entry: its record is still in the current stage
+					const uint32_t ra = sbase0 + (uint32_t)(buf * BWD_BATCH * 3) * 16u + gid * SREC_BYTES;
+					r0 = lds128(ra); r1 = lds128(ra + 16);
+				}
+				else { r0 = __ldg(rec + 3 * (size_t)gid); r1 = __ldg(rec + 3 * (size_t)gid + 1); }      // L2-resident: staged moments ago
 				const float X = r1.x - cxw, Y = r1.y - cyw, o = r1.z;
 				const float M0 = dw[2 * h], Mx = dw[2 * h + 1];
 				const float Sx = X * M0 - Mx, Sy = Y * M0 - My;
 				const float Sxx = X * X * M0 - 2.0f * X * Mx + Mxx;
 				const float Sxy = X * Y * M0 - X * My - Y * Mx + Mxy;
 				const float Syy = Y * Y * M0 - 2.0f * Y * My + Myy;
+				if (DET)
+				{
+					float* e = ebuf + (warp * BWD_BATCH + gid) * NS;
+					e[0] = du[2 * h]; e[1] = du[2 * h + 1]; e[2] = c2; e[3] = M0;
+					e[4] = -o * (r0.x * Sx + r0.y * Sy); e[5] = -o * (r0.z * Sy + r0.y * Sx); e[6] = o * Sxx; e[7] = o * Sxy;
+					e[8] = o * Syy;
+					if (MAPS) e[9] = dinvd;
+					continue;
+				}
 				float* a = acc + 12 * (size_t)gid;
 				red_add_v4(a, du[2 * h], du[2 * h + 1], c2, M0);
 				red_add_v4(a + 4, -o * (r0.x * Sx + r0.y * Sy), -o * (r0.z * Sy + r0.y * Sx), o * Sxx, o * Sxy);
@@ -509,10 +538,37 @@ __global__ void __launch_bounds__(256, 4) render_backward_kernel(const uint2* __
 				const uint32_t sa = wbase + (nrows * STASH_LD + lane) * 4;
 				asm volatile("st.shared.f32 [%0], %1;" ::"r"(sa), "f"(wv) : "memory");
 				asm volatile("st.shared.f32 [%0+%2], %1;" ::"r"(sa), "f"(uv), "n"(BW_OFF_U) : "memory");
-				if (lane == 0) asm volatile("st.shared.f32 [%0+%2], %1;" ::"r"(wbase + nrows * 4), "f"(r2.w), "n"(BW_OFF_ROWID(NCH)) : "memory");
+				if (lane == 0) asm volatile("st.shared.f32 [%0+%2], %1;" ::"r"(wbase + nrows * 4), "f"(DET ? __uint_as_float(jj) : r2.w), "n"(BW_OFF_ROWID(NCH)) : "memory");
 			}
 			nrows++;
 			if (nrows == 16) flush_rows();
+		}
+		if (DET)
+		{
+			flush_rows();
+			__syncthreads();
+			// 4 threads per batch entry j, components k0, k0 + 4, k0 + 8: the 8 warps' rows added in warp order, then zeroed
+			const int j = tid >> 2;
+			if (j < n)
+			{
+				const uint32_t gid = __float_as_uint(S.rec[buf][3 * j + 2].w);
+				const uint2 rc = rect[gid];
+				const uint32_t minx = rc.x & 0xffffu, maxx = rc.x >> 16, miny = rc.y & 0xffffu;
+				const unsigned long long slot = (unsigned long long)slot_offset[gid] + (blockIdx.y - miny) * (maxx - minx) + (blockIdx.x - minx);
+				for (int k = tid & 3; k < NS; k += 4)
+				{
+					float s = ebuf[j * NS + k];
+					ebuf[j * NS + k] = 0.0f;
+#pragma unroll
+					for (int w = 1; w < 8; w++)
+					{
+						s += ebuf[(w * BWD_BATCH + j) * NS + k];
+						ebuf[(w * BWD_BATCH + j) * NS + k] = 0.0f;
+					}
+					if (slot < num_slots) parts[slot * NS + k] = s;       // out of range only for blobs that do not match R (det_gather flags it)
+				}
+			}
+			__syncthreads();
 		}
 		__syncwarp();
 		if (lane == 0) mbar_arrive(&S.empty[buf]);           // this warp no longer reads the stage (stashed rows carry their own data)
@@ -557,6 +613,36 @@ int launch_render_backward(const ImageState& img, const BinningState& b, const G
 	else
 		render_backward_kernel<false><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
 			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, acc, nullptr, nullptr);
+	GSB_LAUNCHED();
+	GSB_CUDA_OK(cudaGetLastError());
+	return GSB_OK;
+}
+
+// Deterministic render backward (DESIGN.md §5i): per-instance partials into `parts` (R slots of DET_NS floats), slot bases
+// `slot_offset` from det_scan_kernel.  The accumulator is not touched here: det_gather_kernel writes all of it.
+int launch_render_backward_det(const ImageState& img, const BinningState& b, const GeomState& g, long long R, int W, int H,
+	const float* bg, const float* dL_dpix, const float* dL_dinvdepth, const float* dL_dalpha, float* parts, const uint32_t* slot_offset,
+	cudaStream_t stream)
+{
+	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
+	const bool maps = dL_dinvdepth || dL_dalpha;
+	const void* kernel = maps ? (const void*)render_backward_kernel<true, true> : (const void*)render_backward_kernel<false, true>;
+	const size_t smem = (maps ? sizeof(BwdSmem<4>) : sizeof(BwdSmem<3>)) + size_t(8) * BWD_BATCH * DET_NS(maps) * sizeof(float);
+	if (int e = ensure_dyn_smem(kernel, (int)smem)) return e;
+	{
+		// instances behind a tile's last contributor (and tiles with none) are never visited: their slots must read as zero
+		ProfScope prof(K_DET_CLEAR, stream);
+		GSB_CUDA_OK(cudaMemsetAsync(parts, 0, size_t(R) * DET_NS(maps) * sizeof(float), stream));
+	}
+	ProfScope prof(K_RENDER_BWD, stream);
+	if (maps)
+		render_backward_kernel<true, true><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
+			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, nullptr, dL_dinvdepth, dL_dalpha, parts, slot_offset, g.rect,
+			(unsigned long long)R);
+	else
+		render_backward_kernel<false, true><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
+			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, nullptr, nullptr, nullptr, parts, slot_offset, g.rect,
+			(unsigned long long)R);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;

@@ -11,6 +11,8 @@ campos (gsb_backward_camera).  `antialiasing` (forward and backward, the same va
 that the 0.3 px^2 dilation no longer inflates sub-pixel splats (gsb_forward_antialiased / gsb_backward_antialiased).  `raw`
 (forward and backward) takes the model's leaf parameters (features_dc, features_rest, scaling, rotation) in place of sh, scales
 and rotations, and applies exp / F.normalize / the SH concatenation inside the kernels (gsb_forward_raw / gsb_backward_raw).
+`deterministic` (backward) sums the per-Gaussian gradients in a fixed order: the same bytes on every run
+(gsb_backward_deterministic).
 """
 from __future__ import annotations
 
@@ -240,7 +242,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R,
                                  binningBuffer, imageBuffer, lambda_sh_sparsity, debug, *, prune_mask=None, quant=None,
                                  accumulate_into=None, want_conic=False, view_means2D=None, dL_dinvdepth=None, dL_dalpha=None,
-                                 camera_grads=False, antialiasing=False, raw=None):
+                                 camera_grads=False, antialiasing=False, raw=None, deterministic=False):
     """rasterize_points.h:65-88 RasterizeGaussiansBackwardCUDA ->
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     `accumulate_into`: the same 8-tuple from a previous call; gradients are added in place (view-batch accumulation);
@@ -252,7 +254,9 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     `raw`: the backward of a forward with the same `raw` (gsb_backward_raw).  The 8-tuple then becomes the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, None, dL_dfeatures_dc, dL_dfeatures_rest, dL_dscaling, dL_drotation):
     the SH gradient split at coefficient 1, scaling / rotation chained through exp / F.normalize; dL_dcolors only with colors
-    (else None), the SH gradients None with colors, and no dL_dcov3D.  `accumulate_into` takes that 9-tuple."""
+    (else None), the SH gradients None with colors, and no dL_dcov3D.  `accumulate_into` takes that 9-tuple.
+    `deterministic`: sum the per-Gaussian gradients in a fixed order instead of with float atomics (gsb_backward_deterministic):
+    the same inputs give the same bytes on every run, in every mode above; the values agree with the default path to rounding."""
     device = _device_of(means3D)
     if raw is not None:
         want_sh = not _present(colors)
@@ -306,7 +310,13 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                 C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
                 *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4))
         stream = _lib.current_stream(device)
-        if raw is not None:
+        if deterministic:
+            # per-instance partial slots, from the caching allocator on the current stream (freed in stream order after the call)
+            det_ws = torch.empty(int(L.gsb_deterministic_workspace_bytes(P, int(R))), dtype=torch.uint8, device=device)
+            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
+            st = L.gsb_backward_deterministic(*head, C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None,
+                                              int(bool(antialiasing)), det_ws.data_ptr(), stream)
+        elif raw is not None:
             rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]])
             st = L.gsb_backward_raw(*head, C.byref(raw_s), C.byref(rg), int(bool(antialiasing)), stream)
         else:

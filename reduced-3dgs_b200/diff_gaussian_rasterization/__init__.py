@@ -14,7 +14,8 @@ debug=True (reference :85 hard-wires a device sync after every stage); gradients
 because the kernels write every element.  GaussianRasterizer.forward also takes keyword-only `raw_params`, the model's leaf
 tensors (features_dc, features_rest, scaling, rotation) in place of shs / scales / rotations: exp, F.normalize and the SH
 concatenation then run inside the kernels, and the gradients of the four tensors are the kernels' own outputs
-(_RasterizeGaussiansRaw).
+(_RasterizeGaussiansRaw).  GaussianRasterizationSettings' keyword-only `deterministic` (default: torch's deterministic-algorithms
+flag) selects the backward that sums each Gaussian's gradients in a fixed order (the same bytes on every run).
 """
 from typing import NamedTuple
 
@@ -70,6 +71,13 @@ def _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_
     return out, (out[1], out[2])
 
 
+def _deterministic(raster_settings):
+    """The settings' `deterministic`: an explicit bool wins; None follows torch.are_deterministic_algorithms_enabled(), read when
+    the backward runs."""
+    d = getattr(raster_settings, "deterministic", None)
+    return torch.are_deterministic_algorithms_enabled() if d is None else bool(d)
+
+
 def _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp,
               sh, degrees, geomBuffer, binningBuffer, imgBuffer, **kw):
     """The backward both ops share: the _C call from the saved state.  -> (its gradient tuple, the gradients of the camera
@@ -84,6 +92,8 @@ def _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, co
             ctx.lambda_sh_sparsity, rs.debug)
     kw.update(prune_mask=ctx.prune_mask, dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need),
               antialiasing=rs.antialiasing)
+    if _deterministic(rs):
+        kw.update(deterministic=True)
     g = _call(_C.rasterize_gaussians_backward, args, kw,
               "snapshot_bw.dump", "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
     if ctx.camera_meta is None:
@@ -201,19 +211,25 @@ class _ReferenceSettings(NamedTuple):
 
 class GaussianRasterizationSettings(_ReferenceSettings):
     """The reference's 12-field settings tuple (its `_fields`, length and positional layout are unchanged) plus upstream 3DGS's
-    trailing `antialiasing` flag, given as a keyword or as a 13th positional argument; default False."""
+    trailing `antialiasing` flag, given as a keyword or as a 13th positional argument; default False.
+    `deterministic` (keyword only): True sums the backward's per-Gaussian gradients in a fixed order, so the same inputs give the
+    same bytes on every run; False keeps the faster atomic summation; None (default) follows torch.use_deterministic_algorithms,
+    read when the backward runs."""
     antialiasing = False
+    deterministic = None
 
-    def __new__(cls, *args, antialiasing=False, **kwargs):
+    def __new__(cls, *args, antialiasing=False, deterministic=None, **kwargs):
         if len(args) == len(_ReferenceSettings._fields) + 1:
             *args, antialiasing = args
         self = super().__new__(cls, *args, **kwargs)
         self.antialiasing = bool(antialiasing)
+        self.deterministic = None if deterministic is None else bool(deterministic)
         return self
 
     def _replace(self, **kwargs):
         antialiasing = kwargs.pop("antialiasing", self.antialiasing)
-        return type(self)(*super()._replace(**kwargs), antialiasing=antialiasing)
+        deterministic = kwargs.pop("deterministic", self.deterministic)
+        return type(self)(*super()._replace(**kwargs), antialiasing=antialiasing, deterministic=deterministic)
 
 
 class GaussianRasterizer(nn.Module):

@@ -181,6 +181,10 @@ def lib():
         L.gsb_backward_raw.restype = C.c_int
         L.gsb_backward_raw.argtypes = L.gsb_backward_camera.argtypes[:-1] + [C.POINTER(GsbRawParams), C.POINTER(GsbRawGrads), C.c_int32,
                                                                              C.c_void_p]
+        L.gsb_deterministic_workspace_bytes.restype = C.c_size_t
+        L.gsb_deterministic_workspace_bytes.argtypes = [C.c_int32, C.c_int64]
+        L.gsb_backward_deterministic.restype = C.c_int
+        L.gsb_backward_deterministic.argtypes = L.gsb_backward_raw.argtypes[:-1] + [C.c_void_p, C.c_void_p]
         L.gsb_mark_visible.restype = C.c_int
         L.gsb_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_export_binning.restype = C.c_int
@@ -219,7 +223,7 @@ def profile_enable(on: bool):
 
 def profile_read() -> dict:
     """{kernel name: (total ms, launches)} since the previous read (waits for the recorded events)."""
-    n = 16
+    n = 32
     names = (C.c_char_p * n)()
     ms = (C.c_double * n)()
     cnt = (C.c_uint64 * n)()
@@ -236,7 +240,7 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_forward_maps", "gsb_backward_maps", "gsb_camera_grad_workspace_bytes", "gsb_backward_camera",
                     "gsb_forward_antialiased", "gsb_backward_antialiased", "gsb_adam_step", "gsb_densify_stats",
                     "gsb_densify_workspace_bytes", "gsb_densify_split_std_offset", "gsb_densify_plan", "gsb_densify_emit",
-                    "gsb_forward_raw", "gsb_backward_raw"]
+                    "gsb_forward_raw", "gsb_backward_raw", "gsb_deterministic_workspace_bytes", "gsb_backward_deterministic"]
 
 
 def check(status: int):
