@@ -155,6 +155,20 @@ GSB_API int gsb_forward_statistics(const GsbScene* scene, const GsbCamera* cam,
                 float* out_color, int32_t* radii, int64_t* num_rendered,
                 int32_t* touched_pixels, float* transmittance_sum, void* stream);
 
+/* Deterministic gsb_forward_statistics (DESIGN.md §5j): the same outputs, and the same bytes on every run.  Each per-warp sum of
+ * transmittances is rounded to a multiple of 2^-36 and added as a 64-bit integer, so the order of the additions does not matter;
+ * each total is then rounded to float once (relative error below 1e-7 against the exact sum of the per-warp sums).
+ * gsb_statistics_workspace_bytes: the workspace size for P Gaussians (8 bytes per Gaussian); one workspace serves every camera.
+ * Errors (GSB_EINVAL, nothing launched): those of gsb_forward_statistics, and workspace NULL with P > 0.
+ * GSB_ERANGE: width * height >= 2^28 (a Gaussian's total, at most width * height, must fit 64 bits at 2^36 per unit). */
+GSB_API size_t gsb_statistics_workspace_bytes(int32_t P);
+GSB_API int gsb_forward_statistics_deterministic(const GsbScene* scene, const GsbCamera* cam,
+                gsb_alloc_fn geom_alloc, void* geom_user,
+                gsb_alloc_fn binning_alloc, void* binning_user,
+                gsb_alloc_fn image_alloc, void* image_user,
+                float* out_color, int32_t* radii, int64_t* num_rendered,
+                int32_t* touched_pixels, float* transmittance_sum, char* workspace, void* stream);
+
 /* Backward from the blobs of the paired forward.  Fully asynchronous on `stream`. */
 GSB_API int gsb_backward(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
                  const char* geom_blob, const char* binning_blob, const char* image_blob,
@@ -362,6 +376,17 @@ GSB_API int gsb_min_redundancy_value(int32_t P, const int32_t* redundancy_values
 GSB_API size_t gsb_kmeans_workspace_bytes(int64_t n_values, int32_t n_centers);
 GSB_API int gsb_kmeans(const float* values, int64_t n_values, const float* centers_in, int32_t n_centers, float tol, int32_t max_iterations,
                 int32_t* ids, float* centers_out, char* workspace, void* stream);
+
+/* Deterministic k-means (DESIGN.md §5j): the arguments, sort, assignment and tie rule, update, stopping rule and 16-iteration host
+ * poll of gsb_kmeans; only the centre sums change.  Each cluster's values are added in an order that is a function of the input
+ * alone (fixed-size chunks and blocks of the sorted values, aligned pairwise trees; not of the grid, SM count, stream or workspace
+ * address), so the same input gives the same centres and ids on every run and every H100.
+ * workspace: gsb_kmeans_deterministic_workspace_bytes(n_values, n_centers) bytes of device memory, 16-byte aligned.
+ * Errors (GSB_EINVAL, nothing launched): those of gsb_kmeans, and a workspace that is not 16-byte aligned.
+ * GSB_ERANGE: n_values >= 2^30. */
+GSB_API size_t gsb_kmeans_deterministic_workspace_bytes(int64_t n_values, int32_t n_centers);
+GSB_API int gsb_kmeans_deterministic(const float* values, int64_t n_values, const float* centers_in, int32_t n_centers, float tol,
+                int32_t max_iterations, int32_t* ids, float* centers_out, char* workspace, void* stream);
 
 /* Exact k nearest neighbours of points [P,3] (fp32) — the reference's second extension simple_knn._C (submodules/simple-knn:
  * distCUDA2, distIndex2, distIndexQ).  Squared distances d = (p - q).(p - q) evaluated as the reference evaluates them; the query

@@ -103,7 +103,8 @@ int launch_scatter_sort(const GeomState&, const BinningState&, const ImageState&
 int launch_sort_large(const GeomState&, const BinningState&, const ImageState&, int, int, uint32_t, uint32_t, cudaStream_t);
 int launch_export_binning(const GeomState&, const BinningState&, const ImageState&, int, int, uint64_t*, uint32_t*, cudaStream_t);
 int launch_render_forward(const ImageState&, const BinningState&, const GeomState&, int, int, const float*, float*, int32_t*, float*, float*, float*,
-	cudaStream_t);
+	bool, cudaStream_t);
+int launch_stats_fixed_to_float(int, const unsigned long long*, float*, cudaStream_t);
 int launch_sh_stats_update(int, int, const int*, const float*, const float*, const float*, const int*, const int*, const float*, float*, float*,
 	float*, float*, float*, cudaStream_t);
 int launch_pixel_size(int, const float*, int, const float*, const float*, const int*, const int*, float*, cudaStream_t);
@@ -113,6 +114,8 @@ int launch_l1_ssim_forward(const float*, const float*, int, int, int, float*, fl
 int launch_l1_ssim_backward(const float*, const float*, int, int, int, const float*, float, const float*, float, const float*, float*, cudaStream_t);
 size_t kmeans_workspace_bytes(long long, int);
 int launch_kmeans(const float*, long long, const float*, int, float, int, int*, float*, char*, cudaStream_t);
+size_t kmeans_deterministic_workspace_bytes(long long, int);
+int launch_kmeans_deterministic(const float*, long long, const float*, int, float, int, int*, float*, char*, cudaStream_t);
 size_t knn_workspace_bytes(long long, long long);
 int launch_knn(const float*, long long, int, const int32_t*, long long, const int32_t*, long long, float*, float*, int32_t*, char*, cudaStream_t);
 int launch_render_backward(const ImageState&, const BinningState&, const GeomState&, int, int, int, const float*, const float*, const float*,
@@ -256,7 +259,7 @@ static thread_local std::map<int, HostSide> t_host;
 static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
 	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
 	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, int32_t* touched_pixels, float* transmittance,
-	float* out_invdepth, float* out_alpha, bool aa, void* stream_, const GsbRawParams* raw = nullptr)
+	float* out_invdepth, float* out_alpha, bool aa, void* stream_, const GsbRawParams* raw = nullptr, bool fixed_point_stats = false)
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	if (int e = check_scene(scene, cam, raw)) return e;
@@ -321,7 +324,7 @@ static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_f
 	}
 	if (R > 0) if (int e = launch_sort_large(g, b, img, W, H, hc[4], hc[5], stream)) return e;
 	if (int e = launch_render_forward(img, b, g, W, H, cam->background, out_color, touched_pixels, transmittance, out_invdepth, out_alpha,
-		stream)) return e;
+		fixed_point_stats, stream)) return e;
 	return GSB_OK;
 }
 
@@ -368,6 +371,32 @@ int gsb_forward_statistics(const GsbScene* scene, const GsbCamera* cam, gsb_allo
 	}
 	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
 		num_rendered, nullptr, touched_pixels, transmittance_sum, nullptr, nullptr, false, stream);
+}
+
+size_t gsb_statistics_workspace_bytes(int32_t P) { return (P > 0 ? size_t(P) * sizeof(unsigned long long) : 0) + 256; }
+
+int gsb_forward_statistics_deterministic(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
+	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
+	float* out_color, int32_t* radii, int64_t* num_rendered, int32_t* touched_pixels, float* transmittance_sum, char* workspace,
+	void* stream)
+{
+	if (!scene || scene->P < 0) { set_error("statistics_deterministic: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if (scene->P > 0 && (!touched_pixels || !transmittance_sum)) { set_error("statistics output pointers missing"); return GSB_EINVAL; }
+	if (scene->P > 0 && !workspace) { set_error("statistics_deterministic: workspace is NULL"); return GSB_EINVAL; }
+	if (cam && (long long)cam->width * cam->height >= (1ll << 28))
+	{
+		set_error("statistics_deterministic: %d x %d pixels; the 64-bit fixed-point sums need W * H < 2^28", cam->width, cam->height);
+		return GSB_ERANGE;
+	}
+	unsigned long long* fixed = reinterpret_cast<unsigned long long*>(workspace);
+	if (scene->P > 0)
+	{
+		GSB_CUDA_OK(cudaMemsetAsync(touched_pixels, 0, size_t(scene->P) * sizeof(int32_t), (cudaStream_t)stream));
+		GSB_CUDA_OK(cudaMemsetAsync(fixed, 0, size_t(scene->P) * sizeof(unsigned long long), (cudaStream_t)stream));
+	}
+	if (int e = forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
+		num_rendered, nullptr, touched_pixels, reinterpret_cast<float*>(fixed), nullptr, nullptr, false, stream, nullptr, true)) return e;
+	return launch_stats_fixed_to_float(scene->P, fixed, transmittance_sum, (cudaStream_t)stream);
 }
 
 int gsb_sh_statistics_update(int32_t P, int32_t M, const int32_t* degrees, const float* means3D, const float* campos, const float* shs,
@@ -428,6 +457,24 @@ int gsb_kmeans(const float* values, int64_t n_values, const float* centers_in, i
 	if (!centers_in || !centers_out || (n_values > 0 && (!values || !ids || !workspace))) { set_error("kmeans: NULL argument"); return GSB_EINVAL; }
 	if (n_values >= (1ll << 30)) { set_error("kmeans: 2^30 or more values (the look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
 	return launch_kmeans(values, n_values, centers_in, n_centers, tol, max_iterations, ids, centers_out, workspace, (cudaStream_t)stream);
+}
+
+size_t gsb_kmeans_deterministic_workspace_bytes(int64_t n_values, int32_t n_centers)
+{
+	return kmeans_deterministic_workspace_bytes(n_values < 0 ? 0 : n_values, n_centers);
+}
+
+int gsb_kmeans_deterministic(const float* values, int64_t n_values, const float* centers_in, int32_t n_centers, float tol,
+	int32_t max_iterations, int32_t* ids, float* centers_out, char* workspace, void* stream)
+{
+	if (n_values < 0 || n_centers <= 0 || max_iterations < 0) { set_error("kmeans_deterministic: bad sizes"); return GSB_EINVAL; }
+	if (!centers_in || !centers_out || (n_values > 0 && (!values || !ids || !workspace)))
+	{ set_error("kmeans_deterministic: NULL argument"); return GSB_EINVAL; }
+	if (reinterpret_cast<uintptr_t>(workspace) & 15) { set_error("kmeans_deterministic: workspace is not 16-byte aligned"); return GSB_EINVAL; }
+	if (n_values >= (1ll << 30))
+	{ set_error("kmeans_deterministic: 2^30 or more values (the look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
+	return launch_kmeans_deterministic(values, n_values, centers_in, n_centers, tol, max_iterations, ids, centers_out, workspace,
+		(cudaStream_t)stream);
 }
 
 size_t gsb_knn_workspace_bytes(int32_t P, int32_t n_queries) { return knn_workspace_bytes(P < 0 ? 0 : P, n_queries); }

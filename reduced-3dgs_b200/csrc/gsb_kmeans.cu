@@ -13,7 +13,8 @@
 //   * update + convergence test on the device: later iterations see the `done` flag and exit immediately, the host only
 //     looks at the flag every few iterations (same stopping rule as the reference, without a sync per iteration).
 // Cluster ids / sizes are exact; centre values differ from the reference in float summation order only (the reference's own
-// order is arbitrary: atomics).
+// order is arbitrary: atomics).  gsb_kmeans_deterministic replaces the accumulate step by km_det_block_kernel +
+// km_det_cluster_kernel, which add each cluster's values in an order fixed by the input (see below, DESIGN.md §5j).
 #include "gsb_common.cuh"
 
 namespace gsb {
@@ -352,6 +353,141 @@ __global__ void __launch_bounds__(256) km_ids_kernel(const float* __restrict__ v
 		ids[i] = km_assign(S, K, values[i]);
 }
 
+// ------------------------------------------------------------------------------------------------ deterministic centre sums
+// The order in which gsb_kmeans_deterministic adds a cluster's values (DESIGN.md §5j; restated in oracle/kmeans_det_order.py) is a
+// function of the sorted values and their ids alone.  Sorted position p lies in block b = p / 4096 and, inside it, in chunk
+// t = (p % 4096) / 16.  With -0.0f, the exact identity of IEEE addition, standing for "no value":
+//   leaf(b, t, k)  = (((-0 + v_p0) + v_p1) + ...) over the positions of chunk t with id k, ascending;
+//   part(b, k)     = aligned pairwise tree over t = 0..255 of leaf(b, t, k): (0+1), (2+3), ..., then (01+23), ...;
+//   lane(l, k)     = (((-0 + part(l, k)) + part(l + 256, k)) + ...) over the blocks b = l (mod 256), ascending;
+//   sum(k)         = (aligned pairwise tree over l = 0..255 of lane(l, k)) + (+0.0f).
+// The final +0 turns the -0 of an empty (or all -0) cluster into the +0 of the default path's zeroed accumulator.  A run of one
+// cluster across many blocks is summed by all their CTAs (part) and then 256 threads (lane); no thread walks a long run.
+#define KM_DET_BLOCK (256 * KM_CHUNK)
+
+struct KmDetPart {
+	int k;               // cluster
+	float sum;           // part(b, k)
+};
+
+// 256 floats, one per thread, added as an aligned pairwise tree; the result is valid in thread 0.  s_tree: 8 floats of shared memory.
+__device__ __forceinline__ float km_det_tree256(float x, float* s_tree)
+{
+	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+	// offset o: lane l (a multiple of 2o) adds lane l + o, which holds the partial of [l + o, l + 2o); the other lanes compute
+	// values no later step reads
+#pragma unroll
+	for (int o = 1; o < 32; o <<= 1) x = __fadd_rn(x, __shfl_down_sync(0xffffffffu, x, o));
+	if (lane == 0) s_tree[warp] = x;
+	__syncthreads();
+	float r = 0.0f;
+	if (threadIdx.x == 0)
+		r = __fadd_rn(__fadd_rn(__fadd_rn(s_tree[0], s_tree[1]), __fadd_rn(s_tree[2], s_tree[3])),
+			__fadd_rn(__fadd_rn(s_tree[4], s_tree[5]), __fadd_rn(s_tree[6], s_tree[7])));
+	return r;
+}
+
+// One CTA per block of 4096 sorted values: the ids (km_assign, as the default path), the exact sizes (integer atomics), and
+// part(b, k) for every cluster k present in the block, one round per cluster in increasing k, appended to the block's list.
+__global__ void __launch_bounds__(256) km_det_block_kernel(const uint32_t* __restrict__ sorted_keys, long long n, const float* __restrict__ centres,
+	int K, int* __restrict__ sizes, KmDetPart* __restrict__ parts, int* __restrict__ part_count, int* __restrict__ span_lo,
+	int* __restrict__ span_hi, const KmState* __restrict__ state)
+{
+	if (state->done) return;
+	__shared__ KmCentres S;
+	__shared__ int s_min[8];
+	__shared__ float s_tree[8];
+	__shared__ int s_cnt[8];
+	km_load_sorted_centres(S, centres, K);
+	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const long long a = (long long)blockIdx.x * KM_DET_BLOCK + (long long)tid * KM_CHUNK;
+	float v[KM_CHUNK];
+	int id[KM_CHUNK];
+	if (a + KM_CHUNK <= n)
+	{
+		const uint4* src = reinterpret_cast<const uint4*>(sorted_keys + a);
+#pragma unroll
+		for (int q = 0; q < KM_CHUNK / 4; q++)
+		{
+			const uint4 k4 = src[q];
+			v[4 * q] = key_float(k4.x); v[4 * q + 1] = key_float(k4.y); v[4 * q + 2] = key_float(k4.z); v[4 * q + 3] = key_float(k4.w);
+		}
+	}
+	else
+	{
+#pragma unroll
+		for (int i = 0; i < KM_CHUNK; i++) v[i] = a + i < n ? key_float(sorted_keys[a + i]) : 0.0f;
+	}
+#pragma unroll
+	for (int i = 0; i < KM_CHUNK; i++) id[i] = a + i < n ? km_assign(S, K, v[i]) : 0x7fffffff;
+
+	int prev = -1, r = 0;
+	for (;;)
+	{
+		int mine = 0x7fffffff;
+#pragma unroll
+		for (int i = 0; i < KM_CHUNK; i++) if (id[i] > prev && id[i] < mine) mine = id[i];
+		mine = __reduce_min_sync(0xffffffffu, mine);
+		if (lane == 0) s_min[warp] = mine;
+		__syncthreads();
+		int k = s_min[0];
+#pragma unroll
+		for (int w = 1; w < 8; w++) k = min(k, s_min[w]);
+		if (k == 0x7fffffff) break;                                   // uniform: every thread read the same s_min
+		float leaf = -0.0f;
+		int cnt = 0;
+#pragma unroll
+		for (int i = 0; i < KM_CHUNK; i++) if (id[i] == k) { leaf = __fadd_rn(leaf, v[i]); cnt++; }
+		cnt = __reduce_add_sync(0xffffffffu, cnt);
+		if (lane == 0) s_cnt[warp] = cnt;
+		const float part = km_det_tree256(leaf, s_tree);              // its barrier also orders the s_cnt stores before the read below
+		if (tid == 0)
+		{
+			int c = 0;
+#pragma unroll
+			for (int w = 0; w < 8; w++) c += s_cnt[w];
+			parts[(size_t)blockIdx.x * K + r] = KmDetPart{ k, part };
+			atomicAdd(&sizes[k], c);
+			atomicMin(&span_lo[k], (int)blockIdx.x);
+			atomicMax(&span_hi[k], (int)blockIdx.x);
+		}
+		r++;
+		prev = k;
+	}
+	if (tid == 0) part_count[blockIdx.x] = r;
+}
+
+// One CTA per cluster: lane(l, k) over the blocks of its span, then the pairwise tree over the 256 lanes; writes sums[k] and resets
+// the span for the next iteration.
+__global__ void __launch_bounds__(256) km_det_cluster_kernel(const KmDetPart* __restrict__ parts, const int* __restrict__ part_count, int K,
+	float* __restrict__ sums, int* __restrict__ span_lo, int* __restrict__ span_hi, const KmState* __restrict__ state)
+{
+	if (state->done) return;
+	__shared__ float s_tree[8];
+	const int k = blockIdx.x, tid = threadIdx.x;
+	const int lo = span_lo[k], hi = span_hi[k];
+	float acc = -0.0f;
+	if (lo <= hi)
+		for (int b = lo + ((tid - lo % 256 + 256) % 256); b <= hi; b += 256)         // the blocks b = tid (mod 256) in [lo, hi]
+		{
+			const KmDetPart* p = parts + (size_t)b * K;
+			const int c = part_count[b];
+			for (int j = 0; j < c; j++)
+			{
+				const KmDetPart e = p[j];
+				if (e.k == k) { acc = __fadd_rn(acc, e.sum); break; }
+				if (e.k > k) break;                                              // a block's list is in increasing k
+			}
+		}
+	const float s = km_det_tree256(acc, s_tree);
+	if (tid == 0)
+	{
+		sums[k] = __fadd_rn(s, 0.0f);
+		span_lo[k] = 0x7fffffff;
+		span_hi[k] = -1;
+	}
+}
+
 // ------------------------------------------------------------------------------------------------ host
 struct KmWorkspace {
 	uint32_t* keys0; uint32_t* keys1; uint32_t* hist; KmSortPlan* plan; uint32_t* lookback; uint32_t* tickets;
@@ -377,14 +513,38 @@ static KmWorkspace km_carve(char* base, long long n, int K)
 
 size_t kmeans_workspace_bytes(long long n, int K) { return km_carve(nullptr, n, K).bytes; }
 
-int launch_kmeans(const float* values, long long n, const float* centres_in, int K, float tol, int max_iterations, int* ids, float* centres,
-	char* workspace, cudaStream_t stream)
+// The deterministic path's workspace: the default's, then per block of 4096 values a list of up to K parts and its length, and
+// the per-cluster block spans.
+struct KmDetWorkspace {
+	KmDetPart* parts; int* part_count; int* span_lo; int* span_hi; size_t n_blocks; size_t bytes;
+};
+static KmDetWorkspace km_det_carve(char* base, long long n, int K)
+{
+	const size_t head = km_carve(nullptr, n, K).bytes;
+	Carver c(base ? base + head : nullptr);
+	KmDetWorkspace d;
+	const size_t nn = n > 0 ? (size_t)n : 1;
+	d.n_blocks = (nn + KM_DET_BLOCK - 1) / KM_DET_BLOCK;
+	d.parts = c.take<KmDetPart>(d.n_blocks * (size_t)std::max(K, 1));
+	d.part_count = c.take<int>(d.n_blocks);
+	d.span_lo = c.take<int>(KM_MAX_K); d.span_hi = c.take<int>(KM_MAX_K);
+	d.bytes = head + c.off + 256;
+	return d;
+}
+
+size_t kmeans_deterministic_workspace_bytes(long long n, int K) { return km_det_carve(nullptr, n, K).bytes; }
+
+// det: the centre sums of km_det_block_kernel / km_det_cluster_kernel instead of km_accumulate_kernel; everything else is shared.
+static int km_run(const float* values, long long n, const float* centres_in, int K, float tol, int max_iterations, int* ids, float* centres,
+	char* workspace, bool det, cudaStream_t stream)
 {
 	if (K <= 0 || K > KM_MAX_K) { set_error("kmeans: number of centres must be in 1..%d", KM_MAX_K); return GSB_EINVAL; }
 	ProfScope prof(K_KMEANS, stream);
 	GSB_CUDA_OK(cudaMemcpyAsync(centres, centres_in, sizeof(float) * K, cudaMemcpyDeviceToDevice, stream));
 	if (n <= 0) return GSB_OK;
 	KmWorkspace w = km_carve(workspace, n, K);
+	KmDetWorkspace dw{};
+	if (det) dw = km_det_carve(workspace, n, K);
 	const int grid_ids = (int)std::min<long long>((n + 255) / 256, GSB_NUM_SMS * 8);
 	if (max_iterations > 0)
 	{
@@ -395,6 +555,12 @@ int launch_kmeans(const float* values, long long n, const float* centres_in, int
 		GSB_CUDA_OK(cudaMemsetAsync(w.sums, 0, sizeof(float) * KM_MAX_K, stream));
 		GSB_CUDA_OK(cudaMemsetAsync(w.sizes, 0, sizeof(int) * KM_MAX_K, stream));
 		GSB_CUDA_OK(cudaMemsetAsync(w.state, 0, sizeof(KmState), stream));
+		if (det)
+		{
+			// empty spans (lo > hi); km_det_cluster_kernel restores them after every iteration
+			GSB_CUDA_OK(cudaMemsetAsync(dw.span_lo, 0x7f, sizeof(int) * KM_MAX_K, stream));
+			GSB_CUDA_OK(cudaMemsetAsync(dw.span_hi, 0xff, sizeof(int) * KM_MAX_K, stream));
+		}
 		km_keys_hist_kernel<<<GSB_NUM_SMS * 4, 256, 0, stream>>>(values, n, w.keys0, w.hist);
 		GSB_LAUNCHED();
 		km_sort_plan_kernel<<<1, 256, 0, stream>>>(w.hist, n, w.plan);
@@ -420,7 +586,14 @@ int launch_kmeans(const float* values, long long n, const float* centres_in, int
 			const int batch = std::min(16, max_iterations - launched);
 			for (int i = 0; i < batch; i++)
 			{
-				km_accumulate_kernel<<<grid_acc, 256, 0, stream>>>(sorted, n, centres, K, w.sums, w.sizes, w.state);
+				if (det)
+				{
+					km_det_block_kernel<<<(unsigned)dw.n_blocks, 256, 0, stream>>>(sorted, n, centres, K, w.sizes, dw.parts, dw.part_count,
+						dw.span_lo, dw.span_hi, w.state);
+					GSB_LAUNCHED();
+					km_det_cluster_kernel<<<K, 256, 0, stream>>>(dw.parts, dw.part_count, K, w.sums, dw.span_lo, dw.span_hi, w.state);
+				}
+				else km_accumulate_kernel<<<grid_acc, 256, 0, stream>>>(sorted, n, centres, K, w.sums, w.sizes, w.state);
 				GSB_LAUNCHED();
 				km_update_kernel<<<1, 256, 0, stream>>>(centres, K, w.sums, w.sizes, tol, max_iterations, w.state);
 				GSB_LAUNCHED();
@@ -435,6 +608,18 @@ int launch_kmeans(const float* values, long long n, const float* centres_in, int
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
+}
+
+int launch_kmeans(const float* values, long long n, const float* centres_in, int K, float tol, int max_iterations, int* ids, float* centres,
+	char* workspace, cudaStream_t stream)
+{
+	return km_run(values, n, centres_in, K, tol, max_iterations, ids, centres, workspace, false, stream);
+}
+
+int launch_kmeans_deterministic(const float* values, long long n, const float* centres_in, int K, float tol, int max_iterations, int* ids,
+	float* centres, char* workspace, cudaStream_t stream)
+{
+	return km_run(values, n, centres_in, K, tol, max_iterations, ids, centres, workspace, true, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ pair sort (gsb_knn.cu)

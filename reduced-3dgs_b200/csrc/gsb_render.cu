@@ -61,7 +61,11 @@ __device__ __forceinline__ float2 lds64(uint32_t addr)
 // MAPS = true also composites the inverse-depth map D = sum (1/depth) * alpha * T over the same pairs, with the colour channels'
 // operation sequence, and writes D and the alpha map 1 - final_T.  1/depth (IEEE division) is computed once per staged instance and
 // replaces the depth in the shared-memory copy of the record (r2.z), which the forward reads nowhere else.
-template <bool STATS, bool MAPS>
+#define STATS_FIXED_SCALE 68719476736.0f        // 2^36: one unit of the fixed-point transmittance sums is 2^-36
+// FIXED = true (with STATS) is the deterministic statistics forward (DESIGN.md §5j): `transmittance` then points to 64-bit
+// integers, and each (warp, Gaussian) sum ts is rounded to a multiple of 2^-36 and added with an integer atomic, whose total
+// does not depend on the order of the additions.  stats_fixed_to_float_kernel turns the totals into floats.
+template <bool STATS, bool MAPS, bool FIXED = false>
 __global__ void __launch_bounds__(256, 6) render_forward_kernel(const uint2* __restrict__ ranges,
 	const uint32_t* __restrict__ point_list,
 	int W, int H, const float4* __restrict__ rec, const float* __restrict__ bg,
@@ -146,7 +150,8 @@ __global__ void __launch_bounds__(256, 6) render_forward_kernel(const uint2* __r
 						{
 							const uint32_t gid = s_id[c0 + bit];
 							atomicAdd(&touched_pixels[gid], (int)__popc(cm));
-							atomicAdd(&transmittance[gid], ts);
+							if (FIXED) atomicAdd(reinterpret_cast<unsigned long long*>(transmittance) + gid, __float2ull_rn(ts * STATS_FIXED_SCALE));
+							else atomicAdd(&transmittance[gid], ts);
 						}
 					}
 				}
@@ -577,12 +582,34 @@ __global__ void __launch_bounds__(256, DET ? 3 : 4) render_backward_kernel(const
 }
 
 // ------------------------------------------------------------------------------------------------
+// The fixed-point totals of render_forward_kernel<true, false, true> as floats: one rounding each (the scaling is exact).
+__global__ void __launch_bounds__(256) stats_fixed_to_float_kernel(int P, const unsigned long long* __restrict__ fixed, float* __restrict__ out)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i < P) out[i] = __fmul_rn(__ull2float_rn(fixed[i]), 1.0f / STATS_FIXED_SCALE);
+}
+
+int launch_stats_fixed_to_float(int P, const unsigned long long* fixed, float* out, cudaStream_t stream)
+{
+	if (P <= 0) return GSB_OK;
+	ProfScope prof(K_TOOLS, stream);
+	stats_fixed_to_float_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, fixed, out);
+	GSB_LAUNCHED();
+	GSB_CUDA_OK(cudaGetLastError());
+	return GSB_OK;
+}
+
+// fixed_point: `transmittance` is the 64-bit fixed-point workspace of the deterministic statistics forward.
 int launch_render_forward(const ImageState& img, const BinningState& b, const GeomState& g, int W, int H, const float* bg,
-	float* out_color, int32_t* touched_pixels, float* transmittance, float* out_invdepth, float* out_alpha, cudaStream_t stream)
+	float* out_color, int32_t* touched_pixels, float* transmittance, float* out_invdepth, float* out_alpha, bool fixed_point,
+	cudaStream_t stream)
 {
 	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
 	ProfScope prof(K_RENDER_FWD, stream);
-	if (touched_pixels && transmittance)
+	if (touched_pixels && transmittance && fixed_point)
+		render_forward_kernel<true, false, true><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
+			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, touched_pixels, transmittance, nullptr, nullptr);
+	else if (touched_pixels && transmittance)
 		render_forward_kernel<true, false><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
 			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, touched_pixels, transmittance, nullptr, nullptr);
 	else if (out_invdepth && out_alpha)

@@ -12,7 +12,8 @@ that the 0.3 px^2 dilation no longer inflates sub-pixel splats (gsb_forward_anti
 (forward and backward) takes the model's leaf parameters (features_dc, features_rest, scaling, rotation) in place of sh, scales
 and rotations, and applies exp / F.normalize / the SH concatenation inside the kernels (gsb_forward_raw / gsb_backward_raw).
 `deterministic` (backward) sums the per-Gaussian gradients in a fixed order: the same bytes on every run
-(gsb_backward_deterministic).
+(gsb_backward_deterministic).  `calculate_colours_variance` and `kmeans_cuda` take the same keyword (None: torch's
+deterministic-algorithms flag) for their statistics and centre sums (gsb_forward_statistics_deterministic, gsb_kmeans_deterministic).
 """
 from __future__ import annotations
 
@@ -156,7 +157,8 @@ def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, 
 
 def _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
              tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug, packed_counts=None,
-             prune_mask=None, quant=None, debug_out=None, statistics=None, return_maps=False, antialiasing=False, raw=None):
+             prune_mask=None, quant=None, debug_out=None, statistics=None, return_maps=False, antialiasing=False, raw=None,
+             statistics_workspace=None):
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")          # rasterize_points.cu:158-161
     device = _device_of(means3D)
@@ -195,6 +197,8 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
         stream = _lib.current_stream(device)
         if raw_s is not None:
             st = L.gsb_forward_raw(*head, dbg_ptr, *map_ptrs, C.byref(raw_s), int(bool(antialiasing)), stream)
+        elif statistics is not None and statistics_workspace is not None:
+            st = L.gsb_forward_statistics_deterministic(*head, ptr(statistics[0]), ptr(statistics[1]), statistics_workspace.data_ptr(), stream)
         elif statistics is not None:                             # (touched_pixels int32 [P,1], transmittance_sum f32 [P,1]) to fill
             st = L.gsb_forward_statistics(*head, ptr(statistics[0]), ptr(statistics[1]), stream)
         elif antialiasing or maps is not None:
@@ -330,11 +334,14 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
 
 
 def calculate_colours_variance(cam_positions, means3D, opacity, scales, rotations, cam_viewmatrices, cam_projmatrices, tan_fovxs,
-                               tan_fovys, image_height, image_width, sh, degrees, max_sh_deg):
+                               tan_fovys, image_height, image_width, sh, degrees, max_sh_deg, *, deterministic=None):
     """reduced_3dgs.h:28-43 Reduced3DGS::calculateColourVariance (reduced_3dgs.cu:41-203) ->
     (average colour distance to each lower SH truncation [P, max_sh_deg], weighted colour variance [P,1,3], weighted mean colour [P,1,3]).
     Per camera: one forward with the visibility statistics on (gsb_forward_statistics) + one fused statistics kernel
-    (gsb_sh_statistics_update) in place of the reference's ~30 ATen ops; the camera parameters are read back once, not per camera."""
+    (gsb_sh_statistics_update) in place of the reference's ~30 ATen ops; the camera parameters are read back once, not per camera.
+    `deterministic`: sum the transmittances in 64-bit fixed point (gsb_forward_statistics_deterministic), the same bytes on every
+    run; None follows torch.are_deterministic_algorithms_enabled() at the call, an explicit bool wins."""
+    det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")          # reduced_3dgs.cu:57-60
     device = _device_of(means3D)
@@ -360,9 +367,13 @@ def calculate_colours_variance(cam_positions, means3D, opacity, scales, rotation
     touched = torch.empty((P, 1), dtype=torch.int32, device=device)
     tsum = torch.empty((P, 1), dtype=torch.float32, device=device)
     stream = _lib.current_stream(device)
+    det_kw = {}
+    if det:
+        # one fixed-point workspace for all cameras (each forward clears it)
+        det_kw["statistics_workspace"] = torch.empty(int(L.gsb_statistics_workspace_bytes(P)), dtype=torch.uint8, device=device)
     for i in range(n_cams):
         _, _, radii, _, _, _ = _forward(bg, means3D, empty, opacity, scales, rotations, 1.0, empty, views[i], projs[i], txs[i], tys[i],
-                                        Hs[i], Ws[i], sh, deg, cam_positions[i], False, False, statistics=(touched, tsum))
+                                        Hs[i], Ws[i], sh, deg, cam_positions[i], False, False, statistics=(touched, tsum), **det_kw)
         with on_device(device):
             _lib.check(L.gsb_sh_statistics_update(P, M, ptr(deg), ptr(means3D), cam_positions[i].data_ptr(), ptr(sh), ptr(radii), ptr(touched),
                                                   ptr(tsum), ptr(wsum), ptr(wsumsq), ptr(dist), ptr(mean), ptr(var), stream))
@@ -417,9 +428,12 @@ def allocate_minimum_redundancy_value(redundancy_values, neighbours_indices, int
     return (out,)
 
 
-def kmeans_cuda(values, centers, tol, max_iterations):
+def kmeans_cuda(values, centers, tol, max_iterations, *, deterministic=None):
     """reduced_3dgs.h:21-26 Reduced3DGS::kmeans (reduced_3dgs.cu:289-338) -> (ids int32 [n,1], centers float32 [k]).
-    `values` is the [n,1] column of one attribute, `centers` the [k] initial centres (gaussian_model.py:36-41)."""
+    `values` is the [n,1] column of one attribute, `centers` the [k] initial centres (gaussian_model.py:36-41).
+    `deterministic`: add each cluster's values in an order fixed by the input (gsb_kmeans_deterministic), the same centres and ids
+    on every run; None follows torch.are_deterministic_algorithms_enabled() at the call, an explicit bool wins."""
+    det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
     device = _device_of(values)
     L = _lib.lib()
     v = f32(values, device)
@@ -427,10 +441,12 @@ def kmeans_cuda(values, centers, tol, max_iterations):
     n, k = int(values.size(0)), int(centers.size(0))
     ids = torch.zeros((n, 1), dtype=torch.int32, device=device)
     out = torch.empty((k,), dtype=torch.float32, device=device)
+    ws_bytes, run = ((L.gsb_kmeans_deterministic_workspace_bytes, L.gsb_kmeans_deterministic) if det else
+                     (L.gsb_kmeans_workspace_bytes, L.gsb_kmeans))
     with on_device(device):
-        ws = torch.empty(int(L.gsb_kmeans_workspace_bytes(n, k)), dtype=torch.uint8, device=device)
-        _lib.check(L.gsb_kmeans(ptr(v.reshape(-1)) if n else None, n, ptr(c.reshape(-1)), k, float(tol), int(max_iterations),
-                                ptr(ids), out.data_ptr(), ws.data_ptr(), _lib.current_stream(device)))
+        ws = torch.empty(int(ws_bytes(n, k)), dtype=torch.uint8, device=device)
+        _lib.check(run(ptr(v.reshape(-1)) if n else None, n, ptr(c.reshape(-1)), k, float(tol), int(max_iterations),
+                       ptr(ids), out.data_ptr(), ws.data_ptr(), _lib.current_stream(device)))
     return ids, out
 
 

@@ -133,6 +133,10 @@ def lib():
         L.gsb_forward_statistics.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p,
                                              ALLOC_FN, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
                                              C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gsb_statistics_workspace_bytes.restype = C.c_size_t
+        L.gsb_statistics_workspace_bytes.argtypes = [C.c_int32]
+        L.gsb_forward_statistics_deterministic.restype = C.c_int
+        L.gsb_forward_statistics_deterministic.argtypes = L.gsb_forward_statistics.argtypes[:-1] + [C.c_void_p, C.c_void_p]
         L.gsb_sh_statistics_update.restype = C.c_int
         L.gsb_sh_statistics_update.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 13
         L.gsb_min_projected_pixel_size.restype = C.c_int
@@ -148,6 +152,10 @@ def lib():
         L.gsb_kmeans.restype = C.c_int
         L.gsb_kmeans.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
+        L.gsb_kmeans_deterministic_workspace_bytes.restype = C.c_size_t
+        L.gsb_kmeans_deterministic_workspace_bytes.argtypes = [C.c_int64, C.c_int32]
+        L.gsb_kmeans_deterministic.restype = C.c_int
+        L.gsb_kmeans_deterministic.argtypes = L.gsb_kmeans.argtypes
         L.gsb_knn_workspace_bytes.restype = C.c_size_t
         L.gsb_knn_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
         L.gsb_knn.restype = C.c_int
@@ -240,7 +248,9 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_forward_maps", "gsb_backward_maps", "gsb_camera_grad_workspace_bytes", "gsb_backward_camera",
                     "gsb_forward_antialiased", "gsb_backward_antialiased", "gsb_adam_step", "gsb_densify_stats",
                     "gsb_densify_workspace_bytes", "gsb_densify_split_std_offset", "gsb_densify_plan", "gsb_densify_emit",
-                    "gsb_forward_raw", "gsb_backward_raw", "gsb_deterministic_workspace_bytes", "gsb_backward_deterministic"]
+                    "gsb_forward_raw", "gsb_backward_raw", "gsb_deterministic_workspace_bytes", "gsb_backward_deterministic",
+                    "gsb_statistics_workspace_bytes", "gsb_forward_statistics_deterministic",
+                    "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic"]
 
 
 def check(status: int):
