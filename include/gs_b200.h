@@ -521,6 +521,55 @@ GSB_API int gsb_densify_emit(const GsbDensifyTensor* tensors, int32_t n, int32_t
                 int64_t n_clones_kept, int64_t n_split, int64_t n_children_kept, const float* rotation, const float* samples,
                 float split_scale_factor, void* stream);
 
+/* ---- resolution-aware redundancy pruning (gs_b200.densify.calculate_redundancy_metric / mercy_points, DESIGN.md §5k) ----
+ *
+ * gsb_redundancy_score: the reference's Scene.calculate_redundancy_metric (scene/__init__.py:142-174) in one call, fully
+ * asynchronous on `stream`:
+ *   pixel_sizes[i]   = gsb_min_projected_pixel_size of centre i (the reference's cube_size);
+ *   radius[i]        = ((pixel_sizes[i] * pixel_scale) * sqrt(3)) / 2 in fp32;
+ *   the K nearest neighbours of each centre (gsb_knn, indices only);
+ *   red[i]           = 1 + the number of neighbours n (index >= 0) whose ellipsoid, scales grown by radius[i] and rotated by
+ *                      Gaussian i's own rotation (the reference's quirk), contains centre i;
+ *   min_redundancy[j] = min(P, red[j], min over the i that hit j of red[i]).
+ * scales / rotations are the activated values (exp(scaling), normalised quaternions).  Missing neighbours (P <= K) are neither
+ * tested nor counted.  The result is deterministic (integer minima).  workspace: gsb_redundancy_workspace_bytes(P, K) bytes.
+ * Errors (GSB_EINVAL, nothing launched): P < 0 or P >= 2^30, K outside 1..GSB_KNN_MAX_K, n_cameras < 0 or > 1024, and with
+ * P > 0 a NULL pointer (the camera arrays only when n_cameras > 0). */
+GSB_API size_t gsb_redundancy_workspace_bytes(int32_t P, int32_t K);
+GSB_API int gsb_redundancy_score(int32_t P, const float* means3D, const float* scales, const float* rotations, int32_t n_cameras,
+                const float* w2ndc, const float* w2ndc_inverse, const int32_t* image_heights, const int32_t* image_widths,
+                float pixel_scale, int32_t K, int32_t* min_redundancy /* [P] */, float* pixel_sizes /* [P] */, void* workspace,
+                void* stream);
+
+/* gsb_mercy_plan: the statistics and the prune mask of the reference's GaussianModel.mercy_points (gaussian_model.py:524-551),
+ * asynchronous on `stream`.  counts: int32 [P] (the redundancy score); opacity_logits: fp32 [P] (sigmoid is applied here).
+ *   thresholds[0] = mean + lambda_mercy * std of the counts (mean and unbiased variance formed in fp64 from exact integer sums,
+ *                   each rounded to fp32, then fp32 ops; exact while sum(c^2) < 2^63);
+ *   a row is redundant if (float)count > fp32(max(thresholds[0], mercy_minimum)) (Python's max: a NaN threshold stays NaN);
+ *   mask[i] (u8) per type:
+ *     GSB_MERCY_REDUNDANCY_OPACITY          redundant and opacity < the lower median of the redundant rows' opacities
+ *     GSB_MERCY_REDUNDANCY_RANDOM           redundant and draws[j] < 0.5, j = the row's rank among the redundant rows
+ *     GSB_MERCY_OPACITY                     opacity < torch.quantile(opacity, quantile_q)
+ *     GSB_MERCY_REDUNDANCY_OPACITY_OPACITY  the first type, or opacity < min(torch.quantile(opacity, quantile_q), 0.05)
+ *     GSB_MERCY_REDUNDANCY                  redundant (the reference's branch for any other type string)
+ *   thresholds[1] = the opacity threshold of the two quantile types (NaN if an opacity is NaN), else 0;
+ *   counts_out[0] = redundant rows, counts_out[1] = masked rows (int64, device).
+ * The median is NaN (nothing pruned by it) with no redundant row or a NaN among them.  The quantile has no size limit.
+ * The random type is two calls: without draws it writes thresholds and counts_out[0] only; the caller draws counts_out[0]
+ * uniforms and calls again with them (n_draws = their number).  workspace: gsb_mercy_workspace_bytes(P) bytes.
+ * Errors (GSB_EINVAL, nothing launched): P < 0 or P >= 2^30, an unknown type, NULL workspace / thresholds / counts_out,
+ * draws for another type or with n_draws < 0, and with P > 0 NULL counts / mask, or NULL opacity_logits for a type that reads
+ * them. */
+#define GSB_MERCY_REDUNDANCY_OPACITY 0
+#define GSB_MERCY_REDUNDANCY_RANDOM 1
+#define GSB_MERCY_OPACITY 2
+#define GSB_MERCY_REDUNDANCY_OPACITY_OPACITY 3
+#define GSB_MERCY_REDUNDANCY 4
+GSB_API size_t gsb_mercy_workspace_bytes(int32_t P);
+GSB_API int gsb_mercy_plan(int32_t P, const int32_t* counts, const float* opacity_logits, int32_t type, float lambda_mercy,
+                double mercy_minimum, float quantile_q, const float* draws, int64_t n_draws, void* workspace, uint8_t* mask,
+                float* thresholds /* [2] */, int64_t* counts_out /* [2] */, void* stream);
+
 /* Number of kernels this library has launched since load (bench.py reports it as gpu_launches). */
 GSB_API uint64_t gsb_launch_count(void);
 

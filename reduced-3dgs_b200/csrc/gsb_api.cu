@@ -110,6 +110,7 @@ int launch_sh_stats_update(int, int, const int*, const float*, const float*, con
 int launch_pixel_size(int, const float*, int, const float*, const float*, const int*, const int*, float*, cudaStream_t);
 int launch_sphere_ellipsoid(int, const float*, const float*, const float*, const int*, const float*, int, int*, uint8_t*, cudaStream_t);
 int launch_min_redundancy(int, const int*, const int*, const uint8_t*, int, int*, cudaStream_t);
+int launch_redundancy_fused(int, const float*, const float*, const float*, const int*, const float*, float, int, int*, cudaStream_t);
 int launch_l1_ssim_forward(const float*, const float*, int, int, int, float*, float*, cudaStream_t);
 int launch_l1_ssim_backward(const float*, const float*, int, int, int, const float*, float, const float*, float, const float*, float*, cudaStream_t);
 size_t kmeans_workspace_bytes(long long, int);
@@ -675,6 +676,34 @@ int gsb_export_image(const char* image_blob, int32_t W, int32_t H, float* final_
 	if (n_contrib) GSB_CUDA_OK(cudaMemcpyAsync(n_contrib, img.n_contrib, N * 4, cudaMemcpyDeviceToDevice, stream));
 	if (ranges) GSB_CUDA_OK(cudaMemcpyAsync(ranges, img.ranges, T * 8, cudaMemcpyDeviceToDevice, stream));
 	return GSB_OK;
+}
+
+// [P, K] int32 neighbour indices, then the kNN's own workspace
+static size_t redundancy_knn_offset(int P, int K) { return ((size_t)P * K * sizeof(int32_t) + 255) & ~size_t(255); }
+
+size_t gsb_redundancy_workspace_bytes(int32_t P, int32_t K)
+{
+	const int p = P < 0 ? 0 : P, k = K < 0 ? 0 : K;
+	return redundancy_knn_offset(p, k) + knn_workspace_bytes(p, -1);
+}
+
+int gsb_redundancy_score(int32_t P, const float* means3D, const float* scales, const float* rotations, int32_t n_cameras,
+	const float* w2ndc, const float* w2ndc_inverse, const int32_t* image_heights, const int32_t* image_widths, float pixel_scale,
+	int32_t K, int32_t* min_redundancy, float* pixel_sizes, void* workspace, void* stream)
+{
+	if (P < 0 || P >= (1 << 30)) { set_error("redundancy_score: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
+	if (K < 1 || K > GSB_KNN_MAX_K) { set_error("redundancy_score: K = %d is outside 1..%d", K, GSB_KNN_MAX_K); return GSB_EINVAL; }
+	if (n_cameras < 0 || n_cameras > 1024) { set_error("redundancy_score: n_cameras = %d is outside 0..1024", n_cameras); return GSB_EINVAL; }
+	if (P == 0) return GSB_OK;
+	if (!means3D || !scales || !rotations || !min_redundancy || !pixel_sizes || !workspace ||
+		(n_cameras > 0 && (!w2ndc || !w2ndc_inverse || !image_heights || !image_widths)))
+	{ set_error("redundancy_score: NULL argument"); return GSB_EINVAL; }
+	const cudaStream_t st = (cudaStream_t)stream;
+	int32_t* nb = static_cast<int32_t*>(workspace);
+	char* knn_ws = static_cast<char*>(workspace) + redundancy_knn_offset(P, K);
+	if (int e = launch_pixel_size(P, means3D, n_cameras, w2ndc, w2ndc_inverse, image_heights, image_widths, pixel_sizes, st)) return e;
+	if (int e = launch_knn(means3D, P, K, nullptr, P, nullptr, -1, nullptr, nullptr, nb, knn_ws, st)) return e;
+	return launch_redundancy_fused(P, means3D, scales, rotations, nb, pixel_sizes, pixel_scale, K, min_redundancy, st);
 }
 
 } // extern "C"

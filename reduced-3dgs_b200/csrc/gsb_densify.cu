@@ -54,8 +54,6 @@ struct PlanArgs {
 	int P, mode, screen_test;
 };
 
-// torch.sigmoid on CUDA: 1 / (1 + exp(-x)), IEEE division
-__device__ __forceinline__ float sigmoid_torch(float x) { return __fdiv_rn(1.0f, __fadd_rn(1.0f, exp_ref(-x))); }
 // torch.max(t, dim=1).values of a row: NaN if any element is NaN
 __device__ __forceinline__ float max3_torch(float a, float b, float c)
 {

@@ -203,41 +203,59 @@ int launch_pixel_size(int P, const float* means3D, int n_cams, const float* w2nd
 // Sphere / ellipsoid intersection against the k nearest neighbours (redundancy_score.cu:119-160 + buildRotationMatrixCUDA
 // :186-205, fused: the 3x3 rotation is rebuilt from the quaternion in registers instead of a [P,3,3] tensor round trip).
 // Reference quirk kept: the rotation used for neighbour i is the CURRENT Gaussian's (`R[idx]`, :143), not the neighbour's.
-// One warp handles 32 Gaussians; the neighbour list rows are read with coalesced loads (lane = neighbour slot).
+// The centre, radius and rotation of one Gaussian, and the test of one neighbour against them; sphere_ellipsoid_kernel and
+// redundancy_fused_kernel share them.
+struct SphereProbe { float cx, cy, cz, rad, m00, m01, m02, m10, m11, m12, m20, m21, m22; };
+// The loads are issued in the order centre, radius, rotation (the caller sets s.rad between the two calls).
+__device__ __forceinline__ void sphere_centre(SphereProbe& s, const float* __restrict__ means3D, int idx)
+{
+	s.cx = means3D[3 * idx]; s.cy = means3D[3 * idx + 1]; s.cz = means3D[3 * idx + 2];
+}
+__device__ __forceinline__ void sphere_rotation(SphereProbe& s, const float* __restrict__ rotations, int idx)
+{
+	const float4 q = reinterpret_cast<const float4*>(rotations)[idx];
+	const float r = q.x, x = q.y, y = q.z, z = q.w;
+	// column-major mat3(c0 | c1 | c2) of redundancy_score.cu:201-204, in the operation order of the reference build (its SASS)
+	const float rz = __fmul_rn(r, z), ry = __fmul_rn(r, y), yz = __fmul_rn(y, z), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
+	s.m00 = __fsub_rn(1.f, __fmul_rn(2.f, __fadd_rn(yy, zz)));
+	s.m01 = __fmul_rn(2.f, __fmaf_rn(x, y, rz)); s.m02 = __fmul_rn(2.f, __fmaf_rn(x, z, -ry));
+	s.m10 = __fmul_rn(2.f, __fmaf_rn(x, y, -rz)); s.m11 = __fsub_rn(1.f, __fmul_rn(2.f, __fmaf_rn(x, x, zz)));
+	s.m12 = __fmul_rn(2.f, __fmaf_rn(r, x, yz));
+	s.m20 = __fmul_rn(2.f, __fmaf_rn(x, z, ry)); s.m21 = __fmul_rn(2.f, __fmaf_rn(-r, x, yz));
+	s.m22 = __fsub_rn(1.f, __fmul_rn(2.f, __fmaf_rn(x, x, yy)));
+}
+// true if the centre lies inside neighbour n's ellipsoid with its scales grown by the sphere radius
+__device__ __forceinline__ bool sphere_hits(const SphereProbe& s, const float* __restrict__ means3D, const float* __restrict__ scales, int n)
+{
+	const float dx = __fsub_rn(s.cx, means3D[3 * n]), dy = __fsub_rn(s.cy, means3D[3 * n + 1]), dz = __fsub_rn(s.cz, means3D[3 * n + 2]);
+	const float sx = __fadd_rn(scales[3 * n], s.rad), sy = __fadd_rn(scales[3 * n + 1], s.rad), sz = __fadd_rn(scales[3 * n + 2], s.rad);
+	// row vector times matrix: component c = dot(column c, d), contracted as fma(d.z, m2, fma(d.x, m0, d.y*m1))
+	const float lx = __fmaf_rn(dz, s.m02, __fmaf_rn(dx, s.m00, __fmul_rn(dy, s.m01)));
+	const float ly = __fmaf_rn(dz, s.m12, __fmaf_rn(dx, s.m10, __fmul_rn(dy, s.m11)));
+	const float lz = __fmaf_rn(dz, s.m22, __fmaf_rn(dx, s.m20, __fmul_rn(dy, s.m21)));
+	// glm::pow(v, vec3(2)) is the full powf (the reference build does not reduce it to a product)
+	const float bx = __frcp_rn(powf(sx, 2.0f)), by = __frcp_rn(powf(sy, 2.0f)), bz = __frcp_rn(powf(sz, 2.0f));
+	const float dot = __fmaf_rn(bz, powf(lz, 2.0f), __fmaf_rn(bx, powf(lx, 2.0f), __fmul_rn(by, powf(ly, 2.0f))));
+	return dot < 1.0f;
+}
+
+// One thread per Gaussian; the neighbour list row is [knn] int32.
 __global__ void __launch_bounds__(256) sphere_ellipsoid_kernel(int P, const float* __restrict__ means3D, const float* __restrict__ scales,
 	const float* __restrict__ rotations, const int* __restrict__ neighbours, const float* __restrict__ sphere_radius, int knn,
 	int* __restrict__ redundancy_values, uint8_t* __restrict__ intersection_mask)
 {
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if (idx >= P) return;
-	const float cx = means3D[3 * idx], cy = means3D[3 * idx + 1], cz = means3D[3 * idx + 2];
-	const float rad = sphere_radius[idx];
-	const float4 q = reinterpret_cast<const float4*>(rotations)[idx];
-	const float r = q.x, x = q.y, y = q.z, z = q.w;
-	// column-major mat3(c0 | c1 | c2) of redundancy_score.cu:201-204, in the operation order of the reference build (its SASS)
-	const float rz = __fmul_rn(r, z), ry = __fmul_rn(r, y), yz = __fmul_rn(y, z), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
-	const float m00 = __fsub_rn(1.f, __fmul_rn(2.f, __fadd_rn(yy, zz)));
-	const float m01 = __fmul_rn(2.f, __fmaf_rn(x, y, rz)), m02 = __fmul_rn(2.f, __fmaf_rn(x, z, -ry));
-	const float m10 = __fmul_rn(2.f, __fmaf_rn(x, y, -rz)), m11 = __fsub_rn(1.f, __fmul_rn(2.f, __fmaf_rn(x, x, zz)));
-	const float m12 = __fmul_rn(2.f, __fmaf_rn(r, x, yz));
-	const float m20 = __fmul_rn(2.f, __fmaf_rn(x, z, ry)), m21 = __fmul_rn(2.f, __fmaf_rn(-r, x, yz));
-	const float m22 = __fsub_rn(1.f, __fmul_rn(2.f, __fmaf_rn(x, x, yy)));
+	SphereProbe s;
+	sphere_centre(s, means3D, idx);
+	s.rad = sphere_radius[idx];
+	sphere_rotation(s, rotations, idx);
 	const int* nb = neighbours + (size_t)idx * knn;
 	uint8_t* mk = intersection_mask + (size_t)idx * knn;
 	int count = 0;
 	for (int i = 0; i < knn; i++)
 	{
-		const int n = nb[i];
-		const float dx = __fsub_rn(cx, means3D[3 * n]), dy = __fsub_rn(cy, means3D[3 * n + 1]), dz = __fsub_rn(cz, means3D[3 * n + 2]);
-		const float sx = __fadd_rn(scales[3 * n], rad), sy = __fadd_rn(scales[3 * n + 1], rad), sz = __fadd_rn(scales[3 * n + 2], rad);
-		// row vector times matrix: component c = dot(column c, d), contracted as fma(d.z, m2, fma(d.x, m0, d.y*m1))
-		const float lx = __fmaf_rn(dz, m02, __fmaf_rn(dx, m00, __fmul_rn(dy, m01)));
-		const float ly = __fmaf_rn(dz, m12, __fmaf_rn(dx, m10, __fmul_rn(dy, m11)));
-		const float lz = __fmaf_rn(dz, m22, __fmaf_rn(dx, m20, __fmul_rn(dy, m21)));
-		// glm::pow(v, vec3(2)) is the full powf (the reference build does not reduce it to a product)
-		const float bx = __frcp_rn(powf(sx, 2.0f)), by = __frcp_rn(powf(sy, 2.0f)), bz = __frcp_rn(powf(sz, 2.0f));
-		const float dot = __fmaf_rn(bz, powf(lz, 2.0f), __fmaf_rn(bx, powf(lx, 2.0f), __fmul_rn(by, powf(ly, 2.0f))));
-		const bool hit = dot < 1.0f;
+		const bool hit = sphere_hits(s, means3D, scales, nb[i]);
 		mk[i] = hit ? 1 : 0;
 		count += hit ? 1 : 0;
 	}
@@ -285,6 +303,55 @@ int launch_min_redundancy(int P, const int* redundancy_values, const int* neighb
 		min_redundancy_kernel<<<(unsigned)((E + 255) / 256), 256, 0, stream>>>(P, redundancy_values, neighbours, intersection_mask, knn, minimum);
 		GSB_LAUNCHED();
 	}
+	GSB_CUDA_OK(cudaGetLastError());
+	return GSB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// The whole of Scene.calculate_redundancy_metric after the kNN (scene/__init__.py:153-173) in one pass, one thread per Gaussian i:
+//   radius  = ((cube_size[i] * pixel_scale) * sqrt(3)) / 2        torch's fp32 order (division by 2 is exact)
+//   hits    = the neighbours k whose grown ellipsoid contains centre i (sphere_hits); slots holding -1 (missing) are skipped
+//   red_i   = |hits| + 1                                           the "+1" for the Gaussian itself
+//   minimum[i]   = min(minimum[i], red_i)                          the self column the reference concatenates
+//   minimum[n_k] = min(minimum[n_k], red_i) for each hit k         allocate_minimum_redundancy_value
+// `minimum` is filled with P before.  Integer minima do not depend on the order, so the result is deterministic.  The hit bits
+// stay in a register: no [P, K] mask and no [P, K + 1] copies.
+__global__ void __launch_bounds__(256) redundancy_fused_kernel(int P, const float* __restrict__ means3D, const float* __restrict__ scales,
+	const float* __restrict__ rotations, const int* __restrict__ neighbours, const float* __restrict__ cube_size, float pixel_scale, int knn,
+	int* __restrict__ minimum)
+{
+	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= P) return;
+	SphereProbe s;
+	sphere_centre(s, means3D, idx);
+	s.rad = __fdiv_rn(__fmul_rn(__fmul_rn(cube_size[idx], pixel_scale), __fsqrt_rn(3.0f)), 2.0f);
+	sphere_rotation(s, rotations, idx);
+	const int* nb = neighbours + (size_t)idx * knn;
+	unsigned long long hits = 0;
+	for (int i = 0; i < knn; i++)
+	{
+		const int n = nb[i];
+		if (n >= 0 && sphere_hits(s, means3D, scales, n)) hits |= 1ull << i;
+	}
+	const int red = __popcll(hits) + 1;
+	atomicMin(&minimum[idx], red);
+	while (hits)
+	{
+		const int i = __ffsll((long long)hits) - 1;
+		hits &= hits - 1;
+		atomicMin(&minimum[nb[i]], red);
+	}
+}
+
+int launch_redundancy_fused(int P, const float* means3D, const float* scales, const float* rotations, const int* neighbours,
+	const float* cube_size, float pixel_scale, int knn, int* minimum, cudaStream_t stream)
+{
+	if (P <= 0) return GSB_OK;
+	ProfScope prof(K_TOOLS, stream);
+	fill_int_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, P, minimum);
+	GSB_LAUNCHED();
+	redundancy_fused_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, means3D, scales, rotations, neighbours, cube_size, pixel_scale, knn, minimum);
+	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
 }

@@ -1,11 +1,14 @@
 """Native densification: the reference's GaussianModel.densify_and_prune / prune / prune_points / add_densification_stats
-(scene/gaussian_model.py:553-695) on the model and its optimizer state, row for row (DESIGN.md §5g).
+(scene/gaussian_model.py:553-695) on the model and its optimizer state, row for row (DESIGN.md §5g), and its resolution-aware
+redundancy pruning, Scene.calculate_redundancy_metric + GaussianModel.mercy_points (DESIGN.md §5k).
 
     from gs_b200 import densify
     GaussianModel.densify_and_prune = densify.densify_and_prune      # INTEGRATION.md section D
     GaussianModel.prune = densify.prune
     GaussianModel.prune_points = densify.prune_points
     GaussianModel.add_densification_stats = densify.add_densification_stats
+    GaussianModel.mercy_points = densify.mercy_points
+    Scene.calculate_redundancy_metric = densify.calculate_redundancy_metric
 
 The signatures are the reference's methods with `self` -> `model`.  The results are the reference's: the same rows in the same
 order ([kept originals][kept clones][kept first children][kept second children]), the same values, the same optimizer state
@@ -112,6 +115,85 @@ def prune_points(model, mask, store_grads=False):
         raise RuntimeError(f"densify: the prune mask must be a bool tensor [{P}] on {dev}")
     counts, ws, _ = _plan(model, groups, P, dev, gsl.DENSIFY_PRUNE_MASK, mask=mask.contiguous())
     _emit(model, groups, P, dev, ws, counts, store_grads, gather_stats=True)
+
+
+MERCY_TYPES = (("redundancy_opacity", gsl.MERCY_REDUNDANCY_OPACITY), ("redundancy_random", gsl.MERCY_REDUNDANCY_RANDOM),
+               ("opacity", gsl.MERCY_OPACITY), ("redundancy_opacity_opacity", gsl.MERCY_REDUNDANCY_OPACITY_OPACITY))
+MERCY_QUANTILE = {gsl.MERCY_OPACITY: 0.045, gsl.MERCY_REDUNDANCY_OPACITY_OPACITY: 0.03}
+
+
+def calculate_redundancy_metric(scene, pixel_scale=1.0, num_neighbours=30):
+    """The reference's Scene.calculate_redundancy_metric -> (min_redundancy int32 [P, 1], cube_size fp32 [P, 1]): the pixel
+    size, the kNN, the intersection test and the minimum in one native call with no host synchronisation and no [P, K] mask
+    or [P, K + 1] copies.  Missing neighbours (P <= num_neighbours) are not counted.  1 <= num_neighbours <= 64."""
+    cams = scene.getTrainCameras()
+    g = scene.gaussians
+    xyz = g._xyz
+    if not torch.is_tensor(xyz) or not xyz.is_cuda or xyz.dtype != torch.float32 or xyz.dim() != 2 or xyz.shape[1] != 3:
+        raise RuntimeError("densify: the model's _xyz must be an fp32 CUDA tensor [P, 3]")
+    dev, P = xyz.device, xyz.shape[0]
+    K = int(num_neighbours)
+    f32 = lambda t: t.detach().to(device=dev, dtype=torch.float32).contiguous()  # noqa: E731
+    xyz, scales, rots = f32(xyz), f32(g.get_scaling), f32(g.get_rotation)
+    if tuple(scales.shape) != (P, 3) or tuple(rots.shape) != (P, 4):
+        raise RuntimeError(f"densify: get_scaling / get_rotation must be [{P}, 3] / [{P}, 4]")
+    n = len(cams)
+    if n:
+        w2ndc = f32(torch.stack([c.full_proj_transform for c in cams], dim=0))
+        inv = f32(torch.stack([c.inverse_full_proj_transform for c in cams], dim=0))
+        if tuple(w2ndc.shape) != (n, 4, 4) or tuple(inv.shape) != (n, 4, 4):
+            raise RuntimeError("densify: the cameras' full_proj_transform / inverse_full_proj_transform must be 4 x 4")
+    else:
+        w2ndc = inv = None
+    heights = torch.tensor([c.image_height for c in cams], device=dev, dtype=torch.int32)
+    widths = torch.tensor([c.image_width for c in cams], device=dev, dtype=torch.int32)
+    L = gsl.lib()
+    red = torch.empty((P, 1), dtype=torch.int32, device=dev)
+    cube = torch.empty((P, 1), dtype=torch.float32, device=dev)
+    ws = torch.empty(L.gsb_redundancy_workspace_bytes(P, K) if 1 <= K <= 64 else 0, dtype=torch.uint8, device=dev)  # else refused
+    ptr = lambda t: None if t is None or t.numel() == 0 else t.data_ptr()  # noqa: E731
+    with gsl.on_device(dev):
+        gsl.check(L.gsb_redundancy_score(P, ptr(xyz), ptr(scales), ptr(rots), n, ptr(w2ndc), ptr(inv), ptr(heights),
+                                         ptr(widths), float(pixel_scale), K, ptr(red), ptr(cube), ptr(ws), gsl.current_stream(dev)))
+    return red, cube
+
+
+def mercy_points(model, densification_statistics_dict, lambda_mercy=2, mercy_minimum=2, mercy_type='redundancy_opacity'):
+    """The reference's mercy_points: threshold the redundancy counts in model._splatted_num_accum (int32 [P, 1, 1], [P, 1] or
+    [P]) at max(mean + lambda_mercy * std, mercy_minimum), choose the rows to prune by mercy_type and prune them with
+    prune_points' plan and emit.  The statistics dictionary gets the reference's types and shapes.  One host read-back (the
+    prune's counts); 'redundancy_random' has a second one, the number of uniforms to draw."""
+    groups, P, dev = _validate(model, False)
+    c = getattr(model, "_splatted_num_accum", None)
+    if (not torch.is_tensor(c) or c.dtype != torch.int32 or c.device != dev or not c.is_contiguous()
+            or tuple(c.shape) not in ((P, 1, 1), (P, 1), (P,))):
+        raise RuntimeError(f"densify: _splatted_num_accum must be a contiguous int32 tensor [{P}, 1, 1], [{P}, 1] or [{P}] on {dev}")
+    code = next((v for k, v in MERCY_TYPES if mercy_type == k), gsl.MERCY_REDUNDANCY)
+    q = MERCY_QUANTILE.get(code, 0.0)
+    logits = next(p for name, _, p, _ in groups if name == "opacity")
+    L = gsl.lib()
+    ws = torch.empty(L.gsb_mercy_workspace_bytes(P), dtype=torch.uint8, device=dev)
+    mask = torch.empty(P, dtype=torch.uint8, device=dev)
+    thr = torch.empty(2, dtype=torch.float32, device=dev)
+    cnt = torch.empty(2, dtype=torch.int64, device=dev)
+
+    def plan(draws=None, n_draws=-1):
+        with gsl.on_device(dev):
+            gsl.check(L.gsb_mercy_plan(P, c.data_ptr(), logits.data_ptr(), code, lambda_mercy, mercy_minimum, q,
+                                       None if draws is None else draws.data_ptr(), n_draws, ws.data_ptr(), mask.data_ptr(),
+                                       thr.data_ptr(), cnt.data_ptr(), gsl.current_stream(dev)))
+    plan()
+    if code == gsl.MERCY_REDUNDANCY_RANDOM:
+        # the reference's torch.rand(mask[mask].shape): one draw per redundant row, also when there is none
+        draws = torch.rand((int(cnt[0]),), device=dev)
+        plan(draws if draws.numel() else torch.zeros(1, device=dev), draws.numel())
+    counts, pws, _ = _plan(model, groups, P, dev, gsl.DENSIFY_PRUNE_MASK, mask=mask)
+    _emit(model, groups, P, dev, pws, counts, False, gather_stats=True)
+    densification_statistics_dict["n_points_mercied"] = cnt[1].clone()
+    # the reference's mean of squeeze(): [1], or 0-dim for a single row
+    densification_statistics_dict["redundancy_threshold"] = thr[0].clone() if P == 1 else thr[0:1].clone()
+    densification_statistics_dict["opacity_threshold"] = (thr[1].clone() if code == gsl.MERCY_OPACITY else thr[1:2].clone()
+                                                          if code == gsl.MERCY_REDUNDANCY_OPACITY_OPACITY else 0)
 
 
 # ------------------------------------------------------------------------------------------------ internals

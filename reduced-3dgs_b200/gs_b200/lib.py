@@ -80,6 +80,7 @@ DENSIFY_MAX_TENSORS = 16       # GSB_DENSIFY_MAX_TENSORS
 DENSIFY_COUNTS = 8             # GSB_DENSIFY_COUNTS
 DENSIFY_CLONE_SPLIT, DENSIFY_PRUNE, DENSIFY_PRUNE_MASK = 0, 1, 2
 DENSIFY_COPY, DENSIFY_XYZ, DENSIFY_SCALING = 0, 1, 2
+MERCY_REDUNDANCY_OPACITY, MERCY_REDUNDANCY_RANDOM, MERCY_OPACITY, MERCY_REDUNDANCY_OPACITY_OPACITY, MERCY_REDUNDANCY = 0, 1, 2, 3, 4
 
 
 _lib = None
@@ -217,6 +218,16 @@ def lib():
         L.gsb_densify_emit.restype = C.c_int
         L.gsb_densify_emit.argtypes = [C.POINTER(GsbDensifyTensor), C.c_int32, C.c_int32, C.c_void_p] + [C.c_int64] * 4 + \
             [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
+        L.gsb_redundancy_workspace_bytes.restype = C.c_size_t
+        L.gsb_redundancy_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
+        L.gsb_redundancy_score.restype = C.c_int
+        L.gsb_redundancy_score.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gsb_mercy_workspace_bytes.restype = C.c_size_t
+        L.gsb_mercy_workspace_bytes.argtypes = [C.c_int32]
+        L.gsb_mercy_plan.restype = C.c_int
+        L.gsb_mercy_plan.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_double, C.c_float, C.c_void_p,
+                                     C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_profile_enable.restype = None
         L.gsb_profile_enable.argtypes = [C.c_int]
         L.gsb_profile_read.restype = C.c_int
@@ -250,7 +261,8 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_densify_workspace_bytes", "gsb_densify_split_std_offset", "gsb_densify_plan", "gsb_densify_emit",
                     "gsb_forward_raw", "gsb_backward_raw", "gsb_deterministic_workspace_bytes", "gsb_backward_deterministic",
                     "gsb_statistics_workspace_bytes", "gsb_forward_statistics_deterministic",
-                    "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic"]
+                    "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic", "gsb_redundancy_workspace_bytes",
+                    "gsb_redundancy_score", "gsb_mercy_workspace_bytes", "gsb_mercy_plan"]
 
 
 def check(status: int):
