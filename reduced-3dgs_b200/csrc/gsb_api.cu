@@ -95,15 +95,11 @@ static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter
 	"det_gather", "det_clear" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
-int launch_preprocess(const GsbScene*, const GsbCamera*, const GeomState&, const ImageState&, const BinPlan&, int32_t*, const GsbDebug*, bool,
-	const GsbRawParams*, cudaStream_t);
 int launch_mark_visible(int, const float*, const float*, uint8_t*, cudaStream_t);
 int launch_tile_scan(const ImageState&, const GeomState&, const BinPlan&, int, int, cudaStream_t);
 int launch_scatter_sort(const GeomState&, const BinningState&, const ImageState&, const BinPlan&, int, long long, int, int, cudaStream_t);
 int launch_sort_large(const GeomState&, const BinningState&, const ImageState&, int, int, uint32_t, uint32_t, cudaStream_t);
 int launch_export_binning(const GeomState&, const BinningState&, const ImageState&, int, int, uint64_t*, uint32_t*, cudaStream_t);
-int launch_render_forward(const ImageState&, const BinningState&, const GeomState&, int, int, const float*, float*, int32_t*, float*, float*, float*,
-	bool, cudaStream_t);
 int launch_stats_fixed_to_float(int, const unsigned long long*, float*, cudaStream_t);
 int launch_sh_stats_update(int, int, const int*, const float*, const float*, const float*, const int*, const int*, const float*, float*, float*,
 	float*, float*, float*, cudaStream_t);
@@ -119,13 +115,7 @@ size_t kmeans_deterministic_workspace_bytes(long long, int);
 int launch_kmeans_deterministic(const float*, long long, const float*, int, float, int, int*, float*, char*, cudaStream_t);
 size_t knn_workspace_bytes(long long, long long);
 int launch_knn(const float*, long long, int, const int32_t*, long long, const int32_t*, long long, float*, float*, int32_t*, char*, cudaStream_t);
-int launch_render_backward(const ImageState&, const BinningState&, const GeomState&, int, int, int, const float*, const float*, const float*,
-	const float*, float*, cudaStream_t);
-int launch_preprocess_backward(const GsbScene*, const GsbCamera*, const GeomState&, const int32_t*, const float*, const GsbGrads*, bool, float,
-	float*, bool, const GsbRawParams*, const GsbRawGrads*, cudaStream_t);
 size_t det_workspace_bytes(int, long long);
-int launch_render_backward_deterministic(const ImageState&, const BinningState&, const GeomState&, int, long long, int, int, const float*,
-	const float*, const float*, const float*, float*, char*, cudaStream_t);
 size_t camera_grad_workspace_bytes(int);
 int launch_camera_grad_finish(int, const float*, float*, float*, float*, cudaStream_t);
 
@@ -164,7 +154,8 @@ static int check_backward_raw(const GsbScene* scene, const GsbGrads* grads, cons
 	return GSB_OK;
 }
 
-static int check_scene(const GsbScene* s, const GsbCamera* c, const GsbRawParams* raw = nullptr)
+// raw: the entry point has run check_raw, which replaces the checks of the activated inputs
+static int check_scene(const GsbScene* s, const GsbCamera* c, bool raw)
 {
 	if (!s || !c) { set_error("scene / camera is NULL"); return GSB_EINVAL; }
 	if (s->P < 0) { set_error("P < 0"); return GSB_EINVAL; }
@@ -181,13 +172,33 @@ static int check_scene(const GsbScene* s, const GsbCamera* c, const GsbRawParams
 		return GSB_OK;
 	}
 	if (!s->opacities) { set_error("opacities missing"); return GSB_EINVAL; }
-	if (raw) return check_raw(s, raw);
+	if (raw) return GSB_OK;
 	// diff_gaussian_rasterization/__init__.py:203-207
 	if ((s->shs == nullptr) == (s->colors_precomp == nullptr)) { set_error("Please provide excatly one of either SHs or precomputed colors!"); return GSB_EINVAL; }
 	const bool sr = s->scales != nullptr && s->rotations != nullptr;
 	if (sr == (s->cov3D_precomp != nullptr) || ((s->scales != nullptr) != (s->rotations != nullptr)))
 	{ set_error("Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!"); return GSB_EINVAL; }
 	if (s->shs && !s->sh_packed && (!s->degrees || s->M <= 0)) { set_error("dense SH needs degrees and M > 0"); return GSB_EINVAL; }
+	return GSB_OK;
+}
+
+// Checks that several entry points make first; `fn` names the entry point in the message.
+static int check_scene_arg(const char* fn, const GsbScene* s)
+{
+	if (!s || s->P < 0) { set_error("%s: scene is NULL or P < 0", fn); return GSB_EINVAL; }
+	return GSB_OK;
+}
+
+static int check_maps_pair(const char* fn, const float* out_invdepth, const float* out_alpha)
+{
+	if ((out_invdepth == nullptr) != (out_alpha == nullptr))
+	{ set_error("%s: give both map outputs (invdepth and alpha) or neither", fn); return GSB_EINVAL; }
+	return GSB_OK;
+}
+
+static int check_camera_workspace(const char* fn, const BackwardRequest& r)
+{
+	if (r.want_cam() && !r.cam_workspace) { set_error("%s: a camera gradient is requested but the workspace is NULL", fn); return GSB_EINVAL; }
 	return GSB_OK;
 }
 
@@ -257,34 +268,31 @@ struct HostSide {
 static thread_local std::map<int, HostSide> t_host;
 }
 
-static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
-	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
-	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, int32_t* touched_pixels, float* transmittance,
-	float* out_invdepth, float* out_alpha, bool aa, void* stream_, const GsbRawParams* raw = nullptr, bool fixed_point_stats = false)
+static int forward_impl(const ForwardRequest& r)
 {
-	cudaStream_t stream = (cudaStream_t)stream_;
-	if (int e = check_scene(scene, cam, raw)) return e;
-	if (!out_color || !num_rendered || (scene->P > 0 && !radii)) { set_error("output pointers missing"); return GSB_EINVAL; }
-	*num_rendered = 0;
-	const int P = scene->P, W = cam->width, H = cam->height;
+	const GsbScene* scene = r.scene; const cudaStream_t stream = r.stream;
+	if (int e = check_scene(scene, r.cam, r.raw != nullptr)) return e;
+	if (!r.out_color || !r.num_rendered || (scene->P > 0 && !r.radii)) { set_error("output pointers missing"); return GSB_EINVAL; }
+	*r.num_rendered = 0;
+	const int P = scene->P, W = r.cam->width, H = r.cam->height;
 	const size_t N = size_t(W) * H;
 	if (P == 0)
 	{
 		// rasterize_points.cu:170,184-185: P == 0 returns the zero-initialised image (no background); the maps are zero too
-		GSB_CUDA_OK(cudaMemsetAsync(out_color, 0, 3 * N * sizeof(float), stream));
-		if (out_invdepth) GSB_CUDA_OK(cudaMemsetAsync(out_invdepth, 0, N * sizeof(float), stream));
-		if (out_alpha) GSB_CUDA_OK(cudaMemsetAsync(out_alpha, 0, N * sizeof(float), stream));
+		GSB_CUDA_OK(cudaMemsetAsync(r.out_color, 0, 3 * N * sizeof(float), stream));
+		if (r.out_invdepth) GSB_CUDA_OK(cudaMemsetAsync(r.out_invdepth, 0, N * sizeof(float), stream));
+		if (r.out_alpha) GSB_CUDA_OK(cudaMemsetAsync(r.out_alpha, 0, N * sizeof(float), stream));
 		return GSB_OK;
 	}
 	const BinPlan plan = make_bin_plan(P, W, H, scene->quant != nullptr);
-	char* geom_blob = geom_alloc(geom_user, gsb_geom_bytes(P));
-	char* img_blob = image_alloc(image_user, gsb_image_bytes_for(P, W, H, scene->quant != nullptr));
+	char* geom_blob = r.geom_alloc(r.geom_user, gsb_geom_bytes(P));
+	char* img_blob = r.image_alloc(r.image_user, gsb_image_bytes_for(P, W, H, scene->quant != nullptr));
 	if (!geom_blob || !img_blob) { set_error("scratch allocation failed"); return GSB_ENOMEM; }
 	GeomState g = GeomState::carve(geom_blob, P);
 	ImageState img = ImageState::carve(img_blob, W, H, nullptr, plan.priv ? plan.ctas : 0);
 	GSB_CUDA_OK(cudaMemsetAsync(g.counters, 0, 16 * sizeof(uint32_t), stream));
 	if (!plan.priv) GSB_CUDA_OK(cudaMemsetAsync(img.tile_count, 0, ImageState::tiles(W, H) * sizeof(uint32_t), stream));
-	if (int e = launch_preprocess(scene, cam, g, img, plan, radii, debug, aa, raw, stream)) return e;
+	if (int e = launch_preprocess(r, g, img, plan)) return e;
 	if (int e = launch_tile_scan(img, g, plan, W, H, stream)) return e;
 
 	// The instance count R sizes the binning blob (rasterizer_impl.cu:445-450 reads it back and stalls the device meanwhile).
@@ -303,7 +311,7 @@ static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_f
 	BinningState b{};
 	if (cap > 0)
 	{
-		char* bin_blob = binning_alloc(binning_user, gsb_binning_bytes(cap));
+		char* bin_blob = r.binning_alloc(r.binning_user, gsb_binning_bytes(cap));
 		if (!bin_blob) { set_error("binning allocation failed"); return GSB_ENOMEM; }
 		b = BinningState::carve(bin_blob, cap);
 		if (int e = launch_scatter_sort(g, b, img, plan, P, cap, W, H, stream)) return e;
@@ -314,64 +322,68 @@ static int forward_impl(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_f
 	if (hc[6]) { set_error("the (Gaussian, tile) instance count does not fit 31 bits"); return GSB_ERANGE; }
 	const long long R = hc[0];
 	if (R > hs.r_hint || 2 * R < hs.r_hint) hs.r_hint = R;       // grows with the workload, restarts when a much smaller one begins
-	*num_rendered = R;
+	*r.num_rendered = R;
 	if (cap == 0 || R > cap)
 	{
 		// first frame of this thread on this device, or more instances than speculated (the guarded kernels above did nothing)
-		char* bin_blob = binning_alloc(binning_user, gsb_binning_bytes(R));
+		char* bin_blob = r.binning_alloc(r.binning_user, gsb_binning_bytes(R));
 		if (!bin_blob) { set_error("binning allocation failed"); return GSB_ENOMEM; }
 		b = BinningState::carve(bin_blob, R);
 		if (int e = launch_scatter_sort(g, b, img, plan, P, R, W, H, stream)) return e;
 	}
 	if (R > 0) if (int e = launch_sort_large(g, b, img, W, H, hc[4], hc[5], stream)) return e;
-	if (int e = launch_render_forward(img, b, g, W, H, cam->background, out_color, touched_pixels, transmittance, out_invdepth, out_alpha,
-		fixed_point_stats, stream)) return e;
-	return GSB_OK;
+	return launch_render_forward(r, img, b, g);
 }
 
 int gsb_forward(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
 	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
 	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, void* stream)
 {
-	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, debug, nullptr, nullptr, nullptr, nullptr, false, stream);
+	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered,
+		debug };
+	r.stream = (cudaStream_t)stream;
+	return forward_impl(r);
 }
 
 int gsb_forward_antialiased(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
 	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
 	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, float* out_invdepth, float* out_alpha, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("forward_antialiased: scene is NULL or P < 0"); return GSB_EINVAL; }
-	if ((out_invdepth == nullptr) != (out_alpha == nullptr))
-	{ set_error("forward_antialiased: give both map outputs (invdepth and alpha) or neither"); return GSB_EINVAL; }
-	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, debug, nullptr, nullptr, out_invdepth, out_alpha, true, stream);
+	if (int e = check_scene_arg("forward_antialiased", scene)) return e;
+	if (int e = check_maps_pair("forward_antialiased", out_invdepth, out_alpha)) return e;
+	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered,
+		debug };
+	r.out_invdepth = out_invdepth; r.out_alpha = out_alpha; r.aa = true; r.stream = (cudaStream_t)stream;
+	return forward_impl(r);
 }
 
 int gsb_forward_maps(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
 	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
 	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, float* out_invdepth, float* out_alpha, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("forward_maps: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if (int e = check_scene_arg("forward_maps", scene)) return e;
 	if (!out_invdepth || !out_alpha) { set_error("forward_maps: map output pointers missing"); return GSB_EINVAL; }
-	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, debug, nullptr, nullptr, out_invdepth, out_alpha, false, stream);
+	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered,
+		debug };
+	r.out_invdepth = out_invdepth; r.out_alpha = out_alpha; r.stream = (cudaStream_t)stream;
+	return forward_impl(r);
 }
 
 int gsb_forward_statistics(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
 	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
 	float* out_color, int32_t* radii, int64_t* num_rendered, int32_t* touched_pixels, float* transmittance_sum, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("scene is NULL"); return GSB_EINVAL; }
+	if (int e = check_scene_arg("forward_statistics", scene)) return e;
 	if (scene->P > 0 && (!touched_pixels || !transmittance_sum)) { set_error("statistics output pointers missing"); return GSB_EINVAL; }
+	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered };
+	r.touched_pixels = touched_pixels; r.transmittance = transmittance_sum; r.stream = (cudaStream_t)stream;
 	if (scene->P > 0)
 	{
 		// reduced_3dgs.cu:117-118: both statistics start from zero for every camera
-		GSB_CUDA_OK(cudaMemsetAsync(touched_pixels, 0, size_t(scene->P) * sizeof(int32_t), (cudaStream_t)stream));
-		GSB_CUDA_OK(cudaMemsetAsync(transmittance_sum, 0, size_t(scene->P) * sizeof(float), (cudaStream_t)stream));
+		GSB_CUDA_OK(cudaMemsetAsync(touched_pixels, 0, size_t(scene->P) * sizeof(int32_t), r.stream));
+		GSB_CUDA_OK(cudaMemsetAsync(transmittance_sum, 0, size_t(scene->P) * sizeof(float), r.stream));
 	}
-	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, nullptr, touched_pixels, transmittance_sum, nullptr, nullptr, false, stream);
+	return forward_impl(r);
 }
 
 size_t gsb_statistics_workspace_bytes(int32_t P) { return (P > 0 ? size_t(P) * sizeof(unsigned long long) : 0) + 256; }
@@ -381,7 +393,7 @@ int gsb_forward_statistics_deterministic(const GsbScene* scene, const GsbCamera*
 	float* out_color, int32_t* radii, int64_t* num_rendered, int32_t* touched_pixels, float* transmittance_sum, char* workspace,
 	void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("statistics_deterministic: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if (int e = check_scene_arg("statistics_deterministic", scene)) return e;
 	if (scene->P > 0 && (!touched_pixels || !transmittance_sum)) { set_error("statistics output pointers missing"); return GSB_EINVAL; }
 	if (scene->P > 0 && !workspace) { set_error("statistics_deterministic: workspace is NULL"); return GSB_EINVAL; }
 	if (cam && (long long)cam->width * cam->height >= (1ll << 28))
@@ -389,15 +401,16 @@ int gsb_forward_statistics_deterministic(const GsbScene* scene, const GsbCamera*
 		set_error("statistics_deterministic: %d x %d pixels; the 64-bit fixed-point sums need W * H < 2^28", cam->width, cam->height);
 		return GSB_ERANGE;
 	}
-	unsigned long long* fixed = reinterpret_cast<unsigned long long*>(workspace);
+	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered };
+	r.touched_pixels = touched_pixels; r.transmittance_fixed = reinterpret_cast<unsigned long long*>(workspace);
+	r.stream = (cudaStream_t)stream;
 	if (scene->P > 0)
 	{
-		GSB_CUDA_OK(cudaMemsetAsync(touched_pixels, 0, size_t(scene->P) * sizeof(int32_t), (cudaStream_t)stream));
-		GSB_CUDA_OK(cudaMemsetAsync(fixed, 0, size_t(scene->P) * sizeof(unsigned long long), (cudaStream_t)stream));
+		GSB_CUDA_OK(cudaMemsetAsync(touched_pixels, 0, size_t(scene->P) * sizeof(int32_t), r.stream));
+		GSB_CUDA_OK(cudaMemsetAsync(r.transmittance_fixed, 0, size_t(scene->P) * sizeof(unsigned long long), r.stream));
 	}
-	if (int e = forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, nullptr, touched_pixels, reinterpret_cast<float*>(fixed), nullptr, nullptr, false, stream, nullptr, true)) return e;
-	return launch_stats_fixed_to_float(scene->P, fixed, transmittance_sum, (cudaStream_t)stream);
+	if (int e = forward_impl(r)) return e;
+	return launch_stats_fixed_to_float(scene->P, r.transmittance_fixed, transmittance_sum, r.stream);
 }
 
 int gsb_sh_statistics_update(int32_t P, int32_t M, const int32_t* degrees, const float* means3D, const float* campos, const float* shs,
@@ -508,47 +521,38 @@ int gsb_min_redundancy_value(int32_t P, const int32_t* redundancy_values, const 
 	return launch_min_redundancy(P, redundancy_values, neighbours, intersection_mask, knn, minimum_redundancy_values, (cudaStream_t)stream);
 }
 
-static int backward_impl(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dview, float* dL_dproj, float* dL_dcampos, char* cam_workspace, bool aa, void* stream_,
-	const GsbRawParams* raw = nullptr, const GsbRawGrads* raw_grads = nullptr, bool det = false, char* det_workspace = nullptr)
+static int backward_impl(const BackwardRequest& r)
 {
-	cudaStream_t stream = (cudaStream_t)stream_;
-	if (int e = check_scene(scene, cam, raw)) return e;
+	const GsbScene* scene = r.scene; const GsbGrads* grads = r.grads; const cudaStream_t stream = r.stream;
+	if (int e = check_scene(scene, r.cam, r.raw != nullptr)) return e;
 	if (!grads) { set_error("grads is NULL"); return GSB_EINVAL; }
-	const int P = scene->P, W = cam->width, H = cam->height;
-	const bool want_cam = dL_dview || dL_dproj || dL_dcampos;
+	const int P = scene->P, W = r.cam->width, H = r.cam->height;
 	if (P == 0)
 	{
 		// no Gaussian, no camera gradient (the camera outputs are always written, also in accumulate mode)
-		if (dL_dview) GSB_CUDA_OK(cudaMemsetAsync(dL_dview, 0, 16 * sizeof(float), stream));
-		if (dL_dproj) GSB_CUDA_OK(cudaMemsetAsync(dL_dproj, 0, 16 * sizeof(float), stream));
-		if (dL_dcampos) GSB_CUDA_OK(cudaMemsetAsync(dL_dcampos, 0, 3 * sizeof(float), stream));
+		if (r.dL_dview) GSB_CUDA_OK(cudaMemsetAsync(r.dL_dview, 0, 16 * sizeof(float), stream));
+		if (r.dL_dproj) GSB_CUDA_OK(cudaMemsetAsync(r.dL_dproj, 0, 16 * sizeof(float), stream));
+		if (r.dL_dcampos) GSB_CUDA_OK(cudaMemsetAsync(r.dL_dcampos, 0, 3 * sizeof(float), stream));
 		return GSB_OK;
 	}
-	if (!geom_blob || !binning_blob || !image_blob || !dL_dout_color || !radii) { set_error("backward inputs missing"); return GSB_EINVAL; }
-	if (raw)
+	if (!r.geom_blob || !r.binning_blob || !r.image_blob || !r.dL_dout_color || !r.radii) { set_error("backward inputs missing"); return GSB_EINVAL; }
+	if (r.raw)
 	{
-		if (!grads->dL_dmeans2D || !grads->dL_dopacity || !grads->dL_dmeans3D || !raw_grads->dL_dscaling || !raw_grads->dL_drotation)
+		if (!grads->dL_dmeans2D || !grads->dL_dopacity || !grads->dL_dmeans3D || !r.raw_grads->dL_dscaling || !r.raw_grads->dL_drotation)
 		{ set_error("gradient output pointers missing"); return GSB_EINVAL; }
 	}
 	else if (!grads->dL_dmeans2D || !grads->dL_dcolors || !grads->dL_dopacity || !grads->dL_dmeans3D || !grads->dL_dcov3D ||
 		!grads->dL_dscales || !grads->dL_drotations || (scene->M > 0 && !grads->dL_dsh))
 	{ set_error("gradient output pointers missing"); return GSB_EINVAL; }
-	GeomState g = GeomState::carve(const_cast<char*>(geom_blob), P);
-	ImageState img = ImageState::carve(const_cast<char*>(image_blob), W, H);
-	BinningState b = BinningState::carve(const_cast<char*>(binning_blob), R);
-	float* acc = reinterpret_cast<float*>(const_cast<char*>(geom_blob) + geom_state_bytes(P));
-	if (int e = det ? launch_render_backward_deterministic(img, b, g, P, R, W, H, cam->background, dL_dout_color, dL_dinvdepth, dL_dalpha,
-			acc, det_workspace, stream)
-		: launch_render_backward(img, b, g, P, W, H, cam->background, dL_dout_color, dL_dinvdepth, dL_dalpha, acc, stream))
+	GeomState g = GeomState::carve(const_cast<char*>(r.geom_blob), P);
+	ImageState img = ImageState::carve(const_cast<char*>(r.image_blob), W, H);
+	BinningState b = BinningState::carve(const_cast<char*>(r.binning_blob), r.R);
+	float* acc = reinterpret_cast<float*>(const_cast<char*>(r.geom_blob) + geom_state_bytes(P));
+	if (int e = r.deterministic ? launch_render_backward_deterministic(r, img, b, g, acc) : launch_render_backward(r, img, b, g, acc, nullptr, nullptr))
 		return e;
-	float* cam_rows = want_cam ? reinterpret_cast<float*>(cam_workspace) : nullptr;
-	if (int e = launch_preprocess_backward(scene, cam, g, radii, acc, grads, dL_dinvdepth != nullptr, lambda_sh_sparsity, cam_rows, aa, raw,
-		raw_grads, stream))
-		return e;
-	if (want_cam) if (int e = launch_camera_grad_finish(P, cam_rows, dL_dview, dL_dproj, dL_dcampos, stream)) return e;
+	if (int e = launch_preprocess_backward(r, g, acc)) return e;
+	if (r.want_cam())
+		if (int e = launch_camera_grad_finish(P, reinterpret_cast<float*>(r.cam_workspace), r.dL_dview, r.dL_dproj, r.dL_dcampos, stream)) return e;
 	return GSB_OK;
 }
 
@@ -556,8 +560,9 @@ int gsb_backward(const GsbScene* scene, const GsbCamera* cam, int64_t R, const i
 	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
 	const GsbGrads* grads, float lambda_sh_sparsity, void* stream)
 {
-	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, nullptr, nullptr,
-		lambda_sh_sparsity, nullptr, nullptr, nullptr, nullptr, false, stream);
+	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads };
+	r.lambda_sh_sparsity = lambda_sh_sparsity; r.stream = (cudaStream_t)stream;
+	return backward_impl(r);
 }
 
 size_t gsb_camera_grad_workspace_bytes(int32_t P) { return camera_grad_workspace_bytes(P); }
@@ -567,11 +572,12 @@ int gsb_backward_camera(const GsbScene* scene, const GsbCamera* cam, int64_t R, 
 	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
 	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("backward_camera: scene is NULL or P < 0"); return GSB_EINVAL; }
-	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
-	{ set_error("backward_camera: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
-	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, false, stream);
+	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
+	r.stream = (cudaStream_t)stream;
+	if (int e = check_scene_arg("backward_camera", scene)) return e;
+	if (int e = check_camera_workspace("backward_camera", r)) return e;
+	return backward_impl(r);
 }
 
 int gsb_backward_antialiased(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
@@ -579,11 +585,12 @@ int gsb_backward_antialiased(const GsbScene* scene, const GsbCamera* cam, int64_
 	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
 	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("backward_antialiased: scene is NULL or P < 0"); return GSB_EINVAL; }
-	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
-	{ set_error("backward_antialiased: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
-	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, true, stream);
+	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
+	r.aa = true; r.stream = (cudaStream_t)stream;
+	if (int e = check_scene_arg("backward_antialiased", scene)) return e;
+	if (int e = check_camera_workspace("backward_antialiased", r)) return e;
+	return backward_impl(r);
 }
 
 int gsb_forward_raw(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
@@ -591,12 +598,13 @@ int gsb_forward_raw(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn ge
 	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, float* out_invdepth, float* out_alpha,
 	const GsbRawParams* raw, int32_t antialiasing, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("forward_raw: scene is NULL or P < 0"); return GSB_EINVAL; }
-	if ((out_invdepth == nullptr) != (out_alpha == nullptr))
-	{ set_error("forward_raw: give both map outputs (invdepth and alpha) or neither"); return GSB_EINVAL; }
+	if (int e = check_scene_arg("forward_raw", scene)) return e;
+	if (int e = check_maps_pair("forward_raw", out_invdepth, out_alpha)) return e;
 	if (int e = check_raw(scene, raw)) return e;
-	return forward_impl(scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii,
-		num_rendered, debug, nullptr, nullptr, out_invdepth, out_alpha, antialiasing != 0, stream, raw);
+	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered,
+		debug };
+	r.out_invdepth = out_invdepth; r.out_alpha = out_alpha; r.aa = antialiasing != 0; r.raw = raw; r.stream = (cudaStream_t)stream;
+	return forward_impl(r);
 }
 
 int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
@@ -605,12 +613,13 @@ int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_t R, con
 	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
 	int32_t antialiasing, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("backward_raw: scene is NULL or P < 0"); return GSB_EINVAL; }
-	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
-	{ set_error("backward_raw: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
+	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
+	r.aa = antialiasing != 0; r.raw = raw; r.raw_grads = raw_grads; r.stream = (cudaStream_t)stream;
+	if (int e = check_scene_arg("backward_raw", scene)) return e;
+	if (int e = check_camera_workspace("backward_raw", r)) return e;
 	if (int e = check_backward_raw(scene, grads, raw, raw_grads)) return e;
-	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, antialiasing != 0, stream, raw, raw_grads);
+	return backward_impl(r);
 }
 
 size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered); }
@@ -621,27 +630,30 @@ int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* cam, int6
 	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
 	int32_t antialiasing, char* det_workspace, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("backward_deterministic: scene is NULL or P < 0"); return GSB_EINVAL; }
+	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
+	r.aa = antialiasing != 0; r.raw = raw; r.raw_grads = raw_grads; r.deterministic = true; r.det_workspace = det_workspace;
+	r.stream = (cudaStream_t)stream;
+	if (int e = check_scene_arg("backward_deterministic", scene)) return e;
 	if (R < 0) { set_error("backward_deterministic: num_rendered < 0"); return GSB_EINVAL; }
 	if (R >= (1ll << 30))
 	{ set_error("backward_deterministic: 2^30 or more instances (the slot scan's look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
 	if (scene->P > 0 && R > 0 && !det_workspace) { set_error("backward_deterministic: det_workspace is NULL"); return GSB_EINVAL; }
-	if ((dL_dviewmatrix || dL_dprojmatrix || dL_dcampos) && !workspace)
-	{ set_error("backward_deterministic: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
+	if (int e = check_camera_workspace("backward_deterministic", r)) return e;
 	if (raw_grads && !raw) { set_error("backward_deterministic: raw_grads given without raw"); return GSB_EINVAL; }
 	if (raw) if (int e = check_backward_raw(scene, grads, raw, raw_grads)) return e;
-	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, antialiasing != 0, stream, raw, raw_grads, true,
-		det_workspace);
+	return backward_impl(r);
 }
 
 int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
 	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
 	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity, void* stream)
 {
-	if (!scene || scene->P < 0) { set_error("backward_maps: scene is NULL or P < 0"); return GSB_EINVAL; }
-	return backward_impl(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, nullptr, nullptr, nullptr, nullptr, false, stream);
+	if (int e = check_scene_arg("backward_maps", scene)) return e;
+	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity };
+	r.stream = (cudaStream_t)stream;
+	return backward_impl(r);
 }
 
 int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present, void* stream)

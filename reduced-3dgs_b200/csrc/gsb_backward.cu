@@ -621,56 +621,41 @@ int launch_camera_grad_finish(int P, const float* rows, float* dview, float* dpr
 	return GSB_OK;
 }
 
-int launch_preprocess_backward(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const int32_t* radii, const float* acc,
-	const GsbGrads* grads, bool maps, float lambda, float* cam_rows, bool aa, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
-	cudaStream_t stream)
+int launch_preprocess_backward(const BackwardRequest& req, const GeomState& g, const float* acc)
 {
+	const GsbScene* s = req.scene; const GsbCamera* cam = req.cam; const GsbRawParams* raw = req.raw;
 	BwdArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
 	a.mod = s->scale_modifier; a.tan_fovx = cam->tan_fovx; a.tan_fovy = cam->tan_fovy;
 	a.focal_y = cam->height / (2.0f * cam->tan_fovy); a.focal_x = cam->width / (2.0f * cam->tan_fovx);   // rasterizer_impl.cu:573-574
-	a.lambda = lambda;
+	a.lambda = req.lambda_sh_sparsity;
 	a.means3D = s->means3D; a.scales = s->scales; a.rotations = s->rotations; a.cov3D_precomp = s->cov3D_precomp;
-	a.shs = s->shs; a.colors_precomp = s->colors_precomp; a.degrees = s->degrees; a.radii = radii;
+	a.shs = s->shs; a.colors_precomp = s->colors_precomp; a.degrees = s->degrees; a.radii = req.radii;
 	a.view = cam->viewmatrix; a.proj = cam->projmatrix; a.campos = cam->campos;
 	a.quant = s->quant != nullptr; if (s->quant) a.q = *s->quant;
-	a.g = g; a.acc = acc; a.out = *grads; a.cam_rows = cam_rows;
+	a.g = g; a.acc = acc; a.out = *req.grads; a.cam_rows = req.want_cam() ? reinterpret_cast<float*>(req.cam_workspace) : nullptr;
 	if (raw)
 	{
 		a.M = raw->features_dc && !s->colors_precomp ? 1 + raw->C : 0;
 		a.scales = raw->scaling; a.rotations = raw->rotation;
 		a.sh_dc = s->colors_precomp ? nullptr : raw->features_dc; a.sh_rest = raw->features_rest; a.n_rest = raw->C;
-		a.out.dL_dscales = raw_grads->dL_dscaling; a.out.dL_drotations = raw_grads->dL_drotation;
-		a.dL_ddc = raw_grads->dL_dfeatures_dc; a.dL_drest = raw_grads->dL_dfeatures_rest;
+		a.out.dL_dscales = req.raw_grads->dL_dscaling; a.out.dL_drotations = req.raw_grads->dL_drotation;
+		a.dL_ddc = req.raw_grads->dL_dfeatures_dc; a.dL_drest = req.raw_grads->dL_dfeatures_rest;
 		auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
 		a.raw_vec4 = al(a.sh_dc) && al(a.sh_rest) && al(a.dL_ddc) && al(a.dL_drest);
 	}
 	const int grid = preprocess_backward_grid(s->P);
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * a.M + 1) + 32 * 6) * sizeof(float);
-	ProfScope prof(K_PREPROCESS_BWD, stream);
-#define GSB_LAUNCH_PB(Q, A, MP, CM, AA)                                                                               \
-	do {                                                                                                             \
-		if (int e = ensure_dyn_smem((const void*)preprocess_backward_kernel<Q, A, MP, CM, AA>, 160 * 1024)) return e;  \
-		preprocess_backward_kernel<Q, A, MP, CM, AA><<<grid, 256, smem, stream>>>(a);                                \
-	} while (0)
-#define GSB_LAUNCH_PB_QA(MP, CM, AA)                                                                                 \
-	do {                                                                                                             \
-		if (a.quant) { if (grads->accumulate) GSB_LAUNCH_PB(IN_QUANT, true, MP, CM, AA); else GSB_LAUNCH_PB(IN_QUANT, false, MP, CM, AA); }  \
-		else if (raw) { if (grads->accumulate) GSB_LAUNCH_PB(IN_RAW, true, MP, CM, AA); else GSB_LAUNCH_PB(IN_RAW, false, MP, CM, AA); }    \
-		else { if (grads->accumulate) GSB_LAUNCH_PB(IN_ACTIVATED, true, MP, CM, AA); else GSB_LAUNCH_PB(IN_ACTIVATED, false, MP, CM, AA); }  \
-	} while (0)
-#define GSB_LAUNCH_PB_MC(AA)                                                                                         \
-	do {                                                                                                             \
-		if (cam_rows) { if (maps) GSB_LAUNCH_PB_QA(true, true, AA); else GSB_LAUNCH_PB_QA(false, true, AA); }        \
-		else { if (maps) GSB_LAUNCH_PB_QA(true, false, AA); else GSB_LAUNCH_PB_QA(false, false, AA); }              \
-	} while (0)
-	if (aa) GSB_LAUNCH_PB_MC(true); else GSB_LAUNCH_PB_MC(false);
-#undef GSB_LAUNCH_PB_MC
-#undef GSB_LAUNCH_PB_QA
-#undef GSB_LAUNCH_PB
-	GSB_LAUNCHED();
-	GSB_CUDA_OK(cudaGetLastError());
-	return GSB_OK;
+	ProfScope prof(K_PREPROCESS_BWD, req.stream);
+	const InputMode in = a.quant ? IN_QUANT : (raw ? IN_RAW : IN_ACTIVATED);
+	return dispatch([&](auto in, auto accumulate, auto maps, auto cam_grad, auto aa) -> int {
+		auto kernel = preprocess_backward_kernel<in, accumulate, maps, cam_grad, aa>;
+		if (int e = ensure_dyn_smem((const void*)kernel, 160 * 1024)) return e;
+		kernel<<<grid, 256, smem, req.stream>>>(a);
+		GSB_LAUNCHED();
+		GSB_CUDA_OK(cudaGetLastError());
+		return GSB_OK;
+	}, in, req.grads->accumulate != 0, req.dL_dinvdepth != nullptr, a.cam_rows != nullptr, req.aa);
 }
 
 } // namespace gsb

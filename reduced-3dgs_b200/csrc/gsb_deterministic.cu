@@ -119,20 +119,18 @@ __global__ void __launch_bounds__(256) det_gather_kernel(int P, int ns, const ui
 	if (k < 12) acc[12 * g + k] = s;
 }
 
-int launch_render_backward_det(const ImageState&, const BinningState&, const GeomState&, long long, int, int, const float*, const float*,
-	const float*, const float*, float*, const uint32_t*, cudaStream_t);
-
 // scan -> deterministic render backward -> gather: writes all 12 floats of every Gaussian's accumulator.
-int launch_render_backward_deterministic(const ImageState& img, const BinningState& b, const GeomState& g, int P, long long R, int W, int H,
-	const float* bg, const float* dL_dpix, const float* dL_dinvdepth, const float* dL_dalpha, float* acc, char* workspace, cudaStream_t stream)
+int launch_render_backward_deterministic(const BackwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g,
+	float* acc)
 {
+	const int P = req.scene->P; const long long R = req.R; const cudaStream_t stream = req.stream;
 	if (R == 0)
 	{
 		// nothing rendered: every rect is empty and every gradient zero
 		GSB_CUDA_OK(cudaMemsetAsync(acc, 0, size_t(P) * 48, stream));
 		return GSB_OK;
 	}
-	DetWorkspace w = DetWorkspace::carve(workspace, P, R);
+	DetWorkspace w = DetWorkspace::carve(req.det_workspace, P, R);
 	{
 		ProfScope prof(K_DET_SCAN, stream);
 		GSB_CUDA_OK(cudaMemsetAsync(w.head, 0, w.head_bytes(), stream));
@@ -141,9 +139,9 @@ int launch_render_backward_deterministic(const ImageState& img, const BinningSta
 		GSB_LAUNCHED();
 		GSB_CUDA_OK(cudaGetLastError());
 	}
-	if (int e = launch_render_backward_det(img, b, g, R, W, H, bg, dL_dpix, dL_dinvdepth, dL_dalpha, w.parts, w.offset, stream)) return e;
+	if (int e = launch_render_backward(req, img, b, g, acc, w.parts, w.offset)) return e;
 	ProfScope prof(K_DET_GATHER, stream);
-	const int ns = (dL_dinvdepth || dL_dalpha) ? 10 : 9;
+	const int ns = (req.dL_dinvdepth || req.dL_dalpha) ? 10 : 9;
 	det_gather_kernel<<<(unsigned)((16ll * P + 255) / 256), 256, 0, stream>>>(P, ns, g.rect, w.offset, w.parts, (unsigned long long)R, w.head,
 		acc);
 	GSB_LAUNCHED();

@@ -419,9 +419,9 @@ int launch_debug_dequant(const GsbQuant* q, int P, float* scales, float* rots, c
 	return GSB_OK;
 }
 
-int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& g, const ImageState& img, const BinPlan& plan, int32_t* radii, const GsbDebug* dbg,
-	bool aa, const GsbRawParams* raw, cudaStream_t stream)
+int launch_preprocess(const ForwardRequest& req, const GeomState& g, const ImageState& img, const BinPlan& plan)
 {
+	const GsbScene* s = req.scene; const GsbCamera* cam = req.cam; const GsbRawParams* raw = req.raw;
 	PreArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
 	a.gx = (cam->width + GSB_TILE_X - 1) / GSB_TILE_X; a.gy = (cam->height + GSB_TILE_Y - 1) / GSB_TILE_Y;
@@ -446,9 +446,9 @@ int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& 
 	a.prune = s->prune_mask;
 	a.quant = s->quant != nullptr;
 	if (s->quant) a.q = *s->quant;
-	a.g = g; a.radii = radii; a.tile_count = img.tile_count;
+	a.g = g; a.radii = req.radii; a.tile_count = img.tile_count;
 	a.hist_priv = plan.priv; a.chunk = plan.chunk; a.T = a.gx * a.gy; a.cta_count = img.cta_count;
-	if (dbg) a.dbg = *dbg;
+	if (req.debug) a.dbg = *req.debug;
 	a.prefiltered = cam->prefiltered;
 	if (raw)
 	{
@@ -463,20 +463,18 @@ int launch_preprocess(const GsbScene* s, const GsbCamera* cam, const GeomState& 
 	const size_t hist_words = plan.priv ? (plan.hist_bytes / 4 + 3) / 4 * 4 : 0;
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE * sizeof(float) : 0) + hist_words * 4 +
 		(a.quant ? size_t(threads / 32) * 32 * IDS_REST_ROW : 0);
-	const int mode = a.quant ? IN_QUANT : (raw ? IN_RAW : IN_ACTIVATED);
-	const void* kernel = mode == IN_QUANT ? (aa ? (const void*)preprocess_kernel<IN_QUANT, true> : (const void*)preprocess_kernel<IN_QUANT, false>)
-	                   : mode == IN_RAW   ? (aa ? (const void*)preprocess_kernel<IN_RAW, true> : (const void*)preprocess_kernel<IN_RAW, false>)
-	                                      : (aa ? (const void*)preprocess_kernel<IN_ACTIVATED, true> : (const void*)preprocess_kernel<IN_ACTIVATED, false>);
-	if (int e = ensure_dyn_smem(kernel, 220 * 1024)) return e;
-	ProfScope prof(K_PREPROCESS, stream);
 	int grid = plan.priv ? plan.ctas : blocks_needed;
 	if (!plan.priv && a.quant && grid > GSB_NUM_SMS * 8) grid = GSB_NUM_SMS * 8;                         // persistent: amortise the table load
-	if (mode == IN_QUANT) { if (aa) preprocess_kernel<IN_QUANT, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<IN_QUANT, false><<<grid, threads, smem, stream>>>(a); }
-	else if (mode == IN_RAW) { if (aa) preprocess_kernel<IN_RAW, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<IN_RAW, false><<<grid, threads, smem, stream>>>(a); }
-	else { if (aa) preprocess_kernel<IN_ACTIVATED, true><<<grid, threads, smem, stream>>>(a); else preprocess_kernel<IN_ACTIVATED, false><<<grid, threads, smem, stream>>>(a); }
-	GSB_LAUNCHED();
-	GSB_CUDA_OK(cudaGetLastError());
-	return GSB_OK;
+	const InputMode in = a.quant ? IN_QUANT : (raw ? IN_RAW : IN_ACTIVATED);
+	return dispatch([&](auto in, auto aa) -> int {
+		auto kernel = preprocess_kernel<in, aa>;
+		if (int e = ensure_dyn_smem((const void*)kernel, 220 * 1024)) return e;
+		ProfScope prof(K_PREPROCESS, req.stream);
+		kernel<<<grid, threads, smem, req.stream>>>(a);
+		GSB_LAUNCHED();
+		GSB_CUDA_OK(cudaGetLastError());
+		return GSB_OK;
+	}, in, req.aa);
 }
 
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t stream)

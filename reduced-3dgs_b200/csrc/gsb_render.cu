@@ -599,80 +599,53 @@ int launch_stats_fixed_to_float(int P, const unsigned long long* fixed, float* o
 	return GSB_OK;
 }
 
-// fixed_point: `transmittance` is the 64-bit fixed-point workspace of the deterministic statistics forward.
-int launch_render_forward(const ImageState& img, const BinningState& b, const GeomState& g, int W, int H, const float* bg,
-	float* out_color, int32_t* touched_pixels, float* transmittance, float* out_invdepth, float* out_alpha, bool fixed_point,
-	cudaStream_t stream)
+int launch_render_forward(const ForwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g)
 {
+	const int W = req.cam->width, H = req.cam->height;
 	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
-	ProfScope prof(K_RENDER_FWD, stream);
-	if (touched_pixels && transmittance && fixed_point)
-		render_forward_kernel<true, false, true><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, touched_pixels, transmittance, nullptr, nullptr);
-	else if (touched_pixels && transmittance)
-		render_forward_kernel<true, false><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, touched_pixels, transmittance, nullptr, nullptr);
-	else if (out_invdepth && out_alpha)
-		render_forward_kernel<false, true><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, nullptr, nullptr, out_invdepth, out_alpha);
-	else
-		render_forward_kernel<false, false><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, out_color, img.tile_max_contrib, nullptr, nullptr, nullptr, nullptr);
-	GSB_LAUNCHED();
-	GSB_CUDA_OK(cudaGetLastError());
-	return GSB_OK;
+	const bool fixed = req.touched_pixels && req.transmittance_fixed;
+	const bool stats = fixed || (req.touched_pixels && req.transmittance);
+	const bool maps = !stats && req.out_invdepth && req.out_alpha;
+	float* const transmittance = fixed ? reinterpret_cast<float*>(req.transmittance_fixed) : req.transmittance;
+	ProfScope prof(K_RENDER_FWD, req.stream);
+	return dispatch([&](auto stats, auto maps, auto fixed) -> int {
+		// four variants exist: <F,F>, <F,T>, <T,F> and <T,F,T> (statistics go without maps; fixed point only with statistics)
+		if constexpr (!(stats && maps) && (stats || !fixed))
+			render_forward_kernel<stats, maps, fixed><<<grid, 256, 0, req.stream>>>(img.ranges, b.point_list, W, H, g.rec,
+				req.cam->background, img.final_T, img.n_contrib, req.out_color, img.tile_max_contrib, stats ? req.touched_pixels : nullptr,
+				stats ? transmittance : nullptr, maps ? req.out_invdepth : nullptr, maps ? req.out_alpha : nullptr);
+		GSB_LAUNCHED();
+		GSB_CUDA_OK(cudaGetLastError());
+		return GSB_OK;
+	}, stats, maps, fixed);
 }
 
-int launch_render_backward(const ImageState& img, const BinningState& b, const GeomState& g, int P, int W, int H, const float* bg,
-	const float* dL_dpix, const float* dL_dinvdepth, const float* dL_dalpha, float* acc, cudaStream_t stream)
+int launch_render_backward(const BackwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g, float* acc,
+	float* parts, const uint32_t* slot_offset)
 {
+	const int W = req.cam->width, H = req.cam->height;
 	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
-	const bool maps = dL_dinvdepth || dL_dalpha;
-	const void* kernel = maps ? (const void*)render_backward_kernel<true> : (const void*)render_backward_kernel<false>;
-	const size_t smem = maps ? sizeof(BwdSmem<4>) : sizeof(BwdSmem<3>);
-	if (int e = ensure_dyn_smem(kernel, (int)smem)) return e;
-	ProfScope prof(K_RENDER_BWD, stream);
-	// the per-Gaussian accumulator the kernel reduces into (12 floats per Gaussian, inside the geometry blob)
-	GSB_CUDA_OK(cudaMemsetAsync(acc, 0, size_t(P) * 48, stream));
-	if (maps)
-		render_backward_kernel<true><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, acc, dL_dinvdepth, dL_dalpha);
-	else
-		render_backward_kernel<false><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, acc, nullptr, nullptr);
-	GSB_LAUNCHED();
-	GSB_CUDA_OK(cudaGetLastError());
-	return GSB_OK;
-}
-
-// Deterministic render backward (DESIGN.md §5i): per-instance partials into `parts` (R slots of DET_NS floats), slot bases
-// `slot_offset` from det_scan_kernel.  The accumulator is not touched here: det_gather_kernel writes all of it.
-int launch_render_backward_det(const ImageState& img, const BinningState& b, const GeomState& g, long long R, int W, int H,
-	const float* bg, const float* dL_dpix, const float* dL_dinvdepth, const float* dL_dalpha, float* parts, const uint32_t* slot_offset,
-	cudaStream_t stream)
-{
-	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
-	const bool maps = dL_dinvdepth || dL_dalpha;
-	const void* kernel = maps ? (const void*)render_backward_kernel<true, true> : (const void*)render_backward_kernel<false, true>;
-	const size_t smem = (maps ? sizeof(BwdSmem<4>) : sizeof(BwdSmem<3>)) + size_t(8) * BWD_BATCH * DET_NS(maps) * sizeof(float);
-	if (int e = ensure_dyn_smem(kernel, (int)smem)) return e;
-	{
-		// instances behind a tile's last contributor (and tiles with none) are never visited: their slots must read as zero
-		ProfScope prof(K_DET_CLEAR, stream);
-		GSB_CUDA_OK(cudaMemsetAsync(parts, 0, size_t(R) * DET_NS(maps) * sizeof(float), stream));
-	}
-	ProfScope prof(K_RENDER_BWD, stream);
-	if (maps)
-		render_backward_kernel<true, true><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, nullptr, dL_dinvdepth, dL_dalpha, parts, slot_offset, g.rect,
-			(unsigned long long)R);
-	else
-		render_backward_kernel<false, true><<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, bg,
-			img.final_T, img.n_contrib, img.tile_max_contrib, dL_dpix, nullptr, nullptr, nullptr, parts, slot_offset, g.rect,
-			(unsigned long long)R);
-	GSB_LAUNCHED();
-	GSB_CUDA_OK(cudaGetLastError());
-	return GSB_OK;
+	const cudaStream_t stream = req.stream;
+	return dispatch([&](auto maps, auto det) -> int {
+		const size_t smem = sizeof(BwdSmem<maps ? 4 : 3>) + (det ? size_t(8) * BWD_BATCH * DET_NS(maps) * sizeof(float) : 0);
+		auto kernel = render_backward_kernel<maps, det>;
+		if (int e = ensure_dyn_smem((const void*)kernel, (int)smem)) return e;
+		if (det)
+		{
+			// instances behind a tile's last contributor (and tiles with none) are never visited: their slots must read as zero
+			ProfScope prof(K_DET_CLEAR, stream);
+			GSB_CUDA_OK(cudaMemsetAsync(parts, 0, size_t(req.R) * DET_NS(maps) * sizeof(float), stream));
+		}
+		ProfScope prof(K_RENDER_BWD, stream);
+		// the per-Gaussian accumulator the kernel reduces into (12 floats per Gaussian, inside the geometry blob)
+		if (!det) GSB_CUDA_OK(cudaMemsetAsync(acc, 0, size_t(req.scene->P) * 48, stream));
+		kernel<<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, req.cam->background,
+			img.final_T, img.n_contrib, img.tile_max_contrib, req.dL_dout_color, det ? nullptr : acc, req.dL_dinvdepth, req.dL_dalpha,
+			parts, slot_offset, det ? g.rect : nullptr, det ? (unsigned long long)req.R : 0ull);
+		GSB_LAUNCHED();
+		GSB_CUDA_OK(cudaGetLastError());
+		return GSB_OK;
+	}, req.dL_dinvdepth || req.dL_dalpha, req.deterministic);
 }
 
 } // namespace gsb
