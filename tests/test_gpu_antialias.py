@@ -6,9 +6,9 @@
      saturate and stop rules, the maps) gives the colour, the maps and every gradient, camera included;
   4. resolution invariance, the point of the feature: one small Gaussian keeps its total alpha across a 4x zoom only with AA;
   5. equivalences: quantised == de-quantised, pruned == compacted, accumulate == sum of calls, quant.grads accumulates;
-  6. translating / rotating the world together with the camera cancels against the camera gradients;
-  7. the same bytes on every run and stream, P = 0 and R = 0, a second device;
-  8. 90 Adam steps through render() with pipe.antialiasing reduce the loss.
+  6. a second device.
+Translation / rotation invariance with the camera, the same bytes on every run and stream and P = 0 / R = 0 are checked with and
+without anti-aliasing in test_gpu_camera.py, and Adam steps through render() with pipe.antialiasing in test_gpu_training.py.
 Observed maxima are printed (pytest -s)."""
 import math
 from functools import partial
@@ -18,6 +18,7 @@ import pytest
 import torch
 
 import ours as O
+import restate64 as R64
 from diff_gaussian_rasterization import _C
 from gs_b200 import synth
 from gs_b200.model import GaussianModelView
@@ -26,26 +27,13 @@ pytestmark = pytest.mark.gpu
 
 DEV = "cuda"
 F64 = torch.float64
-EMPTY = torch.Tensor([])
 H_DIL = 0.3
 
 
 def _config(name):
     """-> (scene, cam on DEV, prune_mask or None, quant or None)."""
-    if name == "c1":
-        W, H = synth.config_image("C1")
-        return synth.config_scene("C1"), synth.make_camera(W, H).to(DEV), None, None
-    W, H = 320, 200
-    box, ls = (1.9 * W / H, 1.9, 1.0), math.log(0.02)
-    if name == "mixed":
-        return synth.make_scene(20_000, 201, mixed_degrees=True, box=box, log_scale_mean=ls), O.yaw_cam(W, H, -5.0), None, None
-    if name == "quant":
-        scene = synth.make_scene(20_000, 202, mixed_degrees=True, box=box, log_scale_mean=ls)
-        return scene, O.yaw_cam(W, H, 4.0), None, synth.quantise_scene(scene)
-    if name == "pruned":
-        scene = synth.make_scene(20_000, 203, sh_degree=2, box=box, log_scale_mean=ls)
-        return scene, O.yaw_cam(W, H, -3.0), synth.prune_mask(scene.P, 204), None
-    raise ValueError(name)
+    scene, cam, prune, quant = O.scene_config("aa", name)
+    return scene, cam.to(DEV), prune, quant
 
 
 # every call here is anti-aliased unless it passes aa=False
@@ -63,21 +51,8 @@ def _rel(a, b):
 
 def _cov2D64(means, cov3D, cam):
     """Undilated screen covariance (a, b, c) in float64 from the kernel's own cov3D, following computeCov2D."""
-    V = cam.world_view_transform.to(DEV, F64)
-    m = means.to(DEV, F64)
-    t = torch.cat([m, torch.ones(m.shape[0], 1, dtype=F64, device=DEV)], 1) @ V
-    tanx, tany = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
-    fx, fy = cam.image_width / (2.0 * tanx), cam.image_height / (2.0 * tany)
-    tz = t[:, 2]
-    tx = (t[:, 0] / tz).clamp(-1.3 * tanx, 1.3 * tanx) * tz
-    ty = (t[:, 1] / tz).clamp(-1.3 * tany, 1.3 * tany) * tz
-    J00, J02, J11, J12 = fx / tz, -fx * tx / (tz * tz), fy / tz, -fy * ty / (tz * tz)
-    Wm = V[:3, :3]
-    T0 = Wm[None, :, 0] * J00[:, None] + Wm[None, :, 2] * J02[:, None]
-    T1 = Wm[None, :, 1] * J11[:, None] + Wm[None, :, 2] * J12[:, None]
-    c = cov3D.to(DEV, F64)
-    S = torch.stack([c[:, 0], c[:, 1], c[:, 2], c[:, 1], c[:, 3], c[:, 4], c[:, 2], c[:, 4], c[:, 5]], 1).view(-1, 3, 3)
-    return (torch.einsum("pi,pij,pj->p", T0, S, T0), torch.einsum("pi,pij,pj->p", T0, S, T1), torch.einsum("pi,pij,pj->p", T1, S, T1))
+    return R64.screen_cov(means.to(DEV, F64), cam.world_view_transform.to(DEV, F64), cov3D.to(DEV, F64), cam.image_width,
+                          cam.image_height, math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5))[2:]
 
 
 @pytest.mark.parametrize("name", ["c1", "quant", "pruned"])
@@ -113,62 +88,14 @@ def test_antialiasing_moves_nothing_but_the_opacity(name):
 
 # ---- 3. float64 restatement of the pipeline ----------------------------------------------------------------------------------
 
-_C0 = 0.28209479177387814
-_C1 = 0.4886025119029199
-_C2 = [1.0925484305920792, -1.0925484305920792, 0.31539156525252005, -1.0925484305920792, 0.5462742152960396]
-_C3 = [-0.5900435899266435, 2.890611442640554, -0.4570457994644658, 0.3731763325901154, -0.4570457994644658, 1.445305721320277,
-       -0.5900435899266435]
-
-
-def _sh_colour(sh, deg, d):
-    x, y, z = d[:, 0:1], d[:, 1:2], d[:, 2:3]
-    deg = deg.view(-1, 1)
-    r = _C0 * sh[:, 0]
-    r = r + (deg > 0) * (-_C1 * y * sh[:, 1] + _C1 * z * sh[:, 2] - _C1 * x * sh[:, 3])
-    xx, yy, zz, xy, yz, xz = x * x, y * y, z * z, x * y, y * z, x * z
-    r = r + (deg > 1) * (_C2[0] * xy * sh[:, 4] + _C2[1] * yz * sh[:, 5] + _C2[2] * (2 * zz - xx - yy) * sh[:, 6] +
-                         _C2[3] * xz * sh[:, 7] + _C2[4] * (xx - yy) * sh[:, 8])
-    r = r + (deg > 2) * (_C3[0] * y * (3 * xx - yy) * sh[:, 9] + _C3[1] * xy * z * sh[:, 10] + _C3[2] * y * (4 * zz - xx - yy) * sh[:, 11] +
-                         _C3[3] * z * (2 * zz - 3 * xx - 3 * yy) * sh[:, 12] + _C3[4] * x * (4 * zz - xx - yy) * sh[:, 13] +
-                         _C3[5] * z * (xx - yy) * sh[:, 14] + _C3[6] * x * (xx - 3 * yy) * sh[:, 15])
-    return r + 0.5
-
-
-def _cov3D_from(scales, rots):
-    r, x, y, z = rots.unbind(1)
-    R = torch.stack([1 - 2 * (y * y + z * z), 2 * (x * y - r * z), 2 * (x * z + r * y),
-                     2 * (x * y + r * z), 1 - 2 * (x * x + z * z), 2 * (y * z - r * x),
-                     2 * (x * z - r * y), 2 * (y * z + r * x), 1 - 2 * (x * x + y * y)], 1).view(-1, 3, 3)
-    M = R * scales[:, None, :]
-    S = M @ M.transpose(1, 2)
-    return torch.stack([S[:, 0, 0], S[:, 0, 1], S[:, 0, 2], S[:, 1, 1], S[:, 1, 2], S[:, 2, 2]], 1)
-
-
 def _render64(x, cam, bg, vis, tiles):
     """float64 AA forward of the visible Gaussians.  x: dict of float64 leaves (means, logit, view, proj, campos, and scales + rots or
     cov3D, sh + deg or colors).  tiles: per 16x16 tile the kernel's depth-sorted Gaussian ids.  -> (colour, invdepth, alpha, n_contrib,
     intermediates, margins)."""
     W, H = cam.image_width, cam.image_height
-    tanx, tany = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
-    P = x["means"].shape[0]
     m = x["means"]
-    mh = torch.cat([m, torch.ones(P, 1, dtype=F64, device=DEV)], 1)
-    t = mh @ x["view"]
-    tx, ty, tz = t[:, 0], t[:, 1], t[:, 2]
-    limx, limy = 1.3 * tanx, 1.3 * tany
-    rx, ry = tx / tz, ty / tz
-    txc = torch.where((rx >= -limx) & (rx <= limx), tx, (rx.clamp(-limx, limx) * tz).detach())
-    tyc = torch.where((ry >= -limy) & (ry <= limy), ty, (ry.clamp(-limy, limy) * tz).detach())
-    fx, fy = W / (2.0 * tanx), H / (2.0 * tany)
-    J00, J02, J11, J12 = fx / tz, -fx * txc / (tz * tz), fy / tz, -fy * tyc / (tz * tz)
-    Wm = x["view"][:3, :3]
-    T0 = Wm[None, :, 0] * J00[:, None] + Wm[None, :, 2] * J02[:, None]
-    T1 = Wm[None, :, 1] * J11[:, None] + Wm[None, :, 2] * J12[:, None]
-    cov = x["cov3D"] if "cov3D" in x else _cov3D_from(x["scales"], x["rots"])
-    S = torch.stack([cov[:, 0], cov[:, 1], cov[:, 2], cov[:, 1], cov[:, 3], cov[:, 4], cov[:, 2], cov[:, 4], cov[:, 5]], 1).view(P, 3, 3)
-    a = torch.einsum("pi,pij,pj->p", T0, S, T0)
-    b = torch.einsum("pi,pij,pj->p", T0, S, T1)
-    c = torch.einsum("pi,pij,pj->p", T1, S, T1)
+    cov = x["cov3D"] if "cov3D" in x else R64.cov3D_from(x["scales"], x["rots"])
+    mh, tz, a, b, c = R64.screen_cov(m, x["view"], cov, W, H, math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5))
     det0 = a * c - b * b
     A, C = a + H_DIL, c + H_DIL
     det1 = A * C - b * b
@@ -184,7 +111,7 @@ def _render64(x, cam, bg, vis, tiles):
     else:
         d = m - x["campos"]
         d = d / d.norm(dim=1, keepdim=True)
-        rgb = torch.clamp_min(_sh_colour(x["sh"], x["deg"], d), 0.0)
+        rgb = torch.clamp_min(R64.sh_colour(x["sh"], x["deg"], d), 0.0)
         rgb.retain_grad()
     invd = 1.0 / tz
     colour = torch.zeros(3, H, W, dtype=F64, device=DEV)
@@ -245,7 +172,7 @@ def test_antialiasing_against_a_float64_restatement(case):
     if case == "colors_precomp":
         extra["colors_precomp"] = torch.rand(scene.P, 3, generator=gen)
     if case == "cov3D_precomp":
-        extra["cov3D_precomp"] = _cov3D_from(scene.scales.to(F64), scene.rotations.to(F64)).float()
+        extra["cov3D_precomp"] = R64.cov3D_from(scene.scales.to(F64), scene.rotations.to(F64)).float()
     dbg = {}
     args, out = _forward(scene, cam, bg, extra=extra, maps=True, dbg=dbg)
     Gc = torch.zeros(3, H, W) if case == "maps_only" else torch.randn(3, H, W, generator=gen)
@@ -408,103 +335,7 @@ def test_aa_accumulate_equals_the_sum_of_two_calls_and_quant_grads_accumulate():
     assert _rel(first["opacity"], gq[2]) <= 1e-6 and _rel(first["scales"], gq[6]) <= 1e-6
 
 
-# ---- 6. camera through AA -----------------------------------------------------------------------------------------------------
-
-@pytest.mark.parametrize("name", ["c1", "quant"])
-def test_aa_translation_invariance_with_the_camera(name):
-    scene, cam, prune, quant = _config(name)
-    H, W = cam.image_height, cam.image_width
-    args, out = _forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), prune, quant)
-    g = _backward(args, out, synth.grad_image(W, H, 225).to(DEV), prune, quant, camera_grads=True)
-    gm, gv, gp, gc = g[3].to(F64), g[8].to(F64), g[9].to(F64), g[10].to(F64)
-    V, Pf = cam.world_view_transform.to(DEV, F64), cam.full_proj_transform.to(DEV, F64)
-    worst = 0.0
-    for k in range(3):
-        terms = [gm[:, k], gc[k:k + 1], -gv[3, :] * V[k, :], -gp[3, :] * Pf[k, :]]
-        s, scale = sum(float(x.sum()) for x in terms), sum(float(x.abs().sum()) for x in terms)
-        worst = max(worst, abs(s) / scale)
-        assert abs(s) <= 1e-5 * scale, (name, k, s, scale)
-    print(f"\n[antialias camera] translation {name}: max |sum| / sum|terms| = {worst:.3e}")
-
-
-def _skew(v):
-    x, y, z = v.tolist()
-    return torch.tensor([[0.0, -z, y], [z, 0.0, -x], [-y, x, 0.0]], dtype=F64, device=DEV)
-
-
-def _qmul(a, b):
-    aw, ax, ay, az = a.unbind(-1)
-    bw, bx, by, bz = b.unbind(-1)
-    return torch.stack([aw * bw - ax * bx - ay * by - az * bz, aw * bx + ax * bw + ay * bz - az * by,
-                        aw * by - ax * bz + ay * bw + az * bx, aw * bz + ax * by - ay * bx + az * bw], -1)
-
-
-def test_aa_rotation_invariance_with_the_camera():
-    scene, cam, _, _ = _config("mixed")
-    H, W = cam.image_height, cam.image_width
-    col = torch.rand(scene.P, 3, generator=torch.Generator().manual_seed(226))
-    args, out = _forward(scene, cam, torch.tensor([0.3, 0.2, 0.1], device=DEV), extra={"colors_precomp": col})
-    g = _backward(args, out, synth.grad_image(W, H, 227).to(DEV), camera_grads=True)
-    gm, gq, gv, gp = g[3].to(F64), g[7].to(F64), g[8].to(F64), g[9].to(F64)
-    m, q = scene.means3D.to(DEV, F64), scene.rotations.to(DEV, F64)
-    V, Pf = cam.world_view_transform.to(DEV, F64), cam.full_proj_transform.to(DEV, F64)
-    worst = 0.0
-    for k in range(3):
-        e = torch.zeros(3, dtype=F64, device=DEV)
-        e[k] = 1.0
-        S = _skew(e)
-        dq = _qmul(torch.cat([torch.zeros(1, dtype=F64, device=DEV), 0.5 * e]).expand_as(q), q)
-        terms = [(gm * (m @ S.T)).sum(1), (gq * dq).sum(1), (gv[:3, :] * (S @ V[:3, :])).reshape(-1), (gp[:3, :] * (S @ Pf[:3, :])).reshape(-1)]
-        s, scale = sum(float(x.sum()) for x in terms), sum(float(x.abs().sum()) for x in terms)
-        worst = max(worst, abs(s) / scale)
-        assert abs(s) <= 1e-5 * scale, (k, s, scale)
-    print(f"\n[antialias camera] rotation: max |sum| / sum|terms| = {worst:.3e}")
-
-
-# ---- 7. determinism and edges -------------------------------------------------------------------------------------------------
-
-def test_aa_is_deterministic_on_any_stream():
-    scene, _, _, _ = _config("mixed")
-    bg = torch.tensor([0.1, 0.3, 0.2], device=DEV)
-    big = O.yaw_cam(320, 200, 1.0)
-    _, f1 = _forward(scene, big, bg, maps=True)
-    _, f2 = _forward(scene, big, bg, maps=True)
-    assert all(O.same(f1[i], f2[i]) for i in (1, 2, 6, 7))
-    cam = O.yaw_cam(8, 4, 2.0)
-    G = torch.randn(3, 4, 8, generator=torch.Generator().manual_seed(228)).to(DEV)
-    args, out = _forward(scene, cam, bg, maps=True)
-    kw = dict(dL_dalpha=torch.ones(1, 4, 8, device=DEV), camera_grads=True)
-    first = _backward(args, out, G, **kw)
-    again = _backward(args, out, G, **kw)
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        a3, o3 = _forward(scene, cam, bg, maps=True)
-        other = _backward(a3, o3, G, **kw)
-    torch.cuda.current_stream().wait_stream(s)
-    torch.cuda.synchronize()
-    assert O.same(o3[1], out[1]) and O.same(o3[7], out[7])
-    for a, b, c in zip(first, again, other):
-        assert O.same(a, b) and O.same(a, c)
-
-
-def test_aa_empty_and_fully_culled_scenes_give_zeros():
-    W, H = 100, 60
-    cam = synth.make_camera(W, H).to(DEV)
-    bg = torch.tensor([0.25, 0.5, 0.75], device=DEV)
-    empty = synth.Scene(torch.zeros(0, 3), torch.zeros(0, 1), torch.zeros(0, 3), torch.zeros(0, 4), torch.zeros(0, 1, 3),
-                        torch.zeros(0, 1, dtype=torch.int32))
-    P = 33
-    means = torch.zeros(P, 3)
-    means[:, 2] = -9.0                                                          # behind the camera: R = 0
-    culled = synth.Scene(means, torch.zeros(P, 1), torch.full((P, 3), 0.1), torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1),
-                         torch.zeros(P, 1, 3), torch.zeros(P, 1, dtype=torch.int32))
-    for scene in (empty, culled):
-        args, out = _forward(scene, cam, bg, maps=True)
-        assert out[0] == 0 and float(out[6].abs().max()) == 0.0 and float(out[7].abs().max()) == 0.0
-        g = _backward(args, out, torch.ones(3, H, W), camera_grads=True, dL_dalpha=torch.ones(1, H, W, device=DEV))
-        assert all(float(t.abs().max()) == 0.0 for t in g if t.numel()), scene.P
-
+# ---- 6. a second device --------------------------------------------------------------------------------------------------------
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs a second GPU")
 def test_aa_on_a_second_device():
@@ -522,60 +353,3 @@ def test_aa_on_a_second_device():
         outs.append((out[1].cpu(), [t.cpu() for t in g]))
     assert O.same(outs[0][0], outs[1][0])
     assert all(O.same(a, b) for a, b in zip(outs[0][1], outs[1][1]))
-
-
-# ---- 8. training --------------------------------------------------------------------------------------------------------------
-
-class _Model:
-    def __init__(self, scene, dev):
-        self._xyz = scene.means3D.to(dev).clone().requires_grad_(True)
-        self._opacity = scene.opacity.to(dev).clone().requires_grad_(True)
-        self._log_scaling = torch.log(scene.scales.to(dev)).requires_grad_(True)
-        self._rotation = scene.rotations.to(dev).clone().requires_grad_(True)
-        self._features = scene.sh.to(dev).clone().requires_grad_(True)
-        self._degrees = scene.degrees.to(dev)
-        self.active_sh_degree = self.max_sh_degree = 3
-        self.per_band_count = [int((scene.degrees == d).sum()) for d in range(4)]
-
-    get_xyz = property(lambda s: s._xyz)
-    get_scaling = property(lambda s: torch.exp(s._log_scaling))
-    get_rotation = property(lambda s: torch.nn.functional.normalize(s._rotation))
-    get_features = property(lambda s: s._features)
-
-    def params(self):
-        return [self._xyz, self._opacity, self._log_scaling, self._rotation, self._features]
-
-
-def test_adam_steps_with_antialiasing_reduce_the_loss():
-    from gaussian_renderer import render
-    from utils.loss_utils import l1_ssim_loss
-    W, H = 256, 192
-    target = synth.make_scene(6_000, 231, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.02), M=16)
-    cams = [O.yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
-    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False, antialiasing=True)
-    bg = torch.tensor([0.1, 0.1, 0.1], device=DEV)
-    with torch.no_grad():
-        gts = [render(c, _Model(target, DEV), pipe, bg)["render"].clone() for c in cams]
-    g = torch.Generator().manual_seed(232)
-    start = synth.Scene(target.means3D + 0.01 * torch.randn(target.means3D.shape, generator=g),
-                        target.opacity + 0.5 * torch.randn(target.opacity.shape, generator=g),
-                        target.scales * torch.exp(0.2 * torch.randn(target.scales.shape, generator=g)),
-                        torch.nn.functional.normalize(target.rotations + 0.1 * torch.randn(target.rotations.shape, generator=g)),
-                        target.sh + 0.1 * torch.randn(target.sh.shape, generator=g), target.degrees)
-    model = _Model(start, DEV)
-    opt = torch.optim.Adam([{"params": [model._xyz], "lr": 2e-4}, {"params": [model._opacity], "lr": 5e-2},
-                            {"params": [model._log_scaling], "lr": 5e-3}, {"params": [model._rotation], "lr": 1e-3},
-                            {"params": [model._features], "lr": 1e-2}])
-    losses = []
-    for it in range(90):
-        k = it % len(cams)
-        opt.zero_grad(set_to_none=True)
-        loss = l1_ssim_loss(render(cams[k], model, pipe, bg)["render"], gts[k], 0.2)
-        loss.backward()
-        for p in model.params():
-            assert p.grad is not None and torch.isfinite(p.grad).all()
-        opt.step()
-        losses.append(float(loss.detach()))
-    first, last = sum(losses[:3]) / 3, sum(losses[-3:]) / 3
-    print(f"\n[antialias training] loss {first:.4f} -> {last:.4f}")
-    assert last < 0.8 * first, (first, last)

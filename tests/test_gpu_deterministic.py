@@ -19,7 +19,7 @@ import backward_edges as BE
 import ours as O
 from diff_gaussian_rasterization import _C
 from gs_b200 import densify, synth
-from test_gpu_fused_activations import NAMES, Model, _adam, _render, _yaw_cam
+from test_gpu_fused_activations import NAMES, Model, _adam, _render
 
 pytestmark = pytest.mark.gpu
 
@@ -109,7 +109,7 @@ def _raw_kw(W, H):
 def test_one_warp_identity_raw(aa):
     W, H = 8, 4
     m = Model(synth.make_scene(20_000, 15, mixed_degrees=True, box=(3.0, 1.9, 1.0), log_scale_mean=math.log(0.03)), 15)
-    cam = _yaw_cam(W, H, 1.0)
+    cam = O.yaw_cam(W, H, 1.0)
     out, raw = _raw_forward(m, cam, aa)
     dL = synth.grad_image(W, H, 3).to(DEV)
     a = _outs(_raw_backward(m, cam, out, raw, dL, aa, **_raw_kw(W, H)))
@@ -290,7 +290,7 @@ def test_dense_1m_reproducible_and_agrees(dense_1m, mode):
 def test_dense_1m_raw_reproducible_and_agrees(dense_1m):
     scene, c = dense_1m
     m = Model(scene, 15)
-    cam = _yaw_cam(W_FULL, H_FULL, 3.0)
+    cam = O.yaw_cam(W_FULL, H_FULL, 3.0)
     out, raw = _raw_forward(m, cam, aa=True)
     dL = synth.grad_image(W_FULL, H_FULL, 3).to(DEV)
     kw = _raw_kw(W_FULL, H_FULL)
@@ -377,7 +377,7 @@ def _train(fused_schedule, seed=5):
     torch.manual_seed(seed)                                   # the split children's samples (torch.normal) come from torch's generator
     W, H = 256, 192
     target = synth.make_scene(6_000, 71, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.04))
-    cams = [_yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
+    cams = [O.yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
     with torch.no_grad():
         gts = [_render(Model(target, 15, norm_range=(0.0, 0.0)), c, False)["render"].clone() for c in cams]
     g = torch.Generator().manual_seed(seed)

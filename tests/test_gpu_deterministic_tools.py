@@ -93,8 +93,7 @@ def test_colour_variance_goldens_under_the_torch_flag():
 
 
 def _dense_views(n, W=1920, H=1080):
-    from test_gpu_fused_activations import _yaw_cam
-    cams = [_yaw_cam(W, H, yaw) for yaw in np.linspace(-20.0, 20.0, n)]
+    cams = [O.yaw_cam(W, H, yaw) for yaw in np.linspace(-20.0, 20.0, n)]
     return dict(positions=torch.stack([c.camera_center for c in cams]), views=torch.stack([c.world_view_transform for c in cams]),
                 projs=torch.stack([c.full_proj_transform for c in cams]),
                 tanx=torch.tensor([math.tan(c.FoVx * 0.5) for c in cams]), tany=torch.tensor([math.tan(c.FoVy * 0.5) for c in cams]),
@@ -320,9 +319,8 @@ def _codebook(values, inverse=lambda x: x, num_clusters=256, tol=0.0001):
 
 def _pipeline(out_dir, tag):
     from test_gpu_deterministic import _train
-    from test_gpu_fused_activations import _yaw_cam
     m, _ = _train(lambda it: it % 2 == 0)
-    cams = [_yaw_cam(256, 192, yaw) for yaw in (-10.0, 0.0, 10.0)]
+    cams = [O.yaw_cam(256, 192, yaw) for yaw in (-10.0, 0.0, 10.0)]
     deg_before = m._degrees.clone()
     # thresholds from the statistics themselves, so that a good share of the Gaussians loses bands
     with torch.no_grad():

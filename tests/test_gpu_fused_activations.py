@@ -16,11 +16,11 @@ model's get_scaling / get_rotation / get_features properties (autograd through t
 import math
 from types import SimpleNamespace
 
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+import ours as O
 from diff_gaussian_rasterization import _C
 from gs_b200 import densify, synth
 from gs_b200.optim import GaussianAdam
@@ -72,26 +72,8 @@ def _pipe(fused, aa=False):
     return SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False, fused_activations=fused, antialiasing=aa)
 
 
-def _yaw_cam(W, H, deg=0.0, grad=False):
-    th = math.radians(deg)
-    Rc2w = np.array([[math.cos(th), 0, math.sin(th)], [0, 1, 0], [-math.sin(th), 0, math.cos(th)]])
-    Cc = Rc2w @ np.array([0.0, 0.0, -4.0])
-    c = synth.make_camera(W, H, Rc2w, -Rc2w.T @ Cc).to(DEV)
-    t = (lambda x: x.detach().clone().requires_grad_()) if grad else (lambda x: x)
-    return SimpleNamespace(FoVx=c.FoVx, FoVy=c.FoVy, image_height=H, image_width=W, world_view_transform=t(c.world_view_transform),
-                           full_proj_transform=t(c.full_proj_transform), camera_center=t(c.camera_center))
-
-
 def _scene(P, W, H, seed, mixed=True, ls=math.log(0.02)):
     return synth.make_scene(P, seed, mixed_degrees=mixed, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=ls)
-
-
-def _bits(t):
-    return t.contiguous().view(torch.int32) if t.dtype == torch.float32 else t
-
-
-def _same(a, b):
-    return a is not None and b is not None and a.shape == b.shape and torch.equal(_bits(a), _bits(b))
 
 
 def _render(m, cam, fused, aa=False, **kw):
@@ -137,9 +119,9 @@ def _check_forward(m, cam, aa, prune=None):
     torch.cuda.synchronize()
     assert o0[0] == o1[0] and o0[0] > 0
     for k in (1, 2, 6, 7):
-        assert _same(o0[k], o1[k]), k
+        assert O.same(o0[k], o1[k]), k
     for k in d0:
-        assert _same(d0[k], d1[k]), k
+        assert O.same(d0[k], d1[k]), k
 
 
 @pytest.mark.parametrize("aa", [False, True])
@@ -148,7 +130,7 @@ def test_forward_bit_identical(Cn, aa):
     W, H = 320, 200
     m = Model(_scene(20_000, W, H, 300 + Cn), Cn, seed=Cn)
     prune = synth.prune_mask(m._xyz.shape[0], 7).to(DEV) if Cn in (3, 15) else None
-    _check_forward(m, _yaw_cam(W, H, -4.0), aa, prune)
+    _check_forward(m, O.yaw_cam(W, H, -4.0), aa, prune)
 
 
 @pytest.mark.parametrize("size", ["c1", "100k_1080p"])
@@ -163,7 +145,7 @@ def test_forward_bit_identical_sizes(size):
         Cn = 15
     m = Model(scene, Cn, seed=5)
     for aa in (False, True):
-        _check_forward(m, _yaw_cam(W, H, 3.0), aa)
+        _check_forward(m, O.yaw_cam(W, H, 3.0), aa)
 
 
 def test_forward_tiny_and_zero_quaternions():
@@ -172,7 +154,7 @@ def test_forward_tiny_and_zero_quaternions():
     with torch.no_grad():
         m._rotation[:50] *= 1e-14                # below the 1e-12 clamp of F.normalize
         m._rotation[50:60] = 0
-    _check_forward(m, _yaw_cam(W, H), False)
+    _check_forward(m, O.yaw_cam(W, H), False)
 
 
 # ---- 2. gradients ---------------------------------------------------------------------------------------------------------------
@@ -211,11 +193,11 @@ def _compare(names, ga, gb, tol=1e-5, tag="", exact=EXACT, floor=None):
         else:
             tol_n = tol
         if name in exact:
-            assert _same(a, b), name
+            assert O.same(a, b), name
         else:
             err = _rel(a, b)
             print(f"{tag} {name:16s} max |fused - activated| / max |activated| = {err:.3e}, "
-                  f"{int((_bits(a) != _bits(b)).sum())} of {a.numel()} differ" + (f" (run-to-run {floor[name]:.3e})" if floor else ""))
+                  f"{int((O.bits(a) != O.bits(b)).sum())} of {a.numel()} differ" + (f" (run-to-run {floor[name]:.3e})" if floor else ""))
             assert err <= tol_n, (name, err)
 
 
@@ -235,7 +217,7 @@ ALL = NAMES + ("view", "proj", "campos", "means2D")
 def test_single_tile_gradients(Cn, size, aa):
     W, H = size
     m = Model(_scene(3_000, W, H, 50 + Cn, ls=math.log(0.05)), Cn, seed=Cn)
-    cam, loss = _yaw_cam(W, H, 2.0, grad=True), _loss_all(_weights(W, H, 9))
+    cam, loss = O.yaw_cam(W, H, 2.0, grad=True), _loss_all(_weights(W, H, 9))
     (m0, c0, p0), (m1, c1, p1) = _both(m, cam, aa, loss, return_maps=True)
     assert int((p0["radii"] > 0).sum()) > 100
     one_warp = W * H <= 32
@@ -247,7 +229,7 @@ def test_single_tile_gradients(Cn, size, aa):
 def test_fullsize_gradients():
     W, H = 1920, 1080
     m = Model(_scene(100_000, W, H, 61, ls=math.log(0.01)), 15, seed=4)
-    cam, loss = _yaw_cam(W, H, 2.0, grad=True), _loss_all(_weights(W, H, 3))
+    cam, loss = O.yaw_cam(W, H, 2.0, grad=True), _loss_all(_weights(W, H, 3))
     (m0, c0, p0), (m1, c1, p1) = _both(m, cam, False, loss, return_maps=True)
     floor = {n: 4 * v for n, v in _floor(m, cam, False, loss, ALL, return_maps=True).items()}
     _compare(ALL, _grads(m0, c0) + [p0["viewspace_points"].grad], _grads(m1, c1) + [p1["viewspace_points"].grad], tag="1080p",
@@ -259,7 +241,7 @@ def test_fullsize_gradients():
 def test_graph_holds_no_activation_nodes():
     W, H = 64, 48
     m = Model(_scene(2_000, W, H, 71), 15)
-    pkg = _render(m, _yaw_cam(W, H), True)
+    pkg = _render(m, O.yaw_cam(W, H), True)
     seen, stack, names, leaves = set(), [pkg["render"].grad_fn], [], set()
     while stack:
         fn = stack.pop()
@@ -282,7 +264,7 @@ def test_invdepth_only_loss():
     W, H = 8, 4
     m = Model(_scene(3_000, W, H, 81, ls=math.log(0.05)), 15)
     w = _weights(W, H, 4)[1]
-    (m0, _, _), (m1, _, _) = _both(m, _yaw_cam(W, H), False, lambda p: (p["invdepth"] * w).sum(), return_maps=True)
+    (m0, _, _), (m1, _, _) = _both(m, O.yaw_cam(W, H), False, lambda p: (p["invdepth"] * w).sum(), return_maps=True)
     _compare(NAMES, [p.grad for p in m0.leaves()], [p.grad for p in m1.leaves()], tag="invdepth-only")
     assert float(m1._features_rest.grad.abs().max()) == 0.0 and float(m1._scaling.grad.abs().max()) > 0
 
@@ -296,11 +278,11 @@ def test_override_color():
     for fused in (False, True):
         mm = m.clone()
         col = colors.clone().requires_grad_()
-        pkg = _render(mm, _yaw_cam(W, H), fused, override_color=col)
+        pkg = _render(mm, O.yaw_cam(W, H), fused, override_color=col)
         (pkg["render"] * w).sum().backward()
         outs.append((mm, col, pkg))
     (m0, col0, p0), (m1, col1, p1) = outs
-    assert _same(p0["render"], p1["render"]) and _same(col0.grad, col1.grad)
+    assert O.same(p0["render"], p1["render"]) and O.same(col0.grad, col1.grad)
     assert int((p0["radii"] > 0).sum()) > 100
     assert m1._features_dc.grad is None and m1._features_rest.grad is None
     _compare(("_xyz", "_opacity", "_scaling", "_rotation"), [getattr(m0, n).grad for n in ("_xyz", "_opacity", "_scaling", "_rotation")],
@@ -311,7 +293,7 @@ def test_lambda_sh_sparsity():
     W, H = 8, 4
     m = Model(_scene(3_000, W, H, 83, ls=math.log(0.05)), 15)
     w = _weights(W, H, 6)[0]
-    (m0, _, _), (m1, _, p1) = _both(m, _yaw_cam(W, H), False, lambda p: (p["render"] * w).sum(), lambda_sh_sparsity=0.5)
+    (m0, _, _), (m1, _, p1) = _both(m, O.yaw_cam(W, H), False, lambda p: (p["render"] * w).sum(), lambda_sh_sparsity=0.5)
     # the sign term's addition may fuse with the colour term differently in the raw kernel: the rest gradients agree to rounding
     _compare(NAMES, [p.grad for p in m0.leaves()], [p.grad for p in m1.leaves()], tag="lambda_sh_sparsity",
              exact=("_features_dc", "_opacity"))
@@ -337,7 +319,7 @@ def _c_raw_backward(m, cam, out, dL, acc=None):
 def test_c_accumulate_is_the_sum_of_two_views():
     W, H = 8, 4                                        # one warp: every backward has one addition order
     m = Model(_scene(3_000, W, H, 84, ls=math.log(0.05)), 8)
-    cams = [_yaw_cam(W, H, -1.0), _yaw_cam(W, H, 1.0)]
+    cams = [O.yaw_cam(W, H, -1.0), O.yaw_cam(W, H, 1.0)]
     outs = [_c_forward(m, c, True, False) for c in cams]
     dLs = [synth.grad_image(W, H, s).to(DEV) for s in (1, 2)]
     g1 = [t.clone() if t is not None else None for t in _c_raw_backward(m, cams[0], outs[0], dLs[0])]
@@ -364,11 +346,11 @@ def test_empty_scene_and_no_instance():
             with torch.no_grad():
                 m._xyz[:, 2] -= 100.0
         m1 = m.clone()
-        p1 = _render(m1, _yaw_cam(W, H), True)
+        p1 = _render(m1, O.yaw_cam(W, H), True)
         p1["render"].sum().backward()
         assert int(p1["radii"].sum()) == 0
         if P:
-            assert _same(p1["render"], _render(m.clone(), _yaw_cam(W, H), False)["render"])
+            assert O.same(p1["render"], _render(m.clone(), O.yaw_cam(W, H), False)["render"])
         for p in m1.leaves():
             assert p.grad is not None and p.grad.shape == p.shape and (p.numel() == 0 or float(p.grad.abs().max()) == 0.0)
 
@@ -380,7 +362,7 @@ def test_run_to_run_and_side_stream():
 
     def run():
         mm = m.clone()
-        pkg = _render(mm, _yaw_cam(W, H), True)
+        pkg = _render(mm, O.yaw_cam(W, H), True)
         (pkg["render"] * w).sum().backward()
         return [pkg["render"]] + [p.grad for p in mm.leaves()]
 
@@ -392,7 +374,7 @@ def test_run_to_run_and_side_stream():
     torch.cuda.current_stream().wait_stream(s)
     torch.cuda.synchronize()
     # the forward is the same bytes on every run and stream; the gradients to the render backward's atomic order
-    assert _same(a[0], b[0]) and _same(a[0], c[0])
+    assert O.same(a[0], b[0]) and O.same(a[0], c[0])
     for x, y, z in zip(a[1:], b[1:], c[1:]):
         assert _rel(y, x) <= 1e-4 and _rel(z, x) <= 1e-4
 
@@ -409,7 +391,7 @@ def test_25_adam_steps_agree():
     W, H = 8, 4
     m = Model(_scene(3_000, W, H, 91, ls=math.log(0.05)), 15)
     gt = torch.rand(3, H, W, device=DEV)
-    cam = _yaw_cam(W, H, 1.0)
+    cam = O.yaw_cam(W, H, 1.0)
     models = [m.clone(), m.clone()]
     opts = [_adam(mm) for mm in models]
     for _ in range(25):
@@ -433,7 +415,7 @@ def test_90_steps_reduce_the_loss():
     from utils.loss_utils import l1_ssim_loss
     W, H = 256, 192
     target = synth.make_scene(6_000, 71, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.04))
-    cams = [_yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
+    cams = [O.yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
     with torch.no_grad():
         gts = [_render(Model(target, 15, norm_range=(0.0, 0.0)), c, False)["render"].clone() for c in cams]
     g = torch.Generator().manual_seed(5)
@@ -468,7 +450,7 @@ def test_render_after_densify_uses_the_new_parameters():
     m.xyz_gradient_accum = torch.zeros(P, 1, device=DEV)
     m.denom = torch.zeros(P, 1, device=DEV)
     m.max_radii2D = torch.zeros(P, device=DEV)
-    cam = _yaw_cam(W, H)
+    cam = O.yaw_cam(W, H)
     pkg = _render(m, cam, True)
     (pkg["render"] * _weights(W, H, 8)[0]).sum().backward()
     m.optimizer.step()
@@ -488,7 +470,7 @@ def test_peak_memory_drops():
     W, H = 1920, 1080
     P = 1_000_000
     m = Model(_scene(P, W, H, 93, ls=math.log(0.004)), 15)
-    cam = _yaw_cam(W, H)
+    cam = O.yaw_cam(W, H)
     w = _weights(W, H, 9)[0]
     peaks = []
     for fused in (False, True, False, True):

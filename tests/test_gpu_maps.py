@@ -4,7 +4,8 @@ parity tests pin to the reference bit for bit.  Every check is a linear identity
   - alpha == 1 - final_T, and invdepth == channel 0 of a render with colour (1/depth, 0, 0) and no background, bitwise;
   - the maps' gradients == the sum of three existing backwards (colour; the 1/depth colour render, chained through
     d(1/z)/dmeans3D in torch; a zero-colour render with background (-1, 0, 0)), within 1e-4 of each array's magnitude;
-  - a few Adam steps on the means with an L1 loss on invdepth alone reduce that loss (sign and scale of the direct depth term)."""
+  - a few Adam steps on the means with an L1 loss on invdepth alone reduce that loss (sign and scale of the direct depth term).
+The maps of P = 0 and R = 0 scenes and their backward are checked with the other options' in test_gpu_camera.py."""
 import math
 from types import SimpleNamespace
 
@@ -26,24 +27,10 @@ EMPTY = torch.Tensor([])
 
 def _config(name):
     """-> (scene, cam, prune_mask or None, quant or None) on the CPU."""
-    if name == "c1":
-        W, H = synth.config_image("C1")
-        return synth.config_scene("C1"), synth.make_camera(W, H), None, None
-    if name == "hd":
-        W, H = 1920, 1080
-        scene = synth.make_scene(300_000, 81, mixed_degrees=True)
-        return scene, synth.make_camera(W, H), None, None
     if name == "staircase" or name.startswith("odd_"):
         case = BE.build(name)                       # the per-element backward's boundary scenes (tests/backward_edges.py)
         return case.scene, case.cam, None, None
-    W, H = 320, 200
-    if name == "quant":
-        scene = synth.make_scene(20_000, 82, mixed_degrees=True, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.03))
-        return scene, synth.make_camera(W, H), None, synth.quantise_scene(scene)
-    if name == "pruned":
-        scene = synth.make_scene(20_000, 83, sh_degree=2, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.03))
-        return scene, synth.make_camera(W, H), synth.prune_mask(scene.P, 84), None
-    raise ValueError(name)
+    return O.scene_config("maps", name)
 
 
 def _invdepth_colours(radii, depths):
@@ -109,28 +96,6 @@ def test_maps_of_the_variable_sh_entry_point():
     # the geometry is the dense path's: so are the maps
     _, dense = O.forward(scene, cam, bg, None, None, maps=True)
     assert torch.equal(mapped[6], dense[6]) and torch.equal(mapped[7], dense[7])
-
-
-def test_maps_of_empty_and_fully_culled_scenes():
-    W, H = 100, 60
-    cam = synth.make_camera(W, H).to(DEV)
-    bg = torch.tensor([0.25, 0.5, 0.75], device=DEV)
-    empty = synth.Scene(torch.zeros(0, 3), torch.zeros(0, 1), torch.zeros(0, 3), torch.zeros(0, 4), torch.zeros(0, 1, 3),
-                        torch.zeros(0, 1, dtype=torch.int32))
-    _, out = O.forward(empty, cam, bg, None, None, maps=True)
-    assert out[0] == 0 and out[6].shape == (1, H, W) and out[7].shape == (1, H, W)
-    assert float(out[6].abs().max()) == 0.0 and float(out[7].abs().max()) == 0.0
-    P = 33
-    means = torch.zeros(P, 3)
-    means[:, 2] = -9.0                                                       # behind the camera: every Gaussian is culled
-    culled = synth.Scene(means, torch.zeros(P, 1), torch.full((P, 3), 0.1), torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1),
-                         torch.zeros(P, 1, 3), torch.zeros(P, 1, dtype=torch.int32))
-    args, out = O.forward(culled, cam, bg, None, None, maps=True)
-    assert out[0] == 0 and int((out[2] > 0).sum()) == 0
-    assert float(out[6].abs().max()) == 0.0 and float(out[7].abs().max()) == 0.0
-    g = O.backward(args, out, torch.ones(3, H, W), None, None, dL_dinvdepth=torch.ones(1, H, W, device=DEV),
-                  dL_dalpha=torch.ones(1, H, W, device=DEV))
-    assert all(float(t.abs().max()) == 0.0 for t in g if t.numel())
 
 
 def _expected_grads(scene, cam, prune, quant, Gc, Gd, Ga):

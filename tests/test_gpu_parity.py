@@ -129,24 +129,21 @@ def test_edge_cases():
     bg = torch.tensor([0.25, 0.5, 0.75])
     E = torch.Tensor([])
 
-    def call(means, op, sc, rot, sh, deg):
-        return _C.rasterize_gaussians(bg.to(d), means.to(d), E, op.to(d), sc.to(d), rot.to(d), 1.0, E, cam.world_view_transform.to(d),
-                                      cam.full_proj_transform.to(d), math.tan(cam.FoVx * .5), math.tan(cam.FoVy * .5), H, W, sh.to(d),
-                                      deg.to(d), cam.camera_center.to(d), False, False)
+    def call(s):
+        return _C.rasterize_gaussians(bg.to(d), s.means3D.to(d), E, s.opacity.to(d), s.scales.to(d), s.rotations.to(d), 1.0, E,
+                                      cam.world_view_transform.to(d), cam.full_proj_transform.to(d), math.tan(cam.FoVx * .5),
+                                      math.tan(cam.FoVy * .5), H, W, s.sh.to(d), s.degrees.to(d), cam.camera_center.to(d), False, False)
+    empty, culled = ours.empty_and_culled_scenes()
     # P == 0 -> zero image WITHOUT background (rasterize_points.cu:184-185)
-    R, color, radii, *_ = call(torch.zeros(0, 3), torch.zeros(0, 1), torch.zeros(0, 3), torch.zeros(0, 4), torch.zeros(0, 1, 3),
-                               torch.zeros(0, 1, dtype=torch.int32))
+    R, color, radii, *_ = call(empty)
     assert R == 0 and float(color.abs().max()) == 0.0 and radii.numel() == 0
     # everything culled -> R == 0, pure background, backward gives zeros
-    P = 33
-    means = torch.zeros(P, 3); means[:, 2] = -9.0
-    q = torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1)
-    out = call(means, torch.zeros(P, 1), torch.full((P, 3), 0.1), q, torch.zeros(P, 1, 3), torch.zeros(P, 1, dtype=torch.int32))
+    out = call(culled)
     assert out[0] == 0 and torch.allclose(out[1], bg.to(d)[:, None, None].expand(3, H, W))
-    g = _C.rasterize_gaussians_backward(bg.to(d), means.to(d), out[2], E, torch.full((P, 3), 0.1).to(d), q.to(d), 1.0, E,
+    g = _C.rasterize_gaussians_backward(bg.to(d), culled.means3D.to(d), out[2], E, culled.scales.to(d), culled.rotations.to(d), 1.0, E,
                                         cam.world_view_transform.to(d), cam.full_proj_transform.to(d), math.tan(cam.FoVx * .5),
-                                        math.tan(cam.FoVy * .5), torch.ones(3, H, W).to(d), torch.zeros(P, 1, 3).to(d),
-                                        torch.zeros(P, 1, dtype=torch.int32).to(d), cam.camera_center.to(d), out[3], 0, out[4], out[5], 0.0, False)
+                                        math.tan(cam.FoVy * .5), torch.ones(3, H, W).to(d), culled.sh.to(d), culled.degrees.to(d),
+                                        cam.camera_center.to(d), out[3], 0, out[4], out[5], 0.0, False)
     assert all(float(t.abs().max()) == 0.0 for t in g)
     # one huge opaque Gaussian covering every tile + one tiny one; compare with the oracle
     means = torch.tensor([[0.0, 0.0, 0.0], [0.3, 0.2, -0.5]])

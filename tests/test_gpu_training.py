@@ -1,69 +1,43 @@
 """GPU: the differentiable path end to end — a few Adam steps through the drop-in packages (gaussian_renderer.render +
 utils.loss_utils.l1_ssim_loss, the loop body of the reference's train.py:93-155) must pull a perturbed scene back towards the
-images of the scene it was perturbed from.  This is a behavioural check of the gradients' SIGN and SCALE across all parameter
-groups (means, opacity logits, log-scales, quaternions, SH), complementary to the element-wise parity tests."""
+images of the scene it was perturbed from, without and with anti-aliasing (pipe.antialiasing).  This is a behavioural check of
+the gradients' SIGN and SCALE across all parameter groups (means, opacity logits, log-scales, quaternions, SH), complementary to
+the element-wise parity tests."""
 import math
-import os
-import sys
 from types import SimpleNamespace
 
 import pytest
 import torch
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.join(os.path.dirname(HERE), "reduced-3dgs_b200"))
-from gs_b200 import synth  # noqa: E402
+import ours as O
+from gs_b200 import synth
 
 pytestmark = pytest.mark.gpu
 
-
-class _Model:
-    """The attributes render() reads from the reference's GaussianModel, with the reference's activations
-    (scene/gaussian_model.py:141-158: exp for scales, normalize for rotations; opacity stays a logit)."""
-
-    def __init__(self, scene, dev):
-        self._xyz = scene.means3D.to(dev).clone().requires_grad_(True)
-        self._opacity = scene.opacity.to(dev).clone().requires_grad_(True)
-        self._log_scaling = torch.log(scene.scales.to(dev)).requires_grad_(True)
-        self._rotation = scene.rotations.to(dev).clone().requires_grad_(True)
-        self._features = scene.sh.to(dev).clone().requires_grad_(True)
-        self._degrees = scene.degrees.to(dev)
-        self.active_sh_degree = self.max_sh_degree = 3
-        self.per_band_count = [int((scene.degrees == d).sum()) for d in range(4)]
-
-    get_xyz = property(lambda s: s._xyz)
-    get_scaling = property(lambda s: torch.exp(s._log_scaling))
-    get_rotation = property(lambda s: torch.nn.functional.normalize(s._rotation))
-    get_features = property(lambda s: s._features)
-
-    def params(self):
-        return [self._xyz, self._opacity, self._log_scaling, self._rotation, self._features]
+# per case: target scene seed, its log-scale mean, perturbation seed
+_CASES = {False: (71, 0.04, 5), True: (231, 0.02, 232)}
 
 
-def test_adam_steps_reduce_the_loss():
+@pytest.mark.parametrize("antialiasing", [False, True], ids=["plain", "aa"])
+def test_adam_steps_reduce_the_loss(antialiasing):
     from gaussian_renderer import render
     from utils.loss_utils import l1_ssim_loss
     dev = torch.device("cuda")
     W, H = 256, 192
-    target_scene = synth.make_scene(6_000, 71, sh_degree=3, mixed_degrees=False, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.04), M=16)
-    cams = []
-    for yaw in (-10.0, 0.0, 10.0):
-        th = math.radians(yaw)
-        import numpy as np
-        Rc2w = np.array([[math.cos(th), 0, math.sin(th)], [0, 1, 0], [-math.sin(th), 0, math.cos(th)]])
-        C = Rc2w @ np.array([0.0, 0.0, -4.0])
-        cams.append(synth.make_camera(W, H, Rc2w, -Rc2w.T @ C).to(dev))
-    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
+    scene_seed, ls, seed = _CASES[antialiasing]
+    target_scene = synth.make_scene(6_000, scene_seed, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(ls), M=16)
+    cams = [O.yaw_cam(W, H, yaw) for yaw in (-10.0, 0.0, 10.0)]
+    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False, antialiasing=antialiasing)
     bg = torch.tensor([0.1, 0.1, 0.1], device=dev)
     with torch.no_grad():
-        gts = [render(c, _Model(target_scene, dev), pipe, bg)["render"].clone() for c in cams]
-    g = torch.Generator().manual_seed(5)
+        gts = [render(c, O.Model(target_scene, dev), pipe, bg)["render"].clone() for c in cams]
+    g = torch.Generator().manual_seed(seed)
     start = synth.Scene(target_scene.means3D + 0.01 * torch.randn(target_scene.means3D.shape, generator=g),
                         target_scene.opacity + 0.5 * torch.randn(target_scene.opacity.shape, generator=g),
                         target_scene.scales * torch.exp(0.2 * torch.randn(target_scene.scales.shape, generator=g)),
                         torch.nn.functional.normalize(target_scene.rotations + 0.1 * torch.randn(target_scene.rotations.shape, generator=g)),
                         target_scene.sh + 0.1 * torch.randn(target_scene.sh.shape, generator=g), target_scene.degrees)
-    model = _Model(start, dev)
+    model = O.Model(start, dev)
     opt = torch.optim.Adam([{"params": [model._xyz], "lr": 2e-4}, {"params": [model._opacity], "lr": 5e-2},
                             {"params": [model._log_scaling], "lr": 5e-3}, {"params": [model._rotation], "lr": 1e-3},
                             {"params": [model._features], "lr": 1e-2}])
@@ -79,6 +53,7 @@ def test_adam_steps_reduce_the_loss():
         opt.step()
         losses.append(float(loss.detach()))
     first, last = sum(losses[:3]) / 3, sum(losses[-3:]) / 3
+    print(f"\n[{'antialias ' if antialiasing else ''}training] loss {first:.4f} -> {last:.4f}")
     assert last < 0.8 * first, (first, last)
     # the densification statistic the reference reads after backward (train.py:139, gaussian_model.py:693-695) is populated
     assert pkg["viewspace_points"].grad is not None and float(pkg["viewspace_points"].grad[:, :2].norm(dim=1).max()) > 0
