@@ -324,6 +324,42 @@ GSB_API int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* c
                  float* dL_dcampos /* [3] or NULL */, char* workspace, const GsbRawParams* raw /* or NULL */,
                  const GsbRawGrads* raw_grads /* or NULL */, int32_t antialiasing, char* det_workspace, void* stream);
 
+/* Per-Gaussian feature channels (DESIGN.md §5l): features [P,F] fp32, composited exactly like a colour channel with background 0,
+ *   out[f](x,y) = sum_i features[i,f] * alpha_i * T_i
+ * over the (pixel, Gaussian) pairs of the colour image, with its alpha, T, 1/255 skip and T < 1e-4 stop and the colour kernel's
+ * arithmetic: channel f equals the colour channel of a colors_precomp render with bg = 0 and colour features[:,f], bit for bit.
+ * The pass reads the blobs of any forward (dense, quantised, raw, anti-aliased, maps, variable-SH inference) and runs no
+ * preprocess, binning or sort of its own; the forward's outputs and blobs are not modified.
+ *   gsb_forward_features:  reads features, writes out [F,H,W] (every element; zeros for P == 0 or no instance).  Same bytes on every run.
+ *   gsb_backward_features: the arguments of gsb_backward_deterministic plus `features`, whose dL_dout [F,H,W] is the gradient of the
+ *                          feature image.  It runs the backward of the colour image (and maps, camera, raw parameters as there), then
+ *                          adds the feature image's share: dL_dfeatures [P,F] (overwritten; zero rows for culled and pruned Gaussians)
+ *                          and, through alpha, the same per-Gaussian gradients the colour image reaches (dL_dopacity, dL_dmeans2D,
+ *                          dL_dmeans3D, dL_dscales / dL_drotations / dL_dcov3D, raw_grads, the camera); dL_dcolors and the SH
+ *                          gradients are the colour image's alone.  det_workspace must be NULL: the feature backward sums with float
+ *                          atomics.  With features NULL this is gsb_backward_deterministic.
+ * Errors (GSB_EINVAL, nothing launched): features NULL (forward), F outside 1..GSB_FEATURES_MAX, P < 0, R < 0, a bad image size, and
+ * with P > 0 a NULL blob, features, out (forward) or dL_dout / dL_dfeatures (backward); in the backward also a non-NULL det_workspace
+ * together with features, and every error of gsb_backward_deterministic. */
+#define GSB_FEATURES_MAX 256
+typedef struct GsbFeatures {
+	int32_t F;                   /* channels, 1..GSB_FEATURES_MAX                              */
+	const float* features;       /* [P,F]                                                      */
+	float* out;                  /* [F,H,W] forward output (unused by the backward)            */
+	const float* dL_dout;        /* [F,H,W] backward input (unused by the forward)             */
+	float* dL_dfeatures;         /* [P,F]   backward output (unused by the forward)            */
+} GsbFeatures;
+GSB_API int gsb_forward_features(const char* geom_blob, int32_t P, const char* binning_blob, int64_t num_rendered,
+                 const char* image_blob, int32_t width, int32_t height, const GsbFeatures* features, void* stream);
+GSB_API int gsb_backward_features(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
+                 const char* geom_blob, const char* binning_blob, const char* image_blob,
+                 const float* dL_dout_color /* [3,H,W] */, const GsbGrads* grads,
+                 const float* dL_dinvdepth /* [1,H,W] or NULL */, const float* dL_dalpha /* [1,H,W] or NULL */,
+                 float lambda_sh_sparsity, float* dL_dviewmatrix /* [16] or NULL */, float* dL_dprojmatrix /* [16] or NULL */,
+                 float* dL_dcampos /* [3] or NULL */, char* workspace, const GsbRawParams* raw /* or NULL */,
+                 const GsbRawGrads* raw_grads /* or NULL */, int32_t antialiasing, char* det_workspace /* NULL with features */,
+                 const GsbFeatures* features /* or NULL */, void* stream);
+
 /* present[i] = view-space z of means3D[i] > 0.2 (auxiliary.h:139-159). */
 GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
                      uint8_t* present, void* stream);

@@ -92,7 +92,7 @@ void prof_end(int kid, cudaStream_t stream)
 }
 static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter", "tile_sort_large", "unused4", "tile_sort", "unused6",
 	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad", "det_scan",
-	"det_gather", "det_clear" };
+	"det_gather", "det_clear", "features_forward", "features_backward" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
 int launch_mark_visible(int, const float*, const float*, uint8_t*, cudaStream_t);
@@ -193,6 +193,17 @@ static int check_maps_pair(const char* fn, const float* out_invdepth, const floa
 {
 	if ((out_invdepth == nullptr) != (out_alpha == nullptr))
 	{ set_error("%s: give both map outputs (invdepth and alpha) or neither", fn); return GSB_EINVAL; }
+	return GSB_OK;
+}
+
+// The feature pass's own arguments (gsb_forward_features / gsb_backward_features).
+static int check_features(const char* fn, const GsbFeatures* f, int P, bool backward)
+{
+	if (!f) { set_error("%s: features is NULL", fn); return GSB_EINVAL; }
+	if (f->F < 1 || f->F > GSB_FEATURES_MAX) { set_error("%s: F = %d channels; 1..%d are supported", fn, f->F, GSB_FEATURES_MAX); return GSB_EINVAL; }
+	if (P > 0 && !f->features) { set_error("%s: features->features is NULL", fn); return GSB_EINVAL; }
+	if (backward && P > 0 && (!f->dL_dout || !f->dL_dfeatures)) { set_error("%s: features->dL_dout / dL_dfeatures is NULL", fn); return GSB_EINVAL; }
+	if (!backward && !f->out) { set_error("%s: features->out is NULL", fn); return GSB_EINVAL; }
 	return GSB_OK;
 }
 
@@ -550,6 +561,7 @@ static int backward_impl(const BackwardRequest& r)
 	float* acc = reinterpret_cast<float*>(const_cast<char*>(r.geom_blob) + geom_state_bytes(P));
 	if (int e = r.deterministic ? launch_render_backward_deterministic(r, img, b, g, acc) : launch_render_backward(r, img, b, g, acc, nullptr, nullptr))
 		return e;
+	if (r.features) if (int e = launch_features_backward(img, b, g, P, W, H, *r.features, acc, stream)) return e;
 	if (int e = launch_preprocess_backward(r, g, acc)) return e;
 	if (r.want_cam())
 		if (int e = launch_camera_grad_finish(P, reinterpret_cast<float*>(r.cam_workspace), r.dL_dview, r.dL_dproj, r.dL_dcampos, stream)) return e;
@@ -641,6 +653,55 @@ int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* cam, int6
 	if (scene->P > 0 && R > 0 && !det_workspace) { set_error("backward_deterministic: det_workspace is NULL"); return GSB_EINVAL; }
 	if (int e = check_camera_workspace("backward_deterministic", r)) return e;
 	if (raw_grads && !raw) { set_error("backward_deterministic: raw_grads given without raw"); return GSB_EINVAL; }
+	if (raw) if (int e = check_backward_raw(scene, grads, raw, raw_grads)) return e;
+	return backward_impl(r);
+}
+
+int gsb_forward_features(const char* geom_blob, int32_t P, const char* binning_blob, int64_t R, const char* image_blob, int32_t W, int32_t H,
+	const GsbFeatures* features, void* stream_)
+{
+	if (int e = check_features("forward_features", features, P, false)) return e;
+	if (P < 0 || R < 0) { set_error("forward_features: P < 0 or num_rendered < 0"); return GSB_EINVAL; }
+	if (W <= 0 || H <= 0) { set_error("forward_features: bad image size %dx%d", W, H); return GSB_EINVAL; }
+	if (P > 0 && (!geom_blob || !binning_blob || !image_blob)) { set_error("forward_features: a blob is NULL"); return GSB_EINVAL; }
+	const cudaStream_t stream = (cudaStream_t)stream_;
+	if (P == 0)
+	{
+		// the forward of an empty scene allocates no blobs; its feature image is zero like its colour image
+		GSB_CUDA_OK(cudaMemsetAsync(features->out, 0, size_t(features->F) * W * H * sizeof(float), stream));
+		return GSB_OK;
+	}
+	GeomState g = GeomState::carve(const_cast<char*>(geom_blob), P);
+	BinningState b = BinningState::carve(const_cast<char*>(binning_blob), R);
+	ImageState img = ImageState::carve(const_cast<char*>(image_blob), W, H);
+	return launch_features_forward(img, b, g, W, H, *features, stream);
+}
+
+int gsb_backward_features(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
+	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
+	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
+	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
+	int32_t antialiasing, char* det_workspace, const GsbFeatures* features, void* stream)
+{
+	if (!features)
+	{
+		if (det_workspace)
+			return gsb_backward_deterministic(scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth,
+				dL_dalpha, lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace, raw, raw_grads, antialiasing, det_workspace,
+				stream);
+	}
+	if (int e = check_scene_arg("backward_features", scene)) return e;
+	if (features)
+	{
+		if (det_workspace) { set_error("backward_features: the feature backward has no deterministic form; det_workspace must be NULL"); return GSB_EINVAL; }
+		if (int e = check_features("backward_features", features, scene->P, true)) return e;
+	}
+	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
+	r.aa = antialiasing != 0; r.raw = raw; r.raw_grads = raw_grads; r.features = features; r.stream = (cudaStream_t)stream;
+	if (R < 0) { set_error("backward_features: num_rendered < 0"); return GSB_EINVAL; }
+	if (int e = check_camera_workspace("backward_features", r)) return e;
+	if (raw_grads && !raw) { set_error("backward_features: raw_grads given without raw"); return GSB_EINVAL; }
 	if (raw) if (int e = check_backward_raw(scene, grads, raw, raw_grads)) return e;
 	return backward_impl(r);
 }

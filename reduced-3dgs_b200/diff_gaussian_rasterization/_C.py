@@ -14,6 +14,9 @@ and rotations, and applies exp / F.normalize / the SH concatenation inside the k
 `deterministic` (backward) sums the per-Gaussian gradients in a fixed order: the same bytes on every run
 (gsb_backward_deterministic).  `calculate_colours_variance` and `kmeans_cuda` take the same keyword (None: torch's
 deterministic-algorithms flag) for their statistics and centre sums (gsb_forward_statistics_deterministic, gsb_kmeans_deterministic).
+`features` (forward, also of the variable-SH entry point) composites a [P, F] fp32 tensor of per-Gaussian features over the pairs of
+the colour image, with background 0, and appends the [F, H, W] image to the outputs (gsb_forward_features); the backward's `features`
+and `dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F] (gsb_backward_features).
 """
 from __future__ import annotations
 
@@ -23,8 +26,8 @@ import math
 import torch
 
 from gs_b200 import lib as _lib
-from gs_b200.lib import (GsbCamera, GsbDebug, GsbGrads, GsbQuant, GsbRawGrads, GsbRawParams, GsbScene, BlobAllocator, f32, on_device,
-                         ptr)
+from gs_b200.lib import (GsbCamera, GsbDebug, GsbFeatures, GsbGrads, GsbQuant, GsbRawGrads, GsbRawParams, GsbScene, BlobAllocator, f32,
+                         on_device, ptr)
 
 RAW_REST_COEFFS = (0, 3, 8, 15)     # _features_rest widths of max SH degree 0..3
 
@@ -68,6 +71,23 @@ def _quant_struct(quant, device, keep):
                  centers.data_ptr())
     keep.append(q)
     return C.pointer(q)
+
+
+def check_features(features, P, cuda=True):
+    """The checks of a `features` argument, made before anything runs: a [P, F] float32 tensor with 1 <= F <= FEATURES_MAX, on a CUDA
+    device unless `cuda` is False (then the caller checks the device later).  -> F."""
+    if not isinstance(features, torch.Tensor):
+        raise RuntimeError(f"features must be a [P, F] tensor, got {type(features).__name__}")
+    if features.dim() != 2 or int(features.shape[0]) != P:
+        raise RuntimeError(f"features must have shape [P, F] with P = {P} Gaussians, got {tuple(features.shape)}")
+    F = int(features.shape[1])
+    if not 1 <= F <= _lib.FEATURES_MAX:
+        raise RuntimeError(f"features has F = {F} channels; 1..{_lib.FEATURES_MAX} are supported")
+    if features.dtype != torch.float32:
+        raise RuntimeError(f"features must be float32, got {features.dtype}")
+    if cuda and not features.is_cuda:
+        raise RuntimeError("features must live on a CUDA device (no CPU path exists)")
+    return F
 
 
 def _present(t):
@@ -158,10 +178,13 @@ def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, 
 def _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
              tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug, packed_counts=None,
              prune_mask=None, quant=None, debug_out=None, statistics=None, return_maps=False, antialiasing=False, raw=None,
-             statistics_workspace=None):
+             statistics_workspace=None, features=None):
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")          # rasterize_points.cu:158-161
+    F = check_features(features, int(means3D.shape[0])) if features is not None else 0
     device = _device_of(means3D)
+    if features is not None and features.device != device:
+        raise RuntimeError(f"features must live on {device}, got {features.device}")
     raw_s = None
     if raw is not None:
         if packed_counts is not None or statistics is not None:
@@ -207,46 +230,56 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
             st = L.gsb_forward(*head, dbg_ptr, stream)
         geomB, binB, imgB = blobs.take("geom"), blobs.take("binning"), blobs.take("image")
         _lib.check(st)
+        feat_img = ()
+        if features is not None:
+            # the feature channels, composited from the blobs this forward left behind
+            feats = f32(features, device)
+            feat_img = (torch.empty((F, H, W), dtype=torch.float32, device=device),)
+            fs = GsbFeatures(F, ptr(feats), feat_img[0].data_ptr(), None, None)
+            _lib.check(L.gsb_forward_features(ptr(geomB), P, ptr(binB), int(R.value), ptr(imgB), W, H, C.byref(fs), stream))
         if debug:
             torch.cuda.synchronize(device)                      # reference CHECK_CUDA(debug) semantics, auxiliary.h:161-168
     if maps is not None:
-        return int(R.value), out_color, radii, geomB, binB, imgB, maps[0], maps[1]
-    return int(R.value), out_color, radii, geomB, binB, imgB
+        return (int(R.value), out_color, radii, geomB, binB, imgB, maps[0], maps[1]) + feat_img
+    return (int(R.value), out_color, radii, geomB, binB, imgB) + feat_img
 
 
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                         projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                        *, prune_mask=None, quant=None, debug_out=None, return_maps=False, antialiasing=False, raw=None):
+                        *, prune_mask=None, quant=None, debug_out=None, return_maps=False, antialiasing=False, raw=None, features=None):
     """rasterize_points.h:43-63 RasterizeGaussiansCUDA -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer).
     `return_maps`: -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer, invdepth [1,H,W], alpha [1,H,W]) with
     invdepth = sum (1/depth) * alpha * T over the pairs that composite the colour and alpha = 1 - final_T (gsb_forward_maps).
     `antialiasing`: opacity-compensated 2D filter (gsb_forward_antialiased); its buffers need the backward's `antialiasing=True`.
     `raw`: (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]), the model's leaf parameters, with sh, scales
     and rotations empty; the kernels read them in place and activate them (gsb_forward_raw).  With colors, features_dc and
-    features_rest are None.  The same output bits as the activated call on cat(dc, rest), exp(scaling), F.normalize(rotation)."""
+    features_rest are None.  The same output bits as the activated call on cat(dc, rest), exp(scaling), F.normalize(rotation).
+    `features`: [P, F] fp32 on the device, 1 <= F <= 256; the tuple ends with the [F, H, W] feature image, each channel composited
+    like a colour channel with background 0 (gsb_forward_features).  Every other output is the call's without it."""
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                     projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                    None, prune_mask, quant, debug_out, return_maps=return_maps, antialiasing=antialiasing, raw=raw)
+                    None, prune_mask, quant, debug_out, return_maps=return_maps, antialiasing=antialiasing, raw=raw, features=features)
 
 
 def rasterize_gaussians_variableSH_bands(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                                          viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh,
                                          perBandPrimitiveCount, cumSumPrimitiveCount, coeffsNum, degrees, campos, prefiltered,
-                                         debug, *, prune_mask=None, debug_out=None, return_maps=False, antialiasing=False):
+                                         debug, *, prune_mask=None, debug_out=None, return_maps=False, antialiasing=False, features=None):
     """rasterize_points.h:18-41 RasterizeGaussiansVariableSHBandsCUDA (inference, packed per-degree SH groups).
     cumSumPrimitiveCount / coeffsNum are implied by perBandPrimitiveCount ([1,4,9,16] per gaussian_renderer:90-92).
-    `return_maps` and `antialiasing` as in rasterize_gaussians."""
+    `return_maps`, `antialiasing` and `features` as in rasterize_gaussians (forward only, like the rest of this path)."""
     counts = [int(v) for v in perBandPrimitiveCount.detach().cpu().tolist()]
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                     projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                    counts, prune_mask, None, debug_out, return_maps=return_maps, antialiasing=antialiasing)
+                    counts, prune_mask, None, debug_out, return_maps=return_maps, antialiasing=antialiasing, features=features)
 
 
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                                  projmatrix, tan_fovx, tan_fovy, dL_dout_color, sh, degrees, campos, geomBuffer, R,
                                  binningBuffer, imageBuffer, lambda_sh_sparsity, debug, *, prune_mask=None, quant=None,
                                  accumulate_into=None, want_conic=False, view_means2D=None, dL_dinvdepth=None, dL_dalpha=None,
-                                 camera_grads=False, antialiasing=False, raw=None, deterministic=False):
+                                 camera_grads=False, antialiasing=False, raw=None, deterministic=False, features=None,
+                                 dL_dfeatures_out=None):
     """rasterize_points.h:65-88 RasterizeGaussiansBackwardCUDA ->
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     `accumulate_into`: the same 8-tuple from a previous call; gradients are added in place (view-batch accumulation);
@@ -260,7 +293,18 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     the SH gradient split at coefficient 1, scaling / rotation chained through exp / F.normalize; dL_dcolors only with colors
     (else None), the SH gradients None with colors, and no dL_dcov3D.  `accumulate_into` takes that 9-tuple.
     `deterministic`: sum the per-Gaussian gradients in a fixed order instead of with float atomics (gsb_backward_deterministic):
-    the same inputs give the same bytes on every run, in every mode above; the values agree with the default path to rounding."""
+    the same inputs give the same bytes on every run, in every mode above; the values agree with the default path to rounding.
+    `features` / `dL_dfeatures_out`: the [P, F] features of the forward's `features` and the gradient of its [F, H, W] image; the
+    feature image's share of the gradients is added to every output above and the tuple ends with dL_dfeatures [P, F]
+    (gsb_backward_features).  Neither `accumulate_into` nor `deterministic` has a feature form: both are refused."""
+    feat_F = 0
+    if features is not None:
+        if accumulate_into is not None:
+            raise RuntimeError("features: the feature backward has no accumulate_into form (view-batch accumulation)")
+        if deterministic:
+            raise RuntimeError("features: the feature backward has no deterministic form; render the features without a gradient "
+                               "(torch.no_grad() or features.detach() and no loss on the image) or turn the deterministic mode off")
+        feat_F = check_features(features, int(means3D.shape[0]))
     device = _device_of(means3D)
     if raw is not None:
         want_sh = not _present(colors)
@@ -314,7 +358,19 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                 C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
                 *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4))
         stream = _lib.current_stream(device)
-        if deterministic:
+        dfeat = ()
+        if features is not None:
+            dLf = f32(dL_dfeatures_out, device)
+            if dLf is None or dLf.numel() != feat_F * H * W:
+                raise RuntimeError(f"dL_dfeatures_out must have F*H*W = {feat_F * H * W} elements")
+            feats = f32(features, device)
+            keep += [dLf, feats]
+            dfeat = (torch.empty((P, feat_F), dtype=torch.float32, device=device),)
+            fs = GsbFeatures(feat_F, ptr(feats), None, dLf.data_ptr(), ptr(dfeat[0]))
+            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
+            st = L.gsb_backward_features(*head, C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None,
+                                         int(bool(antialiasing)), None, C.byref(fs), stream)
+        elif deterministic:
             # per-instance partial slots, from the caching allocator on the current stream (freed in stream order after the call)
             det_ws = torch.empty(int(L.gsb_deterministic_workspace_bytes(P, int(R))), dtype=torch.uint8, device=device)
             rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
@@ -330,7 +386,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         if debug:
             torch.cuda.synchronize(device)
     res = tuple(outs) + ((conic,) if want_conic else ())
-    return res + tuple(cam_out[:3]) if camera_grads else res
+    return (res + tuple(cam_out[:3]) if camera_grads else res) + dfeat
 
 
 def calculate_colours_variance(cam_positions, means3D, opacity, scales, rotations, cam_viewmatrices, cam_projmatrices, tan_fovxs,

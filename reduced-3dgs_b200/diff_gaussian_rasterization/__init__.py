@@ -16,6 +16,9 @@ tensors (features_dc, features_rest, scaling, rotation) in place of shs / scales
 concatenation then run inside the kernels, and the gradients of the four tensors are the kernels' own outputs
 (_RasterizeGaussiansRaw).  GaussianRasterizationSettings' keyword-only `deterministic` (default: torch's deterministic-algorithms
 flag) selects the backward that sums each Gaussian's gradients in a fixed order (the same bytes on every run).
+GaussianRasterizer.forward's keyword-only `features` ([P, F] fp32, 1 <= F <= 256) appends the [F, H, W] image of per-Gaussian
+features composited over the colour pass with background 0; its gradient reaches the features and, through alpha, everything the
+colour gradient reaches.  The feature gradient has no deterministic form: it is refused when the deterministic mode is on.
 """
 from typing import NamedTuple
 
@@ -43,20 +46,26 @@ def _call(fn, args, kw, dump, message):
         raise ex
 
 
-def _apply(op, raster_settings, *args):
+def _apply(op, raster_settings, *args, features=None):
     camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
+    feat = () if features is None else (features,)
     if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera):
         # a learnable camera: the three tensors become inputs of the autograd op so that their gradients have a destination
-        return op.apply(*args, *camera)
-    return op.apply(*args)
+        return op.apply(*args, *camera, *feat)
+    # the features, when given, are the op's last input (after three absent camera slots)
+    return op.apply(*args, *((None,) * 3 + feat if feat else ()))
 
 
-def _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, camera, **kw):
+def _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, camera, features=None, **kw):
     """The forward both ops share: the _C call and the ctx state their backwards read.  `camera` is (viewmatrix, projmatrix,
     campos), raster_settings' own tensors, passed again as inputs only when the camera is learnable, else (None, None, None).
-    -> (_C.rasterize_gaussians' tuple, the op's outputs: (color, radii) or, with return_maps, (color, radii, invdepth, alpha))."""
+    -> (_C.rasterize_gaussians' tuple, the op's outputs: (color, radii) or, with return_maps, (color, radii, invdepth, alpha);
+    with `features` the feature image [F, H, W] comes last)."""
     ctx.camera_meta = None if camera[0] is None else [(t.shape, t.dtype) for t in camera]
+    ctx.return_maps, ctx.has_features = return_maps, features is not None
     kw.update(prune_mask=prune_mask, return_maps=return_maps, antialiasing=raster_settings.antialiasing)
+    if features is not None:
+        kw.update(features=features)
     out = _call(_C.rasterize_gaussians, args, kw,
                 "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
     ctx.raster_settings = raster_settings
@@ -64,11 +73,21 @@ def _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_
     ctx.lambda_sh_sparsity = lambda_sh_sparsity
     ctx.prune_mask = prune_mask
     ctx.mark_non_differentiable(out[2])
-    if return_maps:
-        # a loss on some outputs only: the others' gradients arrive as None and reach the kernels as NULL (zero)
+    feat = (out[-1],) if features is not None else ()
+    if return_maps or features is not None:
+        # a loss on some outputs only: the others' gradients arrive as None and reach the kernels as NULL (zero), and a feature
+        # image without a gradient leaves the backward exactly the call without features
         ctx.set_materialize_grads(False)
-        return out, (out[1], out[2], out[6], out[7])
-    return out, (out[1], out[2])
+    if return_maps:
+        return out, (out[1], out[2], out[6], out[7]) + feat
+    return out, (out[1], out[2]) + feat
+
+
+def _split_grads(ctx, grads):
+    """The incoming gradients after (color, radii) -> (grad_invdepth, grad_alpha, grad_features), None where absent."""
+    grads = list(grads)
+    maps = (grads.pop(0), grads.pop(0)) if ctx.return_maps else (None, None)
+    return maps + (grads.pop(0) if ctx.has_features else None,)
 
 
 def _deterministic(raster_settings):
@@ -79,14 +98,15 @@ def _deterministic(raster_settings):
 
 
 def _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp,
-              sh, degrees, geomBuffer, binningBuffer, imgBuffer, **kw):
+              sh, degrees, geomBuffer, binningBuffer, imgBuffer, features=None, grad_features=None, **kw):
     """The backward both ops share: the _C call from the saved state.  -> (its gradient tuple, the gradients of the camera
-    inputs: () for a constant camera, else one per tensor, None where not needed)."""
+    inputs: () for a constant camera, else one per tensor, None where not needed, dL_dfeatures or None)."""
     rs = ctx.raster_settings
     if grad_out_color is None:
         grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
-    # the camera tensors are the op's last three inputs when it has them
-    camera_need = ctx.needs_input_grad[-3:] if ctx.camera_meta is not None else (False, False, False)
+    # the camera tensors are the op's last three inputs when it has them (followed by the features when given)
+    n = len(ctx.needs_input_grad) - (1 if ctx.has_features else 0)
+    camera_need = ctx.needs_input_grad[n - 3:n] if ctx.camera_meta is not None else (False, False, False)
     args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
             rs.tanfovx, rs.tanfovy, grad_out_color, sh, degrees, rs.campos, geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer,
             ctx.lambda_sh_sparsity, rs.debug)
@@ -94,42 +114,51 @@ def _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, co
               antialiasing=rs.antialiasing)
     if _deterministic(rs):
         kw.update(deterministic=True)
+    if grad_features is not None:
+        kw.update(features=features, dL_dfeatures_out=grad_features)
     g = _call(_C.rasterize_gaussians_backward, args, kw,
               "snapshot_bw.dump", "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
+    dfeat = None
+    if grad_features is not None:
+        g, dfeat = g[:-1], g[-1]                                       # dL_dfeatures comes last
     if ctx.camera_meta is None:
-        return g, ()
+        # the features' gradient follows three absent camera slots
+        return g, (None,) * 3 if ctx.has_features else (), dfeat
     # with camera_grads the tuple ends with (dL_dviewmatrix, dL_dprojmatrix, dL_dcampos)
     return g, tuple(gc.reshape(shape).to(dtype) if n else None
-                    for gc, n, (shape, dtype) in zip(g[-3:] if any(camera_need) else (None,) * 3, camera_need, ctx.camera_meta))
+                    for gc, n, (shape, dtype) in zip(g[-3:] if any(camera_need) else (None,) * 3, camera_need, ctx.camera_meta)), dfeat
 
 
 def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False):
+                        raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, features=None):
     return _apply(_RasterizeGaussians, raster_settings, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations,
-                  cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps)
+                  cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features=features)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, viewmatrix=None,
-                projmatrix=None, campos=None):
+                projmatrix=None, campos=None, features=None):
         args = (raster_settings.bg, means3D, colors_precomp, opacities, scales, rotations, raster_settings.scale_modifier,
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, raster_settings.image_height, raster_settings.image_width, sh, degrees,
                 raster_settings.campos, raster_settings.prefiltered, raster_settings.debug)
         out, outputs = _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, (viewmatrix, projmatrix, campos),
-                                quant=quant)
+                                features, quant=quant)
         ctx.quant = quant
-        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, out[2], sh, out[3], out[4], out[5], degrees)
+        ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, out[2], sh, out[3], out[4], out[5], degrees,
+                              features)
         return outputs
 
     @staticmethod
-    def backward(ctx, grad_out_color, _, grad_invdepth=None, grad_alpha=None):
+    def backward(ctx, grad_out_color, _, *grads):
+        grad_invdepth, grad_alpha, grad_features = _split_grads(ctx, grads)
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer,
-         degrees) = ctx.saved_tensors
-        g, grad_camera = _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, scales, rotations,
-                                   cov3Ds_precomp, sh, degrees, geomBuffer, binningBuffer, imgBuffer, quant=ctx.quant)
+         degrees, features) = ctx.saved_tensors
+        g, grad_camera, grad_feat = _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, scales,
+                                              rotations, cov3Ds_precomp, sh, degrees, geomBuffer, binningBuffer, imgBuffer, features,
+                                              grad_features, quant=ctx.quant)
         (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
          grad_rotations) = g[:8]
         if ctx.quant is not None:
@@ -146,14 +175,15 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (grad_means3D, grad_means2D, grad_sh if need[2] else None, None,
                 grad_colors_precomp if need[4] else None, grad_opacities if need[5] else None,
                 grad_scales if need[6] else None, grad_rotations if need[7] else None,
-                grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None) + grad_camera
+                grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None) + grad_camera + \
+            ((grad_feat if need[-1] else None,) if ctx.has_features else ())
 
 
 def rasterize_gaussians_raw(means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
-                            raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False):
+                            raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, features=None):
     """rasterize_gaussians on the model's raw parameters (see _RasterizeGaussiansRaw)."""
     return _apply(_RasterizeGaussiansRaw, raster_settings, means3D, means2D, features_dc, features_rest, degrees, colors_precomp,
-                  opacities, scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps)
+                  opacities, scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, features=features)
 
 
 class _RasterizeGaussiansRaw(torch.autograd.Function):
@@ -164,7 +194,8 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
-                raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None):
+                raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None,
+                features=None):
         empty = torch.Tensor([])
         with_colors = colors_precomp.numel() > 0
         raw = (None, None, scaling, rotation) if with_colors else (features_dc, features_rest, scaling, rotation)
@@ -173,25 +204,27 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                 raster_settings.image_height, raster_settings.image_width, empty, degrees, raster_settings.campos,
                 raster_settings.prefiltered, raster_settings.debug)
         out, outputs = _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, (viewmatrix, projmatrix, campos),
-                                raw=raw)
+                                features, raw=raw)
         ctx.with_colors = with_colors
         ctx.save_for_backward(colors_precomp, means3D, features_dc, features_rest, scaling, rotation, out[2], out[3], out[4], out[5],
-                              degrees)
+                              degrees, features)
         return outputs
 
     @staticmethod
-    def backward(ctx, grad_out_color, _, grad_invdepth=None, grad_alpha=None):
+    def backward(ctx, grad_out_color, _, *grads):
+        grad_invdepth, grad_alpha, grad_features = _split_grads(ctx, grads)
         (colors_precomp, means3D, features_dc, features_rest, scaling, rotation, radii, geomBuffer, binningBuffer, imgBuffer,
-         degrees) = ctx.saved_tensors
+         degrees, features) = ctx.saved_tensors
         empty = torch.Tensor([])
         raw = (None, None, scaling, rotation) if ctx.with_colors else (features_dc, features_rest, scaling, rotation)
-        g, grad_camera = _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, empty, empty, empty,
-                                   empty, degrees, geomBuffer, binningBuffer, imgBuffer, raw=raw)
+        g, grad_camera, grad_feat = _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, empty, empty,
+                                              empty, empty, degrees, geomBuffer, binningBuffer, imgBuffer, features, grad_features, raw=raw)
         (grad_means2D, grad_colors, grad_opacities, grad_means3D, _, grad_dc, grad_rest, grad_scaling, grad_rotation) = g[:9]
         need = ctx.needs_input_grad
         return (grad_means3D, grad_means2D, grad_dc if need[2] else None, grad_rest if need[3] else None, None,
                 grad_colors if need[5] else None, grad_opacities if need[6] else None, grad_scaling if need[7] else None,
-                grad_rotation if need[8] else None, None, None, None, None) + grad_camera
+                grad_rotation if need[8] else None, None, None, None, None) + grad_camera + \
+            ((grad_feat if need[-1] else None,) if ctx.has_features else ())
 
 
 class _ReferenceSettings(NamedTuple):
@@ -246,12 +279,21 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, degrees=None, colors_precomp=None, scales=None,
                 rotations=None, cov3D_precomp=None, lambda_sh_sparsity=0., *, prune_mask=None, quant=None, return_maps=False,
-                raw_params=None):
+                raw_params=None, features=None):
         """-> (color, radii); with return_maps, (color, radii, invdepth [1,H,W], alpha [1,H,W]), all three differentiable.
         `raw_params`: (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]), the model's leaf tensors, in place
         of shs / scales / rotations (which must then be None, as must cov3D_precomp and quant); with colors_precomp the two
-        feature tensors are None.  The kernels apply exp / F.normalize / the concatenation and return the four gradients."""
+        feature tensors are None.  The kernels apply exp / F.normalize / the concatenation and return the four gradients.
+        `features`: [P, F] fp32 on the device, 1 <= F <= 256; the outputs end with the [F, H, W] feature image (each channel composited
+        like a colour channel with background 0), differentiable w.r.t. the features and, through alpha, the scene and the camera.
+        A feature gradient under the deterministic mode is refused (here when `features` requires grad, else in the backward)."""
         raster_settings = self.raster_settings
+        if features is not None:
+            _C.check_features(features, int(means3D.shape[0]), cuda=False)
+            if features.requires_grad and torch.is_grad_enabled() and _deterministic(raster_settings):
+                raise RuntimeError("features: the feature gradient has no deterministic form; detach the features or turn the "
+                                   "deterministic mode off")
+            _C.check_features(features, int(means3D.shape[0]))
         if raw_params is not None:
             if quant is not None or any(t is not None for t in (shs, scales, rotations, cov3D_precomp)):
                 raise Exception('raw_params replace shs, scales and rotations; leave those, cov3D_precomp and quant None')
@@ -270,6 +312,6 @@ class GaussianRasterizer(nn.Module):
         e = lambda t: empty if t is None else t                                  # absent inputs travel as empty tensors
         if raw_params is not None:
             return rasterize_gaussians_raw(means3D, means2D, e(features_dc), e(features_rest), degrees, e(colors_precomp), e(opacities),
-                                           scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps)
+                                           scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, features)
         return rasterize_gaussians(means3D, means2D, e(shs), degrees, e(colors_precomp), e(opacities), e(scales), e(rotations),
-                                   e(cov3D_precomp), raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps)
+                                   e(cov3D_precomp), raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features)

@@ -12,6 +12,9 @@ fused kernels when present; `return_maps=True` adds the inverse-depth and alpha 
 `_rotation`: exp, F.normalize and the SH concatenation run inside the kernels, which write the four gradients directly
 (DESIGN.md §5h).  It needs a GaussianModel-like `pc` whose scaling_activation is torch.exp and rotation_activation
 torch.nn.functional.normalize; the variable-SH inference path ignores it.
+`features` ([P, F] fp32 on the device, 1 <= F <= 256) adds pkg["features"], the [F, H, W] image of per-Gaussian features composited
+over the colour pass with background 0 (semantic features, normals, per-Gaussian statistics such as the SH degree or the opacity).
+It is differentiable w.r.t. the features and the scene on every path but the variable-SH inference one, which renders it forward only.
 
 A learnable camera needs no argument: when world_view_transform, full_proj_transform or camera_center requires grad, the
 rasterizer returns their gradients (the variable-SH inference path stays non-differentiable).  The rasterizer takes
@@ -78,7 +81,7 @@ def _raw_params(pc, pipe, override_color):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-           lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False, return_maps=False):
+           lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False, return_maps=False, features=None):
     """
     Render the scene.
 
@@ -155,16 +158,18 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
             raster_settings.image_height, raster_settings.image_width, shs, per_band_count, cumsum_count, coeffs_num,
             degrees, raster_settings.campos, raster_settings.prefiltered, raster_settings.debug, prune_mask=prune_mask,
-            return_maps=return_maps, antialiasing=raster_settings.antialiasing)
+            return_maps=return_maps, antialiasing=raster_settings.antialiasing, **({} if features is None else dict(features=features)))
         rendered_image, radii = out[1], out[2]
-        maps = out[6:]
+        maps = out[6:8] if return_maps else ()
+        feature_image = out[-1] if features is not None else None
     else:
         out = rasterizer(
             means3D=means3D, means2D=means2D, shs=shs, degrees=degrees, colors_precomp=colors_precomp, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, lambda_sh_sparsity=lambda_sh_sparsity,
-            prune_mask=prune_mask, quant=quant, return_maps=return_maps, raw_params=raw_params)
+            prune_mask=prune_mask, quant=quant, return_maps=return_maps, raw_params=raw_params, features=features)
         rendered_image, radii = out[0], out[1]
-        maps = out[2:]
+        maps = out[2:4] if return_maps else ()
+        feature_image = out[-1] if features is not None else None
     if measure_fps:
         end_timer.record()
         torch.cuda.synchronize()
@@ -179,4 +184,6 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
            "FPS": fps}
     if return_maps:
         pkg["invdepth"], pkg["alpha"] = maps
+    if features is not None:
+        pkg["features"] = feature_image
     return pkg

@@ -60,6 +60,13 @@ class GsbRawGrads(C.Structure):
                 ("dL_drotation", C.c_void_p)]
 
 
+class GsbFeatures(C.Structure):
+    _fields_ = [("F", C.c_int32), ("features", C.c_void_p), ("out", C.c_void_p), ("dL_dout", C.c_void_p), ("dL_dfeatures", C.c_void_p)]
+
+
+FEATURES_MAX = 256             # GSB_FEATURES_MAX
+
+
 class GsbAdamTensor(C.Structure):
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
                 ("numel", C.c_int64), ("row_width", C.c_int32), ("sh_offset", C.c_int32), ("one_minus_beta1", C.c_float),
@@ -194,6 +201,11 @@ def lib():
         L.gsb_deterministic_workspace_bytes.argtypes = [C.c_int32, C.c_int64]
         L.gsb_backward_deterministic.restype = C.c_int
         L.gsb_backward_deterministic.argtypes = L.gsb_backward_raw.argtypes[:-1] + [C.c_void_p, C.c_void_p]
+        L.gsb_forward_features.restype = C.c_int
+        L.gsb_forward_features.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32,
+                                           C.POINTER(GsbFeatures), C.c_void_p]
+        L.gsb_backward_features.restype = C.c_int
+        L.gsb_backward_features.argtypes = L.gsb_backward_deterministic.argtypes[:-1] + [C.POINTER(GsbFeatures), C.c_void_p]
         L.gsb_mark_visible.restype = C.c_int
         L.gsb_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_export_binning.restype = C.c_int
@@ -262,7 +274,8 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_forward_raw", "gsb_backward_raw", "gsb_deterministic_workspace_bytes", "gsb_backward_deterministic",
                     "gsb_statistics_workspace_bytes", "gsb_forward_statistics_deterministic",
                     "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic", "gsb_redundancy_workspace_bytes",
-                    "gsb_redundancy_score", "gsb_mercy_workspace_bytes", "gsb_mercy_plan"]
+                    "gsb_redundancy_score", "gsb_mercy_workspace_bytes", "gsb_mercy_plan",
+                    "gsb_forward_features", "gsb_backward_features"]
 
 
 def check(status: int):
