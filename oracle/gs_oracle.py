@@ -79,8 +79,9 @@ def mark_visible(means3D, viewmatrix):
 
 
 def preprocess(means3D, scales, scale_modifier, rotations, opacities, shs, degrees, cov3D_precomp, colors_precomp,
-               viewmatrix, projmatrix, campos, W, H, tan_fovx, tan_fovy, packed=None):
-    """forward.cu:354-456 (or :246-350 with packed=(coeffs_num, per_band_count, cumsum))."""
+               viewmatrix, projmatrix, campos, W, H, tan_fovx, tan_fovy, packed=None, antialiasing=False):
+    """forward.cu:354-456 (or :246-350 with packed=(coeffs_num, per_band_count, cumsum)).  `antialiasing`: conic_opacity[:, 3] is
+    o^ = sigmoid * s (the product's gsb_preprocess.cu, DESIGN.md §5e), and aa_sigmoid / aa_s / aa_q [P] hold sigmoid, s and q."""
     means3D = _np(means3D, np.float32)
     P = means3D.shape[0]
     scales, rotations = _np(scales, np.float32), _np(rotations, np.float32)
@@ -96,6 +97,9 @@ def preprocess(means3D, scales, scale_modifier, rotations, opacities, shs, degre
                cov3D=np.zeros((P, 6), np.float32), rgb=np.zeros((P, 3), np.float32),
                conic_opacity=np.zeros((P, 4), np.float32), tiles_touched=np.zeros(P, np.uint32),
                clamped=np.zeros((P, 3), np.uint8))
+    if antialiasing:
+        out.update(aa_sigmoid=np.zeros(P, np.float32), aa_s=np.zeros(P, np.float32), aa_q=np.zeros(P, np.float32))
+    aa = lambda k: _p(out.get(k), f32p)
     if packed is not None:
         cn, pbc, cs = [_np(a, np.int32) for a in packed]
     else:
@@ -107,7 +111,7 @@ def preprocess(means3D, scales, scale_modifier, rotations, opacities, shs, degre
                          0 if packed is None else 1, _p(cn, i32p), _p(pbc, i32p), _p(cs, i32p),
                          _p(out["radii"], i32p), _p(out["means2D"], f32p), _p(out["depths"], f32p), _p(out["cov3D"], f32p),
                          _p(out["rgb"], f32p), _p(out["conic_opacity"], f32p), _p(out["tiles_touched"], u32p),
-                         _p(out["clamped"], u8p))
+                         _p(out["clamped"], u8p), 1 if antialiasing else 0, aa("aa_sigmoid"), aa("aa_s"), aa("aa_q"))
     if colors_precomp is not None:
         out["rgb"] = colors_precomp
     if cov3D_precomp is not None:
@@ -336,7 +340,7 @@ def l1_ssim(image, gt, lambda_dssim=0.2):
 
 def forward(means3D, opacities, scales=None, rotations=None, shs=None, degrees=None, colors_precomp=None,
             cov3D_precomp=None, *, viewmatrix, projmatrix, campos, bg, W, H, tan_fovx, tan_fovy, scale_modifier=1.0,
-            packed=None, prune_mask=None):
+            packed=None, prune_mask=None, antialiasing=False):
     """Whole reference forward (rasterizer_impl.cu:359-504).  `prune_mask` (1 = pruned) is applied with the
     reference-equivalent semantics of SURVEY §8(b): run on the compacted set, scatter per-Gaussian outputs
     back to the original indices."""
@@ -348,9 +352,11 @@ def forward(means3D, opacities, scales=None, rotations=None, shs=None, degrees=N
         sub = lambda a: None if a is None else np.ascontiguousarray(_np(a)[keep])
         out = forward(sub(means3D), sub(opacities), sub(scales), sub(rotations), sub(shs), sub(degrees), sub(colors_precomp),
                       sub(cov3D_precomp), viewmatrix=viewmatrix, projmatrix=projmatrix, campos=campos, bg=bg, W=W, H=H,
-                      tan_fovx=tan_fovx, tan_fovy=tan_fovy, scale_modifier=scale_modifier)
+                      tan_fovx=tan_fovx, tan_fovy=tan_fovy, scale_modifier=scale_modifier, antialiasing=antialiasing)
         full = {}
-        for k in ("radii", "means2D", "depths", "cov3D", "rgb", "conic_opacity", "tiles_touched", "clamped"):
+        for k in ("radii", "means2D", "depths", "cov3D", "rgb", "conic_opacity", "tiles_touched", "clamped", "aa_sigmoid", "aa_s", "aa_q"):
+            if k not in out:
+                continue
             a = out[k]
             z = np.zeros((P,) + a.shape[1:], a.dtype)
             z[idx] = a
@@ -366,7 +372,7 @@ def forward(means3D, opacities, scales=None, rotations=None, shs=None, degrees=N
         # rasterize_points.cu:184-185: P == 0 returns the zero-initialised image (no background)
         return dict(num_rendered=0, color=np.zeros((3, H, W), np.float32), radii=np.zeros(0, np.int32))
     geom = preprocess(means3D, scales, scale_modifier, rotations, opacities, shs, degrees, cov3D_precomp, colors_precomp,
-                      viewmatrix, projmatrix, campos, W, H, tan_fovx, tan_fovy, packed)
+                      viewmatrix, projmatrix, campos, W, H, tan_fovx, tan_fovy, packed, antialiasing)
     binning = bin_and_sort(geom, W, H)
     img = render_forward(geom, binning, bgn, W, H)
     out = {}
@@ -378,9 +384,10 @@ def forward(means3D, opacities, scales=None, rotations=None, shs=None, degrees=N
 
 def backward(fwd, dL_dpix, means3D, scales, rotations, shs, degrees, *, viewmatrix, projmatrix, campos, bg, W, H,
              tan_fovx, tan_fovy, scale_modifier=1.0, lambda_sh_sparsity=0.0, f64=False, colors_precomp=None,
-             cov3D_precomp=None):
+             cov3D_precomp=None, antialiasing=False):
     """Whole reference backward (rasterizer_impl.cu:508-630) from the forward state `fwd`.
-    Returns the 8 gradients of rasterize_points.cu:304 (+ dL_dconic)."""
+    Returns the 8 gradients of rasterize_points.cu:304 (+ dL_dconic).  `antialiasing` needs a forward with antialiasing=True: the
+    backward differentiates o^ = sigmoid * s at that forward's fp32 sigmoid, s and q (DESIGN.md §5e)."""
     L = lib()
     means3D = _np(means3D, np.float32)
     P = means3D.shape[0]
@@ -411,7 +418,8 @@ def backward(fwd, dL_dpix, means3D, scales, rotations, shs, degrees, *, viewmatr
        _p(projmatrix, f32p), W, H, C.c_float(tan_fovx), C.c_float(tan_fovy), _p(campos, f32p),
        _p(g["dL_dmeans2D"], rp), _p(fwd["conic_opacity"], f32p), _p(g["dL_dconic"], rp), _p(g["dL_dopacity"], rp),
        _p(g["dL_dcolors"], rp), _p(g["dL_dmeans3D"], rp), _p(g["dL_dcov3D"], rp), _p(g["dL_dsh"], rp),
-       _p(g["dL_dscales"], rp), _p(g["dL_drotations"], rp), C.c_float(mult))
+       _p(g["dL_dscales"], rp), _p(g["dL_drotations"], rp), C.c_float(mult),
+       *[_p(fwd[k] if antialiasing else None, f32p) for k in ("aa_sigmoid", "aa_s", "aa_q")])
     return g
 
 

@@ -260,7 +260,20 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 			else if (a.cov3D_precomp) { for (int k = 0; k < 6; k++) cov3D[k] = a.cov3D_precomp[6 * idx + k]; }
 			else compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);   // the forward computed exactly this; recomputing is bit-identical
 			float dmean[3], dcov[6];
-			float aa_s = 1.f;                                                 // AA: the opacity factor s, recomputed from cov2D
+			float aa_s = 1.f, aa_q = 0.f;                                     // AA: the forward's opacity factor s and ratio q
+			// AA: s and the clamp decision are the forward's own bits: q is formed again from the same inputs with the forward's
+			// operation order (compute_cov2D_undilated, aa_det_ratio), not from the cov2D products below, whose association differs
+			// (on a needle-thin splat det0 cancels, and an unfused CPU emulation of those products moves s by up to 11 %).  Formed here,
+			// ahead of the cov2D chain; only q and s are kept (CAM + AA, IN = 0, ACC = false still spills 16 bytes, DESIGN.md §5e).
+			if constexpr (AA)
+			{
+				const float* v = a.view;
+				const float3 u = compute_cov2D_undilated(xform_row(v, 0, mx, my, mz), xform_row(v, 1, mx, my, mz), xform_row(v, 2, mx, my, mz),
+					a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, cov3D, v);
+				const float3 d1 = dilate_cov2D(u);
+				aa_q = aa_det_ratio(u, __fmaf_rn(d1.x, d1.z, -__fmul_rn(d1.y, d1.y)));
+				aa_s = __fsqrt_rn(fmaxf(GSB_AA_MIN_RATIO, aa_q));
+			}
 			// ---------------- computeCov2DCUDA, backward.cu:177-307 ----------------
 			{
 				const float* v = a.view;
@@ -305,13 +318,12 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				// cov2D (b the single off-diagonal parameter): dq/da = h (c^2 + h c + b^2) / det1^2, dq/dc = h (a^2 + h a + b^2) / det1^2,
 				// dq/db = -2 b h (a + c + h) / det1^2, and dL/dq = dL/do^ * sigmoid / (2 s) with sigmoid = o^ / s.  The terms are added
 				// whether or not the conic branch above was taken, and dcov (linear in dL/da, dL/db, dL/dc) is formed again from the sums.
+				// s and the clamp decision (aa_s, aa_q) were taken above from the forward's arithmetic.
 				if constexpr (AA)
 				{
 					const float ua = TV0[0] * T0[0] + TV0[1] * T0[1] + TV0[2] * T0[2];
 					const float uc = TV1[0] * T1[0] + TV1[1] * T1[1] + TV1[2] * T1[2];
-					const float q = (ua * uc - cb * cb) / denom;
-					aa_s = sqrtf(fmaxf(GSB_AA_MIN_RATIO, q));
-					if (q > GSB_AA_MIN_RATIO)
+					if (aa_q > GSB_AA_MIN_RATIO)
 					{
 						const float k = acc0.w * (opac / aa_s) * 0.3f / (2.f * aa_s * denom * denom);
 						dL_da += k * (uc * uc + 0.3f * uc + cb * cb);

@@ -17,6 +17,7 @@ import numpy as np
 import torch
 
 import gs_oracle
+import restate64 as R64
 from gs_b200 import synth
 
 GRAD_NAMES = ["dL_dmeans2D", "dL_dcolors", "dL_dopacity", "dL_dmeans3D", "dL_dcov3D", "dL_dsh", "dL_dscales", "dL_drotations"]
@@ -30,15 +31,28 @@ EXCLUDED_BAR = 1e-3
 # 4e-6 of the array's scale (dL_dconic; 2.5e-4 / 2.5e-6 in dL_dscales) on one H100, while the fp32 reference stays well below
 # that; the kernel recovers T with MUFU.RCP, not an IEEE division.  Every other case stays below 0.6 of the default bar.
 BAR_CASE = {"dense_faint": (1e-3, 1e-5)}                 # (R_REL, A_ABS)
+# aa_needles: on a needle whose det0 cancels (a c / det0 >= 1e2) dL_dmeans3D and dL_drotations are ill-conditioned in fp32: the
+# reference arithmetic itself errs by up to 8.5e-3 / 0.35 of the row there, and on one H100 the dL_drotations of a needle with
+# a c / det0 = 6e4 moved by 7 % between two runs (the render backward's atomic order), and one of 278 by 1.7e-3 of its row.  Those
+# two arrays of those needles are not checked per element (compare_aa); every other array of every needle is, and every array of
+# the 72 well-conditioned ones (a c / det0 < 1e2: the 48 bisected to the clamp, 25 clamped ones).
+AA_WELL_CONDITIONED = 1e2
+ILL_CONDITIONED_ARRAYS = ["dL_dmeans3D", "dL_drotations"]
 
 STAIRCASE = [1, 15, 16, 17, 31, 32, 33, 63, 64, 65, 127, 128, 129, 191, 192, 193, 255, 256, 257, 320, 511, 512, 513, 1000]
 TIE_TILE = STAIRCASE.index(129)             # the tile of the tie variant whose Gaussians all share one depth
 ODD_SIZES = [(1, 1), (3, 7), (8, 4), (15, 17), (17, 15), (20, 36), (33, 1)]
 DENSE = ["dense_4k", "dense_12k", "dense_40k", "dense_ties", "dense_faint"]
 CASES = (["staircase", "staircase_ties"] + ["odd_%dx%d" % s for s in ODD_SIZES] + ["large", "saturation"] + DENSE)
+# anti-aliased only (antialiasing=True, DESIGN.md §5e): needle-thin splats around the clamp of s, and sub-pixel splats (s << 1)
+AA_CASES = ["aa_needles", "aa_subpixel"]
+AA_MIN_RATIO = np.float32(2.5e-5)           # the clamp of q = det0 / det1 under s = sqrt(max(2.5e-5, q))
 # the share of the visible Gaussians a case may hold to the global bar instead of the per-element one (observed: see the CPU test)
 EXCLUDED_MAX = {"large": 0.02, "dense_4k": 0.10, "dense_12k": 0.10, "dense_40k": 0.10, "dense_ties": 0.10, "dense_faint": 0.10}
 EXCLUDED_DEFAULT = 0.05
+# with anti-aliasing (observed: see test_antialias_edges_oracle.py): odd_20x36's 420 small splats put 18 % of them next to a
+# borderline pixel once o^ = sigmoid * s is lower
+EXCLUDED_MAX_AA = {"odd_20x36": 0.20}
 
 
 class Case:
@@ -52,9 +66,10 @@ class Case:
                     tan_fovx=math.tan(c.FoVx * 0.5), tan_fovy=math.tan(c.FoVy * 0.5))
 
 
-def pixel_scene(cam, px, py, depth, sigma_px, logits, sh, g, aniso=None):
+def pixel_scene(cam, px, py, depth, sigma_px, logits, sh, g, aniso=None, rots=None):
     """Gaussians placed by their screen centre (px, py), view-space depth and screen-space standard deviation (before the 0.3
-    low-pass), on `cam`; random rotations (their 3D scales are `sigma_px * depth / focal` times `aniso`)."""
+    low-pass), on `cam`; random rotations unless `rots` [P,4] gives them (their 3D scales are `sigma_px * depth / focal` times
+    `aniso`)."""
     P = len(px)
     W, H = cam.image_width, cam.image_height
     tx, ty = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
@@ -68,6 +83,8 @@ def pixel_scene(cam, px, py, depth, sigma_px, logits, sh, g, aniso=None):
     scales = s[:, None] * (np.ones((P, 3)) if aniso is None else np.asarray(aniso, np.float64))
     q = torch.randn(P, 4, generator=g, dtype=torch.float64)
     q = q / q.norm(dim=1, keepdim=True)
+    if rots is not None:
+        q = torch.as_tensor(np.asarray(rots), dtype=torch.float64)
     sh = torch.as_tensor(np.asarray(sh), dtype=torch.float32)
     deg = int(round(math.sqrt(sh.shape[1]))) - 1
     return synth.Scene(torch.from_numpy(world[:, :3]).float().contiguous(), torch.as_tensor(np.asarray(logits), dtype=torch.float32).view(P, 1),
@@ -79,10 +96,15 @@ def _logit(p):
     return math.log(p / (1.0 - p))
 
 
-def _staircase(ties):
+def _aa_isotropic_s(sigma):
+    """s = sqrt(det0 / det1) of an isotropic splat of `sigma` px: sigma^2 / (sigma^2 + 0.3)."""
+    return sigma * sigma / (sigma * sigma + 0.3)
+
+
+def _staircase(ties, aa=False):
     """Tile t of a 6x4-tile image gets exactly STAIRCASE[t] faint Gaussians (2D radius <= 6 px, centred in the tile +-2 px, so
     their rect is that tile alone); opacity 0.0068..0.0082 keeps T above 2.7e-4 after 1 000 of them, so every tile's largest
-    n_contrib (`hi`) is its list length."""
+    n_contrib (`hi`) is its list length.  With `aa` the sigmoid is divided by s (isotropic estimate), so o^ stays in that range."""
     W, H = 96, 64
     cam = synth.make_camera(W, H)
     g = torch.Generator().manual_seed(1001 if ties else 1000)
@@ -96,6 +118,9 @@ def _staircase(ties):
         depth[tiles == TIE_TILE] = 4.25                    # exactly representable: the view-space depths are bit-identical
     sigma = 0.8 + 0.6 * u[:, 3]
     logits = _logit(0.0068) + (_logit(0.0082) - _logit(0.0068)) * u[:, 4]
+    if aa:
+        logits = np.log(1.0 / (1.0 + np.exp(-logits)) / _aa_isotropic_s(sigma))
+        logits = logits - np.log1p(-np.exp(logits))
     sh = torch.randn(P, 4, 3, generator=g).numpy()
     sh[:, 1:] *= 0.15
     scene = pixel_scene(cam, px, py, depth, sigma, logits, sh, g)
@@ -152,9 +177,10 @@ def _large():
     return Case("large", scene, cam, torch.tensor([0.1, 0.1, 0.2]), synth.grad_image(W, H, 3001), large=np.arange(Ns, P))
 
 
-def _saturation():
+def _saturation(aa=False):
     """Stacks of 40 Gaussians per tile, a third of them opaque (logit 8: alpha clamps at 0.99), so T < 1e-4 stops pixels partway
-    down the list; DC colours down to -3 clamp some channels at 0."""
+    down the list; DC colours down to -3 clamp some channels at 0.  With `aa` the splats are 8..16 px instead of 2..6 px: o^ =
+    sigmoid * s exceeds 0.99 only where s > 0.9904, i.e. above 5.5 px."""
     W, H = 80, 48
     cam = synth.make_camera(W, H)
     g = torch.Generator().manual_seed(4000)
@@ -164,14 +190,83 @@ def _saturation():
     px = 16 * (tiles % 5) + 8 + 10 * (u[:, 0] - 0.5)
     py = 16 * (tiles // 5) + 8 + 10 * (u[:, 1] - 0.5)
     depth = 2.5 + 4.0 * u[:, 2]
-    sigma = 2.0 + 4.0 * u[:, 3]
+    sigma = 8.0 + 8.0 * u[:, 3] if aa else 2.0 + 4.0 * u[:, 3]
     logits = np.where(u[:, 4] < 1.0 / 3.0, 8.0, torch.randn(P, generator=g, dtype=torch.float64).numpy())
     sh = 1.5 * torch.randn(P, 1, 3, generator=g).numpy() - 0.5
     scene = pixel_scene(cam, px, py, depth, sigma, logits, sh, g)
     return Case("saturation", scene, cam, torch.tensor([0.5, 0.2, 0.4]), synth.grad_image(W, H, 4001), lam=0.05)
 
 
-def dense_scene(kind):
+def _aa_needles():
+    """256x160, anti-aliased: 400 needles (scales (L, L t, L t), L 2..12 px, thinness t 1e-2..1e-4 log-uniform, random
+    rotations), whose det0 = a c - b^2 cancels (a c / det0 up to ~1e8) and whose q = det0 / det1 spans the clamp at 2.5e-5; plus
+    48 needles lying along the image's x or y axis (b ~ 0, no cancellation) whose width is bisected in fp32 until the forward's
+    q_f lies within 1e-3 relative of the clamp, half on each side.  Sigmoid 0.05..0.999, 60 % of it above 0.9."""
+    W, H = 256, 160
+    cam = synth.make_camera(W, H)
+    g = torch.Generator().manual_seed(6000)
+    Nr, Nt = 400, 48
+    P = Nr + Nt
+    u = torch.rand(P, 6, generator=g, dtype=torch.float64).numpy()
+    px, py = 8 + (W - 16) * u[:, 0], 8 + (H - 16) * u[:, 1]
+    depth = 3.0 + 5.0 * u[:, 2]
+    sigma = 2.0 + 10.0 * u[:, 3]
+    t = 10.0 ** (-2.0 - 2.0 * u[:, 4])
+    aniso = np.stack([np.ones(P), t, t], 1)
+    p = np.where(u[:, 5] < 0.6, 0.9 + 0.099 * u[:, 5] / 0.6, 0.05 + 0.85 * (u[:, 5] - 0.6) / 0.4)
+    logits = np.log(p / (1.0 - p))
+    sh = torch.randn(P, 4, 3, generator=g).numpy()
+    sh[:, 1:] *= 0.2
+    q = torch.randn(P, 4, generator=g, dtype=torch.float64).numpy()
+    q /= np.linalg.norm(q, axis=1, keepdims=True)
+    # the default camera looks along +z: a rotation about z by 0 or 90 degrees keeps the needle's long axis on an image axis
+    half = np.where(np.arange(Nt) % 2 == 0, 0.0, 0.25 * math.pi)
+    q[Nr:] = np.stack([np.cos(half), np.zeros(Nt), np.zeros(Nt), np.sin(half)], 1)
+    sigma[Nr:] = 4.0 + 4.0 * u[Nr:, 3]
+    # target q_f = 2.5e-5 (1 + d), d = +-(1e-5 .. 1e-3): bisect the width factor of each axis-aligned needle on the fp32 forward
+    d = np.where(np.arange(Nt) % 4 < 2, 1.0, -1.0) * 10.0 ** (-5.0 + 2.0 * u[Nr:, 4])
+    target = np.float64(AA_MIN_RATIO) * (1.0 + d)
+    lo, hi = np.full(Nt, -5.0), np.full(Nt, -2.0)                     # log10 of the thinness
+    kw = Case("", None, cam, None, None).cam_kw()
+    for _ in range(60):
+        mid = 0.5 * (lo + hi)
+        aniso[Nr:, 1] = aniso[Nr:, 2] = 10.0 ** mid
+        sub = pixel_scene(cam, px[Nr:], py[Nr:], depth[Nr:], sigma[Nr:], logits[Nr:], sh[Nr:], g, aniso[Nr:], q[Nr:])
+        o = gs_oracle.preprocess(sub.means3D, sub.scales, 1.0, sub.rotations, sub.opacity, sub.sh, sub.degrees, None, None,
+                                 kw["viewmatrix"], kw["projmatrix"], kw["campos"], W, H, kw["tan_fovx"], kw["tan_fovy"],
+                                 antialiasing=True)
+        up = o["aa_q"].astype(np.float64) < target
+        lo, hi = np.where(up, mid, lo), np.where(up, hi, mid)
+    aniso[Nr:, 1] = aniso[Nr:, 2] = 10.0 ** lo
+    up = np.arange(Nt) % 4 < 2
+    aniso[Nr:][up, 1:] = 10.0 ** hi[up, None]                          # the side of the target each one is meant to be on
+    scene = pixel_scene(cam, px, py, depth, sigma, logits, sh, g, aniso, q)
+    return Case("aa_needles", scene, cam, torch.tensor([0.2, 0.3, 0.4]), synth.grad_image(W, H, 6001), lam=0.05,
+                near=np.arange(Nr, P))
+
+
+def _aa_subpixel():
+    """192x128, anti-aliased: 600 splats of 0.05..0.5 px standard deviation (s = 0.008..0.45) with sigmoid 0.5..0.999, so that
+    o^ = sigmoid * s reaches 1/255 near their centres, over 60 of 2..5 px that they are composited with."""
+    W, H = 192, 128
+    cam = synth.make_camera(W, H)
+    g = torch.Generator().manual_seed(6100)
+    Ns, Nb = 600, 60
+    P = Ns + Nb
+    u = torch.rand(P, 5, generator=g, dtype=torch.float64).numpy()
+    px, py = W * u[:, 0], H * u[:, 1]
+    depth = 2.5 + 4.0 * u[:, 2]
+    sigma = np.concatenate([0.05 + 0.45 * u[:Ns, 3], 2.0 + 3.0 * u[Ns:, 3]])
+    aniso = 0.6 + 0.8 * torch.rand(P, 3, generator=g, dtype=torch.float64).numpy()
+    p = np.concatenate([0.5 + 0.499 * u[:Ns, 4], 0.1 + 0.5 * u[Ns:, 4]])
+    logits = np.log(p / (1.0 - p))
+    sh = torch.randn(P, 4, 3, generator=g).numpy()
+    sh[:, 1:] *= 0.2
+    scene = pixel_scene(cam, px, py, depth, sigma, logits, sh, g, aniso)
+    return Case("aa_subpixel", scene, cam, torch.tensor([0.1, 0.2, 0.3]), synth.grad_image(W, H, 6101))
+
+
+def dense_scene(kind, aa=False):
     """The sort-path scenes of test_gpu_parity.test_sort_paths_ties_and_dense_tiles -> (scene, cam, bg).  `dense_faint` is
     `dense_12k` with opacities around sigmoid(-5) = 0.0067: its pixels are not stopped by T, so the backward walks lists of
     more than 8 192 entries."""
@@ -199,33 +294,49 @@ def dense_scene(kind):
     op = torch.randn(P, 1, generator=g) - 2.0
     if kind == "dense_faint":
         op = 0.3 * op - 4.4                              # 0.3 * (N(0,1) - 2) - 4.4 = N(-5, 0.3)
+        if aa:
+            op = op + 3.0                                # s ~ 0.05 for these 0.1 px splats: sigmoid ~ 0.12 keeps o^ ~ 0.006
     sh = torch.randn(P, 1, 3, generator=g)
     deg = torch.zeros(P, 1, dtype=torch.int32)
     scene = synth.Scene(xyz.contiguous(), op, scales.contiguous(), q.contiguous(), sh, deg)
     return scene, synth.make_camera(W, H), torch.zeros(3)
 
 
-def build(name):
+def build(name, aa=False):
+    """The case `name`; `aa` builds the variant of a BE.CASES scene meant to be rendered with antialiasing=True (the AA_CASES
+    always are)."""
+    case = _build(name, aa)
+    case.meta["aa"] = aa or name in AA_CASES
+    return case
+
+
+def _build(name, aa):
+    if name == "aa_needles":
+        return _aa_needles()
+    if name == "aa_subpixel":
+        return _aa_subpixel()
     if name.startswith("staircase"):
-        return _staircase(name.endswith("ties"))
+        return _staircase(name.endswith("ties"), aa)
     if name.startswith("odd_"):
         W, H = (int(v) for v in name[4:].split("x"))
         return _odd(W, H)
     if name == "large":
         return _large()
     if name == "saturation":
-        return _saturation()
-    scene, cam, bg = dense_scene(name)
+        return _saturation(aa)
+    scene, cam, bg = dense_scene(name, aa)
     return Case(name, scene, cam, torch.tensor([0.2, 0.1, 0.3]), synth.grad_image(cam.image_width, cam.image_height, 5000))
 
 
 # ---- the oracle's side -------------------------------------------------------------------------------------------------------
 
-def oracle(case, dL=None, fwd=None):
-    """-> (forward state, fp64 backward, fp32 backward) of the oracle; `fwd` / `dL` override the state / dL/dpixel (near-misses)."""
+def oracle(case, dL=None, fwd=None, aa=False):
+    """-> (forward state, fp64 backward, fp32 backward) of the oracle, anti-aliased with `aa`; `fwd` / `dL` override the state /
+    dL/dpixel (near-misses)."""
     s = case.scene
-    o = fwd if fwd is not None else gs_oracle.forward(s.means3D, s.opacity, s.scales, s.rotations, s.sh, s.degrees, bg=case.bg, **case.cam_kw())
-    kw = dict(bg=case.bg, lambda_sh_sparsity=case.lam, **case.cam_kw())
+    o = fwd if fwd is not None else gs_oracle.forward(s.means3D, s.opacity, s.scales, s.rotations, s.sh, s.degrees, bg=case.bg,
+                                                      antialiasing=aa, **case.cam_kw())
+    kw = dict(bg=case.bg, lambda_sh_sparsity=case.lam, antialiasing=aa, **case.cam_kw())
     dL = case.dL if dL is None else dL
     o64 = gs_oracle.backward(o, dL, s.means3D, s.scales, s.rotations, s.sh, s.degrees, f64=True, **kw)
     o32 = gs_oracle.backward(o, dL, s.means3D, s.scales, s.rotations, s.sh, s.degrees, f64=False, **kw)
@@ -291,7 +402,7 @@ def excluded(case, o):
     return near | (touched & (stats["touched_pixels"] < 2000))
 
 
-def compare(name, o, o64, o32, got, chk, glob=None, verbose=True, bar=(R_REL, A_ABS)):
+def compare(name, o, o64, o32, got, chk, glob=None, verbose=True, bar=(R_REL, A_ABS), arrays=ARRAYS):
     """The per-element check of `got` (a dict of arrays) against the oracle on the Gaussians of mask `chk` -> (ratios, failures).
     The yardsticks are taken per Gaussian (row) of each array: E32 = max over the row of |o32 - o64| and |o64|_row = max over
     the row of |o64|, because the elements of a row share their rounding (they are chained from the same per-Gaussian sums):
@@ -303,7 +414,7 @@ def compare(name, o, o64, o32, got, chk, glob=None, verbose=True, bar=(R_REL, A_
     chk = chk & vis
     r_rel, a_abs = bar
     ratios, failures = {}, []
-    for n in ARRAYS:
+    for n in arrays:
         a = np.asarray(o64[n], np.float64).reshape(P, -1)
         if a.size == 0:
             continue
@@ -334,6 +445,25 @@ def compare(name, o, o64, o32, got, chk, glob=None, verbose=True, bar=(R_REL, A_
     return ratios, failures
 
 
+def well_conditioned(case, o):
+    """Visible Gaussians every gradient array of which compare_aa checks: on aa_needles those with a c / det0 < AA_WELL_CONDITIONED,
+    elsewhere all."""
+    vis = o["radii"] > 0
+    return vis & (cancellation(case, o) < AA_WELL_CONDITIONED) if case.name == "aa_needles" else vis
+
+
+def compare_aa(label, case, o, o64, o32, got, chk, glob=None, bar=(R_REL, A_ABS)):
+    """compare() of an anti-aliased backward: every array on the well-conditioned Gaussians, all but ILL_CONDITIONED_ARRAYS on the
+    others -> failures."""
+    well = well_conditioned(case, o)
+    _, failures = compare(label, o, o64, o32, got, chk & well, glob, bar=bar)
+    if (chk & ~well & (o["radii"] > 0)).any():
+        _, more = compare(label + ", a c / det0 >= %g" % AA_WELL_CONDITIONED, o, o64, o32, got, chk & ~well, bar=bar,
+                          arrays=[n for n in ARRAYS if n not in ILL_CONDITIONED_ARRAYS])
+        failures = failures + more
+    return failures
+
+
 def describe(failures, o, o64, got, W, H, limit=5):
     """Where the failures are: array, Gaussians, the tiles listing them and those tiles' `hi`."""
     tiles, hi = tile_of_instances(o, W), tile_hi(o, W, H)
@@ -362,6 +492,21 @@ def clamp_branch(case, o):
     return (o["radii"] > 0) & ((np.abs(tx / tz) > limx) | (np.abs(ty / tz) > limy))
 
 
+def cancellation(case, o):
+    """a c / det0 of the undilated screen covariance of every Gaussian, in float64 from the oracle's cov3D: how much of det0 =
+    a c - b^2 the fp32 forward loses to cancellation."""
+    kw = case.cam_kw()
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float64))
+    _, _, a, b, c = R64.screen_cov(t(case.scene.means3D.numpy()), t(kw["viewmatrix"].numpy()), t(o["cov3D"]), case.W, case.H,
+                                   kw["tan_fovx"], kw["tan_fovy"])
+    a, b, c = a.numpy(), b.numpy(), c.numpy()
+    with np.errstate(divide="ignore", invalid="ignore"):
+        return np.abs(a * c / (a * c - b * b))
+
+
+AA_MIN_CHECKED = 20                          # per AA property below: at least this many Gaussians checked per element
+
+
 def assert_reaches(case, o, excl):
     """What the case is built for, from the oracle's forward state (so a change to synth cannot quietly drop coverage)."""
     W, H = case.W, case.H
@@ -369,7 +514,10 @@ def assert_reaches(case, o, excl):
     hi = tile_hi(o, W, H)
     counts = (o["ranges"][:, 1] - o["ranges"][:, 0]).astype(np.int64)
     frac = excl[vis].mean() if vis.any() else 0.0
-    assert frac <= EXCLUDED_MAX.get(case.name, EXCLUDED_DEFAULT), (case.name, frac)
+    limit = EXCLUDED_MAX.get(case.name, EXCLUDED_DEFAULT)
+    if case.meta.get("aa"):
+        limit = EXCLUDED_MAX_AA.get(case.name, limit)
+    assert frac <= limit, (case.name, frac)
     if case.name.startswith("staircase"):
         k = case.meta["tile_k"]
         assert np.array_equal(o["tiles_touched"], np.ones_like(o["tiles_touched"])), "every Gaussian's rect is its tile alone"
@@ -393,6 +541,25 @@ def assert_reaches(case, o, excl):
         clamp = clamp_branch(case, o)
         assert clamp[big].sum() >= 8, "the frustum clamp fires for the Gaussians centred beyond 1.3 tan(fov / 2)"
         assert (clamp & ~excl).sum() >= 4, "some of them are checked per element"
+    elif case.name == "aa_needles":
+        chk = vis & ~excl
+        qf = o["aa_q"]
+        above, clamped = chk & (qf > AA_MIN_RATIO), chk & (qf <= AA_MIN_RATIO)
+        rel = qf.astype(np.float64) / np.float64(AA_MIN_RATIO) - 1.0
+        assert (above & (cancellation(case, o) > 1e3)).sum() >= AA_MIN_CHECKED, "needles above the clamp whose det0 cancels"
+        assert clamped.sum() >= AA_MIN_CHECKED, "needles whose q_f is clamped (no gradient through q)"
+        assert (above & (rel <= 1e-3)).sum() >= 8 and (clamped & (rel >= -1e-3)).sum() >= 8, "q_f within 1e-3 of the clamp"
+        # ... and among the Gaussians whose every gradient array is checked (compare_aa), so the clamp decision and the gradient
+        # through q reach dL_dcov3D / dL_dscales / dL_drotations / dL_dmeans3D of checked rows
+        well = well_conditioned(case, o)
+        assert (clamped & well).sum() >= AA_MIN_CHECKED, "clamped needles checked in every array"
+        assert (above & well & (rel <= 1e-3)).sum() >= 8 and (clamped & well & (rel >= -1e-3)).sum() >= 8, "near the clamp, every array"
+        assert (above & well & (rel > 1e-3)).sum() >= 8, "unclamped needles away from the clamp, every array"
+        sig = o["aa_sigmoid"]
+        assert (chk & (sig > 0.9)).sum() >= 100 and sig[chk].min() < 0.1 and sig[chk].max() > 0.99
+    elif case.name == "aa_subpixel":
+        assert ((vis & ~excl) & (o["aa_s"] < 0.1)).sum() >= AA_MIN_CHECKED, "sub-pixel splats: s < 0.1"
+        assert np.abs(o["n_contrib"]).max() > 0
     elif case.name == "saturation":
         assert o["clamped"][vis].any(axis=1).sum() >= 20, "SH colours clamped at 0 in some channels"
         terminated = 0

@@ -27,12 +27,12 @@ def forward_args(scene, cam, bg, extra=None, dev="cuda"):
             EMPTY if col is not None else scene.sh.to(dev), scene.degrees.to(dev), cam.camera_center.to(dev), False, False)
 
 
-def run_forward(scene, cam, bg, extra=None, prune_mask=None, quant=None, dev="cuda"):
-    """-> (args, raw outputs, dict of numpy intermediates in reference layouts)."""
+def run_forward(scene, cam, bg, extra=None, prune_mask=None, quant=None, dev="cuda", aa=False):
+    """-> (args, raw outputs, dict of numpy intermediates in reference layouts); `aa`: antialiasing=True."""
     args = forward_args(scene, cam, bg, extra, dev)
     dbg = {}
     out = _C.rasterize_gaussians(*args, prune_mask=None if prune_mask is None else prune_mask.to(dev),
-                                 quant=None if quant is None else quant.to(dev), debug_out=dbg)
+                                 quant=None if quant is None else quant.to(dev), debug_out=dbg, antialiasing=aa)
     R, color, radii, geomB, binB, imgB = out
     st = _C.export_state(geomB, binB, imgB, R, cam.image_width, cam.image_height, P=scene.means3D.shape[0])
     torch.cuda.synchronize()
@@ -49,14 +49,15 @@ def run_forward(scene, cam, bg, extra=None, prune_mask=None, quant=None, dev="cu
 GRAD_NAMES = ["dL_dmeans2D", "dL_dcolors", "dL_dopacity", "dL_dmeans3D", "dL_dcov3D", "dL_dsh", "dL_dscales", "dL_drotations"]
 
 
-def run_backward(args, out, dL, lam=0.0, prune_mask=None, quant=None):
+def run_backward(args, out, dL, lam=0.0, prune_mask=None, quant=None, aa=False, deterministic=False):
     (bg, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
     R, color, radii, geom, binning, img = out
     dev = means3D.device
     grads = _C.rasterize_gaussians_backward(bg, means3D, radii, colors, scales, rotations, mod, cov, view, proj, tx, ty,
                                             dL.to(dev), sh, degrees, campos, geom, R, binning, img, lam, False,
                                             prune_mask=None if prune_mask is None else prune_mask.to(dev),
-                                            quant=None if quant is None else quant.to(dev), want_conic=True)
+                                            quant=None if quant is None else quant.to(dev), want_conic=True, antialiasing=aa,
+                                            deterministic=deterministic)
     torch.cuda.synchronize()
     res = {n: g.cpu().numpy() for n, g in zip(GRAD_NAMES + ["dL_dconic"], grads)}
     return res

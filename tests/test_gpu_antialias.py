@@ -19,6 +19,7 @@ import torch
 
 import ours as O
 import restate64 as R64
+from render64 import render64
 from diff_gaussian_rasterization import _C
 from gs_b200 import synth
 from gs_b200.model import GaussianModelView
@@ -86,76 +87,7 @@ def test_antialiasing_moves_nothing_but_the_opacity(name):
     assert not torch.equal(plain[1], aa[1]) and float(st1["final_T"].mean()) > float(st0["final_T"].mean())
 
 
-# ---- 3. float64 restatement of the pipeline ----------------------------------------------------------------------------------
-
-def _render64(x, cam, bg, vis, tiles):
-    """float64 AA forward of the visible Gaussians.  x: dict of float64 leaves (means, logit, view, proj, campos, and scales + rots or
-    cov3D, sh + deg or colors).  tiles: per 16x16 tile the kernel's depth-sorted Gaussian ids.  -> (colour, invdepth, alpha, n_contrib,
-    intermediates, margins)."""
-    W, H = cam.image_width, cam.image_height
-    m = x["means"]
-    cov = x["cov3D"] if "cov3D" in x else R64.cov3D_from(x["scales"], x["rots"])
-    mh, tz, a, b, c = R64.screen_cov(m, x["view"], cov, W, H, math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5))
-    det0 = a * c - b * b
-    A, C = a + H_DIL, c + H_DIL
-    det1 = A * C - b * b
-    con = torch.stack([C / det1, -b / det1, A / det1], 1)
-    o_hat = torch.sigmoid(x["logit"].view(-1)) * torch.sqrt(torch.clamp_min(det0 / det1, 2.5e-5))
-    hom = mh @ x["proj"]
-    m_w = 1.0 / (hom[:, 3] + 1e-7)
-    ndc = hom[:, :2] * m_w[:, None]
-    ndc.retain_grad()
-    pix = torch.stack([((ndc[:, 0] + 1.0) * W - 1.0) * 0.5, ((ndc[:, 1] + 1.0) * H - 1.0) * 0.5], 1)
-    if "colors" in x:
-        rgb = x["colors"]
-    else:
-        d = m - x["campos"]
-        d = d / d.norm(dim=1, keepdim=True)
-        rgb = torch.clamp_min(R64.sh_colour(x["sh"], x["deg"], d), 0.0)
-        rgb.retain_grad()
-    invd = 1.0 / tz
-    colour = torch.zeros(3, H, W, dtype=F64, device=DEV)
-    invdepth = torch.zeros(H, W, dtype=F64, device=DEV)
-    alpha_map = torch.zeros(H, W, dtype=F64, device=DEV)
-    n_contrib = torch.zeros(H, W, dtype=torch.int64, device=DEV)
-    margin_a, margin_t = math.inf, math.inf
-    gx = (W + 15) // 16
-    for tile, ids in enumerate(tiles):
-        x0, y0 = (tile % gx) * 16, (tile // gx) * 16
-        ys, xs = torch.meshgrid(torch.arange(y0, min(y0 + 16, H), device=DEV), torch.arange(x0, min(x0 + 16, W), device=DEV), indexing="ij")
-        ys, xs = ys.reshape(-1), xs.reshape(-1)
-        if ids.numel() == 0:
-            colour[:, ys, xs] = bg.to(F64)[:, None]
-            continue
-        assert bool(vis[ids].all())
-        dx = pix[ids, 0][None, :] - xs[:, None].to(F64)
-        dy = pix[ids, 1][None, :] - ys[:, None].to(F64)
-        cc = con[ids]
-        power = -0.5 * (cc[:, 0] * dx * dx + cc[:, 2] * dy * dy) - cc[:, 1] * dx * dy
-        raw = o_hat[ids][None, :] * torch.exp(power)
-        # the reference's backward differentiates alpha = o G through the 0.99 clamp
-        alpha = raw + (torch.clamp_max(raw, 0.99) - raw).detach()
-        with torch.no_grad():
-            keep = (power <= 0) & (alpha >= 1.0 / 255.0)
-            margin_a = min(margin_a, float((alpha - 1.0 / 255.0).abs()[power <= 0].min()))
-            a_eff = torch.where(keep, alpha, torch.zeros_like(alpha))
-            test_T = torch.cumprod(1.0 - a_eff, 1)
-            stop = keep & (test_T < 1e-4)
-            done = torch.cumsum(stop.int(), 1) > 0
-            use = keep & ~done
-            margin_t = min(margin_t, float((test_T - 1e-4).abs()[keep].min()))
-            pos = torch.arange(1, ids.numel() + 1, device=DEV)[None, :]
-            n_contrib[ys, xs] = (use * pos).max(1).values
-        a_use = torch.where(use, alpha, torch.zeros_like(alpha))
-        T_after = torch.cumprod(1.0 - a_use, 1)
-        T_before = torch.cat([torch.ones_like(T_after[:, :1]), T_after[:, :-1]], 1)
-        w = a_use * T_before
-        T_final = T_after[:, -1]
-        colour[:, ys, xs] = (w @ rgb[ids]).T + T_final[None, :] * bg.to(F64)[:, None]
-        invdepth[ys, xs] = w @ invd[ids]
-        alpha_map[ys, xs] = 1.0 - T_final
-    return colour, invdepth[None], alpha_map[None], n_contrib, dict(ndc=ndc, rgb=rgb, cov=cov), (margin_a, margin_t)
-
+# ---- 3. float64 restatement of the pipeline (render64.py) ----------------------------------------------------------------------
 
 def _tiny_scene(seed, P=48):
     return synth.make_scene(P, seed, mixed_degrees=True, box=(1.3, 1.3, 0.8), log_scale_mean=math.log(0.05), M=16, near_frac=0.0)
@@ -193,7 +125,7 @@ def test_antialiasing_against_a_float64_restatement(case):
         x["colors"] = leaf(extra["colors_precomp"])
     else:
         x["sh"], x["deg"] = leaf(scene.sh), scene.degrees.to(DEV)
-    col, invd, alpha, nc, mid, (margin_a, margin_t) = _render64(x, cam, bg, vis, tiles)
+    col, invd, alpha, nc, mid, (margin_a, margin_t) = render64(x, cam, bg, vis, tiles)
     # the restatement took the kernel's decisions: the same last contributor everywhere, and no pair near a threshold
     assert torch.equal(nc, st["n_contrib"].long()), "compositing decisions differ from the kernel's"
     assert margin_a > 1e-7 and margin_t > 1e-9, (margin_a, margin_t)
