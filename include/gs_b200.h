@@ -324,6 +324,30 @@ GSB_API int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* c
                  float* dL_dcampos /* [3] or NULL */, char* workspace, const GsbRawParams* raw /* or NULL */,
                  const GsbRawGrads* raw_grads /* or NULL */, int32_t antialiasing, char* det_workspace, void* stream);
 
+/* Absolute screen-space gradient (AbsGS's homodirectional gradient, gsplat's `absgrad`; DESIGN.md §5m): besides every output of
+ * gsb_backward_deterministic, per Gaussian i
+ *   dL_dmeans2D_abs[i] = (0.5 W o_i sum_p |G dL/dalpha (a dx + b dy)|, 0.5 H o_i sum_p |G dL/dalpha (b dx + c dy)|, 0)
+ * over exactly the (pixel, Gaussian) pairs whose signed terms sum to dL_dmeans2D (same skips, same stop), with (a, b, c) the conic,
+ * o_i the (anti-aliased) opacity and (dx, dy) = mean2D - pixel: the sum of the absolute values of the per-pixel terms that
+ * dL_dmeans2D adds with their signs, so a Gaussian over detail whose pixels pull it in opposite directions keeps a large value.
+ * [P,3] fp32, overwritten; zero rows for culled and pruned Gaussians.  Every other output is bit-identical to the same call without
+ * it (the deterministic path) or agrees within the run-to-run spread of the float atomics (the default path).
+ *   det_workspace NULL: the default backward (float atomics); else gsb_absgrad_deterministic_workspace_bytes(P, num_rendered) bytes
+ *                   and the deterministic backward: dL_dmeans2D_abs is then the same bytes on every run too.
+ * gsb_absgrad_deterministic_workspace_bytes: gsb_deterministic_workspace_bytes plus 8 bytes per instance (48 bytes per instance).
+ * Errors (GSB_EINVAL, nothing launched): scene NULL, P < 0, num_rendered < 0, dL_dmeans2D_abs NULL with P > 0, grads->accumulate != 0
+ * (no view-batch form), a camera gradient without workspace, raw_grads without raw, and with raw the checks of gsb_backward_raw.
+ * GSB_ERANGE: num_rendered >= 2^30 with det_workspace.  There is no feature-channel form (gsb_backward_features). */
+GSB_API size_t gsb_absgrad_deterministic_workspace_bytes(int32_t P, int64_t num_rendered);
+GSB_API int gsb_backward_absgrad(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
+                 const char* geom_blob, const char* binning_blob, const char* image_blob,
+                 const float* dL_dout_color /* [3,H,W] */, const GsbGrads* grads,
+                 const float* dL_dinvdepth /* [1,H,W] or NULL */, const float* dL_dalpha /* [1,H,W] or NULL */,
+                 float lambda_sh_sparsity, float* dL_dviewmatrix /* [16] or NULL */, float* dL_dprojmatrix /* [16] or NULL */,
+                 float* dL_dcampos /* [3] or NULL */, char* workspace, const GsbRawParams* raw /* or NULL */,
+                 const GsbRawGrads* raw_grads /* or NULL */, int32_t antialiasing, char* det_workspace /* or NULL */,
+                 float* dL_dmeans2D_abs /* [P,3] */, void* stream);
+
 /* Per-Gaussian feature channels (DESIGN.md §5l): features [P,F] fp32, composited exactly like a colour channel with background 0,
  *   out[f](x,y) = sum_i features[i,f] * alpha_i * T_i
  * over the (pixel, Gaussian) pairs of the colour image, with its alpha, T, 1/255 skip and T < 1e-4 stop and the colour kernel's
@@ -523,6 +547,23 @@ GSB_API size_t gsb_densify_workspace_bytes(int32_t P);
 GSB_API size_t gsb_densify_split_std_offset(int32_t P);
 GSB_API int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* denom, const float* scaling,
                 const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad, float clone_max_scale,
+                float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
+                void* workspace, int64_t* counts, void* stream);
+
+/* The AbsGS forms (DESIGN.md §5m), for models that also keep xyz_gradient_accum_abs [P] (the norms of gsb_backward_absgrad's
+ * dL_dmeans2D_abs):
+ * gsb_densify_stats_abs: gsb_densify_stats plus, in the same launch, xyz_gradient_accum_abs[i] += sqrt(a0*a0 + a1*a1) of row i of
+ *   viewspace_grad_abs ([P, abs_row_stride], first two columns read).  denom is counted once.  Errors (GSB_EINVAL): those of
+ *   gsb_densify_stats, abs_row_stride < 2, and NULL viewspace_grad_abs / xyz_gradient_accum_abs when P > 0.
+ * gsb_densify_plan_abs: gsb_densify_plan's GSB_DENSIFY_CLONE_SPLIT with the split test on the absolute gradient: clone if
+ *   accum / denom >= max_grad and max(exp(scaling)) <= clone_max_scale (as there); split if accum_abs / denom >= max_grad_abs
+ *   (NaN -> 0) and max(exp(scaling)) > clone_max_scale.  Clones are never split; counts, workspace and row order as there.
+ *   Errors (GSB_EINVAL): those of gsb_densify_plan in that mode, and NULL xyz_gradient_accum_abs when P > 0. */
+GSB_API int gsb_densify_stats_abs(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const float* viewspace_grad_abs,
+                int32_t abs_row_stride, const uint8_t* visibility, const int32_t* radii, float* xyz_gradient_accum,
+                float* xyz_gradient_accum_abs, float* denom, float* max_radii2D, void* stream);
+GSB_API int gsb_densify_plan_abs(int32_t P, const float* xyz_gradient_accum, const float* xyz_gradient_accum_abs, const float* denom,
+                const float* scaling, const float* opacity, float max_grad, float max_grad_abs, float clone_max_scale,
                 float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
                 void* workspace, int64_t* counts, void* stream);
 

@@ -92,7 +92,7 @@ void prof_end(int kid, cudaStream_t stream)
 }
 static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter", "tile_sort_large", "unused4", "tile_sort", "unused6",
 	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad", "det_scan",
-	"det_gather", "det_clear", "features_forward", "features_backward" };
+	"det_gather", "det_clear", "features_forward", "features_backward", "absgrad_finish" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
 int launch_mark_visible(int, const float*, const float*, uint8_t*, cudaStream_t);
@@ -115,7 +115,7 @@ size_t kmeans_deterministic_workspace_bytes(long long, int);
 int launch_kmeans_deterministic(const float*, long long, const float*, int, float, int, int*, float*, char*, cudaStream_t);
 size_t knn_workspace_bytes(long long, long long);
 int launch_knn(const float*, long long, int, const int32_t*, long long, const int32_t*, long long, float*, float*, int32_t*, char*, cudaStream_t);
-size_t det_workspace_bytes(int, long long);
+size_t det_workspace_bytes(int, long long, int);
 size_t camera_grad_workspace_bytes(int);
 int launch_camera_grad_finish(int, const float*, float*, float*, float*, cudaStream_t);
 
@@ -563,6 +563,7 @@ static int backward_impl(const BackwardRequest& r)
 		return e;
 	if (r.features) if (int e = launch_features_backward(img, b, g, P, W, H, *r.features, acc, stream)) return e;
 	if (int e = launch_preprocess_backward(r, g, acc)) return e;
+	if (r.dL_dmeans2D_abs) if (int e = launch_absgrad_finish(r, acc)) return e;
 	if (r.want_cam())
 		if (int e = launch_camera_grad_finish(P, reinterpret_cast<float*>(r.cam_workspace), r.dL_dview, r.dL_dproj, r.dL_dcampos, stream)) return e;
 	return GSB_OK;
@@ -634,7 +635,7 @@ int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_t R, con
 	return backward_impl(r);
 }
 
-size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered); }
+size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered, 10); }
 
 int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
 	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
@@ -653,6 +654,31 @@ int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* cam, int6
 	if (scene->P > 0 && R > 0 && !det_workspace) { set_error("backward_deterministic: det_workspace is NULL"); return GSB_EINVAL; }
 	if (int e = check_camera_workspace("backward_deterministic", r)) return e;
 	if (raw_grads && !raw) { set_error("backward_deterministic: raw_grads given without raw"); return GSB_EINVAL; }
+	if (raw) if (int e = check_backward_raw(scene, grads, raw, raw_grads)) return e;
+	return backward_impl(r);
+}
+
+size_t gsb_absgrad_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered, DET_NS_ABS); }
+
+int gsb_backward_absgrad(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
+	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
+	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
+	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
+	int32_t antialiasing, char* det_workspace, float* dL_dmeans2D_abs, void* stream)
+{
+	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
+		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
+	r.aa = antialiasing != 0; r.raw = raw; r.raw_grads = raw_grads; r.deterministic = det_workspace != nullptr;
+	r.det_workspace = det_workspace; r.dL_dmeans2D_abs = dL_dmeans2D_abs; r.stream = (cudaStream_t)stream;
+	if (int e = check_scene_arg("backward_absgrad", scene)) return e;
+	if (scene->P > 0 && !dL_dmeans2D_abs) { set_error("backward_absgrad: dL_dmeans2D_abs is NULL"); return GSB_EINVAL; }
+	if (grads && grads->accumulate)
+	{ set_error("backward_absgrad: grads->accumulate is set; the absolute gradient has no view-batch accumulation form"); return GSB_EINVAL; }
+	if (R < 0) { set_error("backward_absgrad: num_rendered < 0"); return GSB_EINVAL; }
+	if (det_workspace && R >= (1ll << 30))
+	{ set_error("backward_absgrad: 2^30 or more instances (the slot scan's look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
+	if (int e = check_camera_workspace("backward_absgrad", r)) return e;
+	if (raw_grads && !raw) { set_error("backward_absgrad: raw_grads given without raw"); return GSB_EINVAL; }
 	if (raw) if (int e = check_backward_raw(scene, grads, raw, raw_grads)) return e;
 	return backward_impl(r);
 }

@@ -51,6 +51,8 @@ struct PlanArgs {
 	const float *accum, *denom, *scaling, *opacity, *max_radii2D;
 	const uint8_t* mask;
 	float max_grad, clone_max_scale, min_opacity, max_screen_size, big_scale, split_factor;
+	const float* accum_abs;    // gsb_densify_plan_abs: the split test reads accum_abs / denom against max_grad_abs (NULL otherwise)
+	float max_grad_abs;
 	int P, mode, screen_test;
 };
 
@@ -80,7 +82,15 @@ __device__ __forceinline__ unsigned row_flags(const PlanArgs& a, long long r)
 	// clones are never split.
 	const bool hot = g >= a.max_grad;
 	const bool clone = hot && ms <= a.clone_max_scale;
-	const bool split = hot && ms > a.clone_max_scale;
+	bool split = hot && ms > a.clone_max_scale;
+	if (a.accum_abs)
+	{
+		// AbsGS (DESIGN.md §5m): the split test takes the absolute gradient; a clone's padded value is 0 and its scale passed the
+		// clone test, so clones are still never split
+		float ga = __fdiv_rn(a.accum_abs[r], a.denom[r]);
+		if (isnan(ga)) ga = 0.0f;
+		split = ga >= a.max_grad_abs && ms > a.clone_max_scale;
+	}
 	// prune() after both (:685-689): max_radii2D was reset to zeros by densification_postfix (:620)
 	const bool gone = pruned(a, op, 0.0f, ms);
 	unsigned f = (!split && !gone ? 1u : 0u) | (clone ? 2u : 0u) | (clone && !gone ? 4u : 0u);
@@ -274,16 +284,23 @@ __global__ void __launch_bounds__(DENS_THREADS) densify_emit_kernel(const __grid
 	}
 }
 
-// the per-iteration statistics: train.py:134 and add_densification_stats (gaussian_model.py:693-695)
+// the per-iteration statistics: train.py:134 and add_densification_stats (gaussian_model.py:693-695); ABS also adds the norm of
+// the absolute gradient's first two columns to accum_abs
+template <bool ABS>
 __global__ void __launch_bounds__(DENS_THREADS) densify_stats_kernel(long long P, const float* __restrict__ grad, int grad_stride,
 	const uint8_t* __restrict__ visibility, const int32_t* __restrict__ radii, float* __restrict__ accum, float* __restrict__ denom,
-	float* __restrict__ max_radii2D)
+	float* __restrict__ max_radii2D, const float* __restrict__ grad_abs = nullptr, int abs_stride = 0, float* __restrict__ accum_abs = nullptr)
 {
 	const long long stride = (long long)gridDim.x * DENS_THREADS;
 	for (long long i = (long long)blockIdx.x * DENS_THREADS + threadIdx.x; i < P; i += stride)
 	{
 		const float g0 = grad[i * grad_stride], g1 = grad[i * grad_stride + 1];
 		accum[i] = __fadd_rn(accum[i], __fsqrt_rn(__fadd_rn(__fmul_rn(g0, g0), __fmul_rn(g1, g1))));
+		if (ABS)
+		{
+			const float a0 = grad_abs[i * abs_stride], a1 = grad_abs[i * abs_stride + 1];
+			accum_abs[i] = __fadd_rn(accum_abs[i], __fsqrt_rn(__fadd_rn(__fmul_rn(a0, a0), __fmul_rn(a1, a1))));
+		}
 		const bool vis = visibility[i] != 0;
 		denom[i] = __fadd_rn(denom[i], vis ? 1.0f : 0.0f);
 		if (radii && vis)
@@ -318,16 +335,37 @@ extern "C" int gsb_densify_stats(int32_t P, const float* viewspace_grad, int32_t
 	{ set_error("densify_stats: NULL viewspace_grad / visibility / xyz_gradient_accum / denom"); return GSB_EINVAL; }
 	const cudaStream_t st = (cudaStream_t)stream;
 	ProfScope prof(K_TOOLS, st);
-	densify_stats_kernel<<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii, xyz_gradient_accum,
+	densify_stats_kernel<false><<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii, xyz_gradient_accum,
 		denom, max_radii2D);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
 }
 
-extern "C" int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* denom, const float* scaling,
-	const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad, float clone_max_scale,
-	float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
+extern "C" int gsb_densify_stats_abs(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const float* viewspace_grad_abs,
+	int32_t abs_row_stride, const uint8_t* visibility, const int32_t* radii, float* xyz_gradient_accum, float* xyz_gradient_accum_abs,
+	float* denom, float* max_radii2D, void* stream)
+{
+	if (P < 0) { set_error("densify_stats_abs: P < 0"); return GSB_EINVAL; }
+	if (grad_row_stride < 2 || abs_row_stride < 2)
+	{ set_error("densify_stats_abs: row strides %d / %d; both must be >= 2", grad_row_stride, abs_row_stride); return GSB_EINVAL; }
+	if (radii && !max_radii2D) { set_error("densify_stats_abs: radii given without max_radii2D"); return GSB_EINVAL; }
+	if (P == 0) return GSB_OK;
+	if (!viewspace_grad || !viewspace_grad_abs || !visibility || !xyz_gradient_accum || !xyz_gradient_accum_abs || !denom)
+	{ set_error("densify_stats_abs: NULL viewspace_grad / viewspace_grad_abs / visibility / xyz_gradient_accum(_abs) / denom"); return GSB_EINVAL; }
+	const cudaStream_t st = (cudaStream_t)stream;
+	ProfScope prof(K_TOOLS, st);
+	densify_stats_kernel<true><<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii,
+		xyz_gradient_accum, denom, max_radii2D, viewspace_grad_abs, abs_row_stride, xyz_gradient_accum_abs);
+	GSB_LAUNCHED();
+	GSB_CUDA_OK(cudaGetLastError());
+	return GSB_OK;
+}
+
+// gsb_densify_plan and gsb_densify_plan_abs (xyz_gradient_accum_abs non-NULL: the AbsGS split test)
+static int densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* xyz_gradient_accum_abs, const float* denom,
+	const float* scaling, const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad, float max_grad_abs,
+	float clone_max_scale, float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
 	void* workspace, int64_t* counts, void* stream)
 {
 	if (P < 0 || P >= (1 << 30)) { set_error("densify_plan: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
@@ -356,10 +394,30 @@ extern "C" int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradie
 	a.accum = xyz_gradient_accum; a.denom = denom; a.scaling = scaling; a.opacity = opacity; a.max_radii2D = max_radii2D; a.mask = prune_mask;
 	a.max_grad = max_grad; a.clone_max_scale = clone_max_scale; a.min_opacity = min_opacity; a.max_screen_size = max_screen_size;
 	a.big_scale = big_scale; a.split_factor = split_scale_factor; a.P = P; a.mode = mode; a.screen_test = screen_test ? 1 : 0;
+	a.accum_abs = xyz_gradient_accum_abs; a.max_grad_abs = max_grad_abs;
 	densify_plan_kernel<<<w.n_tiles, DENS_THREADS, 0, st>>>(a, w, reinterpret_cast<long long*>(counts));
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
+}
+
+extern "C" int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* denom, const float* scaling,
+	const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad, float clone_max_scale,
+	float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
+	void* workspace, int64_t* counts, void* stream)
+{
+	return densify_plan(P, mode, xyz_gradient_accum, nullptr, denom, scaling, opacity, max_radii2D, prune_mask, max_grad, 0.0f,
+		clone_max_scale, min_opacity, screen_test, max_screen_size, big_scale, split_scale_factor, workspace, counts, stream);
+}
+
+extern "C" int gsb_densify_plan_abs(int32_t P, const float* xyz_gradient_accum, const float* xyz_gradient_accum_abs, const float* denom,
+	const float* scaling, const float* opacity, float max_grad, float max_grad_abs, float clone_max_scale, float min_opacity,
+	int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor, void* workspace, int64_t* counts, void* stream)
+{
+	if (P > 0 && !xyz_gradient_accum_abs) { set_error("densify_plan_abs: NULL xyz_gradient_accum_abs"); return GSB_EINVAL; }
+	return densify_plan(P, GSB_DENSIFY_CLONE_SPLIT, xyz_gradient_accum, xyz_gradient_accum_abs, denom, scaling, opacity, nullptr, nullptr,
+		max_grad, max_grad_abs, clone_max_scale, min_opacity, screen_test, max_screen_size, big_scale, split_scale_factor, workspace, counts,
+		stream);
 }
 
 extern "C" int gsb_densify_emit(const GsbDensifyTensor* tensors, int32_t n, int32_t P, const void* workspace, int64_t n_kept,

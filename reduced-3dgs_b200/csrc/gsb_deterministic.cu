@@ -12,29 +12,29 @@ namespace gsb {
 #define DET_SCAN_THREADS 1024
 #define DET_SCAN_ITEMS 4                      // Gaussians per thread: 4096 per CTA
 
-// Workspace: [ticket, error flag] | look-back descriptors, one per scan CTA | offset[P] | parts[R * 10]
+// Workspace: [ticket, error flag] | look-back descriptors, one per scan CTA | offset[P] | parts[R * ns] (ns = 10, DET_NS_ABS with absgrad)
 struct DetWorkspace {
 	uint32_t* head;          // [0] = scan ticket, [1] = error flag (slot total != R)
 	uint32_t* lb;            // [scan CTAs] decoupled look-back descriptors (zeroed with head)
 	uint32_t* offset;        // [P] first slot of each Gaussian
-	float* parts;            // [R][10] per-instance partials (9 used without the maps)
+	float* parts;            // [R][ns] per-instance partials (ns = 10, 9 used without the maps; DET_NS_ABS with absgrad)
 	static int scan_ctas(int P) { return (P + DET_SCAN_THREADS * DET_SCAN_ITEMS - 1) / (DET_SCAN_THREADS * DET_SCAN_ITEMS); }
-	static DetWorkspace carve(char* blob, int P, long long R, size_t* bytes = nullptr)
+	static DetWorkspace carve(char* blob, int P, long long R, int ns, size_t* bytes = nullptr)
 	{
 		Carver c(blob); DetWorkspace w;
 		w.head = c.take<uint32_t>(64);
 		w.lb = c.take<uint32_t>(scan_ctas(P));
 		w.offset = c.take<uint32_t>(P);
-		w.parts = c.take<float>(size_t(R) * 10);
+		w.parts = c.take<float>(size_t(R) * ns);
 		if (bytes) *bytes = c.off + 256;
 		return w;
 	}
 	size_t head_bytes() const { return size_t(reinterpret_cast<char*>(offset) - reinterpret_cast<char*>(head)); }
 };
 
-size_t det_workspace_bytes(int P, long long R)
+size_t det_workspace_bytes(int P, long long R, int ns)
 {
-	size_t b; DetWorkspace::carve(nullptr, P < 0 ? 0 : P, R < 0 ? 0 : R, &b); return b;
+	size_t b; DetWorkspace::carve(nullptr, P < 0 ? 0 : P, R < 0 ? 0 : R, ns, &b); return b;
 }
 
 __device__ __forceinline__ uint32_t rect_area(uint2 rc)
@@ -130,7 +130,8 @@ int launch_render_backward_deterministic(const BackwardRequest& req, const Image
 		GSB_CUDA_OK(cudaMemsetAsync(acc, 0, size_t(P) * 48, stream));
 		return GSB_OK;
 	}
-	DetWorkspace w = DetWorkspace::carve(req.det_workspace, P, R);
+	const bool abs = req.dL_dmeans2D_abs != nullptr;
+	DetWorkspace w = DetWorkspace::carve(req.det_workspace, P, R, abs ? DET_NS_ABS : 10);
 	{
 		ProfScope prof(K_DET_SCAN, stream);
 		GSB_CUDA_OK(cudaMemsetAsync(w.head, 0, w.head_bytes(), stream));
@@ -141,7 +142,7 @@ int launch_render_backward_deterministic(const BackwardRequest& req, const Image
 	}
 	if (int e = launch_render_backward(req, img, b, g, acc, w.parts, w.offset)) return e;
 	ProfScope prof(K_DET_GATHER, stream);
-	const int ns = (req.dL_dinvdepth || req.dL_dalpha) ? 10 : 9;
+	const int ns = abs ? DET_NS_ABS : (req.dL_dinvdepth || req.dL_dalpha) ? 10 : 9;
 	det_gather_kernel<<<(unsigned)((16ll * P + 255) / 256), 256, 0, stream>>>(P, ns, g.rect, w.offset, w.parts, (unsigned long long)R, w.head,
 		acc);
 	GSB_LAUNCHED();

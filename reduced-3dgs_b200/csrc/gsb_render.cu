@@ -277,9 +277,16 @@ __device__ __forceinline__ void red_add_v2(float* addr, float a, float b)
 // it culled); after a CTA barrier the threads add the 8 warps' rows in warp order 0..7 and STORE the sum to the instance's slot
 // offset[g] + (ty - miny) * w + (tx - minx) of `parts` (no atomics).  det_gather_kernel then adds each Gaussian's slots in
 // row-major tile order.  The stash rows keep their batch entry index instead of the Gaussian id: the records are still staged.
+//
+// ABS = true also accumulates the absolute screen-space gradient (AbsGS; DESIGN.md §5m), per Gaussian
+//     ax = o * sum_p |w_p (a dx_p + b dy_p)|,   ay = o * sum_p |w_p (b dx_p + c dy_p)|
+// over exactly the pairs the backward visits ((a, b, c) the conic, o the record's opacity), into accumulator slots 10 and 11.  The
+// per-pair factor is linear in the pixel, so nothing is stashed for it: at flush time lane l rebuilds it for stashed row l / 2,
+// component l % 2, from the row's record and the 32 stashed w (zero for the pairs the reference skips), and adds the 32 products
+// in pixel order.  The pair loop is the same instruction stream as without ABS, and no shared memory is added.
 #define DET_NS(MAPS) ((MAPS) ? 10 : 9)       // floats per slot: the accumulator's [dcol0 dcol1 dcol2 dop sx sy cxx cxy cyy (dinvd)]
-template <bool MAPS, bool DET = false>
-__global__ void __launch_bounds__(256, DET ? 3 : 4) render_backward_kernel(const uint2* __restrict__ ranges,
+template <bool MAPS, bool DET = false, bool ABS = false>
+__global__ void __launch_bounds__(256, DET ? (ABS ? 2 : 3) : 4) render_backward_kernel(const uint2* __restrict__ ranges,
 	const uint32_t* __restrict__ point_list,
 	int W, int H, const float4* __restrict__ rec, const float* __restrict__ bg,
 	const float* __restrict__ final_Ts, const uint32_t* __restrict__ n_contrib, const uint32_t* __restrict__ tile_max,
@@ -288,7 +295,7 @@ __global__ void __launch_bounds__(256, DET ? 3 : 4) render_backward_kernel(const
 	unsigned long long num_slots = 0)
 {
 	constexpr int NCH = MAPS ? 4 : 3;
-	constexpr int NS = DET_NS(MAPS);
+	constexpr int NS = ABS ? DET_NS_ABS : DET_NS(MAPS);
 	extern __shared__ __align__(16) unsigned char s_dyn_raw[];
 	BwdSmem<NCH>& S = *reinterpret_cast<BwdSmem<NCH>*>(s_dyn_raw);
 	float* const ebuf = reinterpret_cast<float*>(s_dyn_raw + sizeof(BwdSmem<NCH>));     // DET: [8 warps][BWD_BATCH entries][NS]
@@ -365,6 +372,44 @@ __global__ void __launch_bounds__(256, DET ? 3 : 4) render_backward_kernel(const
 			if (fg < nrows) asm volatile("prefetch.global.L1 [%0];" ::"l"(rec + 3 * (size_t)Wp.rowid[fg]));
 			if (fg + 8 < nrows) asm volatile("prefetch.global.L1 [%0];" ::"l"(rec + 3 * (size_t)Wp.rowid[fg + 8]));
 		}
+		// ABS: lane l sums row l / 2, component l % 2 (rows 0..3 in the 8 lanes of a 128-bit shared-memory phase: no bank conflict),
+		// ahead of the MMAs so that only its result is live across them.
+		// a dx + b dy with dx = X' - qx, dy = Y' - qy (X', Y' relative to the warp centre, qx, qy the pixel's constants) is
+		// K - a qx - b qy, K = a X' + b Y'; (a, b) -> (b, c) for the y component.
+		float absv = 0.f;
+		if (ABS)
+		{
+			const uint32_t ar = lane >> 1;
+			if (ar < nrows)
+			{
+				const uint32_t gid = Wp.rowid[ar];
+				float4 r0, r1;
+				if (DET)
+				{
+					const uint32_t ra = sbase0 + (uint32_t)(buf * BWD_BATCH * 3) * 16u + gid * SREC_BYTES;
+					r0 = lds128(ra); r1 = lds128(ra + 16);
+				}
+				else { r0 = __ldg(rec + 3 * (size_t)gid); r1 = __ldg(rec + 3 * (size_t)gid + 1); }
+				const float ka = (lane & 1) ? r0.y : r0.x, kb = (lane & 1) ? r0.z : r0.y;
+				const float K = ka * (r1.x - cxw) + kb * (r1.y - cyw);
+				const uint32_t wrow = wbase + ar * (STASH_LD * 4);
+				float s = 0.f;
+#pragma unroll
+				for (int j = 0; j < 8; j++)
+				{
+					const float4 w4 = lds128(wrow + 16 * j);
+					const float wq[4] = { w4.x, w4.y, w4.z, w4.w };
+#pragma unroll
+					for (int i = 0; i < 4; i++)
+					{
+						const int p = 4 * j + i;
+						const float v = fmaf(-ka, (float)(p & 7) - 3.5f, fmaf(-kb, (float)(p >> 3) - 1.5f, K));
+						s = fmaf(fabsf(wq[i]), fabsf(v), s);
+					}
+				}
+				absv = r1.z * s;
+			}
+		}
 		float dw[4] = { 0.f, 0.f, 0.f, 0.f }, du[4] = { 0.f, 0.f, 0.f, 0.f };
 		const float* dl = Wp.dlp + (fg < NCH ? fg : 0) * 32;
 #pragma unroll
@@ -399,6 +444,8 @@ __global__ void __launch_bounds__(256, DET ? 3 : 4) render_backward_kernel(const
 			float dinvd = 0.f;
 			if (MAPS) dinvd = __shfl_sync(0xffffffffu, du[2 * h + 1], q1);
 			const uint32_t row = fg + 8 * h;
+			float ax = 0.f, ay = 0.f;
+			if (ABS) { ax = __shfl_sync(0xffffffffu, absv, 2 * row); ay = __shfl_sync(0xffffffffu, absv, 2 * row + 1); }
 			if (ft == 0 && row < nrows)
 			{
 				const uint32_t gid = Wp.rowid[row];
@@ -423,12 +470,14 @@ __global__ void __launch_bounds__(256, DET ? 3 : 4) render_backward_kernel(const
 					e[4] = -o * (r0.x * Sx + r0.y * Sy); e[5] = -o * (r0.z * Sy + r0.y * Sx); e[6] = o * Sxx; e[7] = o * Sxy;
 					e[8] = o * Syy;
 					if (MAPS) e[9] = dinvd;
+					if (ABS) { e[10] = ax; e[11] = ay; }
 					continue;
 				}
 				float* a = acc + 12 * (size_t)gid;
 				red_add_v4(a, du[2 * h], du[2 * h + 1], c2, M0);
 				red_add_v4(a + 4, -o * (r0.x * Sx + r0.y * Sy), -o * (r0.z * Sy + r0.y * Sx), o * Sxx, o * Sxy);
-				if (MAPS) red_add_v2(a + 8, o * Syy, dinvd);
+				if (ABS) red_add_v4(a + 8, o * Syy, dinvd, ax, ay);             // dinvd = 0 without the maps: slot 9 stays zero
+				else if (MAPS) red_add_v2(a + 8, o * Syy, dinvd);
 				else atomicAdd(a + 8, o * Syy);
 			}
 		}
@@ -625,15 +674,16 @@ int launch_render_backward(const BackwardRequest& req, const ImageState& img, co
 	const int W = req.cam->width, H = req.cam->height;
 	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
 	const cudaStream_t stream = req.stream;
-	return dispatch([&](auto maps, auto det) -> int {
-		const size_t smem = sizeof(BwdSmem<maps ? 4 : 3>) + (det ? size_t(8) * BWD_BATCH * DET_NS(maps) * sizeof(float) : 0);
-		auto kernel = render_backward_kernel<maps, det>;
+	return dispatch([&](auto maps, auto det, auto abs) -> int {
+		constexpr int ns = abs ? DET_NS_ABS : DET_NS(maps);
+		const size_t smem = sizeof(BwdSmem<maps ? 4 : 3>) + (det ? size_t(8) * BWD_BATCH * ns * sizeof(float) : 0);
+		auto kernel = render_backward_kernel<maps, det, abs>;
 		if (int e = ensure_dyn_smem((const void*)kernel, (int)smem)) return e;
 		if (det)
 		{
 			// instances behind a tile's last contributor (and tiles with none) are never visited: their slots must read as zero
 			ProfScope prof(K_DET_CLEAR, stream);
-			GSB_CUDA_OK(cudaMemsetAsync(parts, 0, size_t(req.R) * DET_NS(maps) * sizeof(float), stream));
+			GSB_CUDA_OK(cudaMemsetAsync(parts, 0, size_t(req.R) * ns * sizeof(float), stream));
 		}
 		ProfScope prof(K_RENDER_BWD, stream);
 		// the per-Gaussian accumulator the kernel reduces into (12 floats per Gaussian, inside the geometry blob)
@@ -644,7 +694,33 @@ int launch_render_backward(const BackwardRequest& req, const ImageState& img, co
 		GSB_LAUNCHED();
 		GSB_CUDA_OK(cudaGetLastError());
 		return GSB_OK;
-	}, req.dL_dinvdepth || req.dL_dalpha, req.deterministic);
+	}, req.dL_dinvdepth || req.dL_dalpha, req.deterministic, req.dL_dmeans2D_abs != nullptr);
+}
+
+// dL_dmeans2D_abs [P,3] = (0.5 W slot 10, 0.5 H slot 11, 0): the constant factors of backward.cu:583-589, applied as the preprocess
+// backward applies them to slots 4 and 5; culled and pruned Gaussians (radii 0) get zero rows.
+__global__ void __launch_bounds__(256) absgrad_finish_kernel(int P, const int32_t* __restrict__ radii, const float* __restrict__ acc,
+	float half_w, float half_h, float* __restrict__ out)
+{
+	const int i = blockIdx.x * blockDim.x + threadIdx.x;
+	if (i >= P) return;
+	const bool vis = radii[i] > 0;
+	const float2 s = reinterpret_cast<const float2*>(acc)[6 * (size_t)i + 5];
+	out[3 * (size_t)i] = vis ? s.x * half_w : 0.0f;
+	out[3 * (size_t)i + 1] = vis ? s.y * half_h : 0.0f;
+	out[3 * (size_t)i + 2] = 0.0f;
+}
+
+int launch_absgrad_finish(const BackwardRequest& req, const float* acc)
+{
+	const int P = req.scene->P;
+	if (P <= 0) return GSB_OK;
+	ProfScope prof(K_ABSGRAD_FINISH, req.stream);
+	absgrad_finish_kernel<<<(P + 255) / 256, 256, 0, req.stream>>>(P, req.radii, acc, 0.5f * req.cam->width, 0.5f * req.cam->height,
+		req.dL_dmeans2D_abs);
+	GSB_LAUNCHED();
+	GSB_CUDA_OK(cudaGetLastError());
+	return GSB_OK;
 }
 
 } // namespace gsb

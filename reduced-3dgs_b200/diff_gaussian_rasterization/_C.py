@@ -16,7 +16,8 @@ and rotations, and applies exp / F.normalize / the SH concatenation inside the k
 deterministic-algorithms flag) for their statistics and centre sums (gsb_forward_statistics_deterministic, gsb_kmeans_deterministic).
 `features` (forward, also of the variable-SH entry point) composites a [P, F] fp32 tensor of per-Gaussian features over the pairs of
 the colour image, with background 0, and appends the [F, H, W] image to the outputs (gsb_forward_features); the backward's `features`
-and `dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F] (gsb_backward_features).
+and `dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F] (gsb_backward_features).  `absgrad_out` (backward) takes
+a [P, 3] fp32 tensor that receives the absolute screen-space gradient (gsb_backward_absgrad).
 """
 from __future__ import annotations
 
@@ -88,6 +89,24 @@ def check_features(features, P, cuda=True):
     if cuda and not features.is_cuda:
         raise RuntimeError("features must live on a CUDA device (no CPU path exists)")
     return F
+
+
+def check_absgrad_out(absgrad_out, P, accumulate_into=None, features=None, dL_dfeatures_out=None):
+    """The checks of the backward's `absgrad_out`, made before anything runs (the device is checked against means3D's later)."""
+    if accumulate_into is not None:
+        raise RuntimeError("absgrad: the absolute screen-space gradient has no accumulate_into form (view-batch accumulation)")
+    if features is not None or dL_dfeatures_out is not None:
+        raise RuntimeError("absgrad: the feature backward is a separate pass, so the absolute screen-space gradient has no feature form")
+    if not isinstance(absgrad_out, torch.Tensor):
+        raise RuntimeError(f"absgrad_out must be a [P, 3] tensor, got {type(absgrad_out).__name__}")
+    if tuple(absgrad_out.shape) != (P, 3):
+        raise RuntimeError(f"absgrad_out must have shape [P, 3] with P = {P} Gaussians, got {tuple(absgrad_out.shape)}")
+    if absgrad_out.dtype != torch.float32:
+        raise RuntimeError(f"absgrad_out must be float32, got {absgrad_out.dtype}")
+    if not absgrad_out.is_contiguous():
+        raise RuntimeError("absgrad_out must be contiguous (it is written in place)")
+    if not absgrad_out.is_cuda:
+        raise RuntimeError("absgrad_out must live on a CUDA device (no CPU path exists)")
 
 
 def _present(t):
@@ -279,7 +298,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  binningBuffer, imageBuffer, lambda_sh_sparsity, debug, *, prune_mask=None, quant=None,
                                  accumulate_into=None, want_conic=False, view_means2D=None, dL_dinvdepth=None, dL_dalpha=None,
                                  camera_grads=False, antialiasing=False, raw=None, deterministic=False, features=None,
-                                 dL_dfeatures_out=None):
+                                 dL_dfeatures_out=None, absgrad_out=None):
     """rasterize_points.h:65-88 RasterizeGaussiansBackwardCUDA ->
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     `accumulate_into`: the same 8-tuple from a previous call; gradients are added in place (view-batch accumulation);
@@ -296,7 +315,12 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     the same inputs give the same bytes on every run, in every mode above; the values agree with the default path to rounding.
     `features` / `dL_dfeatures_out`: the [P, F] features of the forward's `features` and the gradient of its [F, H, W] image; the
     feature image's share of the gradients is added to every output above and the tuple ends with dL_dfeatures [P, F]
-    (gsb_backward_features).  Neither `accumulate_into` nor `deterministic` has a feature form: both are refused."""
+    (gsb_backward_features).  Neither `accumulate_into` nor `deterministic` has a feature form: both are refused.
+    `absgrad_out`: a contiguous fp32 [P, 3] tensor on the device, overwritten with (sum_p |g_x|, sum_p |g_y|, 0), the per-pixel terms
+    of dL_dmeans2D added as absolute values (AbsGS; gsb_backward_absgrad); every other output is the call's without it (bit for bit
+    with `deterministic`).  It has no `accumulate_into` and no feature form: both are refused before anything runs."""
+    if absgrad_out is not None:
+        check_absgrad_out(absgrad_out, int(means3D.shape[0]), accumulate_into, features, dL_dfeatures_out)
     feat_F = 0
     if features is not None:
         if accumulate_into is not None:
@@ -306,6 +330,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                "(torch.no_grad() or features.detach() and no loss on the image) or turn the deterministic mode off")
         feat_F = check_features(features, int(means3D.shape[0]))
     device = _device_of(means3D)
+    if absgrad_out is not None and absgrad_out.device != device:
+        raise RuntimeError(f"absgrad_out must live on {device}, got {absgrad_out.device}")
     if raw is not None:
         want_sh = not _present(colors)
         raw_s, C_rest = _raw_struct(raw, device, int(means3D.shape[0]), want_sh, sh, scales, rotations, cov3D_precomp, quant)
@@ -370,6 +396,13 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
             st = L.gsb_backward_features(*head, C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None,
                                          int(bool(antialiasing)), None, C.byref(fs), stream)
+        elif absgrad_out is not None:
+            det_ws = None
+            if deterministic:
+                det_ws = torch.empty(int(L.gsb_absgrad_deterministic_workspace_bytes(P, int(R))), dtype=torch.uint8, device=device)
+            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
+            st = L.gsb_backward_absgrad(*head, C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None,
+                                        int(bool(antialiasing)), ptr(det_ws), ptr(absgrad_out), stream)
         elif deterministic:
             # per-instance partial slots, from the caching allocator on the current stream (freed in stream order after the call)
             det_ws = torch.empty(int(L.gsb_deterministic_workspace_bytes(P, int(R))), dtype=torch.uint8, device=device)

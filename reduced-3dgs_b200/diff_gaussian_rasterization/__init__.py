@@ -19,6 +19,9 @@ flag) selects the backward that sums each Gaussian's gradients in a fixed order 
 GaussianRasterizer.forward's keyword-only `features` ([P, F] fp32, 1 <= F <= 256) appends the [F, H, W] image of per-Gaussian
 features composited over the colour pass with background 0; its gradient reaches the features and, through alpha, everything the
 colour gradient reaches.  The feature gradient has no deterministic form: it is refused when the deterministic mode is on.
+GaussianRasterizer.forward's keyword-only `means2D_abs` (a [P, 3] tensor that requires grad, e.g. a zeros leaf) receives as its
+gradient the absolute screen-space gradient (sum_p |g_x|, sum_p |g_y|, 0) of AbsGS (gsb_backward_absgrad), the densification
+statistic whose per-pixel terms cannot cancel; it has no feature form.
 """
 from typing import NamedTuple
 
@@ -46,9 +49,12 @@ def _call(fn, args, kw, dump, message):
         raise ex
 
 
-def _apply(op, raster_settings, *args, features=None):
+def _apply(op, raster_settings, *args, features=None, means2D_abs=None):
     camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
     feat = () if features is None else (features,)
+    if means2D_abs is not None:
+        # means2D_abs is the op's last input, after the features' slot (None when absent)
+        feat = (features, means2D_abs)
     if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera):
         # a learnable camera: the three tensors become inputs of the autograd op so that their gradients have a destination
         return op.apply(*args, *camera, *feat)
@@ -56,13 +62,13 @@ def _apply(op, raster_settings, *args, features=None):
     return op.apply(*args, *((None,) * 3 + feat if feat else ()))
 
 
-def _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, camera, features=None, **kw):
+def _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, camera, features=None, means2D_abs=None, **kw):
     """The forward both ops share: the _C call and the ctx state their backwards read.  `camera` is (viewmatrix, projmatrix,
     campos), raster_settings' own tensors, passed again as inputs only when the camera is learnable, else (None, None, None).
     -> (_C.rasterize_gaussians' tuple, the op's outputs: (color, radii) or, with return_maps, (color, radii, invdepth, alpha);
     with `features` the feature image [F, H, W] comes last)."""
     ctx.camera_meta = None if camera[0] is None else [(t.shape, t.dtype) for t in camera]
-    ctx.return_maps, ctx.has_features = return_maps, features is not None
+    ctx.return_maps, ctx.has_features, ctx.has_abs = return_maps, features is not None, means2D_abs is not None
     kw.update(prune_mask=prune_mask, return_maps=return_maps, antialiasing=raster_settings.antialiasing)
     if features is not None:
         kw.update(features=features)
@@ -104,8 +110,9 @@ def _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, co
     rs = ctx.raster_settings
     if grad_out_color is None:
         grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
-    # the camera tensors are the op's last three inputs when it has them (followed by the features when given)
-    n = len(ctx.needs_input_grad) - (1 if ctx.has_features else 0)
+    # the camera tensors are the op's last three inputs when it has them (followed by the features when given, and by the
+    # features' slot and means2D_abs with absgrad)
+    n = len(ctx.needs_input_grad) - (2 if ctx.has_abs else 1 if ctx.has_features else 0)
     camera_need = ctx.needs_input_grad[n - 3:n] if ctx.camera_meta is not None else (False, False, False)
     args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
             rs.tanfovx, rs.tanfovy, grad_out_color, sh, degrees, rs.campos, geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer,
@@ -116,36 +123,52 @@ def _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, co
         kw.update(deterministic=True)
     if grad_features is not None:
         kw.update(features=features, dL_dfeatures_out=grad_features)
+    dabs = None
+    if ctx.has_abs:
+        dabs = torch.empty((means3D.shape[0], 3), dtype=torch.float32, device=means3D.device)
+        kw.update(absgrad_out=dabs)
     g = _call(_C.rasterize_gaussians_backward, args, kw,
               "snapshot_bw.dump", "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
     dfeat = None
     if grad_features is not None:
         g, dfeat = g[:-1], g[-1]                                       # dL_dfeatures comes last
+    ctx.grad_abs = dabs
     if ctx.camera_meta is None:
-        # the features' gradient follows three absent camera slots
-        return g, (None,) * 3 if ctx.has_features else (), dfeat
+        # the features' gradient (and means2D_abs's) follows three absent camera slots
+        return g, (None,) * 3 if ctx.has_features or ctx.has_abs else (), dfeat
     # with camera_grads the tuple ends with (dL_dviewmatrix, dL_dprojmatrix, dL_dcampos)
     return g, tuple(gc.reshape(shape).to(dtype) if n else None
                     for gc, n, (shape, dtype) in zip(g[-3:] if any(camera_need) else (None,) * 3, camera_need, ctx.camera_meta)), dfeat
 
 
+def _tail(ctx, grad_feat):
+    """The gradients of the op's inputs after the camera: the features (when given, or their absent slot before means2D_abs) and
+    means2D_abs, whose gradient is the absolute screen-space gradient."""
+    need = ctx.needs_input_grad
+    if ctx.has_abs:
+        return (grad_feat if ctx.has_features and need[-2] else None, ctx.grad_abs if need[-1] else None)
+    return (grad_feat if need[-1] else None,) if ctx.has_features else ()
+
+
 def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                        raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, features=None):
+                        raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, features=None,
+                        means2D_abs=None):
     return _apply(_RasterizeGaussians, raster_settings, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations,
-                  cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features=features)
+                  cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features=features,
+                  means2D_abs=means2D_abs)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                 raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, viewmatrix=None,
-                projmatrix=None, campos=None, features=None):
+                projmatrix=None, campos=None, features=None, means2D_abs=None):
         args = (raster_settings.bg, means3D, colors_precomp, opacities, scales, rotations, raster_settings.scale_modifier,
                 cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
                 raster_settings.tanfovy, raster_settings.image_height, raster_settings.image_width, sh, degrees,
                 raster_settings.campos, raster_settings.prefiltered, raster_settings.debug)
         out, outputs = _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, (viewmatrix, projmatrix, campos),
-                                features, quant=quant)
+                                features, means2D_abs, quant=quant)
         ctx.quant = quant
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, out[2], sh, out[3], out[4], out[5], degrees,
                               features)
@@ -175,15 +198,15 @@ class _RasterizeGaussians(torch.autograd.Function):
         return (grad_means3D, grad_means2D, grad_sh if need[2] else None, None,
                 grad_colors_precomp if need[4] else None, grad_opacities if need[5] else None,
                 grad_scales if need[6] else None, grad_rotations if need[7] else None,
-                grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None) + grad_camera + \
-            ((grad_feat if need[-1] else None,) if ctx.has_features else ())
+                grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None) + grad_camera + _tail(ctx, grad_feat)
 
 
 def rasterize_gaussians_raw(means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
-                            raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, features=None):
+                            raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, features=None, means2D_abs=None):
     """rasterize_gaussians on the model's raw parameters (see _RasterizeGaussiansRaw)."""
     return _apply(_RasterizeGaussiansRaw, raster_settings, means3D, means2D, features_dc, features_rest, degrees, colors_precomp,
-                  opacities, scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, features=features)
+                  opacities, scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, features=features,
+                  means2D_abs=means2D_abs)
 
 
 class _RasterizeGaussiansRaw(torch.autograd.Function):
@@ -195,7 +218,7 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
     @staticmethod
     def forward(ctx, means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
                 raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None,
-                features=None):
+                features=None, means2D_abs=None):
         empty = torch.Tensor([])
         with_colors = colors_precomp.numel() > 0
         raw = (None, None, scaling, rotation) if with_colors else (features_dc, features_rest, scaling, rotation)
@@ -204,7 +227,7 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
                 raster_settings.image_height, raster_settings.image_width, empty, degrees, raster_settings.campos,
                 raster_settings.prefiltered, raster_settings.debug)
         out, outputs = _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, (viewmatrix, projmatrix, campos),
-                                features, raw=raw)
+                                features, means2D_abs, raw=raw)
         ctx.with_colors = with_colors
         ctx.save_for_backward(colors_precomp, means3D, features_dc, features_rest, scaling, rotation, out[2], out[3], out[4], out[5],
                               degrees, features)
@@ -223,8 +246,7 @@ class _RasterizeGaussiansRaw(torch.autograd.Function):
         need = ctx.needs_input_grad
         return (grad_means3D, grad_means2D, grad_dc if need[2] else None, grad_rest if need[3] else None, None,
                 grad_colors if need[5] else None, grad_opacities if need[6] else None, grad_scaling if need[7] else None,
-                grad_rotation if need[8] else None, None, None, None, None) + grad_camera + \
-            ((grad_feat if need[-1] else None,) if ctx.has_features else ())
+                grad_rotation if need[8] else None, None, None, None, None) + grad_camera + _tail(ctx, grad_feat)
 
 
 class _ReferenceSettings(NamedTuple):
@@ -279,15 +301,22 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, degrees=None, colors_precomp=None, scales=None,
                 rotations=None, cov3D_precomp=None, lambda_sh_sparsity=0., *, prune_mask=None, quant=None, return_maps=False,
-                raw_params=None, features=None):
+                raw_params=None, features=None, means2D_abs=None):
         """-> (color, radii); with return_maps, (color, radii, invdepth [1,H,W], alpha [1,H,W]), all three differentiable.
         `raw_params`: (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]), the model's leaf tensors, in place
         of shs / scales / rotations (which must then be None, as must cov3D_precomp and quant); with colors_precomp the two
         feature tensors are None.  The kernels apply exp / F.normalize / the concatenation and return the four gradients.
         `features`: [P, F] fp32 on the device, 1 <= F <= 256; the outputs end with the [F, H, W] feature image (each channel composited
         like a colour channel with background 0), differentiable w.r.t. the features and, through alpha, the scene and the camera.
-        A feature gradient under the deterministic mode is refused (here when `features` requires grad, else in the backward)."""
+        A feature gradient under the deterministic mode is refused (here when `features` requires grad, else in the backward).
+        `means2D_abs`: a [P, 3] tensor (a zeros leaf that requires grad); its gradient is the absolute screen-space gradient
+        (sum_p |g_x|, sum_p |g_y|, 0), deterministic with the deterministic mode.  Not together with `features`."""
         raster_settings = self.raster_settings
+        if means2D_abs is not None:
+            if features is not None:
+                raise RuntimeError("means2D_abs: the absolute screen-space gradient has no feature form; render the features separately")
+            if not isinstance(means2D_abs, torch.Tensor) or tuple(means2D_abs.shape) != (int(means3D.shape[0]), 3):
+                raise RuntimeError(f"means2D_abs must be a [P, 3] tensor with P = {int(means3D.shape[0])}")
         if features is not None:
             _C.check_features(features, int(means3D.shape[0]), cuda=False)
             if features.requires_grad and torch.is_grad_enabled() and _deterministic(raster_settings):
@@ -312,6 +341,8 @@ class GaussianRasterizer(nn.Module):
         e = lambda t: empty if t is None else t                                  # absent inputs travel as empty tensors
         if raw_params is not None:
             return rasterize_gaussians_raw(means3D, means2D, e(features_dc), e(features_rest), degrees, e(colors_precomp), e(opacities),
-                                           scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, features)
+                                           scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, features,
+                                           means2D_abs)
         return rasterize_gaussians(means3D, means2D, e(shs), degrees, e(colors_precomp), e(opacities), e(scales), e(rotations),
-                                   e(cov3D_precomp), raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features)
+                                   e(cov3D_precomp), raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features,
+                                   means2D_abs)

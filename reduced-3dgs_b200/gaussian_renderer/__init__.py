@@ -15,6 +15,9 @@ torch.nn.functional.normalize; the variable-SH inference path ignores it.
 `features` ([P, F] fp32 on the device, 1 <= F <= 256) adds pkg["features"], the [F, H, W] image of per-Gaussian features composited
 over the colour pass with background 0 (semantic features, normals, per-Gaussian statistics such as the SH degree or the opacity).
 It is differentiable w.r.t. the features and the scene on every path but the variable-SH inference one, which renders it forward only.
+`absgrad=True` adds pkg["viewspace_points_abs"], a zeros leaf [P, 3] whose .grad after loss.backward() is the absolute screen-space
+gradient (sum_p |g_x|, sum_p |g_y|, 0) of AbsGS, the split statistic of densify_and_prune(max_grad_abs=...) (DESIGN.md §5m).  It needs
+a backward, so the variable-SH inference path refuses it, and it has no feature form.
 
 A learnable camera needs no argument: when world_view_transform, full_proj_transform or camera_center requires grad, the
 rasterizer returns their gradients (the variable-SH inference path stays non-differentiable).  The rasterizer takes
@@ -81,7 +84,7 @@ def _raw_params(pc, pipe, override_color):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-           lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False, return_maps=False, features=None):
+           lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False, return_maps=False, features=None, absgrad=False):
     """
     Render the scene.
 
@@ -90,9 +93,16 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
     # Create zero tensor. We will use it to make pytorch return gradients of the 2D (screen-space) means.
     # (The reference adds 0 to make it a non-leaf and then calls retain_grad(), GR:27-31; a leaf keeps its .grad by itself and
     # saves an elementwise pass over [P,3].)
+    if absgrad and variable_sh_bands:
+        raise RuntimeError("gaussian_renderer.render: absgrad needs the backward; the variable-SH inference path renders forward only")
+    if absgrad and features is not None:
+        raise RuntimeError("gaussian_renderer.render: absgrad has no feature form; render the features in a call without absgrad")
     fused = bool(getattr(pipe, "fused_activations", False)) and not variable_sh_bands
     raw_params = _raw_params(pc, pipe, override_color) if fused else None
     screenspace_points = torch.zeros_like(pc.get_xyz, dtype=pc.get_xyz.dtype, requires_grad=True, device=pc.get_xyz.device)
+    screenspace_points_abs = None
+    if absgrad:
+        screenspace_points_abs = torch.zeros_like(pc.get_xyz, dtype=pc.get_xyz.dtype, requires_grad=True, device=pc.get_xyz.device)
 
     tanfovx = math.tan(viewpoint_camera.FoVx * 0.5)
     tanfovy = math.tan(viewpoint_camera.FoVy * 0.5)
@@ -166,7 +176,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         out = rasterizer(
             means3D=means3D, means2D=means2D, shs=shs, degrees=degrees, colors_precomp=colors_precomp, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, lambda_sh_sparsity=lambda_sh_sparsity,
-            prune_mask=prune_mask, quant=quant, return_maps=return_maps, raw_params=raw_params, features=features)
+            prune_mask=prune_mask, quant=quant, return_maps=return_maps, raw_params=raw_params, features=features,
+            **({} if screenspace_points_abs is None else dict(means2D_abs=screenspace_points_abs)))
         rendered_image, radii = out[0], out[1]
         maps = out[2:4] if return_maps else ()
         feature_image = out[-1] if features is not None else None
@@ -186,4 +197,6 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         pkg["invdepth"], pkg["alpha"] = maps
     if features is not None:
         pkg["features"] = feature_image
+    if absgrad:
+        pkg["viewspace_points_abs"] = screenspace_points_abs
     return pkg

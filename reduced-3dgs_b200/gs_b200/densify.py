@@ -23,6 +23,11 @@ Model contract (duck-typed on the reference's attribute names): the optimizer is
 the six groups "xyz", "f_dc", "f_rest", "opacity", "scaling", "rotation", one fp32 contiguous CUDA param each (f_rest a dense
 [P, C, 3] tensor); `_degrees` int32 [P, 1]; `xyz_gradient_accum`, `denom` fp32 [P, 1]; `max_radii2D` fp32 [P];
 `percent_dense`.  Anything else is refused before the model or the optimizer changes.
+
+AbsGS (DESIGN.md §5m): add_densification_stats(..., viewspace_abs=pkg["viewspace_points_abs"]) also accumulates the norm of the
+absolute screen-space gradient into `xyz_gradient_accum_abs` [P, 1] (created as zeros on the first call), and
+densify_and_prune(..., max_grad_abs=...) splits on accum_abs / denom >= max_grad_abs instead of on the signed statistic.  Every prune
+carries `xyz_gradient_accum_abs`, and densify_and_prune resets it, exactly as `xyz_gradient_accum`, when the model has one.
 """
 from __future__ import annotations
 
@@ -45,18 +50,32 @@ def split_scale_factor(n=SPLIT_N):
     return float(np.float32(1) / np.float32(0.8 * n))
 
 
-def add_densification_stats(model, viewspace_point_tensor, update_filter, radii=None):
+def _check_viewspace_grad(g, P, what):
+    if g is None:
+        raise RuntimeError(f"densify: {what} has no gradient")
+    if (not g.is_cuda or g.dtype != torch.float32 or g.dim() != 2 or g.shape[0] != P or g.shape[1] < 2 or g.stride(1) != 1
+            or (P > 1 and g.stride(0) < 2)):
+        raise RuntimeError(f"densify: the view-space gradient ({what}) must be an fp32 CUDA [P, >= 2] tensor with unit column stride")
+
+
+def add_densification_stats(model, viewspace_point_tensor, update_filter, radii=None, viewspace_abs=None):
     """xyz_gradient_accum += |grad[:, :2]|; denom += update_filter; with radii, also train.py:134's
-    max_radii2D[update_filter] = max(max_radii2D[update_filter], radii[update_filter]).  One launch, no host synchronisation."""
+    max_radii2D[update_filter] = max(max_radii2D[update_filter], radii[update_filter]).  With viewspace_abs (render(absgrad=True)'s
+    pkg["viewspace_points_abs"]), also xyz_gradient_accum_abs += |viewspace_abs.grad[:, :2]| (zeros [P, 1] created on the first call).
+    One launch, no host synchronisation."""
     g = viewspace_point_tensor.grad
     accum, denom = model.xyz_gradient_accum, model.denom
     P = accum.shape[0] if accum.dim() > 0 else -1
-    if g is None:
-        raise RuntimeError("densify: viewspace_point_tensor has no gradient")
+    _check_viewspace_grad(g, P, "viewspace_point_tensor")
     dev = g.device
-    if (not g.is_cuda or g.dtype != torch.float32 or g.dim() != 2 or g.shape[0] != P or g.shape[1] < 2 or g.stride(1) != 1
-            or (P > 1 and g.stride(0) < 2)):
-        raise RuntimeError("densify: the view-space gradient must be an fp32 CUDA [P, >= 2] tensor with unit column stride")
+    ga = None
+    if viewspace_abs is not None:
+        ga = viewspace_abs.grad
+        _check_viewspace_grad(ga, P, "viewspace_abs")
+        if ga.device != dev:
+            raise RuntimeError(f"densify: the gradient of viewspace_abs must live on {dev}")
+        if getattr(model, "xyz_gradient_accum_abs", None) is not None:
+            _check_f32(model.xyz_gradient_accum_abs, (P, 1), dev, "xyz_gradient_accum_abs")
     _check_f32(accum, (P, 1), dev, "xyz_gradient_accum")
     _check_f32(denom, (P, 1), dev, "denom")
     if (update_filter.dtype != torch.bool or update_filter.shape != (P,) or update_filter.device != dev
@@ -68,7 +87,16 @@ def add_densification_stats(model, viewspace_point_tensor, update_filter, radii=
             raise RuntimeError(f"densify: radii must be a contiguous int32 tensor [{P}] on {dev}")
         mr = model.max_radii2D
         _check_f32(mr, (P,), dev, "max_radii2D")
+    if ga is not None and getattr(model, "xyz_gradient_accum_abs", None) is None:
+        model.xyz_gradient_accum_abs = torch.zeros((P, 1), device=dev)
     if P == 0:
+        return
+    if ga is not None:
+        with gsl.on_device(dev):
+            gsl.check(gsl.lib().gsb_densify_stats_abs(P, g.data_ptr(), g.stride(0), ga.data_ptr(), ga.stride(0), update_filter.data_ptr(),
+                                                       None if radii is None else radii.data_ptr(), accum.data_ptr(),
+                                                       model.xyz_gradient_accum_abs.data_ptr(), denom.data_ptr(),
+                                                       None if mr is None else mr.data_ptr(), gsl.current_stream(dev)))
         return
     with gsl.on_device(dev):
         gsl.check(gsl.lib().gsb_densify_stats(P, g.data_ptr(), g.stride(0), update_filter.data_ptr(),
@@ -76,11 +104,16 @@ def add_densification_stats(model, viewspace_point_tensor, update_filter, radii=
                                                None if mr is None else mr.data_ptr(), gsl.current_stream(dev)))
 
 
-def densify_and_prune(model, max_grad, min_opacity, extent, max_screen_size, densification_statistics_dict, store_grads=False):
-    """densify_and_clone + densify_and_split + prune of the reference, in one plan and one emit."""
+def densify_and_prune(model, max_grad, min_opacity, extent, max_screen_size, densification_statistics_dict, store_grads=False,
+                      max_grad_abs=None):
+    """densify_and_clone + densify_and_split + prune of the reference, in one plan and one emit.  max_grad_abs (AbsGS): clone on
+    accum / denom >= max_grad as before, split on xyz_gradient_accum_abs / denom >= max_grad_abs (NaN -> 0); None is the reference's
+    rule."""
     groups, P, dev = _validate(model, store_grads, grads_everywhere=store_grads)
+    if max_grad_abs is not None and getattr(model, "xyz_gradient_accum_abs", None) is None:
+        raise RuntimeError("densify: max_grad_abs needs model.xyz_gradient_accum_abs (add_densification_stats(..., viewspace_abs=...))")
     counts, ws, dcounts = _plan(model, groups, P, dev, gsl.DENSIFY_CLONE_SPLIT, max_grad=max_grad, percent_dense=model.percent_dense,
-                       min_opacity=min_opacity, extent=extent, max_screen_size=max_screen_size)
+                       min_opacity=min_opacity, extent=extent, max_screen_size=max_screen_size, max_grad_abs=max_grad_abs)
     n_kept, C, n_clones_kept, S, n_children, P_out = counts[:6]
     # the reference's draw (gaussian_model.py:633-635): std = exp(scaling) of the split parents, repeated N times
     off = gsl.lib().gsb_densify_split_std_offset(P)
@@ -89,6 +122,8 @@ def densify_and_prune(model, max_grad, min_opacity, extent, max_screen_size, den
     samples = torch.normal(mean=means, std=stds)
     _emit(model, groups, P, dev, ws, counts, store_grads, gather_stats=False, samples=samples)
     model.xyz_gradient_accum = torch.zeros((P_out, 1), device=dev)
+    if getattr(model, "xyz_gradient_accum_abs", None) is not None:
+        model.xyz_gradient_accum_abs = torch.zeros((P_out, 1), device=dev)
     # densification_postfix creates density_gradient_accum after the split's concatenation; the prunes that follow do not index it
     model.density_gradient_accum = torch.zeros((P + C + SPLIT_N * S, 1), device=dev)
     model.denom = torch.zeros((P_out, 1), device=dev)
@@ -243,16 +278,27 @@ def _validate(model, store_grads, grads_everywhere=False):
     _check_f32(getattr(model, "xyz_gradient_accum", None), (P, 1), dev, "xyz_gradient_accum")
     _check_f32(getattr(model, "denom", None), (P, 1), dev, "denom")
     _check_f32(getattr(model, "max_radii2D", None), (P,), dev, "max_radii2D")
+    if getattr(model, "xyz_gradient_accum_abs", None) is not None:
+        _check_f32(model.xyz_gradient_accum_abs, (P, 1), dev, "xyz_gradient_accum_abs")
     return groups, P, dev
 
 
-def _plan(model, groups, P, dev, mode, max_grad=0.0, percent_dense=0.0, min_opacity=0.0, extent=0.0, max_screen_size=None, mask=None):
+def _plan(model, groups, P, dev, mode, max_grad=0.0, percent_dense=0.0, min_opacity=0.0, extent=0.0, max_screen_size=None, mask=None,
+          max_grad_abs=None):
     """Runs the plan and reads its counts back (the one host synchronisation).  The thresholds are the reference's Python
     doubles (percent_dense*extent, 0.1*extent), cast to fp32 by ctypes as torch casts a Python number it compares with."""
     param = {name: p for name, _, p, _ in groups}
     ws = torch.empty(gsl.lib().gsb_densify_workspace_bytes(P), dtype=torch.uint8, device=dev)
     counts = torch.empty(gsl.DENSIFY_COUNTS, dtype=torch.int64, device=dev)
     screen = bool(max_screen_size)
+    if max_grad_abs is not None:
+        with gsl.on_device(dev):
+            gsl.check(gsl.lib().gsb_densify_plan_abs(
+                P, model.xyz_gradient_accum.data_ptr(), model.xyz_gradient_accum_abs.data_ptr(), model.denom.data_ptr(),
+                param["scaling"].data_ptr(), param["opacity"].data_ptr(), max_grad, max_grad_abs, percent_dense * extent, min_opacity,
+                1 if screen else 0, max_screen_size if screen else 0.0, 0.1 * extent, split_scale_factor(), ws.data_ptr(),
+                counts.data_ptr(), gsl.current_stream(dev)))
+        return [int(v) for v in counts.tolist()], ws, counts
     with gsl.on_device(dev):
         gsl.check(gsl.lib().gsb_densify_plan(
             P, mode, model.xyz_gradient_accum.data_ptr(), model.denom.data_ptr(), param["scaling"].data_ptr(),
@@ -289,6 +335,8 @@ def _emit(model, groups, P, dev, ws, counts, store_grads, gather_stats, samples=
     stats = [("_degrees", torch.int32, (1,))]
     if gather_stats:
         stats += [("xyz_gradient_accum", torch.float32, (1,)), ("denom", torch.float32, (1,)), ("max_radii2D", torch.float32, ())]
+        if getattr(model, "xyz_gradient_accum_abs", None) is not None:
+            stats.append(("xyz_gradient_accum_abs", torch.float32, (1,)))
     out_stats = {}
     for attr, dtype, row in stats:
         src = getattr(model, attr)

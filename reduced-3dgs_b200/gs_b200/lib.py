@@ -206,6 +206,10 @@ def lib():
                                            C.POINTER(GsbFeatures), C.c_void_p]
         L.gsb_backward_features.restype = C.c_int
         L.gsb_backward_features.argtypes = L.gsb_backward_deterministic.argtypes[:-1] + [C.POINTER(GsbFeatures), C.c_void_p]
+        L.gsb_absgrad_deterministic_workspace_bytes.restype = C.c_size_t
+        L.gsb_absgrad_deterministic_workspace_bytes.argtypes = [C.c_int32, C.c_int64]
+        L.gsb_backward_absgrad.restype = C.c_int
+        L.gsb_backward_absgrad.argtypes = L.gsb_backward_deterministic.argtypes[:-1] + [C.c_void_p, C.c_void_p]
         L.gsb_mark_visible.restype = C.c_int
         L.gsb_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_export_binning.restype = C.c_int
@@ -226,6 +230,11 @@ def lib():
         L.gsb_densify_split_std_offset.argtypes = [C.c_int32]
         L.gsb_densify_plan.restype = C.c_int
         L.gsb_densify_plan.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.c_float] * 3 + [C.c_int32] + [C.c_float] * 3 + \
+            [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gsb_densify_stats_abs.restype = C.c_int
+        L.gsb_densify_stats_abs.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p] * 7
+        L.gsb_densify_plan_abs.restype = C.c_int
+        L.gsb_densify_plan_abs.argtypes = [C.c_int32] + [C.c_void_p] * 5 + [C.c_float] * 4 + [C.c_int32] + [C.c_float] * 3 + \
             [C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_densify_emit.restype = C.c_int
         L.gsb_densify_emit.argtypes = [C.POINTER(GsbDensifyTensor), C.c_int32, C.c_int32, C.c_void_p] + [C.c_int64] * 4 + \
@@ -275,7 +284,8 @@ EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", 
                     "gsb_statistics_workspace_bytes", "gsb_forward_statistics_deterministic",
                     "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic", "gsb_redundancy_workspace_bytes",
                     "gsb_redundancy_score", "gsb_mercy_workspace_bytes", "gsb_mercy_plan",
-                    "gsb_forward_features", "gsb_backward_features"]
+                    "gsb_forward_features", "gsb_backward_features", "gsb_absgrad_deterministic_workspace_bytes",
+                    "gsb_backward_absgrad", "gsb_densify_stats_abs", "gsb_densify_plan_abs"]
 
 
 def check(status: int):

@@ -1,0 +1,242 @@
+"""CPU: the absolute screen-space gradient (DESIGN.md §5m).  The new entry points (gsb_backward_absgrad, its workspace size,
+gsb_densify_stats_abs, gsb_densify_plan_abs) reject each bad argument before any CUDA call; the Python layer refuses what has no
+absgrad form before anything runs and, against stand-in kernels, carries `absgrad` through both autograd ops and render() while
+leaving the calls without it exactly as they were; and the float64 restatement of the per-pair terms (absgrad64.py) sums, with
+signs, to the fp64 oracle's dL_dmeans2D on the backward-edge scenes, which pins it to the pairs and terms the oracle uses."""
+import ctypes as C
+import math
+from types import SimpleNamespace
+
+import numpy as np
+import pytest
+import torch
+
+import absgrad64
+import backward_edges as BE
+from gs_b200 import lib
+
+NEW = ("gsb_backward_absgrad", "gsb_absgrad_deterministic_workspace_bytes", "gsb_densify_stats_abs", "gsb_densify_plan_abs")
+
+
+def test_symbols_exported():
+    L = lib.lib()
+    for sym in NEW:
+        assert sym in lib.EXPORTED_SYMBOLS
+        getattr(L, sym)
+
+
+def test_workspace_grows_and_adds_eight_bytes_per_instance():
+    L = lib.lib()
+    for P, R in ((0, 0), (1, 1), (1000, 5000), (100_000, 3_000_000)):
+        base, ab = int(L.gsb_deterministic_workspace_bytes(P, R)), int(L.gsb_absgrad_deterministic_workspace_bytes(P, R))
+        assert ab >= base + 8 * R
+    assert L.gsb_absgrad_deterministic_workspace_bytes(1000, 10) < L.gsb_absgrad_deterministic_workspace_bytes(1000, 11_000)
+    assert L.gsb_absgrad_deterministic_workspace_bytes(1000, 10) < L.gsb_absgrad_deterministic_workspace_bytes(100_000, 10)
+
+
+def _bwd(L, scene, R=5, grads=None, out=True, det_ws=None, raw=None, raw_grads=None, cam_out=None, workspace=None):
+    cam = lib.GsbCamera()
+    g = grads if grads is not None else lib.GsbGrads()
+    buf = (C.c_float * 16)()
+    return L.gsb_backward_absgrad(scene, C.byref(cam), R, None, None, None, None, None, C.byref(g), None, None, 0.0, cam_out, None, None,
+                                  workspace, raw, raw_grads, 0, det_ws, C.addressof(buf) if out else None, None)
+
+
+def test_backward_absgrad_rejects_bad_arguments():
+    L = lib.lib()
+    scene = C.byref(lib.GsbScene(P=10))
+    fbuf = (C.c_float * 16)()
+    for sc in (None, C.byref(lib.GsbScene(P=-1))):
+        assert _bwd(L, sc) == -1 and b"P < 0" in L.gsb_last_error()
+    assert _bwd(L, scene, out=False) == -1 and b"dL_dmeans2D_abs is NULL" in L.gsb_last_error()
+    assert _bwd(L, scene, grads=lib.GsbGrads(accumulate=1)) == -1 and b"accumulate" in L.gsb_last_error()
+    assert _bwd(L, scene, R=-1) == -1 and b"num_rendered < 0" in L.gsb_last_error()
+    buf = (C.c_char * 256)()
+    assert _bwd(L, scene, R=1 << 30, det_ws=C.addressof(buf)) == -4 and b"2^30" in L.gsb_last_error()
+    assert _bwd(L, scene, cam_out=C.addressof(fbuf)) == -1 and b"workspace is NULL" in L.gsb_last_error()
+    assert _bwd(L, scene, raw_grads=C.byref(lib.GsbRawGrads())) == -1 and b"raw_grads given without raw" in L.gsb_last_error()
+    assert _bwd(L, scene, raw=C.byref(lib.GsbRawParams(C=4)), raw_grads=C.byref(lib.GsbRawGrads())) == -1
+    assert b"C = 4" in L.gsb_last_error()
+    # valid absgrad arguments go on to the scene checks of the backward (an empty camera is refused there); P = 0 needs no output
+    assert _bwd(L, scene) == -1 and b"image size" in L.gsb_last_error()
+    assert _bwd(L, C.byref(lib.GsbScene(P=0)), out=False) == -1 and b"image size" in L.gsb_last_error()
+
+
+def test_densify_abs_entry_points_reject_bad_arguments():
+    L = lib.lib()
+    b = (C.c_float * 64)()
+    p = C.addressof(b)
+    assert L.gsb_densify_stats_abs(-1, p, 3, p, 3, p, None, p, p, p, None, None) == -1 and b"P < 0" in L.gsb_last_error()
+    assert L.gsb_densify_stats_abs(4, p, 3, p, 1, p, None, p, p, p, None, None) == -1 and b">= 2" in L.gsb_last_error()
+    assert L.gsb_densify_stats_abs(4, p, 3, p, 3, p, p, p, p, p, None, None) == -1 and b"without max_radii2D" in L.gsb_last_error()
+    assert L.gsb_densify_stats_abs(4, p, 3, None, 3, p, None, p, p, p, None, None) == -1 and b"NULL" in L.gsb_last_error()
+    assert L.gsb_densify_stats_abs(4, p, 3, p, 3, p, None, p, None, p, None, None) == -1 and b"NULL" in L.gsb_last_error()
+    assert L.gsb_densify_stats_abs(0, None, 3, None, 3, None, None, None, None, None, None, None) == 0
+    cnt = (C.c_int64 * 8)()
+    args = lambda P, acc_abs, ws=p: (P, p, acc_abs, p, p, p, 0.1, 0.2, 0.01, 0.005, 0, 0.0, 1.0, 0.625, ws, C.addressof(cnt), None)
+    assert L.gsb_densify_plan_abs(*args(4, None)) == -1 and b"xyz_gradient_accum_abs" in L.gsb_last_error()
+    assert L.gsb_densify_plan_abs(*args(4, p, None)) == -1 and b"workspace" in L.gsb_last_error()
+    assert L.gsb_densify_plan_abs(*args(-1, p)) == -1 and b"outside" in L.gsb_last_error()
+
+
+# ---- Python refusals ---------------------------------------------------------------------------------------------------------------
+
+def _backward_call(**kw):
+    from diff_gaussian_rasterization import _C
+    P, H, W = 4, 16, 16
+    z = torch.zeros(P, 3)
+    return _C.rasterize_gaussians_backward(torch.zeros(3), z, torch.ones(P, dtype=torch.int32), torch.empty(0), z, torch.zeros(P, 4), 1.0,
+                                           torch.empty(0), torch.eye(4), torch.eye(4), 1.0, 1.0, torch.zeros(3, H, W), torch.zeros(P, 1, 3),
+                                           torch.zeros(P, 1, dtype=torch.int32), torch.zeros(3), torch.empty(0), 0, torch.empty(0),
+                                           torch.empty(0), 0.0, False, **kw)
+
+
+@pytest.mark.parametrize("kw, msg", [
+    (dict(absgrad_out=torch.zeros(4, 3), accumulate_into=tuple(torch.zeros(1) for _ in range(8))), "accumulate_into"),
+    (dict(absgrad_out=torch.zeros(4, 3), features=torch.zeros(4, 5), dL_dfeatures_out=torch.zeros(5, 16, 16)), "feature"),
+    (dict(absgrad_out=torch.zeros(5, 3)), r"shape \[P, 3\]"),
+    (dict(absgrad_out=torch.zeros(4, 2)), r"shape \[P, 3\]"),
+    (dict(absgrad_out=torch.zeros(4, 3, dtype=torch.float64)), "float32"),
+    (dict(absgrad_out=torch.zeros(3, 4).t()), "contiguous"),
+    (dict(absgrad_out=torch.zeros(4, 3)), "CUDA device"),
+    (dict(absgrad_out="no"), "tensor"),
+])
+def test_backward_refusals_leave_nothing_called(monkeypatch, kw, msg):
+    from gs_b200 import lib as gl
+    monkeypatch.setattr(gl, "lib", lambda: (_ for _ in ()).throw(AssertionError("the library was reached")))
+    with pytest.raises(RuntimeError, match=msg):
+        _backward_call(**kw)
+
+
+class _StubC:
+    """Stands in for the kernels: records every call's keywords and fills absgrad_out with a marker."""
+
+    def __init__(self):
+        self.forward_kwargs, self.backward_kwargs = [], []
+
+    def rasterize_gaussians(self, *args, **kw):
+        self.forward_kwargs.append(kw)
+        means3D, H, W = args[1], args[12], args[13]
+        P = means3D.shape[0]
+        color = (means3D.sum() * 0 + torch.ones(3, H, W)).detach()
+        return (1, color, torch.ones(P, dtype=torch.int32), torch.zeros(8, dtype=torch.uint8), torch.zeros(8, dtype=torch.uint8),
+                torch.zeros(8, dtype=torch.uint8))
+
+    def rasterize_gaussians_backward(self, *args, raw=None, absgrad_out=None, **kw):
+        self.backward_kwargs.append(dict(kw, **({} if absgrad_out is None else dict(absgrad_out=absgrad_out)),
+                                         **({} if raw is None else dict(raw=raw))))
+        P = args[1].shape[0]
+        if absgrad_out is not None:
+            absgrad_out.copy_(torch.tensor([3.0, 4.0, 0.0]).expand(P, 3))
+        if raw is not None:
+            return tuple(torch.full(s, 0.5) if s else None for s in [(P, 3), None, (P, 1), (P, 3), None, (P, 1, 3), (P, 0, 3), (P, 3), (P, 4)])
+        sh = args[13]
+        M = sh.shape[1] if sh.numel() else 0
+        return tuple(torch.full(s, 0.5) for s in [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)])
+
+
+class _CpuModel:
+    def __init__(self, P=4):
+        self.get_xyz = torch.zeros(P, 3, requires_grad=True)
+        self._opacity = torch.zeros(P, 1, requires_grad=True)
+        self._degrees = torch.zeros(P, 1, dtype=torch.int32)
+        self._scaling = torch.zeros(P, 3, requires_grad=True)
+        self._rotation = torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1).requires_grad_(True)
+        self._features_dc = torch.zeros(P, 1, 3, requires_grad=True)
+        self._features_rest = torch.zeros(P, 0, 3, requires_grad=True)
+        self.get_scaling = torch.exp(self._scaling)
+        self.get_rotation = torch.nn.functional.normalize(self._rotation)
+        self.get_features = torch.cat((self._features_dc, self._features_rest), dim=1)
+        self.active_sh_degree = self.max_sh_degree = 0
+        self.scaling_activation, self.rotation_activation = torch.exp, torch.nn.functional.normalize
+
+
+def _render(monkeypatch, fused=False, **kw):
+    import diff_gaussian_rasterization as dgr
+    from gaussian_renderer import render
+    stub = _StubC()
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
+    cam = SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=8, image_width=8, world_view_transform=torch.eye(4),
+                          full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
+    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False, fused_activations=fused)
+    pkg = render(cam, _CpuModel(), pipe, torch.zeros(3), **kw)
+    return stub, pkg
+
+
+@pytest.mark.parametrize("fused", [False, True])
+def test_render_absgrad_reaches_both_ops(monkeypatch, fused):
+    stub, pkg = _render(monkeypatch, fused, absgrad=True)
+    v = pkg["viewspace_points_abs"]
+    assert v.is_leaf and v.requires_grad and tuple(v.shape) == (4, 3) and float(v.abs().sum()) == 0
+    pkg["render"].sum().backward()
+    assert "absgrad_out" in stub.backward_kwargs[0]
+    assert torch.equal(v.grad, torch.tensor([3.0, 4.0, 0.0]).expand(4, 3))
+    assert float(pkg["viewspace_points"].grad[0, 0]) == 0.5
+    assert ("raw" in stub.backward_kwargs[0]) == fused
+
+
+@pytest.mark.parametrize("fused", [False, True])
+def test_render_without_absgrad_is_unchanged(monkeypatch, fused):
+    stub, pkg = _render(monkeypatch, fused)
+    assert "viewspace_points_abs" not in pkg
+    pkg["render"].sum().backward()
+    kw = stub.backward_kwargs[0]
+    assert "absgrad_out" not in kw
+    assert set(kw) == {"prune_mask", "dL_dinvdepth", "dL_dalpha", "camera_grads", "antialiasing"} | ({"raw"} if fused else {"quant"})
+    assert "means2D_abs" not in stub.forward_kwargs[0] and "absgrad_out" not in stub.forward_kwargs[0]
+
+
+def test_absgrad_accumulates_over_backward_calls(monkeypatch):
+    stub, pkg = _render(monkeypatch, absgrad=True)
+    pkg["render"].sum().backward(retain_graph=True)
+    pkg["render"].sum().backward()
+    assert torch.equal(pkg["viewspace_points_abs"].grad, torch.tensor([6.0, 8.0, 0.0]).expand(4, 3))
+
+
+@pytest.mark.parametrize("kw, msg", [(dict(variable_sh_bands=True), "variable-SH"), (dict(features=torch.zeros(4, 2)), "feature")])
+def test_render_refuses_absgrad_without_a_form(monkeypatch, kw, msg):
+    import diff_gaussian_rasterization as dgr
+    calls = []
+    monkeypatch.setattr(dgr._C, "rasterize_gaussians", lambda *a, **k: calls.append(1))
+    from gaussian_renderer import render
+    cam = SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=8, image_width=8, world_view_transform=torch.eye(4),
+                          full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
+    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
+    with pytest.raises(RuntimeError, match=msg):
+        render(cam, _CpuModel(), pipe, torch.zeros(3), absgrad=True, **kw)
+    assert not calls
+
+
+# ---- the float64 restatement against the oracle ---------------------------------------------------------------------------------
+
+_cache = {}
+
+
+def _run(name):
+    if name not in _cache:
+        case = BE.build(name)
+        aa = case.meta["aa"]
+        o, o64, _ = BE.oracle(case, aa=aa)
+        excl = BE.excluded(case, o)
+        signed, ab = absgrad64.pair_sums(o, case.bg.numpy(), case.dL.numpy(), case.W, case.H)
+        _cache[name] = case, o, o64, excl, signed, ab
+    return _cache[name]
+
+
+@pytest.mark.parametrize("name", BE.CASES + BE.AA_CASES)
+def test_restatement_signed_sums_are_the_oracles_means2D(name):
+    case, o, o64, excl, signed, ab = _run(name)
+    ref = np.asarray(o64["dL_dmeans2D"], np.float64).reshape(-1, 3)[:, :2]
+    vis = np.asarray(o["radii"]) > 0
+    chk = vis & ~excl
+    assert chk.sum() > 0
+    err = np.abs(signed - ref).max(axis=1)
+    row = np.maximum(np.abs(ref).max(axis=1), ab.max(axis=1))
+    # agreement to ~1e-6 of the row (the oracle recovers T by division along the list, this by a product): a pair too many or
+    # too few, or a wrong term, moves a row by orders of magnitude more
+    bar = np.maximum(1e-5 * row, 1e-8 * np.abs(ref).max())
+    assert (err[chk] <= bar[chk]).all(), (name, float((err[chk] / np.maximum(row[chk], 1e-30)).max()))
+    # the absolute sums bound the signed ones and are zero exactly where nothing was visited
+    assert (ab + 1e-12 * ab.max() >= np.abs(signed)).all()
+    assert (ab[~vis] == 0).all()
