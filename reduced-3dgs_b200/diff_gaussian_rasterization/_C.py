@@ -5,19 +5,21 @@ behaviour as rasterize_points.h:18-93; tensors in, torch.Tensors out.
 Build-defined extensions (keyword-only, SURVEY §8(b)): `prune_mask` (u8/bool [P], 1 = pruned), `quant`
 (a gs_b200.synth.QuantScene-like object with u8 id planes + [20,256] centres) and `debug_out` (dict that
 receives the forward intermediates in the reference's GeometryState layouts).  `return_maps` (forward) also renders the
-inverse-depth and alpha maps in the same pass; `dL_dinvdepth` / `dL_dalpha` (backward) take their gradients (gs_b200.h
-gsb_forward_maps / gsb_backward_maps).  `camera_grads` (backward) also returns the gradients w.r.t. viewmatrix, projmatrix and
-campos (gsb_backward_camera).  `antialiasing` (forward and backward, the same value for both) scales each Gaussian's opacity so
-that the 0.3 px^2 dilation no longer inflates sub-pixel splats (gsb_forward_antialiased / gsb_backward_antialiased).  `raw`
-(forward and backward) takes the model's leaf parameters (features_dc, features_rest, scaling, rotation) in place of sh, scales
-and rotations, and applies exp / F.normalize / the SH concatenation inside the kernels (gsb_forward_raw / gsb_backward_raw).
-`deterministic` (backward) sums the per-Gaussian gradients in a fixed order: the same bytes on every run
-(gsb_backward_deterministic).  `calculate_colours_variance` and `kmeans_cuda` take the same keyword (None: torch's
-deterministic-algorithms flag) for their statistics and centre sums (gsb_forward_statistics_deterministic, gsb_kmeans_deterministic).
-`features` (forward, also of the variable-SH entry point) composites a [P, F] fp32 tensor of per-Gaussian features over the pairs of
-the colour image, with background 0, and appends the [F, H, W] image to the outputs (gsb_forward_features); the backward's `features`
-and `dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F] (gsb_backward_features).  `absgrad_out` (backward) takes
-a [P, 3] fp32 tensor that receives the absolute screen-space gradient (gsb_backward_absgrad).
+inverse-depth and alpha maps in the same pass (gsb_forward_maps); `dL_dinvdepth` / `dL_dalpha` (backward) take their gradients.
+`camera_grads` (backward) also returns the gradients w.r.t. viewmatrix, projmatrix and campos.  `antialiasing` (forward and
+backward, the same value for both) scales each Gaussian's opacity so that the 0.3 px^2 dilation no longer inflates sub-pixel splats
+(gsb_forward_antialiased).  `raw` (forward and backward) takes the model's leaf parameters (features_dc, features_rest, scaling,
+rotation) in place of sh, scales and rotations, and applies exp / F.normalize / the SH concatenation inside the kernels
+(gsb_forward_raw).  `deterministic` (backward) sums the per-Gaussian gradients in a fixed order: the same bytes on every run.
+`calculate_colours_variance` and `kmeans_cuda` take the same keyword (None: torch's deterministic-algorithms flag) for their
+statistics and centre sums (gsb_forward_statistics_deterministic, gsb_kmeans_deterministic).  `features` (forward, also of the
+variable-SH entry point) composites a [P, F] fp32 tensor of per-Gaussian features over the pairs of the colour image, with
+background 0, and appends the [F, H, W] image to the outputs (gsb_forward_features); the backward's `features` and
+`dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F].  `absgrad_out` (backward) takes a [P, 3] fp32 tensor
+that receives the absolute screen-space gradient.
+
+The backward makes one library call whatever its keywords: gsb_backward_absgrad with `absgrad_out`, else gsb_backward_features,
+which without features is the plain backward, or the deterministic one when given its workspace.
 """
 from __future__ import annotations
 
@@ -303,21 +305,21 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     `accumulate_into`: the same 8-tuple from a previous call; gradients are added in place (view-batch accumulation);
     `view_means2D` ([P,3], accumulate mode): receives THIS view's dL_dmeans2D on its own (per-view densification statistics);
-    `dL_dinvdepth` / `dL_dalpha` ([1,H,W] each, None = zero): gradients of the maps of `return_maps` (gsb_backward_maps);
+    `dL_dinvdepth` / `dL_dalpha` ([1,H,W] each, None = zero): gradients of the maps of `return_maps`;
     `camera_grads`: the tuple (after dL_dconic when `want_conic`) ends with (dL_dviewmatrix [4,4], dL_dprojmatrix [4,4],
-    dL_dcampos [3]) in the layouts of the inputs (gsb_backward_camera); they are this view's gradients, also with `accumulate_into`;
-    `antialiasing`: the backward of a forward with `antialiasing=True` (gsb_backward_antialiased); it must match the forward's flag.
-    `raw`: the backward of a forward with the same `raw` (gsb_backward_raw).  The 8-tuple then becomes the 9-tuple
+    dL_dcampos [3]) in the layouts of the inputs; they are this view's gradients, also with `accumulate_into`;
+    `antialiasing`: the backward of a forward with `antialiasing=True`; it must match the forward's flag.
+    `raw`: the backward of a forward with the same `raw`.  The 8-tuple then becomes the 9-tuple
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, None, dL_dfeatures_dc, dL_dfeatures_rest, dL_dscaling, dL_drotation):
     the SH gradient split at coefficient 1, scaling / rotation chained through exp / F.normalize; dL_dcolors only with colors
     (else None), the SH gradients None with colors, and no dL_dcov3D.  `accumulate_into` takes that 9-tuple.
-    `deterministic`: sum the per-Gaussian gradients in a fixed order instead of with float atomics (gsb_backward_deterministic):
+    `deterministic`: sum the per-Gaussian gradients in a fixed order instead of with float atomics:
     the same inputs give the same bytes on every run, in every mode above; the values agree with the default path to rounding.
     `features` / `dL_dfeatures_out`: the [P, F] features of the forward's `features` and the gradient of its [F, H, W] image; the
-    feature image's share of the gradients is added to every output above and the tuple ends with dL_dfeatures [P, F]
-    (gsb_backward_features).  Neither `accumulate_into` nor `deterministic` has a feature form: both are refused.
+    feature image's share of the gradients is added to every output above and the tuple ends with dL_dfeatures [P, F].
+    Neither `accumulate_into` nor `deterministic` has a feature form: both are refused.
     `absgrad_out`: a contiguous fp32 [P, 3] tensor on the device, overwritten with (sum_p |g_x|, sum_p |g_y|, 0), the per-pixel terms
-    of dL_dmeans2D added as absolute values (AbsGS; gsb_backward_absgrad); every other output is the call's without it (bit for bit
+    of dL_dmeans2D added as absolute values (AbsGS); every other output is the call's without it (bit for bit
     with `deterministic`).  It has no `accumulate_into` and no feature form: both are refused before anything runs."""
     if absgrad_out is not None:
         check_absgrad_out(absgrad_out, int(means3D.shape[0]), accumulate_into, features, dL_dfeatures_out)
@@ -384,7 +386,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                 C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
                 *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4))
         stream = _lib.current_stream(device)
-        dfeat = ()
+        dfeat, fs = (), None
         if features is not None:
             dLf = f32(dL_dfeatures_out, device)
             if dLf is None or dLf.numel() != feat_F * H * W:
@@ -393,28 +395,19 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             keep += [dLf, feats]
             dfeat = (torch.empty((P, feat_F), dtype=torch.float32, device=device),)
             fs = GsbFeatures(feat_F, ptr(feats), None, dLf.data_ptr(), ptr(dfeat[0]))
-            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
-            st = L.gsb_backward_features(*head, C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None,
-                                         int(bool(antialiasing)), None, C.byref(fs), stream)
-        elif absgrad_out is not None:
-            det_ws = None
-            if deterministic:
-                det_ws = torch.empty(int(L.gsb_absgrad_deterministic_workspace_bytes(P, int(R))), dtype=torch.uint8, device=device)
-            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
-            st = L.gsb_backward_absgrad(*head, C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None,
-                                        int(bool(antialiasing)), ptr(det_ws), ptr(absgrad_out), stream)
-        elif deterministic:
+        rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
+        raw_args = (C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None, int(bool(antialiasing)))
+        det_ws = None
+        if deterministic:
             # per-instance partial slots, from the caching allocator on the current stream (freed in stream order after the call)
-            det_ws = torch.empty(int(L.gsb_deterministic_workspace_bytes(P, int(R))), dtype=torch.uint8, device=device)
-            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
-            st = L.gsb_backward_deterministic(*head, C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None,
-                                              int(bool(antialiasing)), det_ws.data_ptr(), stream)
-        elif raw is not None:
-            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]])
-            st = L.gsb_backward_raw(*head, C.byref(raw_s), C.byref(rg), int(bool(antialiasing)), stream)
+            ws_bytes = L.gsb_absgrad_deterministic_workspace_bytes if absgrad_out is not None else L.gsb_deterministic_workspace_bytes
+            det_ws = torch.empty(int(ws_bytes(P, int(R))), dtype=torch.uint8, device=device)
+        if absgrad_out is not None:
+            st = L.gsb_backward_absgrad(*head, *raw_args, ptr(det_ws), ptr(absgrad_out), stream)
         else:
-            # with NULL map and camera pointers this is exactly gsb_backward / gsb_backward_maps
-            st = (L.gsb_backward_antialiased if antialiasing else L.gsb_backward_camera)(*head, stream)
+            # without features this is gsb_backward_deterministic given det_ws, else the plain backward (with NULL map and camera
+            # pointers exactly gsb_backward / gsb_backward_maps)
+            st = L.gsb_backward_features(*head, *raw_args, ptr(det_ws), C.byref(fs) if fs is not None else None, stream)
         _lib.check(st)
         if debug:
             torch.cuda.synchronize(device)

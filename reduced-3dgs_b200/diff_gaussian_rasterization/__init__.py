@@ -6,22 +6,23 @@ _RasterizeGaussians autograd op (:48-167), backed by the H100-native kernels thr
 Differences, all additive: GaussianRasterizer.forward takes keyword-only `prune_mask` and `quant`
 (fused resolution-aware prune mask / codebook de-quantisation, SURVEY §8(b)) and `return_maps` (differentiable inverse-depth
 and alpha maps from the same pass: (color, radii, invdepth, alpha)); a raster_settings.viewmatrix / projmatrix / campos
-that requires grad receives its gradient (gsb_backward_camera), where the reference silently treats the camera as a
+that requires grad receives its gradient, where the reference silently treats the camera as a
 constant; GaussianRasterizationSettings takes upstream 3DGS's trailing `antialiasing` argument (default False; the tuple keeps the
 reference's 12 fields), which turns on the opacity-compensated 2D filter in the forward and the backward; the
 forward no longer forces
 debug=True (reference :85 hard-wires a device sync after every stage); gradients are allocated uninitialised
 because the kernels write every element.  GaussianRasterizer.forward also takes keyword-only `raw_params`, the model's leaf
 tensors (features_dc, features_rest, scaling, rotation) in place of shs / scales / rotations: exp, F.normalize and the SH
-concatenation then run inside the kernels, and the gradients of the four tensors are the kernels' own outputs
-(_RasterizeGaussiansRaw).  GaussianRasterizationSettings' keyword-only `deterministic` (default: torch's deterministic-algorithms
+concatenation then run inside the kernels, and the gradients of the four tensors are the kernels' own outputs.
+GaussianRasterizationSettings' keyword-only `deterministic` (default: torch's deterministic-algorithms
 flag) selects the backward that sums each Gaussian's gradients in a fixed order (the same bytes on every run).
 GaussianRasterizer.forward's keyword-only `features` ([P, F] fp32, 1 <= F <= 256) appends the [F, H, W] image of per-Gaussian
 features composited over the colour pass with background 0; its gradient reaches the features and, through alpha, everything the
 colour gradient reaches.  The feature gradient has no deterministic form: it is refused when the deterministic mode is on.
 GaussianRasterizer.forward's keyword-only `means2D_abs` (a [P, 3] tensor that requires grad, e.g. a zeros leaf) receives as its
-gradient the absolute screen-space gradient (sum_p |g_x|, sum_p |g_y|, 0) of AbsGS (gsb_backward_absgrad), the densification
+gradient the absolute screen-space gradient (sum_p |g_x|, sum_p |g_y|, 0) of AbsGS, the densification
 statistic whose per-pixel terms cannot cancel; it has no feature form.
+Every option goes through the one autograd op, _RasterizeGaussians, each optional input in a slot of its own.
 """
 from typing import NamedTuple
 
@@ -49,51 +50,12 @@ def _call(fn, args, kw, dump, message):
         raise ex
 
 
-def _apply(op, raster_settings, *args, features=None, means2D_abs=None):
-    camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
-    feat = () if features is None else (features,)
-    if means2D_abs is not None:
-        # means2D_abs is the op's last input, after the features' slot (None when absent)
-        feat = (features, means2D_abs)
-    if torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera):
-        # a learnable camera: the three tensors become inputs of the autograd op so that their gradients have a destination
-        return op.apply(*args, *camera, *feat)
-    # the features, when given, are the op's last input (after three absent camera slots)
-    return op.apply(*args, *((None,) * 3 + feat if feat else ()))
-
-
-def _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, camera, features=None, means2D_abs=None, **kw):
-    """The forward both ops share: the _C call and the ctx state their backwards read.  `camera` is (viewmatrix, projmatrix,
-    campos), raster_settings' own tensors, passed again as inputs only when the camera is learnable, else (None, None, None).
-    -> (_C.rasterize_gaussians' tuple, the op's outputs: (color, radii) or, with return_maps, (color, radii, invdepth, alpha);
-    with `features` the feature image [F, H, W] comes last)."""
-    ctx.camera_meta = None if camera[0] is None else [(t.shape, t.dtype) for t in camera]
-    ctx.return_maps, ctx.has_features, ctx.has_abs = return_maps, features is not None, means2D_abs is not None
-    kw.update(prune_mask=prune_mask, return_maps=return_maps, antialiasing=raster_settings.antialiasing)
-    if features is not None:
-        kw.update(features=features)
-    out = _call(_C.rasterize_gaussians, args, kw,
-                "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
-    ctx.raster_settings = raster_settings
-    ctx.num_rendered = out[0]
-    ctx.lambda_sh_sparsity = lambda_sh_sparsity
-    ctx.prune_mask = prune_mask
-    ctx.mark_non_differentiable(out[2])
-    feat = (out[-1],) if features is not None else ()
-    if return_maps or features is not None:
-        # a loss on some outputs only: the others' gradients arrive as None and reach the kernels as NULL (zero), and a feature
-        # image without a gradient leaves the backward exactly the call without features
-        ctx.set_materialize_grads(False)
-    if return_maps:
-        return out, (out[1], out[2], out[6], out[7]) + feat
-    return out, (out[1], out[2]) + feat
-
-
-def _split_grads(ctx, grads):
-    """The incoming gradients after (color, radii) -> (grad_invdepth, grad_alpha, grad_features), None where absent."""
-    grads = list(grads)
-    maps = (grads.pop(0), grads.pop(0)) if ctx.return_maps else (None, None)
-    return maps + (grads.pop(0) if ctx.has_features else None,)
+# The autograd op's inputs, in the order of its forward's parameters: the reference's fourteen (means3D ... cov3Ds_precomp,
+# raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps), then one slot per optional input.  A call that uses no
+# optional input passes the first fourteen only.
+MEANS3D, MEANS2D, SH, DEGREES, COLORS, OPACITIES, SCALES, ROTATIONS, COV3D = range(9)
+VIEWMATRIX, PROJMATRIX, CAMPOS, FEATURES, MEANS2D_ABS, FEATURES_DC, FEATURES_REST, SCALING, ROTATION = range(14, 23)
+N_INPUTS = 23
 
 
 def _deterministic(raster_settings):
@@ -103,150 +65,104 @@ def _deterministic(raster_settings):
     return torch.are_deterministic_algorithms_enabled() if d is None else bool(d)
 
 
-def _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, scales, rotations, cov3Ds_precomp,
-              sh, degrees, geomBuffer, binningBuffer, imgBuffer, features=None, grad_features=None, **kw):
-    """The backward both ops share: the _C call from the saved state.  -> (its gradient tuple, the gradients of the camera
-    inputs: () for a constant camera, else one per tensor, None where not needed, dL_dfeatures or None)."""
-    rs = ctx.raster_settings
-    if grad_out_color is None:
-        grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
-    # the camera tensors are the op's last three inputs when it has them (followed by the features when given, and by the
-    # features' slot and means2D_abs with absgrad)
-    n = len(ctx.needs_input_grad) - (2 if ctx.has_abs else 1 if ctx.has_features else 0)
-    camera_need = ctx.needs_input_grad[n - 3:n] if ctx.camera_meta is not None else (False, False, False)
-    args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
-            rs.tanfovx, rs.tanfovy, grad_out_color, sh, degrees, rs.campos, geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer,
-            ctx.lambda_sh_sparsity, rs.debug)
-    kw.update(prune_mask=ctx.prune_mask, dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha, camera_grads=any(camera_need),
-              antialiasing=rs.antialiasing)
-    if _deterministic(rs):
-        kw.update(deterministic=True)
-    if grad_features is not None:
-        kw.update(features=features, dL_dfeatures_out=grad_features)
-    dabs = None
-    if ctx.has_abs:
-        dabs = torch.empty((means3D.shape[0], 3), dtype=torch.float32, device=means3D.device)
-        kw.update(absgrad_out=dabs)
-    g = _call(_C.rasterize_gaussians_backward, args, kw,
-              "snapshot_bw.dump", "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
-    dfeat = None
-    if grad_features is not None:
-        g, dfeat = g[:-1], g[-1]                                       # dL_dfeatures comes last
-    ctx.grad_abs = dabs
-    if ctx.camera_meta is None:
-        # the features' gradient (and means2D_abs's) follows three absent camera slots
-        return g, (None,) * 3 if ctx.has_features or ctx.has_abs else (), dfeat
-    # with camera_grads the tuple ends with (dL_dviewmatrix, dL_dprojmatrix, dL_dcampos)
-    return g, tuple(gc.reshape(shape).to(dtype) if n else None
-                    for gc, n, (shape, dtype) in zip(g[-3:] if any(camera_need) else (None,) * 3, camera_need, ctx.camera_meta)), dfeat
-
-
-def _tail(ctx, grad_feat):
-    """The gradients of the op's inputs after the camera: the features (when given, or their absent slot before means2D_abs) and
-    means2D_abs, whose gradient is the absolute screen-space gradient."""
-    need = ctx.needs_input_grad
-    if ctx.has_abs:
-        return (grad_feat if ctx.has_features and need[-2] else None, ctx.grad_abs if need[-1] else None)
-    return (grad_feat if need[-1] else None,) if ctx.has_features else ()
-
-
 def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, features=None,
-                        means2D_abs=None):
-    return _apply(_RasterizeGaussians, raster_settings, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations,
-                  cov3Ds_precomp, raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features=features,
-                  means2D_abs=means2D_abs)
+                        means2D_abs=None, raw_params=None):
+    camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
+    if not (torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera)):
+        # a constant camera is read from raster_settings; a learnable one is also an input, so that its gradients have a destination
+        camera = (None,) * 3
+    optional = (*camera, features, means2D_abs, *(raw_params or (None,) * 4))
+    return _RasterizeGaussians.apply(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                                     raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps,
+                                     *(optional if any(t is not None for t in optional) else ()))
 
 
 class _RasterizeGaussians(torch.autograd.Function):
+    """The reference's op with the optional inputs above.  `viewmatrix` / `projmatrix` / `campos` are raster_settings' own tensors,
+    given only when the camera is learnable.  `features_dc` [P,1,3], `features_rest` [P,C,3] (both None with colors_precomp),
+    `scaling` [P,3] (log-scales) and `rotation` [P,4] (unnormalised) are the model's leaf tensors in place of sh, scales and rotations
+    (then empty): the kernels apply get_features / get_scaling / get_rotation themselves and return the gradients of these four
+    tensors directly, so the graph holds no Cat / Exp / Div node and no [P,16,3] copy or gradient exists.
+    -> (color, radii), with return_maps (color, radii, invdepth, alpha); with `features` the feature image [F, H, W] comes last."""
+
     @staticmethod
-    def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, viewmatrix=None,
-                projmatrix=None, campos=None, features=None, means2D_abs=None):
-        args = (raster_settings.bg, means3D, colors_precomp, opacities, scales, rotations, raster_settings.scale_modifier,
-                cov3Ds_precomp, raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx,
-                raster_settings.tanfovy, raster_settings.image_height, raster_settings.image_width, sh, degrees,
-                raster_settings.campos, raster_settings.prefiltered, raster_settings.debug)
-        out, outputs = _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, (viewmatrix, projmatrix, campos),
-                                features, means2D_abs, quant=quant)
-        ctx.quant = quant
+    def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
+                lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None,
+                features=None, means2D_abs=None, features_dc=None, features_rest=None, scaling=None, rotation=None):
+        rs = raster_settings
+        args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
+                rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, degrees, rs.campos, rs.prefiltered, rs.debug)
+        ctx.raw = scaling is not None
+        kw = dict(raw=(features_dc, features_rest, scaling, rotation)) if ctx.raw else dict(quant=quant)
+        kw.update(prune_mask=prune_mask, return_maps=return_maps, antialiasing=rs.antialiasing)
+        if features is not None:
+            kw.update(features=features)
+        out = _call(_C.rasterize_gaussians, args, kw,
+                    "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
+        ctx.raster_settings, ctx.num_rendered, ctx.lambda_sh_sparsity = rs, out[0], lambda_sh_sparsity
+        ctx.prune_mask, ctx.quant, ctx.return_maps, ctx.has_features = prune_mask, quant, return_maps, features is not None
+        ctx.has_abs = means2D_abs is not None
+        ctx.camera_meta = None if viewmatrix is None else [(t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos)]
+        ctx.mark_non_differentiable(out[2])
+        if return_maps or features is not None:
+            # a loss on some outputs only: the others' gradients arrive as None and reach the kernels as NULL (zero), and a feature
+            # image without a gradient leaves the backward exactly the call without features
+            ctx.set_materialize_grads(False)
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, out[2], sh, out[3], out[4], out[5], degrees,
-                              features)
-        return outputs
+                              features, features_dc, features_rest, scaling, rotation)
+        return (out[1], out[2]) + (out[6:8] if return_maps else ()) + (out[-1:] if features is not None else ())
 
     @staticmethod
     def backward(ctx, grad_out_color, _, *grads):
-        grad_invdepth, grad_alpha, grad_features = _split_grads(ctx, grads)
-        (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer,
-         degrees, features) = ctx.saved_tensors
-        g, grad_camera, grad_feat = _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, scales,
-                                              rotations, cov3Ds_precomp, sh, degrees, geomBuffer, binningBuffer, imgBuffer, features,
-                                              grad_features, quant=ctx.quant)
-        (grad_means2D, grad_colors_precomp, grad_opacities, grad_means3D, grad_cov3Ds_precomp, grad_sh, grad_scales,
-         grad_rotations) = g[:8]
+        # after (color, radii): the maps' gradients with return_maps, then the feature image's when given
+        grad_invdepth, grad_alpha = grads[:2] if ctx.return_maps else (None, None)
+        grad_features = grads[-1] if ctx.has_features else None
+        (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer, degrees, features,
+         features_dc, features_rest, scaling, rotation) = ctx.saved_tensors
+        rs = ctx.raster_settings
+        if grad_out_color is None:
+            grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
+        need = ctx.needs_input_grad + (False,) * (N_INPUTS - len(ctx.needs_input_grad))
+        args = (rs.bg, means3D, radii, colors_precomp, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix, rs.projmatrix,
+                rs.tanfovx, rs.tanfovy, grad_out_color, sh, degrees, rs.campos, geomBuffer, ctx.num_rendered, binningBuffer, imgBuffer,
+                ctx.lambda_sh_sparsity, rs.debug)
+        kw = dict(raw=(features_dc, features_rest, scaling, rotation)) if ctx.raw else dict(quant=ctx.quant)
+        kw.update(prune_mask=ctx.prune_mask, dL_dinvdepth=grad_invdepth, dL_dalpha=grad_alpha,
+                  camera_grads=any(need[VIEWMATRIX:CAMPOS + 1]), antialiasing=rs.antialiasing)
+        if _deterministic(rs):
+            kw.update(deterministic=True)
+        if grad_features is not None:
+            kw.update(features=features, dL_dfeatures_out=grad_features)
+        out = [None] * N_INPUTS
+        if ctx.has_abs:
+            out[MEANS2D_ABS] = torch.empty((means3D.shape[0], 3), dtype=torch.float32, device=means3D.device)
+            kw.update(absgrad_out=out[MEANS2D_ABS])
+        g = _call(_C.rasterize_gaussians_backward, args, kw,
+                  "snapshot_bw.dump", "\nAn error occured in backward. Writing snapshot_bw.dump for debugging.\n")
+        # the 8-tuple, or the raw 9-tuple; then the camera gradients (camera_grads) and dL_dfeatures (features)
+        if ctx.raw:
+            (out[MEANS2D], out[COLORS], out[OPACITIES], out[MEANS3D], _, out[FEATURES_DC], out[FEATURES_REST], out[SCALING],
+             out[ROTATION]) = g[:9]
+        else:
+            out[MEANS2D], out[COLORS], out[OPACITIES], out[MEANS3D], out[COV3D], out[SH], out[SCALES], out[ROTATIONS] = g[:8]
+        if kw["camera_grads"]:
+            k = 9 if ctx.raw else 8
+            for i, (t, (shape, dtype)) in enumerate(zip(g[k:k + 3], ctx.camera_meta)):
+                out[VIEWMATRIX + i] = t.reshape(shape).to(dtype)
+        if grad_features is not None:
+            out[FEATURES] = g[-1]
         if ctx.quant is not None:
             # inputs were id planes: the per-Gaussian attribute gradients have no autograd destination; expose them with the
             # semantics of `.grad`: they accumulate over backward calls until the caller resets `quant.grads = None`
-            new = dict(sh=grad_sh, opacity=grad_opacities, scales=grad_scales, rotations=grad_rotations)
+            new = dict(sh=out[SH], opacity=out[OPACITIES], scales=out[SCALES], rotations=out[ROTATIONS])
             old = getattr(ctx.quant, "grads", None)
             if old:
                 for k, t in new.items():
                     old[k].add_(t)
             else:
                 ctx.quant.grads = new
-        need = ctx.needs_input_grad
-        return (grad_means3D, grad_means2D, grad_sh if need[2] else None, None,
-                grad_colors_precomp if need[4] else None, grad_opacities if need[5] else None,
-                grad_scales if need[6] else None, grad_rotations if need[7] else None,
-                grad_cov3Ds_precomp if need[8] else None, None, None, None, None, None) + grad_camera + _tail(ctx, grad_feat)
-
-
-def rasterize_gaussians_raw(means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
-                            raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, features=None, means2D_abs=None):
-    """rasterize_gaussians on the model's raw parameters (see _RasterizeGaussiansRaw)."""
-    return _apply(_RasterizeGaussiansRaw, raster_settings, means3D, means2D, features_dc, features_rest, degrees, colors_precomp,
-                  opacities, scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, features=features,
-                  means2D_abs=means2D_abs)
-
-
-class _RasterizeGaussiansRaw(torch.autograd.Function):
-    """_RasterizeGaussians with the model's leaf tensors as inputs: features_dc [P,1,3], features_rest [P,C,3] (empty with
-    colors_precomp), scaling [P,3] (log-scales), rotation [P,4] (unnormalised).  The kernels apply get_features / get_scaling /
-    get_rotation themselves and return the gradients of these four tensors directly, so the graph holds no Cat / Exp / Div node
-    and no [P,16,3] copy or gradient exists.  Outputs, camera handling and `return_maps` as in _RasterizeGaussians."""
-
-    @staticmethod
-    def forward(ctx, means3D, means2D, features_dc, features_rest, degrees, colors_precomp, opacities, scaling, rotation,
-                raster_settings, lambda_sh_sparsity, prune_mask=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None,
-                features=None, means2D_abs=None):
-        empty = torch.Tensor([])
-        with_colors = colors_precomp.numel() > 0
-        raw = (None, None, scaling, rotation) if with_colors else (features_dc, features_rest, scaling, rotation)
-        args = (raster_settings.bg, means3D, colors_precomp, opacities, empty, empty, raster_settings.scale_modifier, empty,
-                raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
-                raster_settings.image_height, raster_settings.image_width, empty, degrees, raster_settings.campos,
-                raster_settings.prefiltered, raster_settings.debug)
-        out, outputs = _forward(ctx, args, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, (viewmatrix, projmatrix, campos),
-                                features, means2D_abs, raw=raw)
-        ctx.with_colors = with_colors
-        ctx.save_for_backward(colors_precomp, means3D, features_dc, features_rest, scaling, rotation, out[2], out[3], out[4], out[5],
-                              degrees, features)
-        return outputs
-
-    @staticmethod
-    def backward(ctx, grad_out_color, _, *grads):
-        grad_invdepth, grad_alpha, grad_features = _split_grads(ctx, grads)
-        (colors_precomp, means3D, features_dc, features_rest, scaling, rotation, radii, geomBuffer, binningBuffer, imgBuffer,
-         degrees, features) = ctx.saved_tensors
-        empty = torch.Tensor([])
-        raw = (None, None, scaling, rotation) if ctx.with_colors else (features_dc, features_rest, scaling, rotation)
-        g, grad_camera, grad_feat = _backward(ctx, grad_out_color, grad_invdepth, grad_alpha, means3D, radii, colors_precomp, empty, empty,
-                                              empty, empty, degrees, geomBuffer, binningBuffer, imgBuffer, features, grad_features, raw=raw)
-        (grad_means2D, grad_colors, grad_opacities, grad_means3D, _, grad_dc, grad_rest, grad_scaling, grad_rotation) = g[:9]
-        need = ctx.needs_input_grad
-        return (grad_means3D, grad_means2D, grad_dc if need[2] else None, grad_rest if need[3] else None, None,
-                grad_colors if need[5] else None, grad_opacities if need[6] else None, grad_scaling if need[7] else None,
-                grad_rotation if need[8] else None, None, None, None, None) + grad_camera + _tail(ctx, grad_feat)
+        return tuple(t if n else None for t, n in zip(out, need))
 
 
 class _ReferenceSettings(NamedTuple):
@@ -318,15 +234,16 @@ class GaussianRasterizer(nn.Module):
             if not isinstance(means2D_abs, torch.Tensor) or tuple(means2D_abs.shape) != (int(means3D.shape[0]), 3):
                 raise RuntimeError(f"means2D_abs must be a [P, 3] tensor with P = {int(means3D.shape[0])}")
         if features is not None:
-            _C.check_features(features, int(means3D.shape[0]), cuda=False)
-            if features.requires_grad and torch.is_grad_enabled() and _deterministic(raster_settings):
+            refuse = getattr(features, "requires_grad", False) and torch.is_grad_enabled() and _deterministic(raster_settings)
+            # a deterministic feature gradient is refused after the other checks but before the device is looked at
+            _C.check_features(features, int(means3D.shape[0]), cuda=not refuse)
+            if refuse:
                 raise RuntimeError("features: the feature gradient has no deterministic form; detach the features or turn the "
                                    "deterministic mode off")
-            _C.check_features(features, int(means3D.shape[0]))
         if raw_params is not None:
             if quant is not None or any(t is not None for t in (shs, scales, rotations, cov3D_precomp)):
                 raise Exception('raw_params replace shs, scales and rotations; leave those, cov3D_precomp and quant None')
-            features_dc, features_rest, scaling, rotation = raw_params
+            features_dc, features_rest, _, _ = raw_params
             # the SHs are the two feature tensors, and an empty colors_precomp counts as none (the raw op reads it so)
             sh, with_colors = (features_dc, features_rest), colors_precomp is not None and colors_precomp.numel() > 0
         else:
@@ -339,10 +256,6 @@ class GaussianRasterizer(nn.Module):
                 raise Exception('Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!')
         empty = torch.Tensor([])
         e = lambda t: empty if t is None else t                                  # absent inputs travel as empty tensors
-        if raw_params is not None:
-            return rasterize_gaussians_raw(means3D, means2D, e(features_dc), e(features_rest), degrees, e(colors_precomp), e(opacities),
-                                           scaling, rotation, raster_settings, lambda_sh_sparsity, prune_mask, return_maps, features,
-                                           means2D_abs)
         return rasterize_gaussians(means3D, means2D, e(shs), degrees, e(colors_precomp), e(opacities), e(scales), e(rotations),
                                    e(cov3D_precomp), raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features,
-                                   means2D_abs)
+                                   means2D_abs, raw_params)

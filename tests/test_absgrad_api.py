@@ -5,7 +5,6 @@ leaving the calls without it exactly as they were; and the float64 restatement o
 signs, to the fp64 oracle's dL_dmeans2D on the backward-edge scenes, which pins it to the pairs and terms the oracle uses."""
 import ctypes as C
 import math
-from types import SimpleNamespace
 
 import numpy as np
 import pytest
@@ -13,6 +12,7 @@ import torch
 
 import absgrad64
 import backward_edges as BE
+import stub_c
 from gs_b200 import lib
 
 NEW = ("gsb_backward_absgrad", "gsb_absgrad_deterministic_workspace_bytes", "gsb_densify_stats_abs", "gsb_densify_plan_abs")
@@ -108,59 +108,10 @@ def test_backward_refusals_leave_nothing_called(monkeypatch, kw, msg):
         _backward_call(**kw)
 
 
-class _StubC:
-    """Stands in for the kernels: records every call's keywords and fills absgrad_out with a marker."""
-
-    def __init__(self):
-        self.forward_kwargs, self.backward_kwargs = [], []
-
-    def rasterize_gaussians(self, *args, **kw):
-        self.forward_kwargs.append(kw)
-        means3D, H, W = args[1], args[12], args[13]
-        P = means3D.shape[0]
-        color = (means3D.sum() * 0 + torch.ones(3, H, W)).detach()
-        return (1, color, torch.ones(P, dtype=torch.int32), torch.zeros(8, dtype=torch.uint8), torch.zeros(8, dtype=torch.uint8),
-                torch.zeros(8, dtype=torch.uint8))
-
-    def rasterize_gaussians_backward(self, *args, raw=None, absgrad_out=None, **kw):
-        self.backward_kwargs.append(dict(kw, **({} if absgrad_out is None else dict(absgrad_out=absgrad_out)),
-                                         **({} if raw is None else dict(raw=raw))))
-        P = args[1].shape[0]
-        if absgrad_out is not None:
-            absgrad_out.copy_(torch.tensor([3.0, 4.0, 0.0]).expand(P, 3))
-        if raw is not None:
-            return tuple(torch.full(s, 0.5) if s else None for s in [(P, 3), None, (P, 1), (P, 3), None, (P, 1, 3), (P, 0, 3), (P, 3), (P, 4)])
-        sh = args[13]
-        M = sh.shape[1] if sh.numel() else 0
-        return tuple(torch.full(s, 0.5) for s in [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)])
-
-
-class _CpuModel:
-    def __init__(self, P=4):
-        self.get_xyz = torch.zeros(P, 3, requires_grad=True)
-        self._opacity = torch.zeros(P, 1, requires_grad=True)
-        self._degrees = torch.zeros(P, 1, dtype=torch.int32)
-        self._scaling = torch.zeros(P, 3, requires_grad=True)
-        self._rotation = torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1).requires_grad_(True)
-        self._features_dc = torch.zeros(P, 1, 3, requires_grad=True)
-        self._features_rest = torch.zeros(P, 0, 3, requires_grad=True)
-        self.get_scaling = torch.exp(self._scaling)
-        self.get_rotation = torch.nn.functional.normalize(self._rotation)
-        self.get_features = torch.cat((self._features_dc, self._features_rest), dim=1)
-        self.active_sh_degree = self.max_sh_degree = 0
-        self.scaling_activation, self.rotation_activation = torch.exp, torch.nn.functional.normalize
-
-
 def _render(monkeypatch, fused=False, **kw):
-    import diff_gaussian_rasterization as dgr
     from gaussian_renderer import render
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
-    cam = SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=8, image_width=8, world_view_transform=torch.eye(4),
-                          full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
-    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False, fused_activations=fused)
-    pkg = render(cam, _CpuModel(), pipe, torch.zeros(3), **kw)
+    stub = stub_c.StubC().install(monkeypatch)
+    pkg = render(stub_c.camera(), stub_c.Model(), stub_c.pipe(fused_activations=fused), torch.zeros(3), **kw)
     return stub, pkg
 
 
@@ -170,10 +121,10 @@ def test_render_absgrad_reaches_both_ops(monkeypatch, fused):
     v = pkg["viewspace_points_abs"]
     assert v.is_leaf and v.requires_grad and tuple(v.shape) == (4, 3) and float(v.abs().sum()) == 0
     pkg["render"].sum().backward()
-    assert "absgrad_out" in stub.backward_kwargs[0]
-    assert torch.equal(v.grad, torch.tensor([3.0, 4.0, 0.0]).expand(4, 3))
-    assert float(pkg["viewspace_points"].grad[0, 0]) == 0.5
-    assert ("raw" in stub.backward_kwargs[0]) == fused
+    assert "absgrad_out" in stub.backward_calls[0][1]
+    assert torch.equal(v.grad, stub_c.marked("absgrad", (4, 3)))
+    assert float(pkg["viewspace_points"].grad[0, 0]) == stub_c.MARK["dL_dmeans2D"]
+    assert ("raw" in stub.backward_calls[0][1]) == fused
 
 
 @pytest.mark.parametrize("fused", [False, True])
@@ -181,31 +132,26 @@ def test_render_without_absgrad_is_unchanged(monkeypatch, fused):
     stub, pkg = _render(monkeypatch, fused)
     assert "viewspace_points_abs" not in pkg
     pkg["render"].sum().backward()
-    kw = stub.backward_kwargs[0]
+    kw = stub.backward_calls[0][1]
     assert "absgrad_out" not in kw
     assert set(kw) == {"prune_mask", "dL_dinvdepth", "dL_dalpha", "camera_grads", "antialiasing"} | ({"raw"} if fused else {"quant"})
-    assert "means2D_abs" not in stub.forward_kwargs[0] and "absgrad_out" not in stub.forward_kwargs[0]
+    assert "means2D_abs" not in stub.forward_calls[0][1] and "absgrad_out" not in stub.forward_calls[0][1]
 
 
 def test_absgrad_accumulates_over_backward_calls(monkeypatch):
     stub, pkg = _render(monkeypatch, absgrad=True)
     pkg["render"].sum().backward(retain_graph=True)
     pkg["render"].sum().backward()
-    assert torch.equal(pkg["viewspace_points_abs"].grad, torch.tensor([6.0, 8.0, 0.0]).expand(4, 3))
+    assert torch.equal(pkg["viewspace_points_abs"].grad, 2 * stub_c.marked("absgrad", (4, 3)))
 
 
 @pytest.mark.parametrize("kw, msg", [(dict(variable_sh_bands=True), "variable-SH"), (dict(features=torch.zeros(4, 2)), "feature")])
 def test_render_refuses_absgrad_without_a_form(monkeypatch, kw, msg):
-    import diff_gaussian_rasterization as dgr
-    calls = []
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", lambda *a, **k: calls.append(1))
     from gaussian_renderer import render
-    cam = SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=8, image_width=8, world_view_transform=torch.eye(4),
-                          full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
-    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
+    stub = stub_c.StubC().install(monkeypatch)
     with pytest.raises(RuntimeError, match=msg):
-        render(cam, _CpuModel(), pipe, torch.zeros(3), absgrad=True, **kw)
-    assert not calls
+        render(stub_c.camera(), stub_c.Model(), stub_c.pipe(), torch.zeros(3), absgrad=True, **kw)
+    assert not stub.calls
 
 
 # ---- the float64 restatement against the oracle ---------------------------------------------------------------------------------

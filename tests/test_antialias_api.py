@@ -2,11 +2,11 @@
 call, refusal of CPU tensors, and the plumbing of the `antialiasing` flag from GaussianRasterizationSettings and `pipe` to both
 kernels, checked against a stub of `_C` (no GPU, no kernel)."""
 import ctypes as C
-from types import SimpleNamespace
 
 import pytest
 import torch
 
+import stub_c
 from gs_b200 import lib
 
 
@@ -88,40 +88,10 @@ def test_settings_default_to_no_antialiasing():
     assert s._replace(antialiasing=True).antialiasing is True and s._replace(image_height=4).image_height == 4
 
 
-class _StubC:
-    """Stands in for the kernels: records the `antialiasing` keyword of each call and returns outputs of the right shapes."""
-
-    def __init__(self):
-        self.forward_aa, self.backward_aa, self.variable_sh_aa = [], [], []
-
-    def rasterize_gaussians(self, *args, antialiasing=False, return_maps=False, **kw):
-        self.forward_aa.append(antialiasing)
-        means3D, H, W = args[1], args[12], args[13]
-        P = means3D.shape[0]
-        color = torch.ones(3, H, W)
-        out = (1, color, torch.ones(P, dtype=torch.int32), torch.zeros(8, dtype=torch.uint8), torch.zeros(8, dtype=torch.uint8),
-               torch.zeros(8, dtype=torch.uint8))
-        return out + ((torch.zeros(1, H, W), torch.zeros(1, H, W)) if return_maps else ())
-
-    def rasterize_gaussians_backward(self, *args, antialiasing=False, **kw):
-        self.backward_aa.append(antialiasing)
-        means3D, sh = args[1], args[13]
-        P = means3D.shape[0]
-        M = sh.shape[1] if sh.numel() else 0
-        return tuple(torch.full(s, 0.5) for s in [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)])
-
-    def rasterize_gaussians_variableSH_bands(self, *args, antialiasing=False, **kw):
-        self.variable_sh_aa.append(antialiasing)
-        H, W, P = args[12], args[13], args[1].shape[0]
-        return (1, torch.ones(3, H, W), torch.ones(P, dtype=torch.int32), None, None, None)
-
-
 @pytest.mark.parametrize("aa", [False, True])
 def test_settings_flag_reaches_forward_and_backward(monkeypatch, aa):
     import diff_gaussian_rasterization as dgr
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
+    stub = stub_c.StubC().install(monkeypatch)
     P = 5
     settings = dgr.GaussianRasterizationSettings(8, 8, 0.5, 0.5, torch.zeros(3), 1.0, torch.eye(4), torch.eye(4), 0, torch.zeros(3),
                                                  False, False, antialiasing=aa)
@@ -131,38 +101,20 @@ def test_settings_flag_reaches_forward_and_backward(monkeypatch, aa):
                                                 degrees=torch.zeros(P, 1, dtype=torch.int32), scales=torch.ones(P, 3),
                                                 rotations=torch.ones(P, 4))
     (color * 1.0).sum().backward()
-    assert stub.forward_aa == [aa] and stub.backward_aa == [aa]
-    assert float(opac.grad[0, 0]) == 0.5 and float(means.grad[0, 0]) == 0.5
-
-
-class _Model:
-    def __init__(self, P=4):
-        self.get_xyz = torch.zeros(P, 3)
-        self._opacity = torch.zeros(P, 1)
-        self._degrees = torch.zeros(P, 1, dtype=torch.int32)
-        self.get_scaling = torch.ones(P, 3)
-        self.get_rotation = torch.ones(P, 4)
-        self.get_features = torch.zeros(P, 1, 3)
-        self.active_sh_degree = self.max_sh_degree = 0
-        self.per_band_count = [P, 0, 0, 0]
-
-
-def _camera():
-    return SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=8, image_width=8, world_view_transform=torch.eye(4),
-                           full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
+    assert [kw["antialiasing"] for _, kw in stub.forward_calls] == [aa]
+    assert [kw["antialiasing"] for _, kw in stub.backward_calls] == [aa]
+    assert float(opac.grad[0, 0]) == stub_c.MARK["dL_dopacity"] and float(means.grad[0, 0]) == stub_c.MARK["dL_dmeans3D"]
 
 
 @pytest.mark.parametrize("pipe_aa", [None, False, True])
 def test_render_takes_the_flag_from_pipe(monkeypatch, pipe_aa):
-    import diff_gaussian_rasterization as dgr
     import gaussian_renderer
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
-    monkeypatch.setattr(gaussian_renderer, "rasterize_gaussians_variableSH_bands", stub.rasterize_gaussians_variableSH_bands)
-    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
+    stub = stub_c.StubC().install(monkeypatch)
+    pipe = stub_c.pipe()
     if pipe_aa is not None:
         pipe.antialiasing = pipe_aa
     want = bool(pipe_aa)                                    # a pipe without the attribute (reduced-3dgs's) renders without
-    gaussian_renderer.render(_camera(), _Model(), pipe, torch.zeros(3))
-    gaussian_renderer.render(_camera(), _Model(), pipe, torch.zeros(3), variable_sh_bands=True)
-    assert stub.forward_aa == [want] and stub.variable_sh_aa == [want]
+    gaussian_renderer.render(stub_c.camera(), stub_c.Model(), pipe, torch.zeros(3))
+    gaussian_renderer.render(stub_c.camera(), stub_c.Model(), pipe, torch.zeros(3), variable_sh_bands=True)
+    assert [kw["antialiasing"] for _, kw in stub.forward_calls] == [want]
+    assert [kw["antialiasing"] for _, kw in stub.variable_sh_calls] == [want]

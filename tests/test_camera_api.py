@@ -5,6 +5,7 @@ import ctypes as C
 import pytest
 import torch
 
+import stub_c
 from gs_b200 import lib
 
 
@@ -52,38 +53,9 @@ def test_camera_grads_refuse_cpu_tensors():
                                         torch.empty(0), 0.0, False, camera_grads=True)
 
 
-class _StubC:
-    """Stands in for the kernels: records the keyword arguments of each backward and returns gradients of the right shapes."""
-
-    def __init__(self):
-        self.backward_kwargs = []
-
-    def rasterize_gaussians(self, *args, prune_mask=None, quant=None, return_maps=False, **kw):
-        means3D, H, W = args[1], args[12], args[13]
-        P = means3D.shape[0]
-        color = (means3D.sum() * 0 + torch.ones(3, H, W)).detach()
-        out = (1, color, torch.ones(P, dtype=torch.int32), torch.zeros(8, dtype=torch.uint8), torch.zeros(8, dtype=torch.uint8),
-               torch.zeros(8, dtype=torch.uint8))
-        if return_maps:
-            out += (torch.zeros(1, H, W), torch.zeros(1, H, W))
-        return out
-
-    def rasterize_gaussians_backward(self, *args, camera_grads=False, **kw):
-        self.backward_kwargs.append(dict(kw, camera_grads=camera_grads))
-        means3D, sh = args[1], args[13]
-        P = means3D.shape[0]
-        M = sh.shape[1] if sh.numel() else 0
-        res = tuple(torch.full(s, 0.5) for s in [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)])
-        if camera_grads:
-            res += (torch.arange(16.0).view(4, 4), torch.arange(16.0).view(4, 4) + 100, torch.tensor([7.0, 8.0, 9.0]))
-        return res
-
-
 def _render(monkeypatch, view, proj, campos):
     import diff_gaussian_rasterization as dgr
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
+    stub = stub_c.StubC().install(monkeypatch)
     P = 5
     settings = dgr.GaussianRasterizationSettings(image_height=8, image_width=8, tanfovx=0.5, tanfovy=0.5, bg=torch.zeros(3),
                                                  scale_modifier=1.0, viewmatrix=view, projmatrix=proj, sh_degree=0, campos=campos,
@@ -93,14 +65,14 @@ def _render(monkeypatch, view, proj, campos):
                                                     shs=torch.zeros(P, 1, 3), degrees=torch.zeros(P, 1, dtype=torch.int32),
                                                     scales=torch.ones(P, 3), rotations=torch.ones(P, 4))
     color.sum().backward()
-    assert means.grad is not None and float(means.grad[0, 0]) == 0.5
+    assert means.grad is not None and float(means.grad[0, 0]) == stub_c.MARK["dL_dmeans3D"]
     return stub
 
 
 def test_constant_camera_passes_camera_grads_false(monkeypatch):
     view, proj, campos = torch.eye(4), torch.eye(4), torch.zeros(3)
     stub = _render(monkeypatch, view, proj, campos)
-    assert len(stub.backward_kwargs) == 1 and stub.backward_kwargs[0]["camera_grads"] is False
+    assert len(stub.backward_calls) == 1 and stub.backward_calls[0][1]["camera_grads"] is False
     assert view.grad is None and proj.grad is None and campos.grad is None
 
 
@@ -109,10 +81,10 @@ def test_learnable_camera_receives_its_gradients(monkeypatch):
     proj = torch.eye(4)
     campos = torch.zeros(1, 3, requires_grad=True)
     stub = _render(monkeypatch, view, proj, campos)
-    assert stub.backward_kwargs[0]["camera_grads"] is True
-    assert view.grad.dtype == torch.float64 and torch.equal(view.grad, torch.arange(16.0, dtype=torch.float64).view(4, 4))
+    assert stub.backward_calls[0][1]["camera_grads"] is True
+    assert view.grad.dtype == torch.float64 and torch.equal(view.grad, stub_c.marked("dL_dviewmatrix", (4, 4)).double())
     assert proj.grad is None                                                # not requested
-    assert campos.grad.shape == (1, 3) and torch.equal(campos.grad, torch.tensor([[7.0, 8.0, 9.0]]))
+    assert campos.grad.shape == (1, 3) and torch.equal(campos.grad, stub_c.marked("dL_dcampos", (3,)).view(1, 3))
 
 
 def test_learnable_camera_under_no_grad_is_todays_call(monkeypatch):
@@ -121,8 +93,7 @@ def test_learnable_camera_under_no_grad_is_todays_call(monkeypatch):
     seen = []
     orig = dgr._RasterizeGaussians.apply
     monkeypatch.setattr(dgr._RasterizeGaussians, "apply", lambda *a: seen.append(len(a)) or orig(*a))
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
+    stub_c.StubC().install(monkeypatch)
     settings = dgr.GaussianRasterizationSettings(8, 8, 0.5, 0.5, torch.zeros(3), 1.0, view, torch.eye(4), 0, torch.zeros(3), False, False)
     with torch.no_grad():
         dgr.GaussianRasterizer(settings)(torch.zeros(2, 3), torch.zeros(2, 3), torch.zeros(2, 1), shs=torch.zeros(2, 1, 3),

@@ -6,6 +6,7 @@ import ctypes as C
 import pytest
 import torch
 
+import stub_c
 from gs_b200 import lib
 
 
@@ -126,36 +127,9 @@ def test_settings_keyword():
     assert t._replace(deterministic=None).deterministic is None and s._replace(deterministic=True).deterministic is True
 
 
-class _StubC:
-    """Stands in for the kernels: records the keywords of each backward call and returns outputs of the right shapes."""
-
-    def __init__(self):
-        self.backward_kw = []
-
-    def rasterize_gaussians(self, *args, return_maps=False, **kw):
-        means3D, H, W = args[1], args[12], args[13]
-        P = means3D.shape[0]
-        out = (1, torch.ones(3, H, W), torch.ones(P, dtype=torch.int32), torch.zeros(8, dtype=torch.uint8),
-               torch.zeros(8, dtype=torch.uint8), torch.zeros(8, dtype=torch.uint8))
-        return out + ((torch.zeros(1, H, W), torch.zeros(1, H, W)) if return_maps else ())
-
-    def rasterize_gaussians_backward(self, *args, **kw):
-        self.backward_kw.append(dict(kw))
-        means3D, sh = args[1], args[13]
-        P = means3D.shape[0]
-        if kw.get("raw") is not None:
-            C_rest = kw["raw"][1].shape[1]
-            return tuple(None if s is None else torch.full(s, 0.5)
-                         for s in [(P, 3), None, (P, 1), (P, 3), None, (P, 1, 3), (P, C_rest, 3), (P, 3), (P, 4)])
-        M = sh.shape[1] if sh.numel() else 0
-        return tuple(torch.full(s, 0.5) for s in [(P, 3), (P, 3), (P, 1), (P, 3), (P, 6), (P, M, 3), (P, 3), (P, 4)])
-
-
 def _run(monkeypatch, settings, raw=False):
     import diff_gaussian_rasterization as dgr
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
+    stub = stub_c.StubC().install(monkeypatch)
     P = 5
     means = torch.zeros(P, 3, requires_grad=True)
     opac = torch.zeros(P, 1, requires_grad=True)
@@ -168,9 +142,9 @@ def _run(monkeypatch, settings, raw=False):
         color, _ = rz(means, torch.zeros(P, 3, requires_grad=True), opac, shs=torch.zeros(P, 1, 3),
                       degrees=torch.zeros(P, 1, dtype=torch.int32), scales=torch.ones(P, 3), rotations=torch.ones(P, 4))
     (color * 1.0).sum().backward()
-    assert float(opac.grad[0, 0]) == 0.5
-    assert len(stub.backward_kw) == 1
-    return stub.backward_kw[0]
+    assert float(opac.grad[0, 0]) == stub_c.MARK["dL_dopacity"]
+    assert len(stub.backward_calls) == 1
+    return stub.backward_calls[0][1]
 
 
 @pytest.mark.parametrize("raw", [False, True])

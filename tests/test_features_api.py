@@ -4,11 +4,11 @@ call, with gsb_last_error() set, and the Python layer refuses what the feature p
 import ctypes as C
 import os
 import re
-from types import SimpleNamespace
 
 import pytest
 import torch
 
+import stub_c
 from gs_b200 import lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -85,23 +85,9 @@ def test_backward_features_rejects_bad_arguments():
     assert _bwd(L, scene, None, det_ws=C.addressof(buf), R=1 << 30) == -4 and b"2^30" in L.gsb_last_error()
 
 
-class _CpuModel:
-    def __init__(self, P=4):
-        self.get_xyz = torch.zeros(P, 3)
-        self._opacity = torch.zeros(P, 1)
-        self._degrees = torch.zeros(P, 1, dtype=torch.int32)
-        self.get_scaling = torch.full((P, 3), 0.1)
-        self.get_rotation = torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1)
-        self.get_features = torch.zeros(P, 1, 3)
-        self.active_sh_degree = self.max_sh_degree = 0
-
-
 def _render(features, deterministic=None):
     from gaussian_renderer import render
-    cam = SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=16, image_width=16, world_view_transform=torch.eye(4),
-                          full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
-    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
-    return render(cam, _CpuModel(), pipe, torch.zeros(3), features=features)
+    return render(stub_c.camera(16, 16), stub_c.Model(), stub_c.pipe(), torch.zeros(3), features=features)
 
 
 @pytest.fixture

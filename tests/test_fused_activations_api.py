@@ -8,12 +8,11 @@ import os
 import shutil
 import subprocess
 import tempfile
-from types import SimpleNamespace
 
 import pytest
 import torch
-import torch.nn.functional as F
 
+import stub_c
 from gs_b200 import lib
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -197,41 +196,6 @@ def test_raw_keyword_refuses_activated_inputs_and_cpu():
                                torch.zeros(3), False, False, raw=(dc, rest, sc, rot))
 
 
-class _Model:
-    """The reference GaussianModel's attribute names and activations (scene/gaussian_model.py:32-47, 140-163)."""
-
-    def __init__(self, P=6, Cn=15):
-        dc, rest, sc, rot = _leaves(P, Cn)
-        self._xyz = torch.randn(P, 3).requires_grad_()
-        self._features_dc = dc.requires_grad_()
-        self._features_rest = rest.requires_grad_()
-        self._scaling = sc.requires_grad_()
-        self._rotation = rot.requires_grad_()
-        self._opacity = torch.randn(P, 1).requires_grad_()
-        self._degrees = torch.full((P, 1), 3 if Cn == 15 else 0, dtype=torch.int32)
-        self.scaling_activation = torch.exp
-        self.rotation_activation = F.normalize
-        self.active_sh_degree = self.max_sh_degree = {0: 0, 3: 1, 8: 2, 15: 3}[Cn]
-        self.per_band_count = [P, 0, 0, 0]
-
-    get_xyz = property(lambda s: s._xyz)
-    get_scaling = property(lambda s: s.scaling_activation(s._scaling))
-    get_rotation = property(lambda s: s.rotation_activation(s._rotation))
-    get_features = property(lambda s: torch.cat((s._features_dc, s._features_rest), dim=1))
-
-    def leaves(self):
-        return [self._xyz, self._features_dc, self._features_rest, self._scaling, self._rotation, self._opacity]
-
-
-def _camera():
-    return SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=8, image_width=8, world_view_transform=torch.eye(4),
-                           full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
-
-
-def _pipe(**kw):
-    return SimpleNamespace(**{**dict(debug=False, convert_SHs_python=False, compute_cov3D_python=False, fused_activations=True), **kw})
-
-
 @pytest.mark.parametrize("case, msg", [
     ("quant", "quantised"), ("cov3D_python", "compute_cov3D_python"), ("shs_python", "convert_SHs_python"),
     ("scaling_act", "scaling_activation"), ("rotation_act", "rotation_activation"), ("no_act", "scaling_activation"),
@@ -242,7 +206,7 @@ def test_render_refusals_leave_the_model_untouched(monkeypatch, case, msg):
     import gaussian_renderer
     calls = []
     monkeypatch.setattr(dgr._C, "rasterize_gaussians", lambda *a, **k: calls.append(1))
-    pc, pipe = _Model(), _pipe()
+    pc, pipe = stub_c.Model(6, C=15), stub_c.pipe(fused_activations=True)
     if case == "quant":
         pc.quant = object()
     elif case == "cov3D_python":
@@ -259,38 +223,13 @@ def test_render_refusals_leave_the_model_untouched(monkeypatch, case, msg):
         pc._features_rest = [torch.zeros(3, 3, 3), torch.zeros(3, 8, 3)]
     before = [t.detach().clone() for t in pc.leaves() if isinstance(t, torch.Tensor)]
     with pytest.raises(RuntimeError, match=msg):
-        gaussian_renderer.render(_camera(), pc, pipe, torch.zeros(3))
+        gaussian_renderer.render(stub_c.camera(), pc, pipe, torch.zeros(3))
     after = [t for t in pc.leaves() if isinstance(t, torch.Tensor)]
     assert not calls
     assert all(torch.equal(a.detach(), b) and a.grad is None for a, b in zip(after, before))
 
 
 # ---- plumbing against a stub _C ------------------------------------------------------------------------------------------------
-
-class _StubC:
-    def __init__(self):
-        self.fw = []
-        self.bw = []
-        self.out_ptrs = None
-
-    def rasterize_gaussians(self, *args, raw=None, antialiasing=False, return_maps=False, **kw):
-        self.fw.append(dict(raw=raw, sh=args[14], scales=args[4], rotations=args[5], colors=args[2], aa=antialiasing))
-        H, W, P = args[12], args[13], args[1].shape[0]
-        out = (1, torch.ones(3, H, W), torch.ones(P, dtype=torch.int32), torch.zeros(8, dtype=torch.uint8),
-               torch.zeros(8, dtype=torch.uint8), torch.zeros(8, dtype=torch.uint8))
-        return out + ((torch.zeros(1, H, W), torch.zeros(1, H, W)) if return_maps else ())
-
-    def rasterize_gaussians_backward(self, *args, raw=None, **kw):
-        self.bw.append(dict(raw=None if raw is None else [None if t is None else t.data_ptr() for t in raw], kw=kw))
-        P = args[1].shape[0]
-        colors = raw is not None and raw[0] is None
-        Cn = 0 if colors else raw[1].shape[1]
-        outs = [torch.full((P, 3), 0.5), torch.full((P, 3), 0.5) if colors else None, torch.full((P, 1), 0.5), torch.full((P, 3), 0.5),
-                None, None if colors else torch.full((P, 1, 3), 0.25), None if colors else torch.full((P, Cn, 3), 0.125),
-                torch.full((P, 3), 0.75), torch.full((P, 4), 1.5)]
-        self.out_ptrs = [None if t is None else t.data_ptr() for t in outs]
-        return tuple(outs)
-
 
 def _graph_names(root):
     seen, stack, names = set(), [root], []
@@ -306,53 +245,48 @@ def _graph_names(root):
 
 @pytest.mark.parametrize("Cn", [0, 3, 8, 15])
 def test_render_passes_the_parameters_own_storage_and_grads(monkeypatch, Cn):
-    import diff_gaussian_rasterization as dgr
     import gaussian_renderer
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
-    pc = _Model(Cn=Cn)
-    pkg = gaussian_renderer.render(_camera(), pc, _pipe(antialiasing=True), torch.zeros(3))
-    f = stub.fw[0]
-    assert f["aa"] is True
+    stub = stub_c.StubC().install(monkeypatch)
+    pc = stub_c.Model(6, C=Cn)
+    pkg = gaussian_renderer.render(stub_c.camera(), pc, stub_c.pipe(fused_activations=True, antialiasing=True), torch.zeros(3))
+    args, f = stub.forward_calls[0]
+    assert f["antialiasing"] is True
     assert [t.data_ptr() for t in f["raw"]] == [pc._features_dc.data_ptr(), pc._features_rest.data_ptr(), pc._scaling.data_ptr(),
                                                pc._rotation.data_ptr()]
-    assert all(not (isinstance(t, torch.Tensor) and t.numel()) for t in (f["sh"], f["scales"], f["rotations"]))
+    assert all(not (isinstance(t, torch.Tensor) and t.numel()) for t in (args[14], args[4], args[5]))     # sh, scales, rotations
     names = _graph_names(pkg["render"].grad_fn)
     assert not [n for n in names if any(k in n for k in ("Cat", "Exp", "Div", "Norm", "Clamp", "Expand"))], names
     assert names.count("AccumulateGrad") == 7                 # xyz, screen-space points, dc, rest, opacity, scaling, rotation
     pkg["render"].sum().backward()
-    assert stub.bw[0]["raw"] == [t.data_ptr() for t in (pc._features_dc, pc._features_rest, pc._scaling, pc._rotation)]
-    assert stub.bw[0]["kw"]["antialiasing"] is True
+    b = stub.backward_calls[0][1]
+    assert [t.data_ptr() for t in b["raw"]] == [t.data_ptr() for t in (pc._features_dc, pc._features_rest, pc._scaling, pc._rotation)]
+    assert b["antialiasing"] is True
     # the rasterizer's own outputs became .grad: no clone
     got = [pc._features_dc.grad, pc._features_rest.grad, pc._scaling.grad, pc._rotation.grad]
-    assert [g.data_ptr() for g in got[:1] + got[2:]] == [stub.out_ptrs[5], stub.out_ptrs[7], stub.out_ptrs[8]]
+    out_ptrs = stub.backward_output_ptrs[0]
+    assert [g.data_ptr() for g in got[:1] + got[2:]] == [out_ptrs[5], out_ptrs[7], out_ptrs[8]]
     assert all(g.is_contiguous() for g in got) and tuple(got[1].shape) == (6, Cn, 3)
 
 
 def test_render_override_color_reads_no_sh(monkeypatch):
-    import diff_gaussian_rasterization as dgr
     import gaussian_renderer
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians_backward", stub.rasterize_gaussians_backward)
-    pc = _Model()
+    stub = stub_c.StubC().install(monkeypatch)
+    pc = stub_c.Model(6, C=15)
     colors = torch.rand(6, 3, requires_grad=True)
-    pkg = gaussian_renderer.render(_camera(), pc, _pipe(), torch.zeros(3), override_color=colors)
-    assert stub.fw[0]["raw"][:2] == (None, None) and stub.fw[0]["colors"] is colors
+    pkg = gaussian_renderer.render(stub_c.camera(), pc, stub_c.pipe(fused_activations=True), torch.zeros(3), override_color=colors)
+    args, f = stub.forward_calls[0]
+    assert f["raw"][:2] == (None, None) and args[2] is colors
     pkg["render"].sum().backward()
-    assert stub.bw[0]["raw"][:2] == [None, None]
+    assert stub.backward_calls[0][1]["raw"][:2] == (None, None)
     assert pc._features_dc.grad is None and pc._features_rest.grad is None
     assert colors.grad is not None and pc._scaling.grad is not None
 
 
 def test_flag_off_changes_nothing(monkeypatch):
-    import diff_gaussian_rasterization as dgr
     import gaussian_renderer
-    stub = _StubC()
-    monkeypatch.setattr(dgr._C, "rasterize_gaussians", stub.rasterize_gaussians)
-    pc = _Model()
-    for pipe in (_pipe(fused_activations=False), SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)):
-        gaussian_renderer.render(_camera(), pc, pipe, torch.zeros(3))
-    assert [f["raw"] for f in stub.fw] == [None, None]
-    assert all(tuple(f["sh"].shape) == (6, 16, 3) and f["scales"].numel() == 18 for f in stub.fw)
+    stub = stub_c.StubC().install(monkeypatch)
+    pc = stub_c.Model(6, C=15)
+    for pipe in (stub_c.pipe(fused_activations=False), stub_c.pipe()):
+        gaussian_renderer.render(stub_c.camera(), pc, pipe, torch.zeros(3))
+    assert [f.get("raw") for _, f in stub.forward_calls] == [None, None]
+    assert all(tuple(args[14].shape) == (6, 16, 3) and args[4].numel() == 18 for args, _ in stub.forward_calls)

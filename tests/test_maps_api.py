@@ -1,11 +1,11 @@
 """CPU: argument checks of the map entry points (gsb_forward_maps / gsb_backward_maps) and the Python layer's refusal of CPU
 tensors with return_maps; every call below is rejected before the first CUDA call."""
 import ctypes as C
-from types import SimpleNamespace
 
 import pytest
 import torch
 
+import stub_c
 from gs_b200 import lib
 
 
@@ -26,21 +26,7 @@ def test_map_entry_points_reject_bad_scenes():
     assert st < 0 and b"map" in L.gsb_last_error()
 
 
-class _CpuModel:
-    def __init__(self, P=4):
-        self.get_xyz = torch.zeros(P, 3)
-        self._opacity = torch.zeros(P, 1)
-        self._degrees = torch.zeros(P, 1, dtype=torch.int32)
-        self.get_scaling = torch.full((P, 3), 0.1)
-        self.get_rotation = torch.tensor([[1.0, 0, 0, 0]]).repeat(P, 1)
-        self.get_features = torch.zeros(P, 1, 3)
-        self.active_sh_degree = self.max_sh_degree = 0
-
-
 def test_render_with_maps_refuses_cpu_tensors():
     from gaussian_renderer import render
-    cam = SimpleNamespace(FoVx=1.0, FoVy=1.0, image_height=16, image_width=16, world_view_transform=torch.eye(4),
-                          full_proj_transform=torch.eye(4), camera_center=torch.zeros(3))
-    pipe = SimpleNamespace(debug=False, convert_SHs_python=False, compute_cov3D_python=False)
     with pytest.raises(RuntimeError):
-        render(cam, _CpuModel(), pipe, torch.zeros(3), return_maps=True)
+        render(stub_c.camera(16, 16), stub_c.Model(), stub_c.pipe(), torch.zeros(3), return_maps=True)
