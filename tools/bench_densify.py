@@ -16,11 +16,12 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
 import torch
+
+import benchkit
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "reduced-3dgs_b200"))
@@ -71,9 +72,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=5)
     args = ap.parse_args()
     assert torch.cuda.is_available(), "bench_densify needs a GPU"
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                         text=True).stdout.strip().splitlines()
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "nvidia_smi": smi[0] if smi else "n/a"}), flush=True)
+    benchkit.banner()
     P = args.points
     fns = {"ref": rs.densify_and_prune, "native": densify.densify_and_prune}
     times = {k: [] for k in fns}

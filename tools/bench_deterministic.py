@@ -11,24 +11,9 @@ deterministic workspace size.
 """
 import argparse
 import json
-import math
-import os
 import statistics
-import subprocess
-import sys
-from types import SimpleNamespace
 
-import torch
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "reduced-3dgs_b200"))
-import bench  # noqa: E402  (workload and cameras of the benchmark, unchanged)
-from diff_gaussian_rasterization import _C  # noqa: E402
-from gs_b200 import lib as gsl  # noqa: E402
-from gs_b200 import synth  # noqa: E402
-
-E = torch.Tensor([])
+import benchkit
 
 
 def main():
@@ -36,79 +21,28 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "bench_deterministic needs a GPU"
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                         text=True).stdout.strip().splitlines()
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "nvidia_smi": smi[0] if smi else "n/a"}), flush=True)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
+    dev = benchkit.device("bench_deterministic")
+    benchkit.banner()
+    flush = benchkit.l2_flush(dev)
+    from gs_b200 import lib as gsl
     L = gsl.lib()
+    c3 = benchkit.bench_workload("C3", dev)
+    cam = c3.cams[0]
+    dense = benchkit.dense_raw_workload(c3.W, c3.H, dev)
 
-    # C3: bench.py's workload and first camera
-    name, W, H, scene, quant, prune = bench.build_workload(SimpleNamespace(config="C3", points=0), dev, 0, 1)
-    cam = bench.bench_cameras(W, H, 4)[0].to(dev)
-    sd, qd = scene.to(dev), quant.to(dev)
-    tx, ty = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
-    bg = torch.zeros(3, device=dev)
-    G = synth.grad_image(W, H, 1000).to(dev)
-
-    def c3_step(det):
-        fa = (bg, sd.means3D, E, sd.opacity, E, E, 1.0, E, cam.world_view_transform, cam.full_proj_transform, tx, ty, H, W, E, sd.degrees,
-              cam.camera_center, False, False)
-        R, color, radii, gb, bb, ib = _C.rasterize_gaussians(*fa, quant=qd)
-        _C.rasterize_gaussians_backward(bg, sd.means3D, radii, E, E, E, 1.0, E, cam.world_view_transform, cam.full_proj_transform, tx, ty,
-                                        G, E, sd.degrees, cam.camera_center, gb, R, bb, ib, 0.0, False, quant=qd,
-                                        **({"deterministic": True} if det else {}))
-        return R
-
-    # dense 3 M from raw parameters (SH degree 3)
-    dsc = synth.make_scene(3_000_000, 7, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.01))
-    xyz, op = dsc.means3D.to(dev), dsc.opacity.to(dev)
-    raw = (dsc.sh[:, :1].contiguous().to(dev), dsc.sh[:, 1:16].contiguous().to(dev), torch.log(dsc.scales).to(dev),
-           dsc.rotations.contiguous().to(dev))
-    deg = dsc.degrees.to(dev)
-
-    def dense_step(det):
-        fa = (bg, xyz, E, op, E, E, 1.0, E, cam.world_view_transform, cam.full_proj_transform, tx, ty, H, W, E, deg, cam.camera_center,
-              False, False)
-        R, color, radii, gb, bb, ib = _C.rasterize_gaussians(*fa, raw=raw)
-        _C.rasterize_gaussians_backward(bg, xyz, radii, E, E, E, 1.0, E, cam.world_view_transform, cam.full_proj_transform, tx, ty, G, E,
-                                        deg, cam.camera_center, gb, R, bb, ib, 0.0, False, raw=raw,
-                                        **({"deterministic": True} if det else {}))
-        return R
-
-    for wl, step, P in (("C3", c3_step, sd.P), ("dense3M_raw", dense_step, dsc.P)):
-        times = {False: [], True: []}
-        R = 0
-        for i in range(args.warmup + args.steps):
-            for det in (False, True):
-                flush.zero_()
-                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                a.record()
-                R = step(det)
-                b.record()
-                torch.cuda.synchronize()
-                if i >= args.warmup:
-                    times[det].append(a.elapsed_time(b))
-        kernels = {}
-        for det in (False, True):
-            gsl.profile_enable(True)
-            gsl.profile_read()
-            n = 5
-            for _ in range(n):
-                flush.zero_()
-                step(det)
-            torch.cuda.synchronize()
-            kernels[det] = {kn: round(t / n, 4) for kn, (t, _) in gsl.profile_read().items()}
-            gsl.profile_enable(False)
-        base = statistics.median(times[False])
-        for det in (False, True):
-            med = statistics.median(times[det])
-            print(json.dumps({"workload": wl, "arm": "deterministic" if det else "default", "P": int(P), "R": int(R),
-                              "det_workspace_bytes": int(L.gsb_deterministic_workspace_bytes(int(P), int(R))) if det else 0,
+    for name, wl in (("C3", c3), ("dense3M_raw", dense)):
+        arms = {"default": lambda i: benchkit.forward_backward(wl, cam),
+                "deterministic": lambda i: benchkit.forward_backward(wl, cam, bwd={"deterministic": True})}
+        times = benchkit.time_arms(arms, args.steps, args.warmup, flush)
+        kernels = benchkit.kernel_ms(arms, 5, flush, warm=0)
+        P, R = int(wl.scene.P), int(benchkit.forward_backward(wl, cam, backward=False)[0][0])
+        base = statistics.median(times["default"])
+        for k in arms:
+            med = statistics.median(times[k])
+            print(json.dumps({"workload": name, "arm": k, "P": P, "R": R,
+                              "det_workspace_bytes": int(L.gsb_deterministic_workspace_bytes(P, R)) if k == "deterministic" else 0,
                               "fwd_bwd_ms_median": round(med, 4), "ratio_to_default": round(med / base, 4),
-                              "kernels_ms": kernels[det]}), flush=True)
+                              "kernels_ms": kernels[k]}), flush=True)
 
 
 if __name__ == "__main__":

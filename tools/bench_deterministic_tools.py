@@ -5,24 +5,21 @@
 Workloads: `calculate_colours_variance` over 32 cameras at 1920x1080 on a dense 3 M Gaussian scene of SH degree 3 (one call = 32
 statistics forwards + 32 statistics updates), and `kmeans_cuda` with 256 centres drawn from 9 M values (tol 1e-4, at most 500
 iterations: the codebook call of gaussian_model.py) for uniform, normal and 70 % exact-zero values.  Per workload the arms
-`default` and `deterministic` alternate call by call; each call is timed with a CUDA event pair and the median over the calls is
-reported.  Prints the card's name and power limit, then one JSON line per (workload, arm) and the ratio deterministic / default.
+`default` and `deterministic` alternate call by call; each call is timed with a CUDA event pair, L2 is flushed (256 MB write)
+between calls outside the pair, and the median over the calls is reported.  Prints the card's name and power limit, then one
+JSON line per (workload, arm) and the ratio deterministic / default.
 """
 import argparse
 import json
 import math
-import os
 import statistics
-import subprocess
-import sys
 
 import numpy as np
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "reduced-3dgs_b200"))
-from diff_gaussian_rasterization import _C  # noqa: E402
-from gs_b200 import synth  # noqa: E402
+import benchkit
+from diff_gaussian_rasterization import _C  # on sys.path through benchkit
+from gs_b200 import synth
 
 
 def _cameras(n, W, H, dev):
@@ -39,24 +36,6 @@ def _cameras(n, W, H, dev):
                 H=torch.full((n,), H, dtype=torch.int32, device=dev), W=torch.full((n,), W, dtype=torch.int32, device=dev))
 
 
-def _time(fn, arms, reps, warmup):
-    """{arm: [ms per call]}, the arms interleaved call by call."""
-    for _ in range(warmup):
-        for a in arms:
-            fn(a)
-    torch.cuda.synchronize()
-    out = {a: [] for a in arms}
-    for _ in range(reps):
-        for a in arms:
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            fn(a)
-            e1.record()
-            e1.synchronize()
-            out[a].append(e0.elapsed_time(e1))
-    return out
-
-
 def _report(workload, times, extra=None):
     med = {a: statistics.median(t) for a, t in times.items()}
     for a, t in times.items():
@@ -70,13 +49,14 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=2)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "bench_deterministic_tools needs a GPU"
+    dev = benchkit.device("bench_deterministic_tools")
     assert args.reps >= 10, "the medians are taken over at least 10 calls per arm"
-    dev = torch.device("cuda", 0)
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                         text=True).stdout.strip().splitlines()
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "nvidia_smi": smi[0] if smi else "n/a"}), flush=True)
-    arms = ("default", "deterministic")
+    benchkit.banner()
+    flush = benchkit.l2_flush(dev)
+
+    def time_both(fn):
+        """{arm: [ms per call]} of fn(arm) for the arms default and deterministic."""
+        return benchkit.time_arms({a: (lambda i, a=a: fn(a)) for a in ("default", "deterministic")}, args.reps, args.warmup, flush)
 
     # ---- SH-culling statistics: 32 cameras at 1080p, dense 3 M degree-3 scene
     W, H = 1920, 1080
@@ -87,7 +67,7 @@ def main():
         return _C.calculate_colours_variance(ct["positions"], sc.means3D, sc.opacity, sc.scales, sc.rotations, ct["views"], ct["projs"],
                                              ct["tanx"], ct["tany"], ct["H"], ct["W"], sc.sh, sc.degrees, 3,
                                              deterministic=arm == "deterministic")
-    _report("colours_variance_3M_32x1080p", _time(colours, arms, args.reps, args.warmup))
+    _report("colours_variance_3M_32x1080p", time_both(colours))
     del sc, ct
     torch.cuda.empty_cache()
 
@@ -106,7 +86,7 @@ def main():
         def kmeans(arm):
             ids, cc = _C.kmeans_cuda(v, c, 1e-4, 500, deterministic=arm == "deterministic")
             iters[arm] = cc
-        t = _time(kmeans, arms, args.reps, args.warmup)
+        t = time_both(kmeans)
         gap = float((iters["deterministic"] - iters["default"]).abs().max())
         _report(f"kmeans_9M_256_{name}", t, {"max_centre_gap_vs_default": gap})
 

@@ -14,13 +14,14 @@ import json
 import math
 import os
 import statistics
-import subprocess
 import sys
 from types import SimpleNamespace
 
 import numpy as np
 import torch
 import torch.nn.functional as F
+
+import benchkit
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "reduced-3dgs_b200"))
@@ -49,24 +50,13 @@ class Model:
     get_features = property(lambda s: torch.cat((s._features_dc, s._features_rest), dim=1))
 
 
-def card():
-    name = torch.cuda.get_device_name()
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i", str(torch.cuda.current_device())],
-                            capture_output=True, text=True, timeout=30).stdout.strip()
-    except (OSError, subprocess.SubprocessError):
-        pl = "unknown"
-    return name, pl
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--points", type=int, default=3_000_000)
     ap.add_argument("--repeats", type=int, default=20)
     args = ap.parse_args()
     dev = torch.device("cuda")
-    name, pl = card()
-    print(f"device: {name}, power limit {pl}", flush=True)
+    name, pl = torch.cuda.get_device_name(), benchkit.banner().get("power_limit", "unknown")
     W, H = 1920, 1080
     scene = synth.make_scene(args.points, 3, sh_degree=3, mixed_degrees=True)
     m = Model(scene, dev)

@@ -11,10 +11,11 @@ per row.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
+
+import benchkit
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in ("reduced-3dgs_b200", "oracle", os.path.join("tests", "golden")):
@@ -47,8 +48,7 @@ def main():
     from simple_knn import _C as ours
     ref = build_ref_knn.load()
     assert ref is not None, "oracle/_ref/_refKnn.so missing: build it with oracle/build_ref_knn.py"
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "nvidia_smi": smi.strip().splitlines()[0] if smi.strip() else "n/a"}), flush=True)
+    benchkit.banner()
     K = args.K
     for P in [int(s) for s in args.sizes.split(",")]:
         for name, pts in KC.large_inputs(P).items():

@@ -3,6 +3,7 @@ autograd, utils/loss_utils.py:33-65) on the same GPU, 3x1080x1920, forward + bac
 import json, os, sys
 import torch
 import torch.nn.functional as F
+import benchkit
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "reduced-3dgs_b200"))
 from utils import loss_utils as LU
@@ -29,6 +30,7 @@ def timed(fn, reps=20):
 
 
 def main():
+    benchkit.banner()
     g = torch.Generator().manual_seed(0)
     x = torch.rand(3, 1080, 1920, generator=g).cuda().requires_grad_(True)
     y = torch.rand(3, 1080, 1920, generator=g).cuda()

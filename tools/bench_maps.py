@@ -13,23 +13,10 @@ gives per-kernel times (gsb_profile_*).  Prints the card's name and power limit,
 """
 import argparse
 import json
-import math
-import os
-import subprocess
-import sys
-from types import SimpleNamespace
 
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "reduced-3dgs_b200"))
-import bench  # noqa: E402  (workload and cameras of the benchmark, unchanged)
-from diff_gaussian_rasterization import _C  # noqa: E402
-from gs_b200 import lib as gsl  # noqa: E402
-from gs_b200 import synth  # noqa: E402
-
-EMPTY = torch.Tensor([])
+import benchkit
 
 
 def main():
@@ -38,98 +25,43 @@ def main():
     ap.add_argument("--steps", type=int, default=20)
     ap.add_argument("--warmup", type=int, default=5)
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "bench_maps needs a GPU"
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                         text=True).stdout.strip().splitlines()
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "nvidia_smi": smi[0] if smi else "n/a"}), flush=True)
-
-    name, W, H, scene, quant, prune = bench.build_workload(SimpleNamespace(config=args.config, points=0), dev, 0, 1)
-    cams = [c.to(dev) for c in bench.bench_cameras(W, H, 4)]
-    sd = scene.to(dev)
-    qd = None if quant is None else quant.to(dev)
-    prune_d = None if prune is None else prune.to(dev)
-    bg0 = torch.zeros(3, device=dev)
-    G = synth.grad_image(W, H, 1000).to(dev)
+    dev = benchkit.device("bench_maps")
+    benchkit.banner()
+    flush = benchkit.l2_flush(dev)
+    wl = benchkit.bench_workload(args.config, dev)
+    cams, sd, W, H = wl.cams, wl.scene, wl.W, wl.H
     g = torch.Generator().manual_seed(1001)
     Gd = torch.randn(1, H, W, generator=g).to(dev)
     Ga = torch.randn(1, H, W, generator=g).to(dev)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
     ones = torch.ones(sd.P, 3, device=dev)
-
-    def fwd_args(c, colors=EMPTY, bg=bg0):
-        tx, ty = math.tan(c.FoVx * 0.5), math.tan(c.FoVy * 0.5)
-        if qd is not None:
-            return (bg, sd.means3D, colors, EMPTY, EMPTY, EMPTY, 1.0, EMPTY, c.world_view_transform, c.full_proj_transform, tx, ty, H, W,
-                    EMPTY, sd.degrees, c.camera_center, False, False)
-        return (bg, sd.means3D, colors, sd.opacity, sd.scales, sd.rotations, 1.0, EMPTY, c.world_view_transform, c.full_proj_transform,
-                tx, ty, H, W, EMPTY if colors.numel() else sd.sh, sd.degrees, c.camera_center, False, False)
-
-    def fb(a, dL, maps=False, **bkw):
-        out = _C.rasterize_gaussians(*a, prune_mask=prune_d, quant=qd, return_maps=maps)
-        R, color, radii, gb, bb, ib = out[:6]
-        _C.rasterize_gaussians_backward(a[0], a[1], radii, a[2], a[4], a[5], 1.0, EMPTY, a[8], a[9], a[10], a[11], dL, a[14], a[15],
-                                        a[16], gb, R, bb, ib, 0.0, False, prune_mask=prune_d, quant=qd, **bkw)
-        return out
-
     dLd3 = torch.zeros(3, H, W, device=dev)
     dLd3[0] = Gd[0]
     dLa3 = torch.zeros(3, H, W, device=dev)
     dLa3[0] = Ga[0]
 
-    def arm_a(c):
-        fb(fwd_args(c), G)
+    def arm_a(i):
+        benchkit.forward_backward(wl, cams[i % len(cams)])
 
-    def arm_b(c):
-        fb(fwd_args(c), G, maps=True, dL_dinvdepth=Gd, dL_dalpha=Ga)
+    def arm_b(i):
+        benchkit.forward_backward(wl, cams[i % len(cams)], dict(return_maps=True), dict(dL_dinvdepth=Gd, dL_dalpha=Ga))
 
-    def arm_c(c):
-        fb(fwd_args(c), G)
+    def arm_c(i):
+        c = cams[i % len(cams)]
+        benchkit.forward_backward(wl, c)
         V = c.world_view_transform                       # the callers' per-Gaussian depth: view-space z of the means
         z = sd.means3D @ V[:3, 2] + V[3, 2]
         col = torch.zeros(sd.P, 3, device=dev)
         col[:, 0] = 1.0 / z
-        fb(fwd_args(c, col), dLd3)
-        fb(fwd_args(c, ones), dLa3)
+        benchkit.forward_backward(wl, c, dL=dLd3, colors=col)
+        benchkit.forward_backward(wl, c, dL=dLa3, colors=ones)
 
     arms = {"a": arm_a, "b": arm_b, "c": arm_c}
-    for i in range(max(args.warmup, 2)):
-        for fn in arms.values():
-            flush.zero_()
-            fn(cams[i % len(cams)])
-    torch.cuda.synchronize()
-    times = {k: [] for k in arms}
-    for i in range(args.steps):
-        for k, fn in arms.items():
-            flush.zero_()
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            fn(cams[i % len(cams)])
-            e1.record()
-            times[k].append((e0, e1))
-    torch.cuda.synchronize()
-    ms = {k: sorted(a.elapsed_time(b) for a, b in v) for k, v in times.items()}
-    # per-kernel device time, a separate pass per arm with the event brackets on
-    kernels = {}
-    gsl.profile_enable(True)
-    for k, fn in arms.items():
-        for i in range(2):
-            flush.zero_()
-            fn(cams[i % len(cams)])
-        torch.cuda.synchronize()
-        gsl.profile_read()
-        n = min(args.steps, 8)
-        for i in range(n):
-            flush.zero_()
-            fn(cams[i % len(cams)])
-        torch.cuda.synchronize()
-        kernels[k] = {kn: round(t / n, 4) for kn, (t, _) in gsl.profile_read().items()}
-    gsl.profile_enable(False)
+    ms = {k: sorted(v) for k, v in benchkit.time_arms(arms, args.steps, args.warmup, flush).items()}
+    kernels = benchkit.kernel_ms(arms, min(args.steps, 8), flush)
     med = {k: v[len(v) // 2] for k, v in ms.items()}
     for k in arms:
         v = ms[k]
-        print(json.dumps({"arm": k, "config": name, "W": W, "H": H, "P": sd.P, "steps": len(v), "median_ms": round(med[k], 4),
+        print(json.dumps({"arm": k, "config": wl.name, "W": W, "H": H, "P": sd.P, "steps": len(v), "median_ms": round(med[k], 4),
                           "mean_ms": round(sum(v) / len(v), 4), "min_ms": round(v[0], 4), "max_ms": round(v[-1], 4),
                           "kernels_ms_per_step": kernels[k]}), flush=True)
     print(json.dumps({"b_over_a": round(med["b"] / med["a"], 4), "c_over_a": round(med["c"] / med["a"], 4),

@@ -14,12 +14,13 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
 import numpy as np
 import torch
+
+import benchkit
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 for p in ("reduced-3dgs_b200", "tests", os.path.join("tests", "golden")):
@@ -78,14 +79,6 @@ def native_arm(m, cams):
     densify.mercy_points(m, {}, 1.0, 3, "redundancy_opacity_opacity")
 
 
-def card():
-    try:
-        return subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                              text=True).stdout.strip().splitlines()[0]
-    except (OSError, IndexError):
-        return torch.cuda.get_device_name()
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--points", type=int, nargs="+", default=[1_000_000, 3_000_000])
@@ -93,7 +86,7 @@ def main():
     ap.add_argument("--repeats", type=int, default=5)
     a = ap.parse_args()
     assert torch.cuda.is_available(), "bench_mercy needs a GPU"
-    print("card:", card(), flush=True)
+    benchkit.banner()
     cams = [mr.Cam(c, torch.device("cuda")) for c in synth.orbit_cameras(a.cameras, 1920, 1080)]
     for P in a.points:
         xyz = KC.c3_positions(P).cuda()

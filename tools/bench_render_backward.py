@@ -15,15 +15,15 @@ power limit.  Without a GPU it fails.
 """
 import argparse
 import json
-import math
 import os
 import statistics
 import subprocess
 import sys
 import tempfile
-from types import SimpleNamespace
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+import benchkit     # from this script's directory: the parent tree need not have it
+
+ROOT = benchkit.ROOT
 WORKLOADS = ("C3", "dense3M_raw")
 
 
@@ -32,64 +32,36 @@ def measure(tree, steps, warmup, dump):
     sys.path[:0] = [tree, os.path.join(tree, "reduced-3dgs_b200")]
     import numpy as np
     import torch
-    assert torch.cuda.is_available(), "bench_render_backward needs a GPU"
+    dev = benchkit.device("bench_render_backward")
     import bench
-    from diff_gaussian_rasterization import _C
     from gs_b200 import lib as gsl
-    from gs_b200 import synth
     assert os.path.realpath(gsl.__file__).startswith(os.path.realpath(tree) + os.sep), gsl.__file__
-    E = torch.Tensor([])
-    dev = torch.device("cuda", 0)
-    torch.cuda.set_device(dev)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)
-
-    name, W, H, scene, quant, prune = bench.build_workload(SimpleNamespace(config="C3", points=0), dev, 0, 1)
-    cam = bench.bench_cameras(W, H, 4)[0].to(dev)
-    sd, qd = scene.to(dev), quant.to(dev)
-    tx, ty = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
-    bg = torch.zeros(3, device=dev)
-    G = synth.grad_image(W, H, 1000).to(dev)
-
-    def c3_step():
-        fa = (bg, sd.means3D, E, sd.opacity, E, E, 1.0, E, cam.world_view_transform, cam.full_proj_transform, tx, ty, H, W, E, sd.degrees,
-              cam.camera_center, False, False)
-        R, color, radii, gb, bb, ib = _C.rasterize_gaussians(*fa, quant=qd)
-        return R, _C.rasterize_gaussians_backward(bg, sd.means3D, radii, E, E, E, 1.0, E, cam.world_view_transform, cam.full_proj_transform,
-                                                  tx, ty, G, E, sd.degrees, cam.camera_center, gb, R, bb, ib, 0.0, False, quant=qd)
-
-    dsc = synth.make_scene(3_000_000, 7, sh_degree=3, box=(1.9 * W / H, 1.9, 1.0), log_scale_mean=math.log(0.01))
-    xyz, op = dsc.means3D.to(dev), dsc.opacity.to(dev)
-    raw = (dsc.sh[:, :1].contiguous().to(dev), dsc.sh[:, 1:16].contiguous().to(dev), torch.log(dsc.scales).to(dev),
-           dsc.rotations.contiguous().to(dev))
-    deg = dsc.degrees.to(dev)
-
-    def dense_step():
-        fa = (bg, xyz, E, op, E, E, 1.0, E, cam.world_view_transform, cam.full_proj_transform, tx, ty, H, W, E, deg, cam.camera_center,
-              False, False)
-        R, color, radii, gb, bb, ib = _C.rasterize_gaussians(*fa, raw=raw)
-        return R, _C.rasterize_gaussians_backward(bg, xyz, radii, E, E, E, 1.0, E, cam.world_view_transform, cam.full_proj_transform,
-                                                  tx, ty, G, E, deg, cam.camera_center, gb, R, bb, ib, 0.0, False, raw=raw)
+    assert os.path.realpath(bench.__file__).startswith(os.path.realpath(tree) + os.sep), bench.__file__
+    flush = benchkit.l2_flush(dev)
+    c3 = benchkit.bench_workload("C3", dev)
+    cam = c3.cams[0]
 
     samples = {}
     gsl.profile_enable(True)
-    for wl, step, P in zip(WORKLOADS, (c3_step, dense_step), (sd.P, dsc.P)):
-        step_ms, rb_ms = [], []
-        for i in range(warmup + steps):
-            flush.zero_()
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            R, grads = step()
-            b.record()
-            torch.cuda.synchronize()
-            prof = gsl.profile_read()
-            if i >= warmup:
-                step_ms.append(a.elapsed_time(b))
-                rb_ms.append(prof["render_backward"][0])
+    for name, wl in zip(WORKLOADS, (c3, benchkit.dense_raw_workload(c3.W, c3.H, dev))):
+        rb, last = [], []
+
+        def step(i):
+            # the library's event pairs of the previous step, so rb[k + 1] belongs to step k.  The read runs inside this step's
+            # event pair, while the L2 flush in front of it still runs on the GPU; host time it takes beyond the flush counts in
+            # step_ms (render_backward_ms, the kernel's own pair, does not see it)
+            rb.append(gsl.profile_read().get("render_backward", (0.0, 0))[0])
+            last[:] = benchkit.forward_backward(wl, cam)
+
+        step_ms = benchkit.time_arms({name: step}, steps, warmup, flush)[name]
+        rb.append(gsl.profile_read()["render_backward"][0])
+        rb_ms = rb[warmup + 1:]
+        R, grads, P = last[0][0], last[1], wl.scene.P
         rows = torch.as_tensor(np.sort(np.random.default_rng(P).choice(P, bench.DUMP_ROWS, replace=False)), device=dev)
         for i, g in enumerate(grads):                                          # every per-Gaussian output (raw= appends its own)
             if torch.is_tensor(g) and g.dim() and g.shape[0] == P:
-                samples[f"{wl}/{bench.GRAD_NAMES[i] if i < len(bench.GRAD_NAMES) else i}"] = g[rows].float().cpu().numpy()
-        print(json.dumps({"workload": wl, "R": int(R), "steps": steps,
+                samples[f"{name}/{bench.GRAD_NAMES[i] if i < len(bench.GRAD_NAMES) else i}"] = g[rows].float().cpu().numpy()
+        print(json.dumps({"workload": name, "R": int(R), "steps": steps,
                           "render_backward_ms": {"median": round(statistics.median(rb_ms), 4), "min": round(min(rb_ms), 4), "max": round(max(rb_ms), 4)},
                           "step_ms": {"median": round(statistics.median(step_ms), 4), "min": round(min(step_ms), 4), "max": round(max(step_ms), 4)}}),
               flush=True)
@@ -128,9 +100,7 @@ def main():
     import numpy as np
     import torch
     assert torch.cuda.is_available(), "bench_render_backward needs a GPU"
-    smi = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                         text=True).stdout.strip().splitlines()
-    print(json.dumps({"gpu": torch.cuda.get_device_name(0), "nvidia_smi": smi[0] if smi else "n/a"}), flush=True)
+    benchkit.banner()
 
     res = {}                                                                   # (arm, rep) -> {workload: line}
     with tempfile.TemporaryDirectory() as tmp:

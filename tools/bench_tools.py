@@ -13,6 +13,8 @@ import time
 
 import torch
 
+import benchkit
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "reduced-3dgs_b200"))
 sys.path.insert(0, os.path.join(ROOT, "oracle"))
@@ -44,6 +46,7 @@ def main():
     ap.add_argument("--values", type=int, default=9_000_192)
     ap.add_argument("--knn", type=int, default=30)
     a = ap.parse_args()
+    benchkit.banner()
     refC = build_ref.load()
     dev = "cuda"
     W, H = 1920, 1080
