@@ -11,9 +11,12 @@ kernels do; everything after that is float64.
 import numpy as np
 
 
-def pair_sums(state, bg, dL, W, H):
+def pair_sums(state, bg, dL, W, H, dL_dinvdepth=None, dL_dalpha=None):
     """state: means2D [P,2], conic_opacity [P,4], rgb [P,3], point_list, ranges [tiles,2], n_contrib [H,W] (any array-likes).
-    bg [3], dL [3,H,W].  -> (signed [P,2], absolute [P,2]) float64, with the factors 0.5 W / 0.5 H applied."""
+    bg [3], dL [3,H,W].  -> (signed [P,2], absolute [P,2]) float64, with the factors 0.5 W / 0.5 H applied.
+    With the maps' gradients (DESIGN.md §5c; [H,W] each, `state` then also needs depths [P]): dL_dinvdepth is that of one more
+    channel of colour 1/depth (the IEEE fp32 quotient) and background 0, dL_dalpha that of one of colour 0 and background -1
+    (alpha = 1 - final_T)."""
     m2 = np.asarray(state["means2D"], np.float32)
     co = np.asarray(state["conic_opacity"], np.float32)
     rgb = np.asarray(state["rgb"], np.float64)
@@ -22,6 +25,16 @@ def pair_sums(state, bg, dL, W, H):
     nc = np.asarray(state["n_contrib"]).astype(np.int64).reshape(H, W)
     bg = np.asarray(bg, np.float64)
     dL = np.asarray(dL, np.float64).reshape(3, H, W)
+    if dL_dinvdepth is not None or dL_dalpha is not None:
+        # two more channels: colour 1/depth with background 0 under dL_dinvdepth, colour 0 with background -1 under dL_dalpha
+        d = np.asarray(state["depths"], np.float32)
+        inv = np.zeros(d.shape, np.float32)
+        inv[d != 0] = np.float32(1.0) / d[d != 0]
+        rgb = np.concatenate([rgb, inv.astype(np.float64)[:, None], np.zeros((rgb.shape[0], 1))], 1)
+        bg = np.concatenate([bg, [0.0, -1.0]])
+        zero = np.zeros((H, W))
+        dL = np.concatenate([dL, np.stack([zero if m is None else np.asarray(m, np.float64).reshape(H, W)
+                                           for m in (dL_dinvdepth, dL_dalpha)])], 0)
     P = m2.shape[0]
     signed = np.zeros((P, 2), np.float64)
     absol = np.zeros((P, 2), np.float64)
@@ -51,7 +64,7 @@ def pair_sums(state, bg, dL, W, H):
         one_m = 1.0 - a
         T = np.cumprod(np.concatenate([np.ones((a.shape[0], 1)), one_m[:, :-1]], axis=1), axis=1)     # T in front of entry j
         T_final = T[:, -1] * one_m[:, -1]
-        dLp = dL[:, ys, xs].T                                                                          # [pixels, 3]
+        dLp = dL[:, ys, xs].T                                                                          # [pixels, C]
         k = dLp @ rgb[ids].T                                                                           # colour . dL/dpixel
         contrib = k * a * T
         S = np.cumsum(contrib[:, ::-1], axis=1)[:, ::-1] - contrib                                     # entries behind j

@@ -452,14 +452,14 @@ def well_conditioned(case, o):
     return vis & (cancellation(case, o) < AA_WELL_CONDITIONED) if case.name == "aa_needles" else vis
 
 
-def compare_aa(label, case, o, o64, o32, got, chk, glob=None, bar=(R_REL, A_ABS)):
+def compare_aa(label, case, o, o64, o32, got, chk, glob=None, bar=(R_REL, A_ABS), arrays=ARRAYS):
     """compare() of an anti-aliased backward: every array on the well-conditioned Gaussians, all but ILL_CONDITIONED_ARRAYS on the
     others -> failures."""
     well = well_conditioned(case, o)
-    _, failures = compare(label, o, o64, o32, got, chk & well, glob, bar=bar)
+    _, failures = compare(label, o, o64, o32, got, chk & well, glob, bar=bar, arrays=arrays)
     if (chk & ~well & (o["radii"] > 0)).any():
         _, more = compare(label + ", a c / det0 >= %g" % AA_WELL_CONDITIONED, o, o64, o32, got, chk & ~well, bar=bar,
-                          arrays=[n for n in ARRAYS if n not in ILL_CONDITIONED_ARRAYS])
+                          arrays=[n for n in arrays if n not in ILL_CONDITIONED_ARRAYS])
         failures = failures + more
     return failures
 

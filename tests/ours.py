@@ -49,17 +49,26 @@ def run_forward(scene, cam, bg, extra=None, prune_mask=None, quant=None, dev="cu
 GRAD_NAMES = ["dL_dmeans2D", "dL_dcolors", "dL_dopacity", "dL_dmeans3D", "dL_dcov3D", "dL_dsh", "dL_dscales", "dL_drotations"]
 
 
-def run_backward(args, out, dL, lam=0.0, prune_mask=None, quant=None, aa=False, deterministic=False):
+def run_backward(args, out, dL, lam=0.0, prune_mask=None, quant=None, aa=False, deterministic=False, dL_dinvdepth=None,
+                 dL_dalpha=None, features=None, dL_dfeatures_out=None, camera_grads=False):
+    """-> dict of the gradients (GRAD_NAMES and dL_dconic), plus dL_dviewmatrix / dL_dprojmatrix / dL_dcampos with `camera_grads`
+    and dL_dfeatures with `features`; dL_dinvdepth / dL_dalpha [H,W] are the maps' upstream gradients, `features` [P,F] and
+    dL_dfeatures_out [F,H,W] the feature image's (any array-likes)."""
     (bg, means3D, colors, opacity, scales, rotations, mod, cov, view, proj, tx, ty, H, W, sh, degrees, campos, _, _) = args
-    R, color, radii, geom, binning, img = out
+    R, color, radii, geom, binning, img = out[:6]
     dev = means3D.device
+    dev_t = lambda a: None if a is None else torch.as_tensor(a, dtype=torch.float32).to(dev).contiguous()
+    dmap = lambda a: None if a is None else dev_t(a).view(1, H, W)
     grads = _C.rasterize_gaussians_backward(bg, means3D, radii, colors, scales, rotations, mod, cov, view, proj, tx, ty,
                                             dL.to(dev), sh, degrees, campos, geom, R, binning, img, lam, False,
                                             prune_mask=None if prune_mask is None else prune_mask.to(dev),
                                             quant=None if quant is None else quant.to(dev), want_conic=True, antialiasing=aa,
-                                            deterministic=deterministic)
+                                            deterministic=deterministic, dL_dinvdepth=dmap(dL_dinvdepth), dL_dalpha=dmap(dL_dalpha),
+                                            features=dev_t(features), dL_dfeatures_out=dev_t(dL_dfeatures_out),
+                                            camera_grads=camera_grads)
     torch.cuda.synchronize()
-    res = {n: g.cpu().numpy() for n, g in zip(GRAD_NAMES + ["dL_dconic"], grads)}
+    names = GRAD_NAMES + ["dL_dconic"] + (["dL_dviewmatrix", "dL_dprojmatrix", "dL_dcampos"] if camera_grads else [])
+    res = {n: g.cpu().numpy() for n, g in zip(names + (["dL_dfeatures"] if features is not None else []), grads)}
     return res
 
 
