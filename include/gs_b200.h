@@ -131,6 +131,26 @@ GSB_API size_t gsb_image_bytes(int32_t width, int32_t height);
 GSB_API size_t gsb_image_bytes_for(int32_t P, int32_t width, int32_t height, int32_t quantised);
 GSB_API size_t gsb_binning_bytes(int64_t num_rendered);
 
+/* Request checks.  The fourteen rasterizer entry points below (the forwards gsb_forward, _statistics, _statistics_deterministic,
+ * _maps, _antialiased, _raw and the backwards gsb_backward, _maps, _camera, _antialiased, _raw, _deterministic, _absgrad,
+ * _features) check their arguments in one order and stop at the first that fails, before any CUDA call: nothing is launched or
+ * written.  gsb_last_error() then starts with the entry point's name without "gsb_" (e.g. "backward_absgrad: "), except for
+ * the camera and scene checks (forward steps 5 and 6, backward step 8), which are the same for every entry point of a direction
+ * and start with "forward request: " / "backward request: ".  The code is GSB_EINVAL except where marked.  First comes the entry point's own requirement, where its text names one; then, for the
+ * options the entry point has:
+ *   Forward:  1. scene NULL or P < 0;  2. one map output without the other;  3. statistics: a NULL output with P > 0; in the
+ *             deterministic form then a NULL workspace with P > 0, and GSB_ERANGE for width * height >= 2^28;  4. raw parameters:
+ *             the checks listed at gsb_forward_raw;  5. the camera: NULL, a bad image size, a NULL camera tensor;  6. with P > 0 the
+ *             scene's tensors (means3D; the codebooks, or opacities and, without raw parameters, exactly one of shs /
+ *             colors_precomp and of scales + rotations / cov3D_precomp);  7. out_color, num_rendered, and radii with P > 0.
+ *   Backward: 1. scene NULL or P < 0;  2. features: det_workspace given, then the GsbFeatures checks (gsb_backward_features);
+ *             3. absgrad: dL_dmeans2D_abs NULL with P > 0, then grads->accumulate set;  4. num_rendered < 0;  5. deterministic:
+ *             GSB_ERANGE for num_rendered >= 2^30, then det_workspace NULL with P > 0 and num_rendered > 0;  6. a camera output
+ *             without workspace;  7. raw_grads without raw, then with raw the checks listed at gsb_backward_raw;  8. the camera and
+ *             the scene as in forward steps 5 and 6;  9. grads NULL;  10. with P > 0 a NULL blob, dL_dout_color or radii, then a
+ *             NULL gradient output.
+ * Every backward refuses num_rendered < 0 (gsb_backward, _maps, _camera, _antialiased and _raw used to accept it). */
+
 /* Forward.  Writes out_color [3,H,W] and radii [P]; *num_rendered [host] receives R.
  * The stream is never drained: the instance count (which sizes the binning blob, rasterizer_impl.cu:445-450) is copied to the
  * host in the background while scatter / sort are already queued against the capacity recent frames needed, and the host
@@ -159,8 +179,8 @@ GSB_API int gsb_forward_statistics(const GsbScene* scene, const GsbCamera* cam,
  * transmittances is rounded to a multiple of 2^-36 and added as a 64-bit integer, so the order of the additions does not matter;
  * each total is then rounded to float once (relative error below 1e-7 against the exact sum of the per-warp sums).
  * gsb_statistics_workspace_bytes: the workspace size for P Gaussians (8 bytes per Gaussian); one workspace serves every camera.
- * Errors (GSB_EINVAL, nothing launched): those of gsb_forward_statistics, and workspace NULL with P > 0.
- * GSB_ERANGE: width * height >= 2^28 (a Gaussian's total, at most width * height, must fit 64 bits at 2^36 per unit). */
+ * Errors: the request checks; the deterministic form's step 3 adds workspace NULL with P > 0 and GSB_ERANGE for
+ * width * height >= 2^28 (a Gaussian's total, at most width * height, must fit 64 bits at 2^36 per unit). */
 GSB_API size_t gsb_statistics_workspace_bytes(int32_t P);
 GSB_API int gsb_forward_statistics_deterministic(const GsbScene* scene, const GsbCamera* cam,
                 gsb_alloc_fn geom_alloc, void* geom_user,
@@ -180,7 +200,8 @@ GSB_API int gsb_backward(const GsbScene* scene, const GsbCamera* cam, int64_t nu
  *                composite the colour, with the same alpha and T.  depth_i is the preprocess view-space z (GsbDebug.depths),
  *                1/depth_i is an IEEE division; no background term, no normalisation by alpha.
  *   out_alpha    [1,H,W] fp32: 1 - final_T.
- * Both are required.  P == 0 gives zero maps; a scene with no (Gaussian, tile) instance gives invdepth 0 and alpha 0.
+ * Both are required: a NULL one is refused before the request checks.  P == 0 gives zero maps; a scene with no (Gaussian, tile)
+ * instance gives invdepth 0 and alpha 0.
  * Colour, radii, R and the blobs are bit-identical to gsb_forward's, and the maps are the same bytes on every run.
  * Everything else as gsb_forward. */
 GSB_API int gsb_forward_maps(const GsbScene* scene, const GsbCamera* cam,
@@ -284,8 +305,10 @@ typedef struct GsbRawGrads {
  *                   values as the forward's).  grads->dL_dsh, dL_dscales and dL_drotations must be NULL (raw_grads replaces them);
  *                   grads->dL_dcov3D and dL_dcolors may be NULL (not written).  Everything else as gsb_backward_antialiased /
  *                   gsb_backward_camera; per-Gaussian outputs other than the four raw gradients are those of the activated call.
- * Errors (GSB_EINVAL, nothing launched): raw NULL, C not in {0, 3, 8, 15}, a scene field above that must be NULL, and with P > 0
- * NULL scaling / rotation / degrees, or SH pointers that do not match colors_precomp and C. */
+ * Errors: raw NULL, before the request checks.  The raw-parameter checks (forward step 4, backward step 7; also in the backwards
+ * below when they get raw parameters): C not in {0, 3, 8, 15}, a scene field above that must be NULL, and with P > 0 NULL
+ * scaling / rotation / degrees, or SH pointers that do not match colors_precomp and C; in the backward then grads or raw_grads
+ * NULL, a grads field above that must be NULL, and SH gradients that do not match colors_precomp or C. */
 GSB_API int gsb_forward_raw(const GsbScene* scene, const GsbCamera* cam,
                 gsb_alloc_fn geom_alloc, void* geom_user,
                 gsb_alloc_fn binning_alloc, void* binning_user,
@@ -312,9 +335,7 @@ GSB_API int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_
  *                   gsb_backward_antialiased dispatch it.  It pairs with the blobs of any forward with the same anti-aliasing flag.
  *                   No host synchronisation.  A num_rendered > 0 other than the blobs' instance count makes every accumulated
  *                   gradient NaN (and no slot beyond num_rendered is written); num_rendered = 0 means nothing was rendered.
- * Errors (GSB_EINVAL, nothing launched): scene NULL, P < 0, num_rendered < 0, det_workspace NULL with P > 0 and num_rendered > 0,
- * a camera gradient without workspace, raw_grads without raw, and with raw the checks of gsb_backward_raw.
- * GSB_ERANGE: num_rendered >= 2^30. */
+ * Errors: the request checks with backward step 5 (GSB_ERANGE for num_rendered >= 2^30; det_workspace NULL). */
 GSB_API size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered);
 GSB_API int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
                  const char* geom_blob, const char* binning_blob, const char* image_blob,
@@ -335,9 +356,8 @@ GSB_API int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* c
  *   det_workspace NULL: the default backward (float atomics); else gsb_absgrad_deterministic_workspace_bytes(P, num_rendered) bytes
  *                   and the deterministic backward: dL_dmeans2D_abs is then the same bytes on every run too.
  * gsb_absgrad_deterministic_workspace_bytes: gsb_deterministic_workspace_bytes plus 8 bytes per instance (48 bytes per instance).
- * Errors (GSB_EINVAL, nothing launched): scene NULL, P < 0, num_rendered < 0, dL_dmeans2D_abs NULL with P > 0, grads->accumulate != 0
- * (no view-batch form), a camera gradient without workspace, raw_grads without raw, and with raw the checks of gsb_backward_raw.
- * GSB_ERANGE: num_rendered >= 2^30 with det_workspace.  There is no feature-channel form (gsb_backward_features). */
+ * Errors: the request checks with backward step 3 (grads->accumulate is refused: there is no view-batch form) and, with
+ * det_workspace, step 5.  There is no feature-channel form (gsb_backward_features). */
 GSB_API size_t gsb_absgrad_deterministic_workspace_bytes(int32_t P, int64_t num_rendered);
 GSB_API int gsb_backward_absgrad(const GsbScene* scene, const GsbCamera* cam, int64_t num_rendered, const int32_t* radii,
                  const char* geom_blob, const char* binning_blob, const char* image_blob,
@@ -361,10 +381,12 @@ GSB_API int gsb_backward_absgrad(const GsbScene* scene, const GsbCamera* cam, in
  *                          and, through alpha, the same per-Gaussian gradients the colour image reaches (dL_dopacity, dL_dmeans2D,
  *                          dL_dmeans3D, dL_dscales / dL_drotations / dL_dcov3D, raw_grads, the camera); dL_dcolors and the SH
  *                          gradients are the colour image's alone.  det_workspace must be NULL: the feature backward sums with float
- *                          atomics.  With features NULL this is gsb_backward_deterministic.
- * Errors (GSB_EINVAL, nothing launched): features NULL (forward), F outside 1..GSB_FEATURES_MAX, P < 0, R < 0, a bad image size, and
- * with P > 0 a NULL blob, features, out (forward) or dL_dout / dL_dfeatures (backward); in the backward also a non-NULL det_workspace
- * together with features, and every error of gsb_backward_deterministic. */
+ *                          atomics.  With features NULL this is gsb_backward_deterministic when det_workspace is given, and the
+ *                          default (float-atomic) backward otherwise.
+ * Errors of gsb_forward_features (GSB_EINVAL, nothing launched): features NULL, F outside 1..GSB_FEATURES_MAX, a NULL out, P < 0,
+ * R < 0, a bad image size, and with P > 0 a NULL blob or features.
+ * Errors of gsb_backward_features: the request checks with backward step 2 (det_workspace together with features, then F outside
+ * 1..GSB_FEATURES_MAX, and with P > 0 NULL features, dL_dout or dL_dfeatures) or, without features but with det_workspace, step 5. */
 #define GSB_FEATURES_MAX 256
 typedef struct GsbFeatures {
 	int32_t F;                   /* channels, 1..GSB_FEATURES_MAX                              */
