@@ -122,31 +122,29 @@ int launch_camera_grad_finish(int, const float*, float*, float*, float*, cudaStr
 // geometry blob = GeomState followed by the backward's gradient accumulator (12 floats per Gaussian)
 static size_t geom_state_bytes(int P) { size_t b; GeomState::carve(nullptr, P, &b); return (b + 255) & ~size_t(255); }
 
-// The request checks: check_forward / check_backward validate a request before forward_impl / backward_impl make any CUDA call,
-// in the order include/gs_b200.h lists under "Request checks".  `fn` names the entry point, and every message starts with it
-// except those of check_scene, which name the direction.
+// The request checks: check_forward / check_backward validate a request before gsb_forward / gsb_backward make any CUDA call, in
+// the order include/gs_b200.h lists under "Request checks".  Every message starts with the direction, `dir`.
 
-// With raw parameters (gsb_forward_raw / gsb_backward_raw and the backwards that take them): what the scene and the raw struct hold.
-static int check_raw(const char* fn, const GsbScene* s, const GsbRawParams* raw)
+// With raw parameters: what the scene and the raw struct hold.
+static int check_raw(const char* dir, const GsbScene* s, const GsbRawParams* raw)
 {
 	if (raw->C != 0 && raw->C != 3 && raw->C != 8 && raw->C != 15)
-	{ set_error("%s: raw parameters: C = %d rest coefficients; only 0, 3, 8 or 15 (max SH degree 0..3) exist", fn, raw->C); return GSB_EINVAL; }
+	{ set_error("%s: raw parameters: C = %d rest coefficients; only 0, 3, 8 or 15 (max SH degree 0..3) exist", dir, raw->C); return GSB_EINVAL; }
 	if (s->scales || s->rotations || s->shs || s->cov3D_precomp || s->quant || s->sh_packed)
-	{ set_error("%s: raw parameters: the scene's scales, rotations, shs, cov3D_precomp and quant must be NULL and sh_packed 0", fn); return GSB_EINVAL; }
+	{ set_error("%s: raw parameters: the scene's scales, rotations, shs, cov3D_precomp and quant must be NULL and sh_packed 0", dir); return GSB_EINVAL; }
 	if (s->P == 0) return GSB_OK;
-	if (!raw->scaling || !raw->rotation) { set_error("%s: raw parameters: scaling / rotation missing", fn); return GSB_EINVAL; }
+	if (!raw->scaling || !raw->rotation) { set_error("%s: raw parameters: scaling / rotation missing", dir); return GSB_EINVAL; }
 	if (s->colors_precomp)
 	{
-		if (raw->features_dc || raw->features_rest) { set_error("%s: raw parameters: SH given together with colors_precomp", fn); return GSB_EINVAL; }
+		if (raw->features_dc || raw->features_rest) { set_error("%s: raw parameters: SH given together with colors_precomp", dir); return GSB_EINVAL; }
 	}
 	else if (!raw->features_dc || !s->degrees || (raw->features_rest == nullptr) != (raw->C == 0))
-	{ set_error("%s: raw parameters: features_dc, degrees and (for C > 0) features_rest are required without colors_precomp", fn); return GSB_EINVAL; }
+	{ set_error("%s: raw parameters: features_dc, degrees and (for C > 0) features_rest are required without colors_precomp", dir); return GSB_EINVAL; }
 	return GSB_OK;
 }
 
 // The camera and the scene's tensors; the scene itself is non-NULL with P >= 0.  raw: check_raw replaces the checks of the
-// activated inputs.  These checks are the same for every entry point of a direction, and their messages name the direction
-// ("forward request" / "backward request"): a camera or scene error never reads as an error of the entry point's option.
+// activated inputs.
 static int check_scene(const char* dir, const GsbScene* s, const GsbCamera* c, bool raw)
 {
 	if (!c) { set_error("%s: camera is NULL", dir); return GSB_EINVAL; }
@@ -173,84 +171,88 @@ static int check_scene(const char* dir, const GsbScene* s, const GsbCamera* c, b
 	return GSB_OK;
 }
 
-// The feature pass's own arguments (gsb_forward_features / a backward with features).
-static int check_features(const char* fn, const GsbFeatures* f, int P, bool backward)
+// The feature pass's own fields (a request with features).
+static int check_features(const char* dir, const GsbFeatures* f, int P, bool backward)
 {
-	if (!f) { set_error("%s: features is NULL", fn); return GSB_EINVAL; }
-	if (f->F < 1 || f->F > GSB_FEATURES_MAX) { set_error("%s: F = %d channels; 1..%d are supported", fn, f->F, GSB_FEATURES_MAX); return GSB_EINVAL; }
-	if (P > 0 && !f->features) { set_error("%s: features->features is NULL", fn); return GSB_EINVAL; }
-	if (backward && P > 0 && (!f->dL_dout || !f->dL_dfeatures)) { set_error("%s: features->dL_dout / dL_dfeatures is NULL", fn); return GSB_EINVAL; }
-	if (!backward && !f->out) { set_error("%s: features->out is NULL", fn); return GSB_EINVAL; }
+	if (f->F < 1 || f->F > GSB_FEATURES_MAX) { set_error("%s: F = %d channels; 1..%d are supported", dir, f->F, GSB_FEATURES_MAX); return GSB_EINVAL; }
+	if (P > 0 && !f->features) { set_error("%s: features->features is NULL", dir); return GSB_EINVAL; }
+	if (backward && P > 0 && (!f->dL_dout || !f->dL_dfeatures)) { set_error("%s: features->dL_dout / dL_dfeatures is NULL", dir); return GSB_EINVAL; }
+	if (!backward && !f->out) { set_error("%s: features->out is NULL", dir); return GSB_EINVAL; }
 	return GSB_OK;
 }
 
-static int check_forward(const char* fn, const ForwardRequest& r)
+static int check_forward(const GsbForwardRequest& r)
 {
 	const GsbScene* s = r.scene; const GsbCamera* c = r.cam;
-	if (!s || s->P < 0) { set_error("%s: scene is NULL or P < 0", fn); return GSB_EINVAL; }
+	if (!s || s->P < 0) { set_error("forward: scene is NULL or P < 0"); return GSB_EINVAL; }
+	if (r.features) if (int e = check_features("forward", r.features, s->P, false)) return e;
 	if ((r.out_invdepth == nullptr) != (r.out_alpha == nullptr))
-	{ set_error("%s: give both map outputs (invdepth and alpha) or neither", fn); return GSB_EINVAL; }
-	if (r.statistics && s->P > 0 && (!r.touched_pixels || !r.transmittance))
-	{ set_error("%s: statistics output pointers missing", fn); return GSB_EINVAL; }
-	if (r.stats_fixed)
+	{ set_error("forward: give both map outputs (invdepth and alpha) or neither"); return GSB_EINVAL; }
+	if (statistics(r))
 	{
-		if (s->P > 0 && !r.transmittance_fixed) { set_error("%s: workspace is NULL", fn); return GSB_EINVAL; }
-		if (c && (long long)c->width * c->height >= (1ll << 28))
-		{ set_error("%s: %d x %d pixels; the 64-bit fixed-point sums need W * H < 2^28", fn, c->width, c->height); return GSB_ERANGE; }
+		if (!r.touched_pixels || !r.transmittance_sum) { set_error("forward: statistics output pointers missing"); return GSB_EINVAL; }
+		if (r.out_invdepth || r.antialiasing || r.raw)
+		{ set_error("forward: statistics go without the maps, antialiasing and raw parameters"); return GSB_EINVAL; }
+		if (r.deterministic)
+		{
+			if (s->P > 0 && !r.workspace) { set_error("forward: workspace is NULL"); return GSB_EINVAL; }
+			if (c && (long long)c->width * c->height >= (1ll << 28))
+			{ set_error("forward: %d x %d pixels; the 64-bit fixed-point sums need W * H < 2^28", c->width, c->height); return GSB_ERANGE; }
+		}
 	}
-	if (r.raw) if (int e = check_raw(fn, s, r.raw)) return e;
-	if (int e = check_scene("forward request", s, c, r.raw != nullptr)) return e;
-	if (!r.out_color || !r.num_rendered || (s->P > 0 && !r.radii)) { set_error("%s: output pointers missing", fn); return GSB_EINVAL; }
+	if (r.raw) if (int e = check_raw("forward", s, r.raw)) return e;
+	if (int e = check_scene("forward", s, c, r.raw != nullptr)) return e;
+	if (!r.out_color || !r.num_rendered || (s->P > 0 && !r.radii)) { set_error("forward: output pointers missing"); return GSB_EINVAL; }
 	return GSB_OK;
 }
 
-static int check_backward(const char* fn, const BackwardRequest& r)
+static int check_backward(const GsbBackwardRequest& r)
 {
 	const GsbScene* s = r.scene; const GsbGrads* grads = r.grads;
-	if (!s || s->P < 0) { set_error("%s: scene is NULL or P < 0", fn); return GSB_EINVAL; }
+	if (!s || s->P < 0) { set_error("backward: scene is NULL or P < 0"); return GSB_EINVAL; }
 	if (r.features)
 	{
-		if (r.deterministic) { set_error("%s: the feature backward has no deterministic form; det_workspace must be NULL", fn); return GSB_EINVAL; }
-		if (int e = check_features(fn, r.features, s->P, true)) return e;
+		if (r.deterministic) { set_error("backward: the feature backward has no deterministic form; deterministic must be 0"); return GSB_EINVAL; }
+		if (int e = check_features("backward", r.features, s->P, true)) return e;
 	}
-	if (r.absgrad)
+	if (r.dL_dmeans2D_abs)
 	{
-		if (s->P > 0 && !r.dL_dmeans2D_abs) { set_error("%s: dL_dmeans2D_abs is NULL", fn); return GSB_EINVAL; }
+		if (r.features) { set_error("backward: the absolute gradient has no feature form; give features or dL_dmeans2D_abs"); return GSB_EINVAL; }
 		if (grads && grads->accumulate)
-		{ set_error("%s: grads->accumulate is set; the absolute gradient has no view-batch accumulation form", fn); return GSB_EINVAL; }
+		{ set_error("backward: grads->accumulate is set; the absolute gradient has no view-batch accumulation form"); return GSB_EINVAL; }
 	}
-	if (r.R < 0) { set_error("%s: num_rendered < 0", fn); return GSB_EINVAL; }
+	if (r.num_rendered < 0) { set_error("backward: num_rendered < 0"); return GSB_EINVAL; }
 	if (r.deterministic)
 	{
-		if (r.R >= (1ll << 30))
-		{ set_error("%s: 2^30 or more instances (the slot scan's look-back descriptors carry 30-bit counts)", fn); return GSB_ERANGE; }
-		if (s->P > 0 && r.R > 0 && !r.det_workspace) { set_error("%s: det_workspace is NULL", fn); return GSB_EINVAL; }
+		if (r.num_rendered >= (1ll << 30))
+		{ set_error("backward: 2^30 or more instances (the slot scan's look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
+		if (s->P > 0 && r.num_rendered > 0 && !r.det_workspace) { set_error("backward: det_workspace is NULL"); return GSB_EINVAL; }
 	}
-	if (r.want_cam() && !r.cam_workspace) { set_error("%s: a camera gradient is requested but the workspace is NULL", fn); return GSB_EINVAL; }
-	if (r.raw_grads && !r.raw) { set_error("%s: raw_grads given without raw", fn); return GSB_EINVAL; }
+	if (want_cam(r) && !r.camera_workspace) { set_error("backward: a camera gradient is requested but the workspace is NULL"); return GSB_EINVAL; }
+	if (r.raw_grads && !r.raw) { set_error("backward: raw_grads given without raw"); return GSB_EINVAL; }
 	if (r.raw)
 	{
-		if (int e = check_raw(fn, s, r.raw)) return e;
+		if (int e = check_raw("backward", s, r.raw)) return e;
 		const GsbRawGrads* rg = r.raw_grads;
-		if (!rg || !grads) { set_error("%s: grads / raw_grads are NULL", fn); return GSB_EINVAL; }
+		if (!rg || !grads) { set_error("backward: grads / raw_grads are NULL"); return GSB_EINVAL; }
 		if (grads->dL_dsh || grads->dL_dscales || grads->dL_drotations)
-		{ set_error("%s: grads->dL_dsh, dL_dscales and dL_drotations must be NULL (raw_grads replaces them)", fn); return GSB_EINVAL; }
+		{ set_error("backward: grads->dL_dsh, dL_dscales and dL_drotations must be NULL (raw_grads replaces them)"); return GSB_EINVAL; }
 		if (s->colors_precomp && (rg->dL_dfeatures_dc || rg->dL_dfeatures_rest))
-		{ set_error("%s: SH gradients requested together with colors_precomp", fn); return GSB_EINVAL; }
-		if (r.raw->C == 0 && rg->dL_dfeatures_rest) { set_error("%s: dL_dfeatures_rest given with C == 0", fn); return GSB_EINVAL; }
+		{ set_error("backward: SH gradients requested together with colors_precomp"); return GSB_EINVAL; }
+		if (r.raw->C == 0 && rg->dL_dfeatures_rest) { set_error("backward: dL_dfeatures_rest given with C == 0"); return GSB_EINVAL; }
 	}
-	if (int e = check_scene("backward request", s, r.cam, r.raw != nullptr)) return e;
-	if (!grads) { set_error("%s: grads is NULL", fn); return GSB_EINVAL; }
+	if (int e = check_scene("backward", s, r.cam, r.raw != nullptr)) return e;
+	if (!grads) { set_error("backward: grads is NULL"); return GSB_EINVAL; }
 	if (s->P == 0) return GSB_OK;
-	if (!r.geom_blob || !r.binning_blob || !r.image_blob || !r.dL_dout_color || !r.radii) { set_error("%s: backward inputs missing", fn); return GSB_EINVAL; }
+	if (!r.geom_blob || !r.binning_blob || !r.image_blob || !r.dL_dout_color || !r.radii) { set_error("backward: backward inputs missing"); return GSB_EINVAL; }
 	if (r.raw)
 	{
 		if (!grads->dL_dmeans2D || !grads->dL_dopacity || !grads->dL_dmeans3D || !r.raw_grads->dL_dscaling || !r.raw_grads->dL_drotation)
-		{ set_error("%s: gradient output pointers missing", fn); return GSB_EINVAL; }
+		{ set_error("backward: gradient output pointers missing"); return GSB_EINVAL; }
 	}
 	else if (!grads->dL_dmeans2D || !grads->dL_dcolors || !grads->dL_dopacity || !grads->dL_dmeans3D || !grads->dL_dcov3D ||
 		!grads->dL_dscales || !grads->dL_drotations || (s->M > 0 && !grads->dL_dsh))
-	{ set_error("%s: gradient output pointers missing", fn); return GSB_EINVAL; }
+	{ set_error("backward: gradient output pointers missing"); return GSB_EINVAL; }
 	return GSB_OK;
 }
 
@@ -272,7 +274,7 @@ size_t gsb_image_bytes_for(int32_t P, int32_t W, int32_t H, int32_t quantised)
 size_t gsb_binning_bytes(int64_t R) { size_t b; BinningState::carve(nullptr, R, &b); return b + 256; }
 uint64_t gsb_launch_count(void) { return g_launch_count.load(); }
 const char* gsb_last_error(void) { return g_err; }
-const char* gsb_version(void) { return "gs_b200 0.1 (sm_90a)"; }
+const char* gsb_version(void) { return "gs_b200 0.2 (sm_90a)"; }
 
 void gsb_profile_enable(int on)
 {
@@ -320,10 +322,12 @@ struct HostSide {
 static thread_local std::map<int, HostSide> t_host;
 }
 
-static int forward_impl(const char* fn, const ForwardRequest& r)
+int gsb_forward(const GsbForwardRequest* req)
 {
-	if (int e = check_forward(fn, r)) return e;
-	const GsbScene* scene = r.scene; const cudaStream_t stream = r.stream;
+	if (!req) { set_error("forward: request is NULL"); return GSB_EINVAL; }
+	const GsbForwardRequest& r = *req;
+	if (int e = check_forward(r)) return e;
+	const GsbScene* scene = r.scene; const cudaStream_t stream = stream_of(r);
 	*r.num_rendered = 0;
 	const int P = scene->P, W = r.cam->width, H = r.cam->height;
 	const size_t N = size_t(W) * H;
@@ -333,19 +337,21 @@ static int forward_impl(const char* fn, const ForwardRequest& r)
 		GSB_CUDA_OK(cudaMemsetAsync(r.out_color, 0, 3 * N * sizeof(float), stream));
 		if (r.out_invdepth) GSB_CUDA_OK(cudaMemsetAsync(r.out_invdepth, 0, N * sizeof(float), stream));
 		if (r.out_alpha) GSB_CUDA_OK(cudaMemsetAsync(r.out_alpha, 0, N * sizeof(float), stream));
+		// the forward of an empty scene allocates no blobs; its feature image is zero like its colour image
+		if (r.features) GSB_CUDA_OK(cudaMemsetAsync(r.features->out, 0, size_t(r.features->F) * N * sizeof(float), stream));
 		return GSB_OK;
 	}
-	if (r.statistics)
+	if (statistics(r))
 	{
 		// reduced_3dgs.cu:117-118: both statistics start from zero for every camera
 		GSB_CUDA_OK(cudaMemsetAsync(r.touched_pixels, 0, size_t(P) * sizeof(int32_t), stream));
-		if (r.stats_fixed) GSB_CUDA_OK(cudaMemsetAsync(r.transmittance_fixed, 0, size_t(P) * sizeof(unsigned long long), stream));
-		else GSB_CUDA_OK(cudaMemsetAsync(r.transmittance, 0, size_t(P) * sizeof(float), stream));
+		if (stats_fixed(r)) GSB_CUDA_OK(cudaMemsetAsync(transmittance_fixed(r), 0, size_t(P) * sizeof(unsigned long long), stream));
+		else GSB_CUDA_OK(cudaMemsetAsync(r.transmittance_sum, 0, size_t(P) * sizeof(float), stream));
 	}
 	const BinPlan plan = make_bin_plan(P, W, H, scene->quant != nullptr);
 	char* geom_blob = r.geom_alloc(r.geom_user, gsb_geom_bytes(P));
 	char* img_blob = r.image_alloc(r.image_user, gsb_image_bytes_for(P, W, H, scene->quant != nullptr));
-	if (!geom_blob || !img_blob) { set_error("%s: scratch allocation failed", fn); return GSB_ENOMEM; }
+	if (!geom_blob || !img_blob) { set_error("forward: scratch allocation failed"); return GSB_ENOMEM; }
 	GeomState g = GeomState::carve(geom_blob, P);
 	ImageState img = ImageState::carve(img_blob, W, H, nullptr, plan.priv ? plan.ctas : 0);
 	GSB_CUDA_OK(cudaMemsetAsync(g.counters, 0, 16 * sizeof(uint32_t), stream));
@@ -370,14 +376,14 @@ static int forward_impl(const char* fn, const ForwardRequest& r)
 	if (cap > 0)
 	{
 		char* bin_blob = r.binning_alloc(r.binning_user, gsb_binning_bytes(cap));
-		if (!bin_blob) { set_error("%s: binning allocation failed", fn); return GSB_ENOMEM; }
+		if (!bin_blob) { set_error("forward: binning allocation failed"); return GSB_ENOMEM; }
 		b = BinningState::carve(bin_blob, cap);
 		if (int e = launch_scatter_sort(g, b, img, plan, P, cap, W, H, stream)) return e;
 	}
 	GSB_CUDA_OK(cudaEventSynchronize(hs.arrived));
 	const uint32_t* hc = hs.counters;
-	if (hc[3]) { set_error("%s: Point is filtered although prefiltered is set. This shouldn't happen!", fn); return GSB_ECUDA; }
-	if (hc[6]) { set_error("%s: the (Gaussian, tile) instance count does not fit 31 bits", fn); return GSB_ERANGE; }
+	if (hc[3]) { set_error("forward: Point is filtered although prefiltered is set. This shouldn't happen!"); return GSB_ECUDA; }
+	if (hc[6]) { set_error("forward: the (Gaussian, tile) instance count does not fit 31 bits"); return GSB_ERANGE; }
 	const long long R = hc[0];
 	if (R > hs.r_hint || 2 * R < hs.r_hint) hs.r_hint = R;       // grows with the workload, restarts when a much smaller one begins
 	*r.num_rendered = R;
@@ -385,67 +391,17 @@ static int forward_impl(const char* fn, const ForwardRequest& r)
 	{
 		// first frame of this thread on this device, or more instances than speculated (the guarded kernels above did nothing)
 		char* bin_blob = r.binning_alloc(r.binning_user, gsb_binning_bytes(R));
-		if (!bin_blob) { set_error("%s: binning allocation failed", fn); return GSB_ENOMEM; }
+		if (!bin_blob) { set_error("forward: binning allocation failed"); return GSB_ENOMEM; }
 		b = BinningState::carve(bin_blob, R);
 		if (int e = launch_scatter_sort(g, b, img, plan, P, R, W, H, stream)) return e;
 	}
 	if (R > 0) if (int e = launch_sort_large(g, b, img, W, H, hc[4], hc[5], stream)) return e;
 	if (int e = launch_render_forward(r, img, b, g)) return e;
-	return r.stats_fixed ? launch_stats_fixed_to_float(P, r.transmittance_fixed, r.transmittance, stream) : GSB_OK;
-}
-
-int gsb_forward(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
-	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
-	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, void* stream)
-{
-	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered,
-		debug };
-	r.stream = (cudaStream_t)stream;
-	return forward_impl("forward", r);
-}
-
-int gsb_forward_antialiased(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
-	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
-	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, float* out_invdepth, float* out_alpha, void* stream)
-{
-	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered,
-		debug };
-	r.out_invdepth = out_invdepth; r.out_alpha = out_alpha; r.aa = true; r.stream = (cudaStream_t)stream;
-	return forward_impl("forward_antialiased", r);
-}
-
-int gsb_forward_maps(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
-	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
-	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, float* out_invdepth, float* out_alpha, void* stream)
-{
-	if (!out_invdepth || !out_alpha) { set_error("forward_maps: map output pointers missing"); return GSB_EINVAL; }
-	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered,
-		debug };
-	r.out_invdepth = out_invdepth; r.out_alpha = out_alpha; r.stream = (cudaStream_t)stream;
-	return forward_impl("forward_maps", r);
-}
-
-int gsb_forward_statistics(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
-	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
-	float* out_color, int32_t* radii, int64_t* num_rendered, int32_t* touched_pixels, float* transmittance_sum, void* stream)
-{
-	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered };
-	r.statistics = true; r.touched_pixels = touched_pixels; r.transmittance = transmittance_sum; r.stream = (cudaStream_t)stream;
-	return forward_impl("forward_statistics", r);
+	if (stats_fixed(r)) if (int e = launch_stats_fixed_to_float(P, transmittance_fixed(r), r.transmittance_sum, stream)) return e;
+	return r.features ? launch_features_forward(img, b, g, W, H, *r.features, stream) : GSB_OK;
 }
 
 size_t gsb_statistics_workspace_bytes(int32_t P) { return (P > 0 ? size_t(P) * sizeof(unsigned long long) : 0) + 256; }
-
-int gsb_forward_statistics_deterministic(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
-	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
-	float* out_color, int32_t* radii, int64_t* num_rendered, int32_t* touched_pixels, float* transmittance_sum, char* workspace,
-	void* stream)
-{
-	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered };
-	r.statistics = true; r.stats_fixed = true; r.touched_pixels = touched_pixels; r.transmittance = transmittance_sum;
-	r.transmittance_fixed = reinterpret_cast<unsigned long long*>(workspace); r.stream = (cudaStream_t)stream;
-	return forward_impl("forward_statistics_deterministic", r);
-}
 
 int gsb_sh_statistics_update(int32_t P, int32_t M, const int32_t* degrees, const float* means3D, const float* campos, const float* shs,
 	const int32_t* radii, const int32_t* touched_pixels, const float* transmittance_sum, float* weight_sum, float* weight_sq_sum,
@@ -555,163 +511,39 @@ int gsb_min_redundancy_value(int32_t P, const int32_t* redundancy_values, const 
 	return launch_min_redundancy(P, redundancy_values, neighbours, intersection_mask, knn, minimum_redundancy_values, (cudaStream_t)stream);
 }
 
-static int backward_impl(const char* fn, const BackwardRequest& r)
+int gsb_backward(const GsbBackwardRequest* req)
 {
-	if (int e = check_backward(fn, r)) return e;
-	const cudaStream_t stream = r.stream;
+	if (!req) { set_error("backward: request is NULL"); return GSB_EINVAL; }
+	const GsbBackwardRequest& r = *req;
+	if (int e = check_backward(r)) return e;
+	const cudaStream_t stream = stream_of(r);
 	const int P = r.scene->P, W = r.cam->width, H = r.cam->height;
 	if (P == 0)
 	{
 		// no Gaussian, no camera gradient (the camera outputs are always written, also in accumulate mode)
-		if (r.dL_dview) GSB_CUDA_OK(cudaMemsetAsync(r.dL_dview, 0, 16 * sizeof(float), stream));
-		if (r.dL_dproj) GSB_CUDA_OK(cudaMemsetAsync(r.dL_dproj, 0, 16 * sizeof(float), stream));
+		if (r.dL_dviewmatrix) GSB_CUDA_OK(cudaMemsetAsync(r.dL_dviewmatrix, 0, 16 * sizeof(float), stream));
+		if (r.dL_dprojmatrix) GSB_CUDA_OK(cudaMemsetAsync(r.dL_dprojmatrix, 0, 16 * sizeof(float), stream));
 		if (r.dL_dcampos) GSB_CUDA_OK(cudaMemsetAsync(r.dL_dcampos, 0, 3 * sizeof(float), stream));
 		return GSB_OK;
 	}
 	GeomState g = GeomState::carve(const_cast<char*>(r.geom_blob), P);
 	ImageState img = ImageState::carve(const_cast<char*>(r.image_blob), W, H);
-	BinningState b = BinningState::carve(const_cast<char*>(r.binning_blob), r.R);
+	BinningState b = BinningState::carve(const_cast<char*>(r.binning_blob), r.num_rendered);
 	float* acc = reinterpret_cast<float*>(const_cast<char*>(r.geom_blob) + geom_state_bytes(P));
 	if (int e = r.deterministic ? launch_render_backward_deterministic(r, img, b, g, acc) : launch_render_backward(r, img, b, g, acc, nullptr, nullptr))
 		return e;
 	if (r.features) if (int e = launch_features_backward(img, b, g, P, W, H, *r.features, acc, stream)) return e;
 	if (int e = launch_preprocess_backward(r, g, acc)) return e;
 	if (r.dL_dmeans2D_abs) if (int e = launch_absgrad_finish(r, acc)) return e;
-	if (r.want_cam())
-		if (int e = launch_camera_grad_finish(P, reinterpret_cast<float*>(r.cam_workspace), r.dL_dview, r.dL_dproj, r.dL_dcampos, stream)) return e;
+	if (want_cam(r))
+		if (int e = launch_camera_grad_finish(P, reinterpret_cast<float*>(r.camera_workspace), r.dL_dviewmatrix, r.dL_dprojmatrix, r.dL_dcampos,
+			stream)) return e;
 	return GSB_OK;
 }
 
-int gsb_backward(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, float lambda_sh_sparsity, void* stream)
-{
-	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads };
-	r.lambda_sh_sparsity = lambda_sh_sparsity; r.stream = (cudaStream_t)stream;
-	return backward_impl("backward", r);
-}
-
 size_t gsb_camera_grad_workspace_bytes(int32_t P) { return camera_grad_workspace_bytes(P); }
-
-int gsb_backward_camera(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, void* stream)
-{
-	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
-	r.stream = (cudaStream_t)stream;
-	return backward_impl("backward_camera", r);
-}
-
-int gsb_backward_antialiased(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, void* stream)
-{
-	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
-	r.aa = true; r.stream = (cudaStream_t)stream;
-	return backward_impl("backward_antialiased", r);
-}
-
-int gsb_forward_raw(const GsbScene* scene, const GsbCamera* cam, gsb_alloc_fn geom_alloc, void* geom_user,
-	gsb_alloc_fn binning_alloc, void* binning_user, gsb_alloc_fn image_alloc, void* image_user,
-	float* out_color, int32_t* radii, int64_t* num_rendered, const GsbDebug* debug, float* out_invdepth, float* out_alpha,
-	const GsbRawParams* raw, int32_t antialiasing, void* stream)
-{
-	if (!raw) { set_error("forward_raw: raw parameters are NULL"); return GSB_EINVAL; }
-	ForwardRequest r{ scene, cam, geom_alloc, geom_user, binning_alloc, binning_user, image_alloc, image_user, out_color, radii, num_rendered,
-		debug };
-	r.out_invdepth = out_invdepth; r.out_alpha = out_alpha; r.aa = antialiasing != 0; r.raw = raw; r.stream = (cudaStream_t)stream;
-	return forward_impl("forward_raw", r);
-}
-
-int gsb_backward_raw(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
-	int32_t antialiasing, void* stream)
-{
-	if (!raw) { set_error("backward_raw: raw parameters are NULL"); return GSB_EINVAL; }
-	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
-	r.aa = antialiasing != 0; r.raw = raw; r.raw_grads = raw_grads; r.stream = (cudaStream_t)stream;
-	return backward_impl("backward_raw", r);
-}
-
 size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered, 10); }
-
-int gsb_backward_deterministic(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
-	int32_t antialiasing, char* det_workspace, void* stream)
-{
-	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
-	r.aa = antialiasing != 0; r.raw = raw; r.raw_grads = raw_grads; r.deterministic = true; r.det_workspace = det_workspace;
-	r.stream = (cudaStream_t)stream;
-	return backward_impl("backward_deterministic", r);
-}
-
 size_t gsb_absgrad_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered, DET_NS_ABS); }
-
-int gsb_backward_absgrad(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
-	int32_t antialiasing, char* det_workspace, float* dL_dmeans2D_abs, void* stream)
-{
-	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
-	r.aa = antialiasing != 0; r.raw = raw; r.raw_grads = raw_grads; r.deterministic = det_workspace != nullptr;
-	r.det_workspace = det_workspace; r.absgrad = true; r.dL_dmeans2D_abs = dL_dmeans2D_abs; r.stream = (cudaStream_t)stream;
-	return backward_impl("backward_absgrad", r);
-}
-
-int gsb_forward_features(const char* geom_blob, int32_t P, const char* binning_blob, int64_t R, const char* image_blob, int32_t W, int32_t H,
-	const GsbFeatures* features, void* stream_)
-{
-	if (int e = check_features("forward_features", features, P, false)) return e;
-	if (P < 0 || R < 0) { set_error("forward_features: P < 0 or num_rendered < 0"); return GSB_EINVAL; }
-	if (W <= 0 || H <= 0) { set_error("forward_features: bad image size %dx%d", W, H); return GSB_EINVAL; }
-	if (P > 0 && (!geom_blob || !binning_blob || !image_blob)) { set_error("forward_features: a blob is NULL"); return GSB_EINVAL; }
-	const cudaStream_t stream = (cudaStream_t)stream_;
-	if (P == 0)
-	{
-		// the forward of an empty scene allocates no blobs; its feature image is zero like its colour image
-		GSB_CUDA_OK(cudaMemsetAsync(features->out, 0, size_t(features->F) * W * H * sizeof(float), stream));
-		return GSB_OK;
-	}
-	GeomState g = GeomState::carve(const_cast<char*>(geom_blob), P);
-	BinningState b = BinningState::carve(const_cast<char*>(binning_blob), R);
-	ImageState img = ImageState::carve(const_cast<char*>(image_blob), W, H);
-	return launch_features_forward(img, b, g, W, H, *features, stream);
-}
-
-int gsb_backward_features(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity,
-	float* dL_dviewmatrix, float* dL_dprojmatrix, float* dL_dcampos, char* workspace, const GsbRawParams* raw, const GsbRawGrads* raw_grads,
-	int32_t antialiasing, char* det_workspace, const GsbFeatures* features, void* stream)
-{
-	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity, dL_dviewmatrix, dL_dprojmatrix, dL_dcampos, workspace };
-	r.aa = antialiasing != 0; r.raw = raw; r.raw_grads = raw_grads; r.deterministic = det_workspace != nullptr;
-	r.det_workspace = det_workspace; r.features = features; r.stream = (cudaStream_t)stream;
-	return backward_impl("backward_features", r);
-}
-
-int gsb_backward_maps(const GsbScene* scene, const GsbCamera* cam, int64_t R, const int32_t* radii,
-	const char* geom_blob, const char* binning_blob, const char* image_blob, const float* dL_dout_color,
-	const GsbGrads* grads, const float* dL_dinvdepth, const float* dL_dalpha, float lambda_sh_sparsity, void* stream)
-{
-	BackwardRequest r{ scene, cam, R, radii, geom_blob, binning_blob, image_blob, dL_dout_color, grads, dL_dinvdepth, dL_dalpha,
-		lambda_sh_sparsity };
-	r.stream = (cudaStream_t)stream;
-	return backward_impl("backward_maps", r);
-}
 
 int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present, void* stream)
 {

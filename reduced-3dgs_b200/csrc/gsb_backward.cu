@@ -633,7 +633,7 @@ int launch_camera_grad_finish(int P, const float* rows, float* dview, float* dpr
 	return GSB_OK;
 }
 
-int launch_preprocess_backward(const BackwardRequest& req, const GeomState& g, const float* acc)
+int launch_preprocess_backward(const GsbBackwardRequest& req, const GeomState& g, const float* acc)
 {
 	const GsbScene* s = req.scene; const GsbCamera* cam = req.cam; const GsbRawParams* raw = req.raw;
 	BwdArgs a{};
@@ -645,7 +645,7 @@ int launch_preprocess_backward(const BackwardRequest& req, const GeomState& g, c
 	a.shs = s->shs; a.colors_precomp = s->colors_precomp; a.degrees = s->degrees; a.radii = req.radii;
 	a.view = cam->viewmatrix; a.proj = cam->projmatrix; a.campos = cam->campos;
 	a.quant = s->quant != nullptr; if (s->quant) a.q = *s->quant;
-	a.g = g; a.acc = acc; a.out = *req.grads; a.cam_rows = req.want_cam() ? reinterpret_cast<float*>(req.cam_workspace) : nullptr;
+	a.g = g; a.acc = acc; a.out = *req.grads; a.cam_rows = want_cam(req) ? reinterpret_cast<float*>(req.camera_workspace) : nullptr;
 	if (raw)
 	{
 		a.M = raw->features_dc && !s->colors_precomp ? 1 + raw->C : 0;
@@ -658,16 +658,17 @@ int launch_preprocess_backward(const BackwardRequest& req, const GeomState& g, c
 	}
 	const int grid = preprocess_backward_grid(s->P);
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * a.M + 1) + 32 * 6) * sizeof(float);
-	ProfScope prof(K_PREPROCESS_BWD, req.stream);
+	const cudaStream_t stream = stream_of(req);
+	ProfScope prof(K_PREPROCESS_BWD, stream);
 	const InputMode in = a.quant ? IN_QUANT : (raw ? IN_RAW : IN_ACTIVATED);
 	return dispatch([&](auto in, auto accumulate, auto maps, auto cam_grad, auto aa) -> int {
 		auto kernel = preprocess_backward_kernel<in, accumulate, maps, cam_grad, aa>;
 		if (int e = ensure_dyn_smem((const void*)kernel, 160 * 1024)) return e;
-		kernel<<<grid, 256, smem, req.stream>>>(a);
+		kernel<<<grid, 256, smem, stream>>>(a);
 		GSB_LAUNCHED();
 		GSB_CUDA_OK(cudaGetLastError());
 		return GSB_OK;
-	}, in, req.grads->accumulate != 0, req.dL_dinvdepth != nullptr, a.cam_rows != nullptr, req.aa);
+	}, in, req.grads->accumulate != 0, req.dL_dinvdepth != nullptr, a.cam_rows != nullptr, req.antialiasing != 0);
 }
 
 } // namespace gsb

@@ -19,7 +19,7 @@
 //      8-bit LSD radix sort in shared memory (tile_sort_kernel); beyond 8192 instances a single-CTA global-memory radix sort.
 //      The large classes are launched only when non-empty (their sizes ride the R read-back).
 //   Steps 3 and the small-tile part of 4 are launched SPECULATIVELY, before the host knows this frame's instance count
-//   (gsb_api.cu forward_impl): they compare the device-side count with the capacity they were given and do nothing if it is larger.
+//   (gsb_api.cu gsb_forward): they compare the device-side count with the capacity they were given and do nothing if it is larger.
 // The global stable sort by (tile, depth) with ties in emission order (ascending Gaussian id) is exactly "per tile, sort
 // by (depth bits, id)": a Gaussian appears at most once per tile, so the composites are unique and the order is total.
 // When the tile histogram does not fit in shared memory (> 160 KB, i.e. beyond ~8K images) counting and scattering fall
@@ -618,7 +618,7 @@ static bool scatter_prefill()
 
 // Scatter + the per-tile sort classes that are launched unconditionally.  SPECULATIVE: `cap` is the instance capacity the
 // binning blob was carved for; every kernel here compares the device-side instance count with it and exits when it does not
-// fit (forward_impl then repeats the call with the true count).
+// fit (gsb_forward then repeats the call with the true count).
 int launch_scatter_sort(const GeomState& g, const BinningState& b, const ImageState& img, const BinPlan& plan, int P, long long cap, int W, int H,
 	cudaStream_t stream)
 {

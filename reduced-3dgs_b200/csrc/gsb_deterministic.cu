@@ -120,10 +120,10 @@ __global__ void __launch_bounds__(256) det_gather_kernel(int P, int ns, const ui
 }
 
 // scan -> deterministic render backward -> gather: writes all 12 floats of every Gaussian's accumulator.
-int launch_render_backward_deterministic(const BackwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g,
+int launch_render_backward_deterministic(const GsbBackwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g,
 	float* acc)
 {
-	const int P = req.scene->P; const long long R = req.R; const cudaStream_t stream = req.stream;
+	const int P = req.scene->P; const long long R = req.num_rendered; const cudaStream_t stream = stream_of(req);
 	if (R == 0)
 	{
 		// nothing rendered: every rect is empty and every gradient zero

@@ -419,7 +419,7 @@ int launch_debug_dequant(const GsbQuant* q, int P, float* scales, float* rots, c
 	return GSB_OK;
 }
 
-int launch_preprocess(const ForwardRequest& req, const GeomState& g, const ImageState& img, const BinPlan& plan)
+int launch_preprocess(const GsbForwardRequest& req, const GeomState& g, const ImageState& img, const BinPlan& plan)
 {
 	const GsbScene* s = req.scene; const GsbCamera* cam = req.cam; const GsbRawParams* raw = req.raw;
 	PreArgs a{};
@@ -469,12 +469,12 @@ int launch_preprocess(const ForwardRequest& req, const GeomState& g, const Image
 	return dispatch([&](auto in, auto aa) -> int {
 		auto kernel = preprocess_kernel<in, aa>;
 		if (int e = ensure_dyn_smem((const void*)kernel, 220 * 1024)) return e;
-		ProfScope prof(K_PREPROCESS, req.stream);
-		kernel<<<grid, threads, smem, req.stream>>>(a);
+		ProfScope prof(K_PREPROCESS, stream_of(req));
+		kernel<<<grid, threads, smem, stream_of(req)>>>(a);
 		GSB_LAUNCHED();
 		GSB_CUDA_OK(cudaGetLastError());
 		return GSB_OK;
-	}, in, req.aa);
+	}, in, req.antialiasing != 0);
 }
 
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t stream)

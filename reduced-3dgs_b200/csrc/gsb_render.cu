@@ -647,19 +647,19 @@ int launch_stats_fixed_to_float(int P, const unsigned long long* fixed, float* o
 	return GSB_OK;
 }
 
-int launch_render_forward(const ForwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g)
+int launch_render_forward(const GsbForwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g)
 {
 	const int W = req.cam->width, H = req.cam->height;
 	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
-	const bool fixed = req.touched_pixels && req.transmittance_fixed;
-	const bool stats = fixed || (req.touched_pixels && req.transmittance);
+	const bool stats = statistics(req), fixed = stats_fixed(req);
 	const bool maps = !stats && req.out_invdepth && req.out_alpha;
-	float* const transmittance = fixed ? reinterpret_cast<float*>(req.transmittance_fixed) : req.transmittance;
-	ProfScope prof(K_RENDER_FWD, req.stream);
+	float* const transmittance = fixed ? reinterpret_cast<float*>(transmittance_fixed(req)) : req.transmittance_sum;
+	const cudaStream_t stream = stream_of(req);
+	ProfScope prof(K_RENDER_FWD, stream);
 	return dispatch([&](auto stats, auto maps, auto fixed) -> int {
 		// four variants exist: <F,F>, <F,T>, <T,F> and <T,F,T> (statistics go without maps; fixed point only with statistics)
 		if constexpr (!(stats && maps) && (stats || !fixed))
-			render_forward_kernel<stats, maps, fixed><<<grid, 256, 0, req.stream>>>(img.ranges, b.point_list, W, H, g.rec,
+			render_forward_kernel<stats, maps, fixed><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec,
 				req.cam->background, img.final_T, img.n_contrib, req.out_color, img.tile_max_contrib, stats ? req.touched_pixels : nullptr,
 				stats ? transmittance : nullptr, maps ? req.out_invdepth : nullptr, maps ? req.out_alpha : nullptr);
 		GSB_LAUNCHED();
@@ -668,12 +668,12 @@ int launch_render_forward(const ForwardRequest& req, const ImageState& img, cons
 	}, stats, maps, fixed);
 }
 
-int launch_render_backward(const BackwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g, float* acc,
+int launch_render_backward(const GsbBackwardRequest& req, const ImageState& img, const BinningState& b, const GeomState& g, float* acc,
 	float* parts, const uint32_t* slot_offset)
 {
 	const int W = req.cam->width, H = req.cam->height;
 	const dim3 grid((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y);
-	const cudaStream_t stream = req.stream;
+	const cudaStream_t stream = stream_of(req);
 	return dispatch([&](auto maps, auto det, auto abs) -> int {
 		constexpr int ns = abs ? DET_NS_ABS : DET_NS(maps);
 		const size_t smem = sizeof(BwdSmem<maps ? 4 : 3>) + (det ? size_t(8) * BWD_BATCH * ns * sizeof(float) : 0);
@@ -683,18 +683,18 @@ int launch_render_backward(const BackwardRequest& req, const ImageState& img, co
 		{
 			// instances behind a tile's last contributor (and tiles with none) are never visited: their slots must read as zero
 			ProfScope prof(K_DET_CLEAR, stream);
-			GSB_CUDA_OK(cudaMemsetAsync(parts, 0, size_t(req.R) * ns * sizeof(float), stream));
+			GSB_CUDA_OK(cudaMemsetAsync(parts, 0, size_t(req.num_rendered) * ns * sizeof(float), stream));
 		}
 		ProfScope prof(K_RENDER_BWD, stream);
 		// the per-Gaussian accumulator the kernel reduces into (12 floats per Gaussian, inside the geometry blob)
 		if (!det) GSB_CUDA_OK(cudaMemsetAsync(acc, 0, size_t(req.scene->P) * 48, stream));
 		kernel<<<grid, 256, smem, stream>>>(img.ranges, b.point_list, W, H, g.rec, req.cam->background,
 			img.final_T, img.n_contrib, img.tile_max_contrib, req.dL_dout_color, det ? nullptr : acc, req.dL_dinvdepth, req.dL_dalpha,
-			parts, slot_offset, det ? g.rect : nullptr, det ? (unsigned long long)req.R : 0ull);
+			parts, slot_offset, det ? g.rect : nullptr, det ? (unsigned long long)req.num_rendered : 0ull);
 		GSB_LAUNCHED();
 		GSB_CUDA_OK(cudaGetLastError());
 		return GSB_OK;
-	}, req.dL_dinvdepth || req.dL_dalpha, req.deterministic, req.dL_dmeans2D_abs != nullptr);
+	}, req.dL_dinvdepth || req.dL_dalpha, req.deterministic != 0, req.dL_dmeans2D_abs != nullptr);
 }
 
 // dL_dmeans2D_abs [P,3] = (0.5 W slot 10, 0.5 H slot 11, 0): the constant factors of backward.cu:583-589, applied as the preprocess
@@ -711,12 +711,13 @@ __global__ void __launch_bounds__(256) absgrad_finish_kernel(int P, const int32_
 	out[3 * (size_t)i + 2] = 0.0f;
 }
 
-int launch_absgrad_finish(const BackwardRequest& req, const float* acc)
+int launch_absgrad_finish(const GsbBackwardRequest& req, const float* acc)
 {
 	const int P = req.scene->P;
 	if (P <= 0) return GSB_OK;
-	ProfScope prof(K_ABSGRAD_FINISH, req.stream);
-	absgrad_finish_kernel<<<(P + 255) / 256, 256, 0, req.stream>>>(P, req.radii, acc, 0.5f * req.cam->width, 0.5f * req.cam->height,
+	const cudaStream_t stream = stream_of(req);
+	ProfScope prof(K_ABSGRAD_FINISH, stream);
+	absgrad_finish_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, req.radii, acc, 0.5f * req.cam->width, 0.5f * req.cam->height,
 		req.dL_dmeans2D_abs);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());

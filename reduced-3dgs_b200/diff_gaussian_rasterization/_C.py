@@ -5,21 +5,20 @@ behaviour as rasterize_points.h:18-93; tensors in, torch.Tensors out.
 Build-defined extensions (keyword-only, SURVEY §8(b)): `prune_mask` (u8/bool [P], 1 = pruned), `quant`
 (a gs_b200.synth.QuantScene-like object with u8 id planes + [20,256] centres) and `debug_out` (dict that
 receives the forward intermediates in the reference's GeometryState layouts).  `return_maps` (forward) also renders the
-inverse-depth and alpha maps in the same pass (gsb_forward_maps); `dL_dinvdepth` / `dL_dalpha` (backward) take their gradients.
+inverse-depth and alpha maps in the same pass; `dL_dinvdepth` / `dL_dalpha` (backward) take their gradients.
 `camera_grads` (backward) also returns the gradients w.r.t. viewmatrix, projmatrix and campos.  `antialiasing` (forward and
-backward, the same value for both) scales each Gaussian's opacity so that the 0.3 px^2 dilation no longer inflates sub-pixel splats
-(gsb_forward_antialiased).  `raw` (forward and backward) takes the model's leaf parameters (features_dc, features_rest, scaling,
-rotation) in place of sh, scales and rotations, and applies exp / F.normalize / the SH concatenation inside the kernels
-(gsb_forward_raw).  `deterministic` (backward) sums the per-Gaussian gradients in a fixed order: the same bytes on every run.
-`calculate_colours_variance` and `kmeans_cuda` take the same keyword (None: torch's deterministic-algorithms flag) for their
-statistics and centre sums (gsb_forward_statistics_deterministic, gsb_kmeans_deterministic).  `features` (forward, also of the
-variable-SH entry point) composites a [P, F] fp32 tensor of per-Gaussian features over the pairs of the colour image, with
-background 0, and appends the [F, H, W] image to the outputs (gsb_forward_features); the backward's `features` and
-`dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F].  `absgrad_out` (backward) takes a [P, 3] fp32 tensor
-that receives the absolute screen-space gradient.
+backward, the same value for both) scales each Gaussian's opacity so that the 0.3 px^2 dilation no longer inflates sub-pixel splats.
+`raw` (forward and backward) takes the model's leaf parameters (features_dc, features_rest, scaling, rotation) in place of sh,
+scales and rotations, and applies exp / F.normalize / the SH concatenation inside the kernels.  `deterministic` (backward) sums
+the per-Gaussian gradients in a fixed order: the same bytes on every run.  `calculate_colours_variance` and `kmeans_cuda` take the
+same keyword (None: torch's deterministic-algorithms flag) for their statistics and centre sums (the forward request's
+`deterministic`, gsb_kmeans_deterministic).  `features` (forward, also of the variable-SH entry point) composites a [P, F] fp32
+tensor of per-Gaussian features over the pairs of the colour image, with background 0, and appends the [F, H, W] image to the
+outputs; the backward's `features` and `dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F].
+`absgrad_out` (backward) takes a [P, 3] fp32 tensor that receives the absolute screen-space gradient.
 
-The backward makes one library call whatever its keywords: gsb_backward_absgrad with `absgrad_out`, else gsb_backward_features,
-which without features is the plain backward, or the deterministic one when given its workspace.
+Each keyword is one field of the library's request (GsbForwardRequest / GsbBackwardRequest): the forward and the backward make one
+library call, gsb_forward / gsb_backward, whatever their keywords.
 """
 from __future__ import annotations
 
@@ -29,8 +28,8 @@ import math
 import torch
 
 from gs_b200 import lib as _lib
-from gs_b200.lib import (GsbCamera, GsbDebug, GsbFeatures, GsbGrads, GsbQuant, GsbRawGrads, GsbRawParams, GsbScene, BlobAllocator, f32,
-                         on_device, ptr)
+from gs_b200.lib import (GsbBackwardRequest, GsbCamera, GsbDebug, GsbFeatures, GsbForwardRequest, GsbGrads, GsbQuant, GsbRawGrads,
+                         GsbRawParams, GsbScene, BlobAllocator, f32, on_device, ptr)
 
 RAW_REST_COEFFS = (0, 3, 8, 15)     # _features_rest widths of max SH degree 0..3
 
@@ -235,29 +234,27 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
             dbg = GsbDebug(*[ptr(d[k]) for k in ("depths", "means2D", "cov3D", "conic_opacity", "rgb", "tiles_touched", "clamped")])
             dbg_ptr = C.pointer(dbg)
         R = C.c_int64(0)
-        head = (C.byref(scene), C.byref(cam), cbs["geom"], None, cbs["binning"], None, cbs["image"], None, out_color.data_ptr(),
-                ptr(radii), C.byref(R))
-        map_ptrs = (maps[0].data_ptr(), maps[1].data_ptr()) if maps else (None, None)
-        stream = _lib.current_stream(device)
+        req = GsbForwardRequest(scene=C.pointer(scene), cam=C.pointer(cam), geom_alloc=cbs["geom"], binning_alloc=cbs["binning"],
+                                image_alloc=cbs["image"], out_color=out_color.data_ptr(), radii=ptr(radii), num_rendered=C.pointer(R),
+                                debug=dbg_ptr, antialiasing=int(bool(antialiasing)), stream=_lib.current_stream(device))
+        if maps is not None:
+            req.out_invdepth, req.out_alpha = maps[0].data_ptr(), maps[1].data_ptr()
         if raw_s is not None:
-            st = L.gsb_forward_raw(*head, dbg_ptr, *map_ptrs, C.byref(raw_s), int(bool(antialiasing)), stream)
-        elif statistics is not None and statistics_workspace is not None:
-            st = L.gsb_forward_statistics_deterministic(*head, ptr(statistics[0]), ptr(statistics[1]), statistics_workspace.data_ptr(), stream)
-        elif statistics is not None:                             # (touched_pixels int32 [P,1], transmittance_sum f32 [P,1]) to fill
-            st = L.gsb_forward_statistics(*head, ptr(statistics[0]), ptr(statistics[1]), stream)
-        elif antialiasing or maps is not None:
-            st = (L.gsb_forward_antialiased if antialiasing else L.gsb_forward_maps)(*head, dbg_ptr, *map_ptrs, stream)
-        else:
-            st = L.gsb_forward(*head, dbg_ptr, stream)
-        geomB, binB, imgB = blobs.take("geom"), blobs.take("binning"), blobs.take("image")
-        _lib.check(st)
+            req.raw = C.pointer(raw_s)
+        if statistics is not None:                               # (touched_pixels int32 [P,1], transmittance_sum f32 [P,1]) to fill
+            req.touched_pixels, req.transmittance_sum = ptr(statistics[0]), ptr(statistics[1])
+            if statistics_workspace is not None:
+                req.deterministic, req.workspace = 1, statistics_workspace.data_ptr()
         feat_img = ()
         if features is not None:
-            # the feature channels, composited from the blobs this forward left behind
+            # the feature channels, composited from the blobs this forward leaves behind
             feats = f32(features, device)
             feat_img = (torch.empty((F, H, W), dtype=torch.float32, device=device),)
             fs = GsbFeatures(F, ptr(feats), feat_img[0].data_ptr(), None, None)
-            _lib.check(L.gsb_forward_features(ptr(geomB), P, ptr(binB), int(R.value), ptr(imgB), W, H, C.byref(fs), stream))
+            req.features = C.pointer(fs)
+        st = L.gsb_forward(C.byref(req))
+        geomB, binB, imgB = blobs.take("geom"), blobs.take("binning"), blobs.take("image")
+        _lib.check(st)
         if debug:
             torch.cuda.synchronize(device)                      # reference CHECK_CUDA(debug) semantics, auxiliary.h:161-168
     if maps is not None:
@@ -270,13 +267,13 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
                         *, prune_mask=None, quant=None, debug_out=None, return_maps=False, antialiasing=False, raw=None, features=None):
     """rasterize_points.h:43-63 RasterizeGaussiansCUDA -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer).
     `return_maps`: -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer, invdepth [1,H,W], alpha [1,H,W]) with
-    invdepth = sum (1/depth) * alpha * T over the pairs that composite the colour and alpha = 1 - final_T (gsb_forward_maps).
-    `antialiasing`: opacity-compensated 2D filter (gsb_forward_antialiased); its buffers need the backward's `antialiasing=True`.
+    invdepth = sum (1/depth) * alpha * T over the pairs that composite the colour and alpha = 1 - final_T.
+    `antialiasing`: opacity-compensated 2D filter; its buffers need the backward's `antialiasing=True`.
     `raw`: (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]), the model's leaf parameters, with sh, scales
-    and rotations empty; the kernels read them in place and activate them (gsb_forward_raw).  With colors, features_dc and
+    and rotations empty; the kernels read them in place and activate them.  With colors, features_dc and
     features_rest are None.  The same output bits as the activated call on cat(dc, rest), exp(scaling), F.normalize(rotation).
     `features`: [P, F] fp32 on the device, 1 <= F <= 256; the tuple ends with the [F, H, W] feature image, each channel composited
-    like a colour channel with background 0 (gsb_forward_features).  Every other output is the call's without it."""
+    like a colour channel with background 0.  Every other output is the call's without it."""
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                     projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
                     None, prune_mask, quant, debug_out, return_maps=return_maps, antialiasing=antialiasing, raw=raw, features=features)
@@ -382,11 +379,14 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         g = GsbGrads(*[ptr(t) for t in (outs[:8] if raw is None else outs[:4] + [None] * 4)], ptr(conic),
                      1 if accumulate_into is not None else 0, ptr(view_means2D))
         radii = radii.to(device=device, dtype=torch.int32).contiguous()
-        head = (C.byref(scene), C.byref(cam), int(R), ptr(radii), ptr(geomBuffer), ptr(binningBuffer), ptr(imageBuffer), ptr(dL),
-                C.byref(g), ptr(dmaps[0]), ptr(dmaps[1]), float(lambda_sh_sparsity),
-                *([t.data_ptr() for t in cam_out] if camera_grads else [None] * 4))
-        stream = _lib.current_stream(device)
-        dfeat, fs = (), None
+        req = GsbBackwardRequest(scene=C.pointer(scene), cam=C.pointer(cam), num_rendered=int(R), radii=ptr(radii),
+                                 geom_blob=ptr(geomBuffer), binning_blob=ptr(binningBuffer), image_blob=ptr(imageBuffer),
+                                 dL_dout_color=ptr(dL), grads=C.pointer(g), dL_dinvdepth=ptr(dmaps[0]), dL_dalpha=ptr(dmaps[1]),
+                                 lambda_sh_sparsity=float(lambda_sh_sparsity), antialiasing=int(bool(antialiasing)),
+                                 dL_dmeans2D_abs=ptr(absgrad_out), stream=_lib.current_stream(device))
+        if camera_grads:
+            req.dL_dviewmatrix, req.dL_dprojmatrix, req.dL_dcampos, req.camera_workspace = [t.data_ptr() for t in cam_out]
+        dfeat = ()
         if features is not None:
             dLf = f32(dL_dfeatures_out, device)
             if dLf is None or dLf.numel() != feat_F * H * W:
@@ -395,19 +395,16 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             keep += [dLf, feats]
             dfeat = (torch.empty((P, feat_F), dtype=torch.float32, device=device),)
             fs = GsbFeatures(feat_F, ptr(feats), None, dLf.data_ptr(), ptr(dfeat[0]))
-        rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]]) if raw is not None else None
-        raw_args = (C.byref(raw_s) if raw is not None else None, C.byref(rg) if rg is not None else None, int(bool(antialiasing)))
-        det_ws = None
+            req.features = C.pointer(fs)
+        if raw is not None:
+            rg = GsbRawGrads(*[ptr(t) for t in outs[5:9]])
+            req.raw, req.raw_grads = C.pointer(raw_s), C.pointer(rg)
         if deterministic:
             # per-instance partial slots, from the caching allocator on the current stream (freed in stream order after the call)
             ws_bytes = L.gsb_absgrad_deterministic_workspace_bytes if absgrad_out is not None else L.gsb_deterministic_workspace_bytes
             det_ws = torch.empty(int(ws_bytes(P, int(R))), dtype=torch.uint8, device=device)
-        if absgrad_out is not None:
-            st = L.gsb_backward_absgrad(*head, *raw_args, ptr(det_ws), ptr(absgrad_out), stream)
-        else:
-            # without features this is gsb_backward_deterministic given det_ws, else the plain backward (with NULL map and camera
-            # pointers exactly gsb_backward / gsb_backward_maps)
-            st = L.gsb_backward_features(*head, *raw_args, ptr(det_ws), C.byref(fs) if fs is not None else None, stream)
+            req.deterministic, req.det_workspace = 1, ptr(det_ws)
+        st = L.gsb_backward(C.byref(req))
         _lib.check(st)
         if debug:
             torch.cuda.synchronize(device)
@@ -419,9 +416,9 @@ def calculate_colours_variance(cam_positions, means3D, opacity, scales, rotation
                                tan_fovys, image_height, image_width, sh, degrees, max_sh_deg, *, deterministic=None):
     """reduced_3dgs.h:28-43 Reduced3DGS::calculateColourVariance (reduced_3dgs.cu:41-203) ->
     (average colour distance to each lower SH truncation [P, max_sh_deg], weighted colour variance [P,1,3], weighted mean colour [P,1,3]).
-    Per camera: one forward with the visibility statistics on (gsb_forward_statistics) + one fused statistics kernel
+    Per camera: one forward with the visibility statistics on + one fused statistics kernel
     (gsb_sh_statistics_update) in place of the reference's ~30 ATen ops; the camera parameters are read back once, not per camera.
-    `deterministic`: sum the transmittances in 64-bit fixed point (gsb_forward_statistics_deterministic), the same bytes on every
+    `deterministic`: sum the transmittances in 64-bit fixed point (the forward request's `deterministic`), the same bytes on every
     run; None follows torch.are_deterministic_algorithms_enabled() at the call, an explicit bool wins."""
     det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
     if means3D.ndimension() != 2 or means3D.size(1) != 3:

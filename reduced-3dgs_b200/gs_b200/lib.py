@@ -67,6 +67,26 @@ class GsbFeatures(C.Structure):
 FEATURES_MAX = 256             # GSB_FEATURES_MAX
 
 
+class GsbForwardRequest(C.Structure):
+    _fields_ = [("scene", C.POINTER(GsbScene)), ("cam", C.POINTER(GsbCamera)), ("geom_alloc", ALLOC_FN), ("geom_user", C.c_void_p),
+                ("binning_alloc", ALLOC_FN), ("binning_user", C.c_void_p), ("image_alloc", ALLOC_FN), ("image_user", C.c_void_p),
+                ("out_color", C.c_void_p), ("radii", C.c_void_p), ("num_rendered", C.POINTER(C.c_int64)),
+                ("debug", C.POINTER(GsbDebug)), ("out_invdepth", C.c_void_p), ("out_alpha", C.c_void_p), ("antialiasing", C.c_int32),
+                ("raw", C.POINTER(GsbRawParams)), ("touched_pixels", C.c_void_p), ("transmittance_sum", C.c_void_p),
+                ("deterministic", C.c_int32), ("workspace", C.c_void_p), ("features", C.POINTER(GsbFeatures)), ("stream", C.c_void_p)]
+
+
+class GsbBackwardRequest(C.Structure):
+    _fields_ = [("scene", C.POINTER(GsbScene)), ("cam", C.POINTER(GsbCamera)), ("num_rendered", C.c_int64), ("radii", C.c_void_p),
+                ("geom_blob", C.c_void_p), ("binning_blob", C.c_void_p), ("image_blob", C.c_void_p), ("dL_dout_color", C.c_void_p),
+                ("grads", C.POINTER(GsbGrads)), ("dL_dinvdepth", C.c_void_p), ("dL_dalpha", C.c_void_p),
+                ("lambda_sh_sparsity", C.c_float), ("dL_dviewmatrix", C.c_void_p), ("dL_dprojmatrix", C.c_void_p),
+                ("dL_dcampos", C.c_void_p), ("camera_workspace", C.c_void_p), ("antialiasing", C.c_int32),
+                ("raw", C.POINTER(GsbRawParams)), ("raw_grads", C.POINTER(GsbRawGrads)), ("deterministic", C.c_int32),
+                ("det_workspace", C.c_void_p), ("features", C.POINTER(GsbFeatures)), ("dL_dmeans2D_abs", C.c_void_p),
+                ("stream", C.c_void_p)]
+
+
 class GsbAdamTensor(C.Structure):
     _fields_ = [("param", C.c_void_p), ("grad", C.c_void_p), ("exp_avg", C.c_void_p), ("exp_avg_sq", C.c_void_p),
                 ("numel", C.c_int64), ("row_width", C.c_int32), ("sh_offset", C.c_int32), ("one_minus_beta1", C.c_float),
@@ -130,21 +150,9 @@ def lib():
         L.gsb_last_error.restype = C.c_char_p
         L.gsb_version.restype = C.c_char_p
         L.gsb_forward.restype = C.c_int
-        L.gsb_forward.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p,
-                                  ALLOC_FN, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
-                                  C.POINTER(GsbDebug), C.c_void_p]
-        L.gsb_forward_maps.restype = C.c_int
-        L.gsb_forward_maps.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p,
-                                       ALLOC_FN, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
-                                       C.POINTER(GsbDebug), C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_forward_statistics.restype = C.c_int
-        L.gsb_forward_statistics.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), ALLOC_FN, C.c_void_p, ALLOC_FN, C.c_void_p,
-                                             ALLOC_FN, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64),
-                                             C.c_void_p, C.c_void_p, C.c_void_p]
+        L.gsb_forward.argtypes = [C.POINTER(GsbForwardRequest)]
         L.gsb_statistics_workspace_bytes.restype = C.c_size_t
         L.gsb_statistics_workspace_bytes.argtypes = [C.c_int32]
-        L.gsb_forward_statistics_deterministic.restype = C.c_int
-        L.gsb_forward_statistics_deterministic.argtypes = L.gsb_forward_statistics.argtypes[:-1] + [C.c_void_p, C.c_void_p]
         L.gsb_sh_statistics_update.restype = C.c_int
         L.gsb_sh_statistics_update.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 13
         L.gsb_min_projected_pixel_size.restype = C.c_int
@@ -177,39 +185,13 @@ def lib():
         L.gsb_l1_ssim_backward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_float, C.c_void_p,
                                            C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_backward.restype = C.c_int
-        L.gsb_backward.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                   C.c_void_p, C.c_void_p, C.POINTER(GsbGrads), C.c_float, C.c_void_p]
-        L.gsb_backward_maps.restype = C.c_int
-        L.gsb_backward_maps.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                        C.c_void_p, C.c_void_p, C.POINTER(GsbGrads), C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
+        L.gsb_backward.argtypes = [C.POINTER(GsbBackwardRequest)]
         L.gsb_camera_grad_workspace_bytes.restype = C.c_size_t
         L.gsb_camera_grad_workspace_bytes.argtypes = [C.c_int32]
-        L.gsb_backward_camera.restype = C.c_int
-        L.gsb_backward_camera.argtypes = [C.POINTER(GsbScene), C.POINTER(GsbCamera), C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
-                                          C.c_void_p, C.c_void_p, C.POINTER(GsbGrads), C.c_void_p, C.c_void_p, C.c_float, C.c_void_p,
-                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_forward_antialiased.restype = C.c_int
-        L.gsb_forward_antialiased.argtypes = L.gsb_forward_maps.argtypes
-        L.gsb_backward_antialiased.restype = C.c_int
-        L.gsb_backward_antialiased.argtypes = L.gsb_backward_camera.argtypes
-        L.gsb_forward_raw.restype = C.c_int
-        L.gsb_forward_raw.argtypes = L.gsb_forward_maps.argtypes[:-1] + [C.POINTER(GsbRawParams), C.c_int32, C.c_void_p]
-        L.gsb_backward_raw.restype = C.c_int
-        L.gsb_backward_raw.argtypes = L.gsb_backward_camera.argtypes[:-1] + [C.POINTER(GsbRawParams), C.POINTER(GsbRawGrads), C.c_int32,
-                                                                             C.c_void_p]
         L.gsb_deterministic_workspace_bytes.restype = C.c_size_t
         L.gsb_deterministic_workspace_bytes.argtypes = [C.c_int32, C.c_int64]
-        L.gsb_backward_deterministic.restype = C.c_int
-        L.gsb_backward_deterministic.argtypes = L.gsb_backward_raw.argtypes[:-1] + [C.c_void_p, C.c_void_p]
-        L.gsb_forward_features.restype = C.c_int
-        L.gsb_forward_features.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32,
-                                           C.POINTER(GsbFeatures), C.c_void_p]
-        L.gsb_backward_features.restype = C.c_int
-        L.gsb_backward_features.argtypes = L.gsb_backward_deterministic.argtypes[:-1] + [C.POINTER(GsbFeatures), C.c_void_p]
         L.gsb_absgrad_deterministic_workspace_bytes.restype = C.c_size_t
         L.gsb_absgrad_deterministic_workspace_bytes.argtypes = [C.c_int32, C.c_int64]
-        L.gsb_backward_absgrad.restype = C.c_int
-        L.gsb_backward_absgrad.argtypes = L.gsb_backward_deterministic.argtypes[:-1] + [C.c_void_p, C.c_void_p]
         L.gsb_mark_visible.restype = C.c_int
         L.gsb_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
         L.gsb_export_binning.restype = C.c_int
@@ -273,19 +255,16 @@ def profile_read() -> dict:
 
 EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", "gsb_binning_bytes", "gsb_forward", "gsb_backward",
                     "gsb_mark_visible", "gsb_export_binning", "gsb_export_image", "gsb_launch_count", "gsb_last_error",
-                    "gsb_version", "gsb_profile_enable", "gsb_profile_read", "gsb_debug_dequant", "gsb_forward_statistics",
+                    "gsb_version", "gsb_profile_enable", "gsb_profile_read", "gsb_debug_dequant",
                     "gsb_sh_statistics_update", "gsb_min_projected_pixel_size", "gsb_sphere_ellipsoid_intersection",
                     "gsb_min_redundancy_value", "gsb_kmeans_workspace_bytes", "gsb_kmeans", "gsb_l1_ssim_blocks",
                     "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn",
-                    "gsb_forward_maps", "gsb_backward_maps", "gsb_camera_grad_workspace_bytes", "gsb_backward_camera",
-                    "gsb_forward_antialiased", "gsb_backward_antialiased", "gsb_adam_step", "gsb_densify_stats",
+                    "gsb_camera_grad_workspace_bytes", "gsb_adam_step", "gsb_densify_stats",
                     "gsb_densify_workspace_bytes", "gsb_densify_split_std_offset", "gsb_densify_plan", "gsb_densify_emit",
-                    "gsb_forward_raw", "gsb_backward_raw", "gsb_deterministic_workspace_bytes", "gsb_backward_deterministic",
-                    "gsb_statistics_workspace_bytes", "gsb_forward_statistics_deterministic",
+                    "gsb_deterministic_workspace_bytes", "gsb_statistics_workspace_bytes",
                     "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic", "gsb_redundancy_workspace_bytes",
                     "gsb_redundancy_score", "gsb_mercy_workspace_bytes", "gsb_mercy_plan",
-                    "gsb_forward_features", "gsb_backward_features", "gsb_absgrad_deterministic_workspace_bytes",
-                    "gsb_backward_absgrad", "gsb_densify_stats_abs", "gsb_densify_plan_abs"]
+                    "gsb_absgrad_deterministic_workspace_bytes", "gsb_densify_stats_abs", "gsb_densify_plan_abs"]
 
 
 def check(status: int):

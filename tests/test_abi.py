@@ -45,6 +45,8 @@ def test_struct_layouts_match_header():
     assert lib.GsbScene.means3D.offset == 8 and lib.GsbScene.scale_modifier.offset == 8 + 8 * 8
     assert lib.GsbScene.band_count.offset == lib.GsbScene.scale_modifier.offset + 8
     assert ctypes.sizeof(lib.GsbScene) == lib.GsbScene.quant.offset + 8
+    assert ctypes.sizeof(lib.GsbForwardRequest) == 22 * 8 and lib.GsbForwardRequest.stream.offset == 21 * 8
+    assert ctypes.sizeof(lib.GsbBackwardRequest) == 24 * 8 and lib.GsbBackwardRequest.stream.offset == 23 * 8
 
 
 def test_sass_is_hopper_only():
@@ -62,9 +64,11 @@ def test_argument_validation_needs_no_gpu():
     scene.P, scene.M = -1, 0
     cb = lib.ALLOC_FN(lambda user, n: 0)
     R = C.c_int64(0)
-    st = L.gsb_forward(C.byref(scene), C.byref(cam), cb, None, cb, None, cb, None, None, None, C.byref(R), None, None)
+    fwd = lib.GsbForwardRequest(scene=C.pointer(scene), cam=C.pointer(cam), geom_alloc=cb, binning_alloc=cb, image_alloc=cb,
+                                num_rendered=C.pointer(R))
+    st = L.gsb_forward(C.byref(fwd))
     assert st < 0 and len(L.gsb_last_error()) > 0
-    st = L.gsb_backward(C.byref(scene), C.byref(cam), 0, None, None, None, None, None, None, 0.0, None)
+    st = L.gsb_backward(C.byref(lib.GsbBackwardRequest(scene=C.pointer(scene), cam=C.pointer(cam))))
     assert st < 0
     assert L.gsb_mark_visible(-1, None, None, None, None, None) < 0
     assert L.gsb_mark_visible(5, None, None, None, None, None) < 0
@@ -76,7 +80,7 @@ def test_argument_validation_needs_no_gpu():
     assert L.gsb_sh_statistics_update(10, 4, *([None] * 13)) < 0 and b"16" in L.gsb_last_error()      # needs the full SH layout
     assert L.gsb_l1_ssim_forward(None, None, 3, 8, 8, None, None, None) < 0
     assert L.gsb_l1_ssim_backward(None, None, 3, 8, 8, None, 1.0, None, 1.0, None, None, None) < 0
-    assert L.gsb_forward_statistics(None, None, cb, None, cb, None, cb, None, None, None, C.byref(R), None, None, None) < 0
+    assert L.gsb_forward(C.byref(lib.GsbForwardRequest(geom_alloc=cb, binning_alloc=cb, image_alloc=cb, num_rendered=C.pointer(R)))) < 0
     # size helpers are monotone and include the per-kind fixed parts
     assert L.gsb_kmeans_workspace_bytes(10 ** 6, 256) > 8 * 10 ** 6
     assert L.gsb_l1_ssim_blocks(3, 1080, 1920) == 3 * 68 * 120

@@ -1,5 +1,5 @@
-"""CPU: the absolute screen-space gradient (DESIGN.md §5m).  The new entry points (gsb_backward_absgrad, its workspace size,
-gsb_densify_stats_abs, gsb_densify_plan_abs) reject each bad argument before any CUDA call; the Python layer refuses what has no
+"""CPU: the absolute screen-space gradient (DESIGN.md §5m).  The backward request with dL_dmeans2D_abs, its workspace size,
+gsb_densify_stats_abs and gsb_densify_plan_abs reject each bad argument before any CUDA call; the Python layer refuses what has no
 absgrad form before anything runs and, against stand-in kernels, carries `absgrad` through both autograd ops and render() while
 leaving the calls without it exactly as they were; and the float64 restatement of the per-pair terms (absgrad64.py) sums, with
 signs, to the fp64 oracle's dL_dmeans2D on the backward-edge scenes, which pins it to the pairs and terms the oracle uses."""
@@ -15,7 +15,7 @@ import backward_edges as BE
 import stub_c
 from gs_b200 import lib
 
-NEW = ("gsb_backward_absgrad", "gsb_absgrad_deterministic_workspace_bytes", "gsb_densify_stats_abs", "gsb_densify_plan_abs")
+NEW = ("gsb_backward", "gsb_absgrad_deterministic_workspace_bytes", "gsb_densify_stats_abs", "gsb_densify_plan_abs")
 
 
 def test_symbols_exported():
@@ -34,32 +34,36 @@ def test_workspace_grows_and_adds_eight_bytes_per_instance():
     assert L.gsb_absgrad_deterministic_workspace_bytes(1000, 10) < L.gsb_absgrad_deterministic_workspace_bytes(100_000, 10)
 
 
-def _bwd(L, scene, R=5, grads=None, out=True, det_ws=None, raw=None, raw_grads=None, cam_out=None, workspace=None):
-    cam = lib.GsbCamera()
+def _bwd(L, scene, R=5, grads=None, out=True, det_ws=None, raw=None, raw_grads=None, cam_out=None, workspace=None, features=None):
     g = grads if grads is not None else lib.GsbGrads()
     buf = (C.c_float * 16)()
-    return L.gsb_backward_absgrad(scene, C.byref(cam), R, None, None, None, None, None, C.byref(g), None, None, 0.0, cam_out, None, None,
-                                  workspace, raw, raw_grads, 0, det_ws, C.addressof(buf) if out else None, None)
+    req = lib.GsbBackwardRequest(scene=scene, cam=C.pointer(lib.GsbCamera()), num_rendered=R, grads=C.pointer(g), dL_dviewmatrix=cam_out,
+                                 camera_workspace=workspace, raw=raw, raw_grads=raw_grads, deterministic=int(det_ws is not None),
+                                 det_workspace=det_ws, features=features, dL_dmeans2D_abs=C.addressof(buf) if out else None)
+    return L.gsb_backward(C.byref(req))
 
 
 def test_backward_absgrad_rejects_bad_arguments():
     L = lib.lib()
-    scene = C.byref(lib.GsbScene(P=10))
+    scene = C.pointer(lib.GsbScene(P=10))
     fbuf = (C.c_float * 16)()
-    for sc in (None, C.byref(lib.GsbScene(P=-1))):
+    for sc in (None, C.pointer(lib.GsbScene(P=-1))):
         assert _bwd(L, sc) == -1 and b"P < 0" in L.gsb_last_error()
-    assert _bwd(L, scene, out=False) == -1 and b"dL_dmeans2D_abs is NULL" in L.gsb_last_error()
+    feats = lib.GsbFeatures(4, C.addressof(fbuf), None, C.addressof(fbuf), C.addressof(fbuf))
+    assert _bwd(L, scene, features=C.pointer(feats)) == -1 and b"no feature form" in L.gsb_last_error()
     assert _bwd(L, scene, grads=lib.GsbGrads(accumulate=1)) == -1 and b"accumulate" in L.gsb_last_error()
     assert _bwd(L, scene, R=-1) == -1 and b"num_rendered < 0" in L.gsb_last_error()
     buf = (C.c_char * 256)()
     assert _bwd(L, scene, R=1 << 30, det_ws=C.addressof(buf)) == -4 and b"2^30" in L.gsb_last_error()
     assert _bwd(L, scene, cam_out=C.addressof(fbuf)) == -1 and b"workspace is NULL" in L.gsb_last_error()
-    assert _bwd(L, scene, raw_grads=C.byref(lib.GsbRawGrads())) == -1 and b"raw_grads given without raw" in L.gsb_last_error()
-    assert _bwd(L, scene, raw=C.byref(lib.GsbRawParams(C=4)), raw_grads=C.byref(lib.GsbRawGrads())) == -1
+    assert _bwd(L, scene, raw_grads=C.pointer(lib.GsbRawGrads())) == -1 and b"raw_grads given without raw" in L.gsb_last_error()
+    assert _bwd(L, scene, raw=C.pointer(lib.GsbRawParams(C=4)), raw_grads=C.pointer(lib.GsbRawGrads())) == -1
     assert b"C = 4" in L.gsb_last_error()
-    # valid absgrad arguments go on to the scene checks of the backward (an empty camera is refused there); P = 0 needs no output
+    # valid absgrad arguments go on to the scene checks of the backward (an empty camera is refused there), and so does a request
+    # without the output
     assert _bwd(L, scene) == -1 and b"image size" in L.gsb_last_error()
-    assert _bwd(L, C.byref(lib.GsbScene(P=0)), out=False) == -1 and b"image size" in L.gsb_last_error()
+    assert _bwd(L, C.pointer(lib.GsbScene(P=0)), out=False) == -1 and b"image size" in L.gsb_last_error()
+    assert _bwd(L, scene, out=False) == -1 and b"image size" in L.gsb_last_error()
 
 
 def test_densify_abs_entry_points_reject_bad_arguments():

@@ -1,4 +1,4 @@
-"""CPU: the anti-aliased entry points (gsb_forward_antialiased / gsb_backward_antialiased): exported, argument checks before any CUDA
+"""CPU: anti-aliased requests (the `antialiasing` field of GsbForwardRequest / GsbBackwardRequest): argument checks before any CUDA
 call, refusal of CPU tensors, and the plumbing of the `antialiasing` flag from GaussianRasterizationSettings and `pipe` to both
 kernels, checked against a stub of `_C` (no GPU, no kernel)."""
 import ctypes as C
@@ -12,51 +12,52 @@ from gs_b200 import lib
 
 def test_antialiased_symbols_are_exported():
     L = lib.lib()
-    for sym in ("gsb_forward_antialiased", "gsb_backward_antialiased"):
+    for sym in ("gsb_forward", "gsb_backward"):
         assert sym in lib.EXPORTED_SYMBOLS
         getattr(L, sym)
+    assert lib.GsbForwardRequest.antialiasing.size == lib.GsbBackwardRequest.antialiasing.size == 4
 
 
 def _fwd(L, scene, cam, invdepth=None, alpha=None):
-    R = C.c_int64(0)
-    return L.gsb_forward_antialiased(scene, cam, lib.ALLOC_FN(0), None, lib.ALLOC_FN(0), None, lib.ALLOC_FN(0), None, None, None,
-                                     C.byref(R), None, invdepth, alpha, None)
+    req = lib.GsbForwardRequest(scene=scene, cam=cam, num_rendered=C.pointer(C.c_int64(0)), out_invdepth=invdepth, out_alpha=alpha,
+                                antialiasing=1)
+    return L.gsb_forward(C.byref(req))
 
 
 def _bwd(L, scene, cam, view=None, proj=None, campos=None, ws=None):
-    g = lib.GsbGrads()
-    return L.gsb_backward_antialiased(scene, cam, 0, None, None, None, None, None, C.byref(g), None, None, 0.0, view, proj, campos, ws,
-                                      None)
+    req = lib.GsbBackwardRequest(scene=scene, cam=cam, grads=C.pointer(lib.GsbGrads()), dL_dviewmatrix=view, dL_dprojmatrix=proj,
+                                 dL_dcampos=campos, camera_workspace=ws, antialiasing=1)
+    return L.gsb_backward(C.byref(req))
 
 
 def test_forward_antialiased_rejects_bad_arguments():
     L = lib.lib()
     cam = lib.GsbCamera()
-    for scene in (None, C.byref(lib.GsbScene(P=-1))):
-        assert _fwd(L, scene, C.byref(cam)) == -1 and b"P < 0" in L.gsb_last_error()
+    for scene in (None, C.pointer(lib.GsbScene(P=-1))):
+        assert _fwd(L, scene, C.pointer(cam)) == -1 and b"P < 0" in L.gsb_last_error()
     # one map output without the other is refused before the scene / camera are looked at (here: an empty camera struct)
     buf = (C.c_float * 16)()
     for maps in ((C.addressof(buf), None), (None, C.addressof(buf))):
-        assert _fwd(L, C.byref(lib.GsbScene(P=10)), C.byref(cam), *maps) == -1
+        assert _fwd(L, C.pointer(lib.GsbScene(P=10)), C.pointer(cam), *maps) == -1
         assert b"both map outputs" in L.gsb_last_error()
     # both or neither: the call goes on to the usual scene / camera checks
     for maps in ((None, None), (C.addressof(buf), C.addressof(buf))):
-        assert _fwd(L, C.byref(lib.GsbScene(P=10)), C.byref(cam), *maps) == -1
+        assert _fwd(L, C.pointer(lib.GsbScene(P=10)), C.pointer(cam), *maps) == -1
         assert b"map outputs" not in L.gsb_last_error()
 
 
 def test_backward_antialiased_rejects_bad_arguments():
     L = lib.lib()
     cam = lib.GsbCamera()
-    for scene in (None, C.byref(lib.GsbScene(P=-1))):
-        assert _bwd(L, scene, C.byref(cam)) == -1 and b"P < 0" in L.gsb_last_error()
+    for scene in (None, C.pointer(lib.GsbScene(P=-1))):
+        assert _bwd(L, scene, C.pointer(cam)) == -1 and b"P < 0" in L.gsb_last_error()
     buf = (C.c_float * 16)()
     for k in range(3):
         outs = [None, None, None]
         outs[k] = C.addressof(buf)
-        assert _bwd(L, C.byref(lib.GsbScene(P=10)), C.byref(cam), *outs) == -1
+        assert _bwd(L, C.pointer(lib.GsbScene(P=10)), C.pointer(cam), *outs) == -1
         assert b"workspace" in L.gsb_last_error()
-    assert _bwd(L, C.byref(lib.GsbScene(P=10)), C.byref(cam)) == -1
+    assert _bwd(L, C.pointer(lib.GsbScene(P=10)), C.pointer(cam)) == -1
     assert b"workspace" not in L.gsb_last_error()
 
 

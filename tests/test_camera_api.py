@@ -1,4 +1,5 @@
-"""CPU: argument checks of gsb_backward_camera / gsb_camera_grad_workspace_bytes, the Python layer's refusal of CPU tensors with
+"""CPU: argument checks of the camera-gradient backward (gsb_backward's dL_dviewmatrix / dL_dprojmatrix / dL_dcampos) and
+gsb_camera_grad_workspace_bytes, the Python layer's refusal of CPU tensors with
 camera_grads, and the autograd plumbing of a learnable camera, checked against a stub of `_C` (no GPU, no kernel)."""
 import ctypes as C
 
@@ -10,25 +11,26 @@ from gs_b200 import lib
 
 
 def _call(L, scene, cam, view=None, proj=None, campos=None, ws=None):
-    g = lib.GsbGrads()
-    return L.gsb_backward_camera(scene, cam, 0, None, None, None, None, None, C.byref(g), None, None, 0.0, view, proj, campos, ws, None)
+    req = lib.GsbBackwardRequest(scene=scene, cam=cam, grads=C.pointer(lib.GsbGrads()), dL_dviewmatrix=view, dL_dprojmatrix=proj,
+                                 dL_dcampos=campos, camera_workspace=ws)
+    return L.gsb_backward(C.byref(req))
 
 
 def test_backward_camera_rejects_bad_arguments():
     L = lib.lib()
     cam = lib.GsbCamera()
-    for scene in (None, C.byref(lib.GsbScene(P=-1))):
-        assert _call(L, scene, C.byref(cam)) < 0 and len(L.gsb_last_error()) > 0
+    for scene in (None, C.pointer(lib.GsbScene(P=-1))):
+        assert _call(L, scene, C.pointer(cam)) < 0 and len(L.gsb_last_error()) > 0
     # a camera output without a workspace is refused before anything else is looked at (here: an empty camera struct)
     buf = (C.c_float * 16)()
     for k in range(3):
         outs = [None, None, None]
         outs[k] = C.addressof(buf)
         scene = lib.GsbScene(P=10)
-        assert _call(L, C.byref(scene), C.byref(cam), *outs) == -1
+        assert _call(L, C.pointer(scene), C.pointer(cam), *outs) == -1
         assert b"workspace" in L.gsb_last_error()
     # without any camera output the workspace is not needed: the call goes on to the usual scene / camera checks
-    assert _call(L, C.byref(lib.GsbScene(P=10)), C.byref(cam)) == -1
+    assert _call(L, C.pointer(lib.GsbScene(P=10)), C.pointer(cam)) == -1
     assert b"workspace" not in L.gsb_last_error()
 
 

@@ -1,4 +1,4 @@
-"""CPU: the deterministic backward's entry points (gsb_deterministic_workspace_bytes / gsb_backward_deterministic): exported,
+"""CPU: the deterministic backward (gsb_deterministic_workspace_bytes, gsb_backward's `deterministic` / `det_workspace`): exported,
 workspace size, argument checks before any CUDA call, and the plumbing of GaussianRasterizationSettings' `deterministic` keyword
 and torch's deterministic-algorithms flag to `_C.rasterize_gaussians_backward`, checked against a stub of `_C` (no GPU)."""
 import ctypes as C
@@ -20,7 +20,7 @@ def torch_deterministic():
 
 def test_symbols_are_exported():
     L = lib.lib()
-    for sym in ("gsb_deterministic_workspace_bytes", "gsb_backward_deterministic"):
+    for sym in ("gsb_deterministic_workspace_bytes", "gsb_backward"):
         assert sym in lib.EXPORTED_SYMBOLS
         getattr(L, sym)
 
@@ -34,32 +34,33 @@ def test_workspace_size():
 
 
 def _bwd(L, scene, R=0, ws=None, det_ws=None, cam_out=(None, None, None), raw=None, raw_grads=None, grads=None):
-    cam = lib.GsbCamera()
     g = grads if grads is not None else lib.GsbGrads()
-    return L.gsb_backward_deterministic(scene, C.byref(cam), R, None, None, None, None, None, C.byref(g), None, None, 0.0, *cam_out, ws,
-                                        raw, raw_grads, 0, det_ws, None)
+    req = lib.GsbBackwardRequest(scene=scene, cam=C.pointer(lib.GsbCamera()), num_rendered=R, grads=C.pointer(g), camera_workspace=ws,
+                                 raw=raw, raw_grads=raw_grads, deterministic=1, det_workspace=det_ws)
+    req.dL_dviewmatrix, req.dL_dprojmatrix, req.dL_dcampos = cam_out
+    return L.gsb_backward(C.byref(req))
 
 
 def test_backward_deterministic_rejects_bad_arguments():
     L = lib.lib()
-    for scene in (None, C.byref(lib.GsbScene(P=-1))):
+    for scene in (None, C.pointer(lib.GsbScene(P=-1))):
         assert _bwd(L, scene) == -1 and b"P < 0" in L.gsb_last_error()
-    assert _bwd(L, C.byref(lib.GsbScene(P=10)), R=-1) == -1 and b"num_rendered < 0" in L.gsb_last_error()
-    assert _bwd(L, C.byref(lib.GsbScene(P=10)), R=1 << 30) == -4 and b"2^30" in L.gsb_last_error()
+    assert _bwd(L, C.pointer(lib.GsbScene(P=10)), R=-1) == -1 and b"num_rendered < 0" in L.gsb_last_error()
+    assert _bwd(L, C.pointer(lib.GsbScene(P=10)), R=1 << 30) == -4 and b"2^30" in L.gsb_last_error()
     # a NULL workspace is refused only when there is something to sum (P > 0 and R > 0)
-    assert _bwd(L, C.byref(lib.GsbScene(P=10)), R=5) == -1 and b"det_workspace is NULL" in L.gsb_last_error()
+    assert _bwd(L, C.pointer(lib.GsbScene(P=10)), R=5) == -1 and b"det_workspace is NULL" in L.gsb_last_error()
     buf = (C.c_char * 256)()
     for scene, R, ws in ((lib.GsbScene(P=10), 0, None), (lib.GsbScene(P=0), 5, None), (lib.GsbScene(P=10), 5, C.addressof(buf))):
-        assert _bwd(L, C.byref(scene), R=R, det_ws=ws) == -1            # goes on to the camera / scene checks (an empty camera)
+        assert _bwd(L, C.pointer(scene), R=R, det_ws=ws) == -1            # goes on to the camera / scene checks (an empty camera)
         assert b"det_workspace" not in L.gsb_last_error()
     fbuf = (C.c_float * 16)()
     for k in range(3):
         outs = [None, None, None]
         outs[k] = C.addressof(fbuf)
-        assert _bwd(L, C.byref(lib.GsbScene(P=10)), R=5, det_ws=C.addressof(buf), cam_out=outs) == -1
+        assert _bwd(L, C.pointer(lib.GsbScene(P=10)), R=5, det_ws=C.addressof(buf), cam_out=outs) == -1
         assert b"workspace is NULL" in L.gsb_last_error()
     rg = lib.GsbRawGrads()
-    assert _bwd(L, C.byref(lib.GsbScene(P=10)), R=5, det_ws=C.addressof(buf), raw_grads=C.byref(rg)) == -1
+    assert _bwd(L, C.pointer(lib.GsbScene(P=10)), R=5, det_ws=C.addressof(buf), raw_grads=C.pointer(rg)) == -1
     assert b"raw_grads given without raw" in L.gsb_last_error()
 
 
@@ -69,29 +70,29 @@ def test_backward_deterministic_applies_the_raw_checks():
     ws = C.addressof(buf)
     scene = lib.GsbScene(P=10)
     # C outside {0, 3, 8, 15}
-    assert _bwd(L, C.byref(scene), R=5, det_ws=ws, raw=C.byref(lib.GsbRawParams(C=4)), raw_grads=C.byref(lib.GsbRawGrads())) == -1
+    assert _bwd(L, C.pointer(scene), R=5, det_ws=ws, raw=C.pointer(lib.GsbRawParams(C=4)), raw_grads=C.pointer(lib.GsbRawGrads())) == -1
     assert b"C = 4" in L.gsb_last_error()
     # a scene field the raw parameters replace
     fbuf = (C.c_float * 16)()
     s2 = lib.GsbScene(P=10)
     s2.scales = C.addressof(fbuf)
-    assert _bwd(L, C.byref(s2), R=5, det_ws=ws, raw=C.byref(lib.GsbRawParams(C=3)), raw_grads=C.byref(lib.GsbRawGrads())) == -1
+    assert _bwd(L, C.pointer(s2), R=5, det_ws=ws, raw=C.pointer(lib.GsbRawParams(C=3)), raw_grads=C.pointer(lib.GsbRawGrads())) == -1
     assert b"must be NULL" in L.gsb_last_error()
     # raw without raw_grads
     full = lib.GsbRawParams(C.addressof(fbuf), C.addressof(fbuf), 3, C.addressof(fbuf), C.addressof(fbuf))
     s3 = lib.GsbScene(P=10)
     s3.degrees = C.addressof(fbuf)
-    assert _bwd(L, C.byref(s3), R=5, det_ws=ws, raw=C.byref(full)) == -1 and b"raw_grads are NULL" in L.gsb_last_error()
+    assert _bwd(L, C.pointer(s3), R=5, det_ws=ws, raw=C.pointer(full)) == -1 and b"raw_grads are NULL" in L.gsb_last_error()
     # grads->dL_dsh given next to raw_grads
     g = lib.GsbGrads()
     g.dL_dsh = C.addressof(fbuf)
-    assert _bwd(L, C.byref(s3), R=5, det_ws=ws, raw=C.byref(full), raw_grads=C.byref(lib.GsbRawGrads()), grads=g) == -1
+    assert _bwd(L, C.pointer(s3), R=5, det_ws=ws, raw=C.pointer(full), raw_grads=C.pointer(lib.GsbRawGrads()), grads=g) == -1
     assert b"raw_grads replaces them" in L.gsb_last_error()
     # dL_dfeatures_rest with C == 0
     rg = lib.GsbRawGrads()
     rg.dL_dfeatures_rest = C.addressof(fbuf)
     c0 = lib.GsbRawParams(C.addressof(fbuf), None, 0, C.addressof(fbuf), C.addressof(fbuf))
-    assert _bwd(L, C.byref(s3), R=5, det_ws=ws, raw=C.byref(c0), raw_grads=C.byref(rg)) == -1
+    assert _bwd(L, C.pointer(s3), R=5, det_ws=ws, raw=C.pointer(c0), raw_grads=C.pointer(rg)) == -1
     assert b"C == 0" in L.gsb_last_error()
 
 

@@ -1,4 +1,5 @@
-"""CPU: the deterministic SH-culling statistics and k-means (gsb_forward_statistics_deterministic, gsb_kmeans_deterministic):
+"""CPU: the deterministic SH-culling statistics and k-means (a statistics forward request with `deterministic`,
+gsb_kmeans_deterministic):
 exports, workspace sizes, every refused argument (checked before any CUDA call), the `deterministic` keyword of
 `_C.calculate_colours_variance` / `_C.kmeans_cuda` against a stub library, and the float32 restatement of the k-means summation
 order (oracle/kmeans_det_order.py) on hand-made cases."""
@@ -16,8 +17,7 @@ from gs_b200 import lib
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle"))
 import kmeans_det_order as kdo  # noqa: E402
 
-NEW_SYMBOLS = ("gsb_statistics_workspace_bytes", "gsb_forward_statistics_deterministic", "gsb_kmeans_deterministic_workspace_bytes",
-               "gsb_kmeans_deterministic")
+NEW_SYMBOLS = ("gsb_statistics_workspace_bytes", "gsb_forward", "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic")
 
 
 @pytest.fixture
@@ -47,28 +47,29 @@ def test_workspace_sizes():
 
 
 def _stats(L, scene, cam=None, outs=True, ws=None):
+    """A deterministic statistics forward; outs=False leaves out transmittance_sum (one statistics output without the other)."""
     buf = (C.c_float * 16)()
-    p = C.addressof(buf) if outs else None
-    R = C.c_int64(0)
+    p = C.addressof(buf)
     cam = cam if cam is not None else lib.GsbCamera()
-    return L.gsb_forward_statistics_deterministic(scene, C.byref(cam), lib.ALLOC_FN(0), None, lib.ALLOC_FN(0), None, lib.ALLOC_FN(0), None,
-                                                  p, p, C.byref(R), p, p, ws, None)
+    req = lib.GsbForwardRequest(scene=scene, cam=C.pointer(cam), out_color=p, radii=p, num_rendered=C.pointer(C.c_int64(0)),
+                                touched_pixels=p, transmittance_sum=p if outs else None, deterministic=1, workspace=ws)
+    return L.gsb_forward(C.byref(req))
 
 
 def test_statistics_deterministic_rejects_bad_arguments():
     L = lib.lib()
     ws = (C.c_char * 256)()
-    for scene in (None, C.byref(lib.GsbScene(P=-1))):
+    for scene in (None, C.pointer(lib.GsbScene(P=-1))):
         assert _stats(L, scene, ws=C.addressof(ws)) == -1 and b"P < 0" in L.gsb_last_error()
-    assert _stats(L, C.byref(lib.GsbScene(P=10)), outs=False, ws=C.addressof(ws)) == -1
+    assert _stats(L, C.pointer(lib.GsbScene(P=10)), outs=False, ws=C.addressof(ws)) == -1
     assert b"output pointers missing" in L.gsb_last_error()
-    assert _stats(L, C.byref(lib.GsbScene(P=10))) == -1 and b"workspace is NULL" in L.gsb_last_error()
+    assert _stats(L, C.pointer(lib.GsbScene(P=10))) == -1 and b"workspace is NULL" in L.gsb_last_error()
     # W * H = 2^28 is out of range (the check comes before any memory is touched), just below it goes on to the camera checks
     for W, H in ((1 << 14, 1 << 14), (1 << 28, 1), (1 << 15, 1 << 14)):
-        assert _stats(L, C.byref(lib.GsbScene(P=10)), cam=lib.GsbCamera(width=W, height=H), ws=C.addressof(ws)) == -4
+        assert _stats(L, C.pointer(lib.GsbScene(P=10)), cam=lib.GsbCamera(width=W, height=H), ws=C.addressof(ws)) == -4
         assert b"2^28" in L.gsb_last_error()
     for scene, wsp in ((lib.GsbScene(P=0), None), (lib.GsbScene(P=0), C.addressof(ws))):
-        assert _stats(L, C.byref(scene), cam=lib.GsbCamera(width=(1 << 14) - 1, height=1 << 14), ws=wsp) == -1
+        assert _stats(L, C.pointer(scene), cam=lib.GsbCamera(width=(1 << 14) - 1, height=1 << 14), ws=wsp) == -1
         assert b"camera tensors missing" in L.gsb_last_error()
 
 
@@ -123,6 +124,8 @@ def _canon(args, named):
         v = getattr(s, f)
         if isinstance(v, C._Pointer):
             return "non-null" if v else None
+        if isinstance(v, C._CFuncPtr):
+            return "callback"
         return p(v) if t is C.c_void_p and v else v
 
     out = []
@@ -162,15 +165,23 @@ def _colour_inputs(P=6, n_cams=2):
                 sh=r(P, 16, 3), degrees=torch.full((P, 1), 3, dtype=torch.int32), max_sh_deg=3)
 
 
-def _colour_calls(monkeypatch, **kw):
+def _colour_calls(monkeypatch, raw=False, **kw):
+    """The library calls of calculate_colours_variance, canonicalised; raw=True: the forward requests as the library received them."""
     x = _colour_inputs()
     with _stubbed(monkeypatch) as (_C, stub):
         _C.calculate_colours_variance(*x.values(), **kw)
+    if raw:
+        return [args[0]._obj for name, args in stub.calls if name == "gsb_forward"]
     named = {t.data_ptr(): k for k, t in x.items() if isinstance(t, torch.Tensor)}
     named.update({x["cam_positions"][i].data_ptr(): f"campos{i}" for i in range(2)})
     named.update({x["cam_viewmatrices"][i].data_ptr(): f"view{i}" for i in range(2)})
     named.update({x["cam_projmatrices"][i].data_ptr(): f"proj{i}" for i in range(2)})
     return [(name, _canon(args, named)) for name, args in stub.calls]
+
+
+def _deterministic(monkeypatch, **kw):
+    """The `deterministic` field of the first statistics forward request of calculate_colours_variance."""
+    return _colour_calls(monkeypatch, raw=True, **kw)[0].deterministic
 
 
 def _kmeans_calls(monkeypatch, **kw):
@@ -189,11 +200,14 @@ def _names(calls):
 def test_flag_off_keeps_the_old_calls(monkeypatch, torch_deterministic):
     torch.use_deterministic_algorithms(False)
     col = _colour_calls(monkeypatch)
-    assert _names(col) == ["gsb_forward_statistics", "gsb_sh_statistics_update"] * 2
+    assert _names(col) == ["gsb_forward", "gsb_sh_statistics_update"] * 2
     assert col == _colour_calls(monkeypatch, deterministic=False)
-    # the statistics forward's arguments: scene, camera, 3 x (callback, NULL), out_color, radii, &R, touched, tsum, stream
-    fwd = col[0][1]
-    assert len(fwd) == 14 and fwd[3] is None and fwd[-1] == 0
+    # the statistics forward's request: scene, camera, 3 x (callback, NULL), out_color, radii, &R, touched, tsum, stream 0, and
+    # no other option
+    fwd = dict(col[0][1][0])
+    assert len(col[0][1]) == 1 and fwd["geom_alloc"] == "callback" and fwd["geom_user"] is None and fwd["stream"] is None
+    assert all(fwd[k] is not None for k in ("scene", "cam", "out_color", "radii", "num_rendered", "touched_pixels", "transmittance_sum"))
+    assert all(not fwd[k] for k in ("debug", "out_invdepth", "out_alpha", "antialiasing", "raw", "deterministic", "workspace", "features"))
     km = _kmeans_calls(monkeypatch)
     assert _names(km) == ["gsb_kmeans_workspace_bytes", "gsb_kmeans"]
     assert km[0][1] == (100, 8)
@@ -204,14 +218,18 @@ def test_flag_off_keeps_the_old_calls(monkeypatch, torch_deterministic):
 def test_torch_flag_selects_the_deterministic_paths(monkeypatch, torch_deterministic):
     torch.use_deterministic_algorithms(True)
     col = _colour_calls(monkeypatch)
-    assert _names(col) == ["gsb_statistics_workspace_bytes"] + ["gsb_forward_statistics_deterministic", "gsb_sh_statistics_update"] * 2
+    assert _names(col) == ["gsb_statistics_workspace_bytes"] + ["gsb_forward", "gsb_sh_statistics_update"] * 2
     assert col[0][1] == (6,)
     torch.use_deterministic_algorithms(False)
     ref = _colour_calls(monkeypatch)
-    # the old arguments plus ONE workspace, the same for every camera
+    # the old request plus `deterministic` and ONE workspace, the same for every camera
     for (name, det), (_, old) in zip(col[1::2], ref[0::2]):
-        assert det[:-2] == old[:-1] and det[-1] == 0
-    assert col[1][1][-2] == col[3][1][-2]
+        det, old = dict(det[0]), dict(old[0])
+        assert det.pop("deterministic") == 1 and det.pop("workspace") is not None
+        assert old.pop("deterministic") == 0 and old.pop("workspace") is None and det == old
+    torch.use_deterministic_algorithms(True)
+    reqs = _colour_calls(monkeypatch, raw=True)
+    assert len(reqs) == 2 and reqs[0].workspace and reqs[0].workspace == reqs[1].workspace
     torch.use_deterministic_algorithms(True)
     km = _kmeans_calls(monkeypatch)
     assert _names(km) == ["gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic"]
@@ -224,16 +242,16 @@ def test_flag_is_read_at_call_time(monkeypatch, torch_deterministic):
     torch.use_deterministic_algorithms(True)
     assert _names(_kmeans_calls(monkeypatch))[-1] == "gsb_kmeans_deterministic"
     torch.use_deterministic_algorithms(False)
-    assert _names(_colour_calls(monkeypatch))[0] == "gsb_forward_statistics"
+    assert _deterministic(monkeypatch) == 0
 
 
 def test_explicit_bool_wins(monkeypatch, torch_deterministic):
     torch.use_deterministic_algorithms(True)
     assert _names(_kmeans_calls(monkeypatch, deterministic=False))[-1] == "gsb_kmeans"
-    assert _names(_colour_calls(monkeypatch, deterministic=False))[0] == "gsb_forward_statistics"
+    assert _deterministic(monkeypatch, deterministic=False) == 0
     torch.use_deterministic_algorithms(False)
     assert _names(_kmeans_calls(monkeypatch, deterministic=True))[-1] == "gsb_kmeans_deterministic"
-    assert _names(_colour_calls(monkeypatch, deterministic=True))[1] == "gsb_forward_statistics_deterministic"
+    assert _deterministic(monkeypatch, deterministic=True) == 1
 
 
 def test_keyword_only(monkeypatch):

@@ -1,5 +1,5 @@
-"""CPU: the feature-channel entry points (gsb_forward_features / gsb_backward_features) reject each bad argument before any CUDA
-call, with gsb_last_error() set, and the Python layer refuses what the feature pass does not take (CPU tensors, a shape other than
+"""CPU: the feature-channel requests (the `features` field of GsbForwardRequest / GsbBackwardRequest) reject each bad argument before
+any CUDA call, with gsb_last_error() set, and the Python layer refuses what the feature pass does not take (CPU tensors, a shape other than
 [P, F], F out of range, accumulate_into, a feature gradient under the deterministic mode) before anything runs."""
 import ctypes as C
 import os
@@ -16,7 +16,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_symbols_struct_and_limit():
     L = lib.lib()
-    for sym in ("gsb_forward_features", "gsb_backward_features"):
+    for sym in ("gsb_forward", "gsb_backward"):
         assert sym in lib.EXPORTED_SYMBOLS
         getattr(L, sym)
     assert C.sizeof(lib.GsbFeatures) == 8 + 4 * 8 and lib.GsbFeatures.features.offset == 8
@@ -24,10 +24,14 @@ def test_symbols_struct_and_limit():
     assert int(re.search(r"#define GSB_FEATURES_MAX (\d+)", header).group(1)) == lib.FEATURES_MAX == 256
 
 
-def _fwd(L, feats, P=10, R=5, W=16, H=16, blobs=True):
-    buf = (C.c_char * 256)()
-    b = C.addressof(buf) if blobs else None
-    return L.gsb_forward_features(b, P, b, R, b, W, H, None if feats is None else C.byref(feats), None)
+def _fwd(L, feats, P=10, W=16, H=16):
+    buf = (C.c_float * 64)()
+    b = C.addressof(buf)
+    scene = lib.GsbScene(P=P, means3D=b, opacities=b, degrees=b)
+    cam = lib.GsbCamera(width=W, height=H, viewmatrix=b, projmatrix=b, campos=b, background=b)
+    req = lib.GsbForwardRequest(scene=C.pointer(scene), cam=C.pointer(cam), out_color=b, radii=b, num_rendered=C.pointer(C.c_int64(0)),
+                                features=C.pointer(feats))
+    return L.gsb_forward(C.byref(req))
 
 
 def test_forward_features_rejects_bad_arguments():
@@ -35,16 +39,15 @@ def test_forward_features_rejects_bad_arguments():
     fbuf = (C.c_float * 16)()
     p = C.addressof(fbuf)
     cases = [
-        (None, {}, b"features is NULL"),
         (lib.GsbFeatures(0, p, p, None, None), {}, b"F = 0"),
         (lib.GsbFeatures(257, p, p, None, None), {}, b"F = 257"),
         (lib.GsbFeatures(-3, p, p, None, None), {}, b"F = -3"),
         (lib.GsbFeatures(4, None, p, None, None), {}, b"features->features is NULL"),
         (lib.GsbFeatures(4, p, None, None, None), {}, b"out is NULL"),
         (lib.GsbFeatures(4, p, p, None, None), dict(P=-1), b"P < 0"),
-        (lib.GsbFeatures(4, p, p, None, None), dict(R=-1), b"num_rendered < 0"),
         (lib.GsbFeatures(4, p, p, None, None), dict(W=0), b"image size"),
-        (lib.GsbFeatures(4, p, p, None, None), dict(blobs=False), b"blob is NULL"),
+        # with P == 0 the features themselves may be NULL: the request goes on to the scene's checks (a camera without tensors)
+        (lib.GsbFeatures(4, None, p, None, None), dict(P=0, W=0), b"image size"),
     ]
     for feats, kw, msg in cases:
         assert _fwd(L, feats, **kw) == -1, msg
@@ -52,10 +55,10 @@ def test_forward_features_rejects_bad_arguments():
 
 
 def _bwd(L, scene, feats, R=5, det_ws=None, raw=None, raw_grads=None):
-    cam = lib.GsbCamera()
-    g = lib.GsbGrads()
-    return L.gsb_backward_features(scene, C.byref(cam), R, None, None, None, None, None, C.byref(g), None, None, 0.0, None, None, None, None,
-                                   raw, raw_grads, 0, det_ws, None if feats is None else C.byref(feats), None)
+    req = lib.GsbBackwardRequest(scene=scene, cam=C.pointer(lib.GsbCamera()), num_rendered=R, grads=C.pointer(lib.GsbGrads()), raw=raw,
+                                 raw_grads=raw_grads, deterministic=int(det_ws is not None), det_workspace=det_ws,
+                                 features=None if feats is None else C.pointer(feats))
+    return L.gsb_backward(C.byref(req))
 
 
 def test_backward_features_rejects_bad_arguments():
@@ -63,8 +66,8 @@ def test_backward_features_rejects_bad_arguments():
     fbuf = (C.c_float * 16)()
     p = C.addressof(fbuf)
     ok = lib.GsbFeatures(4, p, None, p, p)
-    scene = C.byref(lib.GsbScene(P=10))
-    for sc in (None, C.byref(lib.GsbScene(P=-1))):
+    scene = C.pointer(lib.GsbScene(P=10))
+    for sc in (None, C.pointer(lib.GsbScene(P=-1))):
         assert _bwd(L, sc, ok) == -1 and b"P < 0" in L.gsb_last_error()
     buf = (C.c_char * 256)()
     assert _bwd(L, scene, ok, det_ws=C.addressof(buf)) == -1 and b"no deterministic form" in L.gsb_last_error()
@@ -75,12 +78,12 @@ def test_backward_features_rejects_bad_arguments():
         assert _bwd(L, scene, feats) == -1, msg
         assert msg in L.gsb_last_error(), (msg, L.gsb_last_error())
     assert _bwd(L, scene, ok, R=-1) == -1 and b"num_rendered < 0" in L.gsb_last_error()
-    assert _bwd(L, scene, ok, raw_grads=C.byref(lib.GsbRawGrads())) == -1 and b"raw_grads given without raw" in L.gsb_last_error()
-    assert _bwd(L, scene, ok, raw=C.byref(lib.GsbRawParams(C=4)), raw_grads=C.byref(lib.GsbRawGrads())) == -1
+    assert _bwd(L, scene, ok, raw_grads=C.pointer(lib.GsbRawGrads())) == -1 and b"raw_grads given without raw" in L.gsb_last_error()
+    assert _bwd(L, scene, ok, raw=C.pointer(lib.GsbRawParams(C=4)), raw_grads=C.pointer(lib.GsbRawGrads())) == -1
     assert b"C = 4" in L.gsb_last_error()
     # valid feature arguments go on to the scene checks of the backward (an empty camera is refused there)
     assert _bwd(L, scene, ok) == -1 and b"image size" in L.gsb_last_error()
-    # without features it is gsb_backward_deterministic (with det_workspace) or the plain backward
+    # without features it is the deterministic backward (with det_workspace) or the plain backward
     assert _bwd(L, scene, None, det_ws=None, R=1 << 30) == -1 and b"image size" in L.gsb_last_error()
     assert _bwd(L, scene, None, det_ws=C.addressof(buf), R=1 << 30) == -4 and b"2^30" in L.gsb_last_error()
 

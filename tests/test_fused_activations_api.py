@@ -1,5 +1,5 @@
-"""CPU: rendering from the model's raw parameters (`pipe.fused_activations`, gsb_forward_raw / gsb_backward_raw, DESIGN.md §5h):
-the symbols and struct layouts, the GSB_EINVAL cases of the C entry points (all raised before any CUDA call), every refusal of the
+"""CPU: rendering from the model's raw parameters (`pipe.fused_activations`, the `raw` / `raw_grads` fields of the
+rasterizer requests, DESIGN.md §5h): the struct layouts, the GSB_EINVAL cases of the C calls (all raised before any CUDA call), every refusal of the
 Python layers (raised before anything runs, parameters untouched), and, against a stub of `_C`, that render() hands the
 parameters' own storage to the rasterizer, that the flag reaches the backward, and that the `.grad` tensors are the rasterizer's
 own outputs with no Cat / Exp / Div node in the graph."""
@@ -20,9 +20,10 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 def test_raw_symbols_are_exported():
     L = lib.lib()
-    for sym in ("gsb_forward_raw", "gsb_backward_raw"):
+    for sym in ("gsb_forward", "gsb_backward"):
         assert sym in lib.EXPORTED_SYMBOLS
         getattr(L, sym)
+    assert lib.GsbForwardRequest.raw.size == lib.GsbBackwardRequest.raw.size == lib.GsbBackwardRequest.raw_grads.size == 8
 
 
 def test_raw_struct_layouts_match_header():
@@ -65,25 +66,20 @@ def _raw(Cn=15, dc=_A, rest=_A, scaling=_A, rotation=_A):
 
 
 def _fwd(scene, raw, invdepth=None, alpha=None):
-    L = lib.lib()
-    R = C.c_int64(0)
-    cam = lib.GsbCamera()
-    return L.gsb_forward_raw(C.byref(scene) if scene is not None else None, C.byref(cam), lib.ALLOC_FN(0), None, lib.ALLOC_FN(0), None,
-                             lib.ALLOC_FN(0), None, None, None, C.byref(R), None, invdepth, alpha,
-                             C.byref(raw) if raw is not None else None, 0, None)
+    req = lib.GsbForwardRequest(scene=C.pointer(scene) if scene is not None else None, cam=C.pointer(lib.GsbCamera()),
+                                num_rendered=C.pointer(C.c_int64(0)), out_invdepth=invdepth, out_alpha=alpha, raw=C.pointer(raw))
+    return lib.lib().gsb_forward(C.byref(req))
 
 
 def _bwd(scene, raw, grads=None, raw_grads=None):
-    L = lib.lib()
-    cam = lib.GsbCamera()
     g = grads if grads is not None else lib.GsbGrads()
     rg = raw_grads if raw_grads is not None else lib.GsbRawGrads(_A, _A, _A, _A)
-    return L.gsb_backward_raw(C.byref(scene), C.byref(cam), 0, None, None, None, None, None, C.byref(g), None, None, 0.0, None, None, None,
-                              None, C.byref(raw) if raw is not None else None, C.byref(rg), 0, None)
+    req = lib.GsbBackwardRequest(scene=C.pointer(scene), cam=C.pointer(lib.GsbCamera()), grads=C.pointer(g), raw=C.pointer(raw),
+                                 raw_grads=C.pointer(rg))
+    return lib.lib().gsb_backward(C.byref(req))
 
 
 @pytest.mark.parametrize("case, msg", [
-    ("no_raw", b"raw parameters are NULL"),
     ("C5", b"C = 5"),
     ("scales_set", b"must be NULL"),
     ("shs_set", b"must be NULL"),
@@ -99,9 +95,7 @@ def _bwd(scene, raw, grads=None, raw_grads=None):
 ])
 def test_raw_entry_points_refuse(case, msg):
     scene, raw = _scene(), _raw()
-    if case == "no_raw":
-        raw = None
-    elif case == "C5":
+    if case == "C5":
         raw = _raw(Cn=5)
     elif case == "scales_set":
         scene.scales = _A

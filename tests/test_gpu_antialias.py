@@ -1,4 +1,4 @@
-"""GPU: anti-aliased rendering (`antialiasing=True`, gsb_forward_antialiased / gsb_backward_antialiased, DESIGN.md §5e).
+"""GPU: anti-aliased rendering (`antialiasing=True`, the requests' `antialiasing` field, DESIGN.md §5e).
   1. nothing else moves: radii, tiles, depths, means2D, conic, cov3D, rgb, clamped, R, sorted keys and point_list are bit-identical
      with and without anti-aliasing, and without it conic_opacity[:,3] is the plain sigmoid;
   2. the effective opacity is sigmoid * s, s = sqrt(max(2.5e-5, det0 / det1)), against float64;

@@ -1,4 +1,4 @@
-"""GPU: gradients w.r.t. the camera (viewmatrix, projmatrix, campos; gsb_backward_camera / camera_grads=True).
+"""GPU: gradients w.r.t. the camera (viewmatrix, projmatrix, campos; gsb_backward's camera outputs / camera_grads=True).
   1. nothing else moves: with the camera gradients on, the per-Gaussian outputs taken from the accumulator are bit-identical and
      the computed ones agree to fp32 rounding; with and without anti-aliasing the camera outputs (and with it every output) are
      the same bytes on every run and on any stream; P = 0 and R = 0 give zeros, with the camera gradients, the maps or both;

@@ -1,4 +1,4 @@
-"""GPU: the deterministic backward (`deterministic=True`, gsb_backward_deterministic, DESIGN.md §5i).
+"""GPU: the deterministic backward (`deterministic=True`, gsb_backward's `deterministic`, DESIGN.md §5i).
   1. one-warp identity: on an 8x4 image the default path adds one partial per Gaussian, so both paths give the same values (a zero's
      sign aside) in every output: dense, quantised, pruned, maps, AA, camera gradients, raw; on 3x2 tiles with multi-tile rects the
      two agree per element (the slot arithmetic and the gather); a num_rendered that does not match the blobs gives NaN;

@@ -1,4 +1,4 @@
-"""GPU: per-Gaussian feature channels (`features=[P, F]`, gsb_forward_features / gsb_backward_features) against the colour path,
+"""GPU: per-Gaussian feature channels (`features=[P, F]`, the requests' `features` field) against the colour path,
 which the parity tests pin to the reference, and against a float64 restatement of the compositing:
   - a feature channel equals the colour channel of a colors_precomp = features, bg = 0 render, bit for bit, on the dense, raw,
     quantised and anti-aliased paths, and the variable-SH inference path's feature image equals the dense path's;

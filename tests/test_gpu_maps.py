@@ -1,4 +1,4 @@
-"""GPU: the inverse-depth and alpha maps of `return_maps` (gsb_forward_maps / gsb_backward_maps) against the colour path, which the
+"""GPU: the inverse-depth and alpha maps of `return_maps` (the requests' map fields) against the colour path, which the
 parity tests pin to the reference bit for bit.  Every check is a linear identity:
   - the maps change nothing else (colour, radii, R, final_T, n_contrib, point_list are bit-identical with the maps on);
   - alpha == 1 - final_T, and invdepth == channel 0 of a render with colour (1/depth, 0, 0) and no background, bitwise;

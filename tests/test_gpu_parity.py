@@ -384,7 +384,7 @@ def test_quantised_model_with_override_color():
 
 def test_speculative_binning_across_workload_jumps():
     """The binning blob is carved for the capacity recent frames needed (+6 %) before this frame's instance count is known
-    (gsb_api.cu forward_impl).  A frame whose count outgrows that speculation must be re-launched transparently, and a much
+    (gsb_api.cu gsb_forward).  A frame whose count outgrows that speculation must be re-launched transparently, and a much
     smaller one must not inherit a stale layout: small -> large -> small -> large, every frame compared with the oracle."""
     ours = _ours()
     W, H = 320, 200

@@ -94,7 +94,7 @@ def test_tools_against_live_reference():
 
 
 def test_forward_statistics_against_oracle():
-    """touched_pixels / transmittance_sum of gsb_forward_statistics vs the oracle's renderCUDA restatement."""
+    """touched_pixels / transmittance_sum of a statistics forward vs the oracle's renderCUDA restatement."""
     sys.path.insert(0, os.path.join(os.path.dirname(HERE), "oracle"))
     import gs_oracle as O
     C = _C()

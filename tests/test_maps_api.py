@@ -1,5 +1,5 @@
-"""CPU: argument checks of the map entry points (gsb_forward_maps / gsb_backward_maps) and the Python layer's refusal of CPU
-tensors with return_maps; every call below is rejected before the first CUDA call."""
+"""CPU: argument checks of the map requests (out_invdepth / out_alpha of gsb_forward, dL_dinvdepth / dL_dalpha of gsb_backward) and
+the Python layer's refusal of CPU tensors with return_maps; every call below is rejected before the first CUDA call."""
 import ctypes as C
 
 import pytest
@@ -14,16 +14,16 @@ def test_map_entry_points_reject_bad_scenes():
     cb = lib.ALLOC_FN(lambda user, n: 0)
     R = C.c_int64(0)
     cam = lib.GsbCamera()
+    buf = (C.c_float * 16)()
+    m = C.addressof(buf)
     for scene in (None, lib.GsbScene(P=-1)):
-        sp = None if scene is None else C.byref(scene)
-        st = L.gsb_forward_maps(sp, C.byref(cam), cb, None, cb, None, cb, None, None, None, C.byref(R), None, None, None, None)
+        sp = None if scene is None else C.pointer(scene)
+        fwd = lib.GsbForwardRequest(scene=sp, cam=C.pointer(cam), geom_alloc=cb, binning_alloc=cb, image_alloc=cb, num_rendered=C.pointer(R),
+                                    out_invdepth=m, out_alpha=m)
+        st = L.gsb_forward(C.byref(fwd))
         assert st < 0 and len(L.gsb_last_error()) > 0
-        st = L.gsb_backward_maps(sp, C.byref(cam), 0, None, None, None, None, None, None, None, None, 0.0, None)
+        st = L.gsb_backward(C.byref(lib.GsbBackwardRequest(scene=sp, cam=C.pointer(cam), dL_dinvdepth=m, dL_dalpha=m)))
         assert st < 0 and len(L.gsb_last_error()) > 0
-    # a valid scene without the map outputs
-    scene = lib.GsbScene(P=0)
-    st = L.gsb_forward_maps(C.byref(scene), C.byref(cam), cb, None, cb, None, cb, None, None, None, C.byref(R), None, None, None, None)
-    assert st < 0 and b"map" in L.gsb_last_error()
 
 
 def test_render_with_maps_refuses_cpu_tensors():

@@ -1,4 +1,4 @@
-"""Cost of anti-aliased rendering (antialiasing=True, gsb_forward_antialiased / gsb_backward_antialiased) against the colour step.
+"""Cost of anti-aliased rendering (antialiasing=True, the requests' `antialiasing` field) against the colour step.
 
     python tools/bench_antialias.py [--config C3] [--steps 20] [--warmup 5]
 

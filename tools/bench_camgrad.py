@@ -1,11 +1,11 @@
-"""Cost of the camera gradients (camera_grads=True, gsb_backward_camera) against the colour step.
+"""Cost of the camera gradients (camera_grads=True, gsb_backward's camera outputs) against the colour step.
 
     python tools/bench_camgrad.py [--config C3] [--steps 20] [--warmup 5]
 
 bench.py's workload (C3: 3 M quantised Gaussians, 1920x1080, device-resident), one view per step over its cameras; each step
 is timed with a CUDA event pair, and L2 is flushed (256 MB write) between steps outside the pair.  Arms:
   a          colour forward + backward (gsb_forward / gsb_backward, what bench.py times)
-  b          the same plus the gradients w.r.t. viewmatrix, projmatrix and campos (gsb_backward_camera)
+  b          the same plus the gradients w.r.t. viewmatrix, projmatrix and campos (gsb_backward's camera outputs)
 The arms alternate step by step so that drift of the shared machine hits both alike.  A separate profiled pass per arm gives
 per-kernel times (gsb_profile_*): preprocess_backward and camera_grad (the one-CTA finishing kernel) are the ones that change.
 Prints the card's name and power limit, then one JSON line per arm and a summary line.

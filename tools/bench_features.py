@@ -5,7 +5,7 @@
 bench.py's workload (C3: 3 M quantised Gaussians, mixed SH degrees, 1920x1080, device-resident), one view per step over its
 cameras; each step is timed with a CUDA event pair, and L2 is flushed (256 MB write) between steps outside the pair.  Arms:
   base         colour forward (fwd) / forward + backward (fb), what bench.py times
-  feat_F       the same plus F feature channels (gsb_forward_features / gsb_backward_features), loss on colour and features
+  feat_F       the same plus F feature channels (the requests' `features` field), loss on colour and features
   override_F   the workaround: the colour step plus one colors_precomp render (forward, and backward) per 3 channels
 The arms alternate step by step so that drift of the shared machine hits all of them alike.  --ch sets GSB_FEATURES_CH (the
 channels per CTA of both feature kernels; 0 = the built-in choice).  A profiled pass gives the feature kernels' own device time.

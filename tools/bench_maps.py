@@ -5,7 +5,7 @@
 bench.py's workload (C3: 3 M quantised Gaussians, 1920x1080, device-resident), one view per step over its cameras; each step
 is timed with a CUDA event pair, and L2 is flushed (256 MB write) between steps outside the pair.  Arms:
   a          colour forward + backward (gsb_forward / gsb_backward, what bench.py times)
-  b          colour + both maps forward + backward (gsb_forward_maps / gsb_backward_maps), loss on all three
+  b          colour + both maps forward + backward (the requests' map fields), loss on all three
   c          the emulation of the reference's callers: (a) plus one override_color forward + backward per map
              (colour (1/z, 0, 0) for invdepth, colour (1, 1, 1) on a black background for alpha)
 The arms alternate step by step so that drift of the shared machine hits all of them alike.  A separate profiled pass per arm
