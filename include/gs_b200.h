@@ -305,8 +305,8 @@ typedef struct GsbBackwardRequest {
 	 * Gaussian's partials in row-major tile order.  No host synchronisation.  A num_rendered > 0 other than the blobs' instance
 	 * count makes every accumulated gradient NaN (and no slot beyond num_rendered is written); num_rendered = 0 means nothing was
 	 * rendered.  Every mode above has a deterministic form; the feature channels do not.
-	 * det_workspace: gsb_deterministic_workspace_bytes(P, num_rendered) bytes (slot offsets, scan scratch and 40 bytes per
-	 * instance); with dL_dmeans2D_abs, gsb_absgrad_deterministic_workspace_bytes(P, num_rendered) bytes (8 more per instance). */
+	 * det_workspace: gsb_deterministic_workspace_bytes(P, num_rendered, absgrad) bytes, absgrad != 0 with dL_dmeans2D_abs (slot
+	 * offsets, scan scratch and 40 bytes per instance; with absgrad 8 more per instance). */
 	int32_t deterministic;
 	char* det_workspace;
 	/* Feature channels (GsbFeatures) or NULL: dL_dout [F,H,W] is the gradient of the forward's feature image.  The backward of the
@@ -328,8 +328,7 @@ typedef struct GsbBackwardRequest {
 } GsbBackwardRequest;
 GSB_API int gsb_backward(const GsbBackwardRequest* req);
 GSB_API size_t gsb_camera_grad_workspace_bytes(int32_t P);
-GSB_API size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered);
-GSB_API size_t gsb_absgrad_deterministic_workspace_bytes(int32_t P, int64_t num_rendered);
+GSB_API size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered, int32_t absgrad);
 
 /* present[i] = view-space z of means3D[i] > 0.2 (auxiliary.h:139-159). */
 GSB_API int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix,
@@ -378,22 +377,18 @@ GSB_API int gsb_min_redundancy_value(int32_t P, const int32_t* redundancy_values
 /* 1-D k-means of the codebook quantisation (Reduced3DGS::kmeans, reduced_3dgs.cu:289-338 + reduced_3dgs/kmeans.cu):
  * Lloyd iterations from centers_in until sum|old - new| < tol or max_iterations, then ids[i] = index of the nearest centre
  * (smallest sqrt((c - v)^2), first index on ties).  ids: int32 [n_values]; centers_out: float [n_centers] (n_centers <= 1024;
- * the reference supports exactly 256).  workspace: gsb_kmeans_workspace_bytes(n_values, n_centers) bytes of device memory.
- * Synchronises the stream every 16 iterations (the reference: every iteration). */
-GSB_API size_t gsb_kmeans_workspace_bytes(int64_t n_values, int32_t n_centers);
+ * the reference supports exactly 256).  workspace: gsb_kmeans_workspace_bytes(n_values, n_centers, deterministic) bytes of device
+ * memory, 16-byte aligned with deterministic.  Synchronises the stream every 16 iterations (the reference: every iteration).
+ * deterministic != 0 (DESIGN.md §5j): the same sort, assignment and tie rule, update, stopping rule and host poll; only the centre
+ * sums change.  Each cluster's values are added in an order that is a function of the input alone (fixed-size chunks and blocks of
+ * the sorted values, aligned pairwise trees; not of the grid, SM count, stream or workspace address), so the same input gives the
+ * same centres and ids on every run and every H100.
+ * Errors (nothing launched; gsb_last_error() starts with "kmeans: "): GSB_EINVAL for n_values < 0, n_centers <= 0 or
+ * max_iterations < 0, then NULL centers_in / centers_out or, with n_values > 0, NULL values / ids / workspace, then with
+ * deterministic a workspace that is not 16-byte aligned; GSB_ERANGE for n_values >= 2^30; GSB_EINVAL for n_centers > 1024. */
+GSB_API size_t gsb_kmeans_workspace_bytes(int64_t n_values, int32_t n_centers, int32_t deterministic);
 GSB_API int gsb_kmeans(const float* values, int64_t n_values, const float* centers_in, int32_t n_centers, float tol, int32_t max_iterations,
-                int32_t* ids, float* centers_out, char* workspace, void* stream);
-
-/* Deterministic k-means (DESIGN.md §5j): the arguments, sort, assignment and tie rule, update, stopping rule and 16-iteration host
- * poll of gsb_kmeans; only the centre sums change.  Each cluster's values are added in an order that is a function of the input
- * alone (fixed-size chunks and blocks of the sorted values, aligned pairwise trees; not of the grid, SM count, stream or workspace
- * address), so the same input gives the same centres and ids on every run and every H100.
- * workspace: gsb_kmeans_deterministic_workspace_bytes(n_values, n_centers) bytes of device memory, 16-byte aligned.
- * Errors (GSB_EINVAL, nothing launched): those of gsb_kmeans, and a workspace that is not 16-byte aligned.
- * GSB_ERANGE: n_values >= 2^30. */
-GSB_API size_t gsb_kmeans_deterministic_workspace_bytes(int64_t n_values, int32_t n_centers);
-GSB_API int gsb_kmeans_deterministic(const float* values, int64_t n_values, const float* centers_in, int32_t n_centers, float tol,
-                int32_t max_iterations, int32_t* ids, float* centers_out, char* workspace, void* stream);
+                int32_t deterministic, int32_t* ids, float* centers_out, char* workspace, void* stream);
 
 /* Exact k nearest neighbours of points [P,3] (fp32) — the reference's second extension simple_knn._C (submodules/simple-knn:
  * distCUDA2, distIndex2, distIndexQ).  Squared distances d = (p - q).(p - q) evaluated as the reference evaluates them; the query
@@ -468,16 +463,25 @@ GSB_API int gsb_adam_step(const GsbAdamTensor* tensors, int32_t n, int32_t P, co
  * gsb_densify_stats: per iteration, for i < P (viewspace_grad is [P, grad_row_stride], its first two columns are read):
  *   xyz_gradient_accum[i] += sqrt(g0*g0 + g1*g1);  denom[i] += visibility[i] != 0;
  *   with radii (may be NULL): if visibility[i], max_radii2D[i] = max(max_radii2D[i], (float)radii[i]).
- * Errors (GSB_EINVAL): P < 0, grad_row_stride < 2, a NULL pointer other than radii / max_radii2D when P > 0, radii without
- * max_radii2D. */
-GSB_API int gsb_densify_stats(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const uint8_t* visibility,
-                const int32_t* radii, float* xyz_gradient_accum, float* denom, float* max_radii2D, void* stream);
+ * AbsGS (DESIGN.md §5m), for models that also keep xyz_gradient_accum_abs [P] (the norms of gsb_backward's dL_dmeans2D_abs):
+ * viewspace_grad_abs and xyz_gradient_accum_abs are both set or both NULL.  When set, the same launch also adds
+ *   xyz_gradient_accum_abs[i] += sqrt(a0*a0 + a1*a1) of row i of viewspace_grad_abs ([P, abs_row_stride], first two columns read);
+ * denom is counted once.  abs_row_stride is read only with them.
+ * Errors (GSB_EINVAL), in this order: P < 0; grad_row_stride < 2; one of viewspace_grad_abs / xyz_gradient_accum_abs without the
+ * other (at any P); with them, abs_row_stride < 2; radii without max_radii2D.  Then P == 0 returns GSB_OK without a launch, and
+ * with P > 0 a NULL viewspace_grad / visibility / xyz_gradient_accum / denom is refused. */
+GSB_API int gsb_densify_stats(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const float* viewspace_grad_abs,
+                int32_t abs_row_stride, const uint8_t* visibility, const int32_t* radii, float* xyz_gradient_accum,
+                float* xyz_gradient_accum_abs, float* denom, float* max_radii2D, void* stream);
 
 /* gsb_densify_plan: decides every row of the output and counts them into counts[GSB_DENSIFY_COUNTS] (device int64), which the
  * caller reads back once to size the outputs.  Modes:
  *   GSB_DENSIFY_CLONE_SPLIT  densify_and_prune: grads = accum / denom (NaN -> 0); clone if grads >= max_grad and
  *                            max(exp(scaling)) <= clone_max_scale; split if grads >= max_grad and max(exp(scaling)) > clone_max_scale;
  *                            then prune() over the result with max_radii2D = 0 (the reference has reset it by then).
+ *                            With xyz_gradient_accum_abs (AbsGS, DESIGN.md §5m) the split test takes the absolute gradient: split
+ *                            if accum_abs / denom >= max_grad_abs (NaN -> 0) and max(exp(scaling)) > clone_max_scale; the clone
+ *                            test is as above, so clones are never split.  max_grad_abs is read only with xyz_gradient_accum_abs.
  *   GSB_DENSIFY_PRUNE        prune(): drop sigmoid(opacity) < min_opacity, or with screen_test, max_radii2D > max_screen_size or
  *                            max(exp(scaling)) > big_scale.
  *   GSB_DENSIFY_PRUNE_MASK   prune_points(mask): drop the rows where prune_mask (u8 [P]) is nonzero.
@@ -485,34 +489,18 @@ GSB_API int gsb_densify_stats(int32_t P, const float* viewspace_grad, int32_t gr
  * scaling times split_scale_factor (the fp32 reciprocal of 0.8 * N that torch multiplies by) before the log, and is pruned on
  * its own reduced scaling.  The workspace (gsb_densify_workspace_bytes(P) bytes) keeps the plan for gsb_densify_emit and holds
  * exp(scaling) of the split parents, [n_split, 3] fp32 at byte offset gsb_densify_split_std_offset(P), for the caller's draw.
- * Errors (GSB_EINVAL): P < 0 or P >= 2^30, an unknown mode, NULL workspace / counts, NULL inputs the mode reads (P > 0). */
+ * Errors (GSB_EINVAL): P < 0 or P >= 2^30, an unknown mode, xyz_gradient_accum_abs with a mode other than
+ * GSB_DENSIFY_CLONE_SPLIT, NULL workspace / counts, NULL inputs the mode reads (P > 0). */
 #define GSB_DENSIFY_CLONE_SPLIT 0
 #define GSB_DENSIFY_PRUNE 1
 #define GSB_DENSIFY_PRUNE_MASK 2
 #define GSB_DENSIFY_COUNTS 8      /* kept originals, clones, kept clones, split parents, kept children per copy, P', pruned, 0 */
 GSB_API size_t gsb_densify_workspace_bytes(int32_t P);
 GSB_API size_t gsb_densify_split_std_offset(int32_t P);
-GSB_API int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* denom, const float* scaling,
-                const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad, float clone_max_scale,
-                float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
-                void* workspace, int64_t* counts, void* stream);
-
-/* The AbsGS forms (DESIGN.md §5m), for models that also keep xyz_gradient_accum_abs [P] (the norms of gsb_backward's
- * dL_dmeans2D_abs):
- * gsb_densify_stats_abs: gsb_densify_stats plus, in the same launch, xyz_gradient_accum_abs[i] += sqrt(a0*a0 + a1*a1) of row i of
- *   viewspace_grad_abs ([P, abs_row_stride], first two columns read).  denom is counted once.  Errors (GSB_EINVAL): those of
- *   gsb_densify_stats, abs_row_stride < 2, and NULL viewspace_grad_abs / xyz_gradient_accum_abs when P > 0.
- * gsb_densify_plan_abs: gsb_densify_plan's GSB_DENSIFY_CLONE_SPLIT with the split test on the absolute gradient: clone if
- *   accum / denom >= max_grad and max(exp(scaling)) <= clone_max_scale (as there); split if accum_abs / denom >= max_grad_abs
- *   (NaN -> 0) and max(exp(scaling)) > clone_max_scale.  Clones are never split; counts, workspace and row order as there.
- *   Errors (GSB_EINVAL): those of gsb_densify_plan in that mode, and NULL xyz_gradient_accum_abs when P > 0. */
-GSB_API int gsb_densify_stats_abs(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const float* viewspace_grad_abs,
-                int32_t abs_row_stride, const uint8_t* visibility, const int32_t* radii, float* xyz_gradient_accum,
-                float* xyz_gradient_accum_abs, float* denom, float* max_radii2D, void* stream);
-GSB_API int gsb_densify_plan_abs(int32_t P, const float* xyz_gradient_accum, const float* xyz_gradient_accum_abs, const float* denom,
-                const float* scaling, const float* opacity, float max_grad, float max_grad_abs, float clone_max_scale,
-                float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
-                void* workspace, int64_t* counts, void* stream);
+GSB_API int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* xyz_gradient_accum_abs,
+                const float* denom, const float* scaling, const float* opacity, const float* max_radii2D, const uint8_t* prune_mask,
+                float max_grad, float max_grad_abs, float clone_max_scale, float min_opacity, int32_t screen_test, float max_screen_size,
+                float big_scale, float split_scale_factor, void* workspace, int64_t* counts, void* stream);
 
 /* gsb_densify_emit: writes every output row of every table entry in one launch, from the plan in `workspace` and the counts
  * read back.  Per entry: the [P, row_width] source rows of 4-byte elements (param, and optionally both moments and the grad)

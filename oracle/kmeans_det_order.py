@@ -1,4 +1,4 @@
-"""float32 restatement of gsb_kmeans_deterministic (DESIGN.md §5j): the assignment, the order in which each cluster's values are
+"""float32 restatement of the deterministic gsb_kmeans (DESIGN.md §5j): the assignment, the order in which each cluster's values are
 added, the update and the stopping rule, in numpy.  The device path must reproduce its centres bit for bit, its iteration count and
 its ids.  It is kept apart from gs_oracle so that the goldens made from gs_oracle keep measuring what they measure.
 

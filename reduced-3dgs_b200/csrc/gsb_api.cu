@@ -109,10 +109,8 @@ int launch_min_redundancy(int, const int*, const int*, const uint8_t*, int, int*
 int launch_redundancy_fused(int, const float*, const float*, const float*, const int*, const float*, float, int, int*, cudaStream_t);
 int launch_l1_ssim_forward(const float*, const float*, int, int, int, float*, float*, cudaStream_t);
 int launch_l1_ssim_backward(const float*, const float*, int, int, int, const float*, float, const float*, float, const float*, float*, cudaStream_t);
-size_t kmeans_workspace_bytes(long long, int);
-int launch_kmeans(const float*, long long, const float*, int, float, int, int*, float*, char*, cudaStream_t);
-size_t kmeans_deterministic_workspace_bytes(long long, int);
-int launch_kmeans_deterministic(const float*, long long, const float*, int, float, int, int*, float*, char*, cudaStream_t);
+size_t kmeans_workspace_bytes(long long, int, bool);
+int launch_kmeans(const float*, long long, const float*, int, float, int, int*, float*, char*, bool, cudaStream_t);
 size_t knn_workspace_bytes(long long, long long);
 int launch_knn(const float*, long long, int, const int32_t*, long long, const int32_t*, long long, float*, float*, int32_t*, char*, cudaStream_t);
 size_t det_workspace_bytes(int, long long, int);
@@ -274,7 +272,7 @@ size_t gsb_image_bytes_for(int32_t P, int32_t W, int32_t H, int32_t quantised)
 size_t gsb_binning_bytes(int64_t R) { size_t b; BinningState::carve(nullptr, R, &b); return b + 256; }
 uint64_t gsb_launch_count(void) { return g_launch_count.load(); }
 const char* gsb_last_error(void) { return g_err; }
-const char* gsb_version(void) { return "gs_b200 0.2 (sm_90a)"; }
+const char* gsb_version(void) { return "gs_b200 0.3 (sm_90a)"; }
 
 void gsb_profile_enable(int on)
 {
@@ -452,32 +450,19 @@ int gsb_l1_ssim_backward(const float* image, const float* gt, int32_t channels, 
 		(cudaStream_t)stream);
 }
 
-size_t gsb_kmeans_workspace_bytes(int64_t n_values, int32_t n_centers) { return kmeans_workspace_bytes(n_values, n_centers); }
+size_t gsb_kmeans_workspace_bytes(int64_t n_values, int32_t n_centers, int32_t deterministic)
+{
+	return kmeans_workspace_bytes(n_values, n_centers, deterministic != 0);
+}
 
 int gsb_kmeans(const float* values, int64_t n_values, const float* centers_in, int32_t n_centers, float tol, int32_t max_iterations,
-	int32_t* ids, float* centers_out, char* workspace, void* stream)
+	int32_t deterministic, int32_t* ids, float* centers_out, char* workspace, void* stream)
 {
 	if (n_values < 0 || n_centers <= 0 || max_iterations < 0) { set_error("kmeans: bad sizes"); return GSB_EINVAL; }
 	if (!centers_in || !centers_out || (n_values > 0 && (!values || !ids || !workspace))) { set_error("kmeans: NULL argument"); return GSB_EINVAL; }
+	if (deterministic && (reinterpret_cast<uintptr_t>(workspace) & 15)) { set_error("kmeans: workspace is not 16-byte aligned"); return GSB_EINVAL; }
 	if (n_values >= (1ll << 30)) { set_error("kmeans: 2^30 or more values (the look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
-	return launch_kmeans(values, n_values, centers_in, n_centers, tol, max_iterations, ids, centers_out, workspace, (cudaStream_t)stream);
-}
-
-size_t gsb_kmeans_deterministic_workspace_bytes(int64_t n_values, int32_t n_centers)
-{
-	return kmeans_deterministic_workspace_bytes(n_values < 0 ? 0 : n_values, n_centers);
-}
-
-int gsb_kmeans_deterministic(const float* values, int64_t n_values, const float* centers_in, int32_t n_centers, float tol,
-	int32_t max_iterations, int32_t* ids, float* centers_out, char* workspace, void* stream)
-{
-	if (n_values < 0 || n_centers <= 0 || max_iterations < 0) { set_error("kmeans_deterministic: bad sizes"); return GSB_EINVAL; }
-	if (!centers_in || !centers_out || (n_values > 0 && (!values || !ids || !workspace)))
-	{ set_error("kmeans_deterministic: NULL argument"); return GSB_EINVAL; }
-	if (reinterpret_cast<uintptr_t>(workspace) & 15) { set_error("kmeans_deterministic: workspace is not 16-byte aligned"); return GSB_EINVAL; }
-	if (n_values >= (1ll << 30))
-	{ set_error("kmeans_deterministic: 2^30 or more values (the look-back descriptors carry 30-bit counts)"); return GSB_ERANGE; }
-	return launch_kmeans_deterministic(values, n_values, centers_in, n_centers, tol, max_iterations, ids, centers_out, workspace,
+	return launch_kmeans(values, n_values, centers_in, n_centers, tol, max_iterations, ids, centers_out, workspace, deterministic != 0,
 		(cudaStream_t)stream);
 }
 
@@ -542,8 +527,10 @@ int gsb_backward(const GsbBackwardRequest* req)
 }
 
 size_t gsb_camera_grad_workspace_bytes(int32_t P) { return camera_grad_workspace_bytes(P); }
-size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered, 10); }
-size_t gsb_absgrad_deterministic_workspace_bytes(int32_t P, int64_t num_rendered) { return det_workspace_bytes(P, num_rendered, DET_NS_ABS); }
+size_t gsb_deterministic_workspace_bytes(int32_t P, int64_t num_rendered, int32_t absgrad)
+{
+	return det_workspace_bytes(P, num_rendered, absgrad ? DET_NS_ABS : 10);
+}
 
 int gsb_mark_visible(int32_t P, const float* means3D, const float* viewmatrix, const float* projmatrix, uint8_t* present, void* stream)
 {

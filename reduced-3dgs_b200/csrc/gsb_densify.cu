@@ -51,7 +51,7 @@ struct PlanArgs {
 	const float *accum, *denom, *scaling, *opacity, *max_radii2D;
 	const uint8_t* mask;
 	float max_grad, clone_max_scale, min_opacity, max_screen_size, big_scale, split_factor;
-	const float* accum_abs;    // gsb_densify_plan_abs: the split test reads accum_abs / denom against max_grad_abs (NULL otherwise)
+	const float* accum_abs;    // non-NULL: the split test reads accum_abs / denom against max_grad_abs (AbsGS)
 	float max_grad_abs;
 	int P, mode, screen_test;
 };
@@ -324,53 +324,44 @@ using namespace gsb;
 extern "C" size_t gsb_densify_workspace_bytes(int32_t P) { return densify_carve(nullptr, P).bytes; }
 extern "C" size_t gsb_densify_split_std_offset(int32_t P) { return densify_carve(nullptr, P).std_offset; }
 
-extern "C" int gsb_densify_stats(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const uint8_t* visibility,
-	const int32_t* radii, float* xyz_gradient_accum, float* denom, float* max_radii2D, void* stream)
+extern "C" int gsb_densify_stats(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const float* viewspace_grad_abs,
+	int32_t abs_row_stride, const uint8_t* visibility, const int32_t* radii, float* xyz_gradient_accum, float* xyz_gradient_accum_abs,
+	float* denom, float* max_radii2D, void* stream)
 {
 	if (P < 0) { set_error("densify_stats: P < 0"); return GSB_EINVAL; }
 	if (grad_row_stride < 2) { set_error("densify_stats: grad_row_stride %d < 2", grad_row_stride); return GSB_EINVAL; }
+	const bool abs = viewspace_grad_abs != nullptr;
+	if (abs != (xyz_gradient_accum_abs != nullptr))
+	{ set_error("densify_stats: viewspace_grad_abs and xyz_gradient_accum_abs must be both NULL or both set"); return GSB_EINVAL; }
+	if (abs && abs_row_stride < 2) { set_error("densify_stats: abs_row_stride %d must be >= 2", abs_row_stride); return GSB_EINVAL; }
 	if (radii && !max_radii2D) { set_error("densify_stats: radii given without max_radii2D"); return GSB_EINVAL; }
 	if (P == 0) return GSB_OK;
 	if (!viewspace_grad || !visibility || !xyz_gradient_accum || !denom)
 	{ set_error("densify_stats: NULL viewspace_grad / visibility / xyz_gradient_accum / denom"); return GSB_EINVAL; }
 	const cudaStream_t st = (cudaStream_t)stream;
 	ProfScope prof(K_TOOLS, st);
-	densify_stats_kernel<false><<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii, xyz_gradient_accum,
-		denom, max_radii2D);
+	if (abs)
+		densify_stats_kernel<true><<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii,
+			xyz_gradient_accum, denom, max_radii2D, viewspace_grad_abs, abs_row_stride, xyz_gradient_accum_abs);
+	else
+		densify_stats_kernel<false><<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii,
+			xyz_gradient_accum, denom, max_radii2D);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
 }
 
-extern "C" int gsb_densify_stats_abs(int32_t P, const float* viewspace_grad, int32_t grad_row_stride, const float* viewspace_grad_abs,
-	int32_t abs_row_stride, const uint8_t* visibility, const int32_t* radii, float* xyz_gradient_accum, float* xyz_gradient_accum_abs,
-	float* denom, float* max_radii2D, void* stream)
-{
-	if (P < 0) { set_error("densify_stats_abs: P < 0"); return GSB_EINVAL; }
-	if (grad_row_stride < 2 || abs_row_stride < 2)
-	{ set_error("densify_stats_abs: row strides %d / %d; both must be >= 2", grad_row_stride, abs_row_stride); return GSB_EINVAL; }
-	if (radii && !max_radii2D) { set_error("densify_stats_abs: radii given without max_radii2D"); return GSB_EINVAL; }
-	if (P == 0) return GSB_OK;
-	if (!viewspace_grad || !viewspace_grad_abs || !visibility || !xyz_gradient_accum || !xyz_gradient_accum_abs || !denom)
-	{ set_error("densify_stats_abs: NULL viewspace_grad / viewspace_grad_abs / visibility / xyz_gradient_accum(_abs) / denom"); return GSB_EINVAL; }
-	const cudaStream_t st = (cudaStream_t)stream;
-	ProfScope prof(K_TOOLS, st);
-	densify_stats_kernel<true><<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii,
-		xyz_gradient_accum, denom, max_radii2D, viewspace_grad_abs, abs_row_stride, xyz_gradient_accum_abs);
-	GSB_LAUNCHED();
-	GSB_CUDA_OK(cudaGetLastError());
-	return GSB_OK;
-}
-
-// gsb_densify_plan and gsb_densify_plan_abs (xyz_gradient_accum_abs non-NULL: the AbsGS split test)
-static int densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* xyz_gradient_accum_abs, const float* denom,
-	const float* scaling, const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad, float max_grad_abs,
-	float clone_max_scale, float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
-	void* workspace, int64_t* counts, void* stream)
+// xyz_gradient_accum_abs non-NULL: the AbsGS split test (GSB_DENSIFY_CLONE_SPLIT only)
+extern "C" int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* xyz_gradient_accum_abs,
+	const float* denom, const float* scaling, const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad,
+	float max_grad_abs, float clone_max_scale, float min_opacity, int32_t screen_test, float max_screen_size, float big_scale,
+	float split_scale_factor, void* workspace, int64_t* counts, void* stream)
 {
 	if (P < 0 || P >= (1 << 30)) { set_error("densify_plan: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
 	if (mode != GSB_DENSIFY_CLONE_SPLIT && mode != GSB_DENSIFY_PRUNE && mode != GSB_DENSIFY_PRUNE_MASK)
 	{ set_error("densify_plan: unknown mode %d", mode); return GSB_EINVAL; }
+	if (xyz_gradient_accum_abs && mode != GSB_DENSIFY_CLONE_SPLIT)
+	{ set_error("densify_plan: xyz_gradient_accum_abs given with mode %d; only GSB_DENSIFY_CLONE_SPLIT reads it", mode); return GSB_EINVAL; }
 	if (!workspace || !counts) { set_error("densify_plan: NULL workspace / counts"); return GSB_EINVAL; }
 	if (P > 0)
 	{
@@ -399,25 +390,6 @@ static int densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
-}
-
-extern "C" int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradient_accum, const float* denom, const float* scaling,
-	const float* opacity, const float* max_radii2D, const uint8_t* prune_mask, float max_grad, float clone_max_scale,
-	float min_opacity, int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor,
-	void* workspace, int64_t* counts, void* stream)
-{
-	return densify_plan(P, mode, xyz_gradient_accum, nullptr, denom, scaling, opacity, max_radii2D, prune_mask, max_grad, 0.0f,
-		clone_max_scale, min_opacity, screen_test, max_screen_size, big_scale, split_scale_factor, workspace, counts, stream);
-}
-
-extern "C" int gsb_densify_plan_abs(int32_t P, const float* xyz_gradient_accum, const float* xyz_gradient_accum_abs, const float* denom,
-	const float* scaling, const float* opacity, float max_grad, float max_grad_abs, float clone_max_scale, float min_opacity,
-	int32_t screen_test, float max_screen_size, float big_scale, float split_scale_factor, void* workspace, int64_t* counts, void* stream)
-{
-	if (P > 0 && !xyz_gradient_accum_abs) { set_error("densify_plan_abs: NULL xyz_gradient_accum_abs"); return GSB_EINVAL; }
-	return densify_plan(P, GSB_DENSIFY_CLONE_SPLIT, xyz_gradient_accum, xyz_gradient_accum_abs, denom, scaling, opacity, nullptr, nullptr,
-		max_grad, max_grad_abs, clone_max_scale, min_opacity, screen_test, max_screen_size, big_scale, split_scale_factor, workspace, counts,
-		stream);
 }
 
 extern "C" int gsb_densify_emit(const GsbDensifyTensor* tensors, int32_t n, int32_t P, const void* workspace, int64_t n_kept,

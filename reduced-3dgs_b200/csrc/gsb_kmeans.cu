@@ -13,7 +13,7 @@
 //   * update + convergence test on the device: later iterations see the `done` flag and exit immediately, the host only
 //     looks at the flag every few iterations (same stopping rule as the reference, without a sync per iteration).
 // Cluster ids / sizes are exact; centre values differ from the reference in float summation order only (the reference's own
-// order is arbitrary: atomics).  gsb_kmeans_deterministic replaces the accumulate step by km_det_block_kernel +
+// order is arbitrary: atomics).  gsb_kmeans with `deterministic` replaces the accumulate step by km_det_block_kernel +
 // km_det_cluster_kernel, which add each cluster's values in an order fixed by the input (see below, DESIGN.md §5j).
 #include "gsb_common.cuh"
 
@@ -354,7 +354,7 @@ __global__ void __launch_bounds__(256) km_ids_kernel(const float* __restrict__ v
 }
 
 // ------------------------------------------------------------------------------------------------ deterministic centre sums
-// The order in which gsb_kmeans_deterministic adds a cluster's values (DESIGN.md §5j; restated in oracle/kmeans_det_order.py) is a
+// The order in which the deterministic gsb_kmeans adds a cluster's values (DESIGN.md §5j; restated in oracle/kmeans_det_order.py) is a
 // function of the sorted values and their ids alone.  Sorted position p lies in block b = p / 4096 and, inside it, in chunk
 // t = (p % 4096) / 16.  With -0.0f, the exact identity of IEEE addition, standing for "no value":
 //   leaf(b, t, k)  = (((-0 + v_p0) + v_p1) + ...) over the positions of chunk t with id k, ascending;
@@ -511,8 +511,6 @@ static KmWorkspace km_carve(char* base, long long n, int K)
 	return w;
 }
 
-size_t kmeans_workspace_bytes(long long n, int K) { return km_carve(nullptr, n, K).bytes; }
-
 // The deterministic path's workspace: the default's, then per block of 4096 values a list of up to K parts and its length, and
 // the per-cluster block spans.
 struct KmDetWorkspace {
@@ -532,10 +530,10 @@ static KmDetWorkspace km_det_carve(char* base, long long n, int K)
 	return d;
 }
 
-size_t kmeans_deterministic_workspace_bytes(long long n, int K) { return km_det_carve(nullptr, n, K).bytes; }
+size_t kmeans_workspace_bytes(long long n, int K, bool det) { return det ? km_det_carve(nullptr, n, K).bytes : km_carve(nullptr, n, K).bytes; }
 
 // det: the centre sums of km_det_block_kernel / km_det_cluster_kernel instead of km_accumulate_kernel; everything else is shared.
-static int km_run(const float* values, long long n, const float* centres_in, int K, float tol, int max_iterations, int* ids, float* centres,
+int launch_kmeans(const float* values, long long n, const float* centres_in, int K, float tol, int max_iterations, int* ids, float* centres,
 	char* workspace, bool det, cudaStream_t stream)
 {
 	if (K <= 0 || K > KM_MAX_K) { set_error("kmeans: number of centres must be in 1..%d", KM_MAX_K); return GSB_EINVAL; }
@@ -608,18 +606,6 @@ static int km_run(const float* values, long long n, const float* centres_in, int
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
-}
-
-int launch_kmeans(const float* values, long long n, const float* centres_in, int K, float tol, int max_iterations, int* ids, float* centres,
-	char* workspace, cudaStream_t stream)
-{
-	return km_run(values, n, centres_in, K, tol, max_iterations, ids, centres, workspace, false, stream);
-}
-
-int launch_kmeans_deterministic(const float* values, long long n, const float* centres_in, int K, float tol, int max_iterations, int* ids,
-	float* centres, char* workspace, cudaStream_t stream)
-{
-	return km_run(values, n, centres_in, K, tol, max_iterations, ids, centres, workspace, true, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ pair sort (gsb_knn.cu)

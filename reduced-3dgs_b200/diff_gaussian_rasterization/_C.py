@@ -12,7 +12,7 @@ backward, the same value for both) scales each Gaussian's opacity so that the 0.
 scales and rotations, and applies exp / F.normalize / the SH concatenation inside the kernels.  `deterministic` (backward) sums
 the per-Gaussian gradients in a fixed order: the same bytes on every run.  `calculate_colours_variance` and `kmeans_cuda` take the
 same keyword (None: torch's deterministic-algorithms flag) for their statistics and centre sums (the forward request's
-`deterministic`, gsb_kmeans_deterministic).  `features` (forward, also of the variable-SH entry point) composites a [P, F] fp32
+`deterministic`, gsb_kmeans's `deterministic`).  `features` (forward, also of the variable-SH entry point) composites a [P, F] fp32
 tensor of per-Gaussian features over the pairs of the colour image, with background 0, and appends the [F, H, W] image to the
 outputs; the backward's `features` and `dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F].
 `absgrad_out` (backward) takes a [P, 3] fp32 tensor that receives the absolute screen-space gradient.
@@ -401,8 +401,8 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
             req.raw, req.raw_grads = C.pointer(raw_s), C.pointer(rg)
         if deterministic:
             # per-instance partial slots, from the caching allocator on the current stream (freed in stream order after the call)
-            ws_bytes = L.gsb_absgrad_deterministic_workspace_bytes if absgrad_out is not None else L.gsb_deterministic_workspace_bytes
-            det_ws = torch.empty(int(ws_bytes(P, int(R))), dtype=torch.uint8, device=device)
+            ws_bytes = L.gsb_deterministic_workspace_bytes(P, int(R), int(absgrad_out is not None))
+            det_ws = torch.empty(int(ws_bytes), dtype=torch.uint8, device=device)
             req.deterministic, req.det_workspace = 1, ptr(det_ws)
         st = L.gsb_backward(C.byref(req))
         _lib.check(st)
@@ -510,7 +510,7 @@ def allocate_minimum_redundancy_value(redundancy_values, neighbours_indices, int
 def kmeans_cuda(values, centers, tol, max_iterations, *, deterministic=None):
     """reduced_3dgs.h:21-26 Reduced3DGS::kmeans (reduced_3dgs.cu:289-338) -> (ids int32 [n,1], centers float32 [k]).
     `values` is the [n,1] column of one attribute, `centers` the [k] initial centres (gaussian_model.py:36-41).
-    `deterministic`: add each cluster's values in an order fixed by the input (gsb_kmeans_deterministic), the same centres and ids
+    `deterministic`: add each cluster's values in an order fixed by the input (gsb_kmeans's `deterministic`), the same centres and ids
     on every run; None follows torch.are_deterministic_algorithms_enabled() at the call, an explicit bool wins."""
     det = torch.are_deterministic_algorithms_enabled() if deterministic is None else bool(deterministic)
     device = _device_of(values)
@@ -520,12 +520,10 @@ def kmeans_cuda(values, centers, tol, max_iterations, *, deterministic=None):
     n, k = int(values.size(0)), int(centers.size(0))
     ids = torch.zeros((n, 1), dtype=torch.int32, device=device)
     out = torch.empty((k,), dtype=torch.float32, device=device)
-    ws_bytes, run = ((L.gsb_kmeans_deterministic_workspace_bytes, L.gsb_kmeans_deterministic) if det else
-                     (L.gsb_kmeans_workspace_bytes, L.gsb_kmeans))
     with on_device(device):
-        ws = torch.empty(int(ws_bytes(n, k)), dtype=torch.uint8, device=device)
-        _lib.check(run(ptr(v.reshape(-1)) if n else None, n, ptr(c.reshape(-1)), k, float(tol), int(max_iterations),
-                       ptr(ids), out.data_ptr(), ws.data_ptr(), _lib.current_stream(device)))
+        ws = torch.empty(int(L.gsb_kmeans_workspace_bytes(n, k, int(det))), dtype=torch.uint8, device=device)
+        _lib.check(L.gsb_kmeans(ptr(v.reshape(-1)) if n else None, n, ptr(c.reshape(-1)), k, float(tol), int(max_iterations), int(det),
+                                ptr(ids), out.data_ptr(), ws.data_ptr(), _lib.current_stream(device)))
     return ids, out
 
 

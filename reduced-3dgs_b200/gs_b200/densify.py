@@ -91,16 +91,11 @@ def add_densification_stats(model, viewspace_point_tensor, update_filter, radii=
         model.xyz_gradient_accum_abs = torch.zeros((P, 1), device=dev)
     if P == 0:
         return
-    if ga is not None:
-        with gsl.on_device(dev):
-            gsl.check(gsl.lib().gsb_densify_stats_abs(P, g.data_ptr(), g.stride(0), ga.data_ptr(), ga.stride(0), update_filter.data_ptr(),
-                                                       None if radii is None else radii.data_ptr(), accum.data_ptr(),
-                                                       model.xyz_gradient_accum_abs.data_ptr(), denom.data_ptr(),
-                                                       None if mr is None else mr.data_ptr(), gsl.current_stream(dev)))
-        return
     with gsl.on_device(dev):
-        gsl.check(gsl.lib().gsb_densify_stats(P, g.data_ptr(), g.stride(0), update_filter.data_ptr(),
-                                               None if radii is None else radii.data_ptr(), accum.data_ptr(), denom.data_ptr(),
+        gsl.check(gsl.lib().gsb_densify_stats(P, g.data_ptr(), g.stride(0), None if ga is None else ga.data_ptr(),
+                                               0 if ga is None else ga.stride(0), update_filter.data_ptr(),
+                                               None if radii is None else radii.data_ptr(), accum.data_ptr(),
+                                               None if ga is None else model.xyz_gradient_accum_abs.data_ptr(), denom.data_ptr(),
                                                None if mr is None else mr.data_ptr(), gsl.current_stream(dev)))
 
 
@@ -291,20 +286,14 @@ def _plan(model, groups, P, dev, mode, max_grad=0.0, percent_dense=0.0, min_opac
     ws = torch.empty(gsl.lib().gsb_densify_workspace_bytes(P), dtype=torch.uint8, device=dev)
     counts = torch.empty(gsl.DENSIFY_COUNTS, dtype=torch.int64, device=dev)
     screen = bool(max_screen_size)
-    if max_grad_abs is not None:
-        with gsl.on_device(dev):
-            gsl.check(gsl.lib().gsb_densify_plan_abs(
-                P, model.xyz_gradient_accum.data_ptr(), model.xyz_gradient_accum_abs.data_ptr(), model.denom.data_ptr(),
-                param["scaling"].data_ptr(), param["opacity"].data_ptr(), max_grad, max_grad_abs, percent_dense * extent, min_opacity,
-                1 if screen else 0, max_screen_size if screen else 0.0, 0.1 * extent, split_scale_factor(), ws.data_ptr(),
-                counts.data_ptr(), gsl.current_stream(dev)))
-        return [int(v) for v in counts.tolist()], ws, counts
     with gsl.on_device(dev):
         gsl.check(gsl.lib().gsb_densify_plan(
-            P, mode, model.xyz_gradient_accum.data_ptr(), model.denom.data_ptr(), param["scaling"].data_ptr(),
-            param["opacity"].data_ptr(), model.max_radii2D.data_ptr(), None if mask is None else mask.data_ptr(),
-            max_grad, percent_dense * extent, min_opacity, 1 if screen else 0, max_screen_size if screen else 0.0, 0.1 * extent,
-            split_scale_factor(), ws.data_ptr(), counts.data_ptr(), gsl.current_stream(dev)))
+            P, mode, model.xyz_gradient_accum.data_ptr(),
+            None if max_grad_abs is None else model.xyz_gradient_accum_abs.data_ptr(), model.denom.data_ptr(),
+            param["scaling"].data_ptr(), param["opacity"].data_ptr(), model.max_radii2D.data_ptr(),
+            None if mask is None else mask.data_ptr(), max_grad, 0.0 if max_grad_abs is None else max_grad_abs, percent_dense * extent,
+            min_opacity, 1 if screen else 0, max_screen_size if screen else 0.0, 0.1 * extent, split_scale_factor(), ws.data_ptr(),
+            counts.data_ptr(), gsl.current_stream(dev)))
     return [int(v) for v in counts.tolist()], ws, counts
 
 

@@ -110,6 +110,52 @@ DENSIFY_COPY, DENSIFY_XYZ, DENSIFY_SCALING = 0, 1, 2
 MERCY_REDUNDANCY_OPACITY, MERCY_REDUNDANCY_RANDOM, MERCY_OPACITY, MERCY_REDUNDANCY_OPACITY_OPACITY, MERCY_REDUNDANCY = 0, 1, 2, 3, 4
 
 
+# Every exported function: name -> (restype, argtypes), in the order of include/gs_b200.h.  lib() applies the table, so a symbol
+# cannot be declared without its signature.
+_V, _I32, _I64, _F, _SZ = C.c_void_p, C.c_int32, C.c_int64, C.c_float, C.c_size_t
+SIGNATURES = {
+    "gsb_geom_bytes": (_SZ, [_I32]),
+    "gsb_image_bytes": (_SZ, [_I32, _I32]),
+    "gsb_image_bytes_for": (_SZ, [_I32, _I32, _I32, _I32]),
+    "gsb_binning_bytes": (_SZ, [_I64]),
+    "gsb_forward": (C.c_int, [C.POINTER(GsbForwardRequest)]),
+    "gsb_statistics_workspace_bytes": (_SZ, [_I32]),
+    "gsb_backward": (C.c_int, [C.POINTER(GsbBackwardRequest)]),
+    "gsb_camera_grad_workspace_bytes": (_SZ, [_I32]),
+    "gsb_deterministic_workspace_bytes": (_SZ, [_I32, _I64, _I32]),
+    "gsb_mark_visible": (C.c_int, [_I32, _V, _V, _V, _V, _V]),
+    "gsb_export_binning": (C.c_int, [_V, _I32, _V, _I64, _V, _I32, _I32, _V, _V, _V]),
+    "gsb_export_image": (C.c_int, [_V, _I32, _I32, _V, _V, _V, _V]),
+    "gsb_debug_dequant": (C.c_int, [C.POINTER(GsbQuant), _I32, _V, _V, _V]),
+    "gsb_sh_statistics_update": (C.c_int, [_I32, _I32] + [_V] * 13),
+    "gsb_min_projected_pixel_size": (C.c_int, [_I32, _V, _I32, _V, _V, _V, _V, _V, _V]),
+    "gsb_sphere_ellipsoid_intersection": (C.c_int, [_I32, _V, _V, _V, _V, _V, _I32, _V, _V, _V]),
+    "gsb_min_redundancy_value": (C.c_int, [_I32, _V, _V, _V, _I32, _V, _V]),
+    "gsb_kmeans_workspace_bytes": (_SZ, [_I64, _I32, _I32]),
+    "gsb_kmeans": (C.c_int, [_V, _I64, _V, _I32, _F, _I32, _I32, _V, _V, _V, _V]),
+    "gsb_knn_workspace_bytes": (_SZ, [_I32, _I32]),
+    "gsb_knn": (C.c_int, [_V, _I32, _I32, _V, _I32, _V, _I32, _V, _V, _V, _V, _V]),
+    "gsb_l1_ssim_blocks": (C.c_int64, [_I32, _I32, _I32]),
+    "gsb_l1_ssim_forward": (C.c_int, [_V, _V, _I32, _I32, _I32, _V, _V, _V]),
+    "gsb_l1_ssim_backward": (C.c_int, [_V, _V, _I32, _I32, _I32, _V, _F, _V, _F, _V, _V, _V]),
+    "gsb_adam_step": (C.c_int, [C.POINTER(GsbAdamTensor), _I32, _I32, _V, _V, _V]),
+    "gsb_densify_stats": (C.c_int, [_I32, _V, _I32, _V, _I32] + [_V] * 7),
+    "gsb_densify_workspace_bytes": (_SZ, [_I32]),
+    "gsb_densify_split_std_offset": (_SZ, [_I32]),
+    "gsb_densify_plan": (C.c_int, [_I32, _I32] + [_V] * 7 + [_F] * 4 + [_I32] + [_F] * 3 + [_V] * 3),
+    "gsb_densify_emit": (C.c_int, [C.POINTER(GsbDensifyTensor), _I32, _I32, _V] + [_I64] * 4 + [_V, _V, _F, _V]),
+    "gsb_redundancy_workspace_bytes": (_SZ, [_I32, _I32]),
+    "gsb_redundancy_score": (C.c_int, [_I32, _V, _V, _V, _I32, _V, _V, _V, _V, _F, _I32, _V, _V, _V, _V]),
+    "gsb_mercy_workspace_bytes": (_SZ, [_I32]),
+    "gsb_mercy_plan": (C.c_int, [_I32, _V, _V, _I32, _F, C.c_double, _F, _V, _I64, _V, _V, _V, _V, _V]),
+    "gsb_launch_count": (C.c_uint64, []),
+    "gsb_profile_enable": (None, [C.c_int]),
+    "gsb_profile_read": (C.c_int, [C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
+    "gsb_last_error": (C.c_char_p, []),
+    "gsb_version": (C.c_char_p, []),
+}
+EXPORTED_SYMBOLS = list(SIGNATURES)
+
 _lib = None
 
 
@@ -138,103 +184,9 @@ def lib():
             raise RuntimeError(f"gs_b200: CUDA library {path} is missing — build it with reduced-3dgs_b200/csrc/build.py "
                                "(there is no CPU / PyTorch fallback)")
         L = C.CDLL(path)
-        L.gsb_geom_bytes.restype = C.c_size_t
-        L.gsb_geom_bytes.argtypes = [C.c_int32]
-        L.gsb_image_bytes.restype = C.c_size_t
-        L.gsb_image_bytes.argtypes = [C.c_int32, C.c_int32]
-        L.gsb_image_bytes_for.restype = C.c_size_t
-        L.gsb_image_bytes_for.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32]
-        L.gsb_binning_bytes.restype = C.c_size_t
-        L.gsb_binning_bytes.argtypes = [C.c_int64]
-        L.gsb_launch_count.restype = C.c_uint64
-        L.gsb_last_error.restype = C.c_char_p
-        L.gsb_version.restype = C.c_char_p
-        L.gsb_forward.restype = C.c_int
-        L.gsb_forward.argtypes = [C.POINTER(GsbForwardRequest)]
-        L.gsb_statistics_workspace_bytes.restype = C.c_size_t
-        L.gsb_statistics_workspace_bytes.argtypes = [C.c_int32]
-        L.gsb_sh_statistics_update.restype = C.c_int
-        L.gsb_sh_statistics_update.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 13
-        L.gsb_min_projected_pixel_size.restype = C.c_int
-        L.gsb_min_projected_pixel_size.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                                   C.c_void_p, C.c_void_p]
-        L.gsb_sphere_ellipsoid_intersection.restype = C.c_int
-        L.gsb_sphere_ellipsoid_intersection.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
-                                                        C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_min_redundancy_value.restype = C.c_int
-        L.gsb_min_redundancy_value.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
-        L.gsb_kmeans_workspace_bytes.restype = C.c_size_t
-        L.gsb_kmeans_workspace_bytes.argtypes = [C.c_int64, C.c_int32]
-        L.gsb_kmeans.restype = C.c_int
-        L.gsb_kmeans.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                 C.c_void_p]
-        L.gsb_kmeans_deterministic_workspace_bytes.restype = C.c_size_t
-        L.gsb_kmeans_deterministic_workspace_bytes.argtypes = [C.c_int64, C.c_int32]
-        L.gsb_kmeans_deterministic.restype = C.c_int
-        L.gsb_kmeans_deterministic.argtypes = L.gsb_kmeans.argtypes
-        L.gsb_knn_workspace_bytes.restype = C.c_size_t
-        L.gsb_knn_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
-        L.gsb_knn.restype = C.c_int
-        L.gsb_knn.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
-                              C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_l1_ssim_blocks.restype = C.c_int64
-        L.gsb_l1_ssim_blocks.argtypes = [C.c_int32, C.c_int32, C.c_int32]
-        L.gsb_l1_ssim_forward.restype = C.c_int
-        L.gsb_l1_ssim_forward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_l1_ssim_backward.restype = C.c_int
-        L.gsb_l1_ssim_backward.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_float, C.c_void_p,
-                                           C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_backward.restype = C.c_int
-        L.gsb_backward.argtypes = [C.POINTER(GsbBackwardRequest)]
-        L.gsb_camera_grad_workspace_bytes.restype = C.c_size_t
-        L.gsb_camera_grad_workspace_bytes.argtypes = [C.c_int32]
-        L.gsb_deterministic_workspace_bytes.restype = C.c_size_t
-        L.gsb_deterministic_workspace_bytes.argtypes = [C.c_int32, C.c_int64]
-        L.gsb_absgrad_deterministic_workspace_bytes.restype = C.c_size_t
-        L.gsb_absgrad_deterministic_workspace_bytes.argtypes = [C.c_int32, C.c_int64]
-        L.gsb_mark_visible.restype = C.c_int
-        L.gsb_mark_visible.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_export_binning.restype = C.c_int
-        L.gsb_export_binning.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32,
-                                         C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_export_image.restype = C.c_int
-        L.gsb_export_image.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_debug_dequant.restype = C.c_int
-        L.gsb_debug_dequant.argtypes = [C.POINTER(GsbQuant), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_adam_step.restype = C.c_int
-        L.gsb_adam_step.argtypes = [C.POINTER(GsbAdamTensor), C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_densify_stats.restype = C.c_int
-        L.gsb_densify_stats.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
-                                        C.c_void_p]
-        L.gsb_densify_workspace_bytes.restype = C.c_size_t
-        L.gsb_densify_workspace_bytes.argtypes = [C.c_int32]
-        L.gsb_densify_split_std_offset.restype = C.c_size_t
-        L.gsb_densify_split_std_offset.argtypes = [C.c_int32]
-        L.gsb_densify_plan.restype = C.c_int
-        L.gsb_densify_plan.argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.c_float] * 3 + [C.c_int32] + [C.c_float] * 3 + \
-            [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_densify_stats_abs.restype = C.c_int
-        L.gsb_densify_stats_abs.argtypes = [C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_int32] + [C.c_void_p] * 7
-        L.gsb_densify_plan_abs.restype = C.c_int
-        L.gsb_densify_plan_abs.argtypes = [C.c_int32] + [C.c_void_p] * 5 + [C.c_float] * 4 + [C.c_int32] + [C.c_float] * 3 + \
-            [C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_densify_emit.restype = C.c_int
-        L.gsb_densify_emit.argtypes = [C.POINTER(GsbDensifyTensor), C.c_int32, C.c_int32, C.c_void_p] + [C.c_int64] * 4 + \
-            [C.c_void_p, C.c_void_p, C.c_float, C.c_void_p]
-        L.gsb_redundancy_workspace_bytes.restype = C.c_size_t
-        L.gsb_redundancy_workspace_bytes.argtypes = [C.c_int32, C.c_int32]
-        L.gsb_redundancy_score.restype = C.c_int
-        L.gsb_redundancy_score.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
-                                           C.c_void_p, C.c_float, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_mercy_workspace_bytes.restype = C.c_size_t
-        L.gsb_mercy_workspace_bytes.argtypes = [C.c_int32]
-        L.gsb_mercy_plan.restype = C.c_int
-        L.gsb_mercy_plan.argtypes = [C.c_int32, C.c_void_p, C.c_void_p, C.c_int32, C.c_float, C.c_double, C.c_float, C.c_void_p,
-                                     C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
-        L.gsb_profile_enable.restype = None
-        L.gsb_profile_enable.argtypes = [C.c_int]
-        L.gsb_profile_read.restype = C.c_int
-        L.gsb_profile_read.argtypes = [C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_double), C.POINTER(C.c_uint64)]
+        for name, (restype, argtypes) in SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype, fn.argtypes = restype, argtypes
         _lib = L
     return _lib
 
@@ -251,20 +203,6 @@ def profile_read() -> dict:
     cnt = (C.c_uint64 * n)()
     k = lib().gsb_profile_read(n, names, ms, cnt)
     return {names[i].decode(): (float(ms[i]), int(cnt[i])) for i in range(k)}
-
-
-EXPORTED_SYMBOLS = ["gsb_geom_bytes", "gsb_image_bytes", "gsb_image_bytes_for", "gsb_binning_bytes", "gsb_forward", "gsb_backward",
-                    "gsb_mark_visible", "gsb_export_binning", "gsb_export_image", "gsb_launch_count", "gsb_last_error",
-                    "gsb_version", "gsb_profile_enable", "gsb_profile_read", "gsb_debug_dequant",
-                    "gsb_sh_statistics_update", "gsb_min_projected_pixel_size", "gsb_sphere_ellipsoid_intersection",
-                    "gsb_min_redundancy_value", "gsb_kmeans_workspace_bytes", "gsb_kmeans", "gsb_l1_ssim_blocks",
-                    "gsb_l1_ssim_forward", "gsb_l1_ssim_backward", "gsb_knn_workspace_bytes", "gsb_knn",
-                    "gsb_camera_grad_workspace_bytes", "gsb_adam_step", "gsb_densify_stats",
-                    "gsb_densify_workspace_bytes", "gsb_densify_split_std_offset", "gsb_densify_plan", "gsb_densify_emit",
-                    "gsb_deterministic_workspace_bytes", "gsb_statistics_workspace_bytes",
-                    "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic", "gsb_redundancy_workspace_bytes",
-                    "gsb_redundancy_score", "gsb_mercy_workspace_bytes", "gsb_mercy_plan",
-                    "gsb_absgrad_deterministic_workspace_bytes", "gsb_densify_stats_abs", "gsb_densify_plan_abs"]
 
 
 def check(status: int):

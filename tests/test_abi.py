@@ -72,8 +72,8 @@ def test_argument_validation_needs_no_gpu():
     assert st < 0
     assert L.gsb_mark_visible(-1, None, None, None, None, None) < 0
     assert L.gsb_mark_visible(5, None, None, None, None, None) < 0
-    assert L.gsb_kmeans(None, 10, None, 256, 0.1, 5, None, None, None, None) < 0 and b"kmeans" in L.gsb_last_error()
-    assert L.gsb_kmeans(None, -1, None, 256, 0.1, 5, None, None, None, None) < 0
+    assert L.gsb_kmeans(None, 10, None, 256, 0.1, 5, 0, None, None, None, None) < 0 and b"kmeans" in L.gsb_last_error()
+    assert L.gsb_kmeans(None, -1, None, 256, 0.1, 5, 0, None, None, None, None) < 0
     assert L.gsb_sphere_ellipsoid_intersection(-3, None, None, None, None, None, 4, None, None, None) < 0
     assert L.gsb_min_projected_pixel_size(7, None, 1, None, None, None, None, None, None) < 0
     assert L.gsb_min_redundancy_value(7, None, None, None, 4, None, None) < 0
@@ -82,7 +82,7 @@ def test_argument_validation_needs_no_gpu():
     assert L.gsb_l1_ssim_backward(None, None, 3, 8, 8, None, 1.0, None, 1.0, None, None, None) < 0
     assert L.gsb_forward(C.byref(lib.GsbForwardRequest(geom_alloc=cb, binning_alloc=cb, image_alloc=cb, num_rendered=C.pointer(R)))) < 0
     # size helpers are monotone and include the per-kind fixed parts
-    assert L.gsb_kmeans_workspace_bytes(10 ** 6, 256) > 8 * 10 ** 6
+    assert L.gsb_kmeans_workspace_bytes(10 ** 6, 256, 0) > 8 * 10 ** 6
     assert L.gsb_l1_ssim_blocks(3, 1080, 1920) == 3 * 68 * 120
 
 

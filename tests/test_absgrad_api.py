@@ -1,5 +1,5 @@
 """CPU: the absolute screen-space gradient (DESIGN.md §5m).  The backward request with dL_dmeans2D_abs, its workspace size,
-gsb_densify_stats_abs and gsb_densify_plan_abs reject each bad argument before any CUDA call; the Python layer refuses what has no
+gsb_densify_stats and gsb_densify_plan with their absolute-gradient arguments reject each bad argument before any CUDA call; the Python layer refuses what has no
 absgrad form before anything runs and, against stand-in kernels, carries `absgrad` through both autograd ops and render() while
 leaving the calls without it exactly as they were; and the float64 restatement of the per-pair terms (absgrad64.py) sums, with
 signs, to the fp64 oracle's dL_dmeans2D on the backward-edge scenes, which pins it to the pairs and terms the oracle uses."""
@@ -15,7 +15,7 @@ import backward_edges as BE
 import stub_c
 from gs_b200 import lib
 
-NEW = ("gsb_backward", "gsb_absgrad_deterministic_workspace_bytes", "gsb_densify_stats_abs", "gsb_densify_plan_abs")
+NEW = ("gsb_backward", "gsb_deterministic_workspace_bytes", "gsb_densify_stats", "gsb_densify_plan")
 
 
 def test_symbols_exported():
@@ -28,10 +28,10 @@ def test_symbols_exported():
 def test_workspace_grows_and_adds_eight_bytes_per_instance():
     L = lib.lib()
     for P, R in ((0, 0), (1, 1), (1000, 5000), (100_000, 3_000_000)):
-        base, ab = int(L.gsb_deterministic_workspace_bytes(P, R)), int(L.gsb_absgrad_deterministic_workspace_bytes(P, R))
+        base, ab = int(L.gsb_deterministic_workspace_bytes(P, R, 0)), int(L.gsb_deterministic_workspace_bytes(P, R, 1))
         assert ab >= base + 8 * R
-    assert L.gsb_absgrad_deterministic_workspace_bytes(1000, 10) < L.gsb_absgrad_deterministic_workspace_bytes(1000, 11_000)
-    assert L.gsb_absgrad_deterministic_workspace_bytes(1000, 10) < L.gsb_absgrad_deterministic_workspace_bytes(100_000, 10)
+    assert L.gsb_deterministic_workspace_bytes(1000, 10, 1) < L.gsb_deterministic_workspace_bytes(1000, 11_000, 1)
+    assert L.gsb_deterministic_workspace_bytes(1000, 10, 1) < L.gsb_deterministic_workspace_bytes(100_000, 10, 1)
 
 
 def _bwd(L, scene, R=5, grads=None, out=True, det_ws=None, raw=None, raw_grads=None, cam_out=None, workspace=None, features=None):
@@ -70,17 +70,23 @@ def test_densify_abs_entry_points_reject_bad_arguments():
     L = lib.lib()
     b = (C.c_float * 64)()
     p = C.addressof(b)
-    assert L.gsb_densify_stats_abs(-1, p, 3, p, 3, p, None, p, p, p, None, None) == -1 and b"P < 0" in L.gsb_last_error()
-    assert L.gsb_densify_stats_abs(4, p, 3, p, 1, p, None, p, p, p, None, None) == -1 and b">= 2" in L.gsb_last_error()
-    assert L.gsb_densify_stats_abs(4, p, 3, p, 3, p, p, p, p, p, None, None) == -1 and b"without max_radii2D" in L.gsb_last_error()
-    assert L.gsb_densify_stats_abs(4, p, 3, None, 3, p, None, p, p, p, None, None) == -1 and b"NULL" in L.gsb_last_error()
-    assert L.gsb_densify_stats_abs(4, p, 3, p, 3, p, None, p, None, p, None, None) == -1 and b"NULL" in L.gsb_last_error()
-    assert L.gsb_densify_stats_abs(0, None, 3, None, 3, None, None, None, None, None, None, None) == 0
+    assert L.gsb_densify_stats(-1, p, 3, p, 3, p, None, p, p, p, None, None) == -1 and b"P < 0" in L.gsb_last_error()
+    assert L.gsb_densify_stats(4, p, 3, p, 1, p, None, p, p, p, None, None) == -1 and b">= 2" in L.gsb_last_error()
+    assert L.gsb_densify_stats(4, p, 3, p, 3, p, p, p, p, p, None, None) == -1 and b"without max_radii2D" in L.gsb_last_error()
+    assert L.gsb_densify_stats(4, p, 3, None, 3, p, None, p, p, p, None, None) == -1 and b"NULL" in L.gsb_last_error()
+    assert L.gsb_densify_stats(4, p, 3, p, 3, p, None, p, None, p, None, None) == -1 and b"NULL" in L.gsb_last_error()
+    assert L.gsb_densify_stats(0, None, 3, None, 3, None, None, None, None, None, None, None) == 0
+    # one of the pair without the other is refused at any P
+    for ga, acc_abs in ((p, None), (None, p)):
+        assert L.gsb_densify_stats(0, None, 3, ga, 3, None, None, None, acc_abs, None, None, None) == -1 and b"both" in L.gsb_last_error()
     cnt = (C.c_int64 * 8)()
-    args = lambda P, acc_abs, ws=p: (P, p, acc_abs, p, p, p, 0.1, 0.2, 0.01, 0.005, 0, 0.0, 1.0, 0.625, ws, C.addressof(cnt), None)
-    assert L.gsb_densify_plan_abs(*args(4, None)) == -1 and b"xyz_gradient_accum_abs" in L.gsb_last_error()
-    assert L.gsb_densify_plan_abs(*args(4, p, None)) == -1 and b"workspace" in L.gsb_last_error()
-    assert L.gsb_densify_plan_abs(*args(-1, p)) == -1 and b"outside" in L.gsb_last_error()
+    args = lambda P, acc_abs, ws=p, mode=lib.DENSIFY_CLONE_SPLIT: (P, mode, p, acc_abs, p, p, p, None, None, 0.1, 0.2, 0.01, 0.005, 0,
+                                                                   0.0, 1.0, 0.625, ws, C.addressof(cnt), None)
+    # the absolute accumulator selects the AbsGS split test, which only the clone / split mode has
+    for mode in (lib.DENSIFY_PRUNE, lib.DENSIFY_PRUNE_MASK):
+        assert L.gsb_densify_plan(*args(4, p, mode=mode)) == -1 and b"xyz_gradient_accum_abs" in L.gsb_last_error()
+    assert L.gsb_densify_plan(*args(4, p, None)) == -1 and b"workspace" in L.gsb_last_error()
+    assert L.gsb_densify_plan(*args(-1, p)) == -1 and b"outside" in L.gsb_last_error()
 
 
 # ---- Python refusals ---------------------------------------------------------------------------------------------------------------

@@ -54,13 +54,15 @@ def test_einval():
     L = gsl.lib()
     fake = C.c_void_p(256)
     E = -1
-    assert L.gsb_densify_stats(-1, None, 3, None, None, None, None, None, None) == E
-    assert L.gsb_densify_stats(10, fake, 1, fake, None, fake, fake, None, None) == E            # stride < 2
-    assert L.gsb_densify_stats(10, None, 3, fake, None, fake, fake, None, None) == E            # NULL grad
-    assert L.gsb_densify_stats(10, fake, 3, fake, fake, fake, fake, None, None) == E            # radii without max_radii2D
-    assert L.gsb_densify_stats(0, None, 3, None, None, None, None, None, None) == 0
+    stats = lambda P, grad, stride, vis, radii, accum, denom, max_radii2D: L.gsb_densify_stats(  # noqa: E731
+        P, grad, stride, None, 0, vis, radii, accum, None, denom, max_radii2D, None)                # without the AbsGS pair
+    assert stats(-1, None, 3, None, None, None, None, None) == E
+    assert stats(10, fake, 1, fake, None, fake, fake, None) == E                                # stride < 2
+    assert stats(10, None, 3, fake, None, fake, fake, None) == E                                # NULL grad
+    assert stats(10, fake, 3, fake, fake, fake, fake, None) == E                                # radii without max_radii2D
+    assert stats(0, None, 3, None, None, None, None, None) == 0
     plan = lambda P, mode, ws=fake, counts=fake, mask=None: L.gsb_densify_plan(  # noqa: E731
-        P, mode, fake, fake, fake, fake, fake, mask, 0.0, 1.0, 0.005, 0, 0.0, 10.0, 0.625, ws, counts, None)
+        P, mode, fake, None, fake, fake, fake, fake, mask, 0.0, 0.0, 1.0, 0.005, 0, 0.0, 10.0, 0.625, ws, counts, None)
     assert plan(-1, 0) == E
     assert plan(1 << 30, 0) == E
     assert plan(10, 3) == E
@@ -203,9 +205,10 @@ def test_host_thresholds_and_state_rekeying(monkeypatch):
     # the ctypes float fields hold the fp32 casts of the reference's double products
     f = lambda x: float(np.float32(x))  # noqa: E731
     assert a[1] == gsl.DENSIFY_CLONE_SPLIT
-    argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 6 + [C.c_float] * 3 + [C.c_int32] + [C.c_float] * 3
-    vals = [t(v).value for t, v in zip(argtypes[8:], a[8:15])]
-    assert vals == [f(0.0002), f(pd * extent), f(0.005), 1, f(20), f(0.1 * extent), f(1.0 / f(0.8 * 2))]
+    argtypes = [C.c_int32, C.c_int32] + [C.c_void_p] * 7 + [C.c_float] * 4 + [C.c_int32] + [C.c_float] * 3
+    vals = [t(v).value for t, v in zip(argtypes[9:], a[9:17])]
+    assert vals == [f(0.0002), 0.0, f(pd * extent), f(0.005), 1, f(20), f(0.1 * extent), f(1.0 / f(0.8 * 2))]
+    assert a[3] is None                                                   # no xyz_gradient_accum_abs: the reference's split test
     for g in m.optimizer.param_groups:
         p = g["params"][0]
         if g["name"] in states:

@@ -28,9 +28,9 @@ def test_symbols_are_exported():
 def test_workspace_size():
     L = lib.lib()
     for P, R in ((0, 0), (1, 1), (1000, 5000), (10 ** 6, 7 * 10 ** 6), (3 * 10 ** 6, 4 * 10 ** 7)):
-        assert L.gsb_deterministic_workspace_bytes(P, R) >= P * 4 + R * 36
-    assert L.gsb_deterministic_workspace_bytes(2000, 5000) > L.gsb_deterministic_workspace_bytes(1000, 5000)
-    assert L.gsb_deterministic_workspace_bytes(1000, 6000) > L.gsb_deterministic_workspace_bytes(1000, 5000)
+        assert L.gsb_deterministic_workspace_bytes(P, R, 0) >= P * 4 + R * 36
+    assert L.gsb_deterministic_workspace_bytes(2000, 5000, 0) > L.gsb_deterministic_workspace_bytes(1000, 5000, 0)
+    assert L.gsb_deterministic_workspace_bytes(1000, 6000, 0) > L.gsb_deterministic_workspace_bytes(1000, 5000, 0)
 
 
 def _bwd(L, scene, R=0, ws=None, det_ws=None, cam_out=(None, None, None), raw=None, raw_grads=None, grads=None):

@@ -1,5 +1,5 @@
 """CPU: the deterministic SH-culling statistics and k-means (a statistics forward request with `deterministic`,
-gsb_kmeans_deterministic):
+gsb_kmeans with `deterministic`):
 exports, workspace sizes, every refused argument (checked before any CUDA call), the `deterministic` keyword of
 `_C.calculate_colours_variance` / `_C.kmeans_cuda` against a stub library, and the float32 restatement of the k-means summation
 order (oracle/kmeans_det_order.py) on hand-made cases."""
@@ -17,7 +17,7 @@ from gs_b200 import lib
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle"))
 import kmeans_det_order as kdo  # noqa: E402
 
-NEW_SYMBOLS = ("gsb_statistics_workspace_bytes", "gsb_forward", "gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic")
+NEW_SYMBOLS = ("gsb_statistics_workspace_bytes", "gsb_forward", "gsb_kmeans_workspace_bytes", "gsb_kmeans")
 
 
 @pytest.fixture
@@ -40,10 +40,10 @@ def test_workspace_sizes():
         assert L.gsb_statistics_workspace_bytes(P) >= 8 * P
     assert L.gsb_statistics_workspace_bytes(2000) > L.gsb_statistics_workspace_bytes(1000)
     for n, K in ((0, 1), (1, 1), (4095, 256), (4097, 256), (9 * 10 ** 6, 256), (9 * 10 ** 6, 1024)):
-        assert L.gsb_kmeans_deterministic_workspace_bytes(n, K) >= 8 * n
-        assert L.gsb_kmeans_deterministic_workspace_bytes(n, K) >= L.gsb_kmeans_workspace_bytes(n, K)
-    assert L.gsb_kmeans_deterministic_workspace_bytes(2 * 10 ** 6, 256) > L.gsb_kmeans_deterministic_workspace_bytes(10 ** 6, 256)
-    assert L.gsb_kmeans_deterministic_workspace_bytes(10 ** 6, 1024) > L.gsb_kmeans_deterministic_workspace_bytes(10 ** 6, 256)
+        assert L.gsb_kmeans_workspace_bytes(n, K, 1) >= 8 * n
+        assert L.gsb_kmeans_workspace_bytes(n, K, 1) >= L.gsb_kmeans_workspace_bytes(n, K, 0)
+    assert L.gsb_kmeans_workspace_bytes(2 * 10 ** 6, 256, 1) > L.gsb_kmeans_workspace_bytes(10 ** 6, 256, 1)
+    assert L.gsb_kmeans_workspace_bytes(10 ** 6, 1024, 1) > L.gsb_kmeans_workspace_bytes(10 ** 6, 256, 1)
 
 
 def _stats(L, scene, cam=None, outs=True, ws=None):
@@ -76,8 +76,8 @@ def test_statistics_deterministic_rejects_bad_arguments():
 def _km(L, n=10, K=4, max_it=5, values=True, centers=True, ids=True, out=True, ws=True, ws_off=0):
     buf = (C.c_float * 64)()
     a = C.addressof(buf)
-    return L.gsb_kmeans_deterministic(a if values else None, n, a if centers else None, K, 1e-4, max_it, a if ids else None,
-                                      a if out else None, (a + ws_off) if ws else None, None)
+    return L.gsb_kmeans(a if values else None, n, a if centers else None, K, 1e-4, max_it, 1, a if ids else None, a if out else None,
+                        (a + ws_off) if ws else None, None)
 
 
 def test_kmeans_deterministic_rejects_bad_arguments():
@@ -197,6 +197,12 @@ def _names(calls):
     return [n for n, _ in calls]
 
 
+def _kmeans_run(monkeypatch, **kw):
+    """The name of kmeans_cuda's last library call and the `deterministic` argument it passed."""
+    name, args = _kmeans_calls(monkeypatch, **kw)[-1]
+    return name, args[6]
+
+
 def test_flag_off_keeps_the_old_calls(monkeypatch, torch_deterministic):
     torch.use_deterministic_algorithms(False)
     col = _colour_calls(monkeypatch)
@@ -210,8 +216,8 @@ def test_flag_off_keeps_the_old_calls(monkeypatch, torch_deterministic):
     assert all(not fwd[k] for k in ("debug", "out_invdepth", "out_alpha", "antialiasing", "raw", "deterministic", "workspace", "features"))
     km = _kmeans_calls(monkeypatch)
     assert _names(km) == ["gsb_kmeans_workspace_bytes", "gsb_kmeans"]
-    assert km[0][1] == (100, 8)
-    assert km[1][1] == ("values", 100, "centers", 8, pytest.approx(1e-4), 500, "fresh0", "fresh1", "fresh2", 0)
+    assert km[0][1] == (100, 8, 0)
+    assert km[1][1] == ("values", 100, "centers", 8, pytest.approx(1e-4), 500, 0, "fresh0", "fresh1", "fresh2", 0)
     assert km == _kmeans_calls(monkeypatch, deterministic=False)
 
 
@@ -232,25 +238,26 @@ def test_torch_flag_selects_the_deterministic_paths(monkeypatch, torch_determini
     assert len(reqs) == 2 and reqs[0].workspace and reqs[0].workspace == reqs[1].workspace
     torch.use_deterministic_algorithms(True)
     km = _kmeans_calls(monkeypatch)
-    assert _names(km) == ["gsb_kmeans_deterministic_workspace_bytes", "gsb_kmeans_deterministic"]
-    assert km[1][1] == ("values", 100, "centers", 8, pytest.approx(1e-4), 500, "fresh0", "fresh1", "fresh2", 0)
+    assert _names(km) == ["gsb_kmeans_workspace_bytes", "gsb_kmeans"]
+    assert km[0][1] == (100, 8, 1)
+    assert km[1][1] == ("values", 100, "centers", 8, pytest.approx(1e-4), 500, 1, "fresh0", "fresh1", "fresh2", 0)
 
 
 def test_flag_is_read_at_call_time(monkeypatch, torch_deterministic):
     torch.use_deterministic_algorithms(False)
-    assert _names(_kmeans_calls(monkeypatch))[-1] == "gsb_kmeans"
+    assert _kmeans_run(monkeypatch) == ("gsb_kmeans", 0)
     torch.use_deterministic_algorithms(True)
-    assert _names(_kmeans_calls(monkeypatch))[-1] == "gsb_kmeans_deterministic"
+    assert _kmeans_run(monkeypatch) == ("gsb_kmeans", 1)
     torch.use_deterministic_algorithms(False)
     assert _deterministic(monkeypatch) == 0
 
 
 def test_explicit_bool_wins(monkeypatch, torch_deterministic):
     torch.use_deterministic_algorithms(True)
-    assert _names(_kmeans_calls(monkeypatch, deterministic=False))[-1] == "gsb_kmeans"
+    assert _kmeans_run(monkeypatch, deterministic=False) == ("gsb_kmeans", 0)
     assert _deterministic(monkeypatch, deterministic=False) == 0
     torch.use_deterministic_algorithms(False)
-    assert _names(_kmeans_calls(monkeypatch, deterministic=True))[-1] == "gsb_kmeans_deterministic"
+    assert _kmeans_run(monkeypatch, deterministic=True) == ("gsb_kmeans", 1)
     assert _deterministic(monkeypatch, deterministic=True) == 1
 
 

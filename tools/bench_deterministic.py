@@ -40,7 +40,7 @@ def main():
         for k in arms:
             med = statistics.median(times[k])
             print(json.dumps({"workload": name, "arm": k, "P": P, "R": R,
-                              "det_workspace_bytes": int(L.gsb_deterministic_workspace_bytes(P, R)) if k == "deterministic" else 0,
+                              "det_workspace_bytes": int(L.gsb_deterministic_workspace_bytes(P, R, 0)) if k == "deterministic" else 0,
                               "fwd_bwd_ms_median": round(med, 4), "ratio_to_default": round(med / base, 4),
                               "kernels_ms": kernels[k]}), flush=True)
 
