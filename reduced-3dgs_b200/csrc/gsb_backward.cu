@@ -24,6 +24,10 @@ struct BwdArgs {
 	// _rotation and out.dL_dscales / dL_drotations receive their gradients; the SH rows come from _features_dc / _features_rest
 	// and their gradients go to dL_ddc / dL_drest (either may be NULL: not written); raw_vec4: every SH pointer is 16-byte aligned
 	const float* sh_dc; const float* sh_rest; float* dL_ddc; float* dL_drest; int n_rest; int raw_vec4;
+	// 16-byte alignment of the caller's SH pointers (a contiguous view may start at any float): shs for the M == 16 staging, dL_dsh
+	// (an accumulate_into tensor) for its write-back; the scalar loops take the others.  Rotations are read as one float4: the
+	// Python layer hands over 16-byte aligned rows (lib.aligned16)
+	int sh_vec4, dsh_vec4;
 };
 
 // Camera gradient slots (CAM): 0..11 view[4r+c] (r = 0..3, c = 0..2) at 3r+c; 12..23 proj[4r+j] (j = 0, 1, 3) at 12+3r+{0,1,2};
@@ -172,7 +176,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				if (a.n_rest) raw_block<false, ACC>(a.sh_rest, nullptr, 3 * a.n_rest, 3, base, n_valid, s_row, RS, lane, true, a.raw_vec4);
 			}
 		}
-		else if (have_sh && !QUANT && RL == 48 && n_valid == 32)
+		else if (have_sh && !QUANT && RL == 48 && n_valid == 32 && a.sh_vec4)
 		{
 			// M == 16 fast path: 12 independent 128-bit loads per lane (6 KB contiguous per warp), then scatter to padded rows
 			const float4* src4 = reinterpret_cast<const float4*>(a.shs + base * 48);
@@ -508,7 +512,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 			if (a.dL_drest && a.n_rest)
 				raw_block<true, ACC>(nullptr, a.dL_drest, 3 * a.n_rest, 3, base, n_valid, s_row, RS, lane, have_sh, a.raw_vec4);
 		}
-		else if (a.out.dL_dsh && RL == 48 && n_valid == 32)
+		else if (a.out.dL_dsh && RL == 48 && n_valid == 32 && a.dsh_vec4)
 		{
 			float4* dst4 = reinterpret_cast<float4*>(a.out.dL_dsh + base * 48);
 #pragma unroll
@@ -646,6 +650,7 @@ int launch_preprocess_backward(const GsbBackwardRequest& req, const GeomState& g
 	a.view = cam->viewmatrix; a.proj = cam->projmatrix; a.campos = cam->campos;
 	a.quant = s->quant != nullptr; if (s->quant) a.q = *s->quant;
 	a.g = g; a.acc = acc; a.out = *req.grads; a.cam_rows = want_cam(req) ? reinterpret_cast<float*>(req.camera_workspace) : nullptr;
+	auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
 	if (raw)
 	{
 		a.M = raw->features_dc && !s->colors_precomp ? 1 + raw->C : 0;
@@ -653,9 +658,9 @@ int launch_preprocess_backward(const GsbBackwardRequest& req, const GeomState& g
 		a.sh_dc = s->colors_precomp ? nullptr : raw->features_dc; a.sh_rest = raw->features_rest; a.n_rest = raw->C;
 		a.out.dL_dscales = req.raw_grads->dL_dscaling; a.out.dL_drotations = req.raw_grads->dL_drotation;
 		a.dL_ddc = req.raw_grads->dL_dfeatures_dc; a.dL_drest = req.raw_grads->dL_dfeatures_rest;
-		auto al = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
 		a.raw_vec4 = al(a.sh_dc) && al(a.sh_rest) && al(a.dL_ddc) && al(a.dL_drest);
 	}
+	a.sh_vec4 = al(a.shs); a.dsh_vec4 = al(a.out.dL_dsh);
 	const int grid = preprocess_backward_grid(s->P);
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * a.M + 1) + 32 * 6) * sizeof(float);
 	const cudaStream_t stream = stream_of(req);

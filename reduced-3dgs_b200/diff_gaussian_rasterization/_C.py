@@ -116,8 +116,9 @@ def _present(t):
 
 def _raw_struct(raw, device, P, want_sh, sh, scales, rotations, cov3D_precomp, quant):
     """raw = (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]): the model's leaf tensors, passed by
-    pointer as they are (no copy, no cast), so each must already be a contiguous fp32 tensor on the device.  Everything is
-    checked before anything is launched.  -> (GsbRawParams, C)."""
+    pointer as they are (no cast), so each must already be a contiguous fp32 tensor on the device; only a rotation that does not
+    start on a 16-byte boundary is copied (lib.aligned16: the kernels read its rows as one float4).  Everything is checked before
+    anything is launched.  -> (GsbRawParams, C, the rotation tensor handed over, to keep alive for the call)."""
     if quant is not None:
         raise RuntimeError("raw parameters: a quantised model has no raw fp32 parameters (its kernels activate the codebooks already)")
     if any(_present(t) for t in (sh, scales, rotations, cov3D_precomp)):
@@ -159,7 +160,8 @@ def _raw_struct(raw, device, P, want_sh, sh, scales, rotations, cov3D_precomp, q
     for name, t in checked:
         if not t.is_cuda or t.device != device:
             raise RuntimeError(f"raw parameters: {name} must live on {device}, got {t.device}")
-    return GsbRawParams(ptr(dc) if want_sh else None, ptr(rest) if want_sh else None, C_rest, ptr(scaling), ptr(rotation)), C_rest
+    rotation = _lib.aligned16(rotation)
+    return GsbRawParams(ptr(dc) if want_sh else None, ptr(rest) if want_sh else None, C_rest, ptr(scaling), ptr(rotation)), C_rest, rotation
 
 
 def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, sh, degrees, keep,
@@ -209,7 +211,8 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
     if raw is not None:
         if packed_counts is not None or statistics is not None:
             raise RuntimeError("raw parameters: the packed variable-SH and statistics forwards have no raw form")
-        raw_s, _ = _raw_struct(raw, device, int(means3D.shape[0]), not _present(colors), sh, scales, rotations, cov3D_precomp, quant)
+        raw_s, _, raw_rot = _raw_struct(raw, device, int(means3D.shape[0]), not _present(colors), sh, scales, rotations, cov3D_precomp,
+                                        quant)
     L = _lib.lib()
     keep = []
     H, W = int(image_height), int(image_width)
@@ -333,7 +336,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
         raise RuntimeError(f"absgrad_out must live on {device}, got {absgrad_out.device}")
     if raw is not None:
         want_sh = not _present(colors)
-        raw_s, C_rest = _raw_struct(raw, device, int(means3D.shape[0]), want_sh, sh, scales, rotations, cov3D_precomp, quant)
+        raw_s, C_rest, raw_rot = _raw_struct(raw, device, int(means3D.shape[0]), want_sh, sh, scales, rotations, cov3D_precomp, quant)
     L = _lib.lib()
     keep = []
     H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
