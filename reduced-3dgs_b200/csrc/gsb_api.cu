@@ -559,7 +559,7 @@ int gsb_export_image(const char* image_blob, int32_t W, int32_t H, float* final_
 {
 	cudaStream_t stream = (cudaStream_t)stream_;
 	ImageState img = ImageState::carve(const_cast<char*>(image_blob), W, H);
-	const size_t N = size_t(W) * H, T = size_t((W + 15) / 16) * ((H + 15) / 16);
+	const size_t N = size_t(W) * H, T = ImageState::tiles(W, H);
 	if (final_T) GSB_CUDA_OK(cudaMemcpyAsync(final_T, img.final_T, N * 4, cudaMemcpyDeviceToDevice, stream));
 	if (n_contrib) GSB_CUDA_OK(cudaMemcpyAsync(n_contrib, img.n_contrib, N * 4, cudaMemcpyDeviceToDevice, stream));
 	if (ranges) GSB_CUDA_OK(cudaMemcpyAsync(ranges, img.ranges, T * 8, cudaMemcpyDeviceToDevice, stream));

@@ -40,10 +40,6 @@ struct BwdArgs {
 // One kernel per view runs at a time on the stream, so every
 // element receives exactly one addition per view, in view order: the result is deterministic.  Adding zero is skipped — culled
 // Gaussians and inactive SH bands are most of the rows; the overwrite mode stores them (every element written once, no memset).
-__device__ __forceinline__ void red_add_f32x4(float* addr, float a, float b, float c, float d)
-{
-	asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
-}
 template <bool ACC> __device__ __forceinline__ void put(float* p, float v) { if (ACC) { if (v != 0.0f) atomicAdd(p, v); } else *p = v; }
 
 // Coalesced store of one small per-Gaussian output ([P,WD]) for the 32 Gaussians of a warp: lanes park their WD values in
@@ -101,7 +97,7 @@ __device__ __forceinline__ void raw_block(const float* src, float* dst, int widt
 				float* p = dst + base * width + f;
 				if (ACC)
 				{
-					if (e[0] != 0.f || e[1] != 0.f || e[2] != 0.f || e[3] != 0.f) red_add_f32x4(p, e[0], e[1], e[2], e[3]);
+					if (e[0] != 0.f || e[1] != 0.f || e[2] != 0.f || e[3] != 0.f) red_add_v4(p, e[0], e[1], e[2], e[3]);
 				}
 				else *reinterpret_cast<float4*>(p) = make_float4(e[0], e[1], e[2], e[3]);
 			}
@@ -144,16 +140,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 	const int RL = 3 * a.M, RS = RL + 1;                                  // row length / padded stride (conflict-free per-lane rows)
 	float* s_row = s_dyn + (QUANT ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) + warp * (32 * RS + 32 * 6);
 	float* s_tmp = s_row + 32 * RS;
-	if (QUANT)
-	{
-		for (int i = threadIdx.x; i < GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE; i += blockDim.x)
-		{
-			float v = a.q.centers[i];
-			if (i / GSB_CODEBOOK_SIZE == 17) v = exp_ref(v);
-			s_cb[i] = v;
-		}
-		__syncthreads();
-	}
+	if (QUANT) stage_codebooks(a.q.centers, s_cb);
 	// rasterizer_impl.cu:549-571: sh_sparsity_multiplier = lambda / (n_visible * 15 * 3)
 	const float mult = a.lambda != 0.0f ? a.lambda / (float)((int)a.g.counters[1] * 15 * 3) : 0.0f;
 	// colours given by the caller (override_color): the SH coefficients were not used by the forward, their gradient is zero
@@ -250,9 +237,8 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 			float cov3D[6];
 			if (QUANT)
 			{
-				for (int k = 0; k < 3; k++) sc[k] = s_cb[17 * 256 + isb[k]];
-				qr = s_cb[18 * 256 + (irw & 0xffu)]; qx = s_cb[19 * 256 + ((irw >> 8) & 0xffu)]; qy = s_cb[19 * 256 + ((irw >> 16) & 0xffu)]; qz = s_cb[19 * 256 + (irw >> 24)];
-				normalize_quat(qr, qx, qy, qz);
+				for (int k = 0; k < 3; k++) sc[k] = quant_value(s_cb, CB_SCALING, isb[k]);
+				quant_rotation(s_cb, irw, qr, qx, qy, qz);
 				compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);
 			}
 			else if (RAW)
@@ -523,7 +509,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				float4 o = have_sh ? make_float4(sp[0], sp[1], sp[2], sp[3]) : make_float4(0.f, 0.f, 0.f, 0.f);
 				if (ACC)
 				{
-					if (o.x != 0.f || o.y != 0.f || o.z != 0.f || o.w != 0.f) red_add_f32x4(reinterpret_cast<float*>(dst4 + i * 32 + lane), o.x, o.y, o.z, o.w);
+					if (o.x != 0.f || o.y != 0.f || o.z != 0.f || o.w != 0.f) red_add_v4(reinterpret_cast<float*>(dst4 + i * 32 + lane), o.x, o.y, o.z, o.w);
 				}
 				else dst4[i * 32 + lane] = o;
 			}

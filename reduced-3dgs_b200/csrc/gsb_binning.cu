@@ -591,7 +591,7 @@ __global__ void __launch_bounds__(1024) tile_sort_big_kernel(const uint2* __rest
 // ------------------------------------------------------------------------------------------------
 int launch_tile_scan(const ImageState& img, const GeomState& g, const BinPlan& plan, int W, int H, cudaStream_t stream)
 {
-	const int T = ((W + GSB_TILE_X - 1) / GSB_TILE_X) * ((H + GSB_TILE_Y - 1) / GSB_TILE_Y);
+	const int T = (int)ImageState::tiles(W, H);
 	ProfScope prof(K_SCAN, stream);
 	if (plan.priv)
 	{
@@ -623,8 +623,8 @@ int launch_scatter_sort(const GeomState& g, const BinningState& b, const ImageSt
 	cudaStream_t stream)
 {
 	if (cap <= 0) return GSB_OK;
-	const int gx = (W + GSB_TILE_X - 1) / GSB_TILE_X, gy = (H + GSB_TILE_Y - 1) / GSB_TILE_Y;
-	const int T = gx * gy;
+	const dim3 tiles = tile_grid(W, H);
+	const int gx = tiles.x, gy = tiles.y, T = gx * gy;
 	const uint32_t cap32 = (uint32_t)std::min<long long>(cap, 0x7fffffffll);
 	{
 		ProfScope prof(K_EMIT_KEYS, stream);
@@ -678,7 +678,7 @@ int launch_scatter_sort(const GeomState& g, const BinningState& b, const ImageSt
 int launch_sort_large(const GeomState& g, const BinningState& b, const ImageState& img, int W, int H, uint32_t n_tiles_over_a, uint32_t n_tiles_over_b,
 	cudaStream_t stream)
 {
-	const int T = ((W + GSB_TILE_X - 1) / GSB_TILE_X) * ((H + GSB_TILE_Y - 1) / GSB_TILE_Y);
+	const int T = (int)ImageState::tiles(W, H);
 	constexpr size_t smemB = size_t(GSB_SORT_CAP_B) * 16 + 32 * 256 * 4;
 	if (n_tiles_over_a)
 	{
@@ -721,7 +721,7 @@ __global__ void export_binning_kernel(int T, const uint2* __restrict__ ranges, c
 
 int launch_export_binning(const GeomState& g, const BinningState& b, const ImageState& img, int W, int H, uint64_t* keys, uint32_t* vals, cudaStream_t stream)
 {
-	const int T = ((W + GSB_TILE_X - 1) / GSB_TILE_X) * ((H + GSB_TILE_Y - 1) / GSB_TILE_Y);
+	const int T = (int)ImageState::tiles(W, H);
 	export_binning_kernel<<<T, 128, 0, stream>>>(T, img.ranges, b.point_list, g.rec, keys, vals);
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;

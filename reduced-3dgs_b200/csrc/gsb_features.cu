@@ -6,15 +6,16 @@
 // the tile ranges and the depth-sorted point_list, the 48-byte records (conic, pth, mean, opacity with the anti-aliasing factor applied),
 // n_contrib and tile_max_contrib.  A feature pass therefore runs no preprocess, scan, scatter or sort; it only composites.
 //
-// Layout of work: one CTA per (16x16 tile, chunk of CH channels); 8 warps of 8x4 pixels as in render_forward_kernel.  A batch of 256
-// list entries is staged into shared memory (the record's r0 / r1 and the CH-channel slice of each Gaussian's feature row), and the
-// exact warp-rectangle cull (rect_may_contribute) picks the entries a warp visits.
+// Layout of work: one CTA per (16x16 tile, chunk of CH channels); 8 warps of 8x4 pixels (WarpPixels) as in render_forward_kernel.  A
+// batch of 256 list entries is staged into shared memory (the record's r0 / r1 and the CH-channel slice of each Gaussian's feature
+// row), and the exact warp-rectangle cull (rect_may_contribute) picks the entries a warp visits.
 //
 // Which pairs contribute: a pair (p, i) with list position pos (0-based) contributes iff pos < n_contrib(p) and it passes the alpha
 // tests (power <= 0, power >= pth, alpha >= 1/255).  This is the colour forward's rule restated with its result n_contrib: every
 // candidate pair in front of the last contributor contributed, since a candidate that would drop T below 1e-4 ends the pixel.  The
-// render backward uses the same rule.  The per-pair arithmetic is the colour kernel's (pair_power, exp_loop, the same rounding
-// intrinsics in the same order), so a feature channel equals the colour channel of a colors_precomp = features, bg = 0 render bit for bit.
+// render backward uses the same rule.  The pair is evaluated by the colour kernels' own eval_pair (gsb_common.cuh) and accumulated with
+// the same rounding intrinsics in the same order, so a feature channel equals the colour channel of a colors_precomp = features, bg = 0
+// render bit for bit.
 //
 // Backward (back to front from final_T, the colour backward's T recursion T <- T / (1 - alpha) with MUFU.RCP): per contributing pair
 //     dL/df_c  += alpha T g_c                          (g = dL/dout at the pixel)
@@ -77,17 +78,11 @@ __global__ void __launch_bounds__(256) features_forward_kernel(const uint2* __re
 	__shared__ uint32_t s_id[FEAT_BATCH];
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const int tile = blockIdx.y * gridDim.x + blockIdx.x, c0 = blockIdx.z * CH;
-	const int wx0 = blockIdx.x * GSB_TILE_X + (warp & 1) * 8, wy0 = blockIdx.y * GSB_TILE_Y + (warp >> 1) * 4;
-	const int px = wx0 + (lane & 7), py = wy0 + (lane >> 3);
-	const bool inside = px < W && py < H;
-	const float pxf = (float)px, pyf = (float)py;
-	const float rx0 = (float)wx0, rx1 = (float)(wx0 + 7), ry0 = (float)wy0, ry1 = (float)(wy0 + 3);
-	const size_t pid = (size_t)W * py + px, N = (size_t)W * H;
+	const WarpPixels wp(W, H, warp, lane);
+	const size_t pid = wp.pid, N = (size_t)W * H;
 	const uint32_t hi = tile_max[tile], start = ranges[tile].x;
-	const uint32_t last = inside ? n_contrib[pid] : 0u;
-	uint32_t wmax = last;
-#pragma unroll
-	for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+	const uint32_t last = wp.inside ? n_contrib[pid] : 0u;
+	const uint32_t wmax = warp_max(last);
 
 	float T = 1.0f;
 	float acc[CH];
@@ -104,19 +99,16 @@ __global__ void __launch_bounds__(256) features_forward_kernel(const uint2* __re
 			if (j < n && b + j < wmax)
 			{
 				const float4 r0 = s_rec[2 * j], r1 = s_rec[2 * j + 1];
-				keep = rect_may_contribute(r1.x, r1.y, r0.x, r0.y, r0.z, r0.w, rx0, rx1, ry0, ry1);
+				keep = rect_may_contribute(r0, r1, wp);
 			}
 			unsigned mask = __ballot_sync(0xffffffffu, keep);
 			while (mask)
 			{
 				const int e = cb + __ffs(mask) - 1; mask &= mask - 1;
 				const float4 r0 = s_rec[2 * e], r1 = s_rec[2 * e + 1];
-				// render_forward_kernel's pair arithmetic, operation for operation
-				const float dx = __fsub_rn(r1.x, pxf), dy = __fsub_rn(r1.y, pyf);
-				const float power = pair_power(r0.x, r0.y, r0.z, dx, dy);
-				const float alpha = fminf(0.99f, __fmul_rn(r1.z, exp_loop(power)));
-				const bool v = (b + e < last) && !(power > 0.0f) && !(power < r0.w) && !(alpha < 1.0f / 255.0f);
-				if (v)
+				const PairAlpha pa = eval_pair(r0, r1, wp);
+				const float alpha = pa.alpha;
+				if (pair_passes(b + e < last, pa, r0.w))
 				{
 					const float4* f4 = reinterpret_cast<const float4*>(s_f + e * CH);
 #pragma unroll
@@ -134,7 +126,7 @@ __global__ void __launch_bounds__(256) features_forward_kernel(const uint2* __re
 		}
 		__syncthreads();                                       // the next batch overwrites the staging buffers
 	}
-	if (inside)
+	if (wp.inside)
 	{
 #pragma unroll
 		for (int k = 0; k < CH; k++)
@@ -171,13 +163,6 @@ __device__ __forceinline__ float warp_transpose_sum(float (&v)[NV], int lane, in
 	return v[0];
 }
 
-__device__ __forceinline__ float feat_rcp_approx(float x)
-{
-	float r;
-	asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
-	return r;
-}
-
 template <int CH>
 __global__ void __launch_bounds__(256) features_backward_kernel(const uint2* __restrict__ ranges, const uint32_t* __restrict__ point_list,
 	int W, int H, const float4* __restrict__ rec, const float* __restrict__ final_Ts, const uint32_t* __restrict__ n_contrib,
@@ -192,24 +177,18 @@ __global__ void __launch_bounds__(256) features_backward_kernel(const uint2* __r
 	const int tile = blockIdx.y * gridDim.x + blockIdx.x, c0 = blockIdx.z * CH;
 	const uint32_t hi = tile_max[tile];
 	if (hi == 0) return;
-	const int wx0 = blockIdx.x * GSB_TILE_X + (warp & 1) * 8, wy0 = blockIdx.y * GSB_TILE_Y + (warp >> 1) * 4;
-	const int px = wx0 + (lane & 7), py = wy0 + (lane >> 3);
-	const bool inside = px < W && py < H;
-	const float pxf = (float)px, pyf = (float)py;
-	const float rx0 = (float)wx0, rx1 = (float)(wx0 + 7), ry0 = (float)wy0, ry1 = (float)(wy0 + 3);
-	const size_t pid = (size_t)W * py + px, N = (size_t)W * H;
+	const WarpPixels wp(W, H, warp, lane);
+	const size_t pid = wp.pid, N = (size_t)W * H;
 	const uint32_t start = ranges[tile].x;
-	const uint32_t last = inside ? n_contrib[pid] : 0u;
-	uint32_t wmax = last;
-#pragma unroll
-	for (int o = 16; o > 0; o >>= 1) wmax = max(wmax, __shfl_xor_sync(0xffffffffu, wmax, o));
+	const uint32_t last = wp.inside ? n_contrib[pid] : 0u;
+	const uint32_t wmax = warp_max(last);
 
-	float T = inside ? final_Ts[pid] : 0.0f;
+	float T = wp.inside ? final_Ts[pid] : 0.0f;
 	float g[CH], ar[CH], lf[CH], last_alpha = 0.0f;
 #pragma unroll
 	for (int k = 0; k < CH; k++)
 	{
-		g[k] = (inside && c0 + k < F) ? dL_dout[(size_t)(c0 + k) * N + pid] : 0.0f;
+		g[k] = (wp.inside && c0 + k < F) ? dL_dout[(size_t)(c0 + k) * N + pid] : 0.0f;
 		ar[k] = 0.0f; lf[k] = 0.0f;
 	}
 	// entry j of batch b sits at list position hi - 1 - (b + j): the batches run from the back of the list to the front
@@ -224,7 +203,7 @@ __global__ void __launch_bounds__(256) features_backward_kernel(const uint2* __r
 			if (j < n && hi - 1 - (b + j) < wmax)
 			{
 				const float4 r0 = s_rec[2 * j], r1 = s_rec[2 * j + 1];
-				keep = rect_may_contribute(r1.x, r1.y, r0.x, r0.y, r0.z, r0.w, rx0, rx1, ry0, ry1);
+				keep = rect_may_contribute(r0, r1, wp);
 			}
 			unsigned mask = __ballot_sync(0xffffffffu, keep);
 			while (mask)
@@ -232,11 +211,9 @@ __global__ void __launch_bounds__(256) features_backward_kernel(const uint2* __r
 				const int e = cb + __ffs(mask) - 1; mask &= mask - 1;
 				const uint32_t pos = hi - 1 - (b + e);
 				const float4 r0 = s_rec[2 * e], r1 = s_rec[2 * e + 1];
-				const float dx = __fsub_rn(r1.x, pxf), dy = __fsub_rn(r1.y, pyf);
-				const float power = pair_power(r0.x, r0.y, r0.z, dx, dy);
-				const float G = exp_loop(power);
-				const float alpha = fminf(0.99f, __fmul_rn(r1.z, G));
-				const bool active = (pos < last) && !(power > 0.0f) && !(power < r0.w) && !(alpha < 1.0f / 255.0f);
+				const PairAlpha pa = eval_pair(r0, r1, wp);
+				const float alpha = pa.alpha, dx = pa.dx, dy = pa.dy;
+				const bool active = pair_passes(pos < last, pa, r0.w);
 				if (!__any_sync(0xffffffffu, active)) continue;
 				float v[NV];
 #pragma unroll
@@ -244,7 +221,7 @@ __global__ void __launch_bounds__(256) features_backward_kernel(const uint2* __r
 				if (active)
 				{
 					// render_backward_kernel's recursion: T before this Gaussian, and the "colour behind" of each channel
-					T = T * feat_rcp_approx(1.0f - alpha);
+					T = T * rcp_approx(1.0f - alpha);
 					const float u = alpha * T, oml = 1.0f - last_alpha;
 					const float* f = s_f + e * CH;
 					float dLda = 0.0f;
@@ -257,7 +234,7 @@ __global__ void __launch_bounds__(256) features_backward_kernel(const uint2* __r
 						v[k] = u * g[k];
 					}
 					last_alpha = alpha;
-					const float w = G * (dLda * T);                     // G * dL/dalpha
+					const float w = pa.G * (dLda * T);                     // G * dL/dalpha
 					const float o = r1.z, wx = w * dx, wy = w * dy;
 					v[CH] = w;
 					v[CH + 1] = -o * (r0.x * wx + r0.y * wy);
@@ -281,42 +258,40 @@ __global__ void __launch_bounds__(256) features_backward_kernel(const uint2* __r
 	}
 }
 
-static dim3 features_grid(int W, int H, int F, int ch)
+// Calls f with the chunk width as a std::integral_constant (as dispatch() hands over flags) and the grid: tiles x chunks of it.
+template <class Fn> static int dispatch_ch(int W, int H, int F, Fn&& f)
 {
-	return dim3((W + GSB_TILE_X - 1) / GSB_TILE_X, (H + GSB_TILE_Y - 1) / GSB_TILE_Y, (F + ch - 1) / ch);
+	const int ch = features_ch(F);
+	dim3 grid = tile_grid(W, H);
+	grid.z = (F + ch - 1) / ch;
+	return ch == 8 ? f(std::integral_constant<int, 8>{}, grid) : f(std::integral_constant<int, 16>{}, grid);
 }
 
 int launch_features_forward(const ImageState& img, const BinningState& b, const GeomState& g, int W, int H, const GsbFeatures& f,
 	cudaStream_t stream)
 {
-	const int ch = features_ch(f.F);
 	ProfScope prof(K_FEATURES_FWD, stream);
-	if (ch == 8)
-		features_forward_kernel<8><<<features_grid(W, H, f.F, 8), 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, img.n_contrib,
+	return dispatch_ch(W, H, f.F, [&](auto ch, dim3 grid) -> int {
+		features_forward_kernel<ch><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, img.n_contrib,
 			img.tile_max_contrib, f.features, f.F, f.out);
-	else
-		features_forward_kernel<16><<<features_grid(W, H, f.F, 16), 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, img.n_contrib,
-			img.tile_max_contrib, f.features, f.F, f.out);
-	GSB_LAUNCHED();
-	GSB_CUDA_OK(cudaGetLastError());
-	return GSB_OK;
+		GSB_LAUNCHED();
+		GSB_CUDA_OK(cudaGetLastError());
+		return GSB_OK;
+	});
 }
 
 int launch_features_backward(const ImageState& img, const BinningState& b, const GeomState& g, int P, int W, int H, const GsbFeatures& f,
 	float* acc, cudaStream_t stream)
 {
-	const int ch = features_ch(f.F);
 	ProfScope prof(K_FEATURES_BWD, stream);
 	GSB_CUDA_OK(cudaMemsetAsync(f.dL_dfeatures, 0, size_t(P) * f.F * sizeof(float), stream));
-	if (ch == 8)
-		features_backward_kernel<8><<<features_grid(W, H, f.F, 8), 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, img.final_T,
+	return dispatch_ch(W, H, f.F, [&](auto ch, dim3 grid) -> int {
+		features_backward_kernel<ch><<<grid, 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, img.final_T,
 			img.n_contrib, img.tile_max_contrib, f.features, f.F, f.dL_dout, f.dL_dfeatures, acc);
-	else
-		features_backward_kernel<16><<<features_grid(W, H, f.F, 16), 256, 0, stream>>>(img.ranges, b.point_list, W, H, g.rec, img.final_T,
-			img.n_contrib, img.tile_max_contrib, f.features, f.F, f.dL_dout, f.dL_dfeatures, acc);
-	GSB_LAUNCHED();
-	GSB_CUDA_OK(cudaGetLastError());
-	return GSB_OK;
+		GSB_LAUNCHED();
+		GSB_CUDA_OK(cudaGetLastError());
+		return GSB_OK;
+	});
 }
 
 } // namespace gsb

@@ -109,16 +109,7 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 {
 	constexpr bool QUANT = IN == IN_QUANT, RAW = IN == IN_RAW;
 	extern __shared__ __align__(16) float s_cb[];   // QUANT: [20][256] centres; scaling row holds exp(centre)
-	if (QUANT)
-	{
-		for (int i = threadIdx.x; i < GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE; i += blockDim.x)
-		{
-			float v = a.q.centers[i];
-			if (i / GSB_CODEBOOK_SIZE == 17) v = exp_ref(v);      // get_scaling = exp(_scaling), gaussian_model.py:141-142
-			s_cb[i] = v;
-		}
-		__syncthreads();
-	}
+	if (QUANT) stage_codebooks(a.q.centers, s_cb);
 	uint32_t* s_hist = reinterpret_cast<uint32_t*>(s_cb + (QUANT ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0));
 	// QUANT: per-warp staging buffer of the rest-coefficient ids behind the histogram (16-byte aligned: T * 4 rounded up)
 	uint8_t* s_rest = reinterpret_cast<uint8_t*>(s_hist + ((a.hist_priv ? a.T : 0) + 3) / 4 * 4) + (threadIdx.x >> 5) * (32 * IDS_REST_ROW);
@@ -186,11 +177,11 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 				float opac_raw;
 				if (QUANT)
 				{
-					float r = s_cb[18 * 256 + (ir & 0xffu)], x = s_cb[19 * 256 + ((ir >> 8) & 0xffu)], y = s_cb[19 * 256 + ((ir >> 16) & 0xffu)],
-						z = s_cb[19 * 256 + (ir >> 24)];
-					normalize_quat(r, x, y, z);
-					compute_cov3D(s_cb[17 * 256 + is0], s_cb[17 * 256 + is1], s_cb[17 * 256 + is2], a.mod, r, x, y, z, cov3D);
-					opac_raw = s_cb[16 * 256 + iop];
+					float r, x, y, z;
+					quant_rotation(s_cb, ir, r, x, y, z);
+					compute_cov3D(quant_value(s_cb, CB_SCALING, is0), quant_value(s_cb, CB_SCALING, is1), quant_value(s_cb, CB_SCALING, is2), a.mod,
+						r, x, y, z, cov3D);
+					opac_raw = quant_value(s_cb, CB_OPACITY, iop);
 				}
 				else
 				{
@@ -397,17 +388,19 @@ __global__ void mark_visible_kernel(int P, const float* __restrict__ means3D, co
 	present[idx] = xform_row(view, 2, means3D[3 * idx], means3D[3 * idx + 1], means3D[3 * idx + 2]) > 0.2f;
 }
 
-// Debug/test export of the fused de-quantisation: activated scales [P,3] and normalised rotations [P,4] exactly as
-// preprocess_kernel<IN_QUANT> computes them (compared bit-for-bit with torch.exp / F.normalize in the tests).
+// Debug/test export of the fused de-quantisation: activated scales [P,3] and normalised rotations [P,4] from the staging and the
+// decode of preprocess_kernel<IN_QUANT> (compared bit-for-bit with torch.exp / F.normalize in the tests).
 __global__ void debug_dequant_kernel(int P, GsbQuant q, float* __restrict__ scales, float* __restrict__ rots)
 {
+	__shared__ float s_cb[GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE];
+	stage_codebooks(q.centers, s_cb);
 	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
 	if (idx >= P) return;
 	const uint8_t* is = q.ids_scaling + 3 * (size_t)idx;
 	const uint8_t* ir = q.ids_rot + 4 * (size_t)idx;
-	for (int k = 0; k < 3; k++) scales[3 * (size_t)idx + k] = exp_ref(q.centers[17 * 256 + is[k]]);
-	float r = q.centers[18 * 256 + ir[0]], x = q.centers[19 * 256 + ir[1]], y = q.centers[19 * 256 + ir[2]], z = q.centers[19 * 256 + ir[3]];
-	normalize_quat(r, x, y, z);
+	for (int k = 0; k < 3; k++) scales[3 * (size_t)idx + k] = quant_value(s_cb, CB_SCALING, is[k]);
+	float r, x, y, z;
+	quant_rotation(s_cb, ir[0] | ir[1] << 8 | ir[2] << 16 | (uint32_t)ir[3] << 24, r, x, y, z);
 	reinterpret_cast<float4*>(rots)[idx] = make_float4(r, x, y, z);
 }
 
@@ -424,7 +417,8 @@ int launch_preprocess(const GsbForwardRequest& req, const GeomState& g, const Im
 	const GsbScene* s = req.scene; const GsbCamera* cam = req.cam; const GsbRawParams* raw = req.raw;
 	PreArgs a{};
 	a.P = s->P; a.M = s->M; a.W = cam->width; a.H = cam->height;
-	a.gx = (cam->width + GSB_TILE_X - 1) / GSB_TILE_X; a.gy = (cam->height + GSB_TILE_Y - 1) / GSB_TILE_Y;
+	const dim3 tiles = tile_grid(cam->width, cam->height);
+	a.gx = tiles.x; a.gy = tiles.y;
 	a.mod = s->scale_modifier; a.tan_fovx = cam->tan_fovx; a.tan_fovy = cam->tan_fovy;
 	a.focal_y = cam->height / (2.0f * cam->tan_fovy);                                    // rasterizer_impl.cu:386-387
 	a.focal_x = cam->width / (2.0f * cam->tan_fovx);
