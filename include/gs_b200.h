@@ -582,6 +582,64 @@ GSB_API int gsb_mercy_plan(int32_t P, const int32_t* counts, const float* opacit
                 double mercy_minimum, float quantile_q, const float* draws, int64_t n_draws, void* workspace, uint8_t* mask,
                 float* thresholds /* [2] */, int64_t* counts_out /* [2] */, void* stream);
 
+/* ---- 3DGS-MCMC densification (gs_b200.mcmc, DESIGN.md §5n) ----
+ *
+ * Kheradmand et al., "3D Gaussian Splatting as Markov Chain Monte Carlo" (2024): position noise after every optimizer step, and
+ * every densification interval the dead Gaussians moved onto live ones and the model grown towards a budget.  Notation:
+ * o = sigmoid(opacity_logit) (torch's fp32 sigmoid), s = exp(scaling), q = F.normalize(rotation) (both in torch's fp32 roundings),
+ * R(q) = build_rotation(q).  Every call is asynchronous on `stream`; none reads back to the host.
+ *
+ * gsb_mcmc_noise: for each row i < P, with the gate g = 1 / (1 + exp(-100 ((1 - o) - 0.995))),
+ *   xyz[i] += R diag(s)^2 R^T v,   v = draws[i] * g * noise_lr * xyz_lr   (draws [P, 3]: standard-normal samples),
+ * evaluated in double from the fp32 inputs (the gate from the fp32 o) and rounded once into xyz.  A row whose gate is 0 when torch
+ * evaluates it in fp32 (exp overflows: o above about 0.892) is not written, so it keeps its bytes.  One launch, none for P == 0.
+ * Errors (GSB_EINVAL, nothing launched): P < 0 or P >= 2^30, a non-finite noise_lr / xyz_lr, and with P > 0 a NULL pointer. */
+GSB_API int gsb_mcmc_noise(int32_t P, float* xyz /* [P,3] */, const float* scaling /* [P,3] */, const float* rotation /* [P,4] */,
+                const float* opacity_logits /* [P] */, const float* draws /* [P,3] */, float noise_lr, float xyz_lr, void* stream);
+
+/* gsb_mcmc_plan: samples source rows by opacity and computes their relocated values, in two calls.
+ *   Without draws (n = 0): marks the dead rows (GSB_MCMC_RELOCATE: dead_mask[i] != 0, or with dead_mask NULL o <= min_opacity;
+ *   GSB_MCMC_ADD: none), weighs the candidate rows (the live rows; with ADD every row) W_i = floor(o_i 2^32) (0 for the others and
+ *   for a NaN o), takes the exact inclusive prefix of W in row order and writes counts[GSB_MCMC_COUNTS] (int64, device) = {dead
+ *   rows, total weight, 0, 0}.  The caller reads counts back to size the draws.
+ *   With draws (int64 [n], uniform on [0, 2^62): torch.randint(0, 2**62, (n,))): draw j selects the first row whose prefix exceeds
+ *   floor(d_j * total / 2^62) (a 128-bit product; a draw is taken modulo 2^62), so rows of weight 0 are never selected; a draw
+ *   needs total > 0.  With RELOCATE only the first min(n, dead rows) draws are used.  A source row drawn c times gets N = min(c + 1,
+ *   50) and (paper eq. 9, in double)
+ *     o' = 1 - (1 - o)^(1/N),  D = sum_{i=1..N} sum_{k=0..i-1} C(i-1, k) (-1)^k o'^(k+1) / sqrt(k+1),  s' = s o / D,
+ *   then o' is clamped to [0.005, 1 - 2^-23].  N = 1 gives o' = o and s' = s.  The workspace begins (byte offset 0) with a float4
+ *   [P] table that holds (o', s'0, s'1, s'2) at every sampled source row before the logit / log gsb_mcmc_emit applies.  Counts per
+ *   row are exact (integer atomics) and duplicate sources are resolved here, so the same inputs give the same bytes.
+ *   workspace: gsb_mcmc_workspace_bytes(P) bytes; both calls and gsb_mcmc_emit take the same one.
+ * Errors (GSB_EINVAL, nothing launched): P < 0 or P >= 2^30, an unknown mode, dead_mask with GSB_MCMC_ADD, NULL workspace, draws
+ * with n outside 1..P or no draws with n != 0, NULL counts without draws, with P > 0 NULL opacity_logits, and with draws NULL
+ * scaling. */
+#define GSB_MCMC_RELOCATE 0
+#define GSB_MCMC_ADD 1
+#define GSB_MCMC_COUNTS 4         /* dead rows, total weight, 0, 0 */
+GSB_API size_t gsb_mcmc_workspace_bytes(int32_t P);
+GSB_API int gsb_mcmc_plan(int32_t P, int32_t mode, const float* opacity_logits, const float* scaling, const uint8_t* dead_mask,
+                float min_opacity, int64_t n, const int64_t* draws, void* workspace, int64_t* counts, void* stream);
+
+/* gsb_mcmc_emit: writes the rows of the plan's n draws over a GsbDensifyTensor table, in one launch.  A GSB_DENSIFY_SCALING entry
+ * (row_width 3) stores log(s'), a GSB_MCMC_OPACITY entry (row_width 1) stores log(o' / (1 - o')) (fp32, torch's roundings), a
+ * GSB_DENSIFY_COPY entry copies the source row.
+ *   GSB_MCMC_RELOCATE, in place (dst == src, each moment pair's dst == src): dead row j (the j-th in row order) takes draw j's
+ *     source row; every sampled source takes its relocated opacity / scaling and its moments are zeroed in every entry that has
+ *     them.  The dead rows keep their moments.  Other rows are not written.
+ *   GSB_MCMC_ADD, into [P + n, row_width] destinations: row i < P is row i of the source tensor (a sampled row with its relocated
+ *     opacity / scaling and zero moments); row P + j is draw j's source row (relocated opacity / scaling) with zero moments.  A
+ *     GSB_MCMC_FRESH entry (statistics; no moments) copies rows < P and zeroes the new ones.
+ * Errors (GSB_EINVAL, nothing launched): tensors NULL with n_tensors > 0, n_tensors outside 0..GSB_DENSIFY_MAX_TENSORS, P < 0 or
+ * P >= 2^30, an unknown mode, n outside 0..P, NULL workspace, row_width <= 0, a kind other than COPY / SCALING / MCMC_OPACITY /
+ * MCMC_FRESH, a scaling entry without row_width 3 or an opacity entry without 1, an MCMC_FRESH entry with RELOCATE or with moments,
+ * a grad pointer, a half-given moment pair, with P > 0 a NULL src / dst, with RELOCATE dst != src or a moment dst != its src, a
+ * pointer not 4-byte aligned. */
+#define GSB_MCMC_OPACITY 3
+#define GSB_MCMC_FRESH 4
+GSB_API int gsb_mcmc_emit(const GsbDensifyTensor* tensors, int32_t n_tensors, int32_t P, int32_t mode, int64_t n, const void* workspace,
+                void* stream);
+
 /* Number of kernels this library has launched since load (bench.py reports it as gpu_launches). */
 GSB_API uint64_t gsb_launch_count(void);
 

@@ -16,7 +16,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 OUT_DIR = os.path.join(os.path.dirname(HERE), "gs_b200")
 SO = os.path.join(OUT_DIR, "libgs_b200.so")
-SOURCES = ["gsb_api.cu", "gsb_preprocess.cu", "gsb_binning.cu", "gsb_render.cu", "gsb_backward.cu", "gsb_tools.cu", "gsb_kmeans.cu", "gsb_knn.cu", "gsb_loss.cu", "gsb_adam.cu", "gsb_densify.cu", "gsb_deterministic.cu", "gsb_mercy.cu", "gsb_features.cu"]
+SOURCES = ["gsb_api.cu", "gsb_preprocess.cu", "gsb_binning.cu", "gsb_render.cu", "gsb_backward.cu", "gsb_tools.cu", "gsb_kmeans.cu", "gsb_knn.cu", "gsb_loss.cu", "gsb_adam.cu", "gsb_densify.cu", "gsb_deterministic.cu", "gsb_mercy.cu", "gsb_features.cu", "gsb_mcmc.cu"]
 HEADERS = ["gsb_common.cuh", os.path.join("..", "..", "include", "gs_b200.h")]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",

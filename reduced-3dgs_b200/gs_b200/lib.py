@@ -107,6 +107,8 @@ DENSIFY_MAX_TENSORS = 16       # GSB_DENSIFY_MAX_TENSORS
 DENSIFY_COUNTS = 8             # GSB_DENSIFY_COUNTS
 DENSIFY_CLONE_SPLIT, DENSIFY_PRUNE, DENSIFY_PRUNE_MASK = 0, 1, 2
 DENSIFY_COPY, DENSIFY_XYZ, DENSIFY_SCALING = 0, 1, 2
+MCMC_RELOCATE, MCMC_ADD, MCMC_COUNTS = 0, 1, 4
+MCMC_OPACITY, MCMC_FRESH = 3, 4
 MERCY_REDUNDANCY_OPACITY, MERCY_REDUNDANCY_RANDOM, MERCY_OPACITY, MERCY_REDUNDANCY_OPACITY_OPACITY, MERCY_REDUNDANCY = 0, 1, 2, 3, 4
 
 
@@ -148,6 +150,10 @@ SIGNATURES = {
     "gsb_redundancy_score": (C.c_int, [_I32, _V, _V, _V, _I32, _V, _V, _V, _V, _F, _I32, _V, _V, _V, _V]),
     "gsb_mercy_workspace_bytes": (_SZ, [_I32]),
     "gsb_mercy_plan": (C.c_int, [_I32, _V, _V, _I32, _F, C.c_double, _F, _V, _I64, _V, _V, _V, _V, _V]),
+    "gsb_mcmc_noise": (C.c_int, [_I32] + [_V] * 5 + [_F, _F, _V]),
+    "gsb_mcmc_workspace_bytes": (_SZ, [_I32]),
+    "gsb_mcmc_plan": (C.c_int, [_I32, _I32, _V, _V, _V, _F, _I64, _V, _V, _V, _V]),
+    "gsb_mcmc_emit": (C.c_int, [C.POINTER(GsbDensifyTensor), _I32, _I32, _I32, _I64, _V, _V]),
     "gsb_launch_count": (C.c_uint64, []),
     "gsb_profile_enable": (None, [C.c_int]),
     "gsb_profile_read": (C.c_int, [C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_double), C.POINTER(C.c_uint64)]),
