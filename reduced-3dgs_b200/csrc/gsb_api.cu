@@ -579,7 +579,7 @@ int gsb_redundancy_score(int32_t P, const float* means3D, const float* scales, c
 	const float* w2ndc, const float* w2ndc_inverse, const int32_t* image_heights, const int32_t* image_widths, float pixel_scale,
 	int32_t K, int32_t* min_redundancy, float* pixel_sizes, void* workspace, void* stream)
 {
-	if (P < 0 || P >= (1 << 30)) { set_error("redundancy_score: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
+	if (!rows_ok("redundancy_score", P)) return GSB_EINVAL;
 	if (K < 1 || K > GSB_KNN_MAX_K) { set_error("redundancy_score: K = %d is outside 1..%d", K, GSB_KNN_MAX_K); return GSB_EINVAL; }
 	if (n_cameras < 0 || n_cameras > 1024) { set_error("redundancy_score: n_cameras = %d is outside 0..1024", n_cameras); return GSB_EINVAL; }
 	if (P == 0) return GSB_OK;

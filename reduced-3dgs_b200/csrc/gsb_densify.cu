@@ -12,7 +12,8 @@
 // on an H100: exp == exp_ref, sigmoid == 1 / (1 + exp(-x)) with IEEE division, the norm unfused, division by the Python scalar
 // 0.8 * N a multiplication by its fp32 reciprocal, comparisons against the fp32 casts of the thresholds, log == CUDA logf
 // (what torch.log calls).  torch.bmm's contraction order for the children's offsets depends on the batch size (cuBLAS); the
-// kernel uses the order the probe matched most often, so those values agree only to rounding (DESIGN.md §5g).
+// kernel uses the order the probe matched most often, so those values agree only to rounding (DESIGN.md §5g).  The emit table's
+// checks, the CTA scan, the grid size and the row range are gsb_common.cuh's, shared with gsb_mcmc.cu and gsb_mercy.cu.
 #include "gsb_common.cuh"
 
 namespace gsb {
@@ -118,7 +119,7 @@ __global__ void __launch_bounds__(DENS_THREADS) densify_plan_kernel(const PlanAr
 	__shared__ uint32_t s_tile;
 	__shared__ unsigned long long s_warp[DENS_THREADS / 32];
 	__shared__ uint32_t s_excl[DENS_CH], s_total[DENS_CH];
-	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int tid = threadIdx.x;
 	if (tid == 0) s_tile = atomicAdd(w.ticket, 1u);
 	__syncthreads();
 	const uint32_t tile = s_tile;
@@ -131,24 +132,11 @@ __global__ void __launch_bounds__(DENS_THREADS) densify_plan_kernel(const PlanAr
 		flags[i] = row0 + i < a.P ? row_flags(a, row0 + i) : 0u;
 		mine += pack_flags(flags[i]);
 	}
-	// CTA-wide exclusive scan of the packed counts
-	unsigned long long incl = mine;
-#pragma unroll
-	for (int o = 1; o < 32; o <<= 1) { const unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-	if (lane == 31) s_warp[warp] = incl;
-	__syncthreads();
-	if (warp == 0)
-	{
-		unsigned long long v = lane < DENS_THREADS / 32 ? s_warp[lane] : 0ull;
-#pragma unroll
-		for (int o = 1; o < DENS_THREADS / 32; o <<= 1) { const unsigned long long u = __shfl_up_sync(0xffffffffu, v, o); if (lane >= o) v += u; }
-		if (lane < DENS_THREADS / 32) s_warp[lane] = v;
-	}
-	__syncthreads();
-	unsigned long long run = (warp ? s_warp[warp - 1] : 0ull) + incl - mine;
+	unsigned long long cta_total;
+	unsigned long long run = cta_exclusive<DENS_THREADS>(mine, s_warp, &cta_total);
 	if (tid < DENS_CH)
 	{
-		const uint32_t total = field(s_warp[DENS_THREADS / 32 - 1], tid);
+		const uint32_t total = field(cta_total, tid);
 		s_total[tid] = total;
 		s_excl[tid] = lookback_exclusive(w.lookback, tile, DENS_LB_STRIDE, tid, total);
 	}
@@ -182,12 +170,6 @@ __global__ void __launch_bounds__(DENS_THREADS) densify_plan_kernel(const PlanAr
 		run += pack_flags(f);
 	}
 }
-
-struct EmitTable {
-	GsbDensifyTensor t[GSB_DENSIFY_MAX_TENSORS];
-	double inv_width[GSB_DENSIFY_MAX_TENSORS];
-	int n;
-};
 
 // build_rotation (general_utils.py:78-99) row c of the normalised quaternion's matrix, every torch op rounded on its own
 __device__ __forceinline__ void rotation_row(const float* q4, int c, float R[3])
@@ -225,7 +207,7 @@ __device__ __forceinline__ float child_xyz(const float* q4, const float* smp, fl
 
 // grid.y = table entry; grid.x strides over its P * row_width elements.  Each source element is read once and written to the
 // kept row, the kept clone and the two kept children of its row (a -1 rank skips the destination).
-__global__ void __launch_bounds__(DENS_THREADS) densify_emit_kernel(const __grid_constant__ EmitTable tab, const int4* __restrict__ rows,
+__global__ void __launch_bounds__(DENS_THREADS) densify_emit_kernel(const __grid_constant__ RowTable tab, const int4* __restrict__ rows,
 	long long P, long long clone_base, long long child1_base, long long child2_base, long long S, const float* __restrict__ rotation,
 	const float* __restrict__ samples, float split_factor)
 {
@@ -311,11 +293,9 @@ __global__ void __launch_bounds__(DENS_THREADS) densify_stats_kernel(long long P
 	}
 }
 
-static int grid_for(long long work)
-{
-	const long long want = (work + DENS_THREADS - 1) / DENS_THREADS, cap = (long long)GSB_NUM_SMS * 8;
-	return (int)(want < cap ? (want > 0 ? want : 1) : cap);
-}
+static const TableRules kEmitRules = {"densify_emit", "n",
+	(1u << GSB_DENSIFY_COPY) | (1u << GSB_DENSIFY_XYZ) | (1u << GSB_DENSIFY_SCALING),
+	"%s: tensor %d: unknown kind %d", "%s: tensor %d: an xyz / scaling entry needs row_width 3, got %d", true};
 
 } // namespace gsb
 
@@ -341,10 +321,10 @@ extern "C" int gsb_densify_stats(int32_t P, const float* viewspace_grad, int32_t
 	const cudaStream_t st = (cudaStream_t)stream;
 	ProfScope prof(K_TOOLS, st);
 	if (abs)
-		densify_stats_kernel<true><<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii,
+		densify_stats_kernel<true><<<grid_stride_ctas(P, DENS_THREADS, 8), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii,
 			xyz_gradient_accum, denom, max_radii2D, viewspace_grad_abs, abs_row_stride, xyz_gradient_accum_abs);
 	else
-		densify_stats_kernel<false><<<grid_for(P), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii,
+		densify_stats_kernel<false><<<grid_stride_ctas(P, DENS_THREADS, 8), DENS_THREADS, 0, st>>>(P, viewspace_grad, grad_row_stride, visibility, radii,
 			xyz_gradient_accum, denom, max_radii2D);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
@@ -357,7 +337,7 @@ extern "C" int gsb_densify_plan(int32_t P, int32_t mode, const float* xyz_gradie
 	float max_grad_abs, float clone_max_scale, float min_opacity, int32_t screen_test, float max_screen_size, float big_scale,
 	float split_scale_factor, void* workspace, int64_t* counts, void* stream)
 {
-	if (P < 0 || P >= (1 << 30)) { set_error("densify_plan: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
+	if (!rows_ok("densify_plan", P)) return GSB_EINVAL;
 	if (mode != GSB_DENSIFY_CLONE_SPLIT && mode != GSB_DENSIFY_PRUNE && mode != GSB_DENSIFY_PRUNE_MASK)
 	{ set_error("densify_plan: unknown mode %d", mode); return GSB_EINVAL; }
 	if (xyz_gradient_accum_abs && mode != GSB_DENSIFY_CLONE_SPLIT)
@@ -396,46 +376,24 @@ extern "C" int gsb_densify_emit(const GsbDensifyTensor* tensors, int32_t n, int3
 	int64_t n_clones_kept, int64_t n_split, int64_t n_children_kept, const float* rotation, const float* samples,
 	float split_scale_factor, void* stream)
 {
-	if (n < 0 || n > GSB_DENSIFY_MAX_TENSORS) { set_error("densify_emit: n = %d is outside 0..%d", n, GSB_DENSIFY_MAX_TENSORS); return GSB_EINVAL; }
-	if (n > 0 && !tensors) { set_error("densify_emit: tensor table is NULL"); return GSB_EINVAL; }
-	if (P < 0 || P >= (1 << 30)) { set_error("densify_emit: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
+	if (!rows_ok("densify_emit", P)) return GSB_EINVAL;
 	if (n_kept < 0 || n_clones_kept < 0 || n_split < 0 || n_children_kept < 0 || n_kept > P || n_clones_kept > P || n_split > P ||
 		n_children_kept > n_split)
 	{ set_error("densify_emit: inconsistent counts"); return GSB_EINVAL; }
 	if (!workspace) { set_error("densify_emit: NULL workspace"); return GSB_EINVAL; }
+	// an empty output has no storage (NULL destinations): only a call that writes rows needs its pointers
 	const bool rows_out = n_kept + n_clones_kept + n_children_kept > 0;
-	EmitTable tab{};
-	tab.n = n;
+	RowTable tab{};
+	int max_w;
+	if (!fill_row_table(kEmitRules, tensors, n, rows_out, rows_out, tab, max_w)) return GSB_EINVAL;
 	for (int i = 0; i < n; i++)
-	{
-		const GsbDensifyTensor& k = tensors[i];
-		if (k.row_width <= 0) { set_error("densify_emit: tensor %d: row_width %d <= 0", i, k.row_width); return GSB_EINVAL; }
-		if (k.kind != GSB_DENSIFY_COPY && k.kind != GSB_DENSIFY_XYZ && k.kind != GSB_DENSIFY_SCALING)
-		{ set_error("densify_emit: tensor %d: unknown kind %d", i, k.kind); return GSB_EINVAL; }
-		if (k.kind != GSB_DENSIFY_COPY && k.row_width != 3)
-		{ set_error("densify_emit: tensor %d: an xyz / scaling entry needs row_width 3, got %d", i, k.row_width); return GSB_EINVAL; }
-		// an empty output has no storage (NULL destinations): only a call that writes rows needs its pointers
-		if (rows_out && (!k.exp_avg_src != !k.exp_avg_dst || !k.exp_avg_src != !k.exp_avg_sq_src || !k.exp_avg_src != !k.exp_avg_sq_dst))
-		{ set_error("densify_emit: tensor %d: exp_avg / exp_avg_sq are half given", i); return GSB_EINVAL; }
-		if (rows_out && !k.grad_src != !k.grad_dst) { set_error("densify_emit: tensor %d: grad src / dst half given", i); return GSB_EINVAL; }
-		if (rows_out && (!k.src || !k.dst)) { set_error("densify_emit: tensor %d: NULL src / dst", i); return GSB_EINVAL; }
-		const uintptr_t any = reinterpret_cast<uintptr_t>(k.src) | reinterpret_cast<uintptr_t>(k.dst) |
-			reinterpret_cast<uintptr_t>(k.exp_avg_src) | reinterpret_cast<uintptr_t>(k.exp_avg_dst) |
-			reinterpret_cast<uintptr_t>(k.exp_avg_sq_src) | reinterpret_cast<uintptr_t>(k.exp_avg_sq_dst) |
-			reinterpret_cast<uintptr_t>(k.grad_src) | reinterpret_cast<uintptr_t>(k.grad_dst);
-		if (any & 3u) { set_error("densify_emit: tensor %d: a pointer is not 4-byte aligned", i); return GSB_EINVAL; }
-		if (k.kind == GSB_DENSIFY_XYZ && n_children_kept > 0 && (!rotation || !samples))
+		if (tensors[i].kind == GSB_DENSIFY_XYZ && n_children_kept > 0 && (!rotation || !samples))
 		{ set_error("densify_emit: split children need rotation and samples"); return GSB_EINVAL; }
-		tab.t[i] = k;
-		tab.inv_width[i] = 1.0 / k.row_width;
-	}
 	if (n == 0 || P == 0 || !rows_out) return GSB_OK;
-	int max_w = 1;
-	for (int i = 0; i < n; i++) max_w = tensors[i].row_width > max_w ? tensors[i].row_width : max_w;
 	const DensifyWorkspace w = densify_carve(static_cast<char*>(const_cast<void*>(workspace)), P);
 	const cudaStream_t st = (cudaStream_t)stream;
 	ProfScope prof(K_TOOLS, st);
-	const dim3 grid((unsigned)grid_for((long long)P * max_w), (unsigned)n);
+	const dim3 grid((unsigned)grid_stride_ctas((long long)P * max_w, DENS_THREADS, 8), (unsigned)n);
 	densify_emit_kernel<<<grid, DENS_THREADS, 0, st>>>(tab, w.rows, P, n_kept, n_kept + n_clones_kept, n_kept + n_clones_kept + n_children_kept,
 		n_split, rotation, samples, split_scale_factor);
 	GSB_LAUNCHED();

@@ -10,6 +10,7 @@
 //   mcmc_values_kernel       the relocated opacity and scales of every distinct source (paper eq. 9, in double);
 //   mcmc_emit_*_kernel       the rows: in place over the dead rows (relocate), or into [P + n] copies (add).
 // Every step of the sampler is integer arithmetic and every histogram count is exact, so the same draws give the same bytes.
+// The emit table's checks, the CTA scan, the grid size and the row range are gsb_common.cuh's, shared with gsb_densify.cu.
 #include "gsb_common.cuh"
 
 namespace gsb {
@@ -113,28 +114,6 @@ __device__ __forceinline__ unsigned long long packed_row(const McmcPlanArgs& a, 
 	return (w << MC_DEAD_BITS) | (dead ? 1ull : 0ull);
 }
 
-// exclusive scan of v over the CTA (blockDim.x a multiple of 32, at most 1024); *total = the CTA's sum
-__device__ __forceinline__ unsigned long long cta_exclusive(unsigned long long v, unsigned long long* s_warp, unsigned long long* total)
-{
-	const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-	unsigned long long incl = v;
-#pragma unroll
-	for (int o = 1; o < 32; o <<= 1) { const unsigned long long u = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += u; }
-	__syncthreads();                                   // s_warp may still be read by a previous call
-	if (lane == 31) s_warp[warp] = incl;
-	__syncthreads();
-	if (warp == 0)
-	{
-		unsigned long long x = lane < nw ? s_warp[lane] : 0ull;
-#pragma unroll
-		for (int o = 1; o < 32; o <<= 1) { const unsigned long long u = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += u; }
-		if (lane < nw) s_warp[lane] = x;
-	}
-	__syncthreads();
-	*total = s_warp[nw - 1];
-	return (warp ? s_warp[warp - 1] : 0ull) + incl - v;
-}
-
 __global__ void __launch_bounds__(MC_THREADS) mcmc_reduce_kernel(const McmcPlanArgs a, McmcWorkspace w)
 {
 	__shared__ unsigned long long s_warp[32];
@@ -144,7 +123,7 @@ __global__ void __launch_bounds__(MC_THREADS) mcmc_reduce_kernel(const McmcPlanA
 	for (int i = 0; i < MC_ITEMS; i++)
 		if (row0 + i < a.P) mine += packed_row(a, row0 + i);
 	unsigned long long total;
-	cta_exclusive(mine, s_warp, &total);
+	cta_exclusive<MC_THREADS>(mine, s_warp, &total);
 	if (threadIdx.x == 0) w.tile_sum[blockIdx.x] = total;
 }
 
@@ -157,8 +136,8 @@ __global__ void __launch_bounds__(MC_SCAN_THREADS) mcmc_tile_scan_kernel(McmcWor
 		const uint32_t t = base + threadIdx.x;
 		const unsigned long long s = t < w.n_tiles ? w.tile_sum[t] : 0ull;
 		unsigned long long tw, td;
-		const unsigned long long ew = cta_exclusive(s >> MC_DEAD_BITS, s_warp, &tw);
-		const unsigned long long ed = cta_exclusive(s & ((1ull << MC_DEAD_BITS) - 1), s_warp, &td);
+		const unsigned long long ew = cta_exclusive<MC_SCAN_THREADS>(s >> MC_DEAD_BITS, s_warp, &tw);
+		const unsigned long long ed = cta_exclusive<MC_SCAN_THREADS>(s & ((1ull << MC_DEAD_BITS) - 1), s_warp, &td);
 		if (t < w.n_tiles) { w.tile_w[t] = run_w + ew; w.tile_d[t] = (uint32_t)(run_d + ed); }
 		run_w += tw;
 		run_d += td;
@@ -186,7 +165,7 @@ __global__ void __launch_bounds__(MC_THREADS) mcmc_scan_kernel(const McmcPlanArg
 		mine += p[i];
 	}
 	unsigned long long total;
-	const unsigned long long excl = cta_exclusive(mine, s_warp, &total);
+	const unsigned long long excl = cta_exclusive<MC_THREADS>(mine, s_warp, &total);
 	unsigned long long run_w = w.tile_w[blockIdx.x] + (excl >> MC_DEAD_BITS);
 	uint32_t run_d = w.tile_d[blockIdx.x] + (uint32_t)(excl & ((1ull << MC_DEAD_BITS) - 1));
 #pragma unroll
@@ -267,11 +246,6 @@ __global__ void __launch_bounds__(MC_THREADS) mcmc_values_kernel(McmcWorkspace w
 }
 
 // ------------------------------------------------------------------------------------------------ emit
-struct McmcTable {
-	GsbDensifyTensor t[GSB_DENSIFY_MAX_TENSORS];
-	double inv_width[GSB_DENSIFY_MAX_TENSORS];
-};
-
 // the stored value of a relocated row: inverse_sigmoid(o') = log(o' / (1 - o')) and log(s'), in fp32 as torch evaluates them
 __device__ __forceinline__ uint32_t stored(int kind, const float4& v, int c)
 {
@@ -282,7 +256,7 @@ __device__ __forceinline__ bool relocates(int kind) { return kind == GSB_MCMC_OP
 
 // relocate, in place: element (j, c) of the n_used dead rows.  Dead row j takes its source's row (the relocated value in an opacity
 // / scaling entry); the source's owner draw writes the source's relocated value and zeroes its moments.
-__global__ void __launch_bounds__(MC_THREADS) mcmc_emit_relocate_kernel(const __grid_constant__ McmcTable tab, McmcWorkspace w, long long n)
+__global__ void __launch_bounds__(MC_THREADS) mcmc_emit_relocate_kernel(const __grid_constant__ RowTable tab, McmcWorkspace w, long long n)
 {
 	const GsbDensifyTensor& k = tab.t[blockIdx.y];
 	const int wd = k.row_width;
@@ -309,7 +283,7 @@ __global__ void __launch_bounds__(MC_THREADS) mcmc_emit_relocate_kernel(const __
 // add: every element of the [P + n, row_width] destination.  Rows < P copy the source tensor (a sampled row's opacity / scaling
 // takes its relocated value and its moments are zeroed); row P + j copies draw j's source row (relocated opacity / scaling) with
 // zero moments, or is zero in a GSB_MCMC_FRESH entry.
-__global__ void __launch_bounds__(MC_THREADS) mcmc_emit_add_kernel(const __grid_constant__ McmcTable tab, McmcWorkspace w, long long P,
+__global__ void __launch_bounds__(MC_THREADS) mcmc_emit_add_kernel(const __grid_constant__ RowTable tab, McmcWorkspace w, long long P,
 	long long n)
 {
 	const GsbDensifyTensor& k = tab.t[blockIdx.y];
@@ -341,11 +315,10 @@ __global__ void __launch_bounds__(MC_THREADS) mcmc_emit_add_kernel(const __grid_
 	}
 }
 
-static int mcmc_grid(long long work)
-{
-	const long long want = (work + MC_THREADS - 1) / MC_THREADS, cap = (long long)GSB_NUM_SMS * 8;
-	return (int)(want < cap ? (want > 0 ? want : 1) : cap);
-}
+static const TableRules kEmitRules = {"mcmc_emit", "n_tensors",
+	(1u << GSB_DENSIFY_COPY) | (1u << GSB_DENSIFY_SCALING) | (1u << GSB_MCMC_OPACITY) | (1u << GSB_MCMC_FRESH),
+	"%s: tensor %d: kind %d is not COPY, SCALING, MCMC_OPACITY or MCMC_FRESH",
+	"%s: tensor %d: a scaling entry needs row_width 3, an opacity entry 1; got %d", false};
 
 } // namespace gsb
 
@@ -354,14 +327,14 @@ using namespace gsb;
 extern "C" int gsb_mcmc_noise(int32_t P, float* xyz, const float* scaling, const float* rotation, const float* opacity_logits,
 	const float* draws, float noise_lr, float xyz_lr, void* stream)
 {
-	if (P < 0 || P >= (1 << 30)) { set_error("mcmc_noise: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
+	if (!rows_ok("mcmc_noise", P)) return GSB_EINVAL;
 	if (!isfinite(noise_lr) || !isfinite(xyz_lr)) { set_error("mcmc_noise: noise_lr and xyz_lr must be finite"); return GSB_EINVAL; }
 	if (P == 0) return GSB_OK;
 	if (!xyz || !scaling || !rotation || !opacity_logits || !draws)
 	{ set_error("mcmc_noise: NULL xyz / scaling / rotation / opacity_logits / draws"); return GSB_EINVAL; }
 	const cudaStream_t st = (cudaStream_t)stream;
 	ProfScope prof(K_TOOLS, st);
-	mcmc_noise_kernel<<<mcmc_grid(P), MC_THREADS, 0, st>>>(P, xyz, scaling, rotation, opacity_logits, draws, noise_lr, xyz_lr);
+	mcmc_noise_kernel<<<grid_stride_ctas(P, MC_THREADS, 8), MC_THREADS, 0, st>>>(P, xyz, scaling, rotation, opacity_logits, draws, noise_lr, xyz_lr);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
@@ -372,7 +345,7 @@ extern "C" size_t gsb_mcmc_workspace_bytes(int32_t P) { return mcmc_carve(nullpt
 extern "C" int gsb_mcmc_plan(int32_t P, int32_t mode, const float* opacity_logits, const float* scaling, const uint8_t* dead_mask,
 	float min_opacity, int64_t n, const int64_t* draws, void* workspace, int64_t* counts, void* stream)
 {
-	if (P < 0 || P >= (1 << 30)) { set_error("mcmc_plan: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
+	if (!rows_ok("mcmc_plan", P)) return GSB_EINVAL;
 	if (mode != GSB_MCMC_RELOCATE && mode != GSB_MCMC_ADD) { set_error("mcmc_plan: unknown mode %d", mode); return GSB_EINVAL; }
 	if (dead_mask && mode != GSB_MCMC_RELOCATE) { set_error("mcmc_plan: dead_mask given with GSB_MCMC_ADD"); return GSB_EINVAL; }
 	if (!workspace) { set_error("mcmc_plan: NULL workspace"); return GSB_EINVAL; }
@@ -404,9 +377,9 @@ extern "C" int gsb_mcmc_plan(int32_t P, int32_t mode, const float* opacity_logit
 	}
 	GSB_CUDA_OK(cudaMemsetAsync(w.count, 0, sizeof(uint32_t) * (size_t)P, st));
 	GSB_CUDA_OK(cudaMemsetAsync(w.owner, 0xff, sizeof(uint32_t) * (size_t)P, st));
-	mcmc_sample_kernel<<<mcmc_grid(n), MC_THREADS, 0, st>>>(w, P, mode, n, reinterpret_cast<const long long*>(draws));
+	mcmc_sample_kernel<<<grid_stride_ctas(n, MC_THREADS, 8), MC_THREADS, 0, st>>>(w, P, mode, n, reinterpret_cast<const long long*>(draws));
 	GSB_LAUNCHED();
-	mcmc_values_kernel<<<mcmc_grid(n), MC_THREADS, 0, st>>>(w, mode, n, opacity_logits, scaling);
+	mcmc_values_kernel<<<grid_stride_ctas(n, MC_THREADS, 8), MC_THREADS, 0, st>>>(w, mode, n, opacity_logits, scaling);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;
@@ -415,45 +388,28 @@ extern "C" int gsb_mcmc_plan(int32_t P, int32_t mode, const float* opacity_logit
 extern "C" int gsb_mcmc_emit(const GsbDensifyTensor* tensors, int32_t n_tensors, int32_t P, int32_t mode, int64_t n, const void* workspace,
 	void* stream)
 {
-	if (n_tensors < 0 || n_tensors > GSB_DENSIFY_MAX_TENSORS)
-	{ set_error("mcmc_emit: n_tensors = %d is outside 0..%d", n_tensors, GSB_DENSIFY_MAX_TENSORS); return GSB_EINVAL; }
-	if (n_tensors > 0 && !tensors) { set_error("mcmc_emit: tensor table is NULL"); return GSB_EINVAL; }
-	if (P < 0 || P >= (1 << 30)) { set_error("mcmc_emit: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
+	if (!rows_ok("mcmc_emit", P)) return GSB_EINVAL;
 	if (mode != GSB_MCMC_RELOCATE && mode != GSB_MCMC_ADD) { set_error("mcmc_emit: unknown mode %d", mode); return GSB_EINVAL; }
 	if (n < 0 || n > P) { set_error("mcmc_emit: n = %lld is outside 0..P (= %d)", (long long)n, P); return GSB_EINVAL; }
 	if (!workspace) { set_error("mcmc_emit: NULL workspace"); return GSB_EINVAL; }
-	McmcTable tab{};
-	int max_w = 1;
+	RowTable tab{};
+	int max_w;
+	if (!fill_row_table(kEmitRules, tensors, n_tensors, true, P > 0, tab, max_w)) return GSB_EINVAL;
 	for (int i = 0; i < n_tensors; i++)
 	{
 		const GsbDensifyTensor& k = tensors[i];
-		if (k.row_width <= 0) { set_error("mcmc_emit: tensor %d: row_width %d <= 0", i, k.row_width); return GSB_EINVAL; }
-		if (k.kind != GSB_DENSIFY_COPY && k.kind != GSB_DENSIFY_SCALING && k.kind != GSB_MCMC_OPACITY && k.kind != GSB_MCMC_FRESH)
-		{ set_error("mcmc_emit: tensor %d: kind %d is not COPY, SCALING, MCMC_OPACITY or MCMC_FRESH", i, k.kind); return GSB_EINVAL; }
-		if ((k.kind == GSB_DENSIFY_SCALING && k.row_width != 3) || (k.kind == GSB_MCMC_OPACITY && k.row_width != 1))
-		{ set_error("mcmc_emit: tensor %d: a scaling entry needs row_width 3, an opacity entry 1; got %d", i, k.row_width); return GSB_EINVAL; }
 		if (k.kind == GSB_MCMC_FRESH && (mode != GSB_MCMC_ADD || k.exp_avg_src))
 		{ set_error("mcmc_emit: tensor %d: an MCMC_FRESH entry belongs to GSB_MCMC_ADD and has no moments", i); return GSB_EINVAL; }
 		if (k.grad_src || k.grad_dst) { set_error("mcmc_emit: tensor %d: grad pointers must be NULL", i); return GSB_EINVAL; }
-		if (!k.exp_avg_src != !k.exp_avg_dst || !k.exp_avg_src != !k.exp_avg_sq_src || !k.exp_avg_src != !k.exp_avg_sq_dst)
-		{ set_error("mcmc_emit: tensor %d: exp_avg / exp_avg_sq are half given", i); return GSB_EINVAL; }
-		if (P > 0 && (!k.src || !k.dst)) { set_error("mcmc_emit: tensor %d: NULL src / dst", i); return GSB_EINVAL; }
 		if (mode == GSB_MCMC_RELOCATE && (k.src != k.dst || k.exp_avg_src != k.exp_avg_dst || k.exp_avg_sq_src != k.exp_avg_sq_dst))
 		{ set_error("mcmc_emit: tensor %d: GSB_MCMC_RELOCATE works in place (dst == src for the param and both moments)", i); return GSB_EINVAL; }
-		const uintptr_t any = reinterpret_cast<uintptr_t>(k.src) | reinterpret_cast<uintptr_t>(k.dst) |
-			reinterpret_cast<uintptr_t>(k.exp_avg_src) | reinterpret_cast<uintptr_t>(k.exp_avg_dst) |
-			reinterpret_cast<uintptr_t>(k.exp_avg_sq_src) | reinterpret_cast<uintptr_t>(k.exp_avg_sq_dst);
-		if (any & 3u) { set_error("mcmc_emit: tensor %d: a pointer is not 4-byte aligned", i); return GSB_EINVAL; }
-		tab.t[i] = k;
-		tab.inv_width[i] = 1.0 / k.row_width;
-		max_w = k.row_width > max_w ? k.row_width : max_w;
 	}
 	const long long rows = mode == GSB_MCMC_ADD ? (long long)P + n : n;
 	if (n_tensors == 0 || rows == 0) return GSB_OK;
 	const McmcWorkspace w = mcmc_carve(static_cast<char*>(const_cast<void*>(workspace)), P);
 	const cudaStream_t st = (cudaStream_t)stream;
 	ProfScope prof(K_TOOLS, st);
-	const dim3 grid((unsigned)mcmc_grid(rows * max_w), (unsigned)n_tensors);
+	const dim3 grid((unsigned)grid_stride_ctas(rows * max_w, MC_THREADS, 8), (unsigned)n_tensors);
 	if (mode == GSB_MCMC_ADD) mcmc_emit_add_kernel<<<grid, MC_THREADS, 0, st>>>(tab, w, P, n);
 	else mcmc_emit_relocate_kernel<<<grid, MC_THREADS, 0, st>>>(tab, w, n);
 	GSB_LAUNCHED();

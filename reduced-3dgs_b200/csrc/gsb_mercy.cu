@@ -10,7 +10,8 @@
 //   mercy_select_kernel       the lower median of the redundant rows (torch.median) and the two ranks torch.quantile interpolates;
 //   mercy_mask_kernel       the prune mask and its counts; for 'redundancy_random' the redundant rows' ranks in index order
 //                           (decoupled look-back) pick their draw.
-// Every result is an integer count or an order statistic, so the outputs are the same bytes on every run.
+// Every result is an integer count or an order statistic, so the outputs are the same bytes on every run.  The CTA scan, the grid
+// size and the row range are gsb_common.cuh's, shared with gsb_densify.cu and gsb_mcmc.cu.
 #include "gsb_common.cuh"
 
 namespace gsb {
@@ -183,7 +184,7 @@ __global__ void __launch_bounds__(MERCY_THREADS) mercy_select_kernel(const Mercy
 {
 	constexpr int PER = MERCY_BINS / MERCY_THREADS;
 	__shared__ unsigned long long s_warp[MERCY_THREADS / 32];
-	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int tid = threadIdx.x;
 	const int width = pass_width(pass), nbins = 1 << width;
 	for (int t = 0; t < MERCY_TARGETS; t++)
 	{
@@ -191,13 +192,8 @@ __global__ void __launch_bounds__(MERCY_THREADS) mercy_select_kernel(const Mercy
 		const uint32_t* h = hist + (size_t)t * MERCY_BINS;
 		unsigned long long mine = 0;
 		for (int k = 0; k < PER; k++) { const int b = tid * PER + k; mine += b < nbins ? h[b] : 0u; }
-		unsigned long long incl = mine;
-#pragma unroll
-		for (int o = 1; o < 32; o <<= 1) { const unsigned long long v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-		if (lane == 31) s_warp[warp] = incl;
-		__syncthreads();
-		unsigned long long before = incl - mine, total = 0;
-		for (int k = 0; k < MERCY_THREADS / 32; k++) { if (k < warp) before += s_warp[k]; total += s_warp[k]; }
+		unsigned long long total;
+		const unsigned long long before = cta_exclusive<MERCY_THREADS>(mine, s_warp, &total);
 		if (pass == 0)
 		{
 			if (tid == 0)
@@ -247,8 +243,8 @@ __global__ void __launch_bounds__(MERCY_THREADS) mercy_mask_kernel(const MercyAr
 	uint32_t* __restrict__ lookback, uint32_t* __restrict__ ticket, uint8_t* __restrict__ mask, long long* __restrict__ counts_out)
 {
 	__shared__ uint32_t s_tile, s_excl;
-	__shared__ uint32_t s_warp[MERCY_THREADS / 32], s_warp2[MERCY_THREADS / 32];
-	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	__shared__ uint32_t s_warp[MERCY_THREADS / 32];
+	const int tid = threadIdx.x;
 	if (tid == 0) s_tile = atomicAdd(ticket, 1u);
 	__syncthreads();
 	const uint32_t tile = s_tile;
@@ -262,14 +258,9 @@ __global__ void __launch_bounds__(MERCY_THREADS) mercy_mask_kernel(const MercyAr
 		red[i] = row0 + i < a.P && is_redundant(a.counts[row0 + i], thr);
 		n_red += red[i] ? 1u : 0u;
 	}
-	// CTA-wide exclusive scan of the redundant rows (every CTA takes part so that the look-back chain is complete)
-	uint32_t incl = n_red;
-#pragma unroll
-	for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-	if (lane == 31) s_warp[warp] = incl;
-	__syncthreads();
-	uint32_t run = incl - n_red, cta_total = 0;
-	for (int k = 0; k < MERCY_THREADS / 32; k++) { if (k < warp) run += s_warp[k]; cta_total += s_warp[k]; }
+	// the redundant rows' ranks (every CTA takes part so that the look-back chain is complete)
+	uint32_t cta_total;
+	uint32_t run = cta_exclusive<MERCY_THREADS>(n_red, s_warp, &cta_total);
 	if (a.draws && tid == 0) s_excl = lookback_exclusive(lookback, tile, 1, 0, cta_total);
 	__syncthreads();
 	if (a.draws) run += s_excl;
@@ -296,14 +287,10 @@ __global__ void __launch_bounds__(MERCY_THREADS) mercy_mask_kernel(const MercyAr
 			run += red[i] ? 1u : 0u;
 		}
 	}
-#pragma unroll
-	for (int o = 16; o > 0; o >>= 1) n_pruned += __shfl_xor_sync(0xffffffffu, n_pruned, o);
-	if (lane == 0) s_warp2[warp] = n_pruned;
-	__syncthreads();
+	uint32_t np;
+	cta_exclusive<MERCY_THREADS>(n_pruned, s_warp, &np);
 	if (tid == 0)
 	{
-		uint32_t np = 0;
-		for (int k = 0; k < MERCY_THREADS / 32; k++) np += s_warp2[k];
 		if (cta_total) atomicAdd(reinterpret_cast<unsigned long long*>(counts_out), (unsigned long long)cta_total);
 		if (np) atomicAdd(reinterpret_cast<unsigned long long*>(counts_out + 1), (unsigned long long)np);
 	}
@@ -319,7 +306,7 @@ extern "C" int gsb_mercy_plan(int32_t P, const int32_t* counts, const float* opa
 	double mercy_minimum, float quantile_q, const float* draws, int64_t n_draws, void* workspace, uint8_t* mask, float* thresholds,
 	int64_t* counts_out, void* stream)
 {
-	if (P < 0 || P >= (1 << 30)) { set_error("mercy_plan: P = %d is outside 0..2^30 - 1", P); return GSB_EINVAL; }
+	if (!rows_ok("mercy_plan", P)) return GSB_EINVAL;
 	if (type < GSB_MERCY_REDUNDANCY_OPACITY || type > GSB_MERCY_REDUNDANCY) { set_error("mercy_plan: unknown type %d", type); return GSB_EINVAL; }
 	if (!workspace || !thresholds || !counts_out) { set_error("mercy_plan: NULL workspace / thresholds / counts_out"); return GSB_EINVAL; }
 	if (draws && type != GSB_MERCY_REDUNDANCY_RANDOM) { set_error("mercy_plan: draws are only read by the random type"); return GSB_EINVAL; }
@@ -339,7 +326,7 @@ extern "C" int gsb_mercy_plan(int32_t P, const int32_t* counts, const float* opa
 	MercyArgs a;
 	a.counts = counts; a.logits = opacity_logits; a.draws = draws; a.n_draws = n_draws; a.P = P; a.type = type;
 	a.want_median = want_median; a.want_quantile = want_quantile;
-	const int grid = (int)((P + MERCY_THREADS - 1) / MERCY_THREADS < GSB_NUM_SMS * 2 ? (P + MERCY_THREADS - 1) / MERCY_THREADS : GSB_NUM_SMS * 2);
+	const int grid = grid_stride_ctas(P, MERCY_THREADS, 2);
 	if (P > 0)
 	{
 		mercy_sums_kernel<<<grid, MERCY_THREADS, 0, st>>>(P, counts, w.state);

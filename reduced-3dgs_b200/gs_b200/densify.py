@@ -304,54 +304,72 @@ def _pruned(counts):
 
 def _emit(model, groups, P, dev, ws, counts, store_grads, gather_stats, samples=None):
     n_kept, _, n_clones_kept, S, n_children, P_out = counts[:6]
-    entries, new = [], []
-    for name, g, p, state in groups:
-        dst = torch.empty((P_out,) + tuple(p.shape[1:]), dtype=torch.float32, device=dev)
-        e = gsl.GsbDensifyTensor()
-        e.src, e.dst = p.data_ptr(), dst.data_ptr()
-        e.row_width = p.shape[1:].numel()
-        e.kind = {"xyz": gsl.DENSIFY_XYZ, "scaling": gsl.DENSIFY_SCALING}.get(name, gsl.DENSIFY_COPY)
-        m = v = gr = None
-        if state is not None:
-            m, v = torch.empty_like(dst), torch.empty_like(dst)
-            e.exp_avg_src, e.exp_avg_dst = state["exp_avg"].data_ptr(), m.data_ptr()
-            e.exp_avg_sq_src, e.exp_avg_sq_dst = state["exp_avg_sq"].data_ptr(), v.data_ptr()
-            if store_grads:
-                gr = torch.empty_like(dst)
-                e.grad_src, e.grad_dst = p.grad.data_ptr(), gr.data_ptr()
-        entries.append(e)
-        new.append((name, g, p, state, dst, m, v, gr))
-    stats = [("_degrees", torch.int32, (1,))]
-    if gather_stats:
-        stats += [("xyz_gradient_accum", torch.float32, (1,)), ("denom", torch.float32, (1,)), ("max_radii2D", torch.float32, ())]
-        if getattr(model, "xyz_gradient_accum_abs", None) is not None:
-            stats.append(("xyz_gradient_accum_abs", torch.float32, (1,)))
-    out_stats = {}
-    for attr, dtype, row in stats:
-        src = getattr(model, attr)
-        dst = torch.empty((P_out,) + row, dtype=dtype, device=dev)
-        e = gsl.GsbDensifyTensor()
-        e.src, e.dst, e.row_width, e.kind = src.data_ptr(), dst.data_ptr(), 1, gsl.DENSIFY_COPY
-        entries.append(e)
-        out_stats[attr] = dst
+    entries, install = _resized(model, groups, P_out, dev, {"xyz": gsl.DENSIFY_XYZ, "scaling": gsl.DENSIFY_SCALING},
+                                gsl.DENSIFY_COPY if gather_stats else None, store_grads)
     rot = next(p for name, _, p, _ in groups if name == "rotation")
     table = (gsl.GsbDensifyTensor * len(entries))(*entries)
     with gsl.on_device(dev):
         gsl.check(gsl.lib().gsb_densify_emit(table, len(entries), P, ws.data_ptr(), n_kept, n_clones_kept, S, n_children,
                                               rot.data_ptr(), None if samples is None or samples.numel() == 0 else samples.data_ptr(),
                                               split_scale_factor(), gsl.current_stream(dev)))
-    # the reference's optimizer surgery (_prune_optimizer / cat_tensors_to_optimizer): the state dict object moves to the new
-    # Parameter with the new moments; a group without state only gets its param; .grad travels only with state and store_grads
-    opt = model.optimizer
-    for name, g, p, state, dst, m, v, gr in new:
-        param = nn.Parameter(dst.requires_grad_(True))
+    install()
+
+
+def _entry(src, dst, kind, moments_src=None, moments_dst=None, grad_src=None, grad_dst=None):
+    """One GsbDensifyTensor row of the densify / MCMC emit tables; moments are (exp_avg, exp_avg_sq) pairs."""
+    e = gsl.GsbDensifyTensor()
+    e.src, e.dst = src.data_ptr(), dst.data_ptr()
+    e.row_width = src.shape[1:].numel()
+    e.kind = kind
+    if moments_src is not None:
+        e.exp_avg_src, e.exp_avg_dst = moments_src[0].data_ptr(), moments_dst[0].data_ptr()
+        e.exp_avg_sq_src, e.exp_avg_sq_dst = moments_src[1].data_ptr(), moments_dst[1].data_ptr()
+    if grad_src is not None:
+        e.grad_src, e.grad_dst = grad_src.data_ptr(), grad_dst.data_ptr()
+    return e
+
+
+STATS = ("xyz_gradient_accum", "denom", "max_radii2D", "xyz_gradient_accum_abs")
+
+
+def _resized(model, groups, P_out, dev, kinds, stat_kind, store_grads=False):
+    """The [P_out] rows of a resized model and their emit table entries: each group's param (kind from `kinds`, else COPY), its
+    moments if it has state and then with store_grads its .grad; _degrees (COPY); unless stat_kind is None, the STATS the model has.
+    -> (entries, install).  install(), after the emit, sets the statistics and does the reference's optimizer surgery
+    (_prune_optimizer / cat_tensors_to_optimizer): the state dict object moves to the new Parameter with the new moments; a group
+    without state only gets its param; .grad travels only with state and store_grads."""
+    entries, new = [], []
+    for name, g, p, state in groups:
+        dst = torch.empty((P_out,) + tuple(p.shape[1:]), dtype=torch.float32, device=dev)
+        mv = gr = None
         if state is not None:
-            state["exp_avg"], state["exp_avg_sq"] = m, v
-            del opt.state[p]
-            if gr is not None:
-                param.grad = gr
-            opt.state[param] = state
-        g["params"][0] = param
-        setattr(model, ATTR[name], param)
-    for attr, t in out_stats.items():
-        setattr(model, attr, t)
+            mv = (torch.empty_like(dst), torch.empty_like(dst))
+            if store_grads:
+                gr = torch.empty_like(dst)
+        moments = None if state is None else (state["exp_avg"], state["exp_avg_sq"])
+        entries.append(_entry(p, dst, kinds.get(name, gsl.DENSIFY_COPY), moments, mv, None if gr is None else p.grad, gr))
+        new.append((name, g, p, state, dst, mv, gr))
+    stats = [("_degrees", gsl.DENSIFY_COPY)]
+    if stat_kind is not None:
+        stats += [(k, stat_kind) for k in STATS if getattr(model, k, None) is not None]
+    out_stats = {}
+    for attr, kind in stats:
+        src = getattr(model, attr)
+        out_stats[attr] = torch.empty((P_out,) + tuple(src.shape[1:]), dtype=src.dtype, device=dev)
+        entries.append(_entry(src, out_stats[attr], kind))
+
+    def install():
+        opt = model.optimizer
+        for name, g, p, state, dst, mv, gr in new:
+            param = nn.Parameter(dst.requires_grad_(True))
+            if state is not None:
+                state["exp_avg"], state["exp_avg_sq"] = mv
+                del opt.state[p]
+                if gr is not None:
+                    param.grad = gr
+                opt.state[param] = state
+            g["params"][0] = param
+            setattr(model, ATTR[name], param)
+        for attr, t in out_stats.items():
+            setattr(model, attr, t)
+    return entries, install

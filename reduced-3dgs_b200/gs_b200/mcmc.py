@@ -17,6 +17,8 @@ bytes on every run for the same generator state.  The relocated opacity and scal
 
 Kept quirk of the authors' code (and gsplat's): relocate_gs zeroes the Adam moments of the sampled SOURCE rows; the dead rows that
 receive their parameters keep their own moments.
+
+The emit table entries (densify._entry) and add_new_gs's allocation and optimizer surgery (densify._resized) are densify's.
 """
 from __future__ import annotations
 
@@ -24,7 +26,6 @@ import ctypes as C
 import numbers
 
 import torch
-from torch import nn
 
 from . import densify
 from . import lib as gsl
@@ -69,8 +70,11 @@ def relocate_gs(model, dead_mask=None):
         return
     draws = torch.randint(0, 2 ** 62, (n_dead,), dtype=torch.int64, device=dev)
     _plan(groups, P, dev, gsl.MCMC_RELOCATE, mask, ws, draws)
-    entries = [_entry(name, p, p, state, None) for name, _, p, state in groups]
-    entries.append(_stat_entry(model._degrees, model._degrees, gsl.DENSIFY_COPY))
+    entries = []
+    for name, _, p, state in groups:
+        moments = None if state is None else (state["exp_avg"], state["exp_avg_sq"])
+        entries.append(densify._entry(p, p, KIND.get(name, gsl.DENSIFY_COPY), moments, moments))
+    entries.append(densify._entry(model._degrees, model._degrees, gsl.DENSIFY_COPY))
     _emit(entries, P, dev, gsl.MCMC_RELOCATE, n_dead, ws)
     for _, _, p, _ in groups:
         p.grad = None
@@ -93,32 +97,9 @@ def add_new_gs(model, cap_max):
         return 0
     draws = torch.randint(0, 2 ** 62, (n,), dtype=torch.int64, device=dev)
     _plan(groups, P, dev, gsl.MCMC_ADD, None, ws, draws)
-    entries, new = [], []
-    for name, g, p, state in groups:
-        dst = torch.empty((P + n,) + tuple(p.shape[1:]), dtype=torch.float32, device=dev)
-        mv = (torch.empty_like(dst), torch.empty_like(dst)) if state is not None else None
-        entries.append(_entry(name, p, dst, state, mv))
-        new.append((name, g, p, state, dst, mv))
-    stats = [("_degrees", torch.int32, (1,), gsl.DENSIFY_COPY)] + [
-        (k, torch.float32, row, gsl.MCMC_FRESH) for k, row in (("xyz_gradient_accum", (1,)), ("denom", (1,)), ("max_radii2D", ()),
-                                                                ("xyz_gradient_accum_abs", (1,)))
-        if getattr(model, k, None) is not None]
-    out_stats = {}
-    for attr, dtype, row, kind in stats:
-        out_stats[attr] = torch.empty((P + n,) + row, dtype=dtype, device=dev)
-        entries.append(_stat_entry(getattr(model, attr), out_stats[attr], kind))
+    entries, install = densify._resized(model, groups, P + n, dev, KIND, gsl.MCMC_FRESH)
     _emit(entries, P, dev, gsl.MCMC_ADD, n, ws)
-    opt = model.optimizer
-    for name, g, p, state, dst, mv in new:
-        param = nn.Parameter(dst.requires_grad_(True))
-        if state is not None:
-            state["exp_avg"], state["exp_avg_sq"] = mv
-            del opt.state[p]
-            opt.state[param] = state
-        g["params"][0] = param
-        setattr(model, densify.ATTR[name], param)
-    for attr, t in out_stats.items():
-        setattr(model, attr, t)
+    install()
     return n
 
 
@@ -137,24 +118,6 @@ def _plan(groups, P, dev, mode, mask=None, ws=None, draws=None):
                                           0 if draws is None else draws.numel(), None if draws is None else draws.data_ptr(),
                                           ws.data_ptr(), None if counts is None else counts.data_ptr(), gsl.current_stream(dev)))
     return ws, counts
-
-
-def _entry(name, src, dst, state, moments):
-    e = gsl.GsbDensifyTensor()
-    e.src, e.dst = src.data_ptr(), dst.data_ptr()
-    e.row_width = src.shape[1:].numel()
-    e.kind = KIND.get(name, gsl.DENSIFY_COPY)
-    if state is not None:
-        m, v = moments if moments is not None else (state["exp_avg"], state["exp_avg_sq"])
-        e.exp_avg_src, e.exp_avg_dst = state["exp_avg"].data_ptr(), m.data_ptr()
-        e.exp_avg_sq_src, e.exp_avg_sq_dst = state["exp_avg_sq"].data_ptr(), v.data_ptr()
-    return e
-
-
-def _stat_entry(src, dst, kind):
-    e = gsl.GsbDensifyTensor()
-    e.src, e.dst, e.row_width, e.kind = src.data_ptr(), dst.data_ptr(), 1, kind
-    return e
 
 
 def _emit(entries, P, dev, mode, n, ws):
