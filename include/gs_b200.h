@@ -83,6 +83,11 @@ typedef struct GsbScene {
 	int32_t sh_packed;           /* != 0: variable-SH inference layout, forward.cu:19-36 getSHOffset    */
 	int32_t band_count[4];       /* [host] perBandPrimitiveCount (Gaussians are ordered by degree)      */
 	const uint8_t* prune_mask;   /* [P] or NULL; 1 = pruned: behaves as culled (radii 0, no instances, zero grads) */
+	const float* filter_3D;      /* [P] or NULL: Mip-Splatting's 3D smoothing filter f >= 0 (DESIGN.md §5o).  Each activated scale
+	                                becomes sqrt(s^2 + f^2) (then times scale_modifier) and the opacity sigmoid(logit) * c3,
+	                                c3 = sqrt(prod s_k^2 / prod (s_k^2 + f^2)); a row with f == 0 is the unfiltered arithmetic exactly.
+	                                The filter is a constant (no gradient).  With a filter the backward reads the opacity logits
+	                                (opacities, or quant->ids_opacity).  Not with cov3D_precomp, nor with the statistics forward. */
 	const GsbQuant* quant;       /* [host struct] or NULL; when set, opacities/scales/rotations/shs are ignored */
 } GsbScene;
 
@@ -141,10 +146,11 @@ GSB_API size_t gsb_binning_bytes(int64_t num_rendered);
  * launched or written.  gsb_last_error() then starts with "forward: " or "backward: ".  The code is GSB_EINVAL except where marked.
  *   Forward:  1. scene NULL or P < 0;  2. features: F outside 1..GSB_FEATURES_MAX, a NULL out, and with P > 0 a NULL
  *             features->features;  3. one map output without the other;  4. statistics: one output without the other, then
- *             statistics together with the maps, antialiasing or raw; with deterministic then a NULL workspace with P > 0, and
- *             GSB_ERANGE for width * height >= 2^28;  5. raw parameters: the raw checks (at GsbRawParams);  6. the camera: NULL, a bad
+ *             statistics together with the maps, antialiasing or raw, then with a scene filter_3D; with deterministic then a NULL
+ *             workspace with P > 0, and GSB_ERANGE for width * height >= 2^28;  5. raw parameters: the raw checks (at GsbRawParams);  6. the camera: NULL, a bad
  *             image size, a NULL camera tensor;  7. with P > 0 the scene's tensors (means3D; the codebooks, or opacities and,
- *             without raw parameters, exactly one of shs / colors_precomp and of scales + rotations / cov3D_precomp);
+ *             without raw parameters, exactly one of shs / colors_precomp and of scales + rotations / cov3D_precomp, then a
+ *             filter_3D with cov3D_precomp);
  *             8. out_color, num_rendered, and radii with P > 0.
  *   Backward: 1. scene NULL or P < 0;  2. features: deterministic set, then F outside 1..GSB_FEATURES_MAX, and with P > 0 NULL
  *             features, dL_dout or dL_dfeatures;  3. absgrad: features given, then grads->accumulate set;  4. num_rendered < 0;
@@ -361,6 +367,20 @@ GSB_API int gsb_sh_statistics_update(int32_t P, int32_t M, const int32_t* degree
  * w2ndc / w2ndc_inverse: [n_cameras,4,4] exactly as the reference passes them; heights / widths: int32 [n_cameras] on the device. */
 GSB_API int gsb_min_projected_pixel_size(int32_t P, const float* means3D, int32_t n_cameras, const float* w2ndc, const float* w2ndc_inverse,
                 const int32_t* image_heights, const int32_t* image_widths, float* pixel_sizes /* [P] */, void* stream);
+
+/* Mip-Splatting's 3D smoothing filter (Yu et al., CVPR 2024, compute_3D_filter; DESIGN.md §5o) of every centre, for GsbScene.filter_3D.
+ * Per centre x and camera c, with (x_v, y_v, z) = x in c's view space (xform_row of the transposed world_view_transform, the
+ * preprocess's depth): c sees x if z > 0.2 and u = fl(fl(x_v / max(z, 0.001)) fx) + W/2 lies in [fl32(-0.15 W), fl32(1.15 W)], and
+ * the same for v with y_v, fy and H.  dist = the smallest z of the cameras that see x; a centre no camera sees takes the largest
+ * dist of the seen centres; f = fl(fl(dist / F) * fl32(sqrt(0.2))) with F the largest fx over ALL cameras (Mip-Splatting's choice,
+ * kept).  No seen centre (or no camera): every f is 0.  viewmatrices [n,16] fp32 (world_view_transform, transposed), focals [n,2]
+ * fp32 (fx = W / (2 tan(FoVx / 2)), fy likewise), sizes [n,2] int32 (W, H); any number of cameras.  Two launches, asynchronous on
+ * `stream`, no host read; the same bytes on every run.  workspace: gsb_filter_3d_workspace_bytes() bytes of device memory.
+ * Errors (GSB_EINVAL, nothing launched): P < 0 or P >= 2^30, n_cameras < 0, and with P > 0 a NULL means3D / filter / workspace or,
+ * with n_cameras > 0, a NULL camera array. */
+GSB_API size_t gsb_filter_3d_workspace_bytes(void);
+GSB_API int gsb_filter_3d(int32_t P, const float* means3D, int32_t n_cameras, const float* viewmatrices, const float* focals,
+                const int32_t* sizes, float* filter /* [P] */, void* workspace, void* stream);
 
 /* redundancy_values[i] = number of the knn neighbours whose (scale + sphere_radius[i]) ellipsoid contains centre i,
  * intersection_mask[i,k] = that test per neighbour (Reduced3DGS::intersectionTest, reduced_3dgs.cu:205-243 +

@@ -104,6 +104,7 @@ int launch_stats_fixed_to_float(int, const unsigned long long*, float*, cudaStre
 int launch_sh_stats_update(int, int, const int*, const float*, const float*, const float*, const int*, const int*, const float*, float*, float*,
 	float*, float*, float*, cudaStream_t);
 int launch_pixel_size(int, const float*, int, const float*, const float*, const int*, const int*, float*, cudaStream_t);
+int launch_filter_3d(int, const float*, int, const float*, const float*, const int*, float*, unsigned*, cudaStream_t);
 int launch_sphere_ellipsoid(int, const float*, const float*, const float*, const int*, const float*, int, int*, uint8_t*, cudaStream_t);
 int launch_min_redundancy(int, const int*, const int*, const uint8_t*, int, int*, cudaStream_t);
 int launch_redundancy_fused(int, const float*, const float*, const float*, const int*, const float*, float, int, int*, cudaStream_t);
@@ -166,6 +167,8 @@ static int check_scene(const char* dir, const GsbScene* s, const GsbCamera* c, b
 	if (sr == (s->cov3D_precomp != nullptr) || ((s->scales != nullptr) != (s->rotations != nullptr)))
 	{ set_error("%s: Please provide exactly one of either scale/rotation pair or precomputed 3D covariance!", dir); return GSB_EINVAL; }
 	if (s->shs && !s->sh_packed && (!s->degrees || s->M <= 0)) { set_error("%s: dense SH needs degrees and M > 0", dir); return GSB_EINVAL; }
+	if (s->filter_3D && s->cov3D_precomp)
+	{ set_error("%s: filter_3D filters the scales; it does not go with cov3D_precomp", dir); return GSB_EINVAL; }
 	return GSB_OK;
 }
 
@@ -191,6 +194,7 @@ static int check_forward(const GsbForwardRequest& r)
 		if (!r.touched_pixels || !r.transmittance_sum) { set_error("forward: statistics output pointers missing"); return GSB_EINVAL; }
 		if (r.out_invdepth || r.antialiasing || r.raw)
 		{ set_error("forward: statistics go without the maps, antialiasing and raw parameters"); return GSB_EINVAL; }
+		if (s->filter_3D) { set_error("forward: statistics go without filter_3D (they keep the reference's definition)"); return GSB_EINVAL; }
 		if (r.deterministic)
 		{
 			if (s->P > 0 && !r.workspace) { set_error("forward: workspace is NULL"); return GSB_EINVAL; }
@@ -419,6 +423,19 @@ int gsb_min_projected_pixel_size(int32_t P, const float* means3D, int32_t n_came
 	if (P > 0 && (!means3D || !pixel_sizes || (n_cameras > 0 && (!w2ndc || !w2ndc_inverse || !image_heights || !image_widths))))
 	{ set_error("min_projected_pixel_size: NULL argument"); return GSB_EINVAL; }
 	return launch_pixel_size(P, means3D, n_cameras, w2ndc, w2ndc_inverse, image_heights, image_widths, pixel_sizes, (cudaStream_t)stream);
+}
+
+size_t gsb_filter_3d_workspace_bytes(void) { return 256; }
+
+int gsb_filter_3d(int32_t P, const float* means3D, int32_t n_cameras, const float* viewmatrices, const float* focals, const int32_t* sizes,
+	float* filter, void* workspace, void* stream)
+{
+	if (!rows_ok("filter_3d", P)) return GSB_EINVAL;
+	if (n_cameras < 0) { set_error("filter_3d: n_cameras < 0"); return GSB_EINVAL; }
+	if (P == 0) return GSB_OK;
+	if (!means3D || !filter || !workspace || (n_cameras > 0 && (!viewmatrices || !focals || !sizes)))
+	{ set_error("filter_3d: NULL argument"); return GSB_EINVAL; }
+	return launch_filter_3d(P, means3D, n_cameras, viewmatrices, focals, sizes, filter, static_cast<unsigned*>(workspace), (cudaStream_t)stream);
 }
 
 int gsb_sphere_ellipsoid_intersection(int32_t P, const float* means3D, const float* scales, const float* rotations, const int32_t* neighbours,

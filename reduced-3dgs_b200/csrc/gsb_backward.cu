@@ -28,6 +28,8 @@ struct BwdArgs {
 	// (an accumulate_into tensor) for its write-back; the scalar loops take the others.  Rotations are read as one float4: the
 	// Python layer hands over 16-byte aligned rows (lib.aligned16)
 	int sh_vec4, dsh_vec4;
+	// F3D (appended, as IN_RAW's fields): the [P] filter of DESIGN.md §5o and the opacity logits (NULL with QUANT: the ids are read)
+	const float* filter_3D; const float* opacities;
 };
 
 // Camera gradient slots (CAM): 0..11 view[4r+c] (r = 0..3, c = 0..2) at 3r+c; 12..23 proj[4r+j] (j = 0, 1, 3) at 12+3r+{0,1,2};
@@ -130,7 +132,11 @@ __device__ __forceinline__ void raw_block(const float* src, float* dst, int widt
 // (ExpBackward0), dL/d_rotation = autograd's F.normalize chain (tools/probe_torch_activations.py), the SH gradient row split
 // into its dc and rest parts.  A warp's 32 dc rows (96 floats) and 32 rest rows (96 C floats) are each contiguous and a multiple
 // of 16 bytes: they are staged into the padded rows and written back with 128-bit accesses.
-template <int IN, bool ACC, bool MAPS, bool CAM, bool AA>
+// F3D (Mip-Splatting's 3D filter, DESIGN.md §5o): the scales are filtered again as the forward filtered them (filter_3d), the
+// covariance chain runs on the filtered scales s', and a row with f != 0 then maps the scale gradient g (w.r.t. mod * s') back to s,
+// g s / s' + dL/do^ a sigmoid dc3/ds, and takes dL/dlogit = dL/do^ a c3 sigmoid (1 - sigmoid), with the sigmoid of the logit read
+// again (not o^ / c3, which is 0 / 0 on a flat splat).  A row with f == 0 keeps the unfiltered arithmetic.
+template <int IN, bool ACC, bool MAPS, bool CAM, bool AA, bool F3D>
 __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs a)
 {
 	constexpr bool QUANT = IN == IN_QUANT, RAW = IN == IN_RAW;
@@ -199,8 +205,14 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 		float4 acc0 = make_float4(0.f, 0.f, 0.f, 0.f), acc1 = acc0; float cyy = 0.f, dinvd = 0.f, mx = 0.f, my = 0.f, mz = 0.f, opac = 0.f;
 		float sc[3] = { 0, 0, 0 }, qr = 1, qx = 0, qy = 0, qz = 0;
 		uint32_t isb[3] = { 0, 0, 0 }, irw = 0; int deg_in = 0; unsigned cl_in = 0;
+		float f3d = 0.f, logit = 0.f; uint32_t iop = 0;
 		if (valid)
 		{
+			if (F3D)
+			{
+				f3d = a.filter_3D[idx];
+				if (QUANT) iop = a.q.ids_opacity[idx]; else logit = a.opacities[idx];
+			}
 			acc0 = reinterpret_cast<const float4*>(a.acc)[3 * idx];
 			acc1 = reinterpret_cast<const float4*>(a.acc)[3 * idx + 1];
 			if (MAPS) { const float2 c = reinterpret_cast<const float2*>(a.acc)[6 * idx + 4]; cyy = c.x; dinvd = c.y; }
@@ -235,20 +247,35 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 			const float g2x = acc1.x * (0.5f * a.W), g2y = acc1.y * (0.5f * a.H);
 			const float dconx = -0.5f * acc1.z, dcony = -0.5f * acc1.w, dconz = -0.5f * cyy;
 			float cov3D[6];
+			// F3D: s_act keeps the activated scales, sc becomes the filtered s' the covariance was built from
+			float s_act[3] = { 0, 0, 0 }, c3 = 1.f; Filter3DSquares f3sq;
+			auto filter = [&] {
+				if constexpr (F3D)
+				{
+					for (int k = 0; k < 3; k++) s_act[k] = sc[k];
+					c3 = filter_3d(sc[0], sc[1], sc[2], f3d, &f3sq);
+				}
+			};
 			if (QUANT)
 			{
 				for (int k = 0; k < 3; k++) sc[k] = quant_value(s_cb, CB_SCALING, isb[k]);
 				quant_rotation(s_cb, irw, qr, qx, qy, qz);
+				filter();
 				compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);
 			}
 			else if (RAW)
 			{
 				normalize_quat(qr, qx, qy, qz);
 				for (int k = 0; k < 3; k++) sc[k] = exp_ref(sc[k]);
+				filter();
 				compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);      // bit-identical to the forward's
 			}
 			else if (a.cov3D_precomp) { for (int k = 0; k < 6; k++) cov3D[k] = a.cov3D_precomp[6 * idx + k]; }
-			else compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);   // the forward computed exactly this; recomputing is bit-identical
+			else
+			{
+				filter();
+				compute_cov3D(sc[0], sc[1], sc[2], a.mod, qr, qx, qy, qz, cov3D);   // the forward computed exactly this; recomputing is bit-identical
+			}
 			float dmean[3], dcov[6];
 			float aa_s = 1.f, aa_q = 0.f;                                     // AA: the forward's opacity factor s and ratio q
 			// AA: s and the clamp decision are the forward's own bits: q is formed again from the same inputs with the forward's
@@ -460,10 +487,27 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 				o_rot[1] = 2 * y * (dMt[1][0] + dMt[0][1]) + 2 * z * (dMt[2][0] + dMt[0][2]) + 2 * r * (dMt[1][2] - dMt[2][1]) - 4 * x * (dMt[2][2] + dMt[1][1]);
 				o_rot[2] = 2 * x * (dMt[1][0] + dMt[0][1]) + 2 * r * (dMt[2][0] - dMt[0][2]) + 2 * z * (dMt[1][2] + dMt[2][1]) - 4 * y * (dMt[2][2] + dMt[0][0]);
 				o_rot[3] = 2 * r * (dMt[0][1] - dMt[1][0]) + 2 * x * (dMt[2][0] + dMt[0][2]) + 2 * y * (dMt[1][2] + dMt[2][1]) - 4 * z * (dMt[1][1] + dMt[0][0]);
+				if constexpr (F3D)
+				{
+					if (f3d != 0.f)
+					{
+						// s'_k = sqrt(s_k^2 + f^2): ds'_k/ds_k = s_k / s'_k.  c3 = prod_k s_k / s'_k, so with r = s^2 / s'^2
+						// dc3/ds_k = sqrt(r_i r_j) (1 - r_k) / s'_k, finite at s_k = 0 (flat splats)
+						const float sig = sigmoid_ref(QUANT ? quant_value(s_cb, CB_OPACITY, iop) : logit);
+						const float gs = acc0.w * (AA ? aa_s : 1.f) * sig;
+						float rr[3];
+						for (int k = 0; k < 3; k++) rr[k] = __fdiv_rn(f3sq.a[k], f3sq.b[k]);
+						for (int k = 0; k < 3; k++)
+						{
+							const float dc3 = __fsqrt_rn(rr[(k + 1) % 3] * rr[(k + 2) % 3]) * (1.f - rr[k]) / sc[k];
+							o_sc[k] = o_sc[k] * (s_act[k] / sc[k]) + gs * dc3;
+						}
+					}
+				}
 				if (RAW)
 				{
 					// ExpBackward0: grad * result
-					for (int k = 0; k < 3; k++) o_sc[k] = __fmul_rn(o_sc[k], sc[k]);
+					for (int k = 0; k < 3; k++) o_sc[k] = __fmul_rn(o_sc[k], F3D ? s_act[k] : sc[k]);
 					// F.normalize = q / expand(clamp_min(norm(q), 1e-12)).  DivBackward0: g / d and -g * ((q / d) / d), where q / d is
 					// the normalised (r, x, y, z) above; ExpandBackward0 sums the four as (0 + 2) + (1 + 3); ClampMinBackward0 passes
 					// it where norm >= 1e-12; LinalgVectorNormBackward0: gn * (q / norm), 0 where norm == 0
@@ -486,6 +530,15 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 			o_op[0] = acc0.w * (opac * (1.0f - opac));                                    // backward.cu:433
 			// AA: the record holds o^ = sigmoid * s, so dL/dlogit = dL/do^ * s * sigmoid (1 - sigmoid) = dL/do^ * o^ (1 - o^ / s)
 			if constexpr (AA) o_op[0] = acc0.w * (opac * (1.0f - opac / aa_s));
+			// F3D: o^ = sigmoid * c3 (* s with AA); the sigmoid is read again from the logit
+			if constexpr (F3D)
+			{
+				if (f3d != 0.f)
+				{
+					const float sig = sigmoid_ref(QUANT ? quant_value(s_cb, CB_OPACITY, iop) : logit);
+					o_op[0] = acc0.w * (AA ? aa_s : 1.f) * c3 * (sig * (1.0f - sig));
+				}
+			}
 			for (int k = 0; k < 3; k++) o_m3[k] = dmean[k];
 			for (int k = 0; k < 6; k++) o_cov[k] = dcov[k];
 			o_con[0] = dconx; o_con[1] = dcony; o_con[3] = dconz;
@@ -647,19 +700,20 @@ int launch_preprocess_backward(const GsbBackwardRequest& req, const GeomState& g
 		a.raw_vec4 = al(a.sh_dc) && al(a.sh_rest) && al(a.dL_ddc) && al(a.dL_drest);
 	}
 	a.sh_vec4 = al(a.shs); a.dsh_vec4 = al(a.out.dL_dsh);
+	a.filter_3D = s->filter_3D; a.opacities = s->opacities;
 	const int grid = preprocess_backward_grid(s->P);
 	const size_t smem = (a.quant ? GSB_NUM_CODEBOOKS * GSB_CODEBOOK_SIZE : 0) * sizeof(float) + 8 * (32 * (3 * a.M + 1) + 32 * 6) * sizeof(float);
 	const cudaStream_t stream = stream_of(req);
 	ProfScope prof(K_PREPROCESS_BWD, stream);
 	const InputMode in = a.quant ? IN_QUANT : (raw ? IN_RAW : IN_ACTIVATED);
-	return dispatch([&](auto in, auto accumulate, auto maps, auto cam_grad, auto aa) -> int {
-		auto kernel = preprocess_backward_kernel<in, accumulate, maps, cam_grad, aa>;
+	return dispatch([&](auto in, auto accumulate, auto maps, auto cam_grad, auto aa, auto f3d) -> int {
+		auto kernel = preprocess_backward_kernel<in, accumulate, maps, cam_grad, aa, f3d>;
 		if (int e = ensure_dyn_smem((const void*)kernel, 160 * 1024)) return e;
 		kernel<<<grid, 256, smem, stream>>>(a);
 		GSB_LAUNCHED();
 		GSB_CUDA_OK(cudaGetLastError());
 		return GSB_OK;
-	}, in, req.grads->accumulate != 0, req.dL_dinvdepth != nullptr, a.cam_rows != nullptr, req.antialiasing != 0);
+	}, in, req.grads->accumulate != 0, req.dL_dinvdepth != nullptr, a.cam_rows != nullptr, req.antialiasing != 0, s->filter_3D != nullptr);
 }
 
 } // namespace gsb

@@ -26,6 +26,7 @@ struct PreArgs {
 	// IN_RAW (appended so that the other modes' parameter offsets, and with them their SASS, stay as they were): scales /
 	// rotations above then point at _scaling / _rotation, the SH rows at _features_dc [P,1,3] and _features_rest [P,n_rest,3]
 	const float* sh_dc; const float* sh_rest; int n_rest;
+	const float* filter_3D;                            // F3D (appended for the same reason): the [P] filter of DESIGN.md §5o
 };
 
 // forward.cu:105-159 computeColorFromSH with the accumulation order of the reference build
@@ -104,7 +105,9 @@ static_assert(32 * IDS_REST_ROW == GSB_IDS_STAGE_BYTES_PER_WARP, "staging buffer
 // changes, so binning is the same as without it.
 // IN (gsb_common.cuh InputMode): IN_RAW applies exp to the log-scales and normalize_quat to the rotation on load, and reads SH
 // coefficient k from _features_dc (k == 0) or _features_rest (k >= 1): the same values as the activated tensors, bit for bit.
-template <int IN, bool AA>
+// F3D (Mip-Splatting's 3D filter, DESIGN.md §5o): the activated scales go through filter_3d() before the covariance and the
+// sigmoid is multiplied by its c3 before the AA factor, so everything downstream sees the filtered scale and opacity.
+template <int IN, bool AA, bool F3D>
 __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 {
 	constexpr bool QUANT = IN == IN_QUANT, RAW = IN == IN_RAW;
@@ -142,7 +145,8 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 			const bool pruned = a.prune && a.prune[idx];
 			px = a.means3D[3 * idx]; py = a.means3D[3 * idx + 1]; pz = a.means3D[3 * idx + 2];
 			uint32_t ir = 0, is0 = 0, is1 = 0, is2 = 0, iop = 0;
-			float4 qrot = make_float4(0.f, 0.f, 0.f, 0.f); float sc0 = 0.f, sc1 = 0.f, sc2 = 0.f, opac_in = 0.f;
+			float4 qrot = make_float4(0.f, 0.f, 0.f, 0.f); float sc0 = 0.f, sc1 = 0.f, sc2 = 0.f, opac_in = 0.f, f3d = 0.f, c3 = 1.f;
+			if (F3D) f3d = a.filter_3D[idx];
 			if (QUANT)
 			{
 				ir = reinterpret_cast<const uint32_t*>(a.q.ids_rot)[idx];                      // 4 ids, one load
@@ -179,8 +183,9 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 				{
 					float r, x, y, z;
 					quant_rotation(s_cb, ir, r, x, y, z);
-					compute_cov3D(quant_value(s_cb, CB_SCALING, is0), quant_value(s_cb, CB_SCALING, is1), quant_value(s_cb, CB_SCALING, is2), a.mod,
-						r, x, y, z, cov3D);
+					float e0 = quant_value(s_cb, CB_SCALING, is0), e1 = quant_value(s_cb, CB_SCALING, is1), e2 = quant_value(s_cb, CB_SCALING, is2);
+					if constexpr (F3D) c3 = filter_3d(e0, e1, e2, f3d);
+					compute_cov3D(e0, e1, e2, a.mod, r, x, y, z, cov3D);
 					opac_raw = quant_value(s_cb, CB_OPACITY, iop);
 				}
 				else
@@ -194,12 +199,19 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 					{
 						float r = qrot.x, x = qrot.y, y = qrot.z, z = qrot.w;
 						normalize_quat(r, x, y, z);                                       // get_rotation, gaussian_model.py:145-146
-						compute_cov3D(exp_ref(sc0), exp_ref(sc1), exp_ref(sc2), a.mod, r, x, y, z, cov3D);   // get_scaling, :141-142
+						float e0 = exp_ref(sc0), e1 = exp_ref(sc1), e2 = exp_ref(sc2);       // get_scaling, :141-142
+						if constexpr (F3D) c3 = filter_3d(e0, e1, e2, f3d);
+						compute_cov3D(e0, e1, e2, a.mod, r, x, y, z, cov3D);
 					}
-					else compute_cov3D(sc0, sc1, sc2, a.mod, qrot.x, qrot.y, qrot.z, qrot.w, cov3D);
+					else
+					{
+						if constexpr (F3D) c3 = filter_3d(sc0, sc1, sc2, f3d);
+						compute_cov3D(sc0, sc1, sc2, a.mod, qrot.x, qrot.y, qrot.z, qrot.w, cov3D);
+					}
 					opac_raw = opac_in;
 				}
 				opacity = sigmoid_ref(opac_raw);
+				if (F3D) opacity = __fmul_rn(opacity, c3);
 				const float tx = xform_row(a.view, 0, px, py, pz), ty = xform_row(a.view, 1, px, py, pz);
 				const float3 cov_u = compute_cov2D_undilated(tx, ty, tz, a.focal_x, a.focal_y, a.tan_fovx, a.tan_fovy, cov3D, a.view);
 				const float3 cov = dilate_cov2D(cov_u);
@@ -449,6 +461,7 @@ int launch_preprocess(const GsbForwardRequest& req, const GeomState& g, const Im
 		a.scales = raw->scaling; a.rotations = raw->rotation;
 		a.sh_dc = raw->features_dc; a.sh_rest = raw->features_rest; a.n_rest = raw->C;
 	}
+	a.filter_3D = s->filter_3D;
 	a.sh_vec4 = !a.quant && !a.packed && a.shs && a.M == 16 && (reinterpret_cast<uintptr_t>(a.shs) & 15) == 0;
 	a.rest_aligned = a.quant && (reinterpret_cast<uintptr_t>(a.q.ids_rest) & 15) == 0 && (reinterpret_cast<uintptr_t>(a.q.ids_rot) & 3) == 0;
 	if (a.quant && (reinterpret_cast<uintptr_t>(a.q.ids_rot) & 3) != 0) { set_error("quantised scene: ids_rot must be 4-byte aligned"); return GSB_EINVAL; }
@@ -460,15 +473,15 @@ int launch_preprocess(const GsbForwardRequest& req, const GeomState& g, const Im
 	int grid = plan.priv ? plan.ctas : blocks_needed;
 	if (!plan.priv && a.quant && grid > GSB_NUM_SMS * 8) grid = GSB_NUM_SMS * 8;                         // persistent: amortise the table load
 	const InputMode in = a.quant ? IN_QUANT : (raw ? IN_RAW : IN_ACTIVATED);
-	return dispatch([&](auto in, auto aa) -> int {
-		auto kernel = preprocess_kernel<in, aa>;
+	return dispatch([&](auto in, auto aa, auto f3d) -> int {
+		auto kernel = preprocess_kernel<in, aa, f3d>;
 		if (int e = ensure_dyn_smem((const void*)kernel, 220 * 1024)) return e;
 		ProfScope prof(K_PREPROCESS, stream_of(req));
 		kernel<<<grid, threads, smem, stream_of(req)>>>(a);
 		GSB_LAUNCHED();
 		GSB_CUDA_OK(cudaGetLastError());
 		return GSB_OK;
-	}, in, req.antialiasing != 0);
+	}, in, req.antialiasing != 0, s->filter_3D != nullptr);
 }
 
 int launch_mark_visible(int P, const float* means3D, const float* view, uint8_t* present, cudaStream_t stream)

@@ -7,6 +7,7 @@
 //
 // The reference runs these as ~30 ATen element-wise ops per camera (colour statistics) and one kernel launch + one host
 // synchronisation per camera (pixel size); here each is ONE fused pass over the Gaussians, bandwidth-bound.
+#include <math_constants.h>
 #include "gsb_common.cuh"
 
 namespace gsb {
@@ -194,6 +195,95 @@ int launch_pixel_size(int P, const float* means3D, int n_cams, const float* w2nd
 	if (int e = ensure_dyn_smem((const void*)pixel_size_kernel, 1024 * 32 * 4)) return e;
 	pixel_size_kernel<<<(P + 255) / 256, 256, (size_t)n_cams * 32 * sizeof(float), stream>>>(P, means3D, n_cams, w2ndc, w2ndc_inv, heights, widths,
 		pixel_sizes);
+	GSB_LAUNCHED();
+	GSB_CUDA_OK(cudaGetLastError());
+	return GSB_OK;
+}
+
+// ------------------------------------------------------------------------------------------------
+// Mip-Splatting's compute_3D_filter (DESIGN.md §5o) in two launches and no host read: the torch loop runs about fifteen [P]-wide ops
+// per camera.  Pass 1: one thread per centre walks every camera, staged through shared memory in chunks of F3D_CHUNK (no camera
+// limit), keeps the smallest depth z of the cameras that see it (z > 0.2 and the projection inside the screen grown by 15 % on
+// each side) and adds its depth to the maximum over the seen centres; block 0 also takes the maximum focal length over all cameras.
+// Pass 2: unseen centres take that maximum, and f = (dist / F) * sqrt(0.2).  Both maxima are exact (integer max of the
+// non-negative float bits), so the result is the same bytes on every run.
+#define F3D_CHUNK 256
+#define F3D_CAM 20     // view rows 0..2 as xform_row reads them (m[i], m[4+i], m[8+i], m[12+i]), fx, fy, W/2, H/2, the four screen bounds
+
+__device__ __forceinline__ float f3d_row(const float* __restrict__ d, float x, float y, float z)
+{
+	float t = __fmul_rn(y, d[1]);
+	t = __fmaf_rn(x, d[0], t);
+	t = __fmaf_rn(z, d[2], t);
+	return __fadd_rn(t, d[3]);
+}
+
+__global__ void __launch_bounds__(256) filter_3d_dist_kernel(int P, const float* __restrict__ means3D, int n_cams,
+	const float* __restrict__ views, const float* __restrict__ focals, const int* __restrict__ sizes, float* __restrict__ dist,
+	unsigned* __restrict__ maxima)
+{
+	__shared__ float s_cam[F3D_CHUNK * F3D_CAM];
+	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+	float x = 0.f, y = 0.f, z = 0.f;
+	if (idx < P) { x = means3D[3 * idx]; y = means3D[3 * idx + 1]; z = means3D[3 * idx + 2]; }
+	float best = CUDART_INF_F;
+	for (int c0 = 0; c0 < n_cams; c0 += F3D_CHUNK)
+	{
+		const int nc = min(F3D_CHUNK, n_cams - c0);
+		__syncthreads();
+		for (int c = threadIdx.x; c < nc; c += blockDim.x)
+		{
+			const float* v = views + 16 * (size_t)(c0 + c);
+			float* d = s_cam + F3D_CAM * c;
+			for (int i = 0; i < 3; i++) { d[4 * i] = v[i]; d[4 * i + 1] = v[4 + i]; d[4 * i + 2] = v[8 + i]; d[4 * i + 3] = v[12 + i]; }
+			const float fx = focals[2 * (c0 + c)], fy = focals[2 * (c0 + c) + 1];
+			const int W = sizes[2 * (c0 + c)], H = sizes[2 * (c0 + c) + 1];
+			d[12] = fx; d[13] = fy; d[14] = 0.5f * (float)W; d[15] = 0.5f * (float)H;
+			// torch compares the fp32 tensor with the Python doubles -0.15 * W and W * 1.15 rounded to fp32
+			d[16] = (float)(-0.15 * W); d[17] = (float)(W * 1.15); d[18] = (float)(-0.15 * H); d[19] = (float)(H * 1.15);
+			if (blockIdx.x == 0) atomicMax(&maxima[1], __float_as_uint(fx));
+		}
+		__syncthreads();
+		if (idx < P)
+			for (int c = 0; c < nc; c++)
+			{
+				const float* d = s_cam + F3D_CAM * c;
+				const float tz = f3d_row(d + 8, x, y, z);
+				if (!(tz > 0.2f)) continue;
+				const float zc = fmaxf(tz, 0.001f);
+				const float u = __fadd_rn(__fmul_rn(__fdiv_rn(f3d_row(d, x, y, z), zc), d[12]), d[14]);
+				const float w = __fadd_rn(__fmul_rn(__fdiv_rn(f3d_row(d + 4, x, y, z), zc), d[13]), d[15]);
+				if (u >= d[16] && u <= d[17] && w >= d[18] && w <= d[19]) best = fminf(best, tz);
+			}
+	}
+	if (idx < P) dist[idx] = best;
+	// seen depths are > 0.2, so their bits order as the values; 0 marks "no seen centre"
+	const unsigned m = __reduce_max_sync(0xffffffffu, idx < P && best != CUDART_INF_F ? __float_as_uint(best) : 0u);
+	if ((threadIdx.x & 31) == 0 && m) atomicMax(&maxima[0], m);
+}
+
+__global__ void __launch_bounds__(256) filter_3d_finish_kernel(int P, const unsigned* __restrict__ maxima, float* __restrict__ filter)
+{
+	const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+	if (idx >= P) return;
+	const unsigned seen_max = maxima[0];
+	if (seen_max == 0u) { filter[idx] = 0.f; return; }        // no centre seen, or no camera: Mip-Splatting raises here
+	float d = filter[idx];
+	if (d == CUDART_INF_F) d = __uint_as_float(seen_max);
+	// F is the largest focal over ALL cameras, not over those that see the centre (Mip-Splatting's choice, kept)
+	filter[idx] = __fmul_rn(__fdiv_rn(d, __uint_as_float(maxima[1])), 0.44721359549995793f);   // fp32(sqrt(0.2))
+}
+
+int launch_filter_3d(int P, const float* means3D, int n_cams, const float* views, const float* focals, const int* sizes, float* filter,
+	unsigned* maxima, cudaStream_t stream)
+{
+	if (P <= 0) return GSB_OK;
+	ProfScope prof(K_TOOLS, stream);
+	GSB_CUDA_OK(cudaMemsetAsync(maxima, 0, 2 * sizeof(unsigned), stream));
+	filter_3d_dist_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, means3D, n_cams, views, focals, sizes, filter, maxima);
+	GSB_LAUNCHED();
+	GSB_CUDA_OK(cudaGetLastError());
+	filter_3d_finish_kernel<<<(P + 255) / 256, 256, 0, stream>>>(P, maxima, filter);
 	GSB_LAUNCHED();
 	GSB_CUDA_OK(cudaGetLastError());
 	return GSB_OK;

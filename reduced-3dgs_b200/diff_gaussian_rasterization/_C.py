@@ -16,6 +16,9 @@ same keyword (None: torch's deterministic-algorithms flag) for their statistics 
 tensor of per-Gaussian features over the pairs of the colour image, with background 0, and appends the [F, H, W] image to the
 outputs; the backward's `features` and `dL_dfeatures_out` add that image's gradient and append dL_dfeatures [P, F].
 `absgrad_out` (backward) takes a [P, 3] fp32 tensor that receives the absolute screen-space gradient.
+`filter_3D` (forward, also of the variable-SH entry point, and backward) takes Mip-Splatting's 3D smoothing filter, [P] or [P, 1]
+fp32 on the device (gs_b200.mip.compute_3D_filter): the scales become sqrt(s^2 + f^2) and the opacity sigmoid(logit) * c3 inside the
+kernels (DESIGN.md §5o).  Its backward also needs the opacity logits, `opacity` (not with `quant`, whose ids are read).
 
 Each keyword is one field of the library's request (GsbForwardRequest / GsbBackwardRequest): the forward and the backward make one
 library call, gsb_forward / gsb_backward, whatever their keywords.
@@ -110,6 +113,18 @@ def check_absgrad_out(absgrad_out, P, accumulate_into=None, features=None, dL_df
         raise RuntimeError("absgrad_out must live on a CUDA device (no CPU path exists)")
 
 
+def check_filter_3d(filter_3D, P):
+    """The checks of a `filter_3D` argument, made before anything runs: a [P] or [P, 1] float32 tensor on a CUDA device."""
+    if not isinstance(filter_3D, torch.Tensor):
+        raise RuntimeError(f"filter_3D must be a [P] or [P, 1] tensor, got {type(filter_3D).__name__}")
+    if tuple(filter_3D.shape) not in ((P,), (P, 1)):
+        raise RuntimeError(f"filter_3D must have shape [P] or [P, 1] with P = {P} Gaussians, got {tuple(filter_3D.shape)}")
+    if filter_3D.dtype != torch.float32:
+        raise RuntimeError(f"filter_3D must be float32, got {filter_3D.dtype}")
+    if not filter_3D.is_cuda:
+        raise RuntimeError("filter_3D must live on a CUDA device (no CPU path exists)")
+
+
 def _present(t):
     return t is not None and not (isinstance(t, torch.Tensor) and t.numel() == 0)
 
@@ -165,7 +180,7 @@ def _raw_struct(raw, device, P, want_sh, sh, scales, rotations, cov3D_precomp, q
 
 
 def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, sh, degrees, keep,
-           packed_counts=None, prune_mask=None, quant=None):
+           packed_counts=None, prune_mask=None, quant=None, filter_3D=None):
     means3D = f32(means3D, device)
     P = int(means3D.shape[0]) if means3D is not None else 0
     colors, opacity, scales, rotations = f32(colors, device), f32(opacity, device), f32(scales, device), f32(rotations, device)
@@ -176,7 +191,11 @@ def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, 
         degrees = None
     if prune_mask is not None:
         prune_mask = prune_mask.to(device=device, dtype=torch.uint8).contiguous()
-    keep += [means3D, colors, opacity, scales, rotations, cov3D_precomp, sh, degrees, prune_mask]
+    if filter_3D is not None:
+        if filter_3D.device != device:
+            raise RuntimeError(f"filter_3D must live on {device}, got {filter_3D.device}")
+        filter_3D = filter_3D.detach().reshape(-1).contiguous()
+    keep += [means3D, colors, opacity, scales, rotations, cov3D_precomp, sh, degrees, prune_mask, filter_3D]
     M = 0
     if quant is not None:
         M = 16
@@ -193,6 +212,7 @@ def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, 
         for d in range(4):
             s.band_count[d] = int(packed_counts[d]) if d < len(packed_counts) else 0
     s.prune_mask = ptr(prune_mask)
+    s.filter_3D = ptr(filter_3D)
     s.quant = _quant_struct(quant, device, keep) if quant is not None else None
     return s, P, M
 
@@ -200,9 +220,11 @@ def _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, 
 def _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix, projmatrix,
              tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug, packed_counts=None,
              prune_mask=None, quant=None, debug_out=None, statistics=None, return_maps=False, antialiasing=False, raw=None,
-             statistics_workspace=None, features=None):
+             statistics_workspace=None, features=None, filter_3D=None):
     if means3D.ndimension() != 2 or means3D.size(1) != 3:
         raise RuntimeError("means3D must have dimensions (num_points, 3)")          # rasterize_points.cu:158-161
+    if filter_3D is not None:
+        check_filter_3d(filter_3D, int(means3D.shape[0]))
     F = check_features(features, int(means3D.shape[0])) if features is not None else 0
     device = _device_of(means3D)
     if features is not None and features.device != device:
@@ -218,7 +240,7 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
     H, W = int(image_height), int(image_width)
     with on_device(device):
         scene, P, M = _scene(device, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, sh, degrees,
-                             keep, packed_counts, prune_mask, quant)
+                             keep, packed_counts, prune_mask, quant, filter_3D)
         cam = _camera(device, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, H, W, prefiltered, keep)
         out_color = torch.empty((3, H, W), dtype=torch.float32, device=device)
         maps = None
@@ -267,7 +289,8 @@ def _forward(background, means3D, colors, opacity, scales, rotations, scale_modi
 
 def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                         projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                        *, prune_mask=None, quant=None, debug_out=None, return_maps=False, antialiasing=False, raw=None, features=None):
+                        *, prune_mask=None, quant=None, debug_out=None, return_maps=False, antialiasing=False, raw=None, features=None,
+                        filter_3D=None):
     """rasterize_points.h:43-63 RasterizeGaussiansCUDA -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer).
     `return_maps`: -> (R, color, radii, geomBuffer, binningBuffer, imgBuffer, invdepth [1,H,W], alpha [1,H,W]) with
     invdepth = sum (1/depth) * alpha * T over the pairs that composite the colour and alpha = 1 - final_T.
@@ -276,23 +299,28 @@ def rasterize_gaussians(background, means3D, colors, opacity, scales, rotations,
     and rotations empty; the kernels read them in place and activate them.  With colors, features_dc and
     features_rest are None.  The same output bits as the activated call on cat(dc, rest), exp(scaling), F.normalize(rotation).
     `features`: [P, F] fp32 on the device, 1 <= F <= 256; the tuple ends with the [F, H, W] feature image, each channel composited
-    like a colour channel with background 0.  Every other output is the call's without it."""
+    like a colour channel with background 0.  Every other output is the call's without it.
+    `filter_3D`: [P] or [P, 1] fp32 on the device, Mip-Splatting's 3D filter applied to the scales and the opacity in the kernels;
+    an all-zero filter gives the bytes of the call without it.  Not with cov3D_precomp."""
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                     projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                    None, prune_mask, quant, debug_out, return_maps=return_maps, antialiasing=antialiasing, raw=raw, features=features)
+                    None, prune_mask, quant, debug_out, return_maps=return_maps, antialiasing=antialiasing, raw=raw, features=features,
+                    filter_3D=filter_3D)
 
 
 def rasterize_gaussians_variableSH_bands(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp,
                                          viewmatrix, projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh,
                                          perBandPrimitiveCount, cumSumPrimitiveCount, coeffsNum, degrees, campos, prefiltered,
-                                         debug, *, prune_mask=None, debug_out=None, return_maps=False, antialiasing=False, features=None):
+                                         debug, *, prune_mask=None, debug_out=None, return_maps=False, antialiasing=False, features=None,
+                                         filter_3D=None):
     """rasterize_points.h:18-41 RasterizeGaussiansVariableSHBandsCUDA (inference, packed per-degree SH groups).
     cumSumPrimitiveCount / coeffsNum are implied by perBandPrimitiveCount ([1,4,9,16] per gaussian_renderer:90-92).
-    `return_maps`, `antialiasing` and `features` as in rasterize_gaussians (forward only, like the rest of this path)."""
+    `return_maps`, `antialiasing`, `features` and `filter_3D` as in rasterize_gaussians (forward only, like the rest of this path)."""
     counts = [int(v) for v in perBandPrimitiveCount.detach().cpu().tolist()]
     return _forward(background, means3D, colors, opacity, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
                     projmatrix, tan_fovx, tan_fovy, image_height, image_width, sh, degrees, campos, prefiltered, debug,
-                    counts, prune_mask, None, debug_out, return_maps=return_maps, antialiasing=antialiasing, features=features)
+                    counts, prune_mask, None, debug_out, return_maps=return_maps, antialiasing=antialiasing, features=features,
+                    filter_3D=filter_3D)
 
 
 def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rotations, scale_modifier, cov3D_precomp, viewmatrix,
@@ -300,7 +328,7 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
                                  binningBuffer, imageBuffer, lambda_sh_sparsity, debug, *, prune_mask=None, quant=None,
                                  accumulate_into=None, want_conic=False, view_means2D=None, dL_dinvdepth=None, dL_dalpha=None,
                                  camera_grads=False, antialiasing=False, raw=None, deterministic=False, features=None,
-                                 dL_dfeatures_out=None, absgrad_out=None):
+                                 dL_dfeatures_out=None, absgrad_out=None, filter_3D=None, opacity=None):
     """rasterize_points.h:65-88 RasterizeGaussiansBackwardCUDA ->
     (dL_dmeans2D, dL_dcolors, dL_dopacity, dL_dmeans3D, dL_dcov3D, dL_dsh, dL_dscales, dL_drotations).
     `accumulate_into`: the same 8-tuple from a previous call; gradients are added in place (view-batch accumulation);
@@ -320,7 +348,13 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     Neither `accumulate_into` nor `deterministic` has a feature form: both are refused.
     `absgrad_out`: a contiguous fp32 [P, 3] tensor on the device, overwritten with (sum_p |g_x|, sum_p |g_y|, 0), the per-pixel terms
     of dL_dmeans2D added as absolute values (AbsGS); every other output is the call's without it (bit for bit
-    with `deterministic`).  It has no `accumulate_into` and no feature form: both are refused before anything runs."""
+    with `deterministic`).  It has no `accumulate_into` and no feature form: both are refused before anything runs.
+    `filter_3D`: the forward's filter; `opacity` is then the forward's opacity logits (not with `quant`).  The filter gets no
+    gradient; the scale and opacity gradients are chained through it."""
+    if filter_3D is not None:
+        check_filter_3d(filter_3D, int(means3D.shape[0]))
+        if quant is None and not isinstance(opacity, torch.Tensor):
+            raise RuntimeError("filter_3D: the backward needs the forward's opacity logits (opacity=...)")
     if absgrad_out is not None:
         check_absgrad_out(absgrad_out, int(means3D.shape[0]), accumulate_into, features, dL_dfeatures_out)
     feat_F = 0
@@ -341,9 +375,10 @@ def rasterize_gaussians_backward(background, means3D, radii, colors, scales, rot
     keep = []
     H, W = int(dL_dout_color.size(1)), int(dL_dout_color.size(2))
     with on_device(device):
-        scene, P, M = _scene(device, means3D, colors, None, scales, rotations, scale_modifier, cov3D_precomp, sh, degrees, keep,
-                             None, prune_mask, quant)
-        if quant is None:
+        with_opacity = filter_3D is not None and quant is None
+        scene, P, M = _scene(device, means3D, colors, opacity if with_opacity else None, scales, rotations, scale_modifier,
+                             cov3D_precomp, sh, degrees, keep, None, prune_mask, quant, filter_3D)
+        if quant is None and not with_opacity:
             scene.opacities = means3D.data_ptr() if P > 0 else None      # not read by the backward; keeps check_scene satisfied
         cam = _camera(device, background, viewmatrix, projmatrix, campos, tan_fovx, tan_fovy, H, W, False, keep)
         dL = f32(dL_dout_color, device)

@@ -22,6 +22,8 @@ colour gradient reaches.  The feature gradient has no deterministic form: it is 
 GaussianRasterizer.forward's keyword-only `means2D_abs` (a [P, 3] tensor that requires grad, e.g. a zeros leaf) receives as its
 gradient the absolute screen-space gradient (sum_p |g_x|, sum_p |g_y|, 0) of AbsGS, the densification
 statistic whose per-pixel terms cannot cancel; it has no feature form.
+GaussianRasterizer.forward's keyword-only `filter_3D` ([P] or [P, 1] fp32, gs_b200.mip.compute_3D_filter) applies Mip-Splatting's
+3D smoothing filter to the scales and the opacity inside the kernels; it is a constant (no gradient), as Mip-Splatting's buffer is.
 Every option goes through the one autograd op, _RasterizeGaussians, each optional input in a slot of its own.
 """
 from typing import NamedTuple
@@ -54,8 +56,8 @@ def _call(fn, args, kw, dump, message):
 # raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps), then one slot per optional input.  A call that uses no
 # optional input passes the first fourteen only.
 MEANS3D, MEANS2D, SH, DEGREES, COLORS, OPACITIES, SCALES, ROTATIONS, COV3D = range(9)
-VIEWMATRIX, PROJMATRIX, CAMPOS, FEATURES, MEANS2D_ABS, FEATURES_DC, FEATURES_REST, SCALING, ROTATION = range(14, 23)
-N_INPUTS = 23
+VIEWMATRIX, PROJMATRIX, CAMPOS, FEATURES, MEANS2D_ABS, FEATURES_DC, FEATURES_REST, SCALING, ROTATION, FILTER_3D = range(14, 24)
+N_INPUTS = 24
 
 
 def _deterministic(raster_settings):
@@ -67,12 +69,12 @@ def _deterministic(raster_settings):
 
 def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, features=None,
-                        means2D_abs=None, raw_params=None):
+                        means2D_abs=None, raw_params=None, filter_3D=None):
     camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
     if not (torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera)):
         # a constant camera is read from raster_settings; a learnable one is also an input, so that its gradients have a destination
         camera = (None,) * 3
-    optional = (*camera, features, means2D_abs, *(raw_params or (None,) * 4))
+    optional = (*camera, features, means2D_abs, *(raw_params or (None,) * 4), filter_3D)
     return _RasterizeGaussians.apply(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                                      raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps,
                                      *(optional if any(t is not None for t in optional) else ()))
@@ -83,13 +85,14 @@ class _RasterizeGaussians(torch.autograd.Function):
     given only when the camera is learnable.  `features_dc` [P,1,3], `features_rest` [P,C,3] (both None with colors_precomp),
     `scaling` [P,3] (log-scales) and `rotation` [P,4] (unnormalised) are the model's leaf tensors in place of sh, scales and rotations
     (then empty): the kernels apply get_features / get_scaling / get_rotation themselves and return the gradients of these four
-    tensors directly, so the graph holds no Cat / Exp / Div node and no [P,16,3] copy or gradient exists.
+    tensors directly, so the graph holds no Cat / Exp / Div node and no [P,16,3] copy or gradient exists.  `filter_3D` is
+    Mip-Splatting's 3D filter, a constant: the backward gets it and the opacity logits, and it receives no gradient.
     -> (color, radii), with return_maps (color, radii, invdepth, alpha); with `features` the feature image [F, H, W] comes last."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
                 lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None,
-                features=None, means2D_abs=None, features_dc=None, features_rest=None, scaling=None, rotation=None):
+                features=None, means2D_abs=None, features_dc=None, features_rest=None, scaling=None, rotation=None, filter_3D=None):
         rs = raster_settings
         args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
                 rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, degrees, rs.campos, rs.prefiltered, rs.debug)
@@ -98,6 +101,8 @@ class _RasterizeGaussians(torch.autograd.Function):
         kw.update(prune_mask=prune_mask, return_maps=return_maps, antialiasing=rs.antialiasing)
         if features is not None:
             kw.update(features=features)
+        if filter_3D is not None:
+            kw.update(filter_3D=filter_3D)
         out = _call(_C.rasterize_gaussians, args, kw,
                     "snapshot_fw.dump", "\nAn error occured in forward. Please forward snapshot_fw.dump for debugging.")
         ctx.raster_settings, ctx.num_rendered, ctx.lambda_sh_sparsity = rs, out[0], lambda_sh_sparsity
@@ -110,7 +115,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             # image without a gradient leaves the backward exactly the call without features
             ctx.set_materialize_grads(False)
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, out[2], sh, out[3], out[4], out[5], degrees,
-                              features, features_dc, features_rest, scaling, rotation)
+                              features, features_dc, features_rest, scaling, rotation, filter_3D,
+                              opacities if filter_3D is not None else None)
         return (out[1], out[2]) + (out[6:8] if return_maps else ()) + (out[-1:] if features is not None else ())
 
     @staticmethod
@@ -119,7 +125,7 @@ class _RasterizeGaussians(torch.autograd.Function):
         grad_invdepth, grad_alpha = grads[:2] if ctx.return_maps else (None, None)
         grad_features = grads[-1] if ctx.has_features else None
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer, degrees, features,
-         features_dc, features_rest, scaling, rotation) = ctx.saved_tensors
+         features_dc, features_rest, scaling, rotation, filter_3D, opacities) = ctx.saved_tensors
         rs = ctx.raster_settings
         if grad_out_color is None:
             grad_out_color = torch.zeros((3, rs.image_height, rs.image_width), dtype=torch.float32, device=means3D.device)
@@ -134,6 +140,8 @@ class _RasterizeGaussians(torch.autograd.Function):
             kw.update(deterministic=True)
         if grad_features is not None:
             kw.update(features=features, dL_dfeatures_out=grad_features)
+        if filter_3D is not None:
+            kw.update(filter_3D=filter_3D, opacity=opacities)
         out = [None] * N_INPUTS
         if ctx.has_abs:
             out[MEANS2D_ABS] = torch.empty((means3D.shape[0], 3), dtype=torch.float32, device=means3D.device)
@@ -217,7 +225,7 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, degrees=None, colors_precomp=None, scales=None,
                 rotations=None, cov3D_precomp=None, lambda_sh_sparsity=0., *, prune_mask=None, quant=None, return_maps=False,
-                raw_params=None, features=None, means2D_abs=None):
+                raw_params=None, features=None, means2D_abs=None, filter_3D=None):
         """-> (color, radii); with return_maps, (color, radii, invdepth [1,H,W], alpha [1,H,W]), all three differentiable.
         `raw_params`: (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]), the model's leaf tensors, in place
         of shs / scales / rotations (which must then be None, as must cov3D_precomp and quant); with colors_precomp the two
@@ -226,7 +234,9 @@ class GaussianRasterizer(nn.Module):
         like a colour channel with background 0), differentiable w.r.t. the features and, through alpha, the scene and the camera.
         A feature gradient under the deterministic mode is refused (here when `features` requires grad, else in the backward).
         `means2D_abs`: a [P, 3] tensor (a zeros leaf that requires grad); its gradient is the absolute screen-space gradient
-        (sum_p |g_x|, sum_p |g_y|, 0), deterministic with the deterministic mode.  Not together with `features`."""
+        (sum_p |g_x|, sum_p |g_y|, 0), deterministic with the deterministic mode.  Not together with `features`.
+        `filter_3D`: [P] or [P, 1] fp32 on the device, Mip-Splatting's 3D smoothing filter (a constant): the kernels render with
+        scales sqrt(s^2 + f^2) and opacities sigmoid(logit) * c3, and chain the gradients through both.  Not with cov3D_precomp."""
         raster_settings = self.raster_settings
         if means2D_abs is not None:
             if features is not None:
@@ -258,4 +268,4 @@ class GaussianRasterizer(nn.Module):
         e = lambda t: empty if t is None else t                                  # absent inputs travel as empty tensors
         return rasterize_gaussians(means3D, means2D, e(shs), degrees, e(colors_precomp), e(opacities), e(scales), e(rotations),
                                    e(cov3D_precomp), raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features,
-                                   means2D_abs, raw_params)
+                                   means2D_abs, raw_params, filter_3D)

@@ -18,6 +18,8 @@ It is differentiable w.r.t. the features and the scene on every path but the var
 `absgrad=True` adds pkg["viewspace_points_abs"], a zeros leaf [P, 3] whose .grad after loss.backward() is the absolute screen-space
 gradient (sum_p |g_x|, sum_p |g_y|, 0) of AbsGS, the split statistic of densify_and_prune(max_grad_abs=...) (DESIGN.md §5m).  It needs
 a backward, so the variable-SH inference path refuses it, and it has no feature form.
+`pc.filter_3D` (optional, [P] or [P, 1] fp32 on the device; gs_b200.mip.compute_3D_filter sets it) is Mip-Splatting's 3D smoothing
+filter, applied in the kernels on every path (DESIGN.md §5o); it does not go with pipe.compute_cov3D_python.
 
 A learnable camera needs no argument: when world_view_transform, full_proj_transform or camera_center requires grad, the
 rasterizer returns their gradients (the variable-SH inference path stays non-differentiable).  The rasterizer takes
@@ -97,6 +99,10 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         raise RuntimeError("gaussian_renderer.render: absgrad needs the backward; the variable-SH inference path renders forward only")
     if absgrad and features is not None:
         raise RuntimeError("gaussian_renderer.render: absgrad has no feature form; render the features in a call without absgrad")
+    filter_3D = getattr(pc, "filter_3D", None)
+    if filter_3D is not None and pipe.compute_cov3D_python:
+        raise RuntimeError("gaussian_renderer.render: pc.filter_3D filters the scales inside the kernels; it does not go with "
+                           "pipe.compute_cov3D_python")
     fused = bool(getattr(pipe, "fused_activations", False)) and not variable_sh_bands
     raw_params = _raw_params(pc, pipe, override_color) if fused else None
     screenspace_points = torch.zeros_like(pc.get_xyz, dtype=pc.get_xyz.dtype, requires_grad=True, device=pc.get_xyz.device)
@@ -168,7 +174,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.tanfovx, raster_settings.tanfovy,
             raster_settings.image_height, raster_settings.image_width, shs, per_band_count, cumsum_count, coeffs_num,
             degrees, raster_settings.campos, raster_settings.prefiltered, raster_settings.debug, prune_mask=prune_mask,
-            return_maps=return_maps, antialiasing=raster_settings.antialiasing, **({} if features is None else dict(features=features)))
+            return_maps=return_maps, antialiasing=raster_settings.antialiasing, **({} if features is None else dict(features=features)),
+            **({} if filter_3D is None else dict(filter_3D=filter_3D)))
         rendered_image, radii = out[1], out[2]
         maps = out[6:8] if return_maps else ()
         feature_image = out[-1] if features is not None else None
@@ -177,7 +184,8 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             means3D=means3D, means2D=means2D, shs=shs, degrees=degrees, colors_precomp=colors_precomp, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, lambda_sh_sparsity=lambda_sh_sparsity,
             prune_mask=prune_mask, quant=quant, return_maps=return_maps, raw_params=raw_params, features=features,
-            **({} if screenspace_points_abs is None else dict(means2D_abs=screenspace_points_abs)))
+            **({} if screenspace_points_abs is None else dict(means2D_abs=screenspace_points_abs)),
+            **({} if filter_3D is None else dict(filter_3D=filter_3D)))
         rendered_image, radii = out[0], out[1]
         maps = out[2:4] if return_maps else ()
         feature_image = out[-1] if features is not None else None

@@ -28,6 +28,10 @@ AbsGS (DESIGN.md §5m): add_densification_stats(..., viewspace_abs=pkg["viewspac
 absolute screen-space gradient into `xyz_gradient_accum_abs` [P, 1] (created as zeros on the first call), and
 densify_and_prune(..., max_grad_abs=...) splits on accum_abs / denom >= max_grad_abs instead of on the signed statistic.  Every prune
 carries `xyz_gradient_accum_abs`, and densify_and_prune resets it, exactly as `xyz_gradient_accum`, when the model has one.
+
+Mip-Splatting (DESIGN.md §5o): a model with `filter_3D` ([P, 1] or [P] fp32, gs_b200.mip.compute_3D_filter) has it carried row for
+row by every pass here and in gs_b200.mcmc, a clone, split child or added row taking its source's value, so render() never sees a
+stale row count; recompute it after densifying, as Mip-Splatting does.
 """
 from __future__ import annotations
 
@@ -275,6 +279,9 @@ def _validate(model, store_grads, grads_everywhere=False):
     _check_f32(getattr(model, "max_radii2D", None), (P,), dev, "max_radii2D")
     if getattr(model, "xyz_gradient_accum_abs", None) is not None:
         _check_f32(model.xyz_gradient_accum_abs, (P, 1), dev, "xyz_gradient_accum_abs")
+    f3d = getattr(model, "filter_3D", None)
+    if f3d is not None:
+        _check_f32(f3d, (P, 1) if torch.is_tensor(f3d) and f3d.dim() == 2 else (P,), dev, "filter_3D")
     return groups, P, dev
 
 
@@ -334,7 +341,9 @@ STATS = ("xyz_gradient_accum", "denom", "max_radii2D", "xyz_gradient_accum_abs")
 
 def _resized(model, groups, P_out, dev, kinds, stat_kind, store_grads=False):
     """The [P_out] rows of a resized model and their emit table entries: each group's param (kind from `kinds`, else COPY), its
-    moments if it has state and then with store_grads its .grad; _degrees (COPY); unless stat_kind is None, the STATS the model has.
+    moments if it has state and then with store_grads its .grad; _degrees and, when the model has one, filter_3D (Mip-Splatting's
+    3D filter, DESIGN.md §5o) as COPY, so a child or an added row takes its source's value; unless stat_kind is None, the STATS the
+    model has.
     -> (entries, install).  install(), after the emit, sets the statistics and does the reference's optimizer surgery
     (_prune_optimizer / cat_tensors_to_optimizer): the state dict object moves to the new Parameter with the new moments; a group
     without state only gets its param; .grad travels only with state and store_grads."""
@@ -350,6 +359,8 @@ def _resized(model, groups, P_out, dev, kinds, stat_kind, store_grads=False):
         entries.append(_entry(p, dst, kinds.get(name, gsl.DENSIFY_COPY), moments, mv, None if gr is None else p.grad, gr))
         new.append((name, g, p, state, dst, mv, gr))
     stats = [("_degrees", gsl.DENSIFY_COPY)]
+    if getattr(model, "filter_3D", None) is not None:
+        stats.append(("filter_3D", gsl.DENSIFY_COPY))
     if stat_kind is not None:
         stats += [(k, stat_kind) for k in STATS if getattr(model, k, None) is not None]
     out_stats = {}

@@ -29,7 +29,7 @@ class GsbScene(C.Structure):
                 ("scales", C.c_void_p), ("rotations", C.c_void_p), ("cov3D_precomp", C.c_void_p), ("shs", C.c_void_p),
                 ("colors_precomp", C.c_void_p), ("degrees", C.c_void_p), ("scale_modifier", C.c_float),
                 ("sh_packed", C.c_int32), ("band_count", C.c_int32 * 4), ("prune_mask", C.c_void_p),
-                ("quant", C.POINTER(GsbQuant))]
+                ("filter_3D", C.c_void_p), ("quant", C.POINTER(GsbQuant))]
 
 
 class GsbCamera(C.Structure):
@@ -131,6 +131,8 @@ SIGNATURES = {
     "gsb_debug_dequant": (C.c_int, [C.POINTER(GsbQuant), _I32, _V, _V, _V]),
     "gsb_sh_statistics_update": (C.c_int, [_I32, _I32] + [_V] * 13),
     "gsb_min_projected_pixel_size": (C.c_int, [_I32, _V, _I32, _V, _V, _V, _V, _V, _V]),
+    "gsb_filter_3d_workspace_bytes": (_SZ, []),
+    "gsb_filter_3d": (C.c_int, [_I32, _V, _I32, _V, _V, _V, _V, _V, _V]),
     "gsb_sphere_ellipsoid_intersection": (C.c_int, [_I32, _V, _V, _V, _V, _V, _I32, _V, _V, _V]),
     "gsb_min_redundancy_value": (C.c_int, [_I32, _V, _V, _V, _I32, _V, _V]),
     "gsb_kmeans_workspace_bytes": (_SZ, [_I64, _I32, _I32]),

@@ -75,6 +75,8 @@ def relocate_gs(model, dead_mask=None):
         moments = None if state is None else (state["exp_avg"], state["exp_avg_sq"])
         entries.append(densify._entry(p, p, KIND.get(name, gsl.DENSIFY_COPY), moments, moments))
     entries.append(densify._entry(model._degrees, model._degrees, gsl.DENSIFY_COPY))
+    if getattr(model, "filter_3D", None) is not None:
+        entries.append(densify._entry(model.filter_3D, model.filter_3D, gsl.DENSIFY_COPY))
     _emit(entries, P, dev, gsl.MCMC_RELOCATE, n_dead, ws)
     for _, _, p, _ in groups:
         p.grad = None
