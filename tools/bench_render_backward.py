@@ -1,14 +1,15 @@
-"""`render_backward` of this tree against a checkout of the parent commit, measured in one command.
+"""`render_backward`, `preprocess` and `preprocess_backward` of this tree against a checkout of the parent commit, measured in one command.
 
     git archive HEAD~1 | tar -x -C _trees/parent && python _trees/parent/reduced-3dgs_b200/csrc/build.py
     python tools/bench_render_backward.py --parent-tree _trees/parent [--steps 20] [--warmup 5] [--reps 2]
 
 The parent checkout lies inside the repository (`_trees/` is git-ignored) and is built before the call.  The two trees are measured
 alternately (parent, this, parent, this, ...), each arm in a process of its own that imports bench.py and the library from its
-tree.  Workloads: bench.py's C3 (3 M codebook-quantised Gaussians) and a dense 3 M scene rendered from its raw parameters
-(`raw=`, SH degree 3), both 1920x1080, forward + backward of bench.py's first camera.  Every step is timed with a CUDA event
-pair, L2 is flushed (256 MB write) between steps outside the pair, the library's per-kernel event pairs give `render_backward`
-per step; medians and min..max of the timed steps are reported.  The gradients of the last step (the inputs are the same in
+tree.  Workloads, one per input format of the per-Gaussian kernels: bench.py's C3 (3 M codebook-quantised Gaussians), a dense 3 M
+scene rendered from its raw parameters (`raw=`, SH degree 3) and the same scene activated by torch before the call, all
+1920x1080, forward + backward of bench.py's first camera.  Every step is timed with a CUDA event
+pair, L2 is flushed (256 MB write) between steps outside the pair, the library's per-kernel event pairs give `render_backward`,
+`preprocess` and `preprocess_backward` per step; medians and min..max of the timed steps are reported.  The gradients of the last step (the inputs are the same in
 every step) are kept as seeded row samples, and per gradient array the largest difference between the two trees is printed
 relative to the array's largest magnitude, next to the same figure for two runs of the parent.  Prints the card's name and
 power limit.  Without a GPU it fails.
@@ -24,7 +25,8 @@ import tempfile
 import benchkit     # from this script's directory: the parent tree need not have it
 
 ROOT = benchkit.ROOT
-WORKLOADS = ("C3", "dense3M_raw")
+WORKLOADS = ("C3", "dense3M_raw", "dense3M_activated")
+KERNELS = ("render_backward", "preprocess", "preprocess_backward")
 
 
 def measure(tree, steps, warmup, dump):
@@ -43,28 +45,28 @@ def measure(tree, steps, warmup, dump):
 
     samples = {}
     gsl.profile_enable(True)
-    for name, wl in zip(WORKLOADS, (c3, benchkit.dense_raw_workload(c3.W, c3.H, dev))):
-        rb, last = [], []
+    raw = benchkit.dense_raw_workload(c3.W, c3.H, dev)
+    for name, wl in zip(WORKLOADS, (c3, raw, benchkit.activated_workload(raw))):
+        prof, last = [], []
 
         def step(i):
-            # the library's event pairs of the previous step, so rb[k + 1] belongs to step k.  The read runs inside this step's
+            # the library's event pairs of the previous step, so prof[k + 1] belongs to step k.  The read runs inside this step's
             # event pair, while the L2 flush in front of it still runs on the GPU; host time it takes beyond the flush counts in
-            # step_ms (render_backward_ms, the kernel's own pair, does not see it)
-            rb.append(gsl.profile_read().get("render_backward", (0.0, 0))[0])
+            # step_ms (the kernels' own pairs do not see it)
+            prof.append(gsl.profile_read())
             last[:] = benchkit.forward_backward(wl, cam)
 
         step_ms = benchkit.time_arms({name: step}, steps, warmup, flush)[name]
-        rb.append(gsl.profile_read()["render_backward"][0])
-        rb_ms = rb[warmup + 1:]
+        prof.append(gsl.profile_read())
+        kernel_ms = {k: [p.get(k, (0.0, 0))[0] for p in prof[warmup + 1:]] for k in KERNELS}
         R, grads, P = last[0][0], last[1], wl.scene.P
         rows = torch.as_tensor(np.sort(np.random.default_rng(P).choice(P, bench.DUMP_ROWS, replace=False)), device=dev)
         for i, g in enumerate(grads):                                          # every per-Gaussian output (raw= appends its own)
             if torch.is_tensor(g) and g.dim() and g.shape[0] == P:
                 samples[f"{name}/{bench.GRAD_NAMES[i] if i < len(bench.GRAD_NAMES) else i}"] = g[rows].float().cpu().numpy()
-        print(json.dumps({"workload": name, "R": int(R), "steps": steps,
-                          "render_backward_ms": {"median": round(statistics.median(rb_ms), 4), "min": round(min(rb_ms), 4), "max": round(max(rb_ms), 4)},
-                          "step_ms": {"median": round(statistics.median(step_ms), 4), "min": round(min(step_ms), 4), "max": round(max(step_ms), 4)}}),
-              flush=True)
+        spread = lambda v: {"median": round(statistics.median(v), 4), "min": round(min(v), 4), "max": round(max(v), 4)}
+        print(json.dumps({"workload": name, "R": int(R), "steps": steps, **{f"{k}_ms": spread(v) for k, v in kernel_ms.items()},
+                          "step_ms": spread(step_ms)}), flush=True)
     gsl.profile_enable(False)
     np.savez(dump, **samples)
 
@@ -119,7 +121,7 @@ def main():
             for rep in range(args.reps):
                 p, t = res["parent", rep][wl], res["this", rep][wl]
                 print(json.dumps({"workload": wl, "pair": rep,
-                                  "render_backward_this_over_parent": round(t["render_backward_ms"]["median"] / p["render_backward_ms"]["median"], 4),
+                                  **{f"{k}_this_over_parent": round(t[f"{k}_ms"]["median"] / p[f"{k}_ms"]["median"], 4) for k in KERNELS},
                                   "step_this_over_parent": round(t["step_ms"]["median"] / p["step_ms"]["median"], 4)}), flush=True)
         p0, p1, t0 = (np.load(os.path.join(tmp, f)) for f in ("parent0.npz", "parent1.npz", "this0.npz"))
         own, gap = largest_gaps(p0, p1), largest_gaps(p0, t0)

@@ -1,5 +1,5 @@
-"""What the rasterizer's A/B bench tools share: the card banner, the L2 flush, bench.py's workload and the dense raw-parameter
-scene, one forward + backward call, and the timed loops.
+"""What the rasterizer's A/B bench tools share: the card banner, the L2 flush, bench.py's workload, the dense raw-parameter
+scene and its activated form, one forward + backward call, and the timed loops.
 
 Importing this module puts the repository root and `reduced-3dgs_b200` on sys.path.  bench.py and the library are imported only
 when a function needs them, so a caller that puts another tree in front of sys.path first (tools/bench_render_backward.py
@@ -68,6 +68,16 @@ def dense_raw_workload(W, H, dev):
     scene = SimpleNamespace(P=s.P, means3D=s.means3D.to(dev), opacity=s.opacity.to(dev), degrees=s.degrees.to(dev))
     return SimpleNamespace(W=W, H=H, scene=scene, quant=None, prune=None, raw=raw,
                            G=synth.grad_image(W, H, 1000).to(dev), bg=torch.zeros(3, device=dev))
+
+
+def activated_workload(wl):
+    """The raw-parameter workload `wl` (dense_raw_workload) with its activations applied by torch before the call: scales =
+    exp(_scaling), rotations = F.normalize(_rotation), sh = cat(_features_dc, _features_rest), the same Gaussians in the reference's
+    input format."""
+    dc, rest, scaling, rotation = wl.raw
+    scene = SimpleNamespace(P=wl.scene.P, means3D=wl.scene.means3D, opacity=wl.scene.opacity, degrees=wl.scene.degrees,
+                            scales=torch.exp(scaling), rotations=torch.nn.functional.normalize(rotation), sh=torch.cat((dc, rest), 1))
+    return SimpleNamespace(W=wl.W, H=wl.H, scene=scene, quant=None, prune=None, raw=None, G=wl.G, bg=wl.bg)
 
 
 def forward_backward(wl, cam, fwd=None, bwd=None, dL=None, colors=E, backward=True):
