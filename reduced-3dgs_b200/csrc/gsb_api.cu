@@ -90,8 +90,7 @@ void prof_end(int kid, cudaStream_t stream)
 	}
 	t_prof_cur = nullptr;
 }
-static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter", "tile_sort_large", "unused4", "tile_sort", "unused6",
-	"render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad", "det_scan",
+static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter", "tile_sort_large", "tile_sort", "render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad", "det_scan",
 	"det_gather", "det_clear", "features_forward", "features_backward", "absgrad_finish" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);

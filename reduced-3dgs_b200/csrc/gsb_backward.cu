@@ -419,7 +419,7 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 					wr(1, -kSH_C1 * y); wr(2, kSH_C1 * z); wr(3, -kSH_C1 * x);
 					if (deg > 1)
 					{
-						const float C20 = 1.0925484305920792f, C21 = -1.0925484305920792f, C22 = 0.31539156525252005f, C23 = -1.0925484305920792f, C24 = 0.5462742152960396f;
+						const float C20 = kSH_C2[0], C21 = kSH_C2[1], C22 = kSH_C2[2], C23 = kSH_C2[3], C24 = kSH_C2[4];
 						const float xx = x * x, yy = y * y, zz = z * z, xy = x * y, yz = y * z, xz = x * z;
 						for (int c = 0; c < 3; c++)
 						{
@@ -431,8 +431,8 @@ __global__ void __launch_bounds__(256) preprocess_backward_kernel(const BwdArgs 
 						wr(4, C20 * xy); wr(5, C21 * yz); wr(6, C22 * (2.f * zz - xx - yy)); wr(7, C23 * xz); wr(8, C24 * (xx - yy));
 						if (deg > 2)
 						{
-							const float C30 = -0.5900435899266435f, C31 = 2.890611442640554f, C32 = -0.4570457994644658f, C33 = 0.3731763325901154f,
-								C34 = -0.4570457994644658f, C35 = 1.445305721320277f, C36 = -0.5900435899266435f;
+							const float C30 = kSH_C3[0], C31 = kSH_C3[1], C32 = kSH_C3[2], C33 = kSH_C3[3], C34 = kSH_C3[4], C35 = kSH_C3[5],
+								C36 = kSH_C3[6];
 							for (int c = 0; c < 3; c++)
 							{
 								const float s9 = sh(9, c), s10 = sh(10, c), s11 = sh(11, c), s12 = sh(12, c), s13 = sh(13, c), s14 = sh(14, c), s15 = sh(15, c);

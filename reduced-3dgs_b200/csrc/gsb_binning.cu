@@ -32,33 +32,23 @@
 namespace gsb {
 
 // ------------------------------------------------------------------------------------------------
-// Exclusive scan over the tile counters (T <= a few 10^4): one CTA, 1024 threads, sequential chunks.
+// Exclusive scan over the tile counters (T <= a few 10^4): one CTA, 1024 threads, sequential chunks.  The scan and the running
+// carry are 64-bit: a total beyond 2^32 must not wrap silently.
 __global__ void __launch_bounds__(1024) tile_scan_kernel(const uint32_t* __restrict__ tile_count, int T, uint2* __restrict__ ranges,
 	uint32_t* __restrict__ counters, uint32_t* __restrict__ cursor, uint32_t* __restrict__ cls_list, uint32_t* __restrict__ cls_count)
 {
-	__shared__ uint32_t s_warp[32];
-	__shared__ unsigned long long s_carry;            // 64-bit: a total beyond 2^32 must not wrap silently
-	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-	if (tid == 0) { s_carry = 0; cls_count[0] = 0; cls_count[1] = 0; cls_count[2] = 0; cls_count[3] = 0; }
+	__shared__ unsigned long long s_warp[32];
+	const int tid = threadIdx.x;
+	if (tid == 0) { cls_count[0] = 0; cls_count[1] = 0; cls_count[2] = 0; cls_count[3] = 0; }
 	__syncthreads();
+	unsigned long long carry = 0;
 	for (int base = 0; base < T; base += 1024)
 	{
 		const int t = base + tid;
 		const uint32_t c = t < T ? tile_count[t] : 0u;
-		uint32_t incl = c;
-#pragma unroll
-		for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-		if (lane == 31) s_warp[warp] = incl;
-		__syncthreads();
-		if (warp == 0)
-		{
-			uint32_t w = s_warp[lane];
-#pragma unroll
-			for (int o = 1; o < 32; o <<= 1) { const uint32_t v = __shfl_up_sync(0xffffffffu, w, o); if (lane >= o) w += v; }
-			s_warp[lane] = w;
-		}
-		__syncthreads();
-		const unsigned long long start64 = s_carry + (warp ? s_warp[warp - 1] : 0u) + incl - c;
+		unsigned long long total;
+		const unsigned long long start64 = carry + cta_exclusive<1024>((unsigned long long)c, s_warp, &total);
+		carry += total;
 		const uint32_t start = (uint32_t)start64;       // positions are only used when the total fits 31 bits (checked below)
 		if (t < T)
 		{
@@ -67,14 +57,12 @@ __global__ void __launch_bounds__(1024) tile_scan_kernel(const uint32_t* __restr
 			// tiles too large for the one-CTA-per-tile class are queued for the persistent large-segment kernels
 			if (c > GSB_SORT_CAP_A) { const int k = c > GSB_SORT_CAP_B; cls_list[k * T + atomicAdd(&cls_count[k], 1u)] = t; }
 		}
-		__syncthreads();
-		if (tid == 1023) s_carry = start64 + c;
-		__syncthreads();
 	}
+	__syncthreads();
 	if (tid == 0)
 	{
-		const bool overflow = s_carry >= (1ull << 31);
-		counters[0] = overflow ? 0xffffffffu : (uint32_t)s_carry;   // num_rendered; the saturated value also stops every speculative launch
+		const bool overflow = carry >= (1ull << 31);
+		counters[0] = overflow ? 0xffffffffu : (uint32_t)carry;   // num_rendered; the saturated value also stops every speculative launch
 		counters[6] = overflow ? 1u : 0u;
 		counters[4] = cls_count[0]; counters[5] = cls_count[1];   // read back with R: the host skips the large-tile launches when both are 0
 	}
@@ -191,22 +179,22 @@ __global__ void __launch_bounds__(1024, 1) scatter_priv_kernel(int P, int chunk,
 			rc_n = make_uint2(0, 0); db_n = 0;
 			if (nx < last) { rc_n = __ldcs(&rect[nx]); db_n = __ldcs(&depth_bits[nx]); }
 		}
-		const uint32_t minx = rc.x & 0xffffu, maxx = rc.x >> 16;
-		const uint32_t miny = max(rc.y & 0xffffu, y_lo), maxy = min(rc.y >> 16, y_hi);       // clipped to this band
-		const uint32_t w = maxx - minx, t = maxy > miny ? w * (maxy - miny) : 0u;
+		TileRect tr(rc);
+		tr.miny = max(tr.miny, y_lo); tr.maxy = min(tr.maxy, y_hi);                          // clipped to this band
+		const uint32_t w = tr.width(), t = tr.maxy > tr.miny ? tr.area() : 0u;
 		const bool big = t > 32;
 		if (t && !big)
 		{
 			const uint64_t comp = ((uint64_t)dbits << 32) | (uint32_t)idx;
-			for (uint32_t y = miny; y < maxy; y++)
-				for (uint32_t x = minx; x < maxx; x++) st_u64_policy(&bucket[atomicAdd(&s_cur[(y - y_lo) * gx + x], 1u)], comp, pol);
+			for (uint32_t y = tr.miny; y < tr.maxy; y++)
+				for (uint32_t x = tr.minx; x < tr.maxx; x++) st_u64_policy(&bucket[atomicAdd(&s_cur[(y - y_lo) * gx + x], 1u)], comp, pol);
 		}
 		unsigned bigmask = __ballot_sync(0xffffffffu, big);
 		while (bigmask)
 		{
 			const int src = __ffs(bigmask) - 1; bigmask &= bigmask - 1;
 			const uint32_t bt = __shfl_sync(0xffffffffu, t, src), bw = __shfl_sync(0xffffffffu, w, src);
-			const uint32_t bminx = __shfl_sync(0xffffffffu, minx, src), bminy = __shfl_sync(0xffffffffu, miny, src);
+			const uint32_t bminx = __shfl_sync(0xffffffffu, tr.minx, src), bminy = __shfl_sync(0xffffffffu, tr.miny, src);
 			const uint64_t comp = ((uint64_t)__shfl_sync(0xffffffffu, dbits, src) << 32) | (uint32_t)(idx - lane + src);
 			for (uint32_t k = lane; k < bt; k += 32)
 				st_u64_policy(&bucket[atomicAdd(&s_cur[(bminy - y_lo + k / bw) * gx + bminx + k % bw], 1u)], comp, pol);
@@ -229,14 +217,14 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, const uint32_t* __r
 		rc = rect[idx];
 		if (rc.x | rc.y) dbits = depth_bits[idx];
 	}
-	const uint32_t minx = rc.x & 0xffffu, maxx = rc.x >> 16, miny = rc.y & 0xffffu, maxy = rc.y >> 16;
-	const uint32_t w = maxx - minx, t = w * (maxy - miny);
+	const TileRect tr(rc);
+	const uint32_t w = tr.width(), t = tr.area();
 	const bool big = t > 32;
 	if (t && !big)
 	{
 		const uint64_t comp = ((uint64_t)dbits << 32) | (uint32_t)idx;
-		for (uint32_t y = miny; y < maxy; y++)
-			for (uint32_t x = minx; x < maxx; x++)
+		for (uint32_t y = tr.miny; y < tr.maxy; y++)
+			for (uint32_t x = tr.minx; x < tr.maxx; x++)
 			{
 				const uint32_t tile = y * gx + x;
 				bucket[ranges[tile].x + atomicAdd(&cursor[tile], 1u)] = comp;
@@ -247,7 +235,7 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, const uint32_t* __r
 	{
 		const int src = __ffs(bigmask) - 1; bigmask &= bigmask - 1;
 		const uint32_t bt = __shfl_sync(0xffffffffu, t, src), bw = __shfl_sync(0xffffffffu, w, src);
-		const uint32_t bminx = __shfl_sync(0xffffffffu, minx, src), bminy = __shfl_sync(0xffffffffu, miny, src);
+		const uint32_t bminx = __shfl_sync(0xffffffffu, tr.minx, src), bminy = __shfl_sync(0xffffffffu, tr.miny, src);
 		const uint64_t comp = ((uint64_t)__shfl_sync(0xffffffffu, dbits, src) << 32) | (uint32_t)(idx - lane + src);
 		for (uint32_t k = lane; k < bt; k += 32)
 		{
@@ -261,14 +249,13 @@ __global__ void __launch_bounds__(256) scatter_kernel(int P, const uint32_t* __r
 // Per-tile sort in shared memory: stable LSD radix sort of (depth bits, id) pairs on the 32 depth bits, 8 bits per pass.
 // Warp w owns positions [w*32*ITEMS, (w+1)*32*ITEMS); ranks inside a warp come from match.any, across warps from a
 // per-digit scan of the per-warp counters (the same stable ranking as a onesweep tile, but the whole "array" is the tile).
-// Persistent CTAs walk a queued tile list (LIST is always true now; the one-CTA-per-tile mode is kept for tooling).
-template <int CAP, int THREADS, bool LIST>
+// Persistent CTAs walk a device-side list of queued tiles: the tiles the distribution sort found too clustered.
+template <int CAP, int THREADS>
 __global__ void __launch_bounds__(THREADS) tile_sort_kernel(const uint2* __restrict__ ranges, const uint64_t* __restrict__ bucket,
 	uint32_t* __restrict__ point_list, const uint32_t* __restrict__ cls_list, const uint32_t* __restrict__ cls_count,
 	const uint32_t* __restrict__ counters, uint32_t cap)
 {
 	if (counters[0] > cap) return;                   // speculative launch, see scatter_priv_kernel
-	// LIST == false: cls_list is the per-tile flag array written by tile_sort_dist_kernel (only flagged tiles are sorted here)
 	constexpr int ITEMS = CAP / THREADS, NW = THREADS / 32;
 	extern __shared__ __align__(16) unsigned char s_raw[];
 	uint32_t* kA = reinterpret_cast<uint32_t*>(s_raw);
@@ -281,12 +268,10 @@ __global__ void __launch_bounds__(THREADS) tile_sort_kernel(const uint2* __restr
 	__shared__ uint32_t s_and, s_or;
 	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
 	const unsigned lt = (1u << lane) - 1u;
-	const uint32_t n_work = LIST ? *cls_count : gridDim.x;
+	const uint32_t n_work = *cls_count;
 	for (uint32_t wi = blockIdx.x; wi < n_work; wi += gridDim.x)
 	{
-		const uint32_t tile = LIST ? cls_list[wi] : wi;
-		if (!LIST && cls_list[tile] == 0) continue;
-		const uint2 r = ranges[tile];
+		const uint2 r = ranges[cls_list[wi]];
 		const uint32_t n = r.y - r.x;
 		if (n == 0 || n > (uint32_t)CAP) continue;
 		if (n == 1) { if (tid == 0) point_list[r.x] = (uint32_t)bucket[r.x]; continue; }
@@ -627,7 +612,7 @@ int launch_scatter_sort(const GeomState& g, const BinningState& b, const ImageSt
 	const int gx = tiles.x, gy = tiles.y, T = gx * gy;
 	const uint32_t cap32 = (uint32_t)std::min<long long>(cap, 0x7fffffffll);
 	{
-		ProfScope prof(K_EMIT_KEYS, stream);
+		ProfScope prof(K_SCATTER, stream);
 		if (plan.priv)
 		{
 			if (int e = ensure_dyn_smem((const void*)scatter_priv_kernel, 220 * 1024)) return e;
@@ -654,10 +639,10 @@ int launch_scatter_sort(const GeomState& g, const BinningState& b, const ImageSt
 		}
 	}
 	constexpr size_t smemA = size_t(GSB_SORT_CAP_A) * 16 + 8 * 256 * 4;
-	if (int e = ensure_dyn_smem((const void*)tile_sort_kernel<GSB_SORT_CAP_A, 256, true>, (int)smemA)) return e;
+	if (int e = ensure_dyn_smem((const void*)tile_sort_kernel<GSB_SORT_CAP_A, 256>, (int)smemA)) return e;
 	if (int e = ensure_dyn_smem((const void*)tile_sort_dist_kernel<256, false>, (int)sizeof(DistSmem<256>))) return e;
 	{
-		ProfScope prof(K_SORT_PASS, stream);
+		ProfScope prof(K_TILE_SORT, stream);
 		tile_sort_dist_kernel<256, false><<<T, 256, sizeof(DistSmem<256>), stream>>>(img.ranges, b.bucket, b.point_list, nullptr, nullptr,
 			img.cls_list + 2 * (size_t)T, img.cls_count + 2, g.counters, cap32);
 		GSB_LAUNCHED();
@@ -665,7 +650,7 @@ int launch_scatter_sort(const GeomState& g, const BinningState& b, const ImageSt
 	{
 		ProfScope prof(K_SORT_LARGE, stream);
 		// radix fallback for the tiles the distribution sort queued (device-side list; normally empty: the CTAs exit at once)
-		tile_sort_kernel<GSB_SORT_CAP_A, 256, true><<<GSB_NUM_SMS * 4, 256, smemA, stream>>>(img.ranges, b.bucket, b.point_list, img.cls_list + 2 * (size_t)T,
+		tile_sort_kernel<GSB_SORT_CAP_A, 256><<<GSB_NUM_SMS * 4, 256, smemA, stream>>>(img.ranges, b.bucket, b.point_list, img.cls_list + 2 * (size_t)T,
 			img.cls_count + 2, g.counters, cap32);
 		GSB_LAUNCHED();
 	}
@@ -685,12 +670,12 @@ int launch_sort_large(const GeomState& g, const BinningState& b, const ImageStat
 		// tiles of 2049 .. 8192 instances: the same one-pass distribution sort with 8192 bins on persistent 1024-thread CTAs; a tile
 		// whose depths cluster is queued (device-side list, region 3) for the 4-pass shared-memory radix sort that used to take them all
 		if (int e = ensure_dyn_smem((const void*)tile_sort_dist_kernel<1024, true>, (int)sizeof(DistSmem<1024>))) return e;
-		if (int e = ensure_dyn_smem((const void*)tile_sort_kernel<GSB_SORT_CAP_B, 1024, true>, (int)smemB)) return e;
+		if (int e = ensure_dyn_smem((const void*)tile_sort_kernel<GSB_SORT_CAP_B, 1024>, (int)smemB)) return e;
 		ProfScope prof(K_SORT_LARGE, stream);
 		tile_sort_dist_kernel<1024, true><<<GSB_NUM_SMS, 1024, sizeof(DistSmem<1024>), stream>>>(img.ranges, b.bucket, b.point_list, img.cls_list, img.cls_count,
 			img.cls_list + 3 * (size_t)T, img.cls_count + 3, g.counters, 0xffffffffu);
 		GSB_LAUNCHED();
-		tile_sort_kernel<GSB_SORT_CAP_B, 1024, true><<<GSB_NUM_SMS, 1024, smemB, stream>>>(img.ranges, b.bucket, b.point_list, img.cls_list + 3 * (size_t)T,
+		tile_sort_kernel<GSB_SORT_CAP_B, 1024><<<GSB_NUM_SMS, 1024, smemB, stream>>>(img.ranges, b.bucket, b.point_list, img.cls_list + 3 * (size_t)T,
 			img.cls_count + 3, g.counters, 0xffffffffu);
 		GSB_LAUNCHED();
 	}

@@ -1,9 +1,8 @@
 // gsb_deterministic.cu — the two small kernels around the deterministic render backward (DESIGN.md §5i).
 //
-// Every Gaussian has exactly one instance per tile of its rect (the scatter loops over the rectangle), so the R instances can be
-// given fixed, Gaussian-major slots: instance (g, tile) -> offset[g] + (ty - miny) * w + (tx - minx), offset = exclusive scan of
-// the rect areas in Gaussian order.  render_backward_kernel<*, true> stores one partial per instance into its slot (the 8 warps
-// of the tile added in warp order), and det_gather_kernel adds each Gaussian's slots in row-major tile order into the 12-float
+// The R instances have fixed slots, Gaussian-major and then row-major over the Gaussian's tiles (gsb_common.cuh TileRect):
+// det_scan_kernel computes each Gaussian's first slot, render_backward_kernel<*, true> stores one partial per instance into its
+// slot (the 8 warps of the tile added in warp order), and det_gather_kernel adds each Gaussian's slots in order into the 12-float
 // accumulator the preprocess backward reads.  No float atomics anywhere: the same inputs give the same bytes on every run.
 #include "gsb_common.cuh"
 
@@ -37,18 +36,13 @@ size_t det_workspace_bytes(int P, long long R, int ns)
 	size_t b; DetWorkspace::carve(nullptr, P < 0 ? 0 : P, R < 0 ? 0 : R, ns, &b); return b;
 }
 
-__device__ __forceinline__ uint32_t rect_area(uint2 rc)
-{
-	return ((rc.x >> 16) - (rc.x & 0xffffu)) * ((rc.y >> 16) - (rc.y & 0xffffu));
-}
-
-// offset = exclusive scan of the rect areas; CTAs chain their totals with the decoupled look-back (ticket order).  The CTA
+// offset = exclusive scan of the TileRect areas; CTAs chain their totals with the decoupled look-back (ticket order).  The CTA
 // holding the last Gaussian checks the total against R and raises the error flag on a mismatch.
 __global__ void __launch_bounds__(DET_SCAN_THREADS) det_scan_kernel(int P, const uint2* __restrict__ rect, uint32_t* __restrict__ head,
 	uint32_t* __restrict__ lb, uint32_t* __restrict__ offset, unsigned long long R)
 {
 	__shared__ uint32_t s_tile, s_excl, s_warp[DET_SCAN_THREADS / 32];
-	const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+	const int tid = threadIdx.x;
 	if (tid == 0) s_tile = atomicAdd(&head[0], 1u);
 	__syncthreads();
 	const uint32_t tile = s_tile;
@@ -57,45 +51,26 @@ __global__ void __launch_bounds__(DET_SCAN_THREADS) det_scan_kernel(int P, const
 #pragma unroll
 	for (int i = 0; i < DET_SCAN_ITEMS; i++)
 	{
-		a[i] = base + i < P ? rect_area(rect[base + i]) : 0u;
+		a[i] = base + i < P ? TileRect(rect[base + i]).area() : 0u;
 		sum += a[i];
 	}
-	uint32_t incl = sum;                                   // inclusive warp scan of the per-thread sums
-#pragma unroll
-	for (int o = 1; o < 32; o <<= 1)
+	uint32_t total;
+	const uint32_t cta_excl = cta_exclusive<DET_SCAN_THREADS>(sum, s_warp, &total);
+	if (tid == 0)
 	{
-		const uint32_t v = __shfl_up_sync(0xffffffffu, incl, o);
-		if (lane >= o) incl += v;
-	}
-	if (lane == 31) s_warp[warp] = incl;
-	__syncthreads();
-	if (warp == 0)
-	{
-		uint32_t wv = s_warp[lane], wi = wv;
-#pragma unroll
-		for (int o = 1; o < 32; o <<= 1)
-		{
-			const uint32_t v = __shfl_up_sync(0xffffffffu, wi, o);
-			if (lane >= o) wi += v;
-		}
-		s_warp[lane] = wi - wv;                            // exclusive prefix of the warp totals
-		if (lane == 31)
-		{
-			const uint32_t total = wi;
-			const uint32_t excl = lookback_exclusive(lb, tile, 1, 0, total);
-			s_excl = excl;
-			const long long last = (long long)(tile + 1) * DET_SCAN_THREADS * DET_SCAN_ITEMS;
-			if (last >= P && (unsigned long long)excl + total != R) atomicExch(&head[1], 1u);
-		}
+		const uint32_t excl = lookback_exclusive(lb, tile, 1, 0, total);
+		s_excl = excl;
+		const long long last = (long long)(tile + 1) * DET_SCAN_THREADS * DET_SCAN_ITEMS;
+		if (last >= P && (unsigned long long)excl + total != R) atomicExch(&head[1], 1u);
 	}
 	__syncthreads();
-	uint32_t run = s_excl + s_warp[warp] + incl - sum;
+	uint32_t run = s_excl + cta_excl;
 #pragma unroll
 	for (int i = 0; i < DET_SCAN_ITEMS; i++)
 		if (base + i < P) { offset[base + i] = run; run += a[i]; }
 }
 
-// 16 threads per Gaussian, thread k writes acc[12 g + k]: the sum of component k over the Gaussian's slots in row-major tile order
+// 16 threads per Gaussian, thread k writes acc[12 g + k]: the sum of component k over the Gaussian's slots in slot order
 // (zero for culled and pruned Gaussians and for components the slot does not carry).  With the error flag set the accumulator is
 // filled with NaN, so blobs that do not match R cannot pass for a gradient.
 __global__ void __launch_bounds__(256) det_gather_kernel(int P, int ns, const uint2* __restrict__ rect, const uint32_t* __restrict__ offset,
@@ -105,7 +80,7 @@ __global__ void __launch_bounds__(256) det_gather_kernel(int P, int ns, const ui
 	const long long g = t >> 4;
 	const int k = (int)(t & 15);
 	if (g >= P) return;
-	const uint32_t area = rect_area(rect[g]);
+	const uint32_t area = TileRect(rect[g]).area();
 	const unsigned long long off = offset[g];
 	float s = 0.0f;
 	const bool bad = head[1] != 0 || off + area > R;

@@ -38,16 +38,6 @@ struct KmSortPlan {
 	uint32_t final_buf;
 };
 
-__device__ __forceinline__ uint32_t float_key(float f)
-{
-	const uint32_t u = __float_as_uint(f);
-	return u ^ ((u >> 31) ? 0xffffffffu : 0x80000000u);
-}
-__device__ __forceinline__ float key_float(uint32_t k)
-{
-	return __uint_as_float(k ^ ((k >> 31) ? 0x80000000u : 0xffffffffu));
-}
-
 // ------------------------------------------------------------------------------------------------ radix sort (keys only)
 __global__ void __launch_bounds__(256) km_keys_hist_kernel(const float* __restrict__ values, long long n, uint32_t* __restrict__ keys,
 	uint32_t* __restrict__ hist)

@@ -57,16 +57,6 @@ static KnnLevels knn_levels(long long P)
 	return L;
 }
 
-__device__ __forceinline__ uint32_t knn_fkey(float f)      // order-preserving integer image of a float
-{
-	const uint32_t u = __float_as_uint(f);
-	return u ^ ((u >> 31) ? 0xffffffffu : 0x80000000u);
-}
-__device__ __forceinline__ float knn_funkey(uint32_t k)
-{
-	return __uint_as_float(k ^ ((k >> 31) ? 0x80000000u : 0xffffffffu));
-}
-
 // simple_knn.cu:137 / :228 / :400 `d = point - ref; d.x*d.x + d.y*d.y + d.z*d.z` as the reference's SASS evaluates it
 __device__ __forceinline__ float knn_dist(float px, float py, float pz, float qx, float qy, float qz)
 {
@@ -94,9 +84,6 @@ __device__ __forceinline__ float knn_box_box(const float4& lo, const float4& hi,
 	return __fmaf_rn(gz, gz, __fmaf_rn(gx, gx, __fmul_rn(gy, gy)));
 }
 
-__device__ __forceinline__ float warp_min(float v) { for (int o = 16; o > 0; o >>= 1) v = fminf(v, __shfl_xor_sync(0xffffffffu, v, o)); return v; }
-__device__ __forceinline__ float warp_max(float v) { for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o)); return v; }
-
 // ------------------------------------------------------------------------------------------------ structure
 // bounds[0..2] = min, bounds[3..5] = max of the coordinates as order-preserving integers (NaN ignored); pre-set to 0xff.. / 0.
 __global__ void __launch_bounds__(256) knn_bounds_kernel(const float* __restrict__ points, long long P, uint32_t* __restrict__ bounds)
@@ -109,7 +96,7 @@ __global__ void __launch_bounds__(256) knn_bounds_kernel(const float* __restrict
 	for (int a = 0; a < 3; a++) { mn[a] = warp_min(mn[a]); mx[a] = warp_max(mx[a]); }
 	if ((threadIdx.x & 31) == 0)
 #pragma unroll
-		for (int a = 0; a < 3; a++) { atomicMin(&bounds[a], knn_fkey(mn[a])); atomicMax(&bounds[3 + a], knn_fkey(mx[a])); }
+		for (int a = 0; a < 3; a++) { atomicMin(&bounds[a], float_key(mn[a])); atomicMax(&bounds[3 + a], float_key(mx[a])); }
 }
 
 // distIndexQ's candidate filter: flags[id] = 1 for the first min(N, P) listed ids (simple_knn.cu:577-589 runs P threads); ids
@@ -143,8 +130,8 @@ __device__ __forceinline__ KnnGrid knn_grid(const uint32_t* __restrict__ bounds)
 #pragma unroll
 	for (int a = 0; a < 3; a++)
 	{
-		g.lo[a] = (double)knn_funkey(bounds[a]);
-		const double ext = (double)knn_funkey(bounds[3 + a]) - g.lo[a];
+		g.lo[a] = (double)key_float(bounds[a]);
+		const double ext = (double)key_float(bounds[3 + a]) - g.lo[a];
 		g.scale[a] = (ext > 0.0 && ext <= 1e300) ? 1073741823.0 / ext : 0.0;
 	}
 	return g;

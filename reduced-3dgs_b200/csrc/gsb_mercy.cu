@@ -65,14 +65,8 @@ struct MercyArgs {
 	bool want_median, want_quantile;
 };
 
-// Order-preserving key of a float, NaN above everything (torch sorts NaN last)
-__device__ __forceinline__ uint32_t float_key(float f)
-{
-	if (isnan(f)) return 0xffffffffu;
-	const uint32_t u = __float_as_uint(f);
-	return u ^ ((u >> 31) ? 0xffffffffu : 0x80000000u);
-}
-__device__ __forceinline__ float key_float(uint32_t k) { return __uint_as_float(k & 0x80000000u ? k ^ 0x80000000u : ~k); }
+// float_key with NaN above everything (torch sorts NaN last); key_float decodes it
+__device__ __forceinline__ uint32_t float_key_nan_last(float f) { return isnan(f) ? 0xffffffffu : float_key(f); }
 __device__ __forceinline__ bool is_redundant(int c, float thr) { return (float)c > thr; }
 // torch.minimum: NaN if either is NaN
 __device__ __forceinline__ float min_torch(float a, float b) { return isnan(a) || isnan(b) ? __int_as_float(0x7fc00000) : fminf(a, b); }
@@ -162,7 +156,7 @@ __global__ void __launch_bounds__(MERCY_THREADS) mercy_hist_kernel(const MercyAr
 	}
 	for (int i = blockIdx.x * MERCY_THREADS + threadIdx.x; i < a.P; i += gridDim.x * MERCY_THREADS)
 	{
-		const uint32_t key = float_key(sigmoid_torch(a.logits[i]));
+		const uint32_t key = float_key_nan_last(sigmoid_torch(a.logits[i]));
 		const uint32_t d = (key >> shift) & dmask;
 		const uint32_t high = pass == 0 ? 0u : key >> (shift + width);
 		if (on[0] && high == pre[0] && is_redundant(a.counts[i], thr)) atomicAdd(&s_h[0][d], 1u);

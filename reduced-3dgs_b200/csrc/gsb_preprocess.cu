@@ -44,9 +44,9 @@ __device__ __forceinline__ void sh_to_rgb(int deg, float x, float y, float z, SH
 			const float xx = __fmul_rn(x, x), yy = __fmul_rn(y, y), zz = __fmul_rn(z, z);
 			const float xy = __fmul_rn(x, y), yz = __fmul_rn(y, z), xz = __fmul_rn(x, z);
 			const float zz2 = __fadd_rn(zz, zz);
-			const float w4 = __fmul_rn(xy, 1.0925484305920792f), w5 = __fmul_rn(yz, -1.0925484305920792f);
-			const float w6 = __fmul_rn(__fsub_rn(__fsub_rn(zz2, xx), yy), 0.31539156525252005f);
-			const float w7 = __fmul_rn(xz, -1.0925484305920792f), w8 = __fmul_rn(__fsub_rn(xx, yy), 0.5462742152960396f);
+			const float w4 = __fmul_rn(xy, kSH_C2[0]), w5 = __fmul_rn(yz, kSH_C2[1]);
+			const float w6 = __fmul_rn(__fsub_rn(__fsub_rn(zz2, xx), yy), kSH_C2[2]);
+			const float w7 = __fmul_rn(xz, kSH_C2[3]), w8 = __fmul_rn(__fsub_rn(xx, yy), kSH_C2[4]);
 #pragma unroll
 			for (int c = 0; c < 3; c++)
 			{
@@ -59,13 +59,13 @@ __device__ __forceinline__ void sh_to_rgb(int deg, float x, float y, float z, SH
 			if (deg > 2)
 			{
 				const float q = __fsub_rn(__fmaf_rn(zz, 4.0f, -xx), yy);
-				const float w9 = __fmul_rn(__fmul_rn(y, -0.5900435899266435f), __fmaf_rn(xx, 3.0f, -yy));
-				const float w10 = __fmul_rn(__fmul_rn(xy, 2.890611442640554f), z);
-				const float w11 = __fmul_rn(__fmul_rn(y, -0.4570457994644658f), q);
-				const float w12 = __fmul_rn(__fmul_rn(z, 0.3731763325901154f), __fmaf_rn(yy, -3.0f, __fmaf_rn(xx, -3.0f, zz2)));
-				const float w13 = __fmul_rn(__fmul_rn(x, -0.4570457994644658f), q);
-				const float w14 = __fmul_rn(__fmul_rn(z, 1.445305721320277f), __fsub_rn(xx, yy));
-				const float w15 = __fmul_rn(__fmul_rn(x, -0.5900435899266435f), __fmaf_rn(yy, -3.0f, xx));
+				const float w9 = __fmul_rn(__fmul_rn(y, kSH_C3[0]), __fmaf_rn(xx, 3.0f, -yy));
+				const float w10 = __fmul_rn(__fmul_rn(xy, kSH_C3[1]), z);
+				const float w11 = __fmul_rn(__fmul_rn(y, kSH_C3[2]), q);
+				const float w12 = __fmul_rn(__fmul_rn(z, kSH_C3[3]), __fmaf_rn(yy, -3.0f, __fmaf_rn(xx, -3.0f, zz2)));
+				const float w13 = __fmul_rn(__fmul_rn(x, kSH_C3[4]), q);
+				const float w14 = __fmul_rn(__fmul_rn(z, kSH_C3[5]), __fsub_rn(xx, yy));
+				const float w15 = __fmul_rn(__fmul_rn(x, kSH_C3[6]), __fmaf_rn(yy, -3.0f, xx));
 #pragma unroll
 				for (int c = 0; c < 3; c++)
 				{
@@ -173,7 +173,7 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 				if ((rmax.x - rmin.x) * (rmax.y - rmin.y) == 0) break;
 				radius_i = (int)my_radius;
 				tiles = (rmax.y - rmin.y) * (rmax.x - rmin.x);
-				rect = make_uint2(rmin.x | (rmax.x << 16), rmin.y | (rmax.y << 16));
+				rect = TileRect::pack(rmin, rmax);
 				visible = true;
 			} while (false);
 		}
@@ -301,12 +301,12 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 		// per-tile instance counts (what the reference derives from sorted keys in identifyTileRanges): one RED per
 		// (Gaussian, tile); Gaussians covering more than 32 tiles are spread over the warp
 		{
-			const uint32_t minx = my_rect.x & 0xffffu, maxx = my_rect.x >> 16, miny = my_rect.y & 0xffffu, maxy = my_rect.y >> 16;
-			const uint32_t w = maxx - minx;
+			const TileRect tr(my_rect);
+			const uint32_t w = tr.width();
 			const bool big = my_tiles > 32;
 			if (my_tiles && !big)
-				for (uint32_t y = miny; y < maxy; y++)
-					for (uint32_t x = minx; x < maxx; x++)
+				for (uint32_t y = tr.miny; y < tr.maxy; y++)
+					for (uint32_t x = tr.minx; x < tr.maxx; x++)
 					{
 						if (a.hist_priv) atomicAdd(&s_hist[y * a.gx + x], 1u); else atomicAdd(&a.tile_count[y * a.gx + x], 1u);
 					}
@@ -315,7 +315,7 @@ __global__ void __launch_bounds__(1024, 1) preprocess_kernel(const PreArgs a)
 			{
 				const int src = __ffs(bigmask) - 1; bigmask &= bigmask - 1;
 				const uint32_t bt = __shfl_sync(0xffffffffu, my_tiles, src), bw = __shfl_sync(0xffffffffu, w, src);
-				const uint32_t bminx = __shfl_sync(0xffffffffu, minx, src), bminy = __shfl_sync(0xffffffffu, miny, src);
+				const uint32_t bminx = __shfl_sync(0xffffffffu, tr.minx, src), bminy = __shfl_sync(0xffffffffu, tr.miny, src);
 				for (uint32_t k = threadIdx.x & 31; k < bt; k += 32)
 				{
 					const uint32_t t = (bminy + k / bw) * a.gx + bminx + k % bw;

@@ -257,8 +257,8 @@ __device__ __forceinline__ void red_add_v2(float* addr, float a, float b)
 // summation across warps and tiles changes.  A staged batch is processed in lockstep: every warp flushes its stash at the end of
 // the batch and writes each row's 9 (10 with MAPS) values to its own shared-memory row of the batch entry (ebuf, zero for entries
 // it culled); after a CTA barrier the threads add the 8 warps' rows in warp order 0..7 and STORE the sum to the instance's slot
-// offset[g] + (ty - miny) * w + (tx - minx) of `parts` (no atomics).  det_gather_kernel then adds each Gaussian's slots in
-// row-major tile order.  The stash rows keep their batch entry index instead of the Gaussian id: the records are still staged.
+// of `parts` (gsb_common.cuh TileRect; no atomics).  det_gather_kernel then adds each Gaussian's slots in slot order.  The stash
+// rows keep their batch entry index instead of the Gaussian id: the records are still staged.
 //
 // ABS = true also accumulates the absolute screen-space gradient (AbsGS; DESIGN.md §5m), per Gaussian
 //     ax = o * sum_p |w_p (a dx_p + b dy_p)|,   ay = o * sum_p |w_p (b dx_p + c dy_p)|
@@ -585,9 +585,8 @@ __global__ void __launch_bounds__(256, DET ? (ABS ? 2 : 3) : 4) render_backward_
 			if (j < n)
 			{
 				const uint32_t gid = __float_as_uint(S.rec[buf][3 * j + 2].w);
-				const uint2 rc = rect[gid];
-				const uint32_t minx = rc.x & 0xffffu, maxx = rc.x >> 16, miny = rc.y & 0xffffu;
-				const unsigned long long slot = (unsigned long long)slot_offset[gid] + (blockIdx.y - miny) * (maxx - minx) + (blockIdx.x - minx);
+				const TileRect tr(rect[gid]);
+				const unsigned long long slot = tr.slot(slot_offset[gid], blockIdx.x, blockIdx.y);
 				for (int k = tid & 3; k < NS; k += 4)
 				{
 					float s = ebuf[j * NS + k];
