@@ -191,9 +191,11 @@ def sh_colours(means3D, campos, shs, degrees):
 
 
 def colours_variance(cam_positions, means3D, opacity, scales, rotations, viewmatrices, projmatrices, tan_fovxs, tan_fovys,
-                     image_height, image_width, sh, degrees, max_sh_deg=3):
+                     image_height, image_width, sh, degrees, max_sh_deg=3, alias_mean=True):
     """Reduced3DGS::calculateColourVariance (reduced_3dgs.cu:41-203) restated with numpy fp32 in the reference's op order.
-    Returns (colour distances / wSum [P,3], variance / wSum [P,1,3], mean [P,1,3]) plus the per-camera statistics for tests."""
+    Returns (colour distances / wSum [P,3], variance / wSum [P,1,3], mean [P,1,3]) plus, per camera, the statistics and the
+    whole forward state (preprocess, binning, render) for tests.  `alias_mean=False` takes the pre-update mean in one factor of
+    the variance term: what reduced_3dgs.cu:185-200 reads as, not what it computes (a near-miss for tests)."""
     assert max_sh_deg == 3
     means3D = _np(means3D, np.float32)
     P = means3D.shape[0]
@@ -230,9 +232,9 @@ def colours_variance(cam_positions, means3D, opacity, scales, rotations, viewmat
             coef[np.isnan(coef)] = 0
             mean[present] = mean_old[present] + coef[present].reshape(-1, 1, 1) * (colour[present] - mean_old[present])
             # `auto mean_old = mean;` shares storage: after the in-place index_put_ both factors use the NEW mean (:196-200)
-            variance[present] = variance[present] + t[present].reshape(-1, 1, 1) * (colour[present] - mean[present]) * (colour[present] - mean[present])
-            per_cam.append(dict(touched_pixels=touched, transmittance_sum=img["transmittance_sum"], radii=geom["radii"],
-                                borderline=img["borderline"]))
+            second = mean if alias_mean else mean_old
+            variance[present] = variance[present] + t[present].reshape(-1, 1, 1) * (colour[present] - mean[present]) * (colour[present] - second[present])
+            per_cam.append(dict(geom, **binning, **img))
         return dist_acc / wsum, variance / wsum.reshape(-1, 1, 1), mean, per_cam
 
 

@@ -372,10 +372,23 @@ def excluded(case, o):
       - it contributes there and has fewer than 2 000 contributing pixels: a flipped decision of another Gaussian changes one
         pixel term by at most a factor 1/(1 - alpha) ~ 1.004; over 2 000 or more terms that stays below the per-element bar.
     A power-0 flip (alpha = opacity) excludes every contributor of the pixel."""
-    W, H = case.W, case.H
+    near, count, _ = borderline_pairs(o, case.W, case.H)
+    touched = count > 0
+    if not touched.any():
+        return near
+    stats = o if "touched_pixels" in o else gs_oracle.render_forward_stats(o, o, case.bg, case.W, case.H)
+    return near | (touched & (stats["touched_pixels"] < 2000))
+
+
+def borderline_pairs(o, W, H):
+    """-> (near, count, behind): per Gaussian, whether its pair at some borderline pixel is near a threshold or next to that
+    pixel's termination (a power-0 flip marks every pair of the pixel that passes), at how many borderline pixels its pair passes
+    the alpha test, and at how many of those it lies behind a pair near a threshold (whose flip scales the pixel's T from there
+    on by up to 1 / (1 - 1/255))."""
     P = o["radii"].shape[0]
     near = np.zeros(P, bool)
-    touched = np.zeros(P, bool)
+    count = np.zeros(P, np.int64)
+    behind = np.zeros(P, np.int64)
     gx = (W + 15) // 16
     ys, xs = np.nonzero(o["borderline"])
     for y, x in zip(ys, xs):
@@ -385,6 +398,8 @@ def excluded(case, o):
         power, a = _pair_alpha(o, ids, x, y)
         passes = (power <= 1e-6) & (a >= (1.0 / 255.0) * (1 - 1e-5))
         thr = passes & ((np.abs(a * 255.0 - 1.0) < 1e-5) | (np.abs(a / 0.99 - 1.0) < 1e-5) | (np.abs(power) < 1e-6))
+        if thr.any():
+            behind[ids[passes & (np.arange(ids.size) > np.argmax(thr))]] += 1
         n = int(o["n_contrib"][y, x])
         after = np.nonzero(passes[n:])[0]
         if n > 0:
@@ -394,12 +409,8 @@ def excluded(case, o):
         if (passes & (np.abs(power) < 1e-6)).any():
             thr |= passes
         near[ids[thr]] = True
-        touched[ids[passes]] = True
-    if not touched.any():
-        return near
-    geom = {k: o[k] for k in ("means2D", "rgb", "conic_opacity")}
-    stats = gs_oracle.render_forward_stats(geom, o, case.bg, W, H)
-    return near | (touched & (stats["touched_pixels"] < 2000))
+        count[ids[passes]] += 1
+    return near, count, behind
 
 
 def compare(name, o, o64, o32, got, chk, glob=None, verbose=True, bar=(R_REL, A_ABS), arrays=ARRAYS):

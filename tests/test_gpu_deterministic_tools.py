@@ -1,6 +1,6 @@
 """GPU: the deterministic SH-culling statistics and k-means (DESIGN.md §5j).
-  1. statistics: touched_pixels equal to the default path's, transmittance_sum within 1e-6 of it, the oracle bars of
-     test_forward_statistics_against_oracle, the t1 / t1_large golden bars (2e-5) through calculate_colours_variance under torch's
+  1. statistics: touched_pixels equal to the default path's, transmittance_sum within 1e-6 of it (both paths against the oracle:
+     test_gpu_statistics_edges.py), the t1 / t1_large golden bars (2e-5) through calculate_colours_variance under torch's
      flag, five identical runs of all three outputs at 1920x1080 (1 M Gaussians, 8 cameras) also on a side stream and a second GPU,
      and the edges P = 0, R = 0 and everything outside the view;
   2. k-means: 0 iterations give the default ids; after 1 iteration and at convergence the centres are bit-identical to the float32
@@ -19,6 +19,7 @@ import torch
 
 import ours as O
 import test_gpu_tools as T
+from test_gpu_statistics_edges import stats_forward
 from diff_gaussian_rasterization import _C
 from gs_b200 import densify, ply, synth
 
@@ -43,45 +44,16 @@ def torch_flag(on=True):
 
 
 # ---- 1. statistics -------------------------------------------------------------------------------------------------------------
-def _stats(scene, cam, det, dev=DEV):
-    sc = scene.to(dev)
-    W, H = cam.image_width, cam.image_height
-    tx, ty = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
-    touched = torch.full((scene.P, 1), -7, dtype=torch.int32, device=dev)
-    tsum = torch.full((scene.P, 1), -7.0, device=dev)
-    kw = {}
-    if det:
-        kw["statistics_workspace"] = torch.full((int(_C._lib.lib().gsb_statistics_workspace_bytes(scene.P)),), 0xA5, dtype=torch.uint8,
-                                                device=dev)
-    E = torch.empty(0)
-    R, _, radii, *_ = _C._forward(torch.zeros(3, device=dev), sc.means3D, E, sc.opacity, sc.scales, sc.rotations, 1.0, E,
-                                  cam.world_view_transform.to(dev), cam.full_proj_transform.to(dev), tx, ty, H, W, sc.sh, sc.degrees,
-                                  cam.camera_center.to(dev), False, False, statistics=(touched, tsum), **kw)
-    return R, radii, touched, tsum
-
-
-def test_statistics_match_the_default_path_and_the_oracle():
-    import gs_oracle as GO
+def test_statistics_match_the_default_path():
     c, scene, cams, nb = cases.build_tools_inputs("t1")
     cam = cams[0]
-    R0, r0, t0, s0 = _stats(scene, cam, False)
-    R1, r1, t1, s1 = _stats(scene, cam, True)
+    R0, r0, t0, s0, _ = stats_forward(scene, cam, False)
+    R1, r1, t1, s1, _ = stats_forward(scene, cam, True)
     assert R0 == R1 and torch.equal(r0, r1)
     assert torch.equal(t0, t1) and int(t1.sum()) > 0
     s0, s1 = s0.cpu().numpy().reshape(-1), s1.cpu().numpy().reshape(-1)
     assert np.abs(s1.astype(np.float64) - s0).max() <= 1e-6 * np.abs(s0).max()
     assert np.all((s1 == 0) == (t1.cpu().numpy().reshape(-1) == 0))
-    # the bars of test_gpu_tools.test_forward_statistics_against_oracle
-    W, H = cam.image_width, cam.image_height
-    tx, ty = math.tan(cam.FoVx * 0.5), math.tan(cam.FoVy * 0.5)
-    geom = GO.preprocess(scene.means3D, scene.scales, 1.0, scene.rotations, scene.opacity, scene.sh, scene.degrees, None, None,
-                         cam.world_view_transform, cam.full_proj_transform, cam.camera_center, W, H, tx, ty, None)
-    img = GO.render_forward_stats(geom, GO.bin_and_sort(geom, W, H), np.zeros(3, np.float32), W, H)
-    t_o, t_g = img["touched_pixels"], t1.cpu().numpy().reshape(-1)
-    if not img["borderline"].any():
-        assert np.array_equal(t_o, t_g)
-    assert (t_o != t_g).sum() <= 4 * img["borderline"].sum()
-    T._close(s1, img["transmittance_sum"].astype(np.float32), 1e-5 if not img["borderline"].any() else 1e-3, "transmittance_sum")
 
 
 def test_colour_variance_goldens_under_the_torch_flag():
@@ -138,12 +110,12 @@ def test_statistics_edges():
     cam = cams[0]
     # P = 0 through the C ABI
     empty = synth.Scene(*[t[:0] for t in (scene.means3D, scene.opacity, scene.scales, scene.rotations, scene.sh, scene.degrees)])
-    R, radii, touched, tsum = _stats(empty, cam, True)
+    R, radii, touched, tsum, _ = stats_forward(empty, cam, True)
     assert R == 0 and radii.numel() == 0 and touched.numel() == 0
     # R = 0: everything far outside the view (culled by the frustum test)
     for shift in (torch.tensor([1e4, 0.0, 0.0]), torch.tensor([0.0, -1e4, 0.0])):
         moved = synth.Scene(scene.means3D + shift, scene.opacity, scene.scales, scene.rotations, scene.sh, scene.degrees)
-        R, radii, touched, tsum = _stats(moved, cam, True)
+        R, radii, touched, tsum, _ = stats_forward(moved, cam, True)
         assert R == 0 and int(touched.abs().sum()) == 0 and float(tsum.abs().sum()) == 0.0
     # the Python entry point with no camera and with P = 0
     sc = scene.to(DEV)
