@@ -347,6 +347,26 @@ GSB_API int gsb_export_binning(const char* geom_blob, int32_t P, const char* bin
 GSB_API int gsb_export_image(const char* image_blob, int32_t width, int32_t height, float* final_T, uint32_t* n_contrib,
                      uint32_t* ranges /* [tiles,2] */, void* stream);
 
+/* Contribution statistics of one view (DESIGN.md §5p), from the blobs of a finished gsb_forward (any mode: dense, quantised, raw,
+ * pruned, anti-aliased, filter_3D, maps, features, variable-SH inference) with its P, R = *num_rendered and image size.  A pair
+ * (pixel p, Gaussian i) contributes when the colour forward composited it (list position below n_contrib(p), alpha tests passed);
+ * alpha and the transmittance T in front are the forward's bits, and the pair's weight is w = alpha * T (one rounding).  m(p) =
+ * pixel_weights [H,W] fp32 clamped to [0, 1] on read (NaN reads as 0), or 1 when pixel_weights is NULL.  Outputs, overwritten:
+ *   weight_sum [P] fp32   sum_p m(p) w                     weight_max [P] fp32   max_p w (0 where i contributes nowhere)
+ *   pixels     [P] int32  number of contributing pairs (= the statistics forward's touched_pixels)
+ *   top_id   [H,W] int32  the id of the pixel's pair with the largest w; on an exact tie the earlier one in the list; -1 where none
+ * Culled, pruned and off-screen Gaussians get zeros; P == 0 or R == 0 gives zeros and -1.  Every output is the same bytes on every
+ * run: each (warp, Gaussian) sum is rounded to a multiple of 2^-36 and added as a 64-bit integer (so W * H < 2^28), the maximum is
+ * an integer maximum on the bits of a non-negative float, the count an integer add.  The blobs are read, not written.
+ * workspace: gsb_contributions_workspace_bytes(P) bytes (8 per Gaussian), 8-byte aligned.
+ * Errors, before any CUDA call (gsb_last_error() starts with "contributions: "): GSB_EINVAL for P < 0 or num_rendered < 0, width
+ * or height < 1; GSB_ERANGE for width * height >= 2^28; GSB_EINVAL for a NULL output (top_id, and with P > 0 the three per-Gaussian
+ * ones), a NULL blob with P > 0 or num_rendered > 0, a NULL or misaligned workspace with P > 0. */
+GSB_API size_t gsb_contributions_workspace_bytes(int32_t P);
+GSB_API int gsb_contributions(const char* geom_blob, int32_t P, const char* binning_blob, int64_t num_rendered, const char* image_blob,
+                              int32_t width, int32_t height, const float* pixel_weights /* [H,W] or NULL */, float* weight_sum,
+                              float* weight_max, int32_t* pixels, int32_t* top_id, void* workspace, void* stream);
+
 /* Test helper: the fused de-quantisation on its own -> activated scales [P,3], normalised rotations [P,4]. */
 GSB_API int gsb_debug_dequant(const GsbQuant* quant, int32_t P, float* scales, float* rotations, void* stream);
 

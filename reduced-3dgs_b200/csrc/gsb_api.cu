@@ -91,7 +91,7 @@ void prof_end(int kid, cudaStream_t stream)
 	t_prof_cur = nullptr;
 }
 static const char* kKernelNames[K_COUNT] = { "preprocess", "tile_scan", "scatter", "tile_sort_large", "tile_sort", "render_forward", "render_backward", "preprocess_backward", "mark_visible", "tools", "kmeans", "knn", "camera_grad", "det_scan",
-	"det_gather", "det_clear", "features_forward", "features_backward", "absgrad_finish" };
+	"det_gather", "det_clear", "features_forward", "features_backward", "absgrad_finish", "contributions" };
 
 int launch_debug_dequant(const GsbQuant*, int, float*, float*, cudaStream_t);
 int launch_mark_visible(int, const float*, const float*, uint8_t*, cudaStream_t);
@@ -99,7 +99,6 @@ int launch_tile_scan(const ImageState&, const GeomState&, const BinPlan&, int, i
 int launch_scatter_sort(const GeomState&, const BinningState&, const ImageState&, const BinPlan&, int, long long, int, int, cudaStream_t);
 int launch_sort_large(const GeomState&, const BinningState&, const ImageState&, int, int, uint32_t, uint32_t, cudaStream_t);
 int launch_export_binning(const GeomState&, const BinningState&, const ImageState&, int, int, uint64_t*, uint32_t*, cudaStream_t);
-int launch_stats_fixed_to_float(int, const unsigned long long*, float*, cudaStream_t);
 int launch_sh_stats_update(int, int, const int*, const float*, const float*, const float*, const int*, const int*, const float*, float*, float*,
 	float*, float*, float*, cudaStream_t);
 int launch_pixel_size(int, const float*, int, const float*, const float*, const int*, const int*, float*, cudaStream_t);
@@ -569,6 +568,39 @@ int gsb_export_binning(const char* geom_blob, int32_t P, const char* binning_blo
 	BinningState b = BinningState::carve(const_cast<char*>(binning_blob), R);
 	ImageState img = ImageState::carve(const_cast<char*>(image_blob), W, H);
 	return launch_export_binning(g, b, img, W, H, keys_sorted, point_list, (cudaStream_t)stream);
+}
+
+size_t gsb_contributions_workspace_bytes(int32_t P) { return (P > 0 ? size_t(P) * sizeof(unsigned long long) : 0) + 256; }
+
+// Every refusal of gsb_contributions, before any CUDA call (the order of include/gs_b200.h).
+static int check_contributions(const char* geom_blob, int P, const char* binning_blob, long long R, const char* image_blob, int W, int H,
+	const float* weight_sum, const float* weight_max, const int32_t* pixels, const int32_t* top_id, const void* workspace)
+{
+	if (P < 0 || R < 0) { set_error("contributions: negative size (P = %d, num_rendered = %lld)", P, R); return GSB_EINVAL; }
+	if (W <= 0 || H <= 0) { set_error("contributions: bad image size %dx%d", W, H); return GSB_EINVAL; }
+	if ((long long)W * H >= (1ll << 28))
+	{ set_error("contributions: %d x %d pixels; the 64-bit fixed-point sums need W * H < 2^28", W, H); return GSB_ERANGE; }
+	if (!top_id || (P > 0 && (!weight_sum || !weight_max || !pixels))) { set_error("contributions: an output is NULL"); return GSB_EINVAL; }
+	if ((P > 0 || R > 0) && (!geom_blob || !binning_blob || !image_blob)) { set_error("contributions: a blob is NULL"); return GSB_EINVAL; }
+	if (P > 0 && (!workspace || (reinterpret_cast<uintptr_t>(workspace) & 7)))
+	{ set_error("contributions: the workspace is NULL or not 8-byte aligned"); return GSB_EINVAL; }
+	return GSB_OK;
+}
+
+int gsb_contributions(const char* geom_blob, int32_t P, const char* binning_blob, int64_t R, const char* image_blob, int32_t W, int32_t H,
+	const float* pixel_weights, float* weight_sum, float* weight_max, int32_t* pixels, int32_t* top_id, void* workspace, void* stream)
+{
+	if (int e = check_contributions(geom_blob, P, binning_blob, R, image_blob, W, H, weight_sum, weight_max, pixels, top_id, workspace))
+		return e;
+	GeomState g{}; BinningState b{}; ImageState img{};
+	if (P > 0 && R > 0)
+	{
+		g = GeomState::carve(const_cast<char*>(geom_blob), P);
+		b = BinningState::carve(const_cast<char*>(binning_blob), R);
+		img = ImageState::carve(const_cast<char*>(image_blob), W, H);
+	}
+	return launch_contributions(g, b, img, P, R, W, H, pixel_weights, weight_sum, weight_max, pixels, top_id,
+		static_cast<unsigned long long*>(workspace), (cudaStream_t)stream);
 }
 
 int gsb_export_image(const char* image_blob, int32_t W, int32_t H, float* final_T, uint32_t* n_contrib, uint32_t* ranges, void* stream_)

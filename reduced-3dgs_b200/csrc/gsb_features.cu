@@ -42,23 +42,15 @@ static int features_ch(int F)
 	return forced ? forced : (F <= 8 ? 8 : 16);
 }
 
-// Stages list entries [first, first + n) of a tile (entry k at point_list[base + k]): r0 / r1 of the record, the Gaussian id and the
-// CH-channel slice [c0, c0 + CH) of its feature row (0 past F).
+// Stages list entries [first, first + n) of a tile (stage_records: r0 / r1 of the record and the Gaussian id), then the CH-channel
+// slice [c0, c0 + CH) of each one's feature row (0 past F).
 template <int CH>
 __device__ __forceinline__ void stage_batch(const uint32_t* __restrict__ point_list, const float4* __restrict__ rec,
 	const float* __restrict__ features, int F, int c0, int n, bool backwards, uint32_t base, uint32_t first, float4* s_rec, float* s_f,
 	uint32_t* s_id)
 {
 	const int tid = threadIdx.x;
-	if (tid < n)
-	{
-		const uint32_t k = backwards ? first - tid : first + tid;
-		const uint32_t id = point_list[base + k];
-		s_rec[2 * tid] = rec[3 * (size_t)id];
-		s_rec[2 * tid + 1] = rec[3 * (size_t)id + 1];
-		s_id[tid] = id;
-	}
-	__syncthreads();
+	stage_records(point_list, rec, n, backwards, base, first, s_rec, s_id);
 	// consecutive threads read consecutive channels of one row
 	for (int i = tid; i < n * CH; i += blockDim.x)
 	{

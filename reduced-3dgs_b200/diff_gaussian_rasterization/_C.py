@@ -27,6 +27,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+from typing import NamedTuple
 
 import torch
 
@@ -595,6 +596,62 @@ def export_state(geomBuffer, binningBuffer, imageBuffer, R, W, H, P=0):
         _lib.check(L.gsb_export_image(ptr(imageBuffer), W, H, ptr(final_T), ptr(n_contrib), ptr(ranges), _lib.current_stream(device)))
     out.update(keys=keys, point_list=pl, final_T=final_T, n_contrib=n_contrib, ranges=ranges)
     return out
+
+
+class Contributions(NamedTuple):
+    """One view's contribution statistics (gsb_contributions, DESIGN.md §5p): per Gaussian the sum of its blending weights
+    w = alpha * T (times the clamped pixel weight), their maximum and the number of pixels it composites; per pixel the id of the
+    Gaussian with the largest w (-1 where none)."""
+    weight_sum: torch.Tensor     # [P] float32
+    weight_max: torch.Tensor     # [P] float32
+    pixels: torch.Tensor         # [P] int32
+    top_id: torch.Tensor         # [H, W] int32
+
+
+def check_pixel_weights(pixel_weights, H, W, device=None):
+    """The checks of a `pixel_weights` map, made before anything runs: a contiguous float32 [H, W] or [1, H, W] tensor on `device`
+    (on a CUDA device when `device` is None)."""
+    if not isinstance(pixel_weights, torch.Tensor):
+        raise RuntimeError(f"pixel_weights must be an [H, W] tensor, got {type(pixel_weights).__name__}")
+    if tuple(pixel_weights.shape) not in ((H, W), (1, H, W)):
+        raise RuntimeError(f"pixel_weights must have shape [H, W] or [1, H, W] with H, W = {H}, {W}, got {tuple(pixel_weights.shape)}")
+    if pixel_weights.dtype != torch.float32:
+        raise RuntimeError(f"pixel_weights must be float32, got {pixel_weights.dtype}")
+    if not pixel_weights.is_contiguous():
+        raise RuntimeError("pixel_weights must be contiguous (it is read in place)")
+    if device is None and not pixel_weights.is_cuda:
+        raise RuntimeError("pixel_weights must live on a CUDA device (no CPU path exists)")
+    if device is not None and pixel_weights.device != device:
+        raise RuntimeError(f"pixel_weights must live on {device}, got {pixel_weights.device}")
+
+
+def contributions(geomBuffer, binningBuffer, imageBuffer, R, W, H, P, pixel_weights=None):
+    """The contribution statistics of the forward that left these blobs (its R, image size and P), -> Contributions(weight_sum [P],
+    weight_max [P], pixels [P], top_id [H, W]), views of one allocation.  `pixel_weights`: an [H, W] (or [1, H, W]) fp32 map on the
+    blobs' device, clamped to [0, 1] on read (NaN reads as 0), that weights the sum.  The same bytes on every run; the blobs are only
+    read.  No gradient."""
+    device = imageBuffer.device
+    if not imageBuffer.is_cuda:
+        raise RuntimeError("contributions: the forward's buffers must live on a CUDA device (no CPU path exists)")
+    W, H, P, R = int(W), int(H), int(P), int(R)
+    if pixel_weights is not None:
+        check_pixel_weights(pixel_weights, H, W, device)
+    L = _lib.lib()
+    with on_device(device):
+        ws_words = (int(L.gsb_contributions_workspace_bytes(P)) + 3) // 4
+        # int32 words: weight_sum, weight_max, pixels, top_id, then the 8-byte fixed-point workspace, each on a 256-byte boundary
+        sizes = [P, P, P, H * W, ws_words]
+        offs, total = [], 0
+        for n in sizes:
+            offs.append(total)
+            total += (n + 63) // 64 * 64
+        flat = torch.empty(total, dtype=torch.int32, device=device)
+        ws, pw_sum, pw_max, pix, top = (flat[offs[4]:offs[4] + ws_words], flat[:P].view(torch.float32),
+                                        flat[offs[1]:offs[1] + P].view(torch.float32), flat[offs[2]:offs[2] + P],
+                                        flat[offs[3]:offs[3] + H * W].view(H, W))
+        _lib.check(L.gsb_contributions(ptr(geomBuffer), P, ptr(binningBuffer), R, ptr(imageBuffer), W, H, ptr(pixel_weights), ptr(pw_sum),
+                                       ptr(pw_max), ptr(pix), ptr(top), ptr(ws), _lib.current_stream(device)))
+    return Contributions(pw_sum, pw_max, pix, top)
 
 
 def debug_dequant(quant):

@@ -24,6 +24,9 @@ gradient the absolute screen-space gradient (sum_p |g_x|, sum_p |g_y|, 0) of Abs
 statistic whose per-pixel terms cannot cancel; it has no feature form.
 GaussianRasterizer.forward's keyword-only `filter_3D` ([P] or [P, 1] fp32, gs_b200.mip.compute_3D_filter) applies Mip-Splatting's
 3D smoothing filter to the scales and the opacity inside the kernels; it is a constant (no gradient), as Mip-Splatting's buffer is.
+GaussianRasterizer.forward's keyword-only `contributions=True` appends _C.Contributions(weight_sum [P], weight_max [P], pixels [P],
+top_id [H, W]), the view's per-Gaussian blending-weight statistics from the forward's own blobs (no gradient); `pixel_weights`
+([H, W] fp32) weights the sum.
 Every option goes through the one autograd op, _RasterizeGaussians, each optional input in a slot of its own.
 """
 from typing import NamedTuple
@@ -54,10 +57,11 @@ def _call(fn, args, kw, dump, message):
 
 # The autograd op's inputs, in the order of its forward's parameters: the reference's fourteen (means3D ... cov3Ds_precomp,
 # raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps), then one slot per optional input.  A call that uses no
-# optional input passes the first fourteen only.
+# optional input passes the first fourteen only.  The contributions request (a 1-tuple of the pixel weights, or None) comes last and
+# only when it is made.
 MEANS3D, MEANS2D, SH, DEGREES, COLORS, OPACITIES, SCALES, ROTATIONS, COV3D = range(9)
-VIEWMATRIX, PROJMATRIX, CAMPOS, FEATURES, MEANS2D_ABS, FEATURES_DC, FEATURES_REST, SCALING, ROTATION, FILTER_3D = range(14, 24)
-N_INPUTS = 24
+VIEWMATRIX, PROJMATRIX, CAMPOS, FEATURES, MEANS2D_ABS, FEATURES_DC, FEATURES_REST, SCALING, ROTATION, FILTER_3D, CONTRIBUTIONS = range(14, 25)
+N_INPUTS = 25
 
 
 def _deterministic(raster_settings):
@@ -69,15 +73,19 @@ def _deterministic(raster_settings):
 
 def rasterize_gaussians(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
                         raster_settings, lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, features=None,
-                        means2D_abs=None, raw_params=None, filter_3D=None):
+                        means2D_abs=None, raw_params=None, filter_3D=None, contributions=None):
+    """`contributions`: None, or the request (pixel_weights or None,): the outputs then end with a _C.Contributions."""
     camera = (raster_settings.viewmatrix, raster_settings.projmatrix, raster_settings.campos)
     if not (torch.is_grad_enabled() and any(isinstance(t, torch.Tensor) and t.requires_grad for t in camera)):
         # a constant camera is read from raster_settings; a learnable one is also an input, so that its gradients have a destination
         camera = (None,) * 3
     optional = (*camera, features, means2D_abs, *(raw_params or (None,) * 4), filter_3D)
-    return _RasterizeGaussians.apply(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
-                                     raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps,
-                                     *(optional if any(t is not None for t in optional) else ()))
+    if contributions is not None:
+        optional += (contributions,)
+    out = _RasterizeGaussians.apply(means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp,
+                                    raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps,
+                                    *(optional if any(t is not None for t in optional) else ()))
+    return out if contributions is None else out[:-4] + (_C.Contributions(*out[-4:]),)
 
 
 class _RasterizeGaussians(torch.autograd.Function):
@@ -87,12 +95,15 @@ class _RasterizeGaussians(torch.autograd.Function):
     (then empty): the kernels apply get_features / get_scaling / get_rotation themselves and return the gradients of these four
     tensors directly, so the graph holds no Cat / Exp / Div node and no [P,16,3] copy or gradient exists.  `filter_3D` is
     Mip-Splatting's 3D filter, a constant: the backward gets it and the opacity logits, and it receives no gradient.
-    -> (color, radii), with return_maps (color, radii, invdepth, alpha); with `features` the feature image [F, H, W] comes last."""
+    `contributions` = (pixel_weights or None,) runs _C.contributions on the blobs this forward left.
+    -> (color, radii), with return_maps (color, radii, invdepth, alpha); with `features` the feature image [F, H, W] comes next, and with
+    `contributions` its four tensors (weight_sum, weight_max, pixels, top_id) last, non-differentiable."""
 
     @staticmethod
     def forward(ctx, means3D, means2D, sh, degrees, colors_precomp, opacities, scales, rotations, cov3Ds_precomp, raster_settings,
                 lambda_sh_sparsity, prune_mask=None, quant=None, return_maps=False, viewmatrix=None, projmatrix=None, campos=None,
-                features=None, means2D_abs=None, features_dc=None, features_rest=None, scaling=None, rotation=None, filter_3D=None):
+                features=None, means2D_abs=None, features_dc=None, features_rest=None, scaling=None, rotation=None, filter_3D=None,
+                contributions=None):
         rs = raster_settings
         args = (rs.bg, means3D, colors_precomp, opacities, scales, rotations, rs.scale_modifier, cov3Ds_precomp, rs.viewmatrix,
                 rs.projmatrix, rs.tanfovx, rs.tanfovy, rs.image_height, rs.image_width, sh, degrees, rs.campos, rs.prefiltered, rs.debug)
@@ -109,7 +120,11 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.prune_mask, ctx.quant, ctx.return_maps, ctx.has_features = prune_mask, quant, return_maps, features is not None
         ctx.has_abs = means2D_abs is not None
         ctx.camera_meta = None if viewmatrix is None else [(t.shape, t.dtype) for t in (viewmatrix, projmatrix, campos)]
-        ctx.mark_non_differentiable(out[2])
+        contrib = ()
+        if contributions is not None:
+            contrib = tuple(_C.contributions(out[3], out[4], out[5], out[0], rs.image_width, rs.image_height, means3D.shape[0],
+                                             pixel_weights=contributions[0]))
+        ctx.mark_non_differentiable(out[2], *contrib)
         if return_maps or features is not None:
             # a loss on some outputs only: the others' gradients arrive as None and reach the kernels as NULL (zero), and a feature
             # image without a gradient leaves the backward exactly the call without features
@@ -117,13 +132,14 @@ class _RasterizeGaussians(torch.autograd.Function):
         ctx.save_for_backward(colors_precomp, means3D, scales, rotations, cov3Ds_precomp, out[2], sh, out[3], out[4], out[5], degrees,
                               features, features_dc, features_rest, scaling, rotation, filter_3D,
                               opacities if filter_3D is not None else None)
-        return (out[1], out[2]) + (out[6:8] if return_maps else ()) + (out[-1:] if features is not None else ())
+        return (out[1], out[2]) + (out[6:8] if return_maps else ()) + (out[-1:] if features is not None else ()) + contrib
 
     @staticmethod
     def backward(ctx, grad_out_color, _, *grads):
-        # after (color, radii): the maps' gradients with return_maps, then the feature image's when given
+        # after (color, radii): the maps' gradients with return_maps, then the feature image's when given (the contributions, last,
+        # have none)
         grad_invdepth, grad_alpha = grads[:2] if ctx.return_maps else (None, None)
-        grad_features = grads[-1] if ctx.has_features else None
+        grad_features = grads[2 if ctx.return_maps else 0] if ctx.has_features else None
         (colors_precomp, means3D, scales, rotations, cov3Ds_precomp, radii, sh, geomBuffer, binningBuffer, imgBuffer, degrees, features,
          features_dc, features_rest, scaling, rotation, filter_3D, opacities) = ctx.saved_tensors
         rs = ctx.raster_settings
@@ -225,7 +241,7 @@ class GaussianRasterizer(nn.Module):
 
     def forward(self, means3D, means2D, opacities, shs=None, degrees=None, colors_precomp=None, scales=None,
                 rotations=None, cov3D_precomp=None, lambda_sh_sparsity=0., *, prune_mask=None, quant=None, return_maps=False,
-                raw_params=None, features=None, means2D_abs=None, filter_3D=None):
+                raw_params=None, features=None, means2D_abs=None, filter_3D=None, contributions=False, pixel_weights=None):
         """-> (color, radii); with return_maps, (color, radii, invdepth [1,H,W], alpha [1,H,W]), all three differentiable.
         `raw_params`: (features_dc [P,1,3], features_rest [P,C,3], scaling [P,3], rotation [P,4]), the model's leaf tensors, in place
         of shs / scales / rotations (which must then be None, as must cov3D_precomp and quant); with colors_precomp the two
@@ -236,8 +252,14 @@ class GaussianRasterizer(nn.Module):
         `means2D_abs`: a [P, 3] tensor (a zeros leaf that requires grad); its gradient is the absolute screen-space gradient
         (sum_p |g_x|, sum_p |g_y|, 0), deterministic with the deterministic mode.  Not together with `features`.
         `filter_3D`: [P] or [P, 1] fp32 on the device, Mip-Splatting's 3D smoothing filter (a constant): the kernels render with
-        scales sqrt(s^2 + f^2) and opacities sigmoid(logit) * c3, and chain the gradients through both.  Not with cov3D_precomp."""
+        scales sqrt(s^2 + f^2) and opacities sigmoid(logit) * c3, and chain the gradients through both.  Not with cov3D_precomp.
+        `contributions`: the outputs end with _C.Contributions(weight_sum [P], weight_max [P], pixels [P], top_id [H, W]) of this view
+        (DESIGN.md §5p), no gradient; `pixel_weights` ([H, W] or [1, H, W] fp32 on the device, clamped to [0, 1]) weights the sum."""
         raster_settings = self.raster_settings
+        if pixel_weights is not None:
+            if not contributions:
+                raise RuntimeError("pixel_weights weights the contribution sums; it needs contributions=True")
+            _C.check_pixel_weights(pixel_weights, int(raster_settings.image_height), int(raster_settings.image_width), means3D.device)
         if means2D_abs is not None:
             if features is not None:
                 raise RuntimeError("means2D_abs: the absolute screen-space gradient has no feature form; render the features separately")
@@ -268,4 +290,4 @@ class GaussianRasterizer(nn.Module):
         e = lambda t: empty if t is None else t                                  # absent inputs travel as empty tensors
         return rasterize_gaussians(means3D, means2D, e(shs), degrees, e(colors_precomp), e(opacities), e(scales), e(rotations),
                                    e(cov3D_precomp), raster_settings, lambda_sh_sparsity, prune_mask, quant, return_maps, features,
-                                   means2D_abs, raw_params, filter_3D)
+                                   means2D_abs, raw_params, filter_3D, (pixel_weights,) if contributions else None)

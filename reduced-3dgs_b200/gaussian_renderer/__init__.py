@@ -20,6 +20,9 @@ gradient (sum_p |g_x|, sum_p |g_y|, 0) of AbsGS, the split statistic of densify_
 a backward, so the variable-SH inference path refuses it, and it has no feature form.
 `pc.filter_3D` (optional, [P] or [P, 1] fp32 on the device; gs_b200.mip.compute_3D_filter sets it) is Mip-Splatting's 3D smoothing
 filter, applied in the kernels on every path (DESIGN.md §5o); it does not go with pipe.compute_cov3D_python.
+`contributions=True` adds pkg["contributions"], the view's _C.Contributions(weight_sum [P], weight_max [P], pixels [P], top_id [H, W])
+of the blending weights w = alpha * T (DESIGN.md §5p), on every path; `pixel_weights` ([H, W] fp32 on the device, clamped to [0, 1])
+weights the sum (INTEGRATION.md K: importance pruning, error-weighted scores, per-pixel winners).  No gradient.
 
 A learnable camera needs no argument: when world_view_transform, full_proj_transform or camera_center requires grad, the
 rasterizer returns their gradients (the variable-SH inference path stays non-differentiable).  The rasterizer takes
@@ -36,7 +39,7 @@ import torch.nn.functional as F
 # train.py next to `render`) must stay importable: let submodule lookups continue into same-named packages further down the path.
 __path__ = pkgutil.extend_path(__path__, __name__)
 
-from diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer
+from diff_gaussian_rasterization import GaussianRasterizationSettings, GaussianRasterizer, _C
 from diff_gaussian_rasterization._C import rasterize_gaussians_variableSH_bands
 
 
@@ -86,7 +89,8 @@ def _raw_params(pc, pipe, override_color):
 
 
 def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=1.0, override_color=None,
-           lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False, return_maps=False, features=None, absgrad=False):
+           lambda_sh_sparsity=0., measure_fps=False, variable_sh_bands=False, return_maps=False, features=None, absgrad=False,
+           contributions=False, pixel_weights=None):
     """
     Render the scene.
 
@@ -99,6 +103,10 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         raise RuntimeError("gaussian_renderer.render: absgrad needs the backward; the variable-SH inference path renders forward only")
     if absgrad and features is not None:
         raise RuntimeError("gaussian_renderer.render: absgrad has no feature form; render the features in a call without absgrad")
+    if pixel_weights is not None:
+        if not contributions:
+            raise RuntimeError("gaussian_renderer.render: pixel_weights weights the contribution sums; it needs contributions=True")
+        _C.check_pixel_weights(pixel_weights, int(viewpoint_camera.image_height), int(viewpoint_camera.image_width), pc.get_xyz.device)
     filter_3D = getattr(pc, "filter_3D", None)
     if filter_3D is not None and pipe.compute_cov3D_python:
         raise RuntimeError("gaussian_renderer.render: pc.filter_3D filters the scales inside the kernels; it does not go with "
@@ -178,17 +186,23 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
             **({} if filter_3D is None else dict(filter_3D=filter_3D)))
         rendered_image, radii = out[1], out[2]
         maps = out[6:8] if return_maps else ()
-        feature_image = out[-1] if features is not None else None
+        feature_image = out[6 + 2 * return_maps] if features is not None else None
+        contrib = None
+        if contributions:
+            contrib = _C.contributions(out[3], out[4], out[5], out[0], raster_settings.image_width, raster_settings.image_height,
+                                       means3D.shape[0], pixel_weights=pixel_weights)
     else:
         out = rasterizer(
             means3D=means3D, means2D=means2D, shs=shs, degrees=degrees, colors_precomp=colors_precomp, opacities=opacity,
             scales=scales, rotations=rotations, cov3D_precomp=cov3D_precomp, lambda_sh_sparsity=lambda_sh_sparsity,
             prune_mask=prune_mask, quant=quant, return_maps=return_maps, raw_params=raw_params, features=features,
             **({} if screenspace_points_abs is None else dict(means2D_abs=screenspace_points_abs)),
-            **({} if filter_3D is None else dict(filter_3D=filter_3D)))
+            **({} if filter_3D is None else dict(filter_3D=filter_3D)),
+            **({} if not contributions else dict(contributions=True, pixel_weights=pixel_weights)))
         rendered_image, radii = out[0], out[1]
         maps = out[2:4] if return_maps else ()
-        feature_image = out[-1] if features is not None else None
+        feature_image = out[2 + 2 * return_maps] if features is not None else None
+        contrib = out[-1] if contributions else None
     if measure_fps:
         end_timer.record()
         torch.cuda.synchronize()
@@ -207,4 +221,6 @@ def render(viewpoint_camera, pc, pipe, bg_color: torch.Tensor, scaling_modifier=
         pkg["features"] = feature_image
     if absgrad:
         pkg["viewspace_points_abs"] = screenspace_points_abs
+    if contributions:
+        pkg["contributions"] = contrib
     return pkg

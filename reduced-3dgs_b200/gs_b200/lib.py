@@ -128,6 +128,8 @@ SIGNATURES = {
     "gsb_mark_visible": (C.c_int, [_I32, _V, _V, _V, _V, _V]),
     "gsb_export_binning": (C.c_int, [_V, _I32, _V, _I64, _V, _I32, _I32, _V, _V, _V]),
     "gsb_export_image": (C.c_int, [_V, _I32, _I32, _V, _V, _V, _V]),
+    "gsb_contributions_workspace_bytes": (_SZ, [_I32]),
+    "gsb_contributions": (C.c_int, [_V, _I32, _V, _I64, _V, _I32, _I32] + [_V] * 7),
     "gsb_debug_dequant": (C.c_int, [C.POINTER(GsbQuant), _I32, _V, _V, _V]),
     "gsb_sh_statistics_update": (C.c_int, [_I32, _I32] + [_V] * 13),
     "gsb_min_projected_pixel_size": (C.c_int, [_I32, _V, _I32, _V, _V, _V, _V, _V, _V]),
