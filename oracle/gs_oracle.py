@@ -249,15 +249,17 @@ def min_projected_pixel_size(w2ndc, w2ndc_inv, means3D, image_height, image_widt
     return out
 
 
-def sphere_ellipsoid_intersection(means3D, scales, rotations, neighbours, sphere_radius, knn):
-    """Reduced3DGS::intersectionTest (reduced_3dgs.cu:205-243) -> (redundancy int32 [P,1], mask bool [P,knn], borderline bool [P])."""
+def sphere_ellipsoid_intersection(means3D, scales, rotations, neighbours, sphere_radius, knn, dots=False):
+    """Reduced3DGS::intersectionTest (reduced_3dgs.cu:205-243) -> (redundancy int32 [P,1], mask bool [P,knn], borderline bool [P]),
+    and with dots=True also each pair's `dot` (float32 [P,knn]): a hit is dot < 1."""
     means3D, scales, rotations = _np(means3D, np.float32), _np(scales, np.float32), _np(rotations, np.float32)
     neighbours, sphere_radius = _np(neighbours, np.int32), _np(sphere_radius, np.float32).reshape(-1)
     P = means3D.shape[0]
     red, mask, bl = np.zeros((P, 1), np.int32), np.zeros((P, knn), np.uint8), np.zeros(P, np.uint8)
+    dot = np.zeros((P, knn), np.float32) if dots else None
     lib().gso_sphere_ellipsoid(P, _p(means3D, f32p), _p(scales, f32p), _p(rotations, f32p), _p(neighbours, i32p), _p(sphere_radius, f32p),
-                               int(knn), _p(red, i32p), _p(mask, u8p), _p(bl, u8p))
-    return red, mask.astype(bool), bl.astype(bool)
+                               int(knn), _p(red, i32p), _p(mask, u8p), _p(bl, u8p), _p(dot, f32p))
+    return (red, mask.astype(bool), bl.astype(bool)) + ((dot,) if dots else ())
 
 
 def min_redundancy_value(redundancy_values, neighbours, intersection_mask, knn):
