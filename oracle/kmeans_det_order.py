@@ -59,15 +59,12 @@ def _pairwise(x: np.ndarray) -> np.ndarray:
     return x[..., 0]
 
 
-def cluster_sums(sorted_values: np.ndarray, ids: np.ndarray, K: int) -> np.ndarray:
-    """sum(k) for k = 0..K-1 in the order of the module docstring; sorted_values ascending by float_key, ids their clusters."""
+def block_parts(sorted_values: np.ndarray, ids: np.ndarray, K: int, rows_per_slice: int = 1 << 16):
+    """part(b, k) for every (block, cluster) present -> (part_b, part_k, part), ascending in (b, k).  The dense table of 256 leaves
+    per (block, cluster) is built `rows_per_slice` rows at a time."""
     v = np.asarray(sorted_values, dtype=F32).reshape(-1)
     ids = np.asarray(ids, dtype=np.int64).reshape(-1)
     n = v.shape[0]
-    sums = np.zeros(K, dtype=F32)
-    if n == 0:
-        return sums
-    n_blocks = (n + BLOCK - 1) // BLOCK
     pos = np.arange(n)
     block, chunk = pos // BLOCK, (pos % BLOCK) // CHUNK
     # leaves: one per (block, chunk, cluster) present, each a left fold from -0 over its positions in ascending order
@@ -87,21 +84,38 @@ def cluster_sums(sorted_values: np.ndarray, ids: np.ndarray, K: int) -> np.ndarr
     # part(b, k): a dense row of 256 leaves per (block, cluster) present, -0 where the chunk has no value of the cluster
     bk = leaf_b * K + leaf_k
     pairs, row = np.unique(bk, return_inverse=True)
-    dense = np.full((pairs.shape[0], CHUNKS_PER_BLOCK), -0.0, dtype=F32)
-    dense[row, leaf_t] = leaf
-    with np.errstate(all="ignore"):
-        part = _pairwise(dense)
-    part_b, part_k = pairs // K, pairs % K
-    # lane(l, k) and sum(k)
-    rows = (n_blocks + LANES - 1) // LANES
+    by_row = np.argsort(row, kind="stable")
+    row, leaf_t, leaf = row[by_row], leaf_t[by_row], leaf[by_row]
+    part = np.empty(pairs.shape[0], dtype=F32)
+    for r0 in range(0, pairs.shape[0], rows_per_slice):
+        a, b = np.searchsorted(row, [r0, r0 + rows_per_slice])
+        dense = np.full((min(rows_per_slice, pairs.shape[0] - r0), CHUNKS_PER_BLOCK), -0.0, dtype=F32)
+        dense[row[a:b] - r0, leaf_t[a:b]] = leaf[a:b]
+        with np.errstate(all="ignore"):
+            part[r0:r0 + dense.shape[0]] = _pairwise(dense)
+    return pairs // K, pairs % K, part
+
+
+def lane_sums(lane_pos: np.ndarray, part_k: np.ndarray, part: np.ndarray, K: int) -> np.ndarray:
+    """lane(l, k) and sum(k) from the parts placed at lane_pos: position p goes to lane p % 256, and each lane adds its parts in
+    ascending p.  cluster_sums places part(b, k) at p = b."""
+    rows = (int(lane_pos.max(initial=0)) + LANES) // LANES
     lanes = np.full((K, rows * LANES), -0.0, dtype=F32)
-    lanes[part_k, part_b] = part
+    lanes[part_k, lane_pos] = part
     lanes = lanes.reshape(K, rows, LANES)
     acc = np.full((K, LANES), -0.0, dtype=F32)
     with np.errstate(all="ignore"):
         for r in range(rows):
             acc = acc + lanes[:, r, :]
         return _pairwise(acc) + F32(0.0)
+
+
+def cluster_sums(sorted_values: np.ndarray, ids: np.ndarray, K: int) -> np.ndarray:
+    """sum(k) for k = 0..K-1 in the order of the module docstring; sorted_values ascending by float_key, ids their clusters."""
+    if np.asarray(sorted_values).size == 0:
+        return np.zeros(K, dtype=F32)
+    part_b, part_k, part = block_parts(sorted_values, ids, K)
+    return lane_sums(part_b, part_k, part, K)
 
 
 def update(centres: np.ndarray, sums: np.ndarray, sizes: np.ndarray):

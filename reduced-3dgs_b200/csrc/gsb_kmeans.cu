@@ -194,6 +194,9 @@ __global__ void __launch_bounds__(256) km_sort_pass_kernel(uint32_t* keys0, uint
 
 // ------------------------------------------------------------------------------------------------ Lloyd iteration
 // Sorted centres in shared memory: value ascending, ties by original index; run_start / run_end delimit runs of EQUAL values.
+// The sort key is canonical: -0 sorts as +0 and every NaN as the one +NaN key (after +inf), so centres that compare equal share a
+// key and each run is in original index order.  c[] holds the canonical value (+0, +NaN), which has the same distance to every
+// value as the original (|v - (-0)| == |v - (+0)|, and a NaN distance stays NaN).
 struct KmCentres {
 	float c[KM_MAX_K];
 	int idx[KM_MAX_K];
@@ -201,13 +204,18 @@ struct KmCentres {
 	short run_end[KM_MAX_K];         // one past the run's last element
 };
 
+__device__ __forceinline__ uint32_t km_centre_key(float c)
+{
+	return isnan(c) ? 0xffffffffu : float_key(c == 0.0f ? 0.0f : c);
+}
+
 __device__ void km_load_sorted_centres(KmCentres& S, const float* __restrict__ centres, int K)
 {
 	__shared__ unsigned long long s_key[KM_MAX_K];
 	int Kp = 1;
 	while (Kp < K) Kp <<= 1;
 	for (int i = threadIdx.x; i < Kp; i += blockDim.x)
-		s_key[i] = i < K ? (((unsigned long long)float_key(centres[i]) << 32) | (uint32_t)i) : ~0ull;
+		s_key[i] = i < K ? (((unsigned long long)km_centre_key(centres[i]) << 32) | (uint32_t)i) : ~0ull;
 	__syncthreads();
 	for (int k = 2; k <= Kp; k <<= 1)
 		for (int j = k >> 1; j > 0; j >>= 1)
@@ -249,7 +257,10 @@ __device__ __forceinline__ float km_dist(float v, float c)
 }
 
 // kmeans.cu:83-104: argmin over the centres in ORIGINAL order with a strict `<`, i.e. the smallest distance and, among equal
-// (rounded) distances, the smallest original index; 0 when no distance is below +inf (or the value is NaN).
+// (rounded) distances, the smallest original index; 0 when no distance is below +inf (or the value is NaN).  The rounded distance
+// does not decrease away from v in sorted order, so the minimum is at a neighbour of the lower bound j and every centre at that
+// distance lies in the runs walked outwards from j.  NaN centres sort last, where `c < v` is false as for a centre above v, and
+// their NaN distance never equals dmin; the smallest index of a run is S.idx[run_start] because equal centres share a key.
 __device__ __forceinline__ int km_assign(const KmCentres& S, int K, float v)
 {
 	int lo = 0, hi = K;                                       // lower bound: first centre >= v
