@@ -145,10 +145,11 @@ def render_forward(geom, binning, bg, W, H, f64=False):
     colors = _np(geom["rgb"], np.float32)
     if f64:
         out = np.zeros((3, H, W), np.float64)
+        final_T = np.zeros((H, W), np.float64)
         lib().gso_render_forward_f64(W, H, _p(binning["ranges"], u32p), _p(binning["point_list"], u32p),
                                      _p(geom["means2D"], f32p), _p(colors, f32p), _p(geom["conic_opacity"], f32p),
-                                     _p(bg, f32p), _p(out, f64p))
-        return dict(color64=out)
+                                     _p(bg, f32p), _p(out, f64p), _p(final_T, f64p))
+        return dict(color64=out, final_T64=final_T)
     final_T = np.zeros((H, W), np.float32)
     n_contrib = np.zeros((H, W), np.uint32)
     color = np.zeros((3, H, W), np.float32)
